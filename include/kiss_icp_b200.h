@@ -227,6 +227,39 @@ int kb_pipeline_threshold(const kb_pipeline *p, double *out_sigma);
 /* kernels launched by this pipeline so far (bench "gpu_launches") */
 int kb_pipeline_launch_count(const kb_pipeline *p, unsigned long long *out);
 
+/* ---- checkpoint / restore ----------------------------------------------------------------
+ * The reference leaves a sequence's whole state public: the map (VoxelHashMap::map_,
+ * cpp/kiss_icp/core/VoxelHashMap.hpp:56), pose() / delta() as mutable Sophus::SE3d&
+ * (cpp/kiss_icp/pipeline/KissICP.hpp:79-95) and AdaptiveThreshold::model_sse_ / num_samples_
+ * (cpp/kiss_icp/core/Threshold.hpp:44-46). These calls read and write the same state, exactly.
+ * A pipeline's map is restored with kb_map_load(kb_pipeline_voxel_map(p), ...); there is no
+ * blob format, callers compose the calls they need. */
+/* Replace the map's contents. Layout = kb_map_dump's: voxels int[n_voxels][3] in any order,
+ * counts int[n_voxels], points double[n_points][3] concatenated per voxel in insertion order.
+ * Synchronous: all or nothing. KB_ERR_INVALID_ARG (map, counters and capacity unchanged) for a
+ * duplicate voxel, a count outside [1, max_points_per_voxel], n_points != sum of counts, a
+ * non-finite coordinate, or a point whose voxel (the hot path's own FP64 voxel function) is not
+ * the voxel it is listed under. The _dev form takes device pointers on the map's device. */
+int kb_map_load(kb_map *map, const int *voxels, const int *counts, const double *points, size_t n_voxels,
+                size_t n_points);
+int kb_map_load_dev(kb_map *map, const int *d_voxels, const int *d_counts, const double *d_points, size_t n_voxels,
+                    size_t n_points);
+/* the pipeline's exact state; SE(3) elements in Sophus::SE3d::params() order {qx,qy,qz,qw,tx,ty,tz} */
+typedef struct kb_pipeline_state {
+    double pose[7];
+    double delta[7];
+    double model_sse;
+    int num_samples;
+} kb_pipeline_state;
+int kb_pipeline_get_state(const kb_pipeline *p, kb_pipeline_state *out);
+/* Stores the values bit for bit (no renormalisation: get -> set -> get is the identity) and drops
+ * any prefetched frame. KB_ERR_INVALID_ARG for a non-finite value, num_samples < 1 or
+ * model_sse < 0; KB_ERR_NOT_SE3 for a quaternion whose squared norm is not within 1e-10 of 1. */
+int kb_pipeline_set_state(kb_pipeline *p, const kb_pipeline_state *s);
+/* the stand-alone AdaptiveThreshold's model_sse_ / num_samples_ (same checks as above) */
+int kb_threshold_get_state(const kb_threshold *th, double *model_sse, int *num_samples);
+int kb_threshold_set_state(kb_threshold *th, double model_sse, int num_samples);
+
 #ifdef __cplusplus
 }
 #endif

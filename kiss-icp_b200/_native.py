@@ -82,6 +82,11 @@ class FrameStats(C.Structure):
                 ("n_source", i32), ("map_points", i32), ("map_voxels", i32), ("team", i32)]
 
 
+class PipelineState(C.Structure):
+    """kb_pipeline_state: pose / delta in Sophus::SE3d::params() order {qx,qy,qz,qw,tx,ty,tz}"""
+    _fields_ = [("pose", dbl * 7), ("delta", dbl * 7), ("model_sse", dbl), ("num_samples", i32)]
+
+
 # every exported symbol of include/kiss_icp_b200.h: name -> (restype, argtypes)
 SIGNATURES = {
     "kb_last_error": (C.c_char_p, []),
@@ -158,6 +163,12 @@ SIGNATURES = {
     "kb_pipeline_set_history": (i32, [vp, sz]),
     "kb_pipeline_get_history": (i32, [vp, vp, sz, C.POINTER(sz)]),
     "kb_pipeline_launch_count": (i32, [vp, C.POINTER(C.c_ulonglong)]),
+    "kb_map_load": (i32, [vp, vp, vp, vp, sz, sz]),
+    "kb_map_load_dev": (i32, [vp, vp, vp, vp, sz, sz]),
+    "kb_pipeline_get_state": (i32, [vp, C.POINTER(PipelineState)]),
+    "kb_pipeline_set_state": (i32, [vp, C.POINTER(PipelineState)]),
+    "kb_threshold_get_state": (i32, [vp, C.POINTER(dbl), C.POINTER(i32)]),
+    "kb_threshold_set_state": (i32, [vp, dbl, i32]),
 }
 
 

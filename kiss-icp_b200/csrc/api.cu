@@ -4,6 +4,9 @@
 // point returns KB_ERR_NO_DEVICE.
 #include <cuda_runtime.h>
 
+#include <cub/device/device_scan.cuh>
+#include <cuda/std/functional>
+
 #include <algorithm>
 #include <array>
 #include <chrono>
@@ -559,6 +562,69 @@ struct kb_map {
         if (h_counters[C_STATUS] & ST_TABLE_FULL) return fail(KB_ERR_CUDA, "voxel table overflow (internal capacity bug)");
         return KB_OK;
     }
+    // kb_map_load[_dev]: replace the contents by the validated input, all or nothing. The input goes into an empty
+    // table that is adopted only when k_map_load found nothing wrong; otherwise the map, its counters and the spare
+    // table are left as they were.
+    int load(const int *d_vox, const int *d_cnt, const long long *d_off, const double *d_pts, size_t nv, size_t np) {
+        const size_t want = std::max<size_t>({capacity, pow2_at_least(3 * nv), size_t(1) << 14});
+        if (want > (size_t(1) << 31)) return fail(KB_ERR_INVALID_ARG, "voxel table would exceed 2^31 slots");
+        StallTrace trace("voxel map load");
+        // take_table frees a spare of another size: keep it aside so that a failed load can put it back
+        const bool from_spare = spare.capacity == want;
+        Table keep;
+        if (!from_spare) std::swap(keep, spare);
+        Table nt;
+        const int st = take_table(want, &nt);
+        if (st != KB_OK) {
+            spare = keep;
+            return st;
+        }
+        int h[C_NCOUNTERS] = {0};
+        if (nv) {
+            MapLoadParams P;
+            P.m = view();
+            P.m.slots = nt.slots;
+            P.m.points = nt.points;
+            P.m.head = nt.head;
+            P.m.pcount = nt.pcount;
+            P.m.pending = nt.pending;
+            P.m.counters = nt.counters;
+            P.m.mask = static_cast<unsigned>(want - 1);
+            P.voxels = d_vox;
+            P.counts = d_cnt;
+            P.offsets = d_off;
+            P.points = d_pts;
+            P.n = nv;
+            P.n_points = np;
+            k_map_load<<<std::min<size_t>(2048, (nv * 32 + 255) / 256), 256, 0, ex->stream>>>(P);
+            ++ex->launches;
+            CK(cudaGetLastError());
+        }
+        CK(cudaMemcpyAsync(h, nt.counters, sizeof(h), cudaMemcpyDeviceToHost, ex->stream));
+        RET(ex->sync());
+        const int bad = h[C_STATUS];
+        if (bad) {
+            if (from_spare) {
+                spare = nt;
+            } else {
+                free_table(nt);
+                spare = keep;
+            }
+            if (bad & ST_TABLE_FULL) return fail(KB_ERR_CUDA, "voxel table overflow during load (internal capacity bug)");
+            std::string why;
+            if (bad & ST_LOAD_DUPLICATE) why += " a voxel appears twice;";
+            if (bad & ST_LOAD_COUNT) why += " a count is outside [1, max_points_per_voxel] or the counts do not cover the points;";
+            if (bad & ST_LOAD_NONFINITE) why += " a coordinate is not finite;";
+            if (bad & ST_LOAD_OUTSIDE) why += " a point lies outside its voxel;";
+            return fail(KB_ERR_INVALID_ARG, "map load rejected, the map is unchanged:%s", why.c_str());
+        }
+        free_table(keep);
+        Table old = current();
+        adopt(nt);
+        spare = old;
+        std::memcpy(h_counters, h, sizeof(h_counters));  // the host's grow decision and the kernel's veto read these
+        return KB_OK;
+    }
     // d_pts already on the device
     int update_dev(const double *d_pts, size_t n, bool has_pose, const SE3 &pose, bool do_add, bool do_remove,
                    const V3 &origin) {
@@ -876,6 +942,58 @@ int kb_map_dump(const kb_map *cmap, int *voxels, int *counts, double *points, si
     }
     return KB_OK;
 }
+static int map_load_check(const kb_map *map, const void *voxels, const void *counts, const void *points, size_t n_voxels,
+                          size_t n_points) {
+    if (!map || (n_voxels && (!voxels || !counts)) || (n_points && !points)) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n_voxels > static_cast<size_t>(INT_MAX) || n_points > static_cast<size_t>(INT_MAX))
+        return fail(KB_ERR_INVALID_ARG, "map too large (%zu voxels, %zu points)", n_voxels, n_points);
+    return KB_OK;
+}
+int kb_map_load(kb_map *map, const int *voxels, const int *counts, const double *points, size_t n_voxels, size_t n_points) {
+    RET(map_load_check(map, voxels, counts, points, n_voxels, n_points));
+    std::vector<long long> off(n_voxels);
+    long long total = 0;
+    for (size_t i = 0; i < n_voxels; ++i) {
+        off[i] = total;
+        total += counts[i];
+    }
+    if (total != static_cast<long long>(n_points))
+        return fail(KB_ERR_INVALID_ARG, "map load rejected, the map is unchanged: %zu points, the counts sum to %lld",
+                    n_points, total);
+    CK(cudaSetDevice(map->ex->device));
+    DBuf<int> d_vox, d_cnt;
+    DBuf<long long> d_off;
+    DBuf<double> d_pts;
+    RET(d_vox.ensure(3 * n_voxels));
+    RET(d_cnt.ensure(n_voxels));
+    RET(d_off.ensure(n_voxels));
+    RET(d_pts.ensure(3 * n_points));
+    cudaStream_t s = map->ex->stream;
+    if (n_voxels) {
+        CK(cudaMemcpyAsync(d_vox.p, voxels, 3 * n_voxels * sizeof(int), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_cnt.p, counts, n_voxels * sizeof(int), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_off.p, off.data(), n_voxels * sizeof(long long), cudaMemcpyHostToDevice, s));
+    }
+    if (n_points) CK(cudaMemcpyAsync(d_pts.p, points, 3 * n_points * sizeof(double), cudaMemcpyHostToDevice, s));
+    return map->load(d_vox.p, d_cnt.p, d_off.p, d_pts.p, n_voxels, n_points);
+}
+int kb_map_load_dev(kb_map *map, const int *d_voxels, const int *d_counts, const double *d_points, size_t n_voxels,
+                    size_t n_points) {
+    RET(map_load_check(map, d_voxels, d_counts, d_points, n_voxels, n_points));
+    CK(cudaSetDevice(map->ex->device));
+    DBuf<long long> d_off;
+    DBuf<unsigned char> tmp;
+    RET(d_off.ensure(n_voxels));
+    if (n_voxels) {
+        // per-voxel point offsets: exclusive scan of the counts, accumulated in 64 bits (k_map_load checks them)
+        const int n = static_cast<int>(n_voxels);
+        size_t bytes = 0;
+        CK(cub::DeviceScan::ExclusiveScan(nullptr, bytes, d_counts, d_off.p, ::cuda::std::plus<>{}, 0LL, n, map->ex->stream));
+        RET(tmp.ensure(bytes));
+        CK(cub::DeviceScan::ExclusiveScan(tmp.p, bytes, d_counts, d_off.p, ::cuda::std::plus<>{}, 0LL, n, map->ex->stream));
+    }
+    return map->load(d_voxels, d_counts, d_off.p, d_points, n_voxels, n_points);
+}
 int kb_map_pointcloud(const kb_map *map, double *out_xyz, size_t capacity, size_t *n_out) {
     if (!map || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     const size_t np = static_cast<size_t>(map->h_counters[C_POINTS]);
@@ -1160,6 +1278,25 @@ int kb_threshold_update_model_deviation(kb_threshold *th, const double model_dev
         th->model_sse += model_error * model_error;
         th->num_samples++;
     }
+    return KB_OK;
+}
+// model_sse_ / num_samples_ are public in the reference (Threshold.hpp:44-46)
+static int threshold_state_check(double model_sse, int num_samples) {
+    if (!std::isfinite(model_sse) || model_sse < 0.0) return fail(KB_ERR_INVALID_ARG, "model_sse must be finite and >= 0");
+    if (num_samples < 1) return fail(KB_ERR_INVALID_ARG, "num_samples must be >= 1");
+    return KB_OK;
+}
+int kb_threshold_get_state(const kb_threshold *th, double *model_sse, int *num_samples) {
+    if (!th || !model_sse || !num_samples) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *model_sse = th->model_sse;
+    *num_samples = th->num_samples;
+    return KB_OK;
+}
+int kb_threshold_set_state(kb_threshold *th, double model_sse, int num_samples) {
+    if (!th) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(threshold_state_check(model_sse, num_samples));
+    th->model_sse = model_sse;
+    th->num_samples = num_samples;
     return KB_OK;
 }
 
@@ -1720,6 +1857,47 @@ int kb_pipeline_set_pose(kb_pipeline *p, const double pose[16]) {
 int kb_pipeline_set_delta(kb_pipeline *p, const double delta[16]) {
     if (!p || !delta) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     return pipeline_set(p, p->last.pose, delta);
+}
+// SE3 <-> Sophus::SE3d::params() {qx, qy, qz, qw, tx, ty, tz}: the layout of SE3 itself, copied bit for bit
+static void se3_to_params(const SE3 &T, double a[7]) {
+    const double v[7] = {T.q.x, T.q.y, T.q.z, T.q.w, T.t.x, T.t.y, T.t.z};
+    std::memcpy(a, v, sizeof(v));
+}
+static SE3 se3_from_params(const double a[7]) { return SE3{{a[0], a[1], a[2], a[3]}, {a[4], a[5], a[6]}}; }
+// Sophus's SO3 holds unit quaternions only (it normalises what it is given). The state is stored as given, so the
+// quaternion must already be one: |q|^2 within Sophus's epsilon of 1.
+static bool unit_quaternion(const Q4 &q) {
+    const double n2 = ((q.x * q.x + q.y * q.y) + q.z * q.z) + q.w * q.w;
+    return std::fabs(n2 - 1.0) < kEps;
+}
+int kb_pipeline_get_state(const kb_pipeline *p, kb_pipeline_state *out) {
+    if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    CK(cudaSetDevice(p->ex->device));
+    PipeState s;
+    CK(cudaMemcpyAsync(&s, p->d_state, sizeof(s), cudaMemcpyDeviceToHost, p->ex->stream));
+    RET(p->ex->sync());
+    se3_to_params(s.last_pose, out->pose);
+    se3_to_params(s.last_delta, out->delta);
+    out->model_sse = s.model_sse;
+    out->num_samples = s.num_samples;
+    return KB_OK;
+}
+int kb_pipeline_set_state(kb_pipeline *p, const kb_pipeline_state *s) {
+    if (!p || !s) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    for (int i = 0; i < 7; ++i)
+        if (!std::isfinite(s->pose[i]) || !std::isfinite(s->delta[i])) return fail(KB_ERR_INVALID_ARG, "pose / delta not finite");
+    RET(threshold_state_check(s->model_sse, s->num_samples));
+    const SE3 pose = se3_from_params(s->pose), delta = se3_from_params(s->delta);
+    if (!unit_quaternion(pose.q) || !unit_quaternion(delta.q)) return fail(KB_ERR_NOT_SE3, "quaternion is not of unit norm");
+    CK(cudaSetDevice(p->ex->device));
+    RET(pipeline_push_state(p, pose, delta, s->model_sse, s->num_samples));  // also drops a prefetched front end
+    // no frame has run since: the accessors report the restored state
+    p->has_last = false;
+    se3_to_matrix(pose, p->last.pose);
+    se3_to_matrix(delta, p->last.delta);
+    p->last.model_sse = s->model_sse;
+    p->last.num_samples = s->num_samples;
+    return KB_OK;
 }
 kb_map *kb_pipeline_voxel_map(kb_pipeline *p) { return p ? p->map : nullptr; }
 int kb_pipeline_last_sigma(const kb_pipeline *p, double *out) {

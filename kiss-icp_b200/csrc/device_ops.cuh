@@ -38,7 +38,9 @@ constexpr int BAR_ARRIVE = 32, BAR_TEAM = 64, BAR_TICKET = 96, BAR_WORDS = 128; 
 constexpr int LL_RES = 16;        // est(7) + done flag, final pose(7), spare      // est(7) t_icp(7) final(7) conv cand_total query_total ...
 
 enum Counter { C_LIVE = 0, C_TOMB = 1, C_POINTS = 2, C_STATUS = 3, C_TOUCHED = 4, C_NCOUNTERS = 8 };
-enum StatusBit { ST_TABLE_FULL = 1, ST_NEED_GROW = 2, ST_SKIPPED = 4 };
+enum StatusBit { ST_TABLE_FULL = 1, ST_NEED_GROW = 2, ST_SKIPPED = 4,
+                 // k_map_load's validation (set only in a table that is being loaded; the host discards it then)
+                 ST_LOAD_DUPLICATE = 8, ST_LOAD_COUNT = 16, ST_LOAD_NONFINITE = 32, ST_LOAD_OUTSIDE = 64 };
 
 // core/VoxelUtils.hpp:33-37 — FP64 DIVISION then floor then int cast (bit-exact with the CPU).
 // A DDIV is a long dependent instruction sequence; when voxel_size is an exact power of two (1.0, 0.5, 2.0 ...:
@@ -296,6 +298,30 @@ __device__ __forceinline__ int map_find_or_claim(const MapView &m, int x, int y,
             }
         }
         if (s.w != KB_TOMB && s.x == x && s.y == y && s.z == z) return static_cast<int>(h);
+        h = (h + 1) & m.mask;
+    }
+    atomicOr(&m.counters[C_STATUS], ST_TABLE_FULL);
+    return -1;
+}
+
+// claim for kb_map_load: like map_find_or_claim, but an existing equal key is a duplicate voxel of the input
+// (ST_LOAD_DUPLICATE, -1) instead of a slot to share
+__device__ __forceinline__ int map_claim_new(const MapView &m, int x, int y, int z) {
+    unsigned h = mix_hash(x, y, z) & m.mask;
+    const int4 empty = make_int4(-1, -1, -1, KB_EMPTY);
+    for (unsigned probes = 0; probes <= m.mask; ++probes) {
+        int4 s = m.slots[h];
+        if (s.w == KB_EMPTY) {
+            s = cas_slot(&m.slots[h], empty, make_int4(x, y, z, 0));
+            if (s.w == KB_EMPTY) {
+                atomicAdd(&m.counters[C_LIVE], 1);
+                return static_cast<int>(h);
+            }
+        }
+        if (s.w != KB_TOMB && s.x == x && s.y == y && s.z == z) {
+            atomicOr(&m.counters[C_STATUS], ST_LOAD_DUPLICATE);
+            return -1;
+        }
         h = (h + 1) & m.mask;
     }
     atomicOr(&m.counters[C_STATUS], ST_TABLE_FULL);

@@ -452,6 +452,61 @@ __global__ void k_map_rehash(const MapView from, const MapView to) {
     }
 }
 
+// kb_map_load: a map in kb_map_dump's layout into an EMPTY table, one warp per voxel (grid-stride). Every input is
+// checked here and a violation sets a ST_LOAD_* bit; the host adopts the table only when none is set. Two later
+// phases rely on every point lying inside its voxel without checking it: the eviction scan decides from the key
+// alone, and the ICP team's staged candidate lists are exact only for points inside their voxels.
+struct MapLoadParams {
+    MapView m;                 // the empty table being filled
+    const int *voxels;         // [n][3], any order
+    const int *counts;         // [n]
+    const long long *offsets;  // [n] exclusive scan of counts: first point of each voxel
+    const double *points;      // [n_points][3], concatenated per voxel in insertion order
+    size_t n, n_points;
+};
+__global__ void k_map_load(const MapLoadParams P) {
+    const int lane = threadIdx.x & 31;
+    const size_t gw = (blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x) >> 5;
+    const size_t nw = (static_cast<size_t>(gridDim.x) * blockDim.x) >> 5;
+    const size_t cap3 = static_cast<size_t>(P.m.cap) * 3;
+    const long long np = static_cast<long long>(P.n_points);
+    for (size_t v = gw; v < P.n; v += nw) {
+        const int x = P.voxels[3 * v], y = P.voxels[3 * v + 1], z = P.voxels[3 * v + 2];
+        const int c = P.counts[v];
+        const long long off = P.offsets[v];
+        // the count bounds the block, the block must lie inside the points, and the last one must end where they do
+        // (the offsets of kb_map_load_dev come from counts nobody has checked yet)
+        if (c < 1 || c > P.m.cap || off < 0 || off + c > np || (v + 1 == P.n && off + c != np)) {
+            if (lane == 0) atomicOr(&P.m.counters[C_STATUS], ST_LOAD_COUNT);
+            continue;
+        }
+        int d = 0;
+        if (lane == 0) d = map_claim_new(P.m, x, y, z);
+        d = __shfl_sync(FULL, d, 0);
+        if (d < 0) continue;
+        const double *a = P.points + static_cast<size_t>(off) * 3;
+        double *b = P.m.points + static_cast<size_t>(d) * cap3;
+        int bad = 0;
+        for (int k = lane; k < c; k += 32) {
+            const double px = a[3 * k], py = a[3 * k + 1], pz = a[3 * k + 2];
+            if (!(isfinite(px) && isfinite(py) && isfinite(pz))) {
+                bad |= ST_LOAD_NONFINITE;
+            } else {
+                const int3 q = point_to_voxel(px, py, pz, P.m.vdiv);  // the hot path's own voxel function
+                if (q.x != x || q.y != y || q.z != z) bad |= ST_LOAD_OUTSIDE;
+            }
+            b[3 * k] = px;
+            b[3 * k + 1] = py;
+            b[3 * k + 2] = pz;
+        }
+        if (bad) atomicOr(&P.m.counters[C_STATUS], bad);
+        if (lane == 0) {
+            P.m.slots[d].w = c;
+            atomicAdd(&P.m.counters[C_POINTS], c);
+        }
+    }
+}
+
 // batched GetClosestNeighbor (VoxelHashMap.cpp:46-70): one warp per query, grid-stride.
 // Bandwidth-bound at scale (BASELINE config 5): every query is three dependent DRAM round trips
 // (query, 27 slot probes, candidate blocks), so the kernel is built for memory-level parallelism:

@@ -10,16 +10,63 @@ Two execution modes:
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import numpy as np
 
 from . import _native as N
 from .config import KISSConfig, load_config
-from .mapping import VoxelHashMap, get_voxel_hash_map
+from .mapping import VoxelHashMap, check_value, get_voxel_hash_map
 from .preprocess import get_preprocessor
 from .registration import get_registration
-from .threshold import get_threshold_estimator
+from .threshold import AdaptiveThreshold, get_threshold_estimator
 from .voxelization import voxel_down_sample
+
+STATE_FORMAT_VERSION = 1  # of KissICP.state_dict()
+
+
+def se3_params_from_matrix(T) -> np.ndarray:
+    """4x4 SE(3) -> {qx,qy,qz,qw,tx,ty,tz}, the quaternion exactly as the library computes it from a matrix
+    (Eigen's Quaterniond(Matrix3d); se3.cuh q_from_matrix, same operations in the same order)"""
+    m = [[float(T[i][j]) for j in range(3)] for i in range(3)]
+    c = [0.0] * 4
+    t = m[0][0] + m[1][1] + m[2][2]
+    if t > 0.0:
+        t = math.sqrt(t + 1.0)
+        c[3] = 0.5 * t
+        t = 0.5 / t
+        c[0] = (m[2][1] - m[1][2]) * t
+        c[1] = (m[0][2] - m[2][0]) * t
+        c[2] = (m[1][0] - m[0][1]) * t
+    else:
+        i = 0
+        if m[1][1] > m[0][0]:
+            i = 1
+        if m[2][2] > m[i][i]:
+            i = 2
+        j = (i + 1) % 3
+        k = (j + 1) % 3
+        t = math.sqrt(m[i][i] - m[j][j] - m[k][k] + 1.0)
+        c[i] = 0.5 * t
+        t = 0.5 / t
+        c[3] = (m[k][j] - m[j][k]) * t
+        c[j] = (m[j][i] + m[i][j]) * t
+        c[k] = (m[k][i] + m[i][k]) * t
+    return np.array(c + [float(T[0][3]), float(T[1][3]), float(T[2][3])])
+
+
+def _params_arg(a):
+    a = np.asarray(a, dtype=np.float64).reshape(-1)
+    if a.shape != (7,):
+        raise ValueError("an SE(3) parameter vector has 7 values {qx,qy,qz,qw,tx,ty,tz}")
+    return a
+
+
+def _pose_arg(T):
+    a = np.array(T, dtype=np.float64)
+    if a.shape != (4, 4) or not np.isfinite(a).all():
+        raise ValueError("a pose is a finite 4x4 matrix")
+    return a
 
 
 class _PipelineThreshold:
@@ -230,6 +277,88 @@ class KissICP:
         self._last_delta = np.linalg.inv(self._last_pose) @ new_pose
         self._last_pose = new_pose
         return frame, source
+
+    # -- checkpoint / restore -----------------------------------------------------------------------
+    def state_dict(self):
+        """The sequence's whole state as a dict of numpy arrays (it survives np.savez / np.load):
+        format_version; the config fields; pose_qt, delta_qt (Sophus::SE3d::params() order {qx,qy,qz,qw,tx,ty,tz})
+        and pose, delta (4x4); the adaptive threshold's model_sse, num_samples (NaN and 0 under a fixed threshold);
+        the map as voxels, counts, points (VoxelHashMap.dump()).
+
+        The fused pipeline's pose and delta are the device's quaternions and translations, bit for bit. In modular
+        mode the 4x4 matrices are the state and pose_qt / delta_qt are derived from them."""
+        c = self.config
+        fixed = c.adaptive_threshold.fixed_threshold
+        d = {"format_version": np.array(STATE_FORMAT_VERSION),
+             "voxel_size": np.array(float(c.mapping.voxel_size)), "max_range": np.array(float(c.data.max_range)),
+             "min_range": np.array(float(c.data.min_range)), "deskew": np.array(bool(c.data.deskew)),
+             "max_points_per_voxel": np.array(int(c.mapping.max_points_per_voxel)),
+             "max_num_iterations": np.array(int(c.registration.max_num_iterations)),
+             "convergence_criterion": np.array(float(c.registration.convergence_criterion)),
+             "initial_threshold": np.array(float(c.adaptive_threshold.initial_threshold)),
+             "min_motion_th": np.array(float(c.adaptive_threshold.min_motion_th)),
+             "fixed_threshold": np.array(np.nan if fixed is None else float(fixed))}
+        if self.fused:
+            s = N.PipelineState()
+            N.check(N.lib().kb_pipeline_get_state(self._h, C.byref(s)))
+            pose_qt, delta_qt = np.array(s.pose[:]), np.array(s.delta[:])
+            pose, delta, sse, ns = self.last_pose, self.last_delta, s.model_sse, s.num_samples
+        else:
+            pose, delta = np.array(self._last_pose, dtype=np.float64), np.array(self._last_delta, dtype=np.float64)
+            pose_qt, delta_qt = se3_params_from_matrix(pose), se3_params_from_matrix(delta)
+            sse, ns = (np.nan, 0)  # a fixed threshold has no state
+            if isinstance(self.adaptive_threshold, AdaptiveThreshold):
+                sse, ns = self.adaptive_threshold.get_state()
+        vox, cnt, pts = self.local_map.dump()
+        d.update(pose_qt=pose_qt, delta_qt=delta_qt, pose=pose, delta=delta, model_sse=np.array(float(sse)),
+                 num_samples=np.array(int(ns)), voxels=vox, counts=cnt, points=pts)
+        return d
+
+    def load_state_dict(self, state):
+        """Restore a state_dict() taken in either mode (or an equivalent dict of the oracle's state), all or nothing: on ValueError
+        nothing has changed.
+
+        voxel_size and max_points_per_voxel must equal this pipeline's (ValueError otherwise): the map's voxels
+        and its per-voxel cap depend on them. Every other config field of the dict is ignored; the receiving
+        pipeline keeps its own (max_range, thresholds, iterations ...). A fused pipeline restores pose and delta
+        from pose_qt / delta_qt, exactly; modular mode takes the 4x4 pose / delta. A fixed threshold has no state
+        and ignores model_sse / num_samples; an adaptive one rejects NaN, negative model_sse and num_samples < 1."""
+        d = {k: np.asarray(v) for k, v in state.items()}
+        if int(d["format_version"]) != STATE_FORMAT_VERSION:
+            raise ValueError(f"state format {int(d['format_version'])}, expected {STATE_FORMAT_VERSION}")
+        c = self.config
+        if float(d["voxel_size"]) != float(c.mapping.voxel_size) or \
+                int(d["max_points_per_voxel"]) != int(c.mapping.max_points_per_voxel):
+            raise ValueError(f"state of a map with voxel_size {float(d['voxel_size'])}, max_points_per_voxel "
+                             f"{int(d['max_points_per_voxel'])}; this pipeline has {c.mapping.voxel_size}, "
+                             f"{c.mapping.max_points_per_voxel}")
+        sse, ns = float(d["model_sse"]), int(d["num_samples"])
+        load_map = lambda: self.local_map.load(d["voxels"], d["counts"], d["points"])
+        if self.fused:
+            new, old = N.PipelineState(), N.PipelineState()
+            new.pose[:] = [float(x) for x in _params_arg(d["pose_qt"])]
+            new.delta[:] = [float(x) for x in _params_arg(d["delta_qt"])]
+            new.model_sse, new.num_samples = sse, ns
+            N.check(N.lib().kb_pipeline_get_state(self._h, C.byref(old)))
+            check_value(N.lib().kb_pipeline_set_state(self._h, C.byref(new)))
+            try:
+                load_map()
+            except Exception:
+                N.check(N.lib().kb_pipeline_set_state(self._h, C.byref(old)))
+                raise
+            return
+        pose, delta = _pose_arg(d["pose"]), _pose_arg(d["delta"])
+        if isinstance(self.adaptive_threshold, AdaptiveThreshold):
+            old = self.adaptive_threshold.get_state()
+            self.adaptive_threshold.set_state(sse, ns)
+            try:
+                load_map()
+            except Exception:
+                self.adaptive_threshold.set_state(*old)
+                raise
+        else:
+            load_map()
+        self._last_pose, self._last_delta = pose, delta
 
     def voxelize(self, iframe):
         if self.fused:

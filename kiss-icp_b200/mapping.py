@@ -10,6 +10,24 @@ from . import _native as N
 from .config import KISSConfig
 
 
+def check_value(status: int):
+    """N.check, except that a rejected argument (KB_ERR_INVALID_ARG) raises ValueError: the checkpoint loads report
+    bad input the way numpy and the reference's Python do"""
+    if status == N.KB_ERR_INVALID_ARG:
+        raise ValueError(N.lib().kb_last_error().decode())
+    N.check(status)
+
+
+def _int32_arg(a, name):
+    a = np.asarray(a)
+    if a.size and a.dtype.kind not in "iu":
+        raise ValueError(f"{name} must be integers")
+    b = np.ascontiguousarray(a, dtype=np.int32)
+    if not np.array_equal(a, b):
+        raise ValueError(f"{name} out of int32 range")
+    return b
+
+
 def get_voxel_hash_map(config: KISSConfig):
     return VoxelHashMap(
         voxel_size=config.mapping.voxel_size,
@@ -95,6 +113,17 @@ class VoxelHashMap:
         a, b = N.sz(0), N.sz(0)
         N.check(N.lib().kb_map_dump(self._h, N.ptr(vox), N.ptr(cnt), N.ptr(pts), nv, npnt, C.byref(a), C.byref(b)))
         return vox, cnt, pts
+
+    def load(self, voxels, counts, points):
+        """The inverse of dump(): replace the map's contents with (voxels (V,3), counts (V,), points (P,3)); the
+        voxels may come in any order. Validated on the device and all or nothing: a duplicate voxel, a count outside
+        [1, max_points_per_voxel], P != counts.sum(), a non-finite coordinate or a point outside the voxel it is
+        listed under raises ValueError and leaves the map as it was."""
+        vox, cnt = _int32_arg(voxels, "voxels"), _int32_arg(counts, "counts")
+        pts = np.ascontiguousarray(points, dtype=np.float64)
+        if vox.ndim != 2 or vox.shape[1] != 3 or cnt.shape != (len(vox),) or pts.ndim != 2 or pts.shape[1] != 3:
+            raise ValueError("expected voxels (V, 3), counts (V,) and points (P, 3)")
+        check_value(N.lib().kb_map_load(self._h, N.ptr(vox), N.ptr(cnt), N.ptr(pts), len(vox), len(pts)))
 
     def closest_neighbors(self, queries):
         """batched VoxelHashMap::GetClosestNeighbor (VoxelHashMap.cpp:46-70)."""

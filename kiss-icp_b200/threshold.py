@@ -7,6 +7,7 @@ import numpy as np
 
 from . import _native as N
 from .config import KISSConfig
+from .mapping import check_value
 
 
 def get_threshold_estimator(config: KISSConfig):
@@ -47,3 +48,13 @@ class AdaptiveThreshold:
     def update_model_deviation(self, model_deviation: np.ndarray):
         T = N.mat4_arg(model_deviation)
         N.check(N.lib().kb_threshold_update_model_deviation(self._h, N.ptr(T)))
+
+    def get_state(self):
+        """(model_sse, num_samples): AdaptiveThreshold::model_sse_ / num_samples_ (Threshold.hpp:44-46)"""
+        s, n = N.dbl(0), N.i32(0)
+        N.check(N.lib().kb_threshold_get_state(self._h, C.byref(s), C.byref(n)))
+        return s.value, n.value
+
+    def set_state(self, model_sse: float, num_samples: int):
+        """ValueError for a non-finite or negative model_sse or num_samples < 1"""
+        check_value(N.lib().kb_threshold_set_state(self._h, float(model_sse), int(num_samples)))
