@@ -123,6 +123,27 @@ int kb_registration_last_iterations(const kb_registration *reg, int *out);
 int kb_registration_build_system(kb_registration *reg, const double *xyz, size_t n, const kb_map *map,
                                  double max_correspondence_distance, double kernel_scale, double JTJ[36],
                                  double JTr[6], int *n_correspondences);
+/* B independent AlignPointsToMap problems against one map (Registration.cpp:138-167 each) in one call; no reference
+ * counterpart (its Python layer loops). Hypothesis b aligns xyz[offset[b] .. offset[b] + count[b]) from
+ * initial_guesses[b] (row-major 4x4) with max_correspondence_distance[b] and kernel_scale[b]. Ranges may overlap or
+ * repeat, so one cloud can be tried from many guesses without copying it. Out: poses[b][16], iterations[b], and
+ * inliers[b] (may be NULL): the n_correspondences kb_registration_build_system reports for the source mapped by
+ * poses[b]. Each hypothesis gives, bit for bit, the pose and iteration count of kb_registration_align_points_to_map
+ * on it alone; the hypotheses run side by side on teams of CTAs of one launch. Every argument is checked before any
+ * work starts: KB_ERR_NOT_SE3 for a guess that is not in SE(3), KB_ERR_INVALID_ARG for a range outside
+ * [0, n_points) or a NULL pointer; on error no output is written. B = 0 does nothing. The host form leaves
+ * kb_registration_last_iterations at iterations[B - 1], like a loop of single calls. */
+int kb_registration_align_batch(kb_registration *reg, const double *xyz, size_t n_points, const size_t *offset,
+                                const size_t *count, size_t B, const kb_map *map, const double *initial_guesses,
+                                const double *max_correspondence_distance, const double *kernel_scale, double *poses,
+                                int *iterations, int *inliers);
+/* same with every array (points, ranges, guesses, scalars, outputs) in device memory on the map's device. The ranges,
+ * guesses and scalars are read back first (one small synchronous copy: the launch is planned on the host); the
+ * alignment itself is asynchronous on the map's stream (kb_map_sync). kb_registration_last_iterations is unchanged. */
+int kb_registration_align_batch_dev(kb_registration *reg, const double *d_xyz, size_t n_points, const size_t *d_offset,
+                                    const size_t *d_count, size_t B, const kb_map *map, const double *d_initial_guesses,
+                                    const double *d_max_correspondence_distance, const double *d_kernel_scale,
+                                    double *d_poses, int *d_iterations, int *d_inliers);
 
 /* ---- kiss_icp::Preprocessor (cpp/kiss_icp/core/Preprocessing.hpp:32-45) ----------------- */
 int kb_preprocessor_create(double max_range, double min_range, int deskew, int max_num_threads,

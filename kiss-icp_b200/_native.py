@@ -118,6 +118,8 @@ SIGNATURES = {
     "kb_registration_align_points_to_map": (i32, [vp, vp, sz, vp, vp, dbl, dbl, vp]),
     "kb_registration_last_iterations": (i32, [vp, C.POINTER(i32)]),
     "kb_registration_build_system": (i32, [vp, vp, sz, vp, dbl, dbl, vp, vp, C.POINTER(i32)]),
+    "kb_registration_align_batch": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp]),
+    "kb_registration_align_batch_dev": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp]),
     "kb_preprocessor_create": (i32, [dbl, dbl, i32, i32, C.POINTER(vp)]),
     "kb_preprocessor_destroy": (i32, [vp]),
     "kb_preprocessor_preprocess": (i32, [vp, vp, sz, vp, sz, vp, vp, sz, C.POINTER(sz)]),

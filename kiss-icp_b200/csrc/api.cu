@@ -134,6 +134,13 @@ struct Exec {
     bool bar_dirty = true;  // the barrier words may be non-zero (a kernel without Grid::finish() ran last)
     std::vector<const void *> smem_opted;  // kernels opted in to > 48 KB of dynamic shared memory on THIS context's device
     unsigned next_tag_base() { return (++tag_seq) << 13; }  // 8192 epochs per launch
+    // a launch that uses more epochs (k_icp_batch) takes as many consecutive 8192-epoch blocks as it needs
+    unsigned reserve_tags(size_t epochs) {
+        const unsigned first = tag_seq + 1;
+        tag_seq += static_cast<unsigned>((epochs + 8191) / 8192);
+        return first << 13;
+    }
+    DBuf<uint4> batch_ll;  // all-gather regions of k_icp_batch's slots (allocated by the first batch call)
 
     int init() {
         if (device_count() <= 0) return fail(KB_ERR_NO_DEVICE, "no CUDA device visible (this library has no CPU fallback)");
@@ -677,6 +684,10 @@ struct kb_registration {
     DBuf<double> out;  // pose[16] + sys[NACC]
     DBuf<int> iout;    // iters, ncorr
     int last_iters = 0;
+    DBuf<BatchHyp> bhyp;  // kb_registration_align_batch: team hypotheses, then all hypotheses (inlier pass)
+    DBuf<unsigned> bctl;
+    DBuf<double> bpose;   // outputs of the host entry point
+    DBuf<int> biout;
 };
 
 struct kb_preprocessor {
@@ -1187,6 +1198,182 @@ int kb_registration_build_system(kb_registration *reg, const double *xyz, size_t
     for (int i = 0; i < 6; ++i) JTr[i] = sys[10 + i];
     if (n_correspondences) *n_correspondences = nc;
     return KB_OK;
+}
+
+// kb_registration_align_batch[_dev]. The ranges, guesses and scalars are on the host here (already checked); the points
+// and the outputs are on the device. A hypothesis runs where kb_registration_align_points_to_map would run it: on a
+// team of k_icp_batch when k_icp would give it a team, otherwise as its own k_icp launch on the same stream.
+static int align_batch_check(const kb_registration *reg, const kb_map *map, const double *xyz, size_t n_points,
+                             const size_t *offset, const size_t *count, size_t B, const double *guesses,
+                             const double *max_dist, const double *kscale, const double *poses, const int *iterations,
+                             std::vector<SE3> *g) {
+    if (!reg || !map) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (B == 0) return KB_OK;
+    if (!offset || !count || !guesses || !max_dist || !kscale || !poses || !iterations || (!xyz && n_points))
+        return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (B > static_cast<size_t>(INT_MAX)) return fail(KB_ERR_INVALID_ARG, "too many hypotheses (%zu)", B);
+    size_t total = 0;
+    for (size_t b = 0; b < B; ++b) {
+        if (offset[b] > n_points || count[b] > n_points - offset[b])
+            return fail(KB_ERR_INVALID_ARG, "hypothesis %zu: points [%zu, %zu + %zu) outside [0, %zu)", b, offset[b], offset[b],
+                        count[b], n_points);
+        total += count[b];
+        if (total > static_cast<size_t>(INT_MAX)) return fail(KB_ERR_INVALID_ARG, "more than 2^31 - 1 source points in all");
+    }
+    g->resize(B);
+    for (size_t b = 0; b < B; ++b)
+        if (!to_se3(guesses + 16 * b, &(*g)[b])) return fail(KB_ERR_NOT_SE3, "initial_guesses[%zu] is not in SE(3)", b);
+    return KB_OK;
+}
+static int align_batch_run(kb_registration *reg, kb_map *map, const double *d_xyz, const size_t *offset, const size_t *count,
+                           size_t B, const std::vector<SE3> &g, const double *max_dist, const double *kscale,
+                           double *d_poses, int *d_iters, int *d_inliers) {
+    Exec &ex = *map->ex;
+    CK(cudaSetDevice(ex.device));
+    int live = 0;  // (the host's copy of the counters can be behind a pipeline's map)
+    CK(cudaMemcpyAsync(&live, map->counters + C_LIVE, sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
+    RET(ex.sync());
+    const MapView mv = map->view();
+    // k_icp's choice of the team path (kernels.cuh), made here per hypothesis
+    const bool team_ok = live != 0 && reg->max_iter > 0 && ex.icp_team_q > 0 && mv.cap <= NN_FLAT_CAP &&
+                         (static_cast<unsigned long long>(mv.mask) + 1) * mv.cap < (1ull << 31);
+    std::vector<BatchHyp> hyp;  // the team hypotheses, then all of them (inlier pass)
+    std::vector<size_t> single;
+    int t_max = 0, n_team = 0, n_all = 0;
+    size_t n_single = 1;
+    for (size_t b = 0; b < B; ++b) {
+        const int n = static_cast<int>(count[b]);
+        const int T = team_ok ? icp_team_size(n, ex.icp_team_q, ex.grid, ex.team.smem_bytes) : 0;
+        if (T > 0) {
+            hyp.push_back(BatchHyp{g[b], max_dist[b], kscale[b], static_cast<long long>(offset[b]), n, T, n_team, static_cast<int>(b)});
+            n_team += n;
+            t_max = std::max(t_max, T);
+        } else {
+            single.push_back(b);
+            n_single = std::max(n_single, count[b]);
+        }
+    }
+    const int nh = static_cast<int>(hyp.size());
+    for (size_t b = 0; b < B; ++b) {
+        hyp.push_back(BatchHyp{g[b], max_dist[b], kscale[b], static_cast<long long>(offset[b]), static_cast<int>(count[b]), 0, n_all,
+                               static_cast<int>(b)});
+        n_all += static_cast<int>(count[b]);
+    }
+    RET(reg->bhyp.ensure(hyp.size()));
+    CK(cudaMemcpyAsync(reg->bhyp.p, hyp.data(), hyp.size() * sizeof(BatchHyp), cudaMemcpyHostToDevice, ex.stream));
+    RET(reg->ws.qrec.ensure(std::max<size_t>(n_single, static_cast<size_t>(n_team))));
+    if (!single.empty()) RET(reg->ws.work.ensure(3 * n_single));
+    for (size_t b : single) {
+        IcpParams P{};
+        P.m = mv;
+        P.sc = ex.sc;
+        P.src = d_xyz + 3 * offset[b];
+        P.work = reg->ws.work.p;
+        P.n = static_cast<int>(count[b]);
+        P.guess = g[b];
+        P.max_dist = max_dist[b];
+        P.kscale = kscale[b];
+        P.max_iter = reg->max_iter;
+        P.conv = reg->conv;
+        P.out_pose = d_poses + 16 * b;
+        P.out_iters = d_iters + b;
+        P.use_qcache = 1;
+        P.tag_base = ex.next_tag_base();
+        P.team = ex.team;
+        P.team.qrec = reg->ws.qrec.p;
+        P.icp_team_q = ex.icp_team_q;
+        RET(ex.coop(k_icp, P, std::max<size_t>(QC_BYTES, ex.icp_smem)));
+    }
+    if (nh > 0) {
+        const int slots = ex.grid / t_max;
+        const size_t region = static_cast<size_t>(slots) * 2 * t_max * t_max * NPART;
+        const size_t had = ex.batch_ll.n;
+        RET(ex.batch_ll.ensure(region));
+        if (ex.batch_ll.n != had) CK(cudaMemsetAsync(ex.batch_ll.p, 0, ex.batch_ll.n * sizeof(uint4), ex.stream));
+        RET(reg->bctl.ensure(bctl_words(slots)));
+        CK(cudaMemsetAsync(reg->bctl.p, 0, bctl_words(slots) * sizeof(unsigned), ex.stream));
+        IcpBatchParams P{};
+        P.m = mv;
+        P.sc = ex.sc;
+        P.sc.profile = 0;  // (the profiling stamps belong to single launches)
+        P.team = ex.team;
+        P.team.ll = ex.batch_ll.p;
+        P.team.qrec = reg->ws.qrec.p;
+        P.src = d_xyz;
+        P.hyp = reg->bhyp.p;
+        P.nh = nh;
+        P.n_total = n_team;
+        P.t_max = t_max;
+        P.slots = slots;
+        P.max_iter = reg->max_iter;
+        P.conv = reg->conv;
+        P.tag_base = ex.reserve_tags(static_cast<size_t>(nh) * (static_cast<size_t>(reg->max_iter) + 1) + 1);
+        P.ctl = reg->bctl.p;
+        P.out_pose = d_poses;
+        P.out_iters = d_iters;
+        RET(ex.coop(k_icp_batch, P, std::max<size_t>(QC_BYTES, ex.icp_smem)));
+    }
+    if (d_inliers) {
+        CK(cudaMemsetAsync(d_inliers, 0, B * sizeof(int), ex.stream));
+        if (n_all > 0) {
+            const int blocks = static_cast<int>(std::min<size_t>(static_cast<size_t>(ex.grid) * 8, (static_cast<size_t>(n_all) + 7) / 8));
+            k_align_inliers<<<blocks, 256, 0, ex.stream>>>(mv, d_xyz, reg->bhyp.p + nh, static_cast<int>(B), n_all, d_poses, d_inliers);
+            ++ex.launches;
+            CK(cudaGetLastError());
+        }
+    }
+    return KB_OK;
+}
+int kb_registration_align_batch(kb_registration *reg, const double *xyz, size_t n_points, const size_t *offset,
+                                const size_t *count, size_t B, const kb_map *cmap, const double *initial_guesses,
+                                const double *max_correspondence_distance, const double *kernel_scale, double *poses,
+                                int *iterations, int *inliers) {
+    kb_map *map = const_cast<kb_map *>(cmap);
+    std::vector<SE3> g;
+    RET(align_batch_check(reg, map, xyz, n_points, offset, count, B, initial_guesses, max_correspondence_distance,
+                          kernel_scale, poses, iterations, &g));
+    if (B == 0) return KB_OK;
+    Exec &ex = *map->ex;
+    CK(cudaSetDevice(ex.device));
+    RET(reg->ws.src.ensure(3 * std::max<size_t>(n_points, 1)));
+    RET(reg->bpose.ensure(16 * B));
+    RET(reg->biout.ensure(2 * B));
+    if (n_points) CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n_points * 24, cudaMemcpyHostToDevice, ex.stream));
+    RET(align_batch_run(reg, map, reg->ws.src.p, offset, count, B, g, max_correspondence_distance, kernel_scale, reg->bpose.p,
+                        reg->biout.p, inliers ? reg->biout.p + B : nullptr));
+    CK(cudaMemcpyAsync(poses, reg->bpose.p, 16 * B * sizeof(double), cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(iterations, reg->biout.p, B * sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
+    if (inliers) CK(cudaMemcpyAsync(inliers, reg->biout.p + B, B * sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
+    RET(ex.sync());
+    reg->last_iters = iterations[B - 1];
+    return KB_OK;
+}
+int kb_registration_align_batch_dev(kb_registration *reg, const double *d_xyz, size_t n_points, const size_t *d_offset,
+                                    const size_t *d_count, size_t B, const kb_map *cmap, const double *d_initial_guesses,
+                                    const double *d_max_correspondence_distance, const double *d_kernel_scale,
+                                    double *d_poses, int *d_iterations, int *d_inliers) {
+    kb_map *map = const_cast<kb_map *>(cmap);
+    if (!reg || !map) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (B == 0) return KB_OK;
+    if (!d_offset || !d_count || !d_initial_guesses || !d_max_correspondence_distance || !d_kernel_scale || !d_poses ||
+        !d_iterations || (!d_xyz && n_points))
+        return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (B > static_cast<size_t>(INT_MAX)) return fail(KB_ERR_INVALID_ARG, "too many hypotheses (%zu)", B);
+    // the launch is planned on the host: the ranges, guesses and scalars come back first (the points stay)
+    Exec &ex = *map->ex;
+    CK(cudaSetDevice(ex.device));
+    std::vector<size_t> off(B), cnt(B);
+    std::vector<double> gs(16 * B), md(B), ks(B);
+    CK(cudaMemcpyAsync(off.data(), d_offset, B * sizeof(size_t), cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(cnt.data(), d_count, B * sizeof(size_t), cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(gs.data(), d_initial_guesses, 16 * B * sizeof(double), cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(md.data(), d_max_correspondence_distance, B * sizeof(double), cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(ks.data(), d_kernel_scale, B * sizeof(double), cudaMemcpyDeviceToHost, ex.stream));
+    RET(ex.sync());
+    std::vector<SE3> g;
+    RET(align_batch_check(reg, map, d_xyz, n_points, off.data(), cnt.data(), B, gs.data(), md.data(), ks.data(), d_poses,
+                          d_iterations, &g));
+    return align_batch_run(reg, map, d_xyz, off.data(), cnt.data(), B, g, md.data(), ks.data(), d_poses, d_iterations, d_inliers);
 }
 
 // ------------------------------------------------------------------------------- Preprocessor

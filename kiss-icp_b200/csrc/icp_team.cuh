@@ -102,7 +102,8 @@ struct TeamScratch {
 };
 
 // team size for n source points at q_per_cta points per CTA; 0 when the lists would not fit in shared memory
-__device__ __forceinline__ int icp_team_size(int n, int q_per_cta, int grid, int smem_bytes) {
+// (also called on the host: kb_registration_align_batch plans its teams with it)
+__host__ __device__ __forceinline__ int icp_team_size(int n, int q_per_cta, int grid, int smem_bytes) {
     q_per_cta = max(1, min(q_per_cta, TQ_MAX));
     const int tmax = min(grid, TEAM_MAX);
     if ((n + q_per_cta - 1) / q_per_cta > tmax) q_per_cta = (n + tmax - 1) / tmax;  // small grid (several pipelines per GPU) / big cloud: fuller CTAs
@@ -471,9 +472,10 @@ __device__ __noinline__ void team_refill(Shared &sh, const MapView &m, const Tea
 // when d_S < voxel_size - R (its minimiser is then within one voxel of p, i.e. inside the current neighbourhood).
 // Otherwise (moved > R, or a far match that changed voxel) the point is queued and searched again by a whole warp —
 // ALL warps of the CTA serve that queue.
+template <bool kSlot>
 __device__ __forceinline__ void team_queries(uint4 *ll, Shared &sh, const MapView &m, const TeamSmem sm, const VoxelDiv vdiv, double radius_frac, int nq, int j,
                                           double max_dist, double kscale, int member, int T, unsigned tag,
-                                          unsigned long long *dbg) {
+                                          unsigned long long *dbg, int stride) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int l4 = lane & (TQ_LANES - 1), li = tid / TQ_LANES;
     const double voxel_size = vdiv.v;
@@ -641,7 +643,16 @@ __device__ __forceinline__ void team_queries(uint4 *ll, Shared &sh, const MapVie
     __syncthreads();
     // one copy per reader, all threads storing (21 lanes doing the T rows one after the other is a long serial chain):
     // element e = reader * 21 + value -> row [reader][member], 21 consecutive 16-byte chunks
-    {
+    // (the launch team's region is indexed with the constant TEAM_MAX: a runtime stride changes k_register_frame's code)
+    if constexpr (kSlot) {
+        uint4 *dst = ll + (static_cast<size_t>(tag & 1u) * stride * stride + member) * NPART;
+        const int val = lane;
+        if (val < NPART) {
+            const double v = sh.red[val];
+            for (int reader = warp; reader < T; reader += NWARPS)
+                ll_store(dst + static_cast<size_t>(reader) * stride * NPART + val, v, tag);
+        }
+    } else {
         uint4 *dst = ll + (static_cast<size_t>(tag & 1u) * TEAM_MAX * TEAM_MAX + member) * NPART;
         // thread -> (value = tid % 32 if < 21, readers tid / 32, tid / 32 + 16, ...): a warp stores one reader's row at a time
         const int val = lane;
@@ -660,10 +671,12 @@ __device__ __forceinline__ void team_queries(uint4 *ll, Shared &sh, const MapVie
 // Reader: thread t polls chunks t, t + 512, ... of its T x 21 (a two-line loop: the iteration's code has to stay small)
 // and drops the values into shared memory; after one barrier 21 lanes of warp 15 add the members in order (the same
 // bits in every team CTA) and its last lane solves.
-__device__ __forceinline__ void team_gather(const uint4 *ll, Shared &sh, int T, unsigned tag) {
+template <bool kSlot>
+__device__ __forceinline__ void team_gather(const uint4 *ll, Shared &sh, int T, unsigned tag, int member, int stride) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     double *g = reinterpret_cast<double *>(sh.chunk_pref);  // [T][NPART] (the reduction scratch is done with)
-    const uint4 *base = ll + (static_cast<size_t>(tag & 1u) * TEAM_MAX + blockIdx.x) * TEAM_MAX * NPART;  // my private copy
+    const unsigned me = kSlot ? static_cast<unsigned>(member) : blockIdx.x;
+    const uint4 *base = ll + (static_cast<size_t>(tag & 1u) * stride + me) * stride * NPART;  // my private copy
     const int total = T * NPART;
     unsigned spins = 0;
 #pragma unroll 1
@@ -728,12 +741,18 @@ __device__ __forceinline__ void team_solve(Shared &sh, double conv, bool last_al
     sh.flag = (conv_reached || last_allowed) ? 1 : 0;
 }
 
-// the iterations, on CTAs [0, T) of the launch. Precondition: icp_fill_pass + a grid barrier, map not empty,
-// max_iter > 0, T = icp_team_size(...) > 0. Output in sh.result / sh.iters / sh.cand_total / ... of every team CTA.
-__device__ __noinline__ void op_icp_team(const TeamScratch &ts, const Scratch &sc, Shared &sh, const MapView &m, int n,
-                                         const SE3 &guess, double max_dist, double kscale, int max_iter, double conv,
-                                         unsigned char *dyn_smem, int T, unsigned tag_base) {
-    const int member = static_cast<int>(blockIdx.x);
+// the iterations, on a team of T CTAs. Precondition: icp_fill_pass + a grid barrier, map not empty, max_iter > 0,
+// T = icp_team_size(...) > 0. Output in sh.result / sh.iters / sh.cand_total / ... of every team CTA.
+// kSlot = false: the team is CTAs [0, T) of the launch and ts.ll is sized for TEAM_MAX CTAs (k_register_frame, k_icp).
+// kSlot = true: this CTA is member `slot_member` of a slot of k_icp_batch whose all-gather region ts.ll holds
+// [2][slot_stride][slot_stride][NPART] chunks (slot_stride >= T).
+template <bool kSlot>
+__device__ __forceinline__ void icp_team_iterate(const TeamScratch &ts, const Scratch &sc, Shared &sh, const MapView &m, int n,
+                                                 const SE3 &guess, double max_dist, double kscale, int max_iter, double conv,
+                                                 unsigned char *dyn_smem, int T, unsigned tag_base, int slot_member,
+                                                 int slot_stride) {
+    const int member = kSlot ? slot_member : static_cast<int>(blockIdx.x);
+    const int stride = kSlot ? slot_stride : TEAM_MAX;
     const int nq = member < n ? (n - member + T - 1) / T : 0;
     const TeamSmem sm = team_smem(dyn_smem, ts.smem_bytes, (n + T - 1) / T);
     const VoxelDiv vdiv = m.vdiv;  // (by value into the iteration: `m` itself sits in the kernel's local copy of its parameters)
@@ -776,11 +795,11 @@ __device__ __noinline__ void op_icp_team(const TeamScratch &ts, const Scratch &s
         if (stamp) sc.dbg[64 + 4 * member] = globaltimer_ns();
 #endif
         KB_TCYC(0);
-        team_queries(ll, sh, m, sm, vdiv, ts.radius_frac, nq, j, max_dist, kscale, member, T, tag, dbg);
+        team_queries<kSlot>(ll, sh, m, sm, vdiv, ts.radius_frac, nq, j, max_dist, kscale, member, T, tag, dbg, stride);
 #ifdef KB_PROFILE_TEAM
         if (stamp) sc.dbg[64 + 4 * member + 1] = globaltimer_ns();
 #endif
-        team_gather(ll, sh, T, tag);  // (warp 15 holds the sums: no barrier between them and its solver lane)
+        team_gather<kSlot>(ll, sh, T, tag, member, stride);  // (warp 15 holds the sums: no barrier between them and its solver lane)
 #ifdef KB_PROFILE_TEAM
         if (stamp) sc.dbg[64 + 4 * member + 2] = globaltimer_ns();
 #endif
@@ -798,6 +817,18 @@ __device__ __noinline__ void op_icp_team(const TeamScratch &ts, const Scratch &s
         sh.query_total = static_cast<double>(n) * (j + 1);
     }
     __syncthreads();
+}
+// the team of k_register_frame and k_icp: CTAs [0, T) of the launch, the all-gather region sized for TEAM_MAX
+__device__ __noinline__ void op_icp_team(const TeamScratch &ts, const Scratch &sc, Shared &sh, const MapView &m, int n,
+                                         const SE3 &guess, double max_dist, double kscale, int max_iter, double conv,
+                                         unsigned char *dyn_smem, int T, unsigned tag_base) {
+    icp_team_iterate<false>(ts, sc, sh, m, n, guess, max_dist, kscale, max_iter, conv, dyn_smem, T, tag_base, 0, TEAM_MAX);
+}
+// one team of k_icp_batch: member `member` of a slot whose all-gather region (ts.ll) is sized for `stride` CTAs
+__device__ __noinline__ void op_icp_team_slot(const TeamScratch &ts, const Scratch &sc, Shared &sh, const MapView &m, int n,
+                                              const SE3 &guess, double max_dist, double kscale, int max_iter, double conv,
+                                              unsigned char *dyn_smem, int T, unsigned tag_base, int member, int stride) {
+    icp_team_iterate<true>(ts, sc, sh, m, n, guess, max_dist, kscale, max_iter, conv, dyn_smem, T, tag_base, member, stride);
 }
 
 // result record <-> shared memory (member 0 publishes before a grid barrier, everybody reads after it)

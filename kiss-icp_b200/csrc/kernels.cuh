@@ -387,6 +387,120 @@ __global__ void __launch_bounds__(BLOCK, 1) k_icp(const IcpParams P) {
     }
 }
 
+// ---- kb_registration_align_batch: many AlignPointsToMap problems against one map in ONE launch ----------------
+// One hypothesis of a batch, planned on the host. Its source points are src[src_off, src_off + n); q_off is the
+// index of its first point among the points of all hypotheses of the same list (k_icp_batch: its QList records,
+// k_align_inliers: its points), so the lists are sorted by q_off.
+struct BatchHyp {
+    SE3 guess;
+    double max_dist, kscale;
+    long long src_off;
+    int n;
+    int T;      // team size, icp_team_size(n, ...) on the full grid: the split of the single call
+    int q_off;
+    int out;    // index of the hypothesis in the caller's arrays
+};
+// the hypothesis that owns point q of the list (the last one whose first point is <= q)
+__device__ __forceinline__ int batch_hyp_of(const BatchHyp *hyp, int nh, int q) {
+    int lo = 0, hi = nh - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (hyp[mid].q_off <= q) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+struct IcpBatchParams {
+    MapView m;
+    Scratch sc;
+    TeamScratch team;     // qrec: [n_total] records of this call; ll: the all-gather regions of the slots
+    const double *src;
+    const BatchHyp *hyp;  // [nh] the hypotheses that run on a team
+    int nh, n_total;      // n_total = sum of hyp[].n
+    int t_max, slots;     // a slot is t_max consecutive CTAs; slots = grid / t_max
+    int max_iter;
+    double conv;
+    unsigned tag_base;    // hypothesis h tags its epochs tag_base + h (max_iter + 1) + 1 ... + max_iter
+    unsigned *ctl;        // zeroed per launch, see BCTL_*
+    double *out_pose;     // [B][16] row-major
+    int *out_iters;       // [B]
+};
+// words of IcpBatchParams::ctl (counters on their own 128-byte lines)
+constexpr int BCTL_FILL = 0;      // ticket of the fill pass
+constexpr int BCTL_HYP = 32;      // ticket of the hypotheses
+constexpr int BCTL_SLOT = 64;     // + 32 s: barrier counter of slot s; then [slots][2]: the hypothesis of slot s, by round parity
+__host__ __device__ __forceinline__ int bctl_words(int slots) { return BCTL_SLOT + 32 * slots + 2 * slots; }
+
+// icp_fill_pass over the points of all hypotheses: warp <-> (hypothesis, point), each point moved by its own guess
+__device__ __noinline__ void icp_fill_pass_batch(const Grid &g, Shared &sh, const IcpBatchParams &P) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const double radius = P.team.radius_frac * P.m.voxel_size;
+    const int nwarps = g.size * NWARPS;
+    int q = g.rank + g.size * warp;
+    while (q < P.n_total) {
+        const BatchHyp &H = P.hyp[batch_hyp_of(P.hyp, P.nh, q)];
+        const double *s = P.src + 3 * (H.src_off + (q - H.q_off));
+        const V3 p = se3_act(H.guess, V3{s[0], s[1], s[2]});
+        nn_search_list(P.m, p, lane, sh.wnn[warp], &P.team.qrec[q], radius);
+        unsigned t = 0;
+        if (lane == 0) t = atomicAdd(P.ctl + BCTL_FILL, 1u);
+        q = nwarps + static_cast<int>(__shfl_sync(FULL, t, 0));
+    }
+}
+
+// Phase 1: one fill pass over all hypotheses on the whole grid, one grid barrier. Phase 2: the grid is cut into
+// `slots` slots of t_max CTAs; a slot takes hypotheses through a ticket (one that runs to max_iter does not hold up
+// the others) and runs hypothesis h on its first T_h CTAs, exactly as k_icp runs it on CTAs [0, T_h): same team size,
+// member m owns points m, m + T, ..., partials added in member order. A slot barrier separates its hypotheses: after
+// it, no CTA of the slot still reads the all-gather region, and every epoch tag is new anyway.
+__global__ void __launch_bounds__(BLOCK, 1) k_icp_batch(const IcpBatchParams P) {
+    __shared__ Shared sh;
+    Grid g;
+    g.init(P.sc.bar);
+    icp_fill_pass_batch(g, sh, P);
+    g.sync();
+    const int slot = static_cast<int>(blockIdx.x) / P.t_max;
+    if (slot >= P.slots) return;
+    Grid gs;
+    gs.init_team(P.ctl + BCTL_SLOT + 32 * slot, slot * P.t_max, P.t_max);
+    unsigned *pick = P.ctl + BCTL_SLOT + 32 * P.slots + 2 * slot;
+    TeamScratch ts = P.team;
+    ts.ll = P.team.ll + static_cast<size_t>(slot) * 2 * P.t_max * P.t_max * NPART;
+    for (int r = 0;; ++r) {
+        if (gs.rank == 0 && threadIdx.x == 0) pick[r & 1] = atomicAdd(P.ctl + BCTL_HYP, 1u);
+        gs.sync();
+        const int h = static_cast<int>(__ldcg(pick + (r & 1)));
+        if (h >= P.nh) break;
+        const BatchHyp H = P.hyp[h];
+        if (gs.rank < H.T) {
+            ts.qrec = P.team.qrec + H.q_off;
+            op_icp_team_slot(ts, P.sc, sh, P.m, H.n, H.guess, H.max_dist, H.kscale, P.max_iter, P.conv, kb_dyn_smem, H.T,
+                             P.tag_base + static_cast<unsigned>(h) * static_cast<unsigned>(P.max_iter + 1), gs.rank, P.t_max);
+            if (gs.rank == 0 && threadIdx.x == 0) {
+                se3_to_matrix(sh.result, P.out_pose + 16 * H.out);
+                P.out_iters[H.out] = sh.iters;
+            }
+        }
+    }
+}
+
+// DataAssociation (Registration.cpp:60-77) of every hypothesis' source mapped by its final pose: the correspondences
+// closer than its max_dist, counted into inliers[out] (zeroed by the host). One warp per point.
+__global__ void __launch_bounds__(256) k_align_inliers(const MapView m, const double *src, const BatchHyp *hyp, int nh,
+                                                       int n_total, const double *poses, int *inliers) {
+    __shared__ WarpNN wnn[8];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int q = blockIdx.x * 8 + warp; q < n_total; q += gridDim.x * 8) {
+        const BatchHyp &H = hyp[batch_hyp_of(hyp, nh, q)];
+        const double *s = src + 3 * (H.src_off + (q - H.q_off));
+        const double *T = poses + 16 * H.out;
+        const V3 p{T[0] * s[0] + T[1] * s[1] + T[2] * s[2] + T[3], T[4] * s[0] + T[5] * s[1] + T[6] * s[2] + T[7],
+                   T[8] * s[0] + T[9] * s[1] + T[10] * s[2] + T[11]};
+        const NNResult r = nn_search_warp(m, p, lane, wnn[warp]);
+        if (lane == 0 && r.d < H.max_dist) atomicAdd(&inliers[H.out], 1);
+    }
+}
+
 struct MapUpdParams {
     MapView m;
     Scratch sc;

@@ -2,12 +2,48 @@
 from __future__ import annotations
 
 import ctypes as C
+import sys
 
 import numpy as np
 
 from . import _native as N
 from .config import KISSConfig
 from .mapping import VoxelHashMap
+
+
+def _torch_if_cuda(x):
+    """the torch module when x is a torch CUDA tensor (torch is imported only if the caller already did)"""
+    torch = sys.modules.get("torch")
+    return torch if torch is not None and isinstance(x, torch.Tensor) and x.is_cuda else None
+
+
+def _guesses_arg(G) -> np.ndarray:
+    a = np.ascontiguousarray(G, dtype=np.float64)
+    if a.ndim != 3 or a.shape[1:] != (4, 4):
+        raise RuntimeError("Unable to cast Python instance to C++ type (expected (B, 4, 4) initial guesses)")
+    return a
+
+
+def _ranges_arg(ranges, n_points: int, B: int):
+    """(offsets, counts) as uint64 (size_t); no ranges: each of the B hypotheses uses all points"""
+    if ranges is None:
+        return np.zeros(B, dtype=np.uint64), np.full(B, n_points, dtype=np.uint64)
+    r = np.asarray(ranges)
+    if r.ndim != 2 or r.shape[1] != 2 or (r.size and r.dtype.kind not in "iu"):
+        raise RuntimeError("ranges must be a (B, 2) integer array of (offset, count)")
+    r = r.astype(np.int64)
+    bad = (r[:, 0] < 0) | (r[:, 1] < 0) | (r[:, 0] + r[:, 1] > n_points)
+    if bad.any():
+        k = int(np.argmax(bad))
+        raise IndexError(f"ranges[{k}] = ({r[k, 0]}, {r[k, 1]}) is outside the {n_points} points")
+    return np.ascontiguousarray(r[:, 0], dtype=np.uint64), np.ascontiguousarray(r[:, 1], dtype=np.uint64)
+
+
+def _per_hypothesis(x, B: int) -> np.ndarray:
+    a = np.asarray(x, dtype=np.float64)
+    if a.ndim > 1 or (a.ndim == 1 and a.shape[0] != B):
+        raise RuntimeError(f"expected a scalar or {B} values, got shape {a.shape}")
+    return np.ascontiguousarray(np.broadcast_to(a, (B,)))
 
 
 def get_registration(config: KISSConfig):
@@ -38,6 +74,83 @@ class Registration:
         N.check(N.lib().kb_registration_align_points_to_map(self._h, N.ptr(pts), len(pts), voxel_map._h, N.ptr(g),
                                                             float(max_correspondance_distance), float(kernel), N.ptr(out)))
         return out
+
+    def align_points_to_map_batch(self, points, voxel_map: VoxelHashMap, initial_guesses, max_correspondance_distance,
+                                  kernel, ranges=None, return_inliers: bool = False):
+        """B independent align_points_to_map problems against one map, run side by side in one launch
+        (relocalization, loop-closure checks, multi-hypothesis starts). Each result equals, bit for bit, what
+        align_points_to_map returns for that hypothesis alone.
+
+        points: one (N, 3) cloud with ``ranges`` (B, 2) rows of (offset, count) — ranges may overlap or repeat; no
+        ranges: every hypothesis uses the whole cloud — or a list of B (n_b, 3) clouds. initial_guesses: (B, 4, 4).
+        max_correspondance_distance, kernel: scalars or (B,) arrays.
+        Returns (poses (B, 4, 4), iterations (B,)) and, with return_inliers, inliers (B,): the correspondence count
+        build_system gives for the source mapped by its pose. Torch CUDA tensors in give torch CUDA tensors out
+        (the device entry point); anything else goes through host arrays."""
+        torch = _torch_if_cuda(points[0] if isinstance(points, (list, tuple)) and len(points) else points)
+        if torch is not None:
+            return self._align_batch_dev(torch, points, voxel_map, initial_guesses, max_correspondance_distance, kernel,
+                                         ranges, return_inliers)
+        g = _guesses_arg(initial_guesses)
+        B = len(g)
+        if isinstance(points, (list, tuple)):
+            if ranges is not None:
+                raise RuntimeError("ranges go with a single (N, 3) cloud, not with a list of clouds")
+            clouds = [N.points_arg(p) for p in points]
+            counts = np.array([len(c) for c in clouds], dtype=np.uint64)
+            pts = np.concatenate(clouds) if clouds else np.empty((0, 3))
+            offsets = (np.cumsum(counts) - counts).astype(np.uint64)
+        else:
+            pts = N.points_arg(points)
+            offsets, counts = _ranges_arg(ranges, len(pts), B)
+        if len(counts) != B:
+            raise RuntimeError(f"{len(counts)} point ranges for {B} initial guesses")
+        md = _per_hypothesis(max_correspondance_distance, B)
+        ks = _per_hypothesis(kernel, B)
+        poses = np.empty((B, 4, 4))
+        iters = np.empty(B, dtype=np.int32)
+        inl = np.empty(B, dtype=np.int32) if return_inliers else None
+        N.check(N.lib().kb_registration_align_batch(
+            self._h, N.ptr(pts), len(pts), N.ptr(offsets), N.ptr(counts), B, voxel_map._h, N.ptr(g), N.ptr(md), N.ptr(ks),
+            N.ptr(poses), N.ptr(iters), N.ptr(inl) if inl is not None else None))
+        return (poses, iters, inl) if return_inliers else (poses, iters)
+
+    def _align_batch_dev(self, torch, points, voxel_map, initial_guesses, max_dist, kernel, ranges, return_inliers):
+        if isinstance(points, (list, tuple)):
+            if ranges is not None:
+                raise RuntimeError("ranges go with a single (N, 3) cloud, not with a list of clouds")
+            counts = np.array([p.shape[0] for p in points], dtype=np.uint64)
+            offsets = (np.cumsum(counts) - counts).astype(np.uint64)
+            points = torch.cat(list(points))
+        else:
+            offsets = counts = None
+        dev = points.device
+        if points.ndim != 2 or points.shape[1] != 3:
+            raise RuntimeError("Unable to cast Python instance to C++ type (expected an (N, 3) array)")
+        pts = points.to(torch.float64).contiguous()
+        g = torch.as_tensor(initial_guesses, dtype=torch.float64, device=dev).contiguous()
+        if g.ndim != 3 or g.shape[1:] != (4, 4):
+            raise RuntimeError("Unable to cast Python instance to C++ type (expected (B, 4, 4) initial guesses)")
+        B = g.shape[0]
+        if counts is None:
+            offsets, counts = _ranges_arg(None if ranges is None else np.asarray(torch.as_tensor(ranges).cpu()), len(pts), B)
+        if len(counts) != B:
+            raise RuntimeError(f"{len(counts)} point ranges for {B} initial guesses")
+        as_dev = lambda a, dt: torch.as_tensor(np.ascontiguousarray(a), device=dev).to(dt).contiguous()
+        off_d = as_dev(offsets.astype(np.int64), torch.int64)  # (size_t on the device: non-negative int64, same bits)
+        cnt_d = as_dev(counts.astype(np.int64), torch.int64)
+        md = as_dev(_per_hypothesis(np.asarray(torch.as_tensor(max_dist).cpu()), B), torch.float64)
+        ks = as_dev(_per_hypothesis(np.asarray(torch.as_tensor(kernel).cpu()), B), torch.float64)
+        poses = torch.empty((B, 4, 4), dtype=torch.float64, device=dev)
+        iters = torch.empty(B, dtype=torch.int32, device=dev)
+        inl = torch.empty(B, dtype=torch.int32, device=dev) if return_inliers else None
+        p = lambda t: C.c_void_p(t.data_ptr())
+        torch.cuda.current_stream(dev).synchronize()  # the inputs were made on torch's stream, the map has its own
+        N.check(N.lib().kb_registration_align_batch_dev(
+            self._h, p(pts), len(pts), p(off_d), p(cnt_d), B, voxel_map._h, p(g), p(md), p(ks), p(poses), p(iters),
+            p(inl) if inl is not None else None))
+        N.check(N.lib().kb_map_sync(voxel_map._h))
+        return (poses, iters, inl) if return_inliers else (poses, iters)
 
     @property
     def last_iterations(self) -> int:
