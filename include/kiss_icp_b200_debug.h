@@ -14,15 +14,12 @@ extern "C" {
  * of the second ICP iteration of the last frame (CTA 0); cost of one grid barrier */
 int kb_pipeline_debug_stamps(const kb_pipeline *p, double *ns, int n);
 int kb_debug_barrier_ns(int iters, double *ns_per_barrier);
-/* host evaluation of the ICP loop's structured (Schur complement) solve vs the pivoted LDL^T on the same 16
- * accumulators {sum w, sum w*s (3), lower triangle of sum w*hat(s)^T*hat(s) (6), JTr (6)} */
+/* host evaluation of the ICP loop's structured (Schur complement) solve vs the pivoted LDL^T it falls back to, on the
+ * same 16 accumulators {sum w, sum w*s (3), lower triangle of sum w*hat(s)^T*hat(s) (6), JTr (6)} */
 int kb_debug_icp_schur(const double acc[16], double x_schur[6], double x_ldlt[6], int *used_schur);
-/* host evaluation of the device's two 6x6 LDLT code paths (loop form / register-resident form) */
-int kb_debug_ldlt6(const double A[36], const double b[6], double x_loop[6], double x_unrolled[6]);
-/* host evaluation of the exact vs latency-optimised (reciprocal / sincos) ICP solve step:
+/* host evaluation of the latency-optimised (reciprocal / sincos) ICP solve step the kernels run:
  * x = LDLT solve, T = exp(x) * exp(b) */
-int kb_debug_icp_solve(const double A[36], const double b[6], double x_exact[6], double x_fast[6], double T_exact[16],
-                       double T_fast[16]);
+int kb_debug_icp_solve_fast(const double A[36], const double b[6], double x_fast[6], double T_fast[16]);
 /* work done by the ICP loop of the last RegisterFrame: GetClosestNeighbor calls (iterations x
  * source points) and map points examined — the inputs of the algorithmic-bytes formula */
 int kb_pipeline_last_icp_work(const kb_pipeline *p, double *queries, double *candidates);

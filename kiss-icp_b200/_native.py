@@ -149,8 +149,7 @@ SIGNATURES = {
     "kb_pipeline_last_sigma": (i32, [vp, C.POINTER(dbl)]),
     "kb_pipeline_debug_stamps": (i32, [vp, vp, i32]),
     "kb_pipeline_history_stamps": (i32, [vp, vp, sz, C.POINTER(sz)]),
-    "kb_debug_ldlt6": (i32, [vp, vp, vp, vp]),
-    "kb_debug_icp_solve": (i32, [vp, vp, vp, vp, vp, vp]),
+    "kb_debug_icp_solve_fast": (i32, [vp, vp, vp, vp]),
     "kb_debug_icp_schur": (i32, [vp, vp, vp, C.POINTER(i32)]),
     "kb_debug_barrier_ns": (i32, [i32, C.POINTER(dbl)]),
     "kb_pipeline_last_ds_profile": (i32, [vp, vp]),

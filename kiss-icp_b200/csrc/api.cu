@@ -64,7 +64,86 @@ int device_count() {
     return n;
 }
 
-bool device_is_stuck(int device);
+// the device watchdog's report (device_ops.cuh): mapped host words per device, checked after every synchronisation
+struct WatchdogHost {
+    unsigned *host = nullptr;  // [0] flag [1] code [2] block [3] thread [4] a [5] b
+};
+WatchdogHost g_wd[64];
+int watchdog_init(int device) {
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lock(mu);
+    if (device < 0 || device >= 64 || g_wd[device].host) return KB_OK;
+    unsigned *h = nullptr, *d = nullptr;
+    CK(cudaHostAlloc(&h, 8 * sizeof(unsigned), cudaHostAllocMapped));
+    std::memset(h, 0, 8 * sizeof(unsigned));
+    CK(cudaHostGetDevicePointer(&d, h, 0));
+    CK(cudaMemcpyToSymbol(g_kb_wd_host, &d, sizeof(d)));
+    // give up after 2^24 polls (of the order of 10 s, below the host's 30 s deadline). 2^22 (a second or two) fired once in
+    // ~40 full-file test runs at the FIRST grid barrier of a launch; whether that was a stall or a deadlock is not known.
+    unsigned init[8] = {0, 0, 0, 0, 0, 0, 0, 24};
+    if (const char *e = std::getenv("KB_WATCHDOG_SHIFT")) init[7] = static_cast<unsigned>(std::max(10, std::min(std::atoi(e), 31)));
+    CK(cudaMemcpyToSymbol(g_kb_wd, init, sizeof(init)));
+    g_wd[device].host = h;
+    return KB_OK;
+}
+// where every CTA of the last k_register_frame was (g_kb_marks)
+std::string format_marks(const unsigned m[256]) {
+    std::string out = "phase marks per CTA:";
+    char buf[16];
+    for (int i = 0; i < 160; ++i) {
+        std::snprintf(buf, sizeof(buf), " %x", m[i]);
+        out += buf;
+    }
+    return out;
+}
+// after a synchronisation: did a spin loop of the last launches give up?
+int watchdog_check(int device) {
+    unsigned *h = (device >= 0 && device < 64) ? g_wd[device].host : nullptr;
+    if (!h || !*reinterpret_cast<volatile unsigned *>(h)) return KB_OK;
+    const unsigned code = h[1], block = h[2], thread = h[3], a = h[4], b = h[5];
+    h[0] = 0;
+    unsigned zero = 0;
+    cudaMemcpyToSymbol(g_kb_wd, &zero, sizeof(zero));  // re-arm
+    static const char *names[] = {"?", "grid barrier", "ICP gather", "ICP result record", "ICP team gather", "NN bulk copy"};
+    std::string marks;
+    unsigned m[256];
+    if (cudaMemcpyFromSymbol(m, g_kb_marks, sizeof(m)) == cudaSuccess) marks = "; " + format_marks(m);  // (the launch has ended: a plain copy)
+    cudaGetLastError();
+    return fail(KB_ERR_CUDA, "device watchdog: a kernel gave up waiting at the %s (block %u, thread %u, a=%u, b=%u; grid barrier: a = target, b = counter); "
+                             "the results of that launch are invalid%s",
+                names[code < 6 ? code : 0], block, thread, a, b, marks.c_str());
+}
+
+bool g_stuck[64];
+void device_stuck(int device) {
+    if (device >= 0 && device < 64) g_stuck[device] = true;
+}
+// a launch on this device never ended: cudaFree & co. would block forever, so the destructors leak instead
+bool device_is_stuck(int device) {
+    if (device < 0) {
+        for (bool b : g_stuck)
+            if (b) return true;
+        return false;
+    }
+    return device < 64 && g_stuck[device];
+}
+std::string phase_marks(int device) {
+    // the compute stream is stuck: read the marks on a stream of their own (bounded wait, the copy engine is free)
+    unsigned marks[256];
+    cudaStream_t side = nullptr;
+    if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&side, cudaStreamNonBlocking) != cudaSuccess) return "";
+    std::string out;
+    if (cudaMemcpyFromSymbolAsync(marks, g_kb_marks, sizeof(marks), 0, cudaMemcpyDeviceToHost, side) == cudaSuccess) {
+        const auto t0 = std::chrono::steady_clock::now();
+        cudaError_t q;
+        while ((q = cudaStreamQuery(side)) == cudaErrorNotReady &&
+               std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() < 5.0) {
+        }
+        out = q == cudaSuccess ? format_marks(marks) : "(phase marks unreadable)";
+    }
+    return out;  // (the side stream is leaked with the rest of the stuck context)
+}
+
 template <class T>
 struct DBuf {
     T *p = nullptr;
@@ -114,17 +193,13 @@ size_t pow2_at_least(size_t v) {
     return p;
 }
 
-int watchdog_check_fwd(int device);
-int watchdog_init_fwd(int device);
-void device_stuck_fwd(int device);
-std::string phase_marks_fwd(int device);
-
 // execution context: device, stream, persistent-grid size and the cross-CTA scratch
 struct Exec {
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
     int grid = 0;
+    int sms = 0;  // multiprocessors of the device
     Scratch sc{};  // all pointers null, profiling off
     TeamScratch team{};  // ll / out (qrec belongs to the caller's workspace)
     size_t icp_smem = 96 * 1024;  // dynamic shared memory of the ICP kernels: candidate coordinates of the team's source points (KB_ICP_SMEM_KB)
@@ -146,14 +221,14 @@ struct Exec {
         if (device_count() <= 0) return fail(KB_ERR_NO_DEVICE, "no CUDA device visible (this library has no CPU fallback)");
         device = tl_device;
         CK(cudaSetDevice(device));
-        RET(watchdog_init_fwd(device));
+        RET(watchdog_init(device));
         if (tl_user_stream) {
             stream = tl_user_stream;
         } else {
             CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
             own_stream = true;
         }
-        int sms = 0, coop = 0;
+        int coop = 0;
         CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
         CK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
         if (!coop) return fail(KB_ERR_CUDA, "device does not support cooperative launch");
@@ -194,16 +269,17 @@ struct Exec {
         if (team.out) cudaFree(team.out);
         if (own_stream && stream) cudaStreamDestroy(stream);
     }
+    // opt in to > 48 KB of dynamic shared memory, once per kernel AND device (the attribute is per device)
+    int opt_in_smem(const void *k, size_t bytes) {
+        if (bytes <= 48 * 1024 || std::find(smem_opted.begin(), smem_opted.end(), k) != smem_opted.end()) return KB_OK;
+        CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
+        smem_opted.push_back(k);
+        return KB_OK;
+    }
     template <class P>
     int coop(void (*kern)(P), const P &p, size_t smem = 0, bool self_reset = false) {
         CK(cudaSetDevice(device));
-        if (smem > 48 * 1024) {  // opt in to large dynamic shared memory once per kernel AND device (the attribute is per device)
-            const void *k = reinterpret_cast<const void *>(kern);
-            if (std::find(smem_opted.begin(), smem_opted.end(), k) == smem_opted.end()) {
-                CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-                smem_opted.push_back(k);
-            }
-        }
+        RET(opt_in_smem(reinterpret_cast<const void *>(kern), smem));
         if (!self_reset || bar_dirty)  // kernels that end with Grid::finish() leave the barrier words zeroed themselves
             CK(cudaMemsetAsync(sc.bar, 0, BAR_WORDS * sizeof(unsigned), stream));
         bar_dirty = !self_reset;
@@ -226,7 +302,7 @@ struct Exec {
     // ends is reported as KB_ERR_CUDA instead of hanging the caller (the device watchdog should have fired long before)
     int sync() {
         RET(wait_deadline([&] { return cudaStreamQuery(stream); }, "stream"));
-        return watchdog_check_fwd(device);
+        return watchdog_check(device);
     }
     template <class Q>
     int wait_deadline(Q query, const char *what) {
@@ -241,104 +317,16 @@ struct Exec {
             if (e != cudaErrorNotReady) return fail(KB_ERR_CUDA, "%s wait failed: %s", what, cudaGetErrorString(e));
             if ((spins & 0x3ff) == 0x3ff && limit_s > 0.0 &&
                 std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() > limit_s) {
-                const int wd = watchdog_check_fwd(device);
-                device_stuck_fwd(device);
+                const int wd = watchdog_check(device);
+                device_stuck(device);
                 if (wd != KB_OK) return wd;
                 return fail(KB_ERR_CUDA, "the device did not finish the %s within %.0f s (launch %llu): giving up; %s", what, limit_s, launches,
-                            phase_marks_fwd(device).c_str());
+                            phase_marks(device).c_str());
             }
         }
     }
 };
 
-// the device watchdog's report (device_ops.cuh): mapped host words per device, checked after every synchronisation
-struct WatchdogHost {
-    unsigned *host = nullptr;  // [0] flag [1] code [2] block [3] thread [4] a [5] b
-};
-WatchdogHost g_wd[64];
-int watchdog_init(int device) {
-    static std::mutex mu;
-    std::lock_guard<std::mutex> lock(mu);
-    if (device < 0 || device >= 64 || g_wd[device].host) return KB_OK;
-    unsigned *h = nullptr, *d = nullptr;
-    CK(cudaHostAlloc(&h, 8 * sizeof(unsigned), cudaHostAllocMapped));
-    std::memset(h, 0, 8 * sizeof(unsigned));
-    CK(cudaHostGetDevicePointer(&d, h, 0));
-    CK(cudaMemcpyToSymbol(g_kb_wd_host, &d, sizeof(d)));
-    // give up after 2^24 polls (of the order of 10 s, below the host's 30 s deadline). 2^22 (a second or two) fired once in
-    // ~40 full-file test runs at the FIRST grid barrier of a launch; whether that was a stall or a deadlock is not known.
-    unsigned init[8] = {0, 0, 0, 0, 0, 0, 0, 24};
-    if (const char *e = std::getenv("KB_WATCHDOG_SHIFT")) init[7] = static_cast<unsigned>(std::max(10, std::min(std::atoi(e), 31)));
-    CK(cudaMemcpyToSymbol(g_kb_wd, init, sizeof(init)));
-    g_wd[device].host = h;
-    return KB_OK;
-}
-// after a synchronisation: did a spin loop of the last launches give up?
-int watchdog_check(int device) {
-    unsigned *h = (device >= 0 && device < 64) ? g_wd[device].host : nullptr;
-    if (!h || !*reinterpret_cast<volatile unsigned *>(h)) return KB_OK;
-    const unsigned code = h[1], block = h[2], thread = h[3], a = h[4], b = h[5];
-    h[0] = 0;
-    unsigned zero = 0;
-    cudaMemcpyToSymbol(g_kb_wd, &zero, sizeof(zero));  // re-arm
-    static const char *names[] = {"?", "grid barrier", "ICP gather", "ICP result record", "ICP team gather", "NN bulk copy"};
-    // where every CTA of the last k_register_frame was (the launch has ended: a plain copy)
-    std::string marks;
-    unsigned m[256];
-    if (cudaMemcpyFromSymbol(m, g_kb_marks, sizeof(m)) == cudaSuccess) {
-        marks = "; phase marks per CTA:";
-        char buf[16];
-        for (int i = 0; i < 160; ++i) {
-            std::snprintf(buf, sizeof(buf), " %x", m[i]);
-            marks += buf;
-        }
-    }
-    cudaGetLastError();
-    return fail(KB_ERR_CUDA, "device watchdog: a kernel gave up waiting at the %s (block %u, thread %u, a=%u, b=%u; grid barrier: a = target, b = counter); "
-                             "the results of that launch are invalid%s",
-                names[code < 6 ? code : 0], block, thread, a, b, marks.c_str());
-}
-
-bool g_stuck[64];
-void device_stuck_fwd(int device) {
-    if (device >= 0 && device < 64) g_stuck[device] = true;
-}
-// a launch on this device never ended: cudaFree & co. would block forever, so the destructors leak instead
-bool device_is_stuck(int device) {
-    if (device < 0) {
-        for (bool b : g_stuck)
-            if (b) return true;
-        return false;
-    }
-    return device < 64 && g_stuck[device];
-}
-std::string phase_marks_fwd(int device) {
-    // the compute stream is stuck: read the marks on a stream of their own (bounded wait, the copy engine is free)
-    unsigned marks[256];
-    cudaStream_t side = nullptr;
-    if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&side, cudaStreamNonBlocking) != cudaSuccess) return "";
-    std::string out;
-    if (cudaMemcpyFromSymbolAsync(marks, g_kb_marks, sizeof(marks), 0, cudaMemcpyDeviceToHost, side) == cudaSuccess) {
-        const auto t0 = std::chrono::steady_clock::now();
-        cudaError_t q;
-        while ((q = cudaStreamQuery(side)) == cudaErrorNotReady &&
-               std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() < 5.0) {
-        }
-        if (q == cudaSuccess) {
-            out = "phase marks per CTA:";
-            char buf[16];
-            for (int i = 0; i < 160; ++i) {
-                std::snprintf(buf, sizeof(buf), " %x", marks[i]);
-                out += buf;
-            }
-        } else {
-            out = "(phase marks unreadable)";
-        }
-    }
-    return out;  // (the side stream is leaked with the rest of the stuck context)
-}
-int watchdog_check_fwd(int device) { return watchdog_check(device); }
-int watchdog_init_fwd(int device) { return watchdog_init(device); }
 
 int make_exec(std::shared_ptr<Exec> *out) {
     auto e = std::make_shared<Exec>();
@@ -410,31 +398,35 @@ bool to_se3(const double M[16], SE3 *T) { return se3_from_matrix(M, T); }
 
 // =============================================================================================
 struct kb_map {
+    struct Table {
+        size_t capacity = 0;
+        int4 *slots = nullptr;
+        double *points = nullptr;
+        int *head = nullptr, *pcount = nullptr, *pending = nullptr, *counters = nullptr;
+    };
     std::shared_ptr<Exec> ex;
     double voxel_size, max_distance;
     unsigned cap;
-    size_t capacity = 0;
-    int4 *slots = nullptr;
-    double *points = nullptr;
-    int *head = nullptr;
-    int *pcount = nullptr;
-    int *pending = nullptr;
-    int *counters = nullptr;
+    Table cur;  // the voxel table of the map
+    // the table a rebuild moves the map into. Rebuilds are periodic in steady state (tombstones of voxels that left
+    // max_distance accumulate until load 0.5) and mostly keep the size, so the previous table is kept as a spare
+    // and the two ping-pong: cudaMalloc/cudaFree of a few hundred MB can take milliseconds to hundreds of milliseconds.
+    Table spare;
     int h_counters[C_NCOUNTERS] = {0};
     Work ws;
     DBuf<double> q_in, q_outp, q_outd;
     DBuf<unsigned long long> q_cand;
     bool borrowed = false;
 
-    MapView view() const {
+    MapView view_of(const Table &t) const {
         MapView m;
-        m.slots = slots;
-        m.points = points;
-        m.head = head;
-        m.pcount = pcount;
-        m.pending = pending;
-        m.counters = counters;
-        m.mask = static_cast<unsigned>(capacity - 1);
+        m.slots = t.slots;
+        m.points = t.points;
+        m.head = t.head;
+        m.pcount = t.pcount;
+        m.pending = t.pending;
+        m.counters = t.counters;
+        m.mask = static_cast<unsigned>(t.capacity - 1);
         m.cap = static_cast<int>(cap);
         m.voxel_size = voxel_size;
         m.max_distance = max_distance;
@@ -442,16 +434,7 @@ struct kb_map {
         m.vdiv = make_voxel_div(voxel_size);
         return m;
     }
-    // the table a rebuild moves the map into. Rebuilds are periodic in steady state (tombstones of voxels that left
-    // max_distance accumulate until load 0.5) and mostly keep the size, so the previous table is kept as a spare
-    // and the two ping-pong: cudaMalloc/cudaFree of a few hundred MB can take milliseconds to hundreds of milliseconds.
-    struct Table {
-        size_t capacity = 0;
-        int4 *slots = nullptr;
-        double *points = nullptr;
-        int *head = nullptr, *pcount = nullptr, *pending = nullptr, *counters = nullptr;
-    };
-    Table spare;
+    MapView view() const { return view_of(cur); }
     static void free_table(Table &t) {
         if (t.slots) cudaFree(t.slots);
         if (t.points) cudaFree(t.points);
@@ -461,22 +444,19 @@ struct kb_map {
         if (t.counters) cudaFree(t.counters);
         t = Table{};
     }
-    Table current() const { return Table{capacity, slots, points, head, pcount, pending, counters}; }
-    void adopt(const Table &t) {
-        capacity = t.capacity;
-        slots = t.slots;
-        points = t.points;
-        head = t.head;
-        pcount = t.pcount;
-        pending = t.pending;
-        counters = t.counters;
-    }
     ~kb_map() {
         if (ex && device_is_stuck(ex->device)) return;
         if (ex) cudaSetDevice(ex->device);
-        Table t = current();
-        free_table(t);
+        free_table(cur);
         free_table(spare);
+    }
+    // every slot empty, every counter zero (enqueued on the map's stream)
+    int reset_table(const Table &t) {
+        k_map_fill<<<std::min<size_t>(4096, (t.capacity + 255) / 256), 256, 0, ex->stream>>>(t.slots, t.head, t.pcount, t.capacity);
+        ++ex->launches;
+        CK(cudaGetLastError());
+        CK(cudaMemsetAsync(t.counters, 0, sizeof(int) * C_NCOUNTERS, ex->stream));
+        return KB_OK;
     }
     // an empty table of cap_slots slots: the spare if it has that size, else a fresh allocation
     int take_table(size_t cap_slots, Table *out) {
@@ -499,22 +479,19 @@ struct kb_map {
             if ((e = cudaMalloc(&t.pending, cap_slots * PEND * sizeof(int))) != cudaSuccess) return bail(e);
             if ((e = cudaMalloc(&t.counters, sizeof(int) * C_NCOUNTERS)) != cudaSuccess) return bail(e);
         }
-        k_map_fill<<<std::min<size_t>(4096, (cap_slots + 255) / 256), 256, 0, ex->stream>>>(t.slots, t.head, t.pcount, cap_slots);
-        ++ex->launches;
-        CK(cudaGetLastError());
-        CK(cudaMemsetAsync(t.counters, 0, sizeof(int) * C_NCOUNTERS, ex->stream));
+        RET(reset_table(t));
         *out = t;
         return KB_OK;
     }
     // make room for `extra` more voxels at load factor <= 0.5 (tombstones count as load)
     bool would_grow(size_t extra) const {  // ensure_capacity(extra) would rebuild the table (needs an idle stream)
         const size_t live = static_cast<size_t>(h_counters[C_LIVE]), tomb = static_cast<size_t>(h_counters[C_TOMB]);
-        return !capacity || (live + tomb + extra) * 2 > capacity;
+        return !cur.capacity || (live + tomb + extra) * 2 > cur.capacity;
     }
     int ensure_capacity(size_t extra, size_t force_want = 0) {
         CK(cudaSetDevice(ex->device));
         const size_t live = static_cast<size_t>(h_counters[C_LIVE]), tomb = static_cast<size_t>(h_counters[C_TOMB]);
-        if (!force_want && capacity && (live + tomb + extra) * 2 <= capacity) return KB_OK;
+        if (!force_want && cur.capacity && (live + tomb + extra) * 2 <= cur.capacity) return KB_OK;
         // grow/rebuild target: load factor <= 1/3 right after the rebuild (tombstones then accumulate up to 1/2)
         static const size_t cap_factor = [] {
             const char *e = std::getenv("KB_MAP_CAP_FACTOR");  // tuning aid: slots per expected voxel after a rebuild
@@ -522,22 +499,13 @@ struct kb_map {
         }();
         // never shrink on the hot path: the spare table has the current size, a smaller one would mean cudaMalloc
         const size_t want = force_want ? force_want
-                                       : std::max<size_t>({pow2_at_least(cap_factor * (live + extra)), size_t(1) << 14, capacity});
+                                       : std::max<size_t>({pow2_at_least(cap_factor * (live + extra)), size_t(1) << 14, cur.capacity});
         if (want > (size_t(1) << 31)) return fail(KB_ERR_INVALID_ARG, "voxel table would exceed 2^31 slots");
         StallTrace trace("voxel table rebuild");
         Table nt;
         RET(take_table(want, &nt));
-        if (capacity && live) {
-            MapView from = view();
-            MapView to = from;
-            to.slots = nt.slots;
-            to.points = nt.points;
-            to.head = nt.head;
-            to.pcount = nt.pcount;
-            to.pending = nt.pending;
-            to.counters = nt.counters;
-            to.mask = static_cast<unsigned>(want - 1);
-            k_map_rehash<<<std::min<size_t>(2048, (capacity * 32 + 255) / 256), 256, 0, ex->stream>>>(from, to);
+        if (cur.capacity && live) {
+            k_map_rehash<<<std::min<size_t>(2048, (cur.capacity * 32 + 255) / 256), 256, 0, ex->stream>>>(view(), view_of(nt));
             ++ex->launches;
             CK(cudaGetLastError());
             CK(cudaMemcpyAsync(h_counters, nt.counters, sizeof(int) * C_NCOUNTERS, cudaMemcpyDeviceToHost, ex->stream));
@@ -545,26 +513,25 @@ struct kb_map {
         } else {
             std::memset(h_counters, 0, sizeof(h_counters));
         }
-        Table old = current();
-        adopt(nt);
         free_table(spare);  // (empty unless take_table allocated)
-        spare = old;        // stays allocated: the next same-size rebuild moves back into it
+        spare = cur;        // stays allocated: the next same-size rebuild moves back into it
+        cur = nt;
         return KB_OK;
     }
     // allocate the table AND its spare for `slots` slots now (pipeline creation), so that neither growth nor the
     // periodic tombstone rebuild has to call cudaMalloc while frames are being registered
     int reserve(size_t slots) {
         slots = pow2_at_least(slots);
-        if (slots > capacity) RET(ensure_capacity(0, slots));
-        if (spare.capacity != capacity) {
+        if (slots > cur.capacity) RET(ensure_capacity(0, slots));
+        if (spare.capacity != cur.capacity) {
             Table t;
-            RET(take_table(capacity, &t));  // frees a spare of another size
+            RET(take_table(cur.capacity, &t));  // frees a spare of another size
             spare = t;
         }
         return KB_OK;
     }
     int pull_counters() {
-        CK(cudaMemcpyAsync(h_counters, counters, sizeof(int) * C_NCOUNTERS, cudaMemcpyDeviceToHost, ex->stream));
+        CK(cudaMemcpyAsync(h_counters, cur.counters, sizeof(int) * C_NCOUNTERS, cudaMemcpyDeviceToHost, ex->stream));
         RET(ex->sync());
         if (h_counters[C_STATUS] & ST_TABLE_FULL) return fail(KB_ERR_CUDA, "voxel table overflow (internal capacity bug)");
         return KB_OK;
@@ -573,7 +540,7 @@ struct kb_map {
     // table that is adopted only when k_map_load found nothing wrong; otherwise the map, its counters and the spare
     // table are left as they were.
     int load(const int *d_vox, const int *d_cnt, const long long *d_off, const double *d_pts, size_t nv, size_t np) {
-        const size_t want = std::max<size_t>({capacity, pow2_at_least(3 * nv), size_t(1) << 14});
+        const size_t want = std::max<size_t>({cur.capacity, pow2_at_least(3 * nv), size_t(1) << 14});
         if (want > (size_t(1) << 31)) return fail(KB_ERR_INVALID_ARG, "voxel table would exceed 2^31 slots");
         StallTrace trace("voxel map load");
         // take_table frees a spare of another size: keep it aside so that a failed load can put it back
@@ -589,14 +556,7 @@ struct kb_map {
         int h[C_NCOUNTERS] = {0};
         if (nv) {
             MapLoadParams P;
-            P.m = view();
-            P.m.slots = nt.slots;
-            P.m.points = nt.points;
-            P.m.head = nt.head;
-            P.m.pcount = nt.pcount;
-            P.m.pending = nt.pending;
-            P.m.counters = nt.counters;
-            P.m.mask = static_cast<unsigned>(want - 1);
+            P.m = view_of(nt);
             P.voxels = d_vox;
             P.counts = d_cnt;
             P.offsets = d_off;
@@ -626,9 +586,8 @@ struct kb_map {
             return fail(KB_ERR_INVALID_ARG, "map load rejected, the map is unchanged:%s", why.c_str());
         }
         free_table(keep);
-        Table old = current();
-        adopt(nt);
-        spare = old;
+        spare = cur;
+        cur = nt;
         std::memcpy(h_counters, h, sizeof(h_counters));  // the host's grow decision and the kernel's veto read these
         return KB_OK;
     }
@@ -836,10 +795,7 @@ int kb_map_destroy(kb_map *map) {
 int kb_map_clear(kb_map *map) {
     if (!map) return fail(KB_ERR_INVALID_ARG, "map == NULL");
     CK(cudaSetDevice(map->ex->device));
-    k_map_fill<<<std::min<size_t>(4096, (map->capacity + 255) / 256), 256, 0, map->ex->stream>>>(map->slots, map->head,
-                                                                                             map->pcount, map->capacity);
-    ++map->ex->launches;
-    CK(cudaMemsetAsync(map->counters, 0, sizeof(int) * C_NCOUNTERS, map->ex->stream));
+    RET(map->reset_table(map->cur));
     std::memset(map->h_counters, 0, sizeof(map->h_counters));
     return map->ex->sync();
 }
@@ -870,7 +826,7 @@ int kb_map_compact(kb_map *map) {
     if (!map) return fail(KB_ERR_INVALID_ARG, "map == NULL");
     const size_t live = static_cast<size_t>(map->h_counters[C_LIVE]);
     const size_t want = std::max<size_t>(pow2_at_least(2 * live + 2), size_t(1) << 14);
-    if (want >= map->capacity && map->h_counters[C_TOMB] == 0) return KB_OK;
+    if (want >= map->cur.capacity && map->h_counters[C_TOMB] == 0) return KB_OK;
     RET(map->ensure_capacity(0, want));
     return map->ex->sync();
 }
@@ -1017,8 +973,7 @@ int kb_map_pointcloud(const kb_map *map, double *out_xyz, size_t capacity, size_
 
 static int nn_launch(kb_map *map, const double *d_q, size_t n, double *d_p, double *d_d, unsigned long long *d_cand) {
     if (n == 0) return KB_OK;
-    int sms = 132;  // H100 SXM; replaced by the device's count below
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, map->ex->device);
+    const size_t sms = static_cast<size_t>(map->ex->sms);
     // default: the register-staged kernel (bench.py times both: `nn_kernel`, `nn_kernel.other_variant`);
     // KB_NN_KERNEL=bulk selects the variant that stages the candidate blocks with cp.async.bulk + mbarrier
     // (needs 16-byte aligned blocks: an even max_points_per_voxel <= 32; read per call)
@@ -1029,19 +984,15 @@ static int nn_launch(kb_map *map, const double *d_q, size_t n, double *d_p, doub
     const size_t want = (n * 32 + threads - 1) / threads;
     if (bulk) {
         const size_t smem = static_cast<size_t>(NNB_WARPS) * NNB_BUF;
-        const void *k0 = reinterpret_cast<const void *>(&k_nn_query_bulk<false>), *k1 = reinterpret_cast<const void *>(&k_nn_query_bulk<true>);
-        for (const void *k : {k0, k1})
-            if (std::find(map->ex->smem_opted.begin(), map->ex->smem_opted.end(), k) == map->ex->smem_opted.end()) {
-                CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-                map->ex->smem_opted.push_back(k);
-            }
-        const unsigned blocks = static_cast<unsigned>(std::min<size_t>(want, static_cast<size_t>(sms) * 3));  // 3 CTAs/SM, grid-stride
+        RET(map->ex->opt_in_smem(reinterpret_cast<const void *>(&k_nn_query_bulk<false>), smem));
+        RET(map->ex->opt_in_smem(reinterpret_cast<const void *>(&k_nn_query_bulk<true>), smem));
+        const unsigned blocks = static_cast<unsigned>(std::min<size_t>(want, sms * 3));  // 3 CTAs/SM, grid-stride
         if (d_cand)
             k_nn_query_bulk<true><<<blocks, threads, smem, map->ex->stream>>>(map->view(), d_q, n, d_p, d_d, d_cand);
         else
             k_nn_query_bulk<false><<<blocks, threads, smem, map->ex->stream>>>(map->view(), d_q, n, d_p, d_d, nullptr);
     } else {
-        const unsigned blocks = static_cast<unsigned>(std::min<size_t>(want, static_cast<size_t>(sms) * 4));  // 4 CTAs/SM, grid-stride
+        const unsigned blocks = static_cast<unsigned>(std::min<size_t>(want, sms * 4));  // 4 CTAs/SM, grid-stride
         if (d_cand)
             k_nn_query<true><<<blocks, threads, 0, map->ex->stream>>>(map->view(), d_q, n, d_p, d_d, d_cand);
         else
@@ -1114,6 +1065,35 @@ int kb_registration_destroy(kb_registration *reg) {
     delete reg;
     return KB_OK;
 }
+// one k_icp launch: AlignPointsToMap of the n points at d_src into out_pose / out_iters, or (system_only) one
+// BuildLinearSystem pass at the identity into reg->out[16..] and the correspondence count into reg->iout[1]
+static int icp_launch(kb_registration *reg, Exec &ex, const MapView &m, const double *d_src, int n, const SE3 &guess,
+                      double max_dist, double kscale, double *out_pose, int *out_iters, bool system_only = false) {
+    IcpParams P{};
+    P.m = m;
+    P.sc = ex.sc;
+    P.src = d_src;
+    P.work = reg->ws.work.p;
+    P.n = n;
+    P.guess = guess;
+    P.max_dist = max_dist;
+    P.kscale = kscale;
+    P.max_iter = reg->max_iter;
+    P.conv = reg->conv;
+    P.out_pose = out_pose;
+    P.out_iters = out_iters;
+    if (system_only) {
+        P.system_only = 1;
+        P.out_sys = reg->out.p + 16;
+        P.out_ncorr = reg->iout.p + 1;
+    }
+    P.use_qcache = system_only ? 0 : 1;
+    P.tag_base = ex.next_tag_base();
+    P.team = ex.team;
+    P.team.qrec = reg->ws.qrec.p;
+    P.icp_team_q = ex.icp_team_q;
+    return ex.coop(k_icp, P, system_only ? 0 : std::max<size_t>(QC_BYTES, ex.icp_smem));
+}
 static int registration_run(kb_registration *reg, const double *xyz, size_t n, kb_map *map, const SE3 &guess,
                             double max_dist, double kscale, bool system_only) {
     Exec &ex = *map->ex;
@@ -1124,28 +1104,8 @@ static int registration_run(kb_registration *reg, const double *xyz, size_t n, k
     RET(reg->iout.ensure(2));
     RET(reg->ws.qrec.ensure(std::max<size_t>(n, 1)));
     if (n) CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
-    IcpParams P;
-    P.m = map->view();
-    P.sc = ex.sc;
-    P.src = reg->ws.src.p;
-    P.work = reg->ws.work.p;
-    P.n = static_cast<int>(n);
-    P.guess = guess;
-    P.max_dist = max_dist;
-    P.kscale = kscale;
-    P.max_iter = reg->max_iter;
-    P.conv = reg->conv;
-    P.out_pose = reg->out.p;
-    P.out_iters = reg->iout.p;
-    P.system_only = system_only ? 1 : 0;
-    P.out_sys = reg->out.p + 16;
-    P.out_ncorr = reg->iout.p + 1;
-    P.use_qcache = system_only ? 0 : 1;
-    P.tag_base = ex.next_tag_base();
-    P.team = ex.team;
-    P.team.qrec = reg->ws.qrec.p;
-    P.icp_team_q = ex.icp_team_q;
-    return ex.coop(k_icp, P, system_only ? 0 : std::max<size_t>(QC_BYTES, ex.icp_smem));
+    return icp_launch(reg, ex, map->view(), reg->ws.src.p, static_cast<int>(n), guess, max_dist, kscale, reg->out.p,
+                      reg->iout.p, system_only);
 }
 int kb_registration_align_points_to_map(kb_registration *reg, const double *xyz, size_t n, const kb_map *cmap,
                                         const double initial_guess[16], double max_correspondence_distance,
@@ -1178,24 +1138,7 @@ int kb_registration_build_system(kb_registration *reg, const double *xyz, size_t
     CK(cudaMemcpyAsync(sys, reg->out.p + 16, sizeof(sys), cudaMemcpyDeviceToHost, map->ex->stream));
     CK(cudaMemcpyAsync(&nc, reg->iout.p + 1, sizeof(int), cudaMemcpyDeviceToHost, map->ex->stream));
     RET(map->ex->sync());
-    // same expansion as the device (icp_expand), host side
-    for (int i = 0; i < 36; ++i) JTJ[i] = 0.0;
-    JTJ[0] = JTJ[7] = JTJ[14] = sys[0];
-    JTJ[6 * 3 + 1] = -sys[3];
-    JTJ[6 * 3 + 2] = sys[2];
-    JTJ[6 * 4 + 0] = sys[3];
-    JTJ[6 * 4 + 2] = -sys[1];
-    JTJ[6 * 5 + 0] = -sys[2];
-    JTJ[6 * 5 + 1] = sys[1];
-    JTJ[6 * 3 + 3] = sys[4];
-    JTJ[6 * 4 + 3] = sys[5];
-    JTJ[6 * 4 + 4] = sys[6];
-    JTJ[6 * 5 + 3] = sys[7];
-    JTJ[6 * 5 + 4] = sys[8];
-    JTJ[6 * 5 + 5] = sys[9];
-    for (int i = 0; i < 6; ++i)
-        for (int j = i + 1; j < 6; ++j) JTJ[6 * i + j] = JTJ[6 * j + i];
-    for (int i = 0; i < 6; ++i) JTr[i] = sys[10 + i];
+    icp_expand(sys, JTJ, JTr);
     if (n_correspondences) *n_correspondences = nc;
     return KB_OK;
 }
@@ -1231,19 +1174,16 @@ static int align_batch_run(kb_registration *reg, kb_map *map, const double *d_xy
     Exec &ex = *map->ex;
     CK(cudaSetDevice(ex.device));
     int live = 0;  // (the host's copy of the counters can be behind a pipeline's map)
-    CK(cudaMemcpyAsync(&live, map->counters + C_LIVE, sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(&live, map->cur.counters + C_LIVE, sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
     RET(ex.sync());
     const MapView mv = map->view();
-    // k_icp's choice of the team path (kernels.cuh), made here per hypothesis
-    const bool team_ok = live != 0 && reg->max_iter > 0 && ex.icp_team_q > 0 && mv.cap <= NN_FLAT_CAP &&
-                         (static_cast<unsigned long long>(mv.mask) + 1) * mv.cap < (1ull << 31);
     std::vector<BatchHyp> hyp;  // the team hypotheses, then all of them (inlier pass)
     std::vector<size_t> single;
     int t_max = 0, n_team = 0, n_all = 0;
     size_t n_single = 1;
     for (size_t b = 0; b < B; ++b) {
         const int n = static_cast<int>(count[b]);
-        const int T = team_ok ? icp_team_size(n, ex.icp_team_q, ex.grid, ex.team.smem_bytes) : 0;
+        const int T = icp_team_plan(mv, live, reg->max_iter, ex.icp_team_q, n, ex.grid, ex.team.smem_bytes);
         if (T > 0) {
             hyp.push_back(BatchHyp{g[b], max_dist[b], kscale[b], static_cast<long long>(offset[b]), n, T, n_team, static_cast<int>(b)});
             n_team += n;
@@ -1263,27 +1203,9 @@ static int align_batch_run(kb_registration *reg, kb_map *map, const double *d_xy
     CK(cudaMemcpyAsync(reg->bhyp.p, hyp.data(), hyp.size() * sizeof(BatchHyp), cudaMemcpyHostToDevice, ex.stream));
     RET(reg->ws.qrec.ensure(std::max<size_t>(n_single, static_cast<size_t>(n_team))));
     if (!single.empty()) RET(reg->ws.work.ensure(3 * n_single));
-    for (size_t b : single) {
-        IcpParams P{};
-        P.m = mv;
-        P.sc = ex.sc;
-        P.src = d_xyz + 3 * offset[b];
-        P.work = reg->ws.work.p;
-        P.n = static_cast<int>(count[b]);
-        P.guess = g[b];
-        P.max_dist = max_dist[b];
-        P.kscale = kscale[b];
-        P.max_iter = reg->max_iter;
-        P.conv = reg->conv;
-        P.out_pose = d_poses + 16 * b;
-        P.out_iters = d_iters + b;
-        P.use_qcache = 1;
-        P.tag_base = ex.next_tag_base();
-        P.team = ex.team;
-        P.team.qrec = reg->ws.qrec.p;
-        P.icp_team_q = ex.icp_team_q;
-        RET(ex.coop(k_icp, P, std::max<size_t>(QC_BYTES, ex.icp_smem)));
-    }
+    for (size_t b : single)
+        RET(icp_launch(reg, ex, mv, d_xyz + 3 * offset[b], static_cast<int>(count[b]), g[b], max_dist[b], kscale[b],
+                       d_poses + 16 * b, d_iters + b));
     if (nh > 0) {
         const int slots = ex.grid / t_max;
         const size_t region = static_cast<size_t>(slots) * 2 * t_max * t_max * NPART;
@@ -1511,9 +1433,7 @@ int kb_voxel_down_sample(const double *xyz, size_t n, double voxel_size, double 
 static int correct_kitti_launch(Exec &ex, const double *d_in, double *d_out, size_t n) {
     if (!n) return KB_OK;
     const double angle = (0.205 * M_PI) / 180.0;  // VERTICAL_ANGLE_OFFSET, kiss_icp_pybind.cpp:130
-    int sms = 132;  // H100 SXM; replaced by the device's count below
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ex.device);
-    const unsigned blocks = static_cast<unsigned>(std::min<size_t>((n + 255) / 256, static_cast<size_t>(sms) * 8));
+    const unsigned blocks = static_cast<unsigned>(std::min<size_t>((n + 255) / 256, static_cast<size_t>(ex.sms) * 8));
     k_correct_kitti<<<blocks, 256, 0, ex.stream>>>(d_in, d_out, n, std::sin(angle), std::cos(angle));
     ++ex.launches;
     CK(cudaGetLastError());
@@ -1737,39 +1657,39 @@ static int pipeline_check(kb_pipeline *p, const void *xyz, size_t n, const void 
     return KB_OK;
 }
 
-int kb_pipeline_register_frame(kb_pipeline *p, const double *xyz, size_t n, const double *timestamps, size_t n_timestamps) {
+// the common part of kb_pipeline_register_frame[_f32|_dev]: checks, device, workspace sizing. A frame on the host
+// (elem: bytes per coordinate) and its timestamps are copied into the workspace; elem = 0: both are on the device.
+// *n_ts_used: the timestamps the frame is deskewed with (0: none).
+static int pipeline_stage(kb_pipeline *p, const void *xyz, size_t n, const double *ts, size_t n_ts, size_t elem,
+                          size_t *n_ts_used) {
     bool use_ts;
-    RET(pipeline_check(p, xyz, n, timestamps, n_timestamps, &use_ts));
-    Exec &ex = *p->ex;
-    CK(cudaSetDevice(ex.device));
-    RET(p->ws.ensure(std::max(n, use_ts ? n_timestamps : 0)));
-    RET(p->ws.ensure_pipeline(std::max(n, use_ts ? n_timestamps : 0)));
-    {
+    RET(pipeline_check(p, xyz, n, ts, n_ts, &use_ts));
+    CK(cudaSetDevice(p->ex->device));
+    *n_ts_used = use_ts ? n_ts : 0;
+    RET(p->ws.ensure(std::max(n, *n_ts_used)));
+    RET(p->ws.ensure_pipeline(std::max(n, *n_ts_used)));
+    if (elem) {
         StallTrace t("blocking: H2D enqueue");
-        if (n) CK(cudaMemcpyAsync(p->ws.in.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
-        if (use_ts) CK(cudaMemcpyAsync(p->ws.ts.p, timestamps, n_timestamps * 8, cudaMemcpyHostToDevice, ex.stream));
+        if (n) CK(cudaMemcpyAsync(p->ws.in.p, xyz, n * 3 * elem, cudaMemcpyHostToDevice, p->ex->stream));
+        if (use_ts) CK(cudaMemcpyAsync(p->ws.ts.p, ts, n_ts * 8, cudaMemcpyHostToDevice, p->ex->stream));
     }
-    return pipeline_run(p, p->ws.in.p, n, p->ws.ts.p, use_ts ? n_timestamps : 0);
+    return KB_OK;
+}
+int kb_pipeline_register_frame(kb_pipeline *p, const double *xyz, size_t n, const double *timestamps, size_t n_timestamps) {
+    size_t nt;
+    RET(pipeline_stage(p, xyz, n, timestamps, n_timestamps, sizeof(double), &nt));
+    return pipeline_run(p, p->ws.in.p, n, p->ws.ts.p, nt);
 }
 int kb_pipeline_register_frame_f32(kb_pipeline *p, const float *xyz, size_t n, const double *timestamps, size_t n_timestamps) {
-    bool use_ts;
-    RET(pipeline_check(p, xyz, n, timestamps, n_timestamps, &use_ts));
-    Exec &ex = *p->ex;
-    CK(cudaSetDevice(ex.device));
-    RET(p->ws.ensure(std::max(n, use_ts ? n_timestamps : 0)));
-    RET(p->ws.ensure_pipeline(std::max(n, use_ts ? n_timestamps : 0)));
-    if (n) CK(cudaMemcpyAsync(p->ws.in.p, xyz, n * 12, cudaMemcpyHostToDevice, ex.stream));  // half the bytes of the f64 path
-    if (use_ts) CK(cudaMemcpyAsync(p->ws.ts.p, timestamps, n_timestamps * 8, cudaMemcpyHostToDevice, ex.stream));
-    return pipeline_run(p, p->ws.in.p, n, p->ws.ts.p, use_ts ? n_timestamps : 0, true);
+    size_t nt;
+    RET(pipeline_stage(p, xyz, n, timestamps, n_timestamps, sizeof(float), &nt));  // half the bytes of the f64 path
+    return pipeline_run(p, p->ws.in.p, n, p->ws.ts.p, nt, true);
 }
 int kb_pipeline_register_frame_dev(kb_pipeline *p, const double *d_xyz, size_t n, const double *d_timestamps,
                                    size_t n_timestamps) {
-    bool use_ts;
-    RET(pipeline_check(p, d_xyz, n, d_timestamps, n_timestamps, &use_ts));
-    CK(cudaSetDevice(p->ex->device));
-    RET(p->ws.ensure(std::max(n, use_ts ? n_timestamps : 0)));
-    RET(p->ws.ensure_pipeline(std::max(n, use_ts ? n_timestamps : 0)));
-    return pipeline_run(p, d_xyz, n, d_timestamps, use_ts ? n_timestamps : 0);
+    size_t nt;
+    RET(pipeline_stage(p, d_xyz, n, d_timestamps, n_timestamps, 0, &nt));
+    return pipeline_run(p, d_xyz, n, d_timestamps, nt);
 }
 // ---- queued registration of a whole sequence ------------------------------------------------------------------
 static int queue_init(kb_pipeline *p, size_t max_n, bool any_ts, bool device_input) {
@@ -2102,38 +2022,20 @@ int kb_pipeline_debug_stamps(const kb_pipeline *p, double *ns, int n) {
     for (int i = 0; i < n && i < total; ++i) ns[i] = static_cast<double>(static_cast<long long>(t[i] - t[0]));
     return KB_OK;
 }
-int kb_debug_ldlt6(const double A[36], const double b[6], double x_loop[6], double x_unrolled[6]) {
-    // host evaluation of the two LDLT implementations the device uses (same source, __host__ __device__)
-    if (!A || !b || !x_loop || !x_unrolled) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    ldlt6_solve(A, b, x_loop);
-    ldlt6_solve_reg(A, b, x_unrolled);
-    return KB_OK;
-}
-int kb_debug_icp_solve(const double A[36], const double b[6], double x_exact[6], double x_fast[6], double T_exact[16],
-                       double T_fast[16]) {
-    // host evaluation of the exact and the latency-optimised solve/exp/compose the ICP loop uses
-    if (!A || !b || !x_exact || !x_fast || !T_exact || !T_fast) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    ldlt6_solve_reg(A, b, x_exact);
+int kb_debug_icp_solve_fast(const double A[36], const double b[6], double x_fast[6], double T_fast[16]) {
+    // host evaluation of the latency-optimised solve/exp/compose the ICP loop uses
+    if (!A || !b || !x_fast || !T_fast) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     ldlt6_solve_fast(A, b, x_fast);
-    const SE3 base = se3_exp(b);
-    se3_to_matrix(se3_mul(se3_exp(x_exact), base), T_exact);
-    se3_to_matrix(se3_mul_fast(se3_exp_fast(x_fast), base), T_fast);
+    se3_to_matrix(se3_mul_fast(se3_exp_fast(x_fast), se3_exp(b)), T_fast);
     return KB_OK;
 }
 int kb_debug_icp_schur(const double acc[16], double x_schur[6], double x_ldlt[6], int *used_schur) {
-    // host evaluation: the structured Schur solve vs the pivoted LDL^T on the same 16 accumulators
+    // host evaluation: the structured Schur solve vs the pivoted LDL^T the ICP loop falls back to, on the same 16 accumulators
     if (!acc || !x_schur || !x_ldlt || !used_schur) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     double JTJ[36], JTr[6], rhs[6];
-    for (int i = 0; i < 36; ++i) JTJ[i] = 0.0;
-    JTJ[0] = JTJ[7] = JTJ[14] = acc[0];
-    JTJ[6 * 3 + 1] = -acc[3]; JTJ[6 * 3 + 2] = acc[2]; JTJ[6 * 4 + 0] = acc[3]; JTJ[6 * 4 + 2] = -acc[1];
-    JTJ[6 * 5 + 0] = -acc[2]; JTJ[6 * 5 + 1] = acc[1];
-    JTJ[6 * 3 + 3] = acc[4]; JTJ[6 * 4 + 3] = acc[5]; JTJ[6 * 4 + 4] = acc[6];
-    JTJ[6 * 5 + 3] = acc[7]; JTJ[6 * 5 + 4] = acc[8]; JTJ[6 * 5 + 5] = acc[9];
-    for (int i = 0; i < 6; ++i)
-        for (int j = i + 1; j < 6; ++j) JTJ[6 * i + j] = JTJ[6 * j + i];
-    for (int i = 0; i < 6; ++i) { JTr[i] = acc[10 + i]; rhs[i] = -JTr[i]; }
-    ldlt6_solve_reg(JTJ, rhs, x_ldlt);
+    icp_expand(acc, JTJ, JTr);
+    for (int i = 0; i < 6; ++i) rhs[i] = -JTr[i];
+    ldlt6_solve_fast(JTJ, rhs, x_ldlt);
     *used_schur = icp_solve_schur(acc, x_schur) ? 1 : 0;
     if (!*used_schur) for (int i = 0; i < 6; ++i) x_schur[i] = x_ldlt[i];
     return KB_OK;

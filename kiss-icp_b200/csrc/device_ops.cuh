@@ -1133,8 +1133,9 @@ __device__ __forceinline__ double icp_term(int lane, const V3 &s, const V3 &t, d
     return v;
 }
 
-// expand the 16 accumulators to the (lower-triangle-complete) row-major 6x6 and rhs = -JTr
-__device__ __forceinline__ void icp_expand(const double a[NACC], double JTJ[36], double JTr[6]) {
+// expand the 16 accumulators to the (lower-triangle-complete) row-major 6x6 and JTr
+// (also on the host: kb_registration_build_system, kb_debug_icp_schur)
+__host__ __device__ __forceinline__ void icp_expand(const double a[NACC], double JTJ[36], double JTr[6]) {
     for (int i = 0; i < 36; ++i) JTJ[i] = 0.0;
     JTJ[0] = JTJ[7] = JTJ[14] = a[0];
     // rows 3..5, cols 0..2 : entry (3+i, j) = N[j][i] * w,  N = [[0,z,-y],[-z,0,x],[y,-x,0]]

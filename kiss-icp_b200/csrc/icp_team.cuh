@@ -102,7 +102,6 @@ struct TeamScratch {
 };
 
 // team size for n source points at q_per_cta points per CTA; 0 when the lists would not fit in shared memory
-// (also called on the host: kb_registration_align_batch plans its teams with it)
 __host__ __device__ __forceinline__ int icp_team_size(int n, int q_per_cta, int grid, int smem_bytes) {
     q_per_cta = max(1, min(q_per_cta, TQ_MAX));
     const int tmax = min(grid, TEAM_MAX);
@@ -115,6 +114,17 @@ __host__ __device__ __forceinline__ int icp_team_size(int n, int q_per_cta, int 
     const int warps = (qmax + TQ_PER_WARP - 1) / TQ_PER_WARP;
     if (warps > 0 && 4 * ((smem_bytes - head_bytes) / (warps * 768)) < 24) return 0;
     return T;
+}
+
+// the one decision whether ICP on n source points runs on a team, and on how many CTAs: 0 for the whole-grid loop (or
+// nothing to iterate: empty map, max_iter <= 0). k_register_frame, k_icp and kb_registration_align_batch's planner all
+// take it from here, which keeps a batched alignment bit-identical to the single call.
+__host__ __device__ __forceinline__ int icp_team_plan(const MapView &m, int live, int max_iter, int team_q, int n, int grid,
+                                                      int smem_bytes) {
+    if (live != 0 && max_iter > 0 && team_q > 0 && m.cap <= NN_FLAT_CAP &&
+        (static_cast<unsigned long long>(m.mask) + 1) * m.cap < (1ull << 31))
+        return icp_team_size(n, team_q, grid, smem_bytes);
+    return 0;
 }
 
 // GetClosestNeighbor (core/VoxelHashMap.cpp:46-70) for one point by one warp + the list of candidates that can

@@ -172,11 +172,9 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const FrameParams P
     const SE3 guess = se3_mul(last_pose, last_delta);
     // ICP (KissICP.cpp:50-54)
     const int G = static_cast<int>(gridDim.x);
-    const bool icp_runs = __ldcg(&P.m.counters[C_LIVE]) != 0 && P.max_iter > 0;  // voxel_map.Empty() -> initial_guess
-    int T = 0;
-    if (icp_runs && P.icp_team_q > 0 && P.m.cap <= NN_FLAT_CAP && (static_cast<unsigned long long>(P.m.mask) + 1) * P.m.cap < (1ull << 31)) {
-        T = icp_team_size(n_src, P.icp_team_q, G, P.team.smem_bytes);
-    }
+    const int live = __ldcg(&P.m.counters[C_LIVE]);
+    const bool icp_runs = live != 0 && P.max_iter > 0;  // voxel_map.Empty() -> initial_guess
+    const int T = icp_team_plan(P.m, live, P.max_iter, P.icp_team_q, n_src, G, P.team.smem_bytes);
     if (T > 0) {
         if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[30] = globaltimer_ns();
         icp_fill_pass(g, sh, P.m, fr.src, n_src, guess, P.team.qrec, P.team.radius_frac, P.sc.bar + BAR_TICKET);
@@ -366,11 +364,9 @@ __global__ void __launch_bounds__(BLOCK, 1) k_icp(const IcpParams P) {
         }
         return;
     }
-    int T = 0;
-    if (__ldcg(&P.m.counters[C_LIVE]) != 0 && P.max_iter > 0 && P.icp_team_q > 0 && P.use_qcache && P.m.cap <= NN_FLAT_CAP &&
-        (static_cast<unsigned long long>(P.m.mask) + 1) * P.m.cap < (1ull << 31)) {
-        T = icp_team_size(P.n, P.icp_team_q, static_cast<int>(gridDim.x), P.team.smem_bytes);
-    }
+    const int T = P.use_qcache ? icp_team_plan(P.m, __ldcg(&P.m.counters[C_LIVE]), P.max_iter, P.icp_team_q, P.n,
+                                               static_cast<int>(gridDim.x), P.team.smem_bytes)
+                               : 0;
     if (T > 0) {
         icp_fill_pass(g, sh, P.m, P.src, P.n, P.guess, P.team.qrec, P.team.radius_frac, P.sc.bar + BAR_TICKET);
         g.sync();
@@ -396,7 +392,7 @@ struct BatchHyp {
     double max_dist, kscale;
     long long src_off;
     int n;
-    int T;      // team size, icp_team_size(n, ...) on the full grid: the split of the single call
+    int T;      // team size, icp_team_plan(...) on the full grid: the split of the single call
     int q_off;
     int out;    // index of the hypothesis in the caller's arrays
 };

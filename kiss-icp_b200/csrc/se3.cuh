@@ -294,107 +294,9 @@ KB_HD void se3_to_matrix(const SE3 &T, double M[16]) {
     M[15] = 1.0;
 }
 
-// LDL^T with diagonal pivoting of a symmetric 6x6 (lower triangle of A, row-major) and solve,
-// following Eigen 3.4 LDLT (Lower, unblocked): first-max pivot, |pivot| <= DBL_MIN -> 0 in D^+.
-KB_HD void ldlt6_solve(const double A_in[36], const double b[6], double x[6]) {
-    constexpr int N = 6;
-    double mat[N][N];
-    for (int i = 0; i < N; ++i)
-        for (int j = 0; j < N; ++j) mat[i][j] = A_in[N * i + j];
-    int tr[N];
-    double temp[N];
-    for (int k = 0; k < N; ++k) {
-        int big = k;
-        double best = fabs(mat[k][k]);
-        for (int i = k + 1; i < N; ++i) {
-            const double v = fabs(mat[i][i]);
-            if (v > best) {
-                best = v;
-                big = i;
-            }
-        }
-        tr[k] = big;
-        if (k != big) {
-            const int s = N - big - 1;
-            for (int j = 0; j < k; ++j) {
-                const double t = mat[k][j];
-                mat[k][j] = mat[big][j];
-                mat[big][j] = t;
-            }
-            for (int i = 0; i < s; ++i) {
-                const double t = mat[N - s + i][k];
-                mat[N - s + i][k] = mat[N - s + i][big];
-                mat[N - s + i][big] = t;
-            }
-            {
-                const double t = mat[k][k];
-                mat[k][k] = mat[big][big];
-                mat[big][big] = t;
-            }
-            for (int i = k + 1; i < big; ++i) {
-                const double t = mat[i][k];
-                mat[i][k] = mat[big][i];
-                mat[big][i] = t;
-            }
-        }
-        const int rs = N - k - 1;
-        if (k > 0) {
-            for (int j = 0; j < k; ++j) temp[j] = mat[j][j] * mat[k][j];
-            double acc = 0.0;
-            for (int j = 0; j < k; ++j) acc += mat[k][j] * temp[j];
-            mat[k][k] -= acc;
-            for (int i = 0; i < rs; ++i) {
-                double a2 = 0.0;
-                for (int j = 0; j < k; ++j) a2 += mat[k + 1 + i][j] * temp[j];
-                mat[k + 1 + i][k] -= a2;
-            }
-        }
-        const double akk = mat[k][k];
-        const bool valid = fabs(akk) > 0.0;
-        if (k == 0 && !valid) {
-            for (int j = 0; j < N; ++j) tr[j] = j;
-            break;
-        }
-        if (rs > 0 && valid)
-            for (int i = 0; i < rs; ++i) mat[k + 1 + i][k] /= akk;
-    }
-    double d[N];
-    for (int i = 0; i < N; ++i) d[i] = b[i];
-    for (int k = 0; k < N; ++k)
-        if (tr[k] != k) {
-            const double t = d[k];
-            d[k] = d[tr[k]];
-            d[tr[k]] = t;
-        }
-    for (int i = 0; i < N; ++i) {
-        double acc = d[i];
-        for (int j = 0; j < i; ++j) acc -= mat[i][j] * d[j];
-        d[i] = acc;
-    }
-    for (int i = 0; i < N; ++i) {
-        if (fabs(mat[i][i]) > DBL_MIN)
-            d[i] /= mat[i][i];
-        else
-            d[i] = 0.0;
-    }
-    for (int i = N - 1; i >= 0; --i) {
-        double acc = d[i];
-        for (int j = i + 1; j < N; ++j) acc -= mat[j][i] * d[j];
-        d[i] = acc;
-    }
-    for (int k = N - 1; k >= 0; --k)
-        if (tr[k] != k) {
-            const double t = d[k];
-            d[k] = d[tr[k]];
-            d[tr[k]] = t;
-        }
-    for (int i = 0; i < N; ++i) x[i] = d[i];
-}
-
-// Same algorithm as ldlt6_solve with every index resolved at compile time (pivot swaps are
-// expanded into one guarded block per possible pivot row), so the 6x6 lives in registers
-// instead of local memory: the ICP solve is a single-thread dependent chain and this makes
-// it ~5x shorter. Bit-identical to ldlt6_solve.
+// Pieces of ldlt6_solve_fast (below): LDL^T with diagonal pivoting of a symmetric 6x6 following Eigen 3.4 LDLT (Lower,
+// unblocked), first-max pivot. Every index is resolved at compile time (a pivot swap is expanded into one guarded block
+// per possible pivot row), so the 6x6 lives in registers instead of local memory.
 template <int K, int BIG>
 KB_HD void ldlt6_swap(double (&mat)[6][6]) {
     constexpr int N = 6;
@@ -425,52 +327,6 @@ KB_HD void ldlt6_swap(double (&mat)[6][6]) {
 }
 
 template <int K>
-KB_HD bool ldlt6_step(double (&mat)[6][6], int (&tr)[6]) {
-    constexpr int N = 6;
-    int big = K;
-    double best = fabs(mat[K][K]);
-#pragma unroll
-    for (int i = K + 1; i < N; ++i) {
-        const double v = fabs(mat[i][i]);
-        if (v > best) {
-            best = v;
-            big = i;
-        }
-    }
-    tr[K] = big;
-    if (K + 1 < N && big == K + 1) ldlt6_swap<K, (K + 1 < N ? K + 1 : K)>(mat);
-    if (K + 2 < N && big == K + 2) ldlt6_swap<K, (K + 2 < N ? K + 2 : K)>(mat);
-    if (K + 3 < N && big == K + 3) ldlt6_swap<K, (K + 3 < N ? K + 3 : K)>(mat);
-    if (K + 4 < N && big == K + 4) ldlt6_swap<K, (K + 4 < N ? K + 4 : K)>(mat);
-    if (K + 5 < N && big == K + 5) ldlt6_swap<K, (K + 5 < N ? K + 5 : K)>(mat);
-    constexpr int RS = N - K - 1;
-    if (K > 0) {
-        double temp[6];
-#pragma unroll
-        for (int j = 0; j < K; ++j) temp[j] = mat[j][j] * mat[K][j];
-        double acc = 0.0;
-#pragma unroll
-        for (int j = 0; j < K; ++j) acc += mat[K][j] * temp[j];
-        mat[K][K] -= acc;
-#pragma unroll
-        for (int i = 0; i < RS; ++i) {
-            double a2 = 0.0;
-#pragma unroll
-            for (int j = 0; j < K; ++j) a2 += mat[K + 1 + i][j] * temp[j];
-            mat[K + 1 + i][K] -= a2;
-        }
-    }
-    const double akk = mat[K][K];
-    const bool valid = fabs(akk) > 0.0;
-    if (K == 0 && !valid) return false;  // whole diagonal zero: identity transpositions, stop
-    if (RS > 0 && valid) {
-#pragma unroll
-        for (int i = 0; i < RS; ++i) mat[K + 1 + i][K] /= akk;
-    }
-    return true;
-}
-
-template <int K>
 KB_HD void ldlt6_apply_tr(double (&d)[6], int big) {
 #pragma unroll
     for (int b = K + 1; b < 6; ++b)
@@ -481,68 +337,13 @@ KB_HD void ldlt6_apply_tr(double (&d)[6], int big) {
         }
 }
 
-KB_HD void ldlt6_solve_reg(const double A_in[36], const double b[6], double x[6]) {
-    constexpr int N = 6;
-    double mat[6][6];
-#pragma unroll
-    for (int i = 0; i < N; ++i)
-#pragma unroll
-        for (int j = 0; j < N; ++j) mat[i][j] = A_in[N * i + j];
-    int tr[6] = {0, 1, 2, 3, 4, 5};
-    if (ldlt6_step<0>(mat, tr)) {
-        ldlt6_step<1>(mat, tr);
-        ldlt6_step<2>(mat, tr);
-        ldlt6_step<3>(mat, tr);
-        ldlt6_step<4>(mat, tr);
-        ldlt6_step<5>(mat, tr);
-    } else {
-        tr[0] = 0;
-    }
-    double d[6];
-#pragma unroll
-    for (int i = 0; i < N; ++i) d[i] = b[i];
-    ldlt6_apply_tr<0>(d, tr[0]);
-    ldlt6_apply_tr<1>(d, tr[1]);
-    ldlt6_apply_tr<2>(d, tr[2]);
-    ldlt6_apply_tr<3>(d, tr[3]);
-    ldlt6_apply_tr<4>(d, tr[4]);
-#pragma unroll
-    for (int i = 0; i < N; ++i) {
-        double acc = d[i];
-#pragma unroll
-        for (int j = 0; j < i; ++j) acc -= mat[i][j] * d[j];
-        d[i] = acc;
-    }
-#pragma unroll
-    for (int i = 0; i < N; ++i) {
-        if (fabs(mat[i][i]) > DBL_MIN)
-            d[i] /= mat[i][i];
-        else
-            d[i] = 0.0;
-    }
-#pragma unroll
-    for (int i = N - 1; i >= 0; --i) {
-        double acc = d[i];
-#pragma unroll
-        for (int j = i + 1; j < N; ++j) acc -= mat[j][i] * d[j];
-        d[i] = acc;
-    }
-    ldlt6_apply_tr<4>(d, tr[4]);
-    ldlt6_apply_tr<3>(d, tr[3]);
-    ldlt6_apply_tr<2>(d, tr[2]);
-    ldlt6_apply_tr<1>(d, tr[1]);
-    ldlt6_apply_tr<0>(d, tr[0]);
-#pragma unroll
-    for (int i = 0; i < N; ++i) x[i] = d[i];
-}
-
 // ---- latency-optimised variants for the ICP inner loop -------------------------------------
 // The ICP solve is a single-thread dependent chain executed once per iteration; a DDIV, DSQRT
 // or sin/cos costs an order of magnitude more latency than a DADD/DMUL (tools/latency_probe.cu
-// measures them). These variants use ONE reciprocal where the exact forms divide
-// several times, and one sincos(theta/2) with double-angle identities instead of four
-// separate sin/cos calls. They differ from the exact forms by a few ulps (tests bound the
-// difference at 1e-13 relative) — far inside the 1e-4 m / 1e-4 rad parity budget.
+// measures them). The LDL^T multiplies by ONE reciprocal per pivot where Eigen's divides, and
+// se3_exp_fast takes one sincos(theta/2) with double-angle identities instead of se3_exp's four
+// separate sin/cos calls. They differ from Eigen's LDLT and from se3_exp / se3_mul by a few ulps
+// (tests bound the difference against the oracle) — far inside the 1e-4 m / 1e-4 rad parity budget.
 // ~1-ulp reciprocal: MUFU seed (rcp.approx.ftz.f64, ~20 bits) + two Newton steps in FMA —
 // a fraction of the latency of an IEEE DDIV (host: plain division).
 KB_HD double fast_rcp(double x) {
