@@ -281,6 +281,41 @@ int kb_pipeline_set_state(kb_pipeline *p, const kb_pipeline_state *s);
 int kb_threshold_get_state(const kb_threshold *th, double *model_sse, int *num_samples);
 int kb_threshold_set_state(kb_threshold *th, double model_sse, int num_samples);
 
+/* ---- localization in a fixed prior map ----------------------------------------------------
+ * No reference counterpart. A localizer registers every frame with RegisterFrame (KissICP.cpp:35-68) without the map
+ * update (:61, local_map_.Update) against a prior map that it never writes, and reports how well each frame fits. */
+/* The fit of one frame at its final pose, with that frame's (3 sigma, sigma): n_correspondences = source points whose
+ * nearest map neighbour is closer than 3 sigma (what kb_registration_build_system counts for the source mapped by the
+ * pose), n_source = source points, sum_sq_residual = sum of |r|^2 over the correspondences (unweighted), JTJ = the
+ * Geman-McClure-weighted J^T W J of kb_registration_build_system for the same input, row-major, symmetric: the
+ * information matrix of the pose. Bit-identical from run to run for a given grid size (kb_set_grid_blocks). */
+typedef struct kb_fit {
+    int n_correspondences, n_source;
+    double sum_sq_residual;
+    double JTJ[36];
+} kb_fit;
+/* A pipeline that localizes in `prior` instead of building a map. The prior must be on the pipeline's device (the
+ * calling thread's, kb_set_device) and have cfg's voxel_size and max_points_per_voxel, else KB_ERR_INVALID_ARG; its
+ * max_distance does not matter (nothing is evicted). A pipeline's own map (kb_pipeline_voxel_map of an odometry
+ * pipeline) cannot be a prior. Waits once for the work queued on the prior. The localizer allocates no voxel table;
+ * kb_pipeline_voxel_map returns the prior, borrowed. While localizers exist, every call that would change or free the
+ * prior (kb_map_clear, _update_origin, _update_pose, _add_points, _remove_far, _compact, _load[_dev], _destroy) fails
+ * with KB_ERR_INVALID_ARG and changes nothing; read-only calls keep working. Several localizers, on any host threads,
+ * may share one prior. kb_pipeline_destroy of a localizer waits for its own streams before it releases the prior.
+ * Every other kb_pipeline_* call works as on an odometry pipeline; set_pose seeds the track (e.g. from a
+ * kb_registration_align_batch relocalization). */
+int kb_pipeline_create_localizer(const kb_config *cfg, const kb_map *prior, kb_pipeline **out);
+/* localizers reading the map (0: it may be changed) */
+int kb_map_readers(const kb_map *map, int *out);
+/* the fit of the last frame (all zero before the first); KB_ERR_INVALID_ARG on an odometry pipeline */
+int kb_pipeline_last_fit(const kb_pipeline *p, kb_fit *out);
+/* kb_pipeline_register_frames with one fit per frame in fits_out[count] (may be NULL), read behind the queue like
+ * the poses. Same poses as kb_pipeline_register_frames. A non-NULL fits_out on an odometry pipeline is
+ * KB_ERR_INVALID_ARG. */
+int kb_pipeline_register_frames_fit(kb_pipeline *p, const void *const *xyz, const size_t *n,
+                                    const double *const *timestamps, const size_t *n_timestamps, size_t count,
+                                    int layout, double *poses_out, kb_fit *fits_out);
+
 #ifdef __cplusplus
 }
 #endif

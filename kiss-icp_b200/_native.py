@@ -41,10 +41,10 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/api.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
+    """Compile csrc/api.cu and csrc/localize.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in sources())
     if force or stale:
-        cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH, os.path.join(CSRC, "api.cu")]
+        cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH, os.path.join(CSRC, "api.cu"), os.path.join(CSRC, "localize.cu")]
         if verbose:
             print(" ".join(cmd))
         env = dict(os.environ)
@@ -85,6 +85,11 @@ class FrameStats(C.Structure):
 class PipelineState(C.Structure):
     """kb_pipeline_state: pose / delta in Sophus::SE3d::params() order {qx,qy,qz,qw,tx,ty,tz}"""
     _fields_ = [("pose", dbl * 7), ("delta", dbl * 7), ("model_sse", dbl), ("num_samples", i32)]
+
+
+class Fit(C.Structure):
+    """kb_fit: the fit of one localized frame at its final pose"""
+    _fields_ = [("n_correspondences", i32), ("n_source", i32), ("sum_sq_residual", dbl), ("JTJ", dbl * 36)]
 
 
 # every exported symbol of include/kiss_icp_b200.h: name -> (restype, argtypes)
@@ -170,6 +175,10 @@ SIGNATURES = {
     "kb_pipeline_set_state": (i32, [vp, C.POINTER(PipelineState)]),
     "kb_threshold_get_state": (i32, [vp, C.POINTER(dbl), C.POINTER(i32)]),
     "kb_threshold_set_state": (i32, [vp, dbl, i32]),
+    "kb_pipeline_create_localizer": (i32, [C.POINTER(Config), vp, C.POINTER(vp)]),
+    "kb_map_readers": (i32, [vp, C.POINTER(i32)]),
+    "kb_pipeline_last_fit": (i32, [vp, C.POINTER(Fit)]),
+    "kb_pipeline_register_frames_fit": (i32, [vp, vp, vp, vp, vp, sz, i32, vp, vp]),
 }
 
 

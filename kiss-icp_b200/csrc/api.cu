@@ -9,6 +9,7 @@
 
 #include <algorithm>
 #include <array>
+#include <atomic>
 #include <chrono>
 #include <cmath>
 #include <cstdarg>
@@ -83,6 +84,7 @@ int watchdog_init(int device) {
     unsigned init[8] = {0, 0, 0, 0, 0, 0, 0, 24};
     if (const char *e = std::getenv("KB_WATCHDOG_SHIFT")) init[7] = static_cast<unsigned>(std::max(10, std::min(std::atoi(e), 31)));
     CK(cudaMemcpyToSymbol(g_kb_wd, init, sizeof(init)));
+    CK(localize_watchdog_init(d, init));  // the localizer kernel's module has its own copies
     g_wd[device].host = h;
     return KB_OK;
 }
@@ -104,6 +106,7 @@ int watchdog_check(int device) {
     h[0] = 0;
     unsigned zero = 0;
     cudaMemcpyToSymbol(g_kb_wd, &zero, sizeof(zero));  // re-arm
+    localize_watchdog_rearm();
     static const char *names[] = {"?", "grid barrier", "ICP gather", "ICP result record", "ICP team gather", "NN bulk copy"};
     std::string marks;
     unsigned m[256];
@@ -278,13 +281,17 @@ struct Exec {
     }
     template <class P>
     int coop(void (*kern)(P), const P &p, size_t smem = 0, bool self_reset = false) {
+        return coop_raw(reinterpret_cast<const void *>(kern), const_cast<P *>(&p), smem, self_reset);
+    }
+    // `kern` takes one parameter struct, `param` points to it (a kernel of another device module: localize_kernel())
+    int coop_raw(const void *kern, void *param, size_t smem, bool self_reset) {
         CK(cudaSetDevice(device));
-        RET(opt_in_smem(reinterpret_cast<const void *>(kern), smem));
+        RET(opt_in_smem(kern, smem));
         if (!self_reset || bar_dirty)  // kernels that end with Grid::finish() leave the barrier words zeroed themselves
             CK(cudaMemsetAsync(sc.bar, 0, BAR_WORDS * sizeof(unsigned), stream));
         bar_dirty = !self_reset;
-        void *args[] = {const_cast<P *>(&p)};
-        CK(cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(kern), dim3(grid), dim3(BLOCK), args, smem, stream));
+        void *args[] = {param};
+        CK(cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(BLOCK), args, smem, stream));
         ++launches;
         return KB_OK;
     }
@@ -417,6 +424,9 @@ struct kb_map {
     DBuf<double> q_in, q_outp, q_outd;
     DBuf<unsigned long long> q_cand;
     bool borrowed = false;
+    // localizers reading this map (kb_pipeline_create_localizer), possibly from several host threads: while it is
+    // non-zero every call that would change or free the map fails and changes nothing
+    std::atomic<int> readers{0};
 
     MapView view_of(const Table &t) const {
         MapView m;
@@ -665,6 +675,13 @@ struct kb_pipeline {
     std::shared_ptr<Exec> ex;
     kb_config cfg;
     kb_map *map = nullptr;
+    // a localizer (kb_pipeline_create_localizer): `map` is the prior map, borrowed and never written; every frame
+    // also computes its fit, into fit_dev[0] (blocking calls) or fit_dev[1 + k % Q_DEPTH] (queued frame k)
+    bool localizer = false;
+    DBuf<double> fit_part;           // [FIT_VALS][grid] per-CTA partials of the fit pass
+    FitResult *fit_dev = nullptr;    // [1 + Q_DEPTH]
+    FitResult *fit_host = nullptr;   // [1 + Q_DEPTH] pinned copies
+    FitResult last_fit{};
     Work ws;
     PipeState *d_state = nullptr;
     FrameResult *d_res = nullptr;
@@ -707,7 +724,9 @@ struct kb_pipeline {
         if (res_stream) cudaStreamDestroy(res_stream);
         if (q_res_dev) cudaFree(q_res_dev);
         if (q_res) cudaFreeHost(q_res);
-        delete map;
+        if (fit_dev) cudaFree(fit_dev);
+        if (fit_host) cudaFreeHost(fit_host);
+        if (!localizer) delete map;
         if (d_state) cudaFree(d_state);
         if (d_res) cudaFree(d_res);
         if (h_res) cudaFreeHost(h_res);
@@ -788,12 +807,22 @@ static int map_create_impl(double voxel_size, double max_distance, unsigned cap,
 int kb_map_create(double voxel_size, double max_distance, unsigned max_points_per_voxel, kb_map **out) {
     return map_create_impl(voxel_size, max_distance, max_points_per_voxel, nullptr, out);
 }
+// every call that changes or frees a map fails while localizers read it (kb_pipeline_create_localizer)
+static int map_in_use(const kb_map *map) {
+    const int r = map->readers.load();
+    if (r) return fail(KB_ERR_INVALID_ARG, "the map is in use by %d localizer%s: it cannot be changed or destroyed", r, r == 1 ? "" : "s");
+    return KB_OK;
+}
 int kb_map_destroy(kb_map *map) {
-    if (map && !map->borrowed) delete map;
+    if (map && !map->borrowed) {
+        RET(map_in_use(map));
+        delete map;
+    }
     return KB_OK;
 }
 int kb_map_clear(kb_map *map) {
     if (!map) return fail(KB_ERR_INVALID_ARG, "map == NULL");
+    RET(map_in_use(map));
     CK(cudaSetDevice(map->ex->device));
     RET(map->reset_table(map->cur));
     std::memset(map->h_counters, 0, sizeof(map->h_counters));
@@ -806,24 +835,29 @@ int kb_map_empty(const kb_map *map, int *out_is_empty) {
 }
 int kb_map_update_origin(kb_map *map, const double *xyz, size_t n, const double origin[3]) {
     if (!map || (!xyz && n) || !origin) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(map_in_use(map));
     return map->update_host(xyz, n, false, se3_identity(), true, true, V3{origin[0], origin[1], origin[2]});
 }
 int kb_map_update_pose(kb_map *map, const double *xyz, size_t n, const double pose[16]) {
     if (!map || (!xyz && n) || !pose) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(map_in_use(map));
     SE3 T;
     if (!to_se3(pose, &T)) return fail(KB_ERR_NOT_SE3, "pose is not in SE(3)");
     return map->update_host(xyz, n, true, T, true, true, T.t);
 }
 int kb_map_add_points(kb_map *map, const double *xyz, size_t n) {
     if (!map || (!xyz && n)) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(map_in_use(map));
     return map->update_host(xyz, n, false, se3_identity(), true, false, V3{0, 0, 0});
 }
 int kb_map_remove_far(kb_map *map, const double origin[3]) {
     if (!map || !origin) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(map_in_use(map));
     return map->update_host(nullptr, 0, false, se3_identity(), false, true, V3{origin[0], origin[1], origin[2]});
 }
 int kb_map_compact(kb_map *map) {
     if (!map) return fail(KB_ERR_INVALID_ARG, "map == NULL");
+    RET(map_in_use(map));
     const size_t live = static_cast<size_t>(map->h_counters[C_LIVE]);
     const size_t want = std::max<size_t>(pow2_at_least(2 * live + 2), size_t(1) << 14);
     if (want >= map->cur.capacity && map->h_counters[C_TOMB] == 0) return KB_OK;
@@ -833,6 +867,11 @@ int kb_map_compact(kb_map *map) {
 int kb_map_num_points(const kb_map *map, size_t *out) {
     if (!map || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     *out = static_cast<size_t>(map->h_counters[C_POINTS]);
+    return KB_OK;
+}
+int kb_map_readers(const kb_map *map, int *out) {
+    if (!map || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *out = map->readers.load();
     return KB_OK;
 }
 int kb_map_num_voxels(const kb_map *map, size_t *out) {
@@ -912,6 +951,7 @@ int kb_map_dump(const kb_map *cmap, int *voxels, int *counts, double *points, si
 static int map_load_check(const kb_map *map, const void *voxels, const void *counts, const void *points, size_t n_voxels,
                           size_t n_points) {
     if (!map || (n_voxels && (!voxels || !counts)) || (n_points && !points)) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(map_in_use(map));
     if (n_voxels > static_cast<size_t>(INT_MAX) || n_points > static_cast<size_t>(INT_MAX))
         return fail(KB_ERR_INVALID_ARG, "map too large (%zu voxels, %zu points)", n_voxels, n_points);
     return KB_OK;
@@ -1488,6 +1528,20 @@ static int pipeline_push_state(kb_pipeline *p, const SE3 &pose, const SE3 &delta
     return p->ex->sync();
 }
 
+// the pipeline's device state and result buffers; the state of a new sequence (identity pose and delta, the initial threshold)
+static int pipeline_init_state(kb_pipeline *p) {
+    CK(cudaMalloc(&p->d_state, sizeof(PipeState)));
+    CK(cudaMalloc(&p->d_res, sizeof(FrameResult)));
+    CK(cudaMemsetAsync(p->d_res, 0, sizeof(FrameResult), p->ex->stream));  // (fields a launch does not write are read back too)
+    CK(cudaHostAlloc(&p->h_res, sizeof(FrameResult), cudaHostAllocDefault));
+    std::memset(&p->last, 0, sizeof(p->last));
+    se3_to_matrix(se3_identity(), p->last.pose);
+    se3_to_matrix(se3_identity(), p->last.delta);
+    p->last.model_sse = p->cfg.initial_threshold * p->cfg.initial_threshold;
+    p->last.num_samples = 1;
+    return pipeline_push_state(p, se3_identity(), se3_identity(), p->last.model_sse, 1);
+}
+
 int kb_pipeline_create(const kb_config *cfg, kb_pipeline **out) {
     if (!cfg || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (cfg->max_num_iterations > 8000) return fail(KB_ERR_INVALID_ARG, "max_num_iterations > 8000 is not supported");
@@ -1515,25 +1569,56 @@ int kb_pipeline_create(const kb_config *cfg, kb_pipeline **out) {
             if (st != KB_OK) cudaGetLastError();
         }
     }
-    CK(cudaMalloc(&p->d_state, sizeof(PipeState)));
-    CK(cudaMalloc(&p->d_res, sizeof(FrameResult)));
-    CK(cudaMemsetAsync(p->d_res, 0, sizeof(FrameResult), p->ex->stream));  // (fields a launch does not write are read back too)
-    CK(cudaHostAlloc(&p->h_res, sizeof(FrameResult), cudaHostAllocDefault));
-    std::memset(&p->last, 0, sizeof(p->last));
-    se3_to_matrix(se3_identity(), p->last.pose);
-    se3_to_matrix(se3_identity(), p->last.delta);
-    p->last.model_sse = cfg->initial_threshold * cfg->initial_threshold;
-    p->last.num_samples = 1;
-    RET(pipeline_push_state(p.get(), se3_identity(), se3_identity(), p->last.model_sse, 1));
+    RET(pipeline_init_state(p.get()));
+    *out = p.release();
+    return KB_OK;
+}
+int kb_pipeline_create_localizer(const kb_config *cfg, const kb_map *cprior, kb_pipeline **out) {
+    kb_map *prior = const_cast<kb_map *>(cprior);
+    if (!cfg || !prior || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (cfg->max_num_iterations > 8000) return fail(KB_ERR_INVALID_ARG, "max_num_iterations > 8000 is not supported");
+    if (prior->borrowed)
+        return fail(KB_ERR_INVALID_ARG, "a pipeline's own voxel map cannot be a prior map: dump it and load it into a map of its own");
+    if (prior->voxel_size != cfg->voxel_size || static_cast<long long>(prior->cap) != cfg->max_points_per_voxel)
+        return fail(KB_ERR_INVALID_ARG, "prior map with voxel_size %g, max_points_per_voxel %u; the config has %g, %d", prior->voxel_size,
+                    prior->cap, cfg->voxel_size, cfg->max_points_per_voxel);
+    auto p = std::make_unique<kb_pipeline>();
+    p->localizer = true;  // from here on the destructor leaves the map alone
+    p->map = prior;
+    RET(make_exec(&p->ex));
+    if (p->ex->device != prior->ex->device)
+        return fail(KB_ERR_INVALID_ARG, "the prior map is on device %d, the localizer would run on device %d", prior->ex->device, p->ex->device);
+    p->cfg = *cfg;
+    // everything queued on the map before (a load, updates, asynchronous queries) is complete before a frame reads it
+    RET(prior->ex->sync());
+    CK(cudaSetDevice(p->ex->device));
+    RET(p->fit_part.ensure(static_cast<size_t>(FIT_VALS) * p->ex->grid));
+    CK(cudaMalloc(&p->fit_dev, sizeof(FitResult) * (1 + kb_pipeline::Q_DEPTH)));
+    CK(cudaMemsetAsync(p->fit_dev, 0, sizeof(FitResult) * (1 + kb_pipeline::Q_DEPTH), p->ex->stream));
+    CK(cudaHostAlloc(&p->fit_host, sizeof(FitResult) * (1 + kb_pipeline::Q_DEPTH), cudaHostAllocDefault));
+    RET(pipeline_init_state(p.get()));
+    prior->readers.fetch_add(1);
     *out = p.release();
     return KB_OK;
 }
 int kb_pipeline_destroy(kb_pipeline *p) {
     if (p) {
+        cudaSetDevice(p->ex->device);
+        if (p->localizer) {
+            // the prior must stay readable until this localizer's launches and copies have finished
+            if (!device_is_stuck(p->ex->device)) {
+                p->ex->sync();
+                if (p->copy_stream) cudaStreamSynchronize(p->copy_stream);
+                if (p->res_stream) cudaStreamSynchronize(p->res_stream);
+            }
+            p->map->readers.fetch_sub(1);
+            p->map = nullptr;
+            delete p;
+            return KB_OK;
+        }
         p->map->borrowed = false;
         kb_map *m = p->map;
         p->map = nullptr;
-        cudaSetDevice(p->ex->device);
         delete m;
         delete p;
     }
@@ -1549,10 +1634,12 @@ static size_t pipeline_extra(const kb_pipeline *p, size_t n) {
 
 // enqueue one RegisterFrame on the pipeline's stream; the result goes to `res` (device-visible memory)
 // `next_xyz` (may be null): the frame after this one, already on the device, no timestamps -> its front end is prefetched
+// `fit` (localizers only): where the frame's fit goes
 static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, size_t n, const double *d_ts, size_t n_ts,
-                           bool in_f32, FrameResult *res, const double *next_xyz = nullptr, size_t next_n = 0) {
+                           bool in_f32, FrameResult *res, FitResult *fit, const double *next_xyz = nullptr, size_t next_n = 0) {
     Exec &ex = *p->ex;
-    FrameParams P;
+    LocalizeParams L;
+    FrameParams &P = L;
     P.m = p->map->view();
     P.sc = ex.sc;
     P.team = ex.team;
@@ -1579,7 +1666,12 @@ static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, si
     P.use_qcache = 1;
     P.tag_base = ex.next_tag_base();
     P.in_f32 = in_f32 ? 1 : 0;
-    return ex.coop(k_register_frame, P, std::max<size_t>(QC_BYTES, ex.icp_smem), true);
+    const size_t smem = std::max<size_t>(QC_BYTES, ex.icp_smem);
+    if (p->localizer) {
+        L.fit = FitOut{p->fit_part.p, fit};
+        return ex.coop_raw(localize_kernel(), &L, smem, true);
+    }
+    return ex.coop(k_register_frame<FrameParams>, P, smem, true);
 }
 
 // take over the result of a frame that ran (not vetoed): host mirror of the counters, history
@@ -1587,10 +1679,12 @@ static int pipeline_absorb(kb_pipeline *p, const FrameResult &r, size_t n, long 
     p->last = r;
     p->last_id = id;
     p->has_last = true;
-    p->map->h_counters[C_LIVE] = p->last.map_live;
-    p->map->h_counters[C_TOMB] = p->last.map_tomb;
-    p->map->h_counters[C_POINTS] = p->last.map_points;
-    p->map->h_counters[C_STATUS] = p->last.map_status;
+    if (!p->localizer) {  // (a prior map does not change: its host mirror is its owner's)
+        p->map->h_counters[C_LIVE] = p->last.map_live;
+        p->map->h_counters[C_TOMB] = p->last.map_tomb;
+        p->map->h_counters[C_POINTS] = p->last.map_points;
+        p->map->h_counters[C_STATUS] = p->last.map_status;
+    }
     if (p->history.size() < p->history_cap) {
         kb_frame_stats st;
         std::memcpy(st.pose, p->last.pose, sizeof(st.pose));
@@ -1626,22 +1720,26 @@ static int pipeline_after_veto(kb_pipeline *p, const FrameResult &r, size_t n) {
 // blocking RegisterFrame on device-resident input
 static int pipeline_run(kb_pipeline *p, const double *d_xyz, size_t n, const double *d_ts, size_t n_ts, bool in_f32 = false) {
     Exec &ex = *p->ex;
-    RET(p->map->ensure_capacity(pipeline_extra(p, n)));
+    if (!p->localizer) RET(p->map->ensure_capacity(pipeline_extra(p, n)));
     const long long id = p->next_id++;
     for (int attempt = 0; attempt < 3; ++attempt) {
         {
             StallTrace t("blocking: launch");
-            RET(pipeline_launch(p, id, d_xyz, n, d_ts, n_ts, in_f32, p->d_res));
+            RET(pipeline_launch(p, id, d_xyz, n, d_ts, n_ts, in_f32, p->d_res, p->fit_dev));
         }
         {
             StallTrace t("blocking: result D2H enqueue");
             CK(cudaMemcpyAsync(p->h_res, p->d_res, sizeof(FrameResult), cudaMemcpyDeviceToHost, ex.stream));
+            if (p->localizer) CK(cudaMemcpyAsync(p->fit_host, p->fit_dev, sizeof(FitResult), cudaMemcpyDeviceToHost, ex.stream));
         }
         {
             StallTrace t("blocking: stream sync");
             RET(ex.sync());
         }
-        if (!(p->h_res->map_status & ST_NEED_GROW)) return pipeline_absorb(p, *p->h_res, n, id);
+        if (!(p->h_res->map_status & ST_NEED_GROW)) {
+            if (p->localizer) p->last_fit = p->fit_host[0];
+            return pipeline_absorb(p, *p->h_res, n, id);
+        }
         RET(pipeline_after_veto(p, *p->h_res, n));
     }
     return fail(KB_ERR_CUDA, "voxel table could not be grown (internal capacity bug)");
@@ -1713,6 +1811,20 @@ static int queue_init(kb_pipeline *p, size_t max_n, bool any_ts, bool device_inp
     return KB_OK;
 }
 
+static void fit_to_abi(const FitResult &f, kb_fit *out) {
+    double JTr[6];
+    icp_expand(f.acc, out->JTJ, JTr);  // as kb_registration_build_system expands its accumulators
+    out->n_correspondences = f.n_corr;
+    out->n_source = f.n_src;
+    out->sum_sq_residual = f.sse;
+}
+// a localizer's queued frame was absorbed: its fit (pinned copy `slot`) becomes the last one
+static void absorb_fit(kb_pipeline *p, size_t slot, kb_fit *out) {
+    if (!p->localizer) return;
+    p->last_fit = p->fit_host[slot];
+    if (out) fit_to_abi(p->last_fit, out);
+}
+
 static bool is_pinned(const void *ptr) {
     cudaPointerAttributes a;
     if (cudaPointerGetAttributes(&a, ptr) != cudaSuccess) {
@@ -1741,8 +1853,9 @@ static int queue_upload(kb_pipeline *p, void *dst, const void *src, size_t bytes
     return KB_OK;
 }
 
-int kb_pipeline_register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
-                                const size_t *n_timestamps, size_t count, int layout, double *poses_out) {
+// kb_pipeline_register_frames[_fit]; fits_out (localizers only, may be NULL) receives one fit per frame
+static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
+                           const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out) {
     if (!p || (count && (!xyz || !n))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (layout != KB_FRAMES_HOST_F64 && layout != KB_FRAMES_HOST_F32 && layout != KB_FRAMES_DEVICE_F64)
         return fail(KB_ERR_INVALID_ARG, "unknown frame layout %d", layout);
@@ -1791,11 +1904,11 @@ int kb_pipeline_register_frames(kb_pipeline *p, const void *const *xyz, const si
     while (next_absorb < valid) {
         const size_t inflight = next_submit - next_absorb;
         bool submit = next_submit < valid && inflight + 1 < D;
-        if (submit && inflight > 0 && p->map->would_grow(pipeline_extra(p, n[next_submit]))) submit = false;  // drain first
+        if (submit && inflight > 0 && !p->localizer && p->map->would_grow(pipeline_extra(p, n[next_submit]))) submit = false;  // drain first
         if (submit) {
             const size_t k = next_submit, nk = n[k], ntk = use_ts[k] ? n_timestamps[k] : 0;
             auto &s = p->q[k % D];
-            RET(p->map->ensure_capacity(pipeline_extra(p, nk)));  // rebuilds only with nothing in flight
+            if (!p->localizer) RET(p->map->ensure_capacity(pipeline_extra(p, nk)));  // rebuilds only with nothing in flight
             const bool prefetch = k + 1 < valid && !use_ts[k + 1] && n[k + 1] > 0;
             const double *d_xyz, *d_ts = nullptr, *d_next = nullptr;
             if (dev_in) {
@@ -1812,14 +1925,17 @@ int kb_pipeline_register_frames(kb_pipeline *p, const void *const *xyz, const si
             }
             {
                 StallTrace t("queue: launch");
-                RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32, p->q_res_dev + k % D, d_next,
-                                    prefetch ? n[k + 1] : 0));
+                RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32, p->q_res_dev + k % D,
+                                    p->localizer ? p->fit_dev + 1 + k % D : nullptr, d_next, prefetch ? n[k + 1] : 0));
                 CK(cudaEventRecord(s.done, ex.stream));
                 // result read-back on its own stream: neither the next kernel nor the next H2D waits for it (letting
                 // the kernel write to mapped host memory instead was slower)
                 CK(cudaStreamWaitEvent(p->res_stream, s.done, 0));
                 CK(cudaMemcpyAsync(p->q_res + k % D, p->q_res_dev + k % D, sizeof(FrameResult), cudaMemcpyDeviceToHost,
                                    p->res_stream));
+                if (p->localizer)
+                    CK(cudaMemcpyAsync(p->fit_host + 1 + k % D, p->fit_dev + 1 + k % D, sizeof(FitResult), cudaMemcpyDeviceToHost,
+                                       p->res_stream));
                 CK(cudaEventRecord(s.read, p->res_stream));
             }
             ++next_submit;
@@ -1850,6 +1966,7 @@ int kb_pipeline_register_frames(kb_pipeline *p, const void *const *xyz, const si
             return st;
         }
         if (poses_out) std::memcpy(poses_out + 16 * k, r.pose, sizeof(double) * 16);
+        absorb_fit(p, 1 + k % D, fits_out ? fits_out + k : nullptr);
         ++next_absorb;
     }
     return KB_OK;
@@ -1872,6 +1989,7 @@ int kb_pipeline_register_frames(kb_pipeline *p, const void *const *xyz, const si
                 p->next_id = id0 + static_cast<long long>(k) + 1;
                 if (pipeline_absorb(p, r, n[k], id0 + static_cast<long long>(k)) != KB_OK) break;
                 if (poses_out) std::memcpy(poses_out + 16 * k, r.pose, sizeof(double) * 16);
+                absorb_fit(p, 1 + k % D, fits_out ? fits_out + k : nullptr);
             }
         }
         cudaGetLastError();
@@ -1882,6 +2000,21 @@ int kb_pipeline_register_frames(kb_pipeline *p, const void *const *xyz, const si
         tl_err = bad_msg;
         return bad_status;
     }
+    return KB_OK;
+}
+int kb_pipeline_register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
+                                const size_t *n_timestamps, size_t count, int layout, double *poses_out) {
+    return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, nullptr);
+}
+int kb_pipeline_register_frames_fit(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
+                                    const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out) {
+    if (p && fits_out && !p->localizer) return fail(KB_ERR_INVALID_ARG, "fits are computed by localizers only (kb_pipeline_create_localizer)");
+    return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out);
+}
+int kb_pipeline_last_fit(const kb_pipeline *p, kb_fit *out) {
+    if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (!p->localizer) return fail(KB_ERR_INVALID_ARG, "fits are computed by localizers only (kb_pipeline_create_localizer)");
+    fit_to_abi(p->last_fit, out);
     return KB_OK;
 }
 

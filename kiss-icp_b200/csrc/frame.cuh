@@ -1,0 +1,361 @@
+// KissICP::RegisterFrame as one persistent kernel (k_register_frame) and what it works on. A header of its own:
+// the odometry instantiation is compiled with the other kernels (api.cu), the localizer's in a translation unit of its
+// own (localize.cu), so that neither changes the code generated for the other.
+#pragma once
+
+#include <type_traits>
+
+#include "device_ops.cuh"
+#include "icp_team.cuh"
+
+namespace kb {
+
+// state of one kiss_icp::pipeline::KissICP instance, resident in HBM (KissICP.hpp:87-95)
+struct PipeState {
+    SE3 last_pose;
+    SE3 last_delta;
+    double model_sse;  // AdaptiveThreshold::model_sse_   Threshold.hpp:45
+    int num_samples;   // AdaptiveThreshold::num_samples_ Threshold.hpp:46
+    int vetoed;        // set by a frame that found the voxel table too small: frames already queued behind it
+                       // must not run on the stale state, they return ST_SKIPPED until the host has grown the table
+    long long front_id;  // id of the frame whose preprocessed / downsampled clouds are in Workspace::fr[id & 1]
+                         // (written by the launch that prefetched them), -1: none
+};
+
+// what the host reads back after every RegisterFrame (one small D2H)
+struct FrameResult {
+    double pose[16];   // row-major new pose
+    double delta[16];  // row-major last_delta
+    double sigma;      // adaptive threshold used for this frame
+    double model_sse;
+    int num_samples;
+    int iterations;
+    int n_pre, n_ds, n_src;
+    int map_live, map_tomb, map_points, map_status;
+    int team;          // CTAs of the ICP team (0: the whole-grid loop ran)
+    double icp_candidates;  // map points examined by all ICP iterations of this frame
+    double icp_queries;     // GetClosestNeighbor calls (iterations x source points)
+    double cache_stats[3];  // NN-cache hits / fills / overflows over all iterations
+    unsigned long long t_ns[20];  // %globaltimer at phase boundaries (CTA 0): start, pre, ds1, ds2, icp, map, end
+};
+
+// output of the front end of one frame (Preprocess + Voxelize, KissICP.cpp:38,41): two sets, so that the next
+// frame's front end can be computed while this frame is still being registered
+struct Front {
+    double *pre;  // [n][3] preprocessed frame
+    double *ds1;  // [n][3] frame_downsample (0.5 v)
+    double *src;  // [n][3] source (1.5 v)
+    int *cnt;     // [4] n_pre, n_ds, n_src
+};
+
+struct Workspace {
+    double *tmp;    // [n][3] deskewed points
+    Front fr[2];    // by frame id parity
+    double *work;   // [n][3] source in the map frame (ICP iterate of the whole-grid loop)
+    double *tp;     // [n][3] points being inserted, map frame
+    int *next;      // [n] pending-list links
+    int *touched;   // [n] voxels touched by the current AddPoints
+    DsScratch ds;    // [pow2 >= 2n] downsample scratch tables (0.5 v pass)
+    DsScratch ds2;   // second set for the 1.5 v pass (both are cleared during preprocessing)
+};
+
+struct FrameParams {
+    MapView m;
+    Scratch sc;
+    TeamScratch team;
+    Workspace ws;
+    PipeState *st;
+    FrameResult *res;
+    const double *in;
+    const double *ts;
+    int n, n_ts;
+    int in_f32;  // the frame is float[n][3] instead of double[n][3]
+    long long id;  // frame id (monotonic per pipeline; a frame replayed after a capacity veto keeps its id)
+    // the frame after this one, when the caller already has it on the device (kb_pipeline_register_frames) and its
+    // front end does not depend on this frame's result (no timestamps to deskew with): its preprocessing and
+    // downsampling run on the CTAs the ICP team leaves idle. next_in == nullptr: none.
+    const double *next_in;
+    int next_n, next_in_f32;
+    int deskew;
+    double max_range, min_range, voxel_size;
+    int max_iter;
+    double conv, min_motion_th;
+    int use_qcache;
+    int icp_team_q;  // source points per CTA of the ICP team; 0: whole-grid loop (op_icp)
+    unsigned tag_base;
+};
+
+__device__ __forceinline__ void threshold_update(const SE3 &dev, double min_motion_th, double max_range,
+                                                 double *sse, int *ns) {
+    // AdaptiveThreshold::UpdateModelDeviation  core/Threshold.cpp:38-49
+    const double theta = angle_axis_angle(q_to_matrix(dev.q));
+    const double delta_rot = 2.0 * max_range * sin(theta / 2.0);
+    const double delta_trans = norm(dev.t);
+    const double model_error = delta_trans + delta_rot;
+    if (model_error > min_motion_th) {
+        *sse += model_error * model_error;
+        *ns += 1;
+    }
+}
+
+#define KB_STAMP(i) \
+    if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.res->t_ns[i] = globaltimer_ns()
+
+extern __shared__ __align__(16) unsigned char kb_dyn_smem[];  // QCache[NWARPS][QC_SLOTS] (op_icp) or the TeamSmem layout (op_icp_team)
+
+// Preprocess + Voxelize of one frame on the CTAs of `g` (the whole launch, or the front-end team), KissICP.cpp:38,41,70-75.
+// Three barriers of `g` inside; the caller provides the one behind it. No timestamps => `motion` is not used.
+__device__ __noinline__ void op_front(Grid &g, const Scratch &sc, Shared &sh, const Workspace &ws, const Front &fr,
+                                      const double *in, int n, const double *ts, int n_ts, bool deskew, const SE3 &motion,
+                                      double max_range, double min_range, double voxel_size, bool in_f32,
+                                      unsigned long long *t_ns /* stamps of the profiled launch or nullptr */) {
+    // the downsample scratch tables of both passes are cleared here, under the preprocess barriers
+    ds_clear(g, ws.ds, n);
+    ds_clear(g, ws.ds2, n);
+    op_preprocess(g, sc, sh, in, n, ts, n_ts, deskew, motion, max_range, min_range, ws.tmp, fr.pre, &fr.cnt[0], in_f32);
+    g.sync();
+    if (t_ns && g.rank == 0 && threadIdx.x == 0) t_ns[1] = globaltimer_ns();
+    const int n_pre = __ldcg(&fr.cnt[0]);
+    op_downsample(g, sc, sh, fr.pre, n_pre, voxel_size * 0.5, ws.ds, fr.ds1, &fr.cnt[1], t_ns ? &t_ns[12] : nullptr, true);
+    g.sync();
+    if (t_ns && g.rank == 0 && threadIdx.x == 0) t_ns[2] = globaltimer_ns();
+    const int n_ds = __ldcg(&fr.cnt[1]);
+    op_downsample(g, sc, sh, fr.ds1, n_ds, voxel_size * 1.5, ws.ds2, fr.src, &fr.cnt[2], t_ns ? &t_ns[16] : nullptr, true);
+}
+
+// ---- the fit of a localized frame (k_register_frame<LocalizeParams>, kb_pipeline_last_fit) --------------------------
+// DataAssociation + BuildLinearSystem (Registration.cpp:60-121) of the source mapped by the final pose, formed the way
+// kb_registration_build_system forms them (nn_search_warp, icp_term, expanded by icp_expand on the host), plus the
+// unweighted sum of |r|^2. Deterministic for a grid size: point qi -> CTA qi % G, warp (qi / G) % NWARPS, a lane sums
+// its warp's points in order, the warps of a CTA are added in warp order and the CTA partials in CTA order.
+constexpr int FIT_VALS = NACC + 2;  // accumulators, correspondences, sum of squared residuals
+struct FitResult {
+    double acc[NACC];  // Geman-McClure-weighted accumulators of J^T W J and J^T W r (icp_term's layout)
+    double sse;        // sum of |r|^2 over the correspondences
+    int n_corr, n_src;
+};
+struct FitOut {
+    double *part;    // [FIT_VALS][grid] per-CTA partials (value-major)
+    FitResult *res;  // this frame's fit
+};
+struct LocalizeParams : FrameParams {
+    FitOut fit;
+};
+
+// this CTA's partials of the fit: part[v][cta]. The caller provides the grid barrier behind it.
+__device__ __noinline__ void op_fit(Shared &sh, const MapView &m, const double *src, int n, const SE3 &pose,
+                                    double max_dist, double kscale, double *part) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int G = static_cast<int>(gridDim.x);
+    double acc = 0.0, sse = 0.0;  // lane l < 16 owns accumulator l; r is warp-uniform, so is sse
+    int corr = 0;
+    for (int qi = static_cast<int>(blockIdx.x) + G * warp; qi < n; qi += G * NWARPS) {
+        const V3 p = se3_act(pose, V3{src[3 * qi], src[3 * qi + 1], src[3 * qi + 2]});
+        const NNResult r = nn_search_warp(m, p, lane, sh.wnn[warp]);
+        if (r.d < max_dist) {
+            acc += icp_term(lane, p, r.p, kscale);
+            sse += sqnorm(p - r.p);
+            ++corr;
+        }
+    }
+    if (lane < NACC) sh.warp_d[warp][lane] = acc;
+    if (lane == NACC) sh.warp_d[warp][NACC] = static_cast<double>(corr);
+    if (lane == NACC + 1) sh.warp_d[warp][NACC + 1] = sse;
+    __syncthreads();
+    if (threadIdx.x < FIT_VALS) {
+        double v = 0.0;
+        for (int w = 0; w < NWARPS; ++w) v += sh.warp_d[w][threadIdx.x];
+        part[threadIdx.x * G + static_cast<int>(blockIdx.x)] = v;
+    }
+}
+
+// after the barrier behind op_fit: one CTA adds the partials in CTA order
+__device__ __forceinline__ void fit_finish(const FitOut &fit, int n_src) {
+    const int G = static_cast<int>(gridDim.x);
+    if (threadIdx.x < FIT_VALS) {
+        double v = 0.0;
+        for (int c = 0; c < G; ++c) v += __ldcg(&fit.part[threadIdx.x * G + c]);
+        if (threadIdx.x < NACC)
+            fit.res->acc[threadIdx.x] = v;
+        else if (threadIdx.x == NACC)
+            fit.res->n_corr = static_cast<int>(v);
+        else
+            fit.res->sse = v;
+        if (threadIdx.x == 0) fit.res->n_src = n_src;
+    }
+}
+
+// ---- KissICP::RegisterFrame (pipeline/KissICP.cpp:35-68) as ONE persistent kernel ----------
+//   [front end of this frame, unless a previous launch prefetched it]
+//   capacity check | fill pass (all CTAs) | ICP iterations on the team  ||  front end of the NEXT frame on the rest
+//   map update (all CTAs) | epilogue
+// k_register_frame<LocalizeParams> (a localizer): the same statement against a read-only prior map, without local_map_.Update
+// (KissICP.cpp:61). Nothing is inserted, so there is no capacity check and no veto, and the map-update phase is the
+// fit pass (op_fit) at the final pose. Nothing writes to the map.
+template <class Params>
+__global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
+    constexpr bool LOCALIZE = std::is_same<Params, LocalizeParams>::value;
+    __shared__ Shared sh;
+    Grid g;
+    g.init(P.sc.bar);
+    KB_STAMP(0);
+    const SE3 last_pose = P.st->last_pose;
+    const SE3 last_delta = P.st->last_delta;
+    const double model_sse = P.st->model_sse;
+    const int num_samples = P.st->num_samples;
+    const long long front_id = P.st->front_id;
+    if (!LOCALIZE && P.st->vetoed) {  // written only by an EARLIER launch: uniform across the grid
+        if (blockIdx.x == 0 && threadIdx.x == 0) P.res->map_status = ST_SKIPPED;
+        g.finish();
+        return;
+    }
+    const Front fr = P.ws.fr[P.id & 1];
+    kb_mark(0x100u + (static_cast<unsigned>(P.id) & 0xffu) * 0x10000u);
+    if (front_id != P.id) {  // uniform: written only by an earlier launch
+        op_front(g, P.sc, sh, P.ws, fr, P.in, P.n, P.ts, P.n_ts, P.deskew != 0, last_delta, P.max_range, P.min_range,
+                 P.voxel_size, P.in_f32 != 0, P.sc.profile ? P.res->t_ns : nullptr);
+        g.sync();
+    } else if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) {
+        P.res->t_ns[1] = P.res->t_ns[2] = globaltimer_ns();  // front end prefetched by the previous launch
+    }
+    KB_STAMP(3);
+    const int n_pre = __ldcg(&fr.cnt[0]), n_ds = __ldcg(&fr.cnt[1]), n_src = __ldcg(&fr.cnt[2]);
+    // optimistic table capacity: the host sized the voxel table for the EXPECTED number of new voxels. If this
+    // frame could push the load factor beyond 0.5, nothing has been modified yet: report and let the host grow
+    // the table and replay the frame (rare; first frames of a sequence). The frame's front end stays valid.
+    if (!LOCALIZE) {
+        const long long need = static_cast<long long>(__ldcg(&P.m.counters[C_LIVE])) + __ldcg(&P.m.counters[C_TOMB]) + n_ds;
+        if (need * 2 > static_cast<long long>(P.m.mask) + 1) {
+            if (blockIdx.x == 0 && threadIdx.x == 0) {
+                P.res->map_status = ST_NEED_GROW;
+                P.res->n_ds = n_ds;
+                P.st->vetoed = 1;     // every CTA read it before the first grid barrier
+                P.st->front_id = P.id;  // fr[id & 1] holds this frame's front end: the replay skips it
+            }
+            g.finish();
+            return;  // uniform across the grid
+        }
+    }
+    kb_mark(0x200u);
+    // sigma, initial guess (KissICP.cpp:44,47)
+    const double sigma = sqrt(model_sse / num_samples);
+    const SE3 guess = se3_mul(last_pose, last_delta);
+    // ICP (KissICP.cpp:50-54)
+    const int G = static_cast<int>(gridDim.x);
+    const int live = __ldcg(&P.m.counters[C_LIVE]);
+    const bool icp_runs = live != 0 && P.max_iter > 0;  // voxel_map.Empty() -> initial_guess
+    const int T = icp_team_plan(P.m, live, P.max_iter, P.icp_team_q, n_src, G, P.team.smem_bytes);
+    if (T > 0) {
+        if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[30] = globaltimer_ns();
+        icp_fill_pass(g, sh, P.m, fr.src, n_src, guess, P.team.qrec, P.team.radius_frac, P.sc.bar + BAR_TICKET);
+        if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[31] = globaltimer_ns();
+        kb_mark(0x300u);
+        g.sync();
+        kb_mark(0x400u + static_cast<unsigned>(T));
+        if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[32] = P.res->t_ns[7] = globaltimer_ns();
+        if (static_cast<int>(blockIdx.x) < T) {
+            op_icp_team(P.team, P.sc, sh, P.m, n_src, guess, 3.0 * sigma, sigma, P.max_iter, P.conv,
+                        kb_dyn_smem, T, P.tag_base);
+            if (blockIdx.x == 0 && threadIdx.x == 0) {
+                team_publish(P.team, sh);
+                if (P.sc.profile) P.res->t_ns[10] = globaltimer_ns();  // iterations done (team member 0)
+            }
+        } else if (P.next_in != nullptr && 2 * (G - T) >= G) {
+            // the CTAs the team does not need register nothing now: they run the next frame's front end
+            Grid gf;
+            gf.init_team(P.sc.bar + BAR_TEAM, T, G - T);
+            const Front nf = P.ws.fr[(P.id + 1) & 1];
+            op_front(gf, P.sc, sh, P.ws, nf, P.next_in, P.next_n, nullptr, 0, false, last_delta, P.max_range, P.min_range,
+                     P.voxel_size, P.next_in_f32 != 0, nullptr);
+            if (gf.rank == 0 && threadIdx.x == 0) {
+                P.st->front_id = P.id + 1;  // visible to the next launch
+                if (P.sc.profile) P.res->t_ns[11] = globaltimer_ns();  // (rank 0's own end: the other CTAs may still be emitting)
+            }
+        }
+        kb_mark(0x500u);
+        g.sync();
+        kb_mark(0x600u);
+        if (threadIdx.x == 0) team_collect(P.team, sh);
+        __syncthreads();
+    } else {
+        op_icp(g, P.sc, sh, P.m, fr.src, P.ws.work, n_src, guess, 3.0 * sigma, sigma, P.max_iter, P.conv,
+               P.use_qcache ? reinterpret_cast<QCache *>(kb_dyn_smem) : nullptr, P.tag_base);
+        // Without ICP (empty map, max_iter <= 0) op_icp has no grid-wide rendezvous, and with a prefetched front end
+        // (the replay of a vetoed first frame) neither has anything above. Every CTA must have read the state the
+        // decisions above depend on (vetoed, the map counters) before any CTA starts the map update, which changes it.
+        if (!icp_runs) g.sync();
+    }
+    const SE3 new_pose = sh.result;
+    const int iters = sh.iters;
+    const double icp_cand = sh.cand_total, icp_q = sh.query_total;
+    const double cs0 = sh.cache_stats[0], cs1 = sh.cache_stats[1], cs2 = sh.cache_stats[2];
+    KB_STAMP(4);
+    // Bookkeeping (KissICP.cpp:57-63: model deviation, threshold, delta, pose) is a long chain of single-thread FP64
+    // math; it only needs new_pose, so one thread of the LAST CTA does it now, hidden behind the map update's
+    // first phase (that thread owns no insert work), instead of serially after the map update.
+    // The pipeline state itself is stored after the last barrier: with a prefetched front end and no ICP (empty
+    // map) there may be no barrier between the slowest CTA's read of the state and this point.
+    const bool book = (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0);
+    double sse = model_sse;
+    int ns = num_samples;
+    SE3 delta = last_delta;
+    if (book) {
+        const SE3 dev = se3_mul(se3_inverse(guess), new_pose);
+        threshold_update(dev, P.min_motion_th, P.max_range, &sse, &ns);
+        delta = se3_mul(se3_inverse(last_pose), new_pose);
+        FrameResult *r = P.res;
+        se3_to_matrix(new_pose, r->pose);
+        se3_to_matrix(delta, r->delta);
+        r->sigma = sigma;
+        r->model_sse = sse;
+        r->num_samples = ns;
+        r->iterations = iters;
+        r->icp_queries = icp_q;
+        r->n_pre = n_pre;
+        r->n_ds = n_ds;
+        r->n_src = n_src;
+        r->team = T;
+        r->icp_candidates = icp_cand;
+        r->cache_stats[0] = cs0;
+        r->cache_stats[1] = cs1;
+        r->cache_stats[2] = cs2;
+    }
+    if constexpr (LOCALIZE) {
+        // the fit at the final pose, with this frame's (3 sigma, sigma)
+        op_fit(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part);
+        kb_mark(0x700u);
+    } else {
+        // local_map_.Update(frame_downsample, new_pose) (KissICP.cpp:61)
+        op_map_add(g, sh, P.m, fr.ds1, n_ds, true, new_pose, P.ws.tp, P.ws.next, P.ws.touched, P.sc.profile ? &P.res->t_ns[8] : nullptr);
+        kb_mark(0x700u);
+        op_map_remove_far(P.m, new_pose.t);
+    }
+    kb_mark(0x800u);
+    g.sync();
+    kb_mark(0x900u);
+    KB_STAMP(5);
+    if constexpr (LOCALIZE) {
+        if (blockIdx.x == gridDim.x - 1) fit_finish(P.fit, n_src);
+    }
+    if (book) {
+        P.st->model_sse = sse;
+        P.st->num_samples = ns;
+        P.st->last_delta = delta;
+        P.st->last_pose = new_pose;
+        FrameResult *r = P.res;
+        r->map_live = P.m.counters[C_LIVE];
+        r->map_tomb = P.m.counters[C_TOMB];
+        r->map_points = P.m.counters[C_POINTS];
+        r->map_status = P.m.counters[C_STATUS];
+        if (P.sc.profile) r->t_ns[6] = globaltimer_ns();
+    }
+    g.finish();
+}
+
+}  // namespace kb
+
+// defined in localize.cu, the localizer's device module: its k_register_frame<LocalizeParams> (takes a LocalizeParams)
+// and its copies of the watchdog words
+const void *localize_kernel();
+cudaError_t localize_watchdog_init(unsigned *d_host_words, const unsigned init[8]);
+cudaError_t localize_watchdog_rearm();

@@ -6,11 +6,18 @@ Two execution modes:
     (cpp/kiss_icp/pipeline/KissICP.cpp:35-68) with all state resident in HBM.
   * modular (``fused=False`` or a fixed threshold, which only the Python reference has): the
     reference's own module-by-module sequence (kiss_icp.py:43-75) through the per-module C-ABI.
+
+``KissICP(config, prior_map=vmap)`` is a localizer: the same statement against the prior map ``vmap`` without
+``local_map.update``. The map is never written, ``last_fit`` reports how well each scan fits it, and while the
+localizer exists the map's mutators raise MapInUseError. Build a prior map with existing calls, for example a
+VoxelHashMap with a large max_distance and ``vmap.update(frame_downsample, pose)`` per scan of an odometry run, or
+``vmap.load(...)`` from a state_dict (INTEGRATION.md section 4).
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
+from collections import namedtuple
 
 import numpy as np
 
@@ -23,6 +30,21 @@ from .threshold import AdaptiveThreshold, get_threshold_estimator
 from .voxelization import voxel_down_sample
 
 STATE_FORMAT_VERSION = 1  # of KissICP.state_dict()
+MAP_KEYS = ("voxels", "counts", "points")  # the map's part of an odometry state_dict()
+
+# the fit of a localized scan at its final pose (kb_fit): correspondences closer than 3 sigma, source points,
+# sqrt(sum |r|^2 / n_correspondences) (NaN without correspondences), and the 6x6 information matrix J^T W J
+Fit = namedtuple("Fit", ["n_correspondences", "n_source", "rmse", "information"])
+
+
+def _fit_of(n_corr, n_src, sse, JTJ):
+    """a Fit from the raw values; array arguments give a Fit of arrays"""
+    n = np.asarray(n_corr)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        rmse = np.where(n > 0, np.sqrt(np.asarray(sse, dtype=np.float64) / np.maximum(n, 1)), np.nan)
+    if n.ndim == 0:
+        return Fit(int(n), int(n_src), float(rmse), np.asarray(JTJ, dtype=np.float64).reshape(6, 6))
+    return Fit(n.astype(np.int64), np.asarray(n_src, dtype=np.int64), rmse, np.asarray(JTJ, dtype=np.float64).reshape(-1, 6, 6))
 
 
 def se3_params_from_matrix(T) -> np.ndarray:
@@ -80,12 +102,17 @@ class _PipelineThreshold:
 
 
 class KissICP:
-    def __init__(self, config: KISSConfig | None = None, fused: bool = True):
+    def __init__(self, config: KISSConfig | None = None, fused: bool = True, prior_map: VoxelHashMap | None = None):
+        if prior_map is not None and not isinstance(prior_map, VoxelHashMap):
+            raise TypeError(f"prior_map must be a VoxelHashMap, not {type(prior_map).__name__}")
         self.config = config if config is not None else load_config()
         if self.config.mapping.voxel_size is None:
             self.config.mapping.voxel_size = float(self.config.data.max_range / 100.0)
         self.fused = bool(fused) and self.config.adaptive_threshold.fixed_threshold is None
+        self.localizer = prior_map is not None
         self._h = None
+        if self.localizer:
+            self._check_prior(prior_map)
         if self.fused:
             c = N.Config()
             c.voxel_size = self.config.mapping.voxel_size
@@ -99,9 +126,14 @@ class KissICP:
             c.max_num_threads = self.config.registration.max_num_threads
             c.deskew = int(self.config.data.deskew)
             self._h = N.vp()
-            N.check(N.lib().kb_pipeline_create(C.byref(c), C.byref(self._h)))
-            self.local_map = VoxelHashMap(c.voxel_size, c.max_range, c.max_points_per_voxel,
-                                          _borrowed=N.lib().kb_pipeline_voxel_map(self._h), _owner=self)
+            if self.localizer:
+                # (self.local_map holds the prior: it cannot be collected while the localizer reads it)
+                check_value(N.lib().kb_pipeline_create_localizer(C.byref(c), prior_map._h, C.byref(self._h)))
+                self.local_map = prior_map
+            else:
+                N.check(N.lib().kb_pipeline_create(C.byref(c), C.byref(self._h)))
+                self.local_map = VoxelHashMap(c.voxel_size, c.max_range, c.max_points_per_voxel,
+                                              _borrowed=N.lib().kb_pipeline_voxel_map(self._h), _owner=self)
             self.adaptive_threshold = _PipelineThreshold(self)
         else:
             self._last_pose = np.eye(4)
@@ -109,7 +141,16 @@ class KissICP:
             self.adaptive_threshold = get_threshold_estimator(self.config)
             self.preprocessor = get_preprocessor(self.config)
             self.registration = get_registration(self.config)
-            self.local_map = get_voxel_hash_map(self.config)
+            self.local_map = prior_map if self.localizer else get_voxel_hash_map(self.config)
+            self._last_fit = _fit_of(0, 0, 0.0, np.zeros(36))
+
+    def _check_prior(self, prior_map):
+        vs, mp = N.dbl(0), N.u32(0)
+        N.check(N.lib().kb_map_params(prior_map._h, C.byref(vs), None, C.byref(mp)))
+        c = self.config.mapping
+        if vs.value != float(c.voxel_size) or mp.value != int(c.max_points_per_voxel):
+            raise ValueError(f"prior map with voxel_size {vs.value}, max_points_per_voxel {mp.value}; the config has "
+                             f"{c.voxel_size}, {c.max_points_per_voxel}")
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -147,6 +188,17 @@ class KissICP:
             self._last_delta = np.array(T, dtype=np.float64)
         else:
             N.check(N.lib().kb_pipeline_set_delta(self._h, N.ptr(N.mat4_arg(T))))
+
+    @property
+    def last_fit(self) -> Fit:
+        """the fit of the last scan of a localizer at its final pose (zeros before the first scan)"""
+        if not self.localizer:
+            raise ValueError("fits are computed by localizers only: KissICP(config, prior_map=...)")
+        if not self.fused:
+            return self._last_fit
+        f = N.Fit()
+        N.check(N.lib().kb_pipeline_last_fit(self._h, C.byref(f)))
+        return _fit_of(f.n_correspondences, f.n_source, f.sum_sq_residual, np.array(f.JTJ[:]))
 
     def _sigma_next(self):
         s = N.dbl(0)
@@ -222,31 +274,41 @@ class KissICP:
         N.check(N.lib().kb_pipeline_last_clouds(self._h, N.ptr(pre), a.value, N.ptr(src), b.value))
         return pre, src
 
-    def register_frames(self, frames, timestamps=None):
+    def register_frames(self, frames, timestamps=None, return_fits: bool = False):
         """Register a whole sequence (the dataset loop of python/kiss_icp/pipeline.py:106-112) -> poses (K,4,4).
 
         Same results as K ``register_frame`` calls; the frames are queued on the device (copy of frame k+1
         overlaps the registration of frame k, results are read behind the queue). ``frames`` is a sequence of
-        (N_k,3) arrays, all float64 or all float32; ``timestamps`` a matching sequence (or None)."""
+        (N_k,3) arrays, all float64 or all float32; ``timestamps`` a matching sequence (or None).
+        ``return_fits`` (localizers only) -> (poses, fits): a Fit of arrays, one entry per frame."""
         K = len(frames)
+        if return_fits and not self.localizer:
+            raise ValueError("fits are computed by localizers only: KissICP(config, prior_map=...)")
         if timestamps is None:
             timestamps = [np.empty(0)] * K
         if len(timestamps) != K:
             raise ValueError("frames and timestamps differ in length")
         if not self.fused:
             poses = np.empty((K, 4, 4))
+            fits = []
             for k in range(K):
                 self._register_frame_modular(frames[k], timestamps[k])
                 poses[k] = self._last_pose
-            return poses
+                if return_fits:
+                    fits.append(self._last_fit)
+            if not return_fits:
+                return poses
+            return poses, _fit_of([f.n_correspondences for f in fits], [f.n_source for f in fits],
+                                  [f.rmse ** 2 * f.n_correspondences if f.n_correspondences else 0.0 for f in fits],
+                                  np.array([f.information for f in fits]).reshape(-1, 36))
         arrs = [np.asarray(f) for f in frames]
         f32 = K > 0 and all(a.dtype == np.float32 and a.ndim == 2 and a.shape[1] == 3 for a in arrs)
         pts = [np.ascontiguousarray(a) for a in arrs] if f32 else [N.points_arg(a) for a in arrs]
         ts = [np.ascontiguousarray(np.asarray(t).ravel(), dtype=np.float64) for t in timestamps]
         return self._register_frames_raw([N.ptr(a) for a in pts], [len(a) for a in pts], [N.ptr(t) for t in ts],
-                                         [len(t) for t in ts], 1 if f32 else 0)
+                                         [len(t) for t in ts], 1 if f32 else 0, return_fits=return_fits)
 
-    def _register_frames_raw(self, xyz_ptrs, sizes, ts_ptrs, ts_sizes, layout):
+    def _register_frames_raw(self, xyz_ptrs, sizes, ts_ptrs, ts_sizes, layout, return_fits: bool = False):
         """raw-pointer form (host or device addresses): layout 0 host f64, 1 host f32, 2 device f64"""
         K = len(xyz_ptrs)
         as_vp = lambda v: v if isinstance(v, C.c_void_p) else C.c_void_p(int(v) if v else None)
@@ -255,8 +317,13 @@ class KissICP:
         n = (N.sz * K)(*sizes)
         nt = (N.sz * K)(*ts_sizes)
         poses = np.empty((K, 4, 4))
-        N.check(N.lib().kb_pipeline_register_frames(self._h, X, n, T, nt, K, int(layout), N.ptr(poses)))
-        return poses
+        if not return_fits:
+            N.check(N.lib().kb_pipeline_register_frames(self._h, X, n, T, nt, K, int(layout), N.ptr(poses)))
+            return poses
+        fits = (N.Fit * K)()
+        N.check(N.lib().kb_pipeline_register_frames_fit(self._h, X, n, T, nt, K, int(layout), N.ptr(poses), fits))
+        return poses, _fit_of([f.n_correspondences for f in fits], [f.n_source for f in fits],
+                              [f.sum_sq_residual for f in fits], np.array([f.JTJ[:] for f in fits]).reshape(-1, 36))
 
     def _register_frame_modular(self, frame, timestamps):
         # python/kiss_icp/kiss_icp.py:43-75, line for line, on the per-module device API
@@ -273,17 +340,28 @@ class KissICP:
         )
         model_deviation = np.linalg.inv(initial_guess) @ new_pose
         self.adaptive_threshold.update_model_deviation(model_deviation)
-        self.local_map.update(frame_downsample, new_pose)
+        if self.localizer:  # no local_map.update: the fit at the final pose instead
+            self._last_fit = self._fit_modular(source, new_pose, sigma)
+        else:
+            self.local_map.update(frame_downsample, new_pose)
         self._last_delta = np.linalg.inv(self._last_pose) @ new_pose
         self._last_pose = new_pose
         return frame, source
+
+    def _fit_modular(self, source, pose, sigma):
+        mapped = source @ pose[:3, :3].T + pose[:3, 3]
+        JTJ, _, n = self.registration.build_system(mapped, self.local_map, 3 * sigma, sigma)
+        _, d = self.local_map.closest_neighbors(mapped)
+        near = d < 3 * sigma
+        return _fit_of(n, len(source), float(np.sum(d[near] ** 2)), JTJ)
 
     # -- checkpoint / restore -----------------------------------------------------------------------
     def state_dict(self):
         """The sequence's whole state as a dict of numpy arrays (it survives np.savez / np.load):
         format_version; the config fields; pose_qt, delta_qt (Sophus::SE3d::params() order {qx,qy,qz,qw,tx,ty,tz})
         and pose, delta (4x4); the adaptive threshold's model_sse, num_samples (NaN and 0 under a fixed threshold);
-        the map as voxels, counts, points (VoxelHashMap.dump()).
+        the map as voxels, counts, points (VoxelHashMap.dump()). A localizer's state has no map: its prior map is not
+        part of it.
 
         The fused pipeline's pose and delta are the device's quaternions and translations, bit for bit. In modular
         mode the 4x4 matrices are the state and pose_qt / delta_qt are derived from them."""
@@ -309,14 +387,16 @@ class KissICP:
             sse, ns = (np.nan, 0)  # a fixed threshold has no state
             if isinstance(self.adaptive_threshold, AdaptiveThreshold):
                 sse, ns = self.adaptive_threshold.get_state()
-        vox, cnt, pts = self.local_map.dump()
         d.update(pose_qt=pose_qt, delta_qt=delta_qt, pose=pose, delta=delta, model_sse=np.array(float(sse)),
-                 num_samples=np.array(int(ns)), voxels=vox, counts=cnt, points=pts)
+                 num_samples=np.array(int(ns)))
+        if not self.localizer:  # (a localizer's prior map is not part of its state)
+            vox, cnt, pts = self.local_map.dump()
+            d.update(voxels=vox, counts=cnt, points=pts)
         return d
 
     def load_state_dict(self, state):
         """Restore a state_dict() taken in either mode (or an equivalent dict of the oracle's state), all or nothing: on ValueError
-        nothing has changed.
+        nothing has changed. A localizer rejects a dict that carries a map; an odometry pipeline one that does not.
 
         voxel_size and max_points_per_voxel must equal this pipeline's (ValueError otherwise): the map's voxels
         and its per-voxel cap depend on them. Every other config field of the dict is ignored; the receiving
@@ -326,6 +406,12 @@ class KissICP:
         d = {k: np.asarray(v) for k, v in state.items()}
         if int(d["format_version"]) != STATE_FORMAT_VERSION:
             raise ValueError(f"state format {int(d['format_version'])}, expected {STATE_FORMAT_VERSION}")
+        has_map = [k in d for k in MAP_KEYS]
+        if self.localizer and any(has_map):
+            raise ValueError("the prior map is not part of a localizer's state: the state carries a map")
+        if not self.localizer and not all(has_map):
+            raise ValueError("the state carries no map (voxels, counts, points): a localizer's state cannot restore "
+                             "an odometry pipeline")
         c = self.config
         if float(d["voxel_size"]) != float(c.mapping.voxel_size) or \
                 int(d["max_points_per_voxel"]) != int(c.mapping.max_points_per_voxel):
@@ -333,7 +419,7 @@ class KissICP:
                              f"{int(d['max_points_per_voxel'])}; this pipeline has {c.mapping.voxel_size}, "
                              f"{c.mapping.max_points_per_voxel}")
         sse, ns = float(d["model_sse"]), int(d["num_samples"])
-        load_map = lambda: self.local_map.load(d["voxels"], d["counts"], d["points"])
+        load_map = (lambda: None) if self.localizer else (lambda: self.local_map.load(d["voxels"], d["counts"], d["points"]))
         if self.fused:
             new, old = N.PipelineState(), N.PipelineState()
             new.pose[:] = [float(x) for x in _params_arg(d["pose_qt"])]

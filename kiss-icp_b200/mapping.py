@@ -10,6 +10,11 @@ from . import _native as N
 from .config import KISSConfig
 
 
+class MapInUseError(N.KissB200Error):
+    """A call that would change or free a VoxelHashMap while localizers read it (KissICP(config, prior_map=...)).
+    A RuntimeError; the map is unchanged. It works again once the last localizer using it is gone."""
+
+
 def check_value(status: int):
     """N.check, except that a rejected argument (KB_ERR_INVALID_ARG) raises ValueError: the checkpoint loads report
     bad input the way numpy and the reference's Python do"""
@@ -37,6 +42,9 @@ def get_voxel_hash_map(config: KISSConfig):
 
 
 class VoxelHashMap:
+    """The mutators (clear, update, add_points, remove_far_away_points, compact, load) raise MapInUseError while a
+    localizer uses the map as its prior map."""
+
     def __init__(self, voxel_size: float, max_distance: float, max_points_per_voxel: int, _borrowed=None, _owner=None):
         self._owner = _owner
         self._borrowed = _borrowed is not None
@@ -52,9 +60,20 @@ class VoxelHashMap:
             N._lib.kb_map_destroy(h)
             self._h = None
 
+    def readers(self) -> int:
+        """localizers using this map as their prior map (while > 0 the map cannot be changed)"""
+        r = N.i32(0)
+        N.check(N.lib().kb_map_readers(self._h, C.byref(r)))
+        return r.value
+
+    def _mutated(self, status: int, check=N.check):
+        if status == N.KB_ERR_INVALID_ARG and self.readers() > 0:
+            raise MapInUseError(N.lib().kb_last_error().decode())
+        check(status)
+
     # -- reference surface ---------------------------------------------------------------------
     def clear(self):
-        N.check(N.lib().kb_map_clear(self._h))
+        self._mutated(N.lib().kb_map_clear(self._h))
 
     def empty(self):
         e = N.i32(0)
@@ -67,19 +86,19 @@ class VoxelHashMap:
         pts = N.points_arg(points)
         x = np.ascontiguousarray(pose, dtype=np.float64)
         if x.shape == (4, 4):
-            N.check(N.lib().kb_map_update_pose(self._h, N.ptr(pts), len(pts), N.ptr(x)))
+            self._mutated(N.lib().kb_map_update_pose(self._h, N.ptr(pts), len(pts), N.ptr(x)))
         elif x.shape == (3,):
-            N.check(N.lib().kb_map_update_origin(self._h, N.ptr(pts), len(pts), N.ptr(x)))
+            self._mutated(N.lib().kb_map_update_origin(self._h, N.ptr(pts), len(pts), N.ptr(x)))
         else:
             raise TypeError("_update(): incompatible function arguments (pose (4,4) or origin (3,))")
 
     def add_points(self, points):
         pts = N.points_arg(points)
-        N.check(N.lib().kb_map_add_points(self._h, N.ptr(pts), len(pts)))
+        self._mutated(N.lib().kb_map_add_points(self._h, N.ptr(pts), len(pts)))
 
     def remove_far_away_points(self, origin):
         o = np.ascontiguousarray(origin, dtype=np.float64).reshape(3)
-        N.check(N.lib().kb_map_remove_far(self._h, N.ptr(o)))
+        self._mutated(N.lib().kb_map_remove_far(self._h, N.ptr(o)))
 
     def point_cloud(self) -> np.ndarray:
         n = N.sz(0)
@@ -92,7 +111,7 @@ class VoxelHashMap:
     # -- extras (no reference counterpart in Python; C++ has GetClosestNeighbor) ----------------
     def compact(self):
         """rebuild the table at the smallest capacity (load <= 0.5, no tombstones)"""
-        N.check(N.lib().kb_map_compact(self._h))
+        self._mutated(N.lib().kb_map_compact(self._h))
 
     def num_points(self) -> int:
         n = N.sz(0)
@@ -123,7 +142,7 @@ class VoxelHashMap:
         pts = np.ascontiguousarray(points, dtype=np.float64)
         if vox.ndim != 2 or vox.shape[1] != 3 or cnt.shape != (len(vox),) or pts.ndim != 2 or pts.shape[1] != 3:
             raise ValueError("expected voxels (V, 3), counts (V,) and points (P, 3)")
-        check_value(N.lib().kb_map_load(self._h, N.ptr(vox), N.ptr(cnt), N.ptr(pts), len(vox), len(pts)))
+        self._mutated(N.lib().kb_map_load(self._h, N.ptr(vox), N.ptr(cnt), N.ptr(pts), len(vox), len(pts)), check_value)
 
     def closest_neighbors(self, queries):
         """batched VoxelHashMap::GetClosestNeighbor (VoxelHashMap.cpp:46-70)."""
