@@ -20,6 +20,20 @@ int kb_debug_icp_schur(const double acc[16], double x_schur[6], double x_ldlt[6]
 /* host evaluation of the latency-optimised (reciprocal / sincos) ICP solve step the kernels run:
  * x = LDLT solve, T = exp(x) * exp(b) */
 int kb_debug_icp_solve_fast(const double A[36], const double b[6], double x_fast[6], double T_fast[16]);
+/* device probes: the ICP loop's device code on the GPU, on given inputs (host arrays in and out).
+ * kb_debug_nn_reuse: per entry i, the candidate list made at pf[3i..] and the nearest neighbour then answered at p[3i..]
+ * (point, distance: DBL_MAX and (0,0,0) when there is none), reused[i] = 1 when the list answered, 0 when the point was
+ * searched again. path 0: the ICP team's list (R, staged slots: the map's KB_ICP_RADIUS / KB_ICP_SMEM_KB / KB_ICP_TEAM_Q
+ * at creation); path 1: the whole-grid ICP loop's cache (R = 0.2 voxel_size). */
+int kb_debug_nn_reuse(const kb_map *map, const double *pf, const double *p, size_t n, int path, double *out_points,
+                      double *out_dist, int *out_reused);
+/* the ICP team's solver step on n systems of 16 accumulators (layout of kb_debug_icp_schur): dx[6 n], used_schur[n] (1: the
+ * structured solve, 0: the LDL^T fallback), est[7 n] = exp(dx) as q(4) t(3), converged[n] = (|dx| < conv) */
+int kb_debug_icp_solve_dev(const double *acc, double conv, size_t n, double *dx, int *used_schur, double *est, int *converged);
+/* out[14 n]: per tangent (upsilon, omega), se3_exp_fast then se3_exp, each q(4) t(3) */
+int kb_debug_se3_exp_dev(const double *tangents, size_t n, double *out);
+/* out[n]: the device's fast_rcp (rcp.approx + two Newton steps) of x[n] */
+int kb_debug_fast_rcp_dev(const double *x, size_t n, double *out);
 /* work done by the ICP loop of the last RegisterFrame: GetClosestNeighbor calls (iterations x
  * source points) and map points examined — the inputs of the algorithmic-bytes formula */
 int kb_pipeline_last_icp_work(const kb_pipeline *p, double *queries, double *candidates);

@@ -41,10 +41,11 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/api.cu and csrc/localize.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
+    """Compile csrc/api.cu, csrc/localize.cu and csrc/probe.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in sources())
     if force or stale:
-        cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH, os.path.join(CSRC, "api.cu"), os.path.join(CSRC, "localize.cu")]
+        cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH,
+               *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "probe.cu"))]
         if verbose:
             print(" ".join(cmd))
         env = dict(os.environ)
@@ -156,6 +157,10 @@ SIGNATURES = {
     "kb_pipeline_history_stamps": (i32, [vp, vp, sz, C.POINTER(sz)]),
     "kb_debug_icp_solve_fast": (i32, [vp, vp, vp, vp]),
     "kb_debug_icp_schur": (i32, [vp, vp, vp, C.POINTER(i32)]),
+    "kb_debug_nn_reuse": (i32, [vp, vp, vp, sz, i32, vp, vp, vp]),
+    "kb_debug_icp_solve_dev": (i32, [vp, dbl, sz, vp, vp, vp, vp]),
+    "kb_debug_se3_exp_dev": (i32, [vp, sz, vp]),
+    "kb_debug_fast_rcp_dev": (i32, [vp, sz, vp]),
     "kb_debug_barrier_ns": (i32, [i32, C.POINTER(dbl)]),
     "kb_pipeline_last_ds_profile": (i32, [vp, vp]),
     "kb_pipeline_last_map_profile": (i32, [vp, vp]),

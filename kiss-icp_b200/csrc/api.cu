@@ -25,6 +25,7 @@
 #include "../../include/kiss_icp_b200.h"
 #include "../../include/kiss_icp_b200_debug.h"
 #include "kernels.cuh"
+#include "probe.cuh"
 
 using namespace kb;
 
@@ -2173,6 +2174,80 @@ int kb_debug_icp_schur(const double acc[16], double x_schur[6], double x_ldlt[6]
     if (!*used_schur) for (int i = 0; i < 6; ++i) x_schur[i] = x_ldlt[i];
     return KB_OK;
 }
+// the device probes (probe.cu): host arrays are copied to the device, the probe runs on the stream of `ex`, the results
+// are copied back
+int kb_debug_nn_reuse(const kb_map *map, const double *pf, const double *p, size_t n, int path, double *out_points,
+                      double *out_dist, int *out_reused) {
+    if (device_count() <= 0) return fail(KB_ERR_NO_DEVICE, "no CUDA device visible (this library has no CPU fallback)");
+    if (!map || (n &&(!pf || !p || !out_points || !out_dist || !out_reused))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (path != 0 && path != 1) return fail(KB_ERR_INVALID_ARG, "path must be 0 (ICP team) or 1 (whole-grid ICP loop)");
+    if (n > (size_t(1) << 28)) return fail(KB_ERR_INVALID_ARG, "n > 2^28");
+    if (n == 0) return KB_OK;
+    Exec &ex = *map->ex;
+    CK(cudaSetDevice(ex.device));
+    DBuf<double> d_pf, d_p, d_op, d_od;
+    DBuf<int> d_or;
+    RET(d_pf.ensure(3 * n));
+    RET(d_p.ensure(3 * n));
+    RET(d_op.ensure(3 * n));
+    RET(d_od.ensure(n));
+    RET(d_or.ensure(n));
+    CK(cudaMemcpyAsync(d_pf.p, pf, 24 * n, cudaMemcpyHostToDevice, ex.stream));
+    CK(cudaMemcpyAsync(d_p.p, p, 24 * n, cudaMemcpyHostToDevice, ex.stream));
+    const MapView mv = map->view();
+    CK(probe_nn_reuse(&mv, sizeof(mv), d_pf.p, d_p.p, static_cast<int>(n), path, ex.team.radius_frac, ex.team.smem_bytes,
+                      ex.icp_team_q, d_op.p, d_od.p, d_or.p, ex.stream));
+    ++ex.launches;
+    CK(cudaMemcpyAsync(out_points, d_op.p, 24 * n, cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(out_dist, d_od.p, 8 * n, cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(out_reused, d_or.p, sizeof(int) * n, cudaMemcpyDeviceToHost, ex.stream));
+    return ex.sync();
+}
+int kb_debug_icp_solve_dev(const double *acc, double conv, size_t n, double *dx, int *used_schur, double *est, int *converged) {
+    if (n && (!acc || !dx || !used_schur || !est || !converged)) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n > (size_t(1) << 24)) return fail(KB_ERR_INVALID_ARG, "n > 2^24");
+    DefaultCtx *c;
+    RET(default_ctx(&c));
+    if (n == 0) return KB_OK;
+    Exec &ex = *c->ex;
+    CK(cudaSetDevice(ex.device));
+    DBuf<double> d_acc, d_dx, d_est;
+    DBuf<int> d_used, d_conv;
+    RET(d_acc.ensure(NACC * n));
+    RET(d_dx.ensure(6 * n));
+    RET(d_est.ensure(7 * n));
+    RET(d_used.ensure(n));
+    RET(d_conv.ensure(n));
+    CK(cudaMemcpyAsync(d_acc.p, acc, sizeof(double) * NACC * n, cudaMemcpyHostToDevice, ex.stream));
+    CK(probe_icp_solve(d_acc.p, conv, static_cast<int>(n), d_dx.p, d_used.p, d_est.p, d_conv.p, ex.stream));
+    ++ex.launches;
+    CK(cudaMemcpyAsync(dx, d_dx.p, sizeof(double) * 6 * n, cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(est, d_est.p, sizeof(double) * 7 * n, cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(used_schur, d_used.p, sizeof(int) * n, cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(converged, d_conv.p, sizeof(int) * n, cudaMemcpyDeviceToHost, ex.stream));
+    return ex.sync();
+}
+// one probe with `k_in` doubles in and `k_out` doubles out per entry
+static int probe_map_doubles(const double *in, size_t n, int k_in, double *out, int k_out,
+                             cudaError_t (*probe)(const double *, int, double *, cudaStream_t)) {
+    if (n && (!in || !out)) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n > (size_t(1) << 26)) return fail(KB_ERR_INVALID_ARG, "n > 2^26");
+    DefaultCtx *c;
+    RET(default_ctx(&c));
+    if (n == 0) return KB_OK;
+    Exec &ex = *c->ex;
+    CK(cudaSetDevice(ex.device));
+    DBuf<double> d_in, d_out;
+    RET(d_in.ensure(k_in * n));
+    RET(d_out.ensure(k_out * n));
+    CK(cudaMemcpyAsync(d_in.p, in, sizeof(double) * k_in * n, cudaMemcpyHostToDevice, ex.stream));
+    CK(probe(d_in.p, static_cast<int>(n), d_out.p, ex.stream));
+    ++ex.launches;
+    CK(cudaMemcpyAsync(out, d_out.p, sizeof(double) * k_out * n, cudaMemcpyDeviceToHost, ex.stream));
+    return ex.sync();
+}
+int kb_debug_se3_exp_dev(const double *tangents, size_t n, double *out) { return probe_map_doubles(tangents, n, 6, out, 14, probe_se3_exp); }
+int kb_debug_fast_rcp_dev(const double *x, size_t n, double *out) { return probe_map_doubles(x, n, 1, out, 1, probe_fast_rcp); }
 int kb_debug_barrier_ns(int iters, double *ns_per_barrier) {
     if (!ns_per_barrier || iters < 1) return fail(KB_ERR_INVALID_ARG, "bad argument");
     DefaultCtx *c;

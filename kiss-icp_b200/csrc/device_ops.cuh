@@ -408,18 +408,20 @@ struct WarpNN {
 // when the cache was filled, d* its nearest-neighbour distance then, and S the candidates with
 // |c - p_f| <= d* + 2R. While the query has moved by delta <= R, its true nearest neighbour c'
 // satisfies |c' - p| <= |c* - p| <= d* + delta, hence |c' - p_f| <= d* + 2 delta <= d* + 2R, so
-// c' is in S; every candidate outside S is strictly farther than the minimum, so ties (resolved
-// by the stored reference sequence numbers) are unaffected. The cache is also tied to the
+// c' is in S; every candidate outside S is strictly farther than the minimum. The cache is also tied to the
 // query's VOXEL: GetClosestNeighbor only looks at the 27 voxels around the current voxel, so a
 // query that crosses a voxel face sees a different candidate set and must be re-probed —
 // UNLESS d* + 3R < voxel_size: then every point within d* + 2R of p_f (the whole of S and any
 // would-be closer point) is less than one voxel away from both p_f and p, i.e. inside the
-// 27-voxel neighbourhood of either position, and the voxel does not matter. The map is immutable during
+// 27-voxel neighbourhood of either position, and the set does not depend on the voxel. Its ORDER does: the stored
+// sequence numbers are the reference's visiting order around the fill's voxel only, so they break ties only there;
+// in another voxel a tie or near tie is searched again (icp_cache_answer). The map is immutable during
 // AlignPointsToMap and ICP steps shrink geometrically, so after the first iterations a query
 // costs no global memory traffic at all: ~30-cycle LDS instead of ~300-cycle L2 round trips,
 // and ~10-40 candidates instead of the 135-300 of the full 27-voxel neighbourhood.
 constexpr int QC_MAX = 64;   // cached candidates per query
 constexpr int QC_SLOTS = 2;  // cached queries per warp
+constexpr double QC_RADIUS = 0.2;  // R / voxel_size of the whole-grid ICP loop's cache
 struct QCache {
     int vx, vy, vz;  // voxel of the query at fill time (the reference searches the 27 voxels around it)
     int pad;
@@ -900,12 +902,15 @@ __device__ __forceinline__ NNResult nn_search_cached(const QCache &qc, const V3 
 // from the reference's comparison of rounded sqrt values if some other candidate's squared
 // distance lies within a few ulps above the minimum (two distinct squares rounding to the same
 // root). That near-tie is detected — every lane also tracks its second smallest square — and
-// then the exact routine above is used instead (in practice: never).
-__device__ __forceinline__ NNResult nn_search_cached_fast(const QCache &qc, const V3 &q, int lane) {
+// then the exact routine above is used instead (in practice: never). Exact ties count as near ties (an equal square
+// in the same lane, or a second lane at the minimum): the stored order breaks them like the reference only in the
+// voxel where the cache was filled, so outside it (same_voxel false) a tie returns false and the caller searches again.
+__device__ __forceinline__ bool nn_search_cached_fast(const QCache &qc, const V3 &q, int lane, bool same_voxel, NNResult &out) {
     double b2 = DBL_MAX, s2 = DBL_MAX;
     int bseq = INT_MAX;
     V3 bp{0, 0, 0};
     const int total = qc.total;
+#pragma unroll 4  // (the unroll the compiler chose before the tie test; left to itself it now unrolls further: +700 instructions)
     for (int k = lane; k < total; k += 32) {
         const V3 c{qc.pts[k][0], qc.pts[k][1], qc.pts[k][2]};
         const double d2 = sqnorm(c - q);
@@ -914,16 +919,21 @@ __device__ __forceinline__ NNResult nn_search_cached_fast(const QCache &qc, cons
             b2 = d2;
             bseq = qc.seq[k];
             bp = c;
-        } else if (d2 > b2 && d2 < s2) {
+        } else if (d2 < s2) {
             s2 = d2;
         }
     }
     const double mine = b2;
     nn_reduce(b2, bseq, bp);  // b2 = warp minimum (exact ties: smallest reference sequence number)
     const double lim = b2 * (1.0 + 8.8817841970012523e-16);
-    const bool near = (mine > b2 && mine <= lim) || (s2 <= lim);
-    if (__any_sync(FULL, near)) return nn_search_cached(qc, q, lane);
-    return NNResult{sqrt(b2), bp, qc.full};
+    const unsigned close = __ballot_sync(FULL, mine <= lim);  // lanes at or near the minimum
+    if ((close & (close - 1u)) != 0u || __any_sync(FULL, s2 <= lim)) {
+        if (!same_voxel) return false;
+        out = nn_search_cached(qc, q, lane);
+        return true;
+    }
+    out = NNResult{sqrt(b2), bp, qc.full};
+    return true;
 }
 
 // 24-byte point record -> one 16-byte + one 8-byte load (records are 8-byte aligned, every other one 16-byte)
@@ -1156,6 +1166,17 @@ __host__ __device__ __forceinline__ void icp_expand(const double a[NACC], double
     for (int i = 0; i < 6; ++i) JTr[i] = a[10 + i];
 }
 
+// the cache's answer for the query at p (whole warp), when it has one: the query has moved by <= radius since the fill
+// and is still in the fill's voxel, or in another one with any_voxel and no tie (QCache). false: search again.
+__device__ __forceinline__ bool icp_cache_answer(const QCache &qc, const MapView &m, const V3 &p, double radius, int lane,
+                                                 NNResult &r) {
+    const V3 moved = p - V3{qc.pf[0], qc.pf[1], qc.pf[2]};
+    const int3 v = point_to_voxel(p.x, p.y, p.z, m.vdiv);
+    const bool same_voxel = qc.vx == v.x && qc.vy == v.y && qc.vz == v.z;
+    return qc.total >= 0 && sqnorm(moved) <= radius * radius && (qc.any_voxel || same_voxel) &&
+           nn_search_cached_fast(qc, p, lane, same_voxel, r);
+}
+
 // One DataAssociation + BuildLinearSystem pass of THIS CTA (Registration.cpp:60-121): `pending`
 // is applied to every source point first (TransformPoints, :55-58), the moved point is written
 // back to `work`, and the CTA's partial normal equations go to blk_d[parity][cta][NPART].
@@ -1194,12 +1215,9 @@ __device__ __noinline__ void icp_queries(const Scratch &sc, Shared &sh, const Ma
                 if (first) qc->total = -1;
             }
             __syncwarp();
-            const double radius = 0.2 * m.voxel_size;
-            const V3 moved = p - V3{qc->pf[0], qc->pf[1], qc->pf[2]};
-            const int3 v = point_to_voxel(p.x, p.y, p.z, m.vdiv);
-            if (qc->total >= 0 && sqnorm(moved) <= radius * radius &&
-                (qc->any_voxel || (qc->vx == v.x && qc->vy == v.y && qc->vz == v.z)))
-                r = nn_search_cached_fast(*qc, p, lane), ++n_hit;
+            const double radius = QC_RADIUS * m.voxel_size;
+            if (icp_cache_answer(*qc, m, p, radius, lane, r))
+                ++n_hit;
             else {
                 // whether filling already pays off on the first iteration depends on the size of the first step:
                 // with a good constant-velocity prediction (steady driving) most caches survive it, after a poor one they are refilled on iteration 1 anyway (fill_first = false)

@@ -32,8 +32,9 @@ constexpr int TRED_STRIDE = NACC + 1;  // row of the per-point reduction scratch
 static_assert(TQ_MAX * TRED_STRIDE * 8 <= DS_MAX_CHUNKS * 4, "the reduction scratch lives in Shared::chunk_pref");
 
 // Output of the fill pass for one source point (global memory): the list holds POINT INDICES (slot * cap + k) in the
-// reference's visiting order (voxel_shifts order, then insertion order), so the first strict minimum over the
-// list is the reference's answer, ties included.
+// reference's visiting order (voxel_shifts order, then insertion order) around the voxel where it was made, so for a
+// point in that voxel the first strict minimum over the list is the reference's answer, ties included (in another
+// voxel a tie is searched again: team_list_nn).
 struct QList {
     int count;      // >= 0: idx[0..count) valid; -1: not cacheable (too many candidates / max_points_per_voxel > 32)
     int full;       // points of the whole 27-voxel neighbourhood (bookkeeping of algorithmic bytes)
@@ -469,27 +470,118 @@ __device__ __noinline__ void team_refill(Shared &sh, const MapView &m, const Tea
 #define KB_TCYC(i)
 #endif
 
-// DataAssociation + BuildLinearSystem (Registration.cpp:60-121) for this CTA's source points, iteration j. The loop is a
-// dependent chain, so what counts is the length of the per-point instruction chain: four lanes share a point (8
-// points per warp), each walks a quarter of the candidate list from conflict-free shared memory, two shuffle levels
-// merge them, and the 16 accumulators are split over the four lanes (one 3-level shuffle sum per warp).
+// One source point's nearest neighbour from its staged list, and whether that answer is the reference's (return value;
+// false: the point must be searched again). With `move` the point is first moved by `pending` and stored back. Called by
+// whole warps; four lanes (l4) per point.
 //
 // When is the staged list still exact? Let p_f be where it was made (d* the nearest distance then, the list = all
 // points of the 27 voxels around p_f within d* + 2R of p_f), p the current position with |p - p_f| <= R, and d_S the
 // smallest distance from p to the list. A point x of the CURRENT 27-voxel neighbourhood that is not in the list is
 // either in the old neighbourhood, then |x - p_f| > d* + 2R and |x - p| > d* + R >= d_S; or outside it, then
-// |x - p_f| >= voxel_size and |x - p| >= voxel_size - R. So the list answers exactly when the voxel is unchanged, or
-// when d_S < voxel_size - R (its minimiser is then within one voxel of p, i.e. inside the current neighbourhood).
-// Otherwise (moved > R, or a far match that changed voxel) the point is queued and searched again by a whole warp —
-// ALL warps of the CTA serve that queue.
+// |x - p_f| >= voxel_size and |x - p| >= voxel_size - R. So the list holds the nearest distance when the voxel is
+// unchanged, or when d_S < voxel_size - R (its minimiser is then within one voxel of p, i.e. inside the current
+// neighbourhood). The list's ORDER is the reference's visiting order around the voxel where it was made only: in
+// another voxel the reference visits the 27 voxels around the current one, so a tie or near tie there can resolve to
+// another point, and such a point is searched again as well.
+__device__ __forceinline__ bool team_list_nn(const TeamSmem &sm, TQHead &t, const VoxelDiv &vdiv, double radius, bool have,
+                                             int li, int l4, bool move, const SE3 &pending, V3 &p, double &d, V3 &np,
+                                             unsigned long long *dbg) {
+    const double voxel_size = vdiv.v, r2max = radius * radius;
+    bool ok = false;
+    int cnt = 0;
+    bool same_voxel = false;
+    if (have) {
+        p = V3{t.p[0], t.p[1], t.p[2]};
+        if (move) p = se3_act(pending, p);  // TransformPoints(estimation, source)  Registration.cpp:160
+        const V3 moved = p - V3{t.pf[0], t.pf[1], t.pf[2]};
+        const int3 v = point_to_voxel(p.x, p.y, p.z, vdiv);
+        same_voxel = t.vx == v.x && t.vy == v.y && t.vz == v.z;
+        ok = t.count >= 0 && sqnorm(moved) <= r2max;
+        cnt = ok ? t.count : 0;
+    }
+    KB_WCYC(0);
+    __syncwarp();  // all four lanes have read t.p
+    if (have && l4 == 0 && move) {
+        t.p[0] = p.x;
+        t.p[1] = p.y;
+        t.p[2] = p.z;
+    }
+    // first strict minimum of the squared distance over the list (= reference order); s2 = second smallest
+    // (equal squares count: an exact tie takes the slow exact path below). Lane l4 takes candidates l4, l4 + 4, ...:
+    // row i of the warp's block, column (4 q8 + l4 + 4 i) & 31.
+    double b2 = DBL_MAX, s2 = DBL_MAX;
+    int bk = INT_MAX;
+    const unsigned cbase = static_cast<unsigned>(__cvta_generic_to_shared(sm.coords));
+    const unsigned wbase = cbase + static_cast<unsigned>((li / TQ_PER_WARP) * (sm.K >> 2)) * 768u;
+    const int c0 = 4 * (li & (TQ_PER_WARP - 1)) + l4;
+    constexpr int U = 4;  // (kept small: code size of the loop body matters more than trips)
+    for (int i0 = 0; 4 * i0 + l4 < cnt; i0 += U) {
+        double d2[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {  // independent loads and distances in flight, no branches
+            const int i = i0 + u;
+            const bool in = 4 * i + l4 < cnt;
+            const int ii = in ? i : 0;
+            const unsigned a = wbase + static_cast<unsigned>(ii) * 768u + (static_cast<unsigned>((c0 + 4 * ii) & 31) << 3);
+            const V3 c{lds_f64(a), lds_f64(a + 256u), lds_f64(a + 512u)};
+            const double dd = sqnorm(c - p);
+            d2[u] = in ? dd : DBL_MAX;
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) {  // (no NaNs here: plain compare + select instead of fmin / fmax)
+            const bool lt = d2[u] < b2;
+            const double hi = lt ? b2 : d2[u];
+            b2 = lt ? d2[u] : b2;
+            bk = lt ? 4 * (i0 + u) + l4 : bk;
+            s2 = hi < s2 ? hi : s2;
+        }
+    }
+    KB_WCYC(1);
+#pragma unroll
+    for (int o = 1; o < TQ_LANES; o <<= 1) {
+        const double ob2 = __shfl_xor_sync(FULL, b2, o), os2 = __shfl_xor_sync(FULL, s2, o);
+        const int ok2 = __shfl_xor_sync(FULL, bk, o);
+        const bool take = (ob2 < b2) || (ob2 == b2 && ok2 < bk);
+        const double hi = (ob2 < b2) ? b2 : ob2;  // max(b2, ob2)
+        double ns2 = os2 < s2 ? os2 : s2;
+        ns2 = hi < ns2 ? hi : ns2;
+        bk = take ? ok2 : bk;
+        b2 = (ob2 < b2) ? ob2 : b2;
+        s2 = ns2;
+    }
+    if (cnt > 0) {
+        const unsigned a = tq_coord_addr(cbase, sm.K, li, bk);
+        np = V3{lds_f64(a), lds_f64(a + 256u), lds_f64(a + 512u)};
+        d = sqrt(b2);
+    }
+    KB_WCYC(2);
+    // two squares within a few ulps could round to the same root: then compare rounded roots in reference
+    // order like GetClosestNeighbor does (in practice never)
+    const bool near = cnt > 0 && s2 <= b2 * (1.0 + 8.8817841970012523e-16);
+    if (__any_sync(FULL, near)) {
+        tq_exact_nn(sm, li, l4, cnt, near, p.x, p.y, p.z);
+        if (near) {
+            d = t.nn[3];
+            np = V3{t.nn[0], t.nn[1], t.nn[2]};
+        }
+    }
+    KB_WCYC(3);
+    return ok && (same_voxel || (!near && d < (voxel_size - radius) * (1.0 - 1e-12)));
+}
+
+// DataAssociation + BuildLinearSystem (Registration.cpp:60-121) for this CTA's source points, iteration j. The loop is a
+// dependent chain, so what counts is the length of the per-point instruction chain: four lanes share a point (8
+// points per warp), each walks a quarter of the candidate list from conflict-free shared memory (team_list_nn), two
+// shuffle levels merge them, and the 16 accumulators are split over the four lanes (one 3-level shuffle sum per warp).
+// A point whose list no longer answers exactly (moved > R, or changed voxel with a far match or a tie) is queued and
+// searched again by a whole warp — ALL warps of the CTA serve that queue.
 template <bool kSlot>
 __device__ __forceinline__ void team_queries(uint4 *ll, Shared &sh, const MapView &m, const TeamSmem sm, const VoxelDiv vdiv, double radius_frac, int nq, int j,
                                           double max_dist, double kscale, int member, int T, unsigned tag,
                                           unsigned long long *dbg, int stride) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int l4 = lane & (TQ_LANES - 1), li = tid / TQ_LANES;
-    const double voxel_size = vdiv.v;
-    const double radius = radius_frac * voxel_size, r2max = radius * radius;
+    const double radius = radius_frac * vdiv.v;
     const bool have = li < nq;
     const int par = j & 1;
     double *red = reinterpret_cast<double *>(sh.chunk_pref);  // [TQ_MAX][TRED_STRIDE], free during the ICP
@@ -501,85 +593,7 @@ __device__ __forceinline__ void team_queries(uint4 *ll, Shared &sh, const MapVie
     bool ok = false;
     const int nwarps_q = (nq + TQ_PER_WARP - 1) / TQ_PER_WARP;  // warps that own source points
     if (warp < nwarps_q) {
-        int cnt = 0;
-        bool same_voxel = false;
-        if (have) {
-            p = V3{t.p[0], t.p[1], t.p[2]};
-            if (j > 0) p = se3_act(sh.pending, p);  // TransformPoints(estimation, source)  Registration.cpp:160
-            const V3 moved = p - V3{t.pf[0], t.pf[1], t.pf[2]};
-            const int3 v = point_to_voxel(p.x, p.y, p.z, vdiv);
-            same_voxel = t.vx == v.x && t.vy == v.y && t.vz == v.z;
-            ok = t.count >= 0 && sqnorm(moved) <= r2max;
-            cnt = ok ? t.count : 0;
-        }
-        KB_WCYC(0);
-        __syncwarp();  // all four lanes have read t.p
-        if (have && l4 == 0 && j > 0) {
-            t.p[0] = p.x;
-            t.p[1] = p.y;
-            t.p[2] = p.z;
-        }
-        // first strict minimum of the squared distance over the list (= reference order); s2 = second smallest
-        // (equal squares count: an exact tie takes the slow exact path below). Lane l4 takes candidates l4, l4 + 4, ...:
-        // row i of the warp's block, column (4 q8 + l4 + 4 i) & 31.
-        double b2 = DBL_MAX, s2 = DBL_MAX;
-        int bk = INT_MAX;
-        const unsigned cbase = static_cast<unsigned>(__cvta_generic_to_shared(sm.coords));
-        const unsigned wbase = cbase + static_cast<unsigned>((li / TQ_PER_WARP) * (sm.K >> 2)) * 768u;
-        const int c0 = 4 * (li & (TQ_PER_WARP - 1)) + l4;
-        constexpr int U = 4;  // (kept small: code size of the loop body matters more than trips)
-        for (int i0 = 0; 4 * i0 + l4 < cnt; i0 += U) {
-            double d2[U];
-#pragma unroll
-            for (int u = 0; u < U; ++u) {  // independent loads and distances in flight, no branches
-                const int i = i0 + u;
-                const bool in = 4 * i + l4 < cnt;
-                const int ii = in ? i : 0;
-                const unsigned a = wbase + static_cast<unsigned>(ii) * 768u + (static_cast<unsigned>((c0 + 4 * ii) & 31) << 3);
-                const V3 c{lds_f64(a), lds_f64(a + 256u), lds_f64(a + 512u)};
-                const double dd = sqnorm(c - p);
-                d2[u] = in ? dd : DBL_MAX;
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {  // (no NaNs here: plain compare + select instead of fmin / fmax)
-                const bool lt = d2[u] < b2;
-                const double hi = lt ? b2 : d2[u];
-                b2 = lt ? d2[u] : b2;
-                bk = lt ? 4 * (i0 + u) + l4 : bk;
-                s2 = hi < s2 ? hi : s2;
-            }
-        }
-        KB_WCYC(1);
-#pragma unroll
-        for (int o = 1; o < TQ_LANES; o <<= 1) {
-            const double ob2 = __shfl_xor_sync(FULL, b2, o), os2 = __shfl_xor_sync(FULL, s2, o);
-            const int ok2 = __shfl_xor_sync(FULL, bk, o);
-            const bool take = (ob2 < b2) || (ob2 == b2 && ok2 < bk);
-            const double hi = (ob2 < b2) ? b2 : ob2;  // max(b2, ob2)
-            double ns2 = os2 < s2 ? os2 : s2;
-            ns2 = hi < ns2 ? hi : ns2;
-            bk = take ? ok2 : bk;
-            b2 = (ob2 < b2) ? ob2 : b2;
-            s2 = ns2;
-        }
-        if (cnt > 0) {
-            const unsigned a = tq_coord_addr(cbase, sm.K, li, bk);
-            np = V3{lds_f64(a), lds_f64(a + 256u), lds_f64(a + 512u)};
-            d = sqrt(b2);
-        }
-        KB_WCYC(2);
-        // two squares within a few ulps could round to the same root: then compare rounded roots in reference
-        // order like GetClosestNeighbor does (in practice never)
-        const bool near = cnt > 0 && s2 <= b2 * (1.0 + 8.8817841970012523e-16);
-        if (__any_sync(FULL, near)) {
-            tq_exact_nn(sm, li, l4, cnt, near, p.x, p.y, p.z);
-            if (near) {
-                d = t.nn[3];
-                np = V3{t.nn[0], t.nn[1], t.nn[2]};
-            }
-        }
-        KB_WCYC(3);
-        ok = ok && (same_voxel || d < (voxel_size - radius) * (1.0 - 1e-12));
+        ok = team_list_nn(sm, t, vdiv, radius, have, li, l4, j > 0, sh.pending, p, d, np, dbg);
         if (have && !ok && l4 == 0) sh.refill_q[atomicAdd(&sh.refill_n[par], 1)] = li;
         // this point's 16 entries of J^T w J / J^T w r (lane l4: entries 4 l4 ..) + the gate flag -> row li of the
         // reduction scratch; a stale point writes zeros now and its row again after the re-search
@@ -726,15 +740,12 @@ __device__ __noinline__ void team_solve_ldlt(const double sys[NACC], double dx[6
 __device__ __noinline__ SE3 team_exp_large(const double dx[6]) { return se3_exp_fast(dx); }
 __device__ __noinline__ bool team_norm_below(double n2, double conv) { return sqrt(n2) < conv; }
 
-// one thread: dx = JTJ.ldlt().solve(-JTr), estimation = SE3::exp(dx), convergence test (Registration.cpp:156-157,163)
-__device__ __forceinline__ void team_solve(Shared &sh, double conv, bool last_allowed) {
-    double sys[NACC];
-#pragma unroll
-    for (int i = 0; i < NACC; ++i) sys[i] = sh.red[i];
-    double dx[6];
-    if (!icp_solve_schur(sys, dx)) team_solve_ldlt(sys, dx);  // structured 3x3 Schur solve; cold: pivoted LDL^T
+// dx = JTJ.ldlt().solve(-JTr) and estimation = SE3::exp(dx) (Registration.cpp:156-157) on the 16 accumulators; returns
+// the squared norm of dx. used_schur: the structured solve took the system.
+__device__ __forceinline__ double team_solve_step(const double sys[NACC], double dx[6], SE3 &est, bool &used_schur) {
+    used_schur = icp_solve_schur(sys, dx);
+    if (!used_schur) team_solve_ldlt(sys, dx);  // structured 3x3 Schur solve; cold: pivoted LDL^T
     const double theta_sq = (dx[3] * dx[3] + dx[4] * dx[4]) + dx[5] * dx[5];
-    SE3 est;
     if (theta_sq >= kEps * kEps && theta_sq < 0.01) {
         est = se3_exp_small(dx, theta_sq);
     } else {
@@ -743,12 +754,27 @@ __device__ __forceinline__ void team_solve(Shared &sh, double conv, bool last_al
     double n2 = 0.0;
 #pragma unroll
     for (int i = 0; i < 6; ++i) n2 += dx[i] * dx[i];
-    sh.pending = est;
-    // dx.norm() < convergence_criterion (:163): decided on the square unless it is within rounding of the boundary
+    return n2;
+}
+// dx.norm() < convergence_criterion (:163) for n2 = |dx|^2: decided on the square unless it is within rounding of the boundary
+__device__ __forceinline__ bool team_converged(double n2, double conv) {
     const double c2 = conv * conv;
     bool conv_reached = n2 < c2 * (1.0 - 1e-14);
     if (!conv_reached && n2 <= c2 * (1.0 + 1e-14)) conv_reached = team_norm_below(n2, conv);  // cold
-    sh.flag = (conv_reached || last_allowed) ? 1 : 0;
+    return conv_reached;
+}
+
+// one thread: the solver step of the iteration on the gathered sums -> sh.pending, sh.flag
+__device__ __forceinline__ void team_solve(Shared &sh, double conv, bool last_allowed) {
+    double sys[NACC];
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) sys[i] = sh.red[i];
+    double dx[6];
+    SE3 est;
+    bool used_schur;
+    const double n2 = team_solve_step(sys, dx, est, used_schur);
+    sh.pending = est;
+    sh.flag = (team_converged(n2, conv) || last_allowed) ? 1 : 0;
 }
 
 // the iterations, on a team of T CTAs. Precondition: icp_fill_pass + a grid barrier, map not empty, max_iter > 0,

@@ -151,18 +151,8 @@ def test_structured_schur_solve_matches_ldlt():
     assembled from real correspondences it must agree with the pivoted 6x6 LDL^T, and it must decline
     degenerate systems (which then take the LDL^T path with Eigen's zero-pivot rule)"""
     from kiss_icp_b200 import _native as N
+    from test_device_probes import accumulate
     rng = np.random.default_rng(10)
-
-    def accumulate(S, R, W):
-        acc = np.zeros(16)
-        for s, r, w in zip(S, R, W):
-            x, y, z = s
-            acc[0] += w; acc[1] += w * x; acc[2] += w * y; acc[3] += w * z
-            acc[4] += w * (z * z + y * y); acc[5] += -w * x * y; acc[6] += w * (z * z + x * x)
-            acc[7] += -w * x * z; acc[8] += -w * y * z; acc[9] += w * (y * y + x * x)
-            acc[10:13] += w * r
-            acc[13] += w * (-z * r[1] + y * r[2]); acc[14] += w * (z * r[0] - x * r[2]); acc[15] += w * (-y * r[0] + x * r[1])
-        return acc
 
     for scale in (1.0, 30.0, 100.0):
         for _ in range(25):
