@@ -316,6 +316,60 @@ int kb_pipeline_register_frames_fit(kb_pipeline *p, const void *const *xyz, cons
                                     const double *const *timestamps, const size_t *n_timestamps, size_t count,
                                     int layout, double *poses_out, kb_fit *fits_out);
 
+/* ---- relocalization: a global pose search in a bounded region ----------------------------
+ * No reference counterpart. Finds a scan's pose in a map without an initial pose: every hypothesis of a grid in x, y
+ * and yaw around a centre is scored on the device, the best peaks are refined with kb_registration_align_batch, and
+ * the winner is the refined candidate with the most inliers. Whether to accept it is the caller's decision. */
+/* The grid: Nx = 2 half_cells_x + 1, Ny = 2 half_cells_y + 1, H = n_yaw Nx Ny <= 2^24 hypotheses. Hypothesis
+ * h = (k Ny + (j + half_cells_y)) Nx + (i + half_cells_x), i in [-half_cells_x, half_cells_x], j likewise, k in [0, n_yaw):
+ *   yaw_k = (k - n_yaw / 2) yaw_step (integer division), R_h = Rz(yaw_k) R_c with Rz = [c -s 0; s c 0; 0 0 1] from
+ *   std::cos / std::sin and R_h[r][c] = (Rz[r][0] R_c[0][c] + Rz[r][1] R_c[1][c]) + Rz[r][2] R_c[2][c],
+ *   t_h = (t_c.x + i step, t_c.y + j step, t_c.z).
+ * z, roll and pitch come from the centre. The yaw axis is a full circle when |n_yaw yaw_step - 2 pi| < 1e-9.
+ * max_correspondence_distance and kernel_scale are those of the refinement (kb_registration_align_points_to_map). */
+typedef struct kb_reloc_search {
+    double center[16];              /* row-major SE(3) */
+    int half_cells_x, half_cells_y; /* >= 0 */
+    double step;                    /* metres between grid positions, > 0 */
+    int n_yaw;                      /* >= 1 */
+    double yaw_step;                /* radians, > 0 */
+    int top_k;                      /* peaks refined, 1..256 */
+    double max_correspondence_distance, kernel_scale;
+} kb_reloc_search;
+/* The hypotheses kb_relocalize scores, in order h, as row-major poses[H][16]. Two-call like kb_map_pointcloud: *n_out = H;
+ * poses NULL or cap 0 only queries it, cap < H is KB_ERR_CAPACITY. Host only (works without a device).
+ * KB_ERR_INVALID_ARG for a field outside its range, H > 2^24 or a non-finite centre translation, KB_ERR_NOT_SE3 for a
+ * centre rotation that is not in SO(3). */
+int kb_reloc_hypotheses(const kb_reloc_search *search, double *poses, size_t cap, size_t *n_out);
+typedef struct kb_reloc_result {
+    double pose[16];  /* the winner, refined, row-major */
+    int inliers, iterations, rank; /* its inliers, ICP iterations and index among the candidates */
+    int n_source;
+    int n_hypotheses, n_peaks, n_candidates;
+    double runner_up_pose[16];     /* all zero when there is no runner-up */
+    int runner_up_inliers;         /* -1 when there is no runner-up */
+} kb_reloc_result;
+/* Relocalize the source xyz[n] in map within `search`:
+ *   1. score_h = source points q whose voxel point_to_voxel(R_h p_q + t_h) the map holds, each component computed as
+ *      ((R0 x + R1 y) + R2 z) + t0 (one device launch on the map's stream, integer counts: deterministic);
+ *   2. peaks: h is a peak when no neighbour (i +- 1, j +- 1, k +- 1; k wraps on a full circle; no padding at the edges)
+ *      has a higher score, or the same score and a smaller h;
+ *   3. candidates: the peaks by (score descending, h ascending), the first top_k;
+ *   4. refinement: kb_registration_align_batch of the source from every candidate with the search's thresholds, inliers
+ *      on: each refined pose, iteration count and inlier count is bit for bit that call's. Uses reg's
+ *      max_num_iterations and convergence criterion; kb_registration_last_iterations is unchanged;
+ *   5. winner: the most inliers, ties to the lower rank. Runner-up: the best other candidate (same order) whose refined
+ *      pose is farther from the winner's than 2 step in xy or 2 yaw_step in rotation angle.
+ * candidates (double[top_k][16], the coarse poses), candidate_scores (int[top_k]) and scores (int[H], in order h) may each
+ * be NULL; the first n_candidates entries are written. Host buffers. Only reads the map: allowed while localizers hold it.
+ * Every argument is checked before any work, and on error nothing is written: KB_ERR_INVALID_ARG for a NULL pointer,
+ * n = 0, an empty map, the limits of kb_reloc_hypotheses, or a hypothesis under which a source point's voxel coordinate
+ * would not fit in an int (checked from |t_h| and the largest |p|); KB_ERR_NOT_SE3 for the centre. Handles exist only
+ * where a device does: without one the call returns KB_ERR_NO_DEVICE once the arguments that need no handle (search,
+ * source, out) have passed. */
+int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_map *map, const kb_reloc_search *search,
+                  kb_reloc_result *out, double *candidates, int *candidate_scores, int *scores);
+
 #ifdef __cplusplus
 }
 #endif

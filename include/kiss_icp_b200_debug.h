@@ -34,6 +34,9 @@ int kb_debug_icp_solve_dev(const double *acc, double conv, size_t n, double *dx,
 int kb_debug_se3_exp_dev(const double *tangents, size_t n, double *out);
 /* out[n]: the device's fast_rcp (rcp.approx + two Newton steps) of x[n] */
 int kb_debug_fast_rcp_dev(const double *x, size_t n, double *out);
+/* device time [ms] of the coarse score (k_reloc_score) of the last kb_relocalize on this handle, from CUDA events recorded
+ * around its launch; KB_ERR_INVALID_ARG before the first call */
+int kb_debug_reloc_score_ms(const kb_registration *reg, float *ms);
 /* work done by the ICP loop of the last RegisterFrame: GetClosestNeighbor calls (iterations x
  * source points) and map points examined — the inputs of the algorithmic-bytes formula */
 int kb_pipeline_last_icp_work(const kb_pipeline *p, double *queries, double *candidates);

@@ -7,6 +7,7 @@ from .kiss_icp import KissICP  # noqa: F401
 from .mapping import VoxelHashMap, get_voxel_hash_map  # noqa: F401
 from .preprocess import Preprocessor, get_preprocessor  # noqa: F401
 from .registration import Registration, get_registration  # noqa: F401
+from .relocalization import RelocalizationResult, RelocalizationSearch  # noqa: F401
 from .threshold import AdaptiveThreshold, FixedThreshold, get_threshold_estimator  # noqa: F401
 from .voxelization import voxel_down_sample  # noqa: F401
 from .preprocess import correct_kitti_scan  # noqa: F401

@@ -41,11 +41,12 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/api.cu, csrc/localize.cu and csrc/probe.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
+    """Compile csrc/api.cu, csrc/localize.cu, csrc/probe.cu and csrc/relocalize.cu -> libkiss_icp_b200.so (sm_90a).
+    No-op when up to date."""
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in sources())
     if force or stale:
         cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH,
-               *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "probe.cu"))]
+               *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "probe.cu", "relocalize.cu"))]
         if verbose:
             print(" ".join(cmd))
         env = dict(os.environ)
@@ -91,6 +92,19 @@ class PipelineState(C.Structure):
 class Fit(C.Structure):
     """kb_fit: the fit of one localized frame at its final pose"""
     _fields_ = [("n_correspondences", i32), ("n_source", i32), ("sum_sq_residual", dbl), ("JTJ", dbl * 36)]
+
+
+class RelocSearch(C.Structure):
+    """kb_reloc_search: the hypothesis grid of kb_relocalize"""
+    _fields_ = [("center", dbl * 16), ("half_cells_x", i32), ("half_cells_y", i32), ("step", dbl), ("n_yaw", i32),
+                ("yaw_step", dbl), ("top_k", i32), ("max_correspondence_distance", dbl), ("kernel_scale", dbl)]
+
+
+class RelocResult(C.Structure):
+    """kb_reloc_result"""
+    _fields_ = [("pose", dbl * 16), ("inliers", i32), ("iterations", i32), ("rank", i32), ("n_source", i32),
+                ("n_hypotheses", i32), ("n_peaks", i32), ("n_candidates", i32), ("runner_up_pose", dbl * 16),
+                ("runner_up_inliers", i32)]
 
 
 # every exported symbol of include/kiss_icp_b200.h: name -> (restype, argtypes)
@@ -184,6 +198,9 @@ SIGNATURES = {
     "kb_map_readers": (i32, [vp, C.POINTER(i32)]),
     "kb_pipeline_last_fit": (i32, [vp, C.POINTER(Fit)]),
     "kb_pipeline_register_frames_fit": (i32, [vp, vp, vp, vp, vp, sz, i32, vp, vp]),
+    "kb_reloc_hypotheses": (i32, [C.POINTER(RelocSearch), vp, sz, C.POINTER(sz)]),
+    "kb_relocalize": (i32, [vp, vp, sz, vp, C.POINTER(RelocSearch), C.POINTER(RelocResult), vp, vp, vp]),
+    "kb_debug_reloc_score_ms": (i32, [vp, C.POINTER(C.c_float)]),
 }
 
 

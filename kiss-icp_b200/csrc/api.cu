@@ -26,6 +26,7 @@
 #include "../../include/kiss_icp_b200_debug.h"
 #include "kernels.cuh"
 #include "probe.cuh"
+#include "relocalize.cuh"
 
 using namespace kb;
 
@@ -658,6 +659,15 @@ struct kb_registration {
     DBuf<unsigned> bctl;
     DBuf<double> bpose;   // outputs of the host entry point
     DBuf<int> biout;
+    DBuf<double> rgrid;   // kb_relocalize: rotations [n_yaw][9], then xs [Nx], ys [Ny]
+    DBuf<int> rscore;     // kb_relocalize: scores [H]
+    cudaEvent_t rev[2] = {nullptr, nullptr};  // around the last k_reloc_score (kb_debug_reloc_score_ms)
+    int rev_device = -1;
+    ~kb_registration() {
+        if (device_is_stuck(-1)) return;
+        for (cudaEvent_t e : rev)
+            if (e) cudaEventDestroy(e);
+    }
 };
 
 struct kb_preprocessor {
@@ -1337,6 +1347,223 @@ int kb_registration_align_batch_dev(kb_registration *reg, const double *d_xyz, s
     RET(align_batch_check(reg, map, d_xyz, n_points, off.data(), cnt.data(), B, gs.data(), md.data(), ks.data(), d_poses,
                           d_iterations, &g));
     return align_batch_run(reg, map, d_xyz, off.data(), cnt.data(), B, g, md.data(), ks.data(), d_poses, d_iterations, d_inliers);
+}
+
+// ------------------------------------------------------------------------------- Relocalization
+// The hypothesis grid of a kb_reloc_search. It is enumerated here only: kb_reloc_hypotheses returns it, kb_relocalize
+// scores and refines it.
+struct RelocGrid {
+    int hx, hy, nx, ny, n_yaw;
+    size_t H;
+    bool full_circle;  // the yaw axis wraps
+    std::vector<double> rot;     // [n_yaw][9] R_k = Rz(yaw_k) R_c, row-major
+    std::vector<double> xs, ys;  // [Nx] t_c.x + i step, [Ny] t_c.y + j step
+    double tz;
+    void pose(size_t h, double M[16]) const {
+        const size_t plane = static_cast<size_t>(nx) * ny, k = h / plane, l = h - k * plane, jj = l / nx, ii = l - jj * nx;
+        const double *R = rot.data() + 9 * k;
+        const double out[16] = {R[0], R[1], R[2], xs[ii], R[3], R[4], R[5], ys[jj], R[6], R[7], R[8], tz, 0.0, 0.0, 0.0, 1.0};
+        std::memcpy(M, out, sizeof(out));
+    }
+};
+static int reloc_grid(const kb_reloc_search *s, RelocGrid *g) {
+    constexpr size_t kMaxHyp = size_t(1) << 24;
+    constexpr double kTwoPi = 6.283185307179586;
+    if (s->half_cells_x < 0 || s->half_cells_y < 0) return fail(KB_ERR_INVALID_ARG, "half_cells_x and half_cells_y must be >= 0");
+    if (!(s->step > 0.0) || !std::isfinite(s->step)) return fail(KB_ERR_INVALID_ARG, "step must be finite and > 0");
+    if (s->n_yaw < 1) return fail(KB_ERR_INVALID_ARG, "n_yaw must be >= 1");
+    if (!(s->yaw_step > 0.0) || !std::isfinite(s->yaw_step)) return fail(KB_ERR_INVALID_ARG, "yaw_step must be finite and > 0");
+    if (s->top_k < 1 || s->top_k > 256) return fail(KB_ERR_INVALID_ARG, "top_k must be in [1, 256]");
+    const size_t nx = 2 * static_cast<size_t>(s->half_cells_x) + 1, ny = 2 * static_cast<size_t>(s->half_cells_y) + 1;
+    if (nx > kMaxHyp || ny > kMaxHyp || nx * ny > kMaxHyp || nx * ny * static_cast<size_t>(s->n_yaw) > kMaxHyp)
+        return fail(KB_ERR_INVALID_ARG, "more than 2^24 hypotheses (%zu x %zu positions x %d headings)", nx, ny, s->n_yaw);
+    const double *M = s->center;
+    SE3 c;
+    if (!to_se3(M, &c)) return fail(KB_ERR_NOT_SE3, "search center is not in SE(3)");
+    if (!std::isfinite(M[3]) || !std::isfinite(M[7]) || !std::isfinite(M[11]))
+        return fail(KB_ERR_INVALID_ARG, "search center has a non-finite translation");
+    g->hx = s->half_cells_x;
+    g->hy = s->half_cells_y;
+    g->nx = static_cast<int>(nx);
+    g->ny = static_cast<int>(ny);
+    g->n_yaw = s->n_yaw;
+    g->H = nx * ny * static_cast<size_t>(s->n_yaw);
+    g->full_circle = std::fabs(s->n_yaw * s->yaw_step - kTwoPi) < 1e-9;
+    g->rot.resize(9 * static_cast<size_t>(s->n_yaw));
+    for (int k = 0; k < s->n_yaw; ++k) {
+        const double yaw = static_cast<double>(k - s->n_yaw / 2) * s->yaw_step;
+        const double cs = std::cos(yaw), sn = std::sin(yaw);
+        const double Rz[9] = {cs, -sn, 0.0, sn, cs, 0.0, 0.0, 0.0, 1.0};
+        for (int r = 0; r < 3; ++r)
+            for (int col = 0; col < 3; ++col)
+                g->rot[9 * k + 3 * r + col] = (Rz[3 * r] * M[col] + Rz[3 * r + 1] * M[4 + col]) + Rz[3 * r + 2] * M[8 + col];
+    }
+    g->xs.resize(nx);
+    g->ys.resize(ny);
+    for (size_t i = 0; i < nx; ++i) g->xs[i] = M[3] + static_cast<double>(static_cast<long long>(i) - s->half_cells_x) * s->step;
+    for (size_t j = 0; j < ny; ++j) g->ys[j] = M[7] + static_cast<double>(static_cast<long long>(j) - s->half_cells_y) * s->step;
+    g->tz = M[11];
+    return KB_OK;
+}
+// the peaks of the scores (a neighbour at +-1 in i, j and k beats h with a higher score, or the same score and a smaller
+// index; k wraps on a full circle), by (score descending, h ascending)
+static std::vector<int> reloc_peaks(const RelocGrid &g, const std::vector<int> &sc) {
+    std::vector<int> peaks;
+    for (int k = 0; k < g.n_yaw; ++k)
+        for (int j = 0; j < g.ny; ++j)
+            for (int i = 0; i < g.nx; ++i) {
+                const int h = (k * g.ny + j) * g.nx + i, s = sc[h];
+                bool peak = true;
+                for (int dk = -1; dk <= 1 && peak; ++dk) {
+                    int k2 = k + dk;
+                    if (k2 < 0 || k2 >= g.n_yaw) {
+                        if (!g.full_circle) continue;
+                        k2 = (k2 + g.n_yaw) % g.n_yaw;
+                    }
+                    for (int j2 = std::max(j - 1, 0); j2 <= std::min(j + 1, g.ny - 1) && peak; ++j2)
+                        for (int i2 = std::max(i - 1, 0); i2 <= std::min(i + 1, g.nx - 1); ++i2) {
+                            const int h2 = (k2 * g.ny + j2) * g.nx + i2;  // (h itself, also through a wrap, never beats h)
+                            if (sc[h2] > s || (sc[h2] == s && h2 < h)) {
+                                peak = false;
+                                break;
+                            }
+                        }
+                }
+                if (peak) peaks.push_back(h);
+            }
+    std::sort(peaks.begin(), peaks.end(), [&](int a, int b) { return sc[a] != sc[b] ? sc[a] > sc[b] : a < b; });
+    return peaks;
+}
+// refined candidate b is distinct from the winner a: farther than 2 step in xy or 2 yaw_step in rotation angle
+static bool reloc_distinct(const double *A, const double *B, const kb_reloc_search &s) {
+    double tr = 0.0;  // trace(R_A^T R_B)
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) tr += A[4 * r + c] * B[4 * r + c];
+    const double angle = std::acos(std::max(-1.0, std::min(1.0, (tr - 1.0) / 2.0)));
+    return std::hypot(A[3] - B[3], A[7] - B[7]) > 2.0 * s.step || angle > 2.0 * s.yaw_step;
+}
+
+int kb_reloc_hypotheses(const kb_reloc_search *search, double *poses, size_t cap, size_t *n_out) {
+    if (!search || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RelocGrid g;
+    RET(reloc_grid(search, &g));
+    *n_out = g.H;
+    if (!poses || cap == 0) return KB_OK;
+    if (cap < g.H) return fail(KB_ERR_CAPACITY, "poses buffer too small (%zu < %zu hypotheses)", cap, g.H);
+    for (size_t h = 0; h < g.H; ++h) g.pose(h, poses + 16 * h);
+    return KB_OK;
+}
+
+int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_map *cmap, const kb_reloc_search *search,
+                  kb_reloc_result *out, double *candidates, int *candidate_scores, int *scores) {
+    kb_map *map = const_cast<kb_map *>(cmap);
+    if (!search || !out || !xyz) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n == 0) return fail(KB_ERR_INVALID_ARG, "empty source");
+    RelocGrid g;
+    RET(reloc_grid(search, &g));
+    if (n > static_cast<size_t>(INT_MAX) || n * static_cast<size_t>(search->top_k) > static_cast<size_t>(INT_MAX))
+        return fail(KB_ERR_INVALID_ARG, "%zu source points x top_k %d refinements exceed 2^31 - 1 points", n, search->top_k);
+    if (device_count() <= 0) return fail(KB_ERR_NO_DEVICE, "no CUDA device visible (this library has no CPU fallback)");
+    if (!reg || !map) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    // every voxel coordinate must fit in an int: |(R_h p + t_h)_c| <= |p| (1 + 1e-6: R within SE(3)'s tolerance) + |t_h|_max
+    double pmax = 0.0;
+    for (size_t i = 0; i < n; ++i) {
+        const double r = std::sqrt(xyz[3 * i] * xyz[3 * i] + xyz[3 * i + 1] * xyz[3 * i + 1] + xyz[3 * i + 2] * xyz[3 * i + 2]);
+        if (!std::isfinite(r)) return fail(KB_ERR_INVALID_ARG, "source point %zu is not finite", i);
+        pmax = std::max(pmax, r);
+    }
+    const double tmax = std::max({std::fabs(g.xs.front()), std::fabs(g.xs.back()), std::fabs(g.ys.front()),
+                                  std::fabs(g.ys.back()), std::fabs(g.tz)});
+    const double reach = (pmax * (1.0 + 1e-6) + tmax) / map->voxel_size + 1.0;
+    if (!(reach < 2147483000.0))
+        return fail(KB_ERR_INVALID_ARG, "a hypothesis maps source points to voxel coordinates beyond the int range (%.3g)", reach);
+    Exec &ex = *map->ex;
+    CK(cudaSetDevice(ex.device));
+    int live = 0;  // (the host's copy of the counters can be behind a pipeline's map)
+    CK(cudaMemcpyAsync(&live, map->cur.counters + C_LIVE, sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
+    RET(ex.sync());
+    if (live == 0) return fail(KB_ERR_INVALID_ARG, "the map is empty");
+
+    // 1. the coarse score of every hypothesis (k_reloc_score, relocalize.cu)
+    std::vector<double> grid(g.rot);
+    grid.insert(grid.end(), g.xs.begin(), g.xs.end());
+    grid.insert(grid.end(), g.ys.begin(), g.ys.end());
+    RET(reg->ws.src.ensure(3 * n));
+    RET(reg->rgrid.ensure(grid.size()));
+    RET(reg->rscore.ensure(g.H));
+    if (reg->rev_device != ex.device) {
+        for (cudaEvent_t &e : reg->rev) {
+            if (e) cudaEventDestroy(e);
+            e = nullptr;
+        }
+        CK(cudaEventCreate(&reg->rev[0]));
+        CK(cudaEventCreate(&reg->rev[1]));
+        reg->rev_device = ex.device;
+    }
+    CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
+    CK(cudaMemcpyAsync(reg->rgrid.p, grid.data(), grid.size() * sizeof(double), cudaMemcpyHostToDevice, ex.stream));
+    const MapView mv = map->view();
+    const double *d_rot = reg->rgrid.p, *d_xs = d_rot + g.rot.size(), *d_ys = d_xs + g.nx;
+    CK(cudaEventRecord(reg->rev[0], ex.stream));
+    CK(reloc_score(&mv, sizeof(mv), reg->ws.src.p, static_cast<int>(n), d_rot, g.n_yaw, d_xs, g.nx, d_ys, g.ny, g.tz,
+                   reg->rscore.p, ex.sms, ex.stream));
+    ++ex.launches;
+    CK(cudaEventRecord(reg->rev[1], ex.stream));
+    std::vector<int> sc(g.H);
+    CK(cudaMemcpyAsync(sc.data(), reg->rscore.p, g.H * sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
+    RET(ex.sync());
+
+    // 2-3. peaks and candidates
+    const std::vector<int> peaks = reloc_peaks(g, sc);
+    const size_t K = std::min(peaks.size(), static_cast<size_t>(search->top_k));
+    std::vector<double> cand(16 * K);
+    std::vector<SE3> guesses(K);
+    for (size_t c = 0; c < K; ++c) {
+        g.pose(static_cast<size_t>(peaks[c]), &cand[16 * c]);
+        if (!to_se3(&cand[16 * c], &guesses[c])) return fail(KB_ERR_NOT_SE3, "candidate %zu is not in SE(3)", c);
+    }
+
+    // 4. refinement: align_batch of the source from every candidate, inliers on
+    const std::vector<size_t> off(K, 0), cnt(K, n);
+    const std::vector<double> md(K, search->max_correspondence_distance), ks(K, search->kernel_scale);
+    RET(reg->bpose.ensure(16 * K));
+    RET(reg->biout.ensure(2 * K));
+    RET(align_batch_run(reg, map, reg->ws.src.p, off.data(), cnt.data(), K, guesses, md.data(), ks.data(), reg->bpose.p,
+                        reg->biout.p, reg->biout.p + K));
+    std::vector<double> refined(16 * K);
+    std::vector<int> io(2 * K);  // iterations [K], inliers [K]
+    CK(cudaMemcpyAsync(refined.data(), reg->bpose.p, 16 * K * sizeof(double), cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(io.data(), reg->biout.p, 2 * K * sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
+    RET(ex.sync());
+
+    // 5. winner and runner-up
+    size_t w = 0;
+    for (size_t c = 1; c < K; ++c)
+        if (io[K + c] > io[K + w]) w = c;
+    long long ru = -1;
+    for (size_t c = 0; c < K; ++c)
+        if (c != w && (ru < 0 || io[K + c] > io[K + ru]) && reloc_distinct(&refined[16 * w], &refined[16 * c], *search))
+            ru = static_cast<long long>(c);
+    kb_reloc_result r{};
+    std::memcpy(r.pose, &refined[16 * w], sizeof(r.pose));
+    r.inliers = io[K + w];
+    r.iterations = io[w];
+    r.rank = static_cast<int>(w);
+    r.n_source = static_cast<int>(n);
+    r.n_hypotheses = static_cast<int>(g.H);
+    r.n_peaks = static_cast<int>(peaks.size());
+    r.n_candidates = static_cast<int>(K);
+    r.runner_up_inliers = -1;
+    if (ru >= 0) {
+        std::memcpy(r.runner_up_pose, &refined[16 * ru], sizeof(r.runner_up_pose));
+        r.runner_up_inliers = io[K + ru];
+    }
+    *out = r;
+    if (candidates) std::memcpy(candidates, cand.data(), cand.size() * sizeof(double));
+    if (candidate_scores)
+        for (size_t c = 0; c < K; ++c) candidate_scores[c] = sc[peaks[c]];
+    if (scores) std::memcpy(scores, sc.data(), g.H * sizeof(int));
+    return KB_OK;
 }
 
 // ------------------------------------------------------------------------------- Preprocessor
@@ -2248,6 +2475,13 @@ static int probe_map_doubles(const double *in, size_t n, int k_in, double *out, 
 }
 int kb_debug_se3_exp_dev(const double *tangents, size_t n, double *out) { return probe_map_doubles(tangents, n, 6, out, 14, probe_se3_exp); }
 int kb_debug_fast_rcp_dev(const double *x, size_t n, double *out) { return probe_map_doubles(x, n, 1, out, 1, probe_fast_rcp); }
+int kb_debug_reloc_score_ms(const kb_registration *reg, float *ms) {
+    if (!reg || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (reg->rev_device < 0) return fail(KB_ERR_INVALID_ARG, "no kb_relocalize call on this handle yet");
+    CK(cudaSetDevice(reg->rev_device));
+    CK(cudaEventElapsedTime(ms, reg->rev[0], reg->rev[1]));
+    return KB_OK;
+}
 int kb_debug_barrier_ns(int iters, double *ns_per_barrier) {
     if (!ns_per_barrier || iters < 1) return fail(KB_ERR_INVALID_ARG, "bad argument");
     DefaultCtx *c;

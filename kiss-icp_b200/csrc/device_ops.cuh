@@ -202,7 +202,7 @@ struct Grid {
         __syncthreads();
         if (threadIdx.x == 0) {
             target += static_cast<unsigned>(size);
-            unsigned old;  // release our writes / acquire everybody else's
+            [[maybe_unused]] unsigned old;  // release our writes / acquire everybody else's
             asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], 1;" : "=r"(old) : "l"(bar) : "memory");
             unsigned spins = 0;
             unsigned seen;
@@ -268,11 +268,13 @@ __device__ __forceinline__ int4 cas_slot(int4 *addr, int4 expected, int4 desired
     return o;
 }
 
-// lookup: slot index of voxel (x,y,z) or -1; *cnt = its point count
+// lookup: slot index of voxel (x,y,z) or -1; *cnt = its point count. READ_ONLY reads the slots through the read-only
+// (non-coherent) path: only for kernels during which nothing writes the table (k_reloc_score).
+template <bool READ_ONLY = false>
 __device__ __forceinline__ int map_find(const MapView &m, int x, int y, int z, int *cnt) {
     unsigned h = mix_hash(x, y, z) & m.mask;
     for (unsigned probes = 0; probes <= m.mask; ++probes) {
-        const int4 s = m.slots[h];
+        const int4 s = READ_ONLY ? __ldg(&m.slots[h]) : m.slots[h];
         if (s.w == KB_EMPTY) return -1;
         if (s.w != KB_TOMB && s.x == x && s.y == y && s.z == z) {
             *cnt = s.w;

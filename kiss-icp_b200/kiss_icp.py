@@ -16,6 +16,7 @@ VoxelHashMap with a large max_distance and ``vmap.update(frame_downsample, pose)
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import math
 from collections import namedtuple
 
@@ -24,8 +25,9 @@ import numpy as np
 from . import _native as N
 from .config import KISSConfig, load_config
 from .mapping import VoxelHashMap, check_value, get_voxel_hash_map
-from .preprocess import get_preprocessor
+from .preprocess import Preprocessor, get_preprocessor
 from .registration import get_registration
+from .relocalization import RelocalizationResult, RelocalizationSearch
 from .threshold import AdaptiveThreshold, get_threshold_estimator
 from .voxelization import voxel_down_sample
 
@@ -354,6 +356,35 @@ class KissICP:
         _, d = self.local_map.closest_neighbors(mapped)
         near = d < 3 * sigma
         return _fit_of(n, len(source), float(np.sum(d[near] ** 2)), JTJ)
+
+    # -- relocalization ------------------------------------------------------------------------------
+    def relocalize(self, frame, search: RelocalizationSearch) -> RelocalizationResult:
+        """Find the localizer's pose in its prior map from one scan, without a pose to start from (at power-up, or
+        after the track was lost), and continue the track from there.
+
+        The scan's source is built as register_frame builds it, but without deskewing (there is no motion to deskew
+        with): preprocessing, then the 0.5 voxel_size and 1.5 voxel_size downsamples. Registration.relocalize searches
+        ``search`` with the refinement thresholds of the pipeline's current sigma (3 sigma, sigma): they override the
+        search's max_correspondence_distance and kernel_scale. Then last_pose is the winner and last_delta the
+        identity; the adaptive threshold's state is unchanged. Returns the RelocalizationResult; accepting it (for
+        example by its inliers against n_source and against the runner-up's) is the caller's decision."""
+        if not self.localizer:
+            raise ValueError("relocalization needs a prior map: KissICP(config, prior_map=...)")
+        if not isinstance(search, RelocalizationSearch):
+            raise TypeError(f"search must be a RelocalizationSearch, not {type(search).__name__}")
+        if getattr(self, "_reloc", None) is None:
+            c = self.config
+            self._reloc = (Preprocessor(c.data.max_range, c.data.min_range, False, c.registration.max_num_threads),
+                           self.registration if not self.fused else get_registration(c))
+        pre, reg = self._reloc
+        frame = pre.preprocess(frame, np.empty(0), np.eye(4))
+        source, _ = self.voxelize(frame)
+        sigma = self._sigma_next() if self.fused else self.adaptive_threshold.get_threshold()
+        result = reg.relocalize(source, self.local_map,
+                                dataclasses.replace(search, max_correspondence_distance=3 * sigma, kernel_scale=sigma))
+        self.last_pose = result.pose
+        self.last_delta = np.eye(4)
+        return result
 
     # -- checkpoint / restore -----------------------------------------------------------------------
     def state_dict(self):

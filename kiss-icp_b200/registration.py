@@ -9,6 +9,7 @@ import numpy as np
 from . import _native as N
 from .config import KISSConfig
 from .mapping import VoxelHashMap
+from .relocalization import RelocalizationResult, RelocalizationSearch, relocalize
 
 
 def _torch_if_cuda(x):
@@ -151,6 +152,15 @@ class Registration:
             p(inl) if inl is not None else None))
         N.check(N.lib().kb_map_sync(voxel_map._h))
         return (poses, iters, inl) if return_inliers else (poses, iters)
+
+    def relocalize(self, source, voxel_map: VoxelHashMap, search: RelocalizationSearch,
+                   return_scores: bool = False) -> RelocalizationResult:
+        """Find the pose of ``source`` (N, 3) in ``voxel_map`` without an initial pose: score every hypothesis of
+        ``search`` on the device, refine its top_k peaks with align_points_to_map_batch (bit for bit that call's
+        poses, iterations and inliers) and return the candidate with the most inliers, with the runner-up and, with
+        return_scores, the (n_yaw, Ny, Nx) coarse scores. Only reads the map. Accepting the result is the caller's
+        decision. kb_relocalize in include/kiss_icp_b200.h states every rule."""
+        return relocalize(self._h, source, voxel_map, search, return_scores)
 
     @property
     def last_iterations(self) -> int:
