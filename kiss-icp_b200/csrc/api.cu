@@ -20,6 +20,7 @@
 #include <mutex>
 #include <numeric>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/kiss_icp_b200.h"
@@ -65,6 +66,9 @@ int device_count() {
         return 0;
     }
     return n;
+}
+int require_device() {
+    return device_count() > 0 ? KB_OK : fail(KB_ERR_NO_DEVICE, "no CUDA device visible (this library has no CPU fallback)");
 }
 
 // the device watchdog's report (device_ops.cuh): mapped host words per device, checked after every synchronisation
@@ -123,7 +127,7 @@ bool g_stuck[64];
 void device_stuck(int device) {
     if (device >= 0 && device < 64) g_stuck[device] = true;
 }
-// a launch on this device never ended: cudaFree & co. would block forever, so the destructors leak instead
+// a launch on this device (-1: any device) never ended
 bool device_is_stuck(int device) {
     if (device < 0) {
         for (bool b : g_stuck)
@@ -149,26 +153,85 @@ std::string phase_marks(int device) {
     return out;  // (the side stream is leaked with the rest of the stuck context)
 }
 
-template <class T>
-struct DBuf {
-    T *p = nullptr;
-    size_t n = 0;
-    int ensure(size_t count) {
-        if (count <= n) return KB_OK;
-        if (p) cudaFree(p);
-        p = nullptr;
-        n = 0;
-        // grow with 25% headroom: scan sizes jitter from frame to frame and a cudaFree/cudaMalloc
-        // pair per new maximum would put milliseconds of allocator time on the hot path
-        const size_t want = std::max<size_t>(count + count / 4, 1024);
-        CK(cudaMalloc(&p, want * sizeof(T)));
-        n = want;
-        return KB_OK;
+// Owner of one CUDA resource: device or pinned memory, an event, a stream. It records the device the resource was
+// created on and releases it when it goes, unless a launch on that device never ended: cudaFree & co. would block
+// forever then, so the resource is leaked with the stuck context. (The release calls find the resource's device from
+// the handle: they do not depend on the current device.)
+template <class H, cudaError_t (*Release)(H)>
+struct Owned {
+    H p = nullptr;
+    int device = -1;  // where p was created
+    Owned() = default;
+    Owned(Owned &&o) noexcept { *this = std::move(o); }
+    Owned &operator=(Owned &&o) noexcept {  // (o releases what this owned)
+        std::swap(p, o.p);
+        std::swap(device, o.device);
+        return *this;
     }
-    ~DBuf() {
-        if (p && !device_is_stuck(-1)) cudaFree(p);  // (-1: any device)
+    ~Owned() {
+        if (p && !device_is_stuck(device)) Release(p);
+    }
+
+  protected:
+    // release what this owns, then own what create(&handle) makes on the current device (nothing when it fails)
+    template <class Create>
+    cudaError_t make(Create create) {
+        *this = Owned{};
+        const cudaError_t e = create(&p);
+        if (e == cudaSuccess)
+            cudaGetDevice(&device);
+        else
+            p = nullptr;
+        return e;
     }
 };
+struct Event : Owned<cudaEvent_t, cudaEventDestroy> {
+    cudaError_t create(unsigned flags) { return make([&](cudaEvent_t *e) { return cudaEventCreateWithFlags(e, flags); }); }
+};
+struct Stream : Owned<cudaStream_t, cudaStreamDestroy> {
+    cudaError_t create() { return make([](cudaStream_t *s) { return cudaStreamCreateWithFlags(s, cudaStreamNonBlocking); }); }
+};
+
+template <class T>
+cudaError_t free_device(T *p) { return cudaFree(p); }
+template <class T>
+cudaError_t free_pinned(T *p) { return cudaFreeHost(p); }
+
+// an array of n T in device memory, or in pinned host memory (Pinned)
+template <class T, bool Pinned>
+struct Buffer : Owned<T *, Pinned ? &free_pinned<T> : &free_device<T>> {
+    size_t n = 0;
+    Buffer() = default;
+    Buffer(Buffer &&o) noexcept { *this = std::move(o); }
+    Buffer &operator=(Buffer &&o) noexcept {
+        Buffer::Owned::operator=(std::move(o));
+        std::swap(n, o.n);
+        return *this;
+    }
+    // exactly `count` elements; what the buffer held is released first
+    cudaError_t alloc(size_t count) {
+        const cudaError_t e = this->make([&](T **q) {
+            return Pinned ? cudaHostAlloc(q, count * sizeof(T), cudaHostAllocDefault) : cudaMalloc(q, count * sizeof(T));
+        });
+        n = e == cudaSuccess ? count : 0;
+        return e;
+    }
+    // at least `count` elements. Grown with 25% headroom: scan sizes jitter from frame to frame and a
+    // cudaFree/cudaMalloc pair per new maximum would put milliseconds of allocator time on the hot path
+    int ensure(size_t count) {
+        if (count <= n) return KB_OK;
+        const size_t want = std::max<size_t>(count + count / 4, 1024);
+        const cudaError_t e = alloc(want);
+        if (e != cudaSuccess)
+            return fail(KB_ERR_CUDA, "%s of %zu bytes failed: %s", Pinned ? "cudaHostAlloc" : "cudaMalloc", want * sizeof(T),
+                        cudaGetErrorString(e));
+        return KB_OK;
+    }
+};
+template <class T>
+using DBuf = Buffer<T, false>;
+template <class T>
+using PinBuf = Buffer<T, true>;
 
 // KB_TRACE_STALLS=<ms>: report host-side API calls of the frame paths that block longer than <ms> (diagnostic)
 struct StallTrace {
@@ -202,7 +265,7 @@ size_t pow2_at_least(size_t v) {
 struct Exec {
     int device = 0;
     cudaStream_t stream = nullptr;
-    bool own_stream = false;
+    Stream own_stream;  // (none when the calling thread set a stream: kb_set_stream)
     int grid = 0;
     int sms = 0;  // multiprocessors of the device
     Scratch sc{};  // all pointers null, profiling off
@@ -221,17 +284,28 @@ struct Exec {
         return first << 13;
     }
     DBuf<uint4> batch_ll;  // all-gather regions of k_icp_batch's slots (allocated by the first batch call)
+    std::vector<DBuf<char>> scratch_mem;  // what sc and team point to
 
+    // `view` = a scratch array of `count` elements that lives as long as this context, zeroed on its stream when `zero`
+    template <class T>
+    int scratch(T *&view, size_t count, bool zero) {
+        DBuf<char> b;
+        CK(b.alloc(count * sizeof(T)));
+        if (zero) CK(cudaMemsetAsync(b.p, 0, count * sizeof(T), stream));
+        view = reinterpret_cast<T *>(b.p);
+        scratch_mem.push_back(std::move(b));
+        return KB_OK;
+    }
     int init() {
-        if (device_count() <= 0) return fail(KB_ERR_NO_DEVICE, "no CUDA device visible (this library has no CPU fallback)");
+        RET(require_device());
         device = tl_device;
         CK(cudaSetDevice(device));
         RET(watchdog_init(device));
         if (tl_user_stream) {
             stream = tl_user_stream;
         } else {
-            CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-            own_stream = true;
+            CK(own_stream.create());
+            stream = own_stream.p;
         }
         int coop = 0;
         CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
@@ -239,40 +313,21 @@ struct Exec {
         if (!coop) return fail(KB_ERR_CUDA, "device does not support cooperative launch");
         grid = tl_grid_blocks > 0 ? std::min(tl_grid_blocks, sms) : sms;
         grid = std::min(grid, 256);  // the two-level gather tree of the ICP loop handles up to 16 x 16 CTAs
-        CK(cudaMalloc(&sc.bar, BAR_WORDS * sizeof(unsigned)));
-        CK(cudaMemsetAsync(sc.bar, 0, BAR_WORDS * sizeof(unsigned), stream));
-        CK(cudaMalloc(&sc.blk_d, sizeof(double) * 2 * grid * NPART));
-        CK(cudaMalloc(&sc.blk_i, sizeof(int) * 2 * grid));
-        CK(cudaMalloc(&sc.ll_part, sizeof(uint4) * NPART * grid));
-        CK(cudaMalloc(&sc.ll_res, sizeof(uint4) * LL_RES));
-        CK(cudaMalloc(&sc.ll_group, sizeof(uint4) * NPART * 16));
-        CK(cudaMemsetAsync(sc.ll_group, 0, sizeof(uint4) * NPART * 16, stream));
-        CK(cudaMemsetAsync(sc.ll_part, 0, sizeof(uint4) * NPART * grid, stream));
-        CK(cudaMemsetAsync(sc.ll_res, 0, sizeof(uint4) * LL_RES, stream));
-        CK(cudaMalloc(&team.ll, sizeof(uint4) * 2 * NPART * TEAM_MAX * TEAM_MAX));  // 11 MB: one copy of the partials per reader
-        CK(cudaMemsetAsync(team.ll, 0, sizeof(uint4) * 2 * NPART * TEAM_MAX * TEAM_MAX, stream));
-        CK(cudaMalloc(&team.out, sizeof(double) * 16));
+        RET(scratch(sc.bar, BAR_WORDS, true));
+        RET(scratch(sc.blk_d, 2 * grid * NPART, false));
+        RET(scratch(sc.blk_i, 2 * grid, false));
+        RET(scratch(sc.ll_part, NPART * grid, true));
+        RET(scratch(sc.ll_res, LL_RES, true));
+        RET(scratch(sc.ll_group, NPART * 16, true));
+        RET(scratch(team.ll, 2 * NPART * TEAM_MAX * TEAM_MAX, true));  // 11 MB: one copy of the partials per reader
+        RET(scratch(team.out, 16, false));
+        RET(scratch(sc.dbg, 64 + 4 * grid, true));
         if (const char *e = std::getenv("KB_ICP_TEAM_Q")) icp_team_q = std::max(0, std::min(std::atoi(e), TQ_MAX));
         if (const char *e = std::getenv("KB_ICP_SMEM_KB")) icp_smem = static_cast<size_t>(std::max(60, std::min(std::atoi(e), 180))) * 1024;
         team.smem_bytes = static_cast<int>(icp_smem);
         team.radius_frac = 0.2;
         if (const char *e = std::getenv("KB_ICP_RADIUS")) team.radius_frac = std::max(0.01, std::min(std::atof(e), 0.45));
-        CK(cudaMalloc(&sc.dbg, sizeof(unsigned long long) * (64 + 4 * grid)));
-        CK(cudaMemsetAsync(sc.dbg, 0, sizeof(unsigned long long) * (64 + 4 * grid), stream));
         return KB_OK;
-    }
-    ~Exec() {
-        if (device_is_stuck(device)) return;
-        if (sc.bar) cudaFree(sc.bar);
-        if (sc.blk_d) cudaFree(sc.blk_d);
-        if (sc.blk_i) cudaFree(sc.blk_i);
-        if (sc.ll_part) cudaFree(sc.ll_part);
-        if (sc.ll_res) cudaFree(sc.ll_res);
-        if (sc.ll_group) cudaFree(sc.ll_group);
-        if (sc.dbg) cudaFree(sc.dbg);
-        if (team.ll) cudaFree(team.ll);
-        if (team.out) cudaFree(team.out);
-        if (own_stream && stream) cudaStreamDestroy(stream);
     }
     // opt in to > 48 KB of dynamic shared memory, once per kernel AND device (the attribute is per device)
     int opt_in_smem(const void *k, size_t bytes) {
@@ -401,17 +456,15 @@ struct Work {
     }
 };
 
-bool to_se3(const double M[16], SE3 *T) { return se3_from_matrix(M, T); }
-
 }  // namespace
 
 // =============================================================================================
 struct kb_map {
     struct Table {
         size_t capacity = 0;
-        int4 *slots = nullptr;
-        double *points = nullptr;
-        int *head = nullptr, *pcount = nullptr, *pending = nullptr, *counters = nullptr;
+        DBuf<int4> slots;
+        DBuf<double> points;
+        DBuf<int> head, pcount, pending, counters;
     };
     std::shared_ptr<Exec> ex;
     double voxel_size, max_distance;
@@ -432,12 +485,12 @@ struct kb_map {
 
     MapView view_of(const Table &t) const {
         MapView m;
-        m.slots = t.slots;
-        m.points = t.points;
-        m.head = t.head;
-        m.pcount = t.pcount;
-        m.pending = t.pending;
-        m.counters = t.counters;
+        m.slots = t.slots.p;
+        m.points = t.points.p;
+        m.head = t.head.p;
+        m.pcount = t.pcount.p;
+        m.pending = t.pending.p;
+        m.counters = t.counters.p;
         m.mask = static_cast<unsigned>(t.capacity - 1);
         m.cap = static_cast<int>(cap);
         m.voxel_size = voxel_size;
@@ -447,53 +500,36 @@ struct kb_map {
         return m;
     }
     MapView view() const { return view_of(cur); }
-    static void free_table(Table &t) {
-        if (t.slots) cudaFree(t.slots);
-        if (t.points) cudaFree(t.points);
-        if (t.head) cudaFree(t.head);
-        if (t.pcount) cudaFree(t.pcount);
-        if (t.pending) cudaFree(t.pending);
-        if (t.counters) cudaFree(t.counters);
-        t = Table{};
-    }
-    ~kb_map() {
-        if (ex && device_is_stuck(ex->device)) return;
-        if (ex) cudaSetDevice(ex->device);
-        free_table(cur);
-        free_table(spare);
-    }
     // every slot empty, every counter zero (enqueued on the map's stream)
     int reset_table(const Table &t) {
-        k_map_fill<<<std::min<size_t>(4096, (t.capacity + 255) / 256), 256, 0, ex->stream>>>(t.slots, t.head, t.pcount, t.capacity);
+        k_map_fill<<<std::min<size_t>(4096, (t.capacity + 255) / 256), 256, 0, ex->stream>>>(t.slots.p, t.head.p, t.pcount.p, t.capacity);
         ++ex->launches;
         CK(cudaGetLastError());
-        CK(cudaMemsetAsync(t.counters, 0, sizeof(int) * C_NCOUNTERS, ex->stream));
+        CK(cudaMemsetAsync(t.counters.p, 0, sizeof(int) * C_NCOUNTERS, ex->stream));
         return KB_OK;
     }
-    // an empty table of cap_slots slots: the spare if it has that size, else a fresh allocation
+    // an empty table of cap_slots slots: the spare if it has that size, else a fresh allocation (the spare is released)
     int take_table(size_t cap_slots, Table *out) {
         Table t;
         if (spare.capacity == cap_slots) {
-            t = spare;
-            spare = Table{};
+            t = std::exchange(spare, Table{});
         } else {
-            free_table(spare);
+            spare = Table{};
             t.capacity = cap_slots;
-            auto bail = [&](cudaError_t e) {
-                free_table(t);
-                return fail(KB_ERR_CUDA, "voxel table allocation (%zu slots): %s", cap_slots, cudaGetErrorString(e));
-            };
             cudaError_t e;
-            if ((e = cudaMalloc(&t.slots, cap_slots * sizeof(int4))) != cudaSuccess) return bail(e);
-            if ((e = cudaMalloc(&t.points, cap_slots * cap * 3 * sizeof(double))) != cudaSuccess) return bail(e);
-            if ((e = cudaMalloc(&t.head, cap_slots * sizeof(int))) != cudaSuccess) return bail(e);
-            if ((e = cudaMalloc(&t.pcount, cap_slots * sizeof(int))) != cudaSuccess) return bail(e);
-            if ((e = cudaMalloc(&t.pending, cap_slots * PEND * sizeof(int))) != cudaSuccess) return bail(e);
-            if ((e = cudaMalloc(&t.counters, sizeof(int) * C_NCOUNTERS)) != cudaSuccess) return bail(e);
+            if ((e = t.slots.alloc(cap_slots)) != cudaSuccess || (e = t.points.alloc(cap_slots * cap * 3)) != cudaSuccess ||
+                (e = t.head.alloc(cap_slots)) != cudaSuccess || (e = t.pcount.alloc(cap_slots)) != cudaSuccess ||
+                (e = t.pending.alloc(cap_slots * PEND)) != cudaSuccess || (e = t.counters.alloc(C_NCOUNTERS)) != cudaSuccess)
+                return fail(KB_ERR_CUDA, "voxel table allocation (%zu slots): %s", cap_slots, cudaGetErrorString(e));
         }
         RET(reset_table(t));
-        *out = t;
+        *out = std::move(t);
         return KB_OK;
+    }
+    // the live-voxel count on the device (the host's copy of the counters can be behind a pipeline's map)
+    int pull_live(int *live) {
+        CK(cudaMemcpyAsync(live, cur.counters.p + C_LIVE, sizeof(int), cudaMemcpyDeviceToHost, ex->stream));
+        return ex->sync();
     }
     // make room for `extra` more voxels at load factor <= 0.5 (tombstones count as load)
     bool would_grow(size_t extra) const {  // ensure_capacity(extra) would rebuild the table (needs an idle stream)
@@ -520,14 +556,12 @@ struct kb_map {
             k_map_rehash<<<std::min<size_t>(2048, (cur.capacity * 32 + 255) / 256), 256, 0, ex->stream>>>(view(), view_of(nt));
             ++ex->launches;
             CK(cudaGetLastError());
-            CK(cudaMemcpyAsync(h_counters, nt.counters, sizeof(int) * C_NCOUNTERS, cudaMemcpyDeviceToHost, ex->stream));
+            CK(cudaMemcpyAsync(h_counters, nt.counters.p, sizeof(int) * C_NCOUNTERS, cudaMemcpyDeviceToHost, ex->stream));
             RET(ex->sync());
         } else {
             std::memset(h_counters, 0, sizeof(h_counters));
         }
-        free_table(spare);  // (empty unless take_table allocated)
-        spare = cur;        // stays allocated: the next same-size rebuild moves back into it
-        cur = nt;
+        spare = std::exchange(cur, std::move(nt));  // stays allocated: the next same-size rebuild moves back into it
         return KB_OK;
     }
     // allocate the table AND its spare for `slots` slots now (pipeline creation), so that neither growth nor the
@@ -535,15 +569,11 @@ struct kb_map {
     int reserve(size_t slots) {
         slots = pow2_at_least(slots);
         if (slots > cur.capacity) RET(ensure_capacity(0, slots));
-        if (spare.capacity != cur.capacity) {
-            Table t;
-            RET(take_table(cur.capacity, &t));  // frees a spare of another size
-            spare = t;
-        }
+        if (spare.capacity != cur.capacity) RET(take_table(cur.capacity, &spare));  // releases the spare of another size first
         return KB_OK;
     }
     int pull_counters() {
-        CK(cudaMemcpyAsync(h_counters, cur.counters, sizeof(int) * C_NCOUNTERS, cudaMemcpyDeviceToHost, ex->stream));
+        CK(cudaMemcpyAsync(h_counters, cur.counters.p, sizeof(int) * C_NCOUNTERS, cudaMemcpyDeviceToHost, ex->stream));
         RET(ex->sync());
         if (h_counters[C_STATUS] & ST_TABLE_FULL) return fail(KB_ERR_CUDA, "voxel table overflow (internal capacity bug)");
         return KB_OK;
@@ -555,14 +585,14 @@ struct kb_map {
         const size_t want = std::max<size_t>({cur.capacity, pow2_at_least(3 * nv), size_t(1) << 14});
         if (want > (size_t(1) << 31)) return fail(KB_ERR_INVALID_ARG, "voxel table would exceed 2^31 slots");
         StallTrace trace("voxel map load");
-        // take_table frees a spare of another size: keep it aside so that a failed load can put it back
+        // take_table releases a spare of another size: keep it aside so that a failed load can put it back
         const bool from_spare = spare.capacity == want;
         Table keep;
         if (!from_spare) std::swap(keep, spare);
         Table nt;
         const int st = take_table(want, &nt);
         if (st != KB_OK) {
-            spare = keep;
+            spare = std::move(keep);
             return st;
         }
         int h[C_NCOUNTERS] = {0};
@@ -579,16 +609,11 @@ struct kb_map {
             ++ex->launches;
             CK(cudaGetLastError());
         }
-        CK(cudaMemcpyAsync(h, nt.counters, sizeof(h), cudaMemcpyDeviceToHost, ex->stream));
+        CK(cudaMemcpyAsync(h, nt.counters.p, sizeof(h), cudaMemcpyDeviceToHost, ex->stream));
         RET(ex->sync());
         const int bad = h[C_STATUS];
         if (bad) {
-            if (from_spare) {
-                spare = nt;
-            } else {
-                free_table(nt);
-                spare = keep;
-            }
+            spare = std::move(from_spare ? nt : keep);
             if (bad & ST_TABLE_FULL) return fail(KB_ERR_CUDA, "voxel table overflow during load (internal capacity bug)");
             std::string why;
             if (bad & ST_LOAD_DUPLICATE) why += " a voxel appears twice;";
@@ -597,9 +622,7 @@ struct kb_map {
             if (bad & ST_LOAD_OUTSIDE) why += " a point lies outside its voxel;";
             return fail(KB_ERR_INVALID_ARG, "map load rejected, the map is unchanged:%s", why.c_str());
         }
-        free_table(keep);
-        spare = cur;
-        cur = nt;
+        spare = std::exchange(cur, std::move(nt));
         std::memcpy(h_counters, h, sizeof(h_counters));  // the host's grow decision and the kernel's veto read these
         return KB_OK;
     }
@@ -661,13 +684,7 @@ struct kb_registration {
     DBuf<int> biout;
     DBuf<double> rgrid;   // kb_relocalize: rotations [n_yaw][9], then xs [Nx], ys [Ny]
     DBuf<int> rscore;     // kb_relocalize: scores [H]
-    cudaEvent_t rev[2] = {nullptr, nullptr};  // around the last k_reloc_score (kb_debug_reloc_score_ms)
-    int rev_device = -1;
-    ~kb_registration() {
-        if (device_is_stuck(-1)) return;
-        for (cudaEvent_t e : rev)
-            if (e) cudaEventDestroy(e);
-    }
+    Event rev[2];  // around the last k_reloc_score (kb_debug_reloc_score_ms), on the device of that call
 };
 
 struct kb_preprocessor {
@@ -690,13 +707,13 @@ struct kb_pipeline {
     // also computes its fit, into fit_dev[0] (blocking calls) or fit_dev[1 + k % Q_DEPTH] (queued frame k)
     bool localizer = false;
     DBuf<double> fit_part;           // [FIT_VALS][grid] per-CTA partials of the fit pass
-    FitResult *fit_dev = nullptr;    // [1 + Q_DEPTH]
-    FitResult *fit_host = nullptr;   // [1 + Q_DEPTH] pinned copies
+    DBuf<FitResult> fit_dev;         // [1 + Q_DEPTH]
+    PinBuf<FitResult> fit_host;      // [1 + Q_DEPTH] copies
     FitResult last_fit{};
     Work ws;
-    PipeState *d_state = nullptr;
-    FrameResult *d_res = nullptr;
-    FrameResult *h_res = nullptr;  // pinned
+    DBuf<PipeState> d_state;
+    DBuf<FrameResult> d_res;
+    PinBuf<FrameResult> h_res;
     FrameResult last{};
     bool has_last = false;
     long long next_id = 0;  // id of the next frame to register (Workspace::fr[id & 1] holds its front end)
@@ -710,37 +727,15 @@ struct kb_pipeline {
     static constexpr int Q_DEPTH = 4;  // frame k registering, k+1 being prefetched by the same launch, k+2 / k+3 copying
     struct Slot {
         DBuf<double> in, ts;  // device copy of one queued frame
-        void *pin_xyz = nullptr, *pin_ts = nullptr;  // pinned staging, used only when the caller's memory is pageable
-        size_t pin_xyz_bytes = 0, pin_ts_bytes = 0;
-        cudaEvent_t copied = nullptr, done = nullptr, read = nullptr;
+        PinBuf<unsigned char> pin_xyz, pin_ts;  // staging, used only when the caller's memory is pageable
+        Event copied, done, read;
     };
     Slot q[Q_DEPTH];
-    cudaStream_t copy_stream = nullptr, res_stream = nullptr;
-    FrameResult *q_res = nullptr;      // [Q_DEPTH] pinned host copies of the frame results
-    FrameResult *q_res_dev = nullptr;  // [Q_DEPTH] device side: where the kernels write them
+    Stream copy_stream, res_stream;
+    PinBuf<FrameResult> q_res;    // [Q_DEPTH] host copies of the frame results
+    DBuf<FrameResult> q_res_dev;  // [Q_DEPTH] device side: where the kernels write them
     ~kb_pipeline() {
-        if (ex && device_is_stuck(ex->device)) {
-            map = nullptr;  // (leaked on purpose)
-            return;
-        }
-        if (ex) cudaSetDevice(ex->device);
-        for (Slot &s : q) {
-            if (s.pin_xyz) cudaFreeHost(s.pin_xyz);
-            if (s.pin_ts) cudaFreeHost(s.pin_ts);
-            if (s.copied) cudaEventDestroy(s.copied);
-            if (s.done) cudaEventDestroy(s.done);
-            if (s.read) cudaEventDestroy(s.read);
-        }
-        if (copy_stream) cudaStreamDestroy(copy_stream);
-        if (res_stream) cudaStreamDestroy(res_stream);
-        if (q_res_dev) cudaFree(q_res_dev);
-        if (q_res) cudaFreeHost(q_res);
-        if (fit_dev) cudaFree(fit_dev);
-        if (fit_host) cudaFreeHost(fit_host);
         if (!localizer) delete map;
-        if (d_state) cudaFree(d_state);
-        if (d_res) cudaFree(d_res);
-        if (h_res) cudaFreeHost(h_res);
     }
 };
 
@@ -853,7 +848,7 @@ int kb_map_update_pose(kb_map *map, const double *xyz, size_t n, const double po
     if (!map || (!xyz && n) || !pose) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     RET(map_in_use(map));
     SE3 T;
-    if (!to_se3(pose, &T)) return fail(KB_ERR_NOT_SE3, "pose is not in SE(3)");
+    if (!se3_from_matrix(pose, &T)) return fail(KB_ERR_NOT_SE3, "pose is not in SE(3)");
     return map->update_host(xyz, n, true, T, true, true, T.t);
 }
 int kb_map_add_points(kb_map *map, const double *xyz, size_t n) {
@@ -1103,7 +1098,7 @@ int kb_map_sync(const kb_map *map) {
 int kb_registration_create(int max_num_iterations, double convergence_criterion, int max_num_threads,
                            kb_registration **out) {
     if (!out) return fail(KB_ERR_INVALID_ARG, "out == NULL");
-    if (device_count() <= 0) return fail(KB_ERR_NO_DEVICE, "no CUDA device visible (this library has no CPU fallback)");
+    RET(require_device());
     if (max_num_iterations > 8000) return fail(KB_ERR_INVALID_ARG, "max_num_iterations > 8000 is not supported");
     auto r = new kb_registration();
     r->max_iter = max_num_iterations;
@@ -1164,7 +1159,7 @@ int kb_registration_align_points_to_map(kb_registration *reg, const double *xyz,
     kb_map *map = const_cast<kb_map *>(cmap);
     if (!reg || !map || (!xyz && n) || !initial_guess || !out_pose) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     SE3 g;
-    if (!to_se3(initial_guess, &g)) return fail(KB_ERR_NOT_SE3, "initial_guess is not in SE(3)");
+    if (!se3_from_matrix(initial_guess, &g)) return fail(KB_ERR_NOT_SE3, "initial_guess is not in SE(3)");
     RET(registration_run(reg, xyz, n, map, g, max_correspondence_distance, kernel_scale, false));
     int it = 0;
     CK(cudaMemcpyAsync(out_pose, reg->out.p, 16 * sizeof(double), cudaMemcpyDeviceToHost, map->ex->stream));
@@ -1216,7 +1211,7 @@ static int align_batch_check(const kb_registration *reg, const kb_map *map, cons
     }
     g->resize(B);
     for (size_t b = 0; b < B; ++b)
-        if (!to_se3(guesses + 16 * b, &(*g)[b])) return fail(KB_ERR_NOT_SE3, "initial_guesses[%zu] is not in SE(3)", b);
+        if (!se3_from_matrix(guesses + 16 * b, &(*g)[b])) return fail(KB_ERR_NOT_SE3, "initial_guesses[%zu] is not in SE(3)", b);
     return KB_OK;
 }
 static int align_batch_run(kb_registration *reg, kb_map *map, const double *d_xyz, const size_t *offset, const size_t *count,
@@ -1224,9 +1219,8 @@ static int align_batch_run(kb_registration *reg, kb_map *map, const double *d_xy
                            double *d_poses, int *d_iters, int *d_inliers) {
     Exec &ex = *map->ex;
     CK(cudaSetDevice(ex.device));
-    int live = 0;  // (the host's copy of the counters can be behind a pipeline's map)
-    CK(cudaMemcpyAsync(&live, map->cur.counters + C_LIVE, sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
-    RET(ex.sync());
+    int live = 0;
+    RET(map->pull_live(&live));
     const MapView mv = map->view();
     std::vector<BatchHyp> hyp;  // the team hypotheses, then all of them (inlier pass)
     std::vector<size_t> single;
@@ -1379,7 +1373,7 @@ static int reloc_grid(const kb_reloc_search *s, RelocGrid *g) {
         return fail(KB_ERR_INVALID_ARG, "more than 2^24 hypotheses (%zu x %zu positions x %d headings)", nx, ny, s->n_yaw);
     const double *M = s->center;
     SE3 c;
-    if (!to_se3(M, &c)) return fail(KB_ERR_NOT_SE3, "search center is not in SE(3)");
+    if (!se3_from_matrix(M, &c)) return fail(KB_ERR_NOT_SE3, "search center is not in SE(3)");
     if (!std::isfinite(M[3]) || !std::isfinite(M[7]) || !std::isfinite(M[11]))
         return fail(KB_ERR_INVALID_ARG, "search center has a non-finite translation");
     g->hx = s->half_cells_x;
@@ -1463,7 +1457,7 @@ int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_ma
     RET(reloc_grid(search, &g));
     if (n > static_cast<size_t>(INT_MAX) || n * static_cast<size_t>(search->top_k) > static_cast<size_t>(INT_MAX))
         return fail(KB_ERR_INVALID_ARG, "%zu source points x top_k %d refinements exceed 2^31 - 1 points", n, search->top_k);
-    if (device_count() <= 0) return fail(KB_ERR_NO_DEVICE, "no CUDA device visible (this library has no CPU fallback)");
+    RET(require_device());
     if (!reg || !map) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     // every voxel coordinate must fit in an int: |(R_h p + t_h)_c| <= |p| (1 + 1e-6: R within SE(3)'s tolerance) + |t_h|_max
     double pmax = 0.0;
@@ -1479,9 +1473,8 @@ int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_ma
         return fail(KB_ERR_INVALID_ARG, "a hypothesis maps source points to voxel coordinates beyond the int range (%.3g)", reach);
     Exec &ex = *map->ex;
     CK(cudaSetDevice(ex.device));
-    int live = 0;  // (the host's copy of the counters can be behind a pipeline's map)
-    CK(cudaMemcpyAsync(&live, map->cur.counters + C_LIVE, sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
-    RET(ex.sync());
+    int live = 0;
+    RET(map->pull_live(&live));
     if (live == 0) return fail(KB_ERR_INVALID_ARG, "the map is empty");
 
     // 1. the coarse score of every hypothesis (k_reloc_score, relocalize.cu)
@@ -1491,24 +1484,19 @@ int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_ma
     RET(reg->ws.src.ensure(3 * n));
     RET(reg->rgrid.ensure(grid.size()));
     RET(reg->rscore.ensure(g.H));
-    if (reg->rev_device != ex.device) {
-        for (cudaEvent_t &e : reg->rev) {
-            if (e) cudaEventDestroy(e);
-            e = nullptr;
-        }
-        CK(cudaEventCreate(&reg->rev[0]));
-        CK(cudaEventCreate(&reg->rev[1]));
-        reg->rev_device = ex.device;
+    if (reg->rev[1].device != ex.device) {  // (rev[1] is made last: both exist on that device)
+        CK(reg->rev[0].create(cudaEventDefault));
+        CK(reg->rev[1].create(cudaEventDefault));
     }
     CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
     CK(cudaMemcpyAsync(reg->rgrid.p, grid.data(), grid.size() * sizeof(double), cudaMemcpyHostToDevice, ex.stream));
     const MapView mv = map->view();
     const double *d_rot = reg->rgrid.p, *d_xs = d_rot + g.rot.size(), *d_ys = d_xs + g.nx;
-    CK(cudaEventRecord(reg->rev[0], ex.stream));
+    CK(cudaEventRecord(reg->rev[0].p, ex.stream));
     CK(reloc_score(&mv, sizeof(mv), reg->ws.src.p, static_cast<int>(n), d_rot, g.n_yaw, d_xs, g.nx, d_ys, g.ny, g.tz,
                    reg->rscore.p, ex.sms, ex.stream));
     ++ex.launches;
-    CK(cudaEventRecord(reg->rev[1], ex.stream));
+    CK(cudaEventRecord(reg->rev[1].p, ex.stream));
     std::vector<int> sc(g.H);
     CK(cudaMemcpyAsync(sc.data(), reg->rscore.p, g.H * sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
     RET(ex.sync());
@@ -1520,7 +1508,7 @@ int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_ma
     std::vector<SE3> guesses(K);
     for (size_t c = 0; c < K; ++c) {
         g.pose(static_cast<size_t>(peaks[c]), &cand[16 * c]);
-        if (!to_se3(&cand[16 * c], &guesses[c])) return fail(KB_ERR_NOT_SE3, "candidate %zu is not in SE(3)", c);
+        if (!se3_from_matrix(&cand[16 * c], &guesses[c])) return fail(KB_ERR_NOT_SE3, "candidate %zu is not in SE(3)", c);
     }
 
     // 4. refinement: align_batch of the source from every candidate, inliers on
@@ -1588,7 +1576,7 @@ int kb_preprocessor_preprocess(kb_preprocessor *pre, const double *xyz, size_t n
     if (!pre || (!xyz && n) || (!timestamps && n_timestamps) || !relative_motion || !n_out)
         return fail(KB_ERR_INVALID_ARG, "NULL argument");
     SE3 T;
-    if (!to_se3(relative_motion, &T)) return fail(KB_ERR_NOT_SE3, "relative_motion is not in SE(3)");
+    if (!se3_from_matrix(relative_motion, &T)) return fail(KB_ERR_NOT_SE3, "relative_motion is not in SE(3)");
     const bool do_deskew = pre->deskew && n_timestamps > 0;
     if (do_deskew && n_timestamps < n)
         return fail(KB_ERR_OUT_OF_RANGE, "timestamps (%zu) shorter than frame (%zu): the reference throws std::out_of_range",
@@ -1645,7 +1633,7 @@ int kb_threshold_compute(const kb_threshold *th, double *out_sigma) {
 int kb_threshold_update_model_deviation(kb_threshold *th, const double model_deviation[16]) {
     if (!th || !model_deviation) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     SE3 T;
-    if (!to_se3(model_deviation, &T)) return fail(KB_ERR_NOT_SE3, "model_deviation is not in SE(3)");
+    if (!se3_from_matrix(model_deviation, &T)) return fail(KB_ERR_NOT_SE3, "model_deviation is not in SE(3)");
     // scalar bookkeeping (Threshold.cpp:38-49); inside RegisterFrame the same update runs on the device
     const double theta = angle_axis_angle(q_to_matrix(T.q));
     const double delta_rot = 2.0 * th->max_range * std::sin(theta / 2.0);
@@ -1752,16 +1740,16 @@ static int pipeline_push_state(kb_pipeline *p, const SE3 &pose, const SE3 &delta
     s.num_samples = ns;
     s.vetoed = 0;
     s.front_id = -1;
-    CK(cudaMemcpyAsync(p->d_state, &s, sizeof(s), cudaMemcpyHostToDevice, p->ex->stream));
+    CK(cudaMemcpyAsync(p->d_state.p, &s, sizeof(s), cudaMemcpyHostToDevice, p->ex->stream));
     return p->ex->sync();
 }
 
 // the pipeline's device state and result buffers; the state of a new sequence (identity pose and delta, the initial threshold)
 static int pipeline_init_state(kb_pipeline *p) {
-    CK(cudaMalloc(&p->d_state, sizeof(PipeState)));
-    CK(cudaMalloc(&p->d_res, sizeof(FrameResult)));
-    CK(cudaMemsetAsync(p->d_res, 0, sizeof(FrameResult), p->ex->stream));  // (fields a launch does not write are read back too)
-    CK(cudaHostAlloc(&p->h_res, sizeof(FrameResult), cudaHostAllocDefault));
+    CK(p->d_state.alloc(1));
+    CK(p->d_res.alloc(1));
+    CK(cudaMemsetAsync(p->d_res.p, 0, sizeof(FrameResult), p->ex->stream));  // (fields a launch does not write are read back too)
+    CK(p->h_res.alloc(1));
     std::memset(&p->last, 0, sizeof(p->last));
     se3_to_matrix(se3_identity(), p->last.pose);
     se3_to_matrix(se3_identity(), p->last.delta);
@@ -1821,35 +1809,26 @@ int kb_pipeline_create_localizer(const kb_config *cfg, const kb_map *cprior, kb_
     RET(prior->ex->sync());
     CK(cudaSetDevice(p->ex->device));
     RET(p->fit_part.ensure(static_cast<size_t>(FIT_VALS) * p->ex->grid));
-    CK(cudaMalloc(&p->fit_dev, sizeof(FitResult) * (1 + kb_pipeline::Q_DEPTH)));
-    CK(cudaMemsetAsync(p->fit_dev, 0, sizeof(FitResult) * (1 + kb_pipeline::Q_DEPTH), p->ex->stream));
-    CK(cudaHostAlloc(&p->fit_host, sizeof(FitResult) * (1 + kb_pipeline::Q_DEPTH), cudaHostAllocDefault));
+    CK(p->fit_dev.alloc(1 + kb_pipeline::Q_DEPTH));
+    CK(cudaMemsetAsync(p->fit_dev.p, 0, sizeof(FitResult) * (1 + kb_pipeline::Q_DEPTH), p->ex->stream));
+    CK(p->fit_host.alloc(1 + kb_pipeline::Q_DEPTH));
     RET(pipeline_init_state(p.get()));
     prior->readers.fetch_add(1);
     *out = p.release();
     return KB_OK;
 }
 int kb_pipeline_destroy(kb_pipeline *p) {
-    if (p) {
+    if (p && p->localizer) {
+        // the prior must stay readable until this localizer's launches and copies have finished
         cudaSetDevice(p->ex->device);
-        if (p->localizer) {
-            // the prior must stay readable until this localizer's launches and copies have finished
-            if (!device_is_stuck(p->ex->device)) {
-                p->ex->sync();
-                if (p->copy_stream) cudaStreamSynchronize(p->copy_stream);
-                if (p->res_stream) cudaStreamSynchronize(p->res_stream);
-            }
-            p->map->readers.fetch_sub(1);
-            p->map = nullptr;
-            delete p;
-            return KB_OK;
+        if (!device_is_stuck(p->ex->device)) {
+            p->ex->sync();
+            if (p->copy_stream.p) cudaStreamSynchronize(p->copy_stream.p);
+            if (p->res_stream.p) cudaStreamSynchronize(p->res_stream.p);
         }
-        p->map->borrowed = false;
-        kb_map *m = p->map;
-        p->map = nullptr;
-        delete m;
-        delete p;
+        p->map->readers.fetch_sub(1);
     }
+    delete p;  // (an odometry pipeline deletes its own map)
     return KB_OK;
 }
 
@@ -1878,7 +1857,7 @@ static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, si
     P.next_n = static_cast<int>(next_n);
     P.next_in_f32 = in_f32 ? 1 : 0;
     P.ws = p->ws.view();
-    P.st = p->d_state;
+    P.st = p->d_state.p;
     P.res = res;
     P.in = d_xyz;
     P.ts = d_ts;
@@ -1937,12 +1916,48 @@ static int pipeline_absorb(kb_pipeline *p, const FrameResult &r, size_t n, long 
     return KB_OK;
 }
 
-// a vetoed frame modified nothing: grow the table for its now known voxel count and let frames run again
-static int pipeline_after_veto(kb_pipeline *p, const FrameResult &r, size_t n) {
-    ++p->grow_retries;
-    p->map->h_counters[C_STATUS] = 0;
-    CK(cudaMemsetAsync(&p->d_state->vetoed, 0, sizeof(int), p->ex->stream));
-    return p->map->ensure_capacity(std::max<size_t>(static_cast<size_t>(r.n_ds), pipeline_extra(p, n)) + 1);
+static void fit_to_abi(const FitResult &f, kb_fit *out) {
+    double JTr[6];
+    icp_expand(f.acc, out->JTJ, JTr);  // as kb_registration_build_system expands its accumulators
+    out->n_correspondences = f.n_corr;
+    out->n_source = f.n_src;
+    out->sum_sq_residual = f.sse;
+}
+
+enum Taken { TAKEN_ABSORBED, TAKEN_VETOED, TAKEN_SKIPPED };
+
+// take over the result `r` of frame `id` (n points in), blocking or queued, once its launch has ended:
+// - vetoed: the table was too small and the frame modified nothing; the frames queued behind it are skipped on the
+//   device. When they have ended, the table is grown for the frame's now known voxel count and the veto is cleared:
+//   the frame can be replayed.
+// - skipped: the frame did not run.
+// - absorbed: pipeline_absorb; the pose goes to pose_out, and a localizer's fit (pinned copy `fit_slot`) becomes the
+//   last one and goes to fit_out (either may be null).
+static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long id, size_t fit_slot, double *pose_out,
+                       kb_fit *fit_out, Taken *taken) {
+    RET(watchdog_check(p->ex->device));  // (a spin loop that gave up invalidates the launch)
+    if (r.map_status & ST_NEED_GROW) {
+        *taken = TAKEN_VETOED;
+        RET(p->ex->sync());
+        if (p->res_stream.p) CK(cudaStreamSynchronize(p->res_stream.p));
+        ++p->grow_retries;
+        p->map->h_counters[C_STATUS] = 0;
+        CK(cudaMemsetAsync(&p->d_state.p->vetoed, 0, sizeof(int), p->ex->stream));
+        return p->map->ensure_capacity(std::max<size_t>(static_cast<size_t>(r.n_ds), pipeline_extra(p, n)) + 1);
+    }
+    if (r.map_status & ST_SKIPPED) {
+        *taken = TAKEN_SKIPPED;
+        return KB_OK;
+    }
+    *taken = TAKEN_ABSORBED;
+    p->next_id = id + 1;
+    RET(pipeline_absorb(p, r, n, id));
+    if (pose_out) std::memcpy(pose_out, r.pose, sizeof(double) * 16);
+    if (p->localizer) {
+        p->last_fit = p->fit_host.p[fit_slot];
+        if (fit_out) fit_to_abi(p->last_fit, fit_out);
+    }
+    return KB_OK;
 }
 
 // blocking RegisterFrame on device-resident input
@@ -1953,22 +1968,21 @@ static int pipeline_run(kb_pipeline *p, const double *d_xyz, size_t n, const dou
     for (int attempt = 0; attempt < 3; ++attempt) {
         {
             StallTrace t("blocking: launch");
-            RET(pipeline_launch(p, id, d_xyz, n, d_ts, n_ts, in_f32, p->d_res, p->fit_dev));
+            RET(pipeline_launch(p, id, d_xyz, n, d_ts, n_ts, in_f32, p->d_res.p, p->fit_dev.p));
         }
         {
             StallTrace t("blocking: result D2H enqueue");
-            CK(cudaMemcpyAsync(p->h_res, p->d_res, sizeof(FrameResult), cudaMemcpyDeviceToHost, ex.stream));
-            if (p->localizer) CK(cudaMemcpyAsync(p->fit_host, p->fit_dev, sizeof(FitResult), cudaMemcpyDeviceToHost, ex.stream));
+            CK(cudaMemcpyAsync(p->h_res.p, p->d_res.p, sizeof(FrameResult), cudaMemcpyDeviceToHost, ex.stream));
+            if (p->localizer) CK(cudaMemcpyAsync(p->fit_host.p, p->fit_dev.p, sizeof(FitResult), cudaMemcpyDeviceToHost, ex.stream));
         }
         {
             StallTrace t("blocking: stream sync");
             RET(ex.sync());
         }
-        if (!(p->h_res->map_status & ST_NEED_GROW)) {
-            if (p->localizer) p->last_fit = p->fit_host[0];
-            return pipeline_absorb(p, *p->h_res, n, id);
-        }
-        RET(pipeline_after_veto(p, *p->h_res, n));
+        Taken taken;
+        RET(take_result(p, *p->h_res.p, n, id, 0, nullptr, nullptr, &taken));
+        if (taken == TAKEN_ABSORBED) return KB_OK;
+        if (taken == TAKEN_SKIPPED) return fail(KB_ERR_CUDA, "the frame was skipped behind a vetoed one (internal error)");
     }
     return fail(KB_ERR_CUDA, "voxel table could not be grown (internal capacity bug)");
 }
@@ -2019,17 +2033,17 @@ int kb_pipeline_register_frame_dev(kb_pipeline *p, const double *d_xyz, size_t n
 }
 // ---- queued registration of a whole sequence ------------------------------------------------------------------
 static int queue_init(kb_pipeline *p, size_t max_n, bool any_ts, bool device_input) {
-    if (!p->copy_stream) {
-        CK(cudaStreamCreateWithFlags(&p->copy_stream, cudaStreamNonBlocking));
+    if (!p->q_res_dev.p) {  // (made last: a failed first call is redone whole)
+        CK(p->copy_stream.create());
         for (auto &s : p->q) {
-            CK(cudaEventCreateWithFlags(&s.copied, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&s.read, cudaEventDisableTiming));
+            CK(s.copied.create(cudaEventDisableTiming));
+            CK(s.done.create(cudaEventDisableTiming));
+            CK(s.read.create(cudaEventDisableTiming));
         }
-        CK(cudaStreamCreateWithFlags(&p->res_stream, cudaStreamNonBlocking));
-        CK(cudaHostAlloc(&p->q_res, sizeof(FrameResult) * kb_pipeline::Q_DEPTH, cudaHostAllocDefault));
-        CK(cudaMalloc(&p->q_res_dev, sizeof(FrameResult) * kb_pipeline::Q_DEPTH));
-        CK(cudaMemsetAsync(p->q_res_dev, 0, sizeof(FrameResult) * kb_pipeline::Q_DEPTH, p->ex->stream));
+        CK(p->res_stream.create());
+        CK(p->q_res.alloc(kb_pipeline::Q_DEPTH));
+        CK(p->q_res_dev.alloc(kb_pipeline::Q_DEPTH));
+        CK(cudaMemsetAsync(p->q_res_dev.p, 0, sizeof(FrameResult) * kb_pipeline::Q_DEPTH, p->ex->stream));
     }
     if (!device_input)
         for (auto &s : p->q) {
@@ -2037,20 +2051,6 @@ static int queue_init(kb_pipeline *p, size_t max_n, bool any_ts, bool device_inp
             if (any_ts) RET(s.ts.ensure(std::max<size_t>(max_n, 1)));
         }
     return KB_OK;
-}
-
-static void fit_to_abi(const FitResult &f, kb_fit *out) {
-    double JTr[6];
-    icp_expand(f.acc, out->JTJ, JTr);  // as kb_registration_build_system expands its accumulators
-    out->n_correspondences = f.n_corr;
-    out->n_source = f.n_src;
-    out->sum_sq_residual = f.sse;
-}
-// a localizer's queued frame was absorbed: its fit (pinned copy `slot`) becomes the last one
-static void absorb_fit(kb_pipeline *p, size_t slot, kb_fit *out) {
-    if (!p->localizer) return;
-    p->last_fit = p->fit_host[slot];
-    if (out) fit_to_abi(p->last_fit, out);
 }
 
 static bool is_pinned(const void *ptr) {
@@ -2064,20 +2064,14 @@ static bool is_pinned(const void *ptr) {
 
 // host -> device on the copy stream; pageable sources go through this slot's pinned staging buffer so that the copy
 // is truly asynchronous (the memcpy into it overlaps the frame being registered)
-static int queue_upload(kb_pipeline *p, void *dst, const void *src, size_t bytes, void **pin, size_t *pin_bytes) {
+static int queue_upload(kb_pipeline *p, void *dst, const void *src, size_t bytes, PinBuf<unsigned char> &pin) {
     if (!bytes) return KB_OK;
     if (!is_pinned(src)) {
-        if (*pin_bytes < bytes) {
-            if (*pin) cudaFreeHost(*pin);
-            *pin = nullptr;
-            *pin_bytes = 0;
-            CK(cudaHostAlloc(pin, bytes + bytes / 4, cudaHostAllocDefault));
-            *pin_bytes = bytes + bytes / 4;
-        }
-        std::memcpy(*pin, src, bytes);
-        src = *pin;
+        RET(pin.ensure(bytes));
+        std::memcpy(pin.p, src, bytes);
+        src = pin.p;
     }
-    CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, p->copy_stream));
+    CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, p->copy_stream.p));
     return KB_OK;
 }
 
@@ -2123,10 +2117,14 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
     auto upload = [&](size_t u) -> int {  // host layouts: frame u -> slot u % D on the copy stream
         auto &s = p->q[u % D];
         StallTrace t("queue: H2D enqueue");
-        RET(queue_upload(p, s.in.p, xyz[u], n[u] * (f32 ? 12 : 24), &s.pin_xyz, &s.pin_xyz_bytes));
-        if (use_ts[u]) RET(queue_upload(p, s.ts.p, timestamps[u], n_timestamps[u] * 8, &s.pin_ts, &s.pin_ts_bytes));
-        CK(cudaEventRecord(s.copied, p->copy_stream));
+        RET(queue_upload(p, s.in.p, xyz[u], n[u] * (f32 ? 12 : 24), s.pin_xyz));
+        if (use_ts[u]) RET(queue_upload(p, s.ts.p, timestamps[u], n_timestamps[u] * 8, s.pin_ts));
+        CK(cudaEventRecord(s.copied.p, p->copy_stream.p));
         return KB_OK;
+    };
+    auto take = [&](size_t k, Taken *taken) {  // the result of frame k, once its launch and read-back have ended
+        return take_result(p, p->q_res.p[k % D], n[k], id0 + static_cast<long long>(k), 1 + k % D,
+                           poses_out ? poses_out + 16 * k : nullptr, fits_out ? fits_out + k : nullptr, taken);
     };
     auto run = [&]() -> int {
     while (next_absorb < valid) {
@@ -2145,26 +2143,26 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
                 if (prefetch) d_next = static_cast<const double *>(xyz[k + 1]);
             } else {
                 for (; next_upload <= k + (prefetch ? 1 : 0); ++next_upload) RET(upload(next_upload));
-                CK(cudaStreamWaitEvent(ex.stream, s.copied, 0));
-                if (prefetch) CK(cudaStreamWaitEvent(ex.stream, p->q[(k + 1) % D].copied, 0));
+                CK(cudaStreamWaitEvent(ex.stream, s.copied.p, 0));
+                if (prefetch) CK(cudaStreamWaitEvent(ex.stream, p->q[(k + 1) % D].copied.p, 0));
                 d_xyz = s.in.p;
                 d_ts = s.ts.p;
                 if (prefetch) d_next = p->q[(k + 1) % D].in.p;
             }
             {
                 StallTrace t("queue: launch");
-                RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32, p->q_res_dev + k % D,
-                                    p->localizer ? p->fit_dev + 1 + k % D : nullptr, d_next, prefetch ? n[k + 1] : 0));
-                CK(cudaEventRecord(s.done, ex.stream));
+                RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32, p->q_res_dev.p + k % D,
+                                    p->localizer ? p->fit_dev.p + 1 + k % D : nullptr, d_next, prefetch ? n[k + 1] : 0));
+                CK(cudaEventRecord(s.done.p, ex.stream));
                 // result read-back on its own stream: neither the next kernel nor the next H2D waits for it (letting
                 // the kernel write to mapped host memory instead was slower)
-                CK(cudaStreamWaitEvent(p->res_stream, s.done, 0));
-                CK(cudaMemcpyAsync(p->q_res + k % D, p->q_res_dev + k % D, sizeof(FrameResult), cudaMemcpyDeviceToHost,
-                                   p->res_stream));
+                CK(cudaStreamWaitEvent(p->res_stream.p, s.done.p, 0));
+                CK(cudaMemcpyAsync(p->q_res.p + k % D, p->q_res_dev.p + k % D, sizeof(FrameResult), cudaMemcpyDeviceToHost,
+                                   p->res_stream.p));
                 if (p->localizer)
-                    CK(cudaMemcpyAsync(p->fit_host + 1 + k % D, p->fit_dev + 1 + k % D, sizeof(FitResult), cudaMemcpyDeviceToHost,
-                                       p->res_stream));
-                CK(cudaEventRecord(s.read, p->res_stream));
+                    CK(cudaMemcpyAsync(p->fit_host.p + 1 + k % D, p->fit_dev.p + 1 + k % D, sizeof(FitResult),
+                                       cudaMemcpyDeviceToHost, p->res_stream.p));
+                CK(cudaEventRecord(s.read.p, p->res_stream.p));
             }
             ++next_submit;
             continue;
@@ -2172,29 +2170,19 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
         const size_t k = next_absorb;
         {
             StallTrace t("queue: wait for oldest frame");
-            cudaEvent_t ev = p->q[k % D].read;  // also frees this slot's buffers for frame k + D
+            cudaEvent_t ev = p->q[k % D].read.p;  // also frees this slot's buffers for frame k + D
             RET(ex.wait_deadline([&] { return cudaEventQuery(ev); }, "queued frame"));
         }
-        const FrameResult r = p->q_res[k % D];
-        if (r.map_status & ST_NEED_GROW) {  // frames queued behind it were skipped on the device: replay from k
-            if (++attempts >= 3) return fail(KB_ERR_CUDA, "voxel table could not be grown (internal capacity bug)");
-            RET(ex.sync());
-            CK(cudaStreamSynchronize(p->res_stream));
-            RET(pipeline_after_veto(p, r, n[k]));
+        Taken taken;
+        RET(take(k, &taken));
+        if (taken == TAKEN_VETOED) {  // replay from k
             next_submit = k;
             next_upload = k;
+            if (++attempts >= 3) return fail(KB_ERR_CUDA, "voxel table could not be grown (internal capacity bug)");
             continue;
         }
+        if (taken == TAKEN_SKIPPED) return fail(KB_ERR_CUDA, "queued frame %zu was skipped behind a vetoed one (internal error)", k);
         attempts = 0;
-        RET(watchdog_check(ex.device));
-        p->next_id = id0 + static_cast<long long>(k) + 1;
-        const int st = pipeline_absorb(p, r, n[k], id0 + static_cast<long long>(k));
-        if (st != KB_OK) {
-            ex.sync();
-            return st;
-        }
-        if (poses_out) std::memcpy(poses_out + 16 * k, r.pose, sizeof(double) * 16);
-        absorb_fit(p, 1 + k % D, fits_out ? fits_out + k : nullptr);
         ++next_absorb;
     }
     return KB_OK;
@@ -2204,21 +2192,11 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
         // an error in the middle of the queue: launches may still be in flight and finished frames not absorbed. Let them
         // finish and absorb what completed, so that the host mirrors (pose, counters, last clouds) match the device.
         const std::string msg = tl_err;
-        if (!device_is_stuck(ex.device) && cudaStreamSynchronize(p->copy_stream) == cudaSuccess && ex.sync() == KB_OK &&
-            cudaStreamSynchronize(p->res_stream) == cudaSuccess) {
-            for (; next_absorb < next_submit; ++next_absorb) {
-                const size_t k = next_absorb;
-                const FrameResult r = p->q_res[k % D];
-                if (r.map_status & ST_NEED_GROW) {
-                    pipeline_after_veto(p, r, n[k]);  // clears the sticky veto; the frames behind it were skipped
-                    break;
-                }
-                if (r.map_status & ST_SKIPPED) break;
-                p->next_id = id0 + static_cast<long long>(k) + 1;
-                if (pipeline_absorb(p, r, n[k], id0 + static_cast<long long>(k)) != KB_OK) break;
-                if (poses_out) std::memcpy(poses_out + 16 * k, r.pose, sizeof(double) * 16);
-                absorb_fit(p, 1 + k % D, fits_out ? fits_out + k : nullptr);
-            }
+        if (!device_is_stuck(ex.device) && cudaStreamSynchronize(p->copy_stream.p) == cudaSuccess && ex.sync() == KB_OK &&
+            cudaStreamSynchronize(p->res_stream.p) == cudaSuccess) {
+            // up to an error, a veto (cleared: the frames behind it were skipped) or a skipped frame
+            Taken taken;
+            while (next_absorb < next_submit && take(next_absorb, &taken) == KB_OK && taken == TAKEN_ABSORBED) ++next_absorb;
         }
         cudaGetLastError();
         tl_err = msg;
@@ -2311,7 +2289,7 @@ int kb_pipeline_delta(const kb_pipeline *p, double out[16]) {
 }
 static int pipeline_set(kb_pipeline *p, const double pose[16], const double delta[16]) {
     SE3 a, b;
-    if (!to_se3(pose, &a) || !to_se3(delta, &b)) return fail(KB_ERR_NOT_SE3, "matrix is not in SE(3)");
+    if (!se3_from_matrix(pose, &a) || !se3_from_matrix(delta, &b)) return fail(KB_ERR_NOT_SE3, "matrix is not in SE(3)");
     CK(cudaSetDevice(p->ex->device));
     RET(pipeline_push_state(p, a, b, p->last.model_sse, p->last.num_samples));
     std::memcpy(p->last.pose, pose, sizeof(double) * 16);
@@ -2342,7 +2320,7 @@ int kb_pipeline_get_state(const kb_pipeline *p, kb_pipeline_state *out) {
     if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     CK(cudaSetDevice(p->ex->device));
     PipeState s;
-    CK(cudaMemcpyAsync(&s, p->d_state, sizeof(s), cudaMemcpyDeviceToHost, p->ex->stream));
+    CK(cudaMemcpyAsync(&s, p->d_state.p, sizeof(s), cudaMemcpyDeviceToHost, p->ex->stream));
     RET(p->ex->sync());
     se3_to_params(s.last_pose, out->pose);
     se3_to_params(s.last_delta, out->delta);
@@ -2405,7 +2383,7 @@ int kb_debug_icp_schur(const double acc[16], double x_schur[6], double x_ldlt[6]
 // are copied back
 int kb_debug_nn_reuse(const kb_map *map, const double *pf, const double *p, size_t n, int path, double *out_points,
                       double *out_dist, int *out_reused) {
-    if (device_count() <= 0) return fail(KB_ERR_NO_DEVICE, "no CUDA device visible (this library has no CPU fallback)");
+    RET(require_device());
     if (!map || (n &&(!pf || !p || !out_points || !out_dist || !out_reused))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (path != 0 && path != 1) return fail(KB_ERR_INVALID_ARG, "path must be 0 (ICP team) or 1 (whole-grid ICP loop)");
     if (n > (size_t(1) << 28)) return fail(KB_ERR_INVALID_ARG, "n > 2^28");
@@ -2477,9 +2455,9 @@ int kb_debug_se3_exp_dev(const double *tangents, size_t n, double *out) { return
 int kb_debug_fast_rcp_dev(const double *x, size_t n, double *out) { return probe_map_doubles(x, n, 1, out, 1, probe_fast_rcp); }
 int kb_debug_reloc_score_ms(const kb_registration *reg, float *ms) {
     if (!reg || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (reg->rev_device < 0) return fail(KB_ERR_INVALID_ARG, "no kb_relocalize call on this handle yet");
-    CK(cudaSetDevice(reg->rev_device));
-    CK(cudaEventElapsedTime(ms, reg->rev[0], reg->rev[1]));
+    if (reg->rev[1].device < 0) return fail(KB_ERR_INVALID_ARG, "no kb_relocalize call on this handle yet");
+    CK(cudaSetDevice(reg->rev[1].device));
+    CK(cudaEventElapsedTime(ms, reg->rev[0].p, reg->rev[1].p));
     return KB_OK;
 }
 int kb_debug_barrier_ns(int iters, double *ns_per_barrier) {
