@@ -307,14 +307,27 @@ typedef struct kb_fit {
 int kb_pipeline_create_localizer(const kb_config *cfg, const kb_map *prior, kb_pipeline **out);
 /* localizers reading the map (0: it may be changed) */
 int kb_map_readers(const kb_map *map, int *out);
-/* the fit of the last frame (all zero before the first); KB_ERR_INVALID_ARG on an odometry pipeline */
+/* the fit of the last frame (all zero before the first); KB_ERR_INVALID_ARG on an odometry pipeline without fit
+ * reporting (kb_pipeline_set_fit_reporting) */
 int kb_pipeline_last_fit(const kb_pipeline *p, kb_fit *out);
 /* kb_pipeline_register_frames with one fit per frame in fits_out[count] (may be NULL), read behind the queue like
- * the poses. Same poses as kb_pipeline_register_frames. A non-NULL fits_out on an odometry pipeline is
- * KB_ERR_INVALID_ARG. */
+ * the poses. Same poses as kb_pipeline_register_frames. A non-NULL fits_out on an odometry pipeline without fit
+ * reporting is KB_ERR_INVALID_ARG. */
 int kb_pipeline_register_frames_fit(kb_pipeline *p, const void *const *xyz, const size_t *n,
                                     const double *const *timestamps, const size_t *n_timestamps, size_t count,
                                     int layout, double *poses_out, kb_fit *fits_out);
+/* Fit reporting of an odometry pipeline (off when it is created). With it on, every registered frame also gets a kb_fit,
+ * defined as a localizer's, against the pipeline's own map as that frame's ICP saw it: before the frame's
+ * local_map_.Update (KissICP.cpp:61), which would put the scan's own points in the map. kb_pipeline_last_fit and
+ * kb_pipeline_register_frames_fit then work as on a localizer. A frame vetoed for table capacity gets the fit of its
+ * replay. Poses, iterations, the threshold state and the map are bit for bit those of reporting off; the frames run a
+ * kernel of their own, which costs one more grid barrier and the fit pass per frame. Enabling allocates the fit buffers
+ * and resets the last fit to zeros (KB_ERR_CUDA if that fails; reporting stays off), enabling it again is a no-op;
+ * disabling releases them. A localizer always reports: enabled = 1 is a no-op, 0 is KB_ERR_INVALID_ARG.
+ * KB_ERR_INVALID_ARG for p == NULL. */
+int kb_pipeline_set_fit_reporting(kb_pipeline *p, int enabled);
+/* *out = 1 if the pipeline reports fits (a localizer, or fit reporting on), else 0; KB_ERR_INVALID_ARG for NULL */
+int kb_pipeline_fit_reporting(const kb_pipeline *p, int *out);
 
 /* ---- relocalization: a global pose search in a bounded region ----------------------------
  * No reference counterpart. Finds a scan's pose in a map without an initial pose: every hypothesis of a grid in x, y

@@ -11,7 +11,9 @@ extern "C" {
 #endif
 
 /* profiling aids (no reference counterpart): raw %globaltimer stamps [ns, relative to stamp 0]
- * of the second ICP iteration of the last frame (CTA 0); cost of one grid barrier */
+ * of the second ICP iteration of the last frame (CTA 0), among them [30..32] the ICP fill pass and [35, 36] the fit pass
+ * of an odometry pipeline with fit reporting (its start, and the end of the grid barrier behind it); cost of one grid
+ * barrier */
 int kb_pipeline_debug_stamps(const kb_pipeline *p, double *ns, int n);
 int kb_debug_barrier_ns(int iters, double *ns_per_barrier);
 /* host evaluation of the ICP loop's structured (Schur complement) solve vs the pivoted LDL^T it falls back to, on the

@@ -41,12 +41,12 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/api.cu, csrc/localize.cu, csrc/probe.cu and csrc/relocalize.cu -> libkiss_icp_b200.so (sm_90a).
-    No-op when up to date."""
+    """Compile csrc/api.cu, csrc/localize.cu, csrc/odometry_fit.cu, csrc/probe.cu and csrc/relocalize.cu
+    -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in sources())
     if force or stale:
         cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH,
-               *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "probe.cu", "relocalize.cu"))]
+               *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "odometry_fit.cu", "probe.cu", "relocalize.cu"))]
         if verbose:
             print(" ".join(cmd))
         env = dict(os.environ)
@@ -198,6 +198,8 @@ SIGNATURES = {
     "kb_map_readers": (i32, [vp, C.POINTER(i32)]),
     "kb_pipeline_last_fit": (i32, [vp, C.POINTER(Fit)]),
     "kb_pipeline_register_frames_fit": (i32, [vp, vp, vp, vp, vp, sz, i32, vp, vp]),
+    "kb_pipeline_set_fit_reporting": (i32, [vp, i32]),
+    "kb_pipeline_fit_reporting": (i32, [vp, C.POINTER(i32)]),
     "kb_reloc_hypotheses": (i32, [C.POINTER(RelocSearch), vp, sz, C.POINTER(sz)]),
     "kb_relocalize": (i32, [vp, vp, sz, vp, C.POINTER(RelocSearch), C.POINTER(RelocResult), vp, vp, vp]),
     "kb_debug_reloc_score_ms": (i32, [vp, C.POINTER(C.c_float)]),

@@ -91,6 +91,7 @@ int watchdog_init(int device) {
     if (const char *e = std::getenv("KB_WATCHDOG_SHIFT")) init[7] = static_cast<unsigned>(std::max(10, std::min(std::atoi(e), 31)));
     CK(cudaMemcpyToSymbol(g_kb_wd, init, sizeof(init)));
     CK(localize_watchdog_init(d, init));  // the localizer kernel's module has its own copies
+    CK(odometry_fit_watchdog_init(d, init));  // and so has the fit-reporting odometry kernel's
     g_wd[device].host = h;
     return KB_OK;
 }
@@ -113,6 +114,7 @@ int watchdog_check(int device) {
     unsigned zero = 0;
     cudaMemcpyToSymbol(g_kb_wd, &zero, sizeof(zero));  // re-arm
     localize_watchdog_rearm();
+    odometry_fit_watchdog_rearm();
     static const char *names[] = {"?", "grid barrier", "ICP gather", "ICP result record", "ICP team gather", "NN bulk copy"};
     std::string marks;
     unsigned m[256];
@@ -703,9 +705,12 @@ struct kb_pipeline {
     std::shared_ptr<Exec> ex;
     kb_config cfg;
     kb_map *map = nullptr;
-    // a localizer (kb_pipeline_create_localizer): `map` is the prior map, borrowed and never written; every frame
-    // also computes its fit, into fit_dev[0] (blocking calls) or fit_dev[1 + k % Q_DEPTH] (queued frame k)
+    // a localizer (kb_pipeline_create_localizer): `map` is the prior map, borrowed and never written
     bool localizer = false;
+    bool fit_reporting = false;  // an odometry pipeline that reports fits (kb_pipeline_set_fit_reporting)
+    // a pipeline that reports fits computes one per frame, into fit_dev[0] (blocking calls) or fit_dev[1 + k % Q_DEPTH]
+    // (queued frame k)
+    bool reports_fits() const { return localizer || fit_reporting; }
     DBuf<double> fit_part;           // [FIT_VALS][grid] per-CTA partials of the fit pass
     DBuf<FitResult> fit_dev;         // [1 + Q_DEPTH]
     PinBuf<FitResult> fit_host;      // [1 + Q_DEPTH] copies
@@ -1758,6 +1763,21 @@ static int pipeline_init_state(kb_pipeline *p) {
     return pipeline_push_state(p, se3_identity(), se3_identity(), p->last.model_sse, 1);
 }
 
+// the buffers of a pipeline that reports fits (on the pipeline's device); the last fit becomes all zero
+static int pipeline_alloc_fit(kb_pipeline *p) {
+    RET(p->fit_part.ensure(static_cast<size_t>(FIT_VALS) * p->ex->grid));
+    CK(p->fit_dev.alloc(1 + kb_pipeline::Q_DEPTH));
+    CK(cudaMemsetAsync(p->fit_dev.p, 0, sizeof(FitResult) * (1 + kb_pipeline::Q_DEPTH), p->ex->stream));
+    CK(p->fit_host.alloc(1 + kb_pipeline::Q_DEPTH));
+    p->last_fit = FitResult{};
+    return KB_OK;
+}
+static void pipeline_free_fit(kb_pipeline *p) {
+    p->fit_part = DBuf<double>{};
+    p->fit_dev = DBuf<FitResult>{};
+    p->fit_host = PinBuf<FitResult>{};
+}
+
 int kb_pipeline_create(const kb_config *cfg, kb_pipeline **out) {
     if (!cfg || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (cfg->max_num_iterations > 8000) return fail(KB_ERR_INVALID_ARG, "max_num_iterations > 8000 is not supported");
@@ -1808,10 +1828,7 @@ int kb_pipeline_create_localizer(const kb_config *cfg, const kb_map *cprior, kb_
     // everything queued on the map before (a load, updates, asynchronous queries) is complete before a frame reads it
     RET(prior->ex->sync());
     CK(cudaSetDevice(p->ex->device));
-    RET(p->fit_part.ensure(static_cast<size_t>(FIT_VALS) * p->ex->grid));
-    CK(p->fit_dev.alloc(1 + kb_pipeline::Q_DEPTH));
-    CK(cudaMemsetAsync(p->fit_dev.p, 0, sizeof(FitResult) * (1 + kb_pipeline::Q_DEPTH), p->ex->stream));
-    CK(p->fit_host.alloc(1 + kb_pipeline::Q_DEPTH));
+    RET(pipeline_alloc_fit(p.get()));
     RET(pipeline_init_state(p.get()));
     prior->readers.fetch_add(1);
     *out = p.release();
@@ -1841,12 +1858,11 @@ static size_t pipeline_extra(const kb_pipeline *p, size_t n) {
 
 // enqueue one RegisterFrame on the pipeline's stream; the result goes to `res` (device-visible memory)
 // `next_xyz` (may be null): the frame after this one, already on the device, no timestamps -> its front end is prefetched
-// `fit` (localizers only): where the frame's fit goes
+// `fit` (pipelines that report fits only): where the frame's fit goes
 static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, size_t n, const double *d_ts, size_t n_ts,
                            bool in_f32, FrameResult *res, FitResult *fit, const double *next_xyz = nullptr, size_t next_n = 0) {
     Exec &ex = *p->ex;
-    LocalizeParams L;
-    FrameParams &P = L;
+    FrameParams P;
     P.m = p->map->view();
     P.sc = ex.sc;
     P.team = ex.team;
@@ -1875,8 +1891,16 @@ static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, si
     P.in_f32 = in_f32 ? 1 : 0;
     const size_t smem = std::max<size_t>(QC_BYTES, ex.icp_smem);
     if (p->localizer) {
+        LocalizeParams L;
+        static_cast<FrameParams &>(L) = P;
         L.fit = FitOut{p->fit_part.p, fit};
         return ex.coop_raw(localize_kernel(), &L, smem, true);
+    }
+    if (p->fit_reporting) {
+        OdometryFitParams F;
+        static_cast<FrameParams &>(F) = P;
+        F.fit = FitOut{p->fit_part.p, fit};
+        return ex.coop_raw(odometry_fit_kernel(), &F, smem, true);
     }
     return ex.coop(k_register_frame<FrameParams>, P, smem, true);
 }
@@ -1931,8 +1955,8 @@ enum Taken { TAKEN_ABSORBED, TAKEN_VETOED, TAKEN_SKIPPED };
 //   device. When they have ended, the table is grown for the frame's now known voxel count and the veto is cleared:
 //   the frame can be replayed.
 // - skipped: the frame did not run.
-// - absorbed: pipeline_absorb; the pose goes to pose_out, and a localizer's fit (pinned copy `fit_slot`) becomes the
-//   last one and goes to fit_out (either may be null).
+// - absorbed: pipeline_absorb; the pose goes to pose_out, and the fit of a pipeline that reports fits (pinned copy
+//   `fit_slot`) becomes the last one and goes to fit_out (either may be null).
 static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long id, size_t fit_slot, double *pose_out,
                        kb_fit *fit_out, Taken *taken) {
     RET(watchdog_check(p->ex->device));  // (a spin loop that gave up invalidates the launch)
@@ -1953,7 +1977,7 @@ static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long
     p->next_id = id + 1;
     RET(pipeline_absorb(p, r, n, id));
     if (pose_out) std::memcpy(pose_out, r.pose, sizeof(double) * 16);
-    if (p->localizer) {
+    if (p->reports_fits()) {
         p->last_fit = p->fit_host.p[fit_slot];
         if (fit_out) fit_to_abi(p->last_fit, fit_out);
     }
@@ -1973,7 +1997,7 @@ static int pipeline_run(kb_pipeline *p, const double *d_xyz, size_t n, const dou
         {
             StallTrace t("blocking: result D2H enqueue");
             CK(cudaMemcpyAsync(p->h_res.p, p->d_res.p, sizeof(FrameResult), cudaMemcpyDeviceToHost, ex.stream));
-            if (p->localizer) CK(cudaMemcpyAsync(p->fit_host.p, p->fit_dev.p, sizeof(FitResult), cudaMemcpyDeviceToHost, ex.stream));
+            if (p->reports_fits()) CK(cudaMemcpyAsync(p->fit_host.p, p->fit_dev.p, sizeof(FitResult), cudaMemcpyDeviceToHost, ex.stream));
         }
         {
             StallTrace t("blocking: stream sync");
@@ -2075,7 +2099,11 @@ static int queue_upload(kb_pipeline *p, void *dst, const void *src, size_t bytes
     return KB_OK;
 }
 
-// kb_pipeline_register_frames[_fit]; fits_out (localizers only, may be NULL) receives one fit per frame
+static const char *const kNoFits =
+    "fits are computed by localizers (kb_pipeline_create_localizer) and by odometry pipelines with fit reporting on "
+    "(kb_pipeline_set_fit_reporting)";
+
+// kb_pipeline_register_frames[_fit]; fits_out (pipelines that report fits only, may be NULL) receives one fit per frame
 static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
                            const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out) {
     if (!p || (count && (!xyz || !n))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
@@ -2152,14 +2180,14 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
             {
                 StallTrace t("queue: launch");
                 RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32, p->q_res_dev.p + k % D,
-                                    p->localizer ? p->fit_dev.p + 1 + k % D : nullptr, d_next, prefetch ? n[k + 1] : 0));
+                                    p->reports_fits() ? p->fit_dev.p + 1 + k % D : nullptr, d_next, prefetch ? n[k + 1] : 0));
                 CK(cudaEventRecord(s.done.p, ex.stream));
                 // result read-back on its own stream: neither the next kernel nor the next H2D waits for it (letting
                 // the kernel write to mapped host memory instead was slower)
                 CK(cudaStreamWaitEvent(p->res_stream.p, s.done.p, 0));
                 CK(cudaMemcpyAsync(p->q_res.p + k % D, p->q_res_dev.p + k % D, sizeof(FrameResult), cudaMemcpyDeviceToHost,
                                    p->res_stream.p));
-                if (p->localizer)
+                if (p->reports_fits())
                     CK(cudaMemcpyAsync(p->fit_host.p + 1 + k % D, p->fit_dev.p + 1 + k % D, sizeof(FitResult),
                                        cudaMemcpyDeviceToHost, p->res_stream.p));
                 CK(cudaEventRecord(s.read.p, p->res_stream.p));
@@ -2214,13 +2242,36 @@ int kb_pipeline_register_frames(kb_pipeline *p, const void *const *xyz, const si
 }
 int kb_pipeline_register_frames_fit(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
                                     const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out) {
-    if (p && fits_out && !p->localizer) return fail(KB_ERR_INVALID_ARG, "fits are computed by localizers only (kb_pipeline_create_localizer)");
+    if (p && fits_out && !p->reports_fits()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
     return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out);
 }
 int kb_pipeline_last_fit(const kb_pipeline *p, kb_fit *out) {
     if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (!p->localizer) return fail(KB_ERR_INVALID_ARG, "fits are computed by localizers only (kb_pipeline_create_localizer)");
+    if (!p->reports_fits()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
     fit_to_abi(p->last_fit, out);
+    return KB_OK;
+}
+int kb_pipeline_set_fit_reporting(kb_pipeline *p, int enabled) {
+    if (!p) return fail(KB_ERR_INVALID_ARG, "p == NULL");
+    if (p->localizer) return enabled ? KB_OK : fail(KB_ERR_INVALID_ARG, "a localizer always reports fits");
+    if (!enabled) {
+        p->fit_reporting = false;
+        pipeline_free_fit(p);  // (no launch of this pipeline is in flight between calls)
+        return KB_OK;
+    }
+    if (p->fit_reporting) return KB_OK;
+    CK(cudaSetDevice(p->ex->device));
+    const int st = pipeline_alloc_fit(p);
+    if (st != KB_OK) {
+        pipeline_free_fit(p);
+        return st;
+    }
+    p->fit_reporting = true;
+    return KB_OK;
+}
+int kb_pipeline_fit_reporting(const kb_pipeline *p, int *out) {
+    if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *out = p->reports_fits() ? 1 : 0;
     return KB_OK;
 }
 

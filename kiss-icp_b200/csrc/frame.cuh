@@ -1,6 +1,7 @@
 // KissICP::RegisterFrame as one persistent kernel (k_register_frame) and what it works on. A header of its own:
-// the odometry instantiation is compiled with the other kernels (api.cu), the localizer's in a translation unit of its
-// own (localize.cu), so that neither changes the code generated for the other.
+// the odometry instantiation is compiled with the other kernels (api.cu), the localizer's and the fit-reporting
+// odometry's each in a translation unit of its own (localize.cu, odometry_fit.cu), so that none changes the code
+// generated for another.
 #pragma once
 
 #include <type_traits>
@@ -123,7 +124,7 @@ __device__ __noinline__ void op_front(Grid &g, const Scratch &sc, Shared &sh, co
     op_downsample(g, sc, sh, fr.ds1, n_ds, voxel_size * 1.5, ws.ds2, fr.src, &fr.cnt[2], t_ns ? &t_ns[16] : nullptr, true);
 }
 
-// ---- the fit of a localized frame (k_register_frame<LocalizeParams>, kb_pipeline_last_fit) --------------------------
+// ---- the fit of a frame (k_register_frame<LocalizeParams> / <OdometryFitParams>, kb_pipeline_last_fit) --------------
 // DataAssociation + BuildLinearSystem (Registration.cpp:60-121) of the source mapped by the final pose, formed the way
 // kb_registration_build_system forms them (nn_search_warp, icp_term, expanded by icp_expand on the host), plus the
 // unweighted sum of |r|^2. Deterministic for a grid size: point qi -> CTA qi % G, warp (qi / G) % NWARPS, a lane sums
@@ -139,6 +140,11 @@ struct FitOut {
     FitResult *res;  // this frame's fit
 };
 struct LocalizeParams : FrameParams {
+    FitOut fit;
+};
+// an odometry pipeline that reports fits (kb_pipeline_set_fit_reporting): the odometry statement, plus the fit
+// against the map as this frame's ICP saw it, i.e. before the frame's own points are inserted
+struct OdometryFitParams : FrameParams {
     FitOut fit;
 };
 
@@ -192,9 +198,12 @@ __device__ __forceinline__ void fit_finish(const FitOut &fit, int n_src) {
 // k_register_frame<LocalizeParams> (a localizer): the same statement against a read-only prior map, without local_map_.Update
 // (KissICP.cpp:61). Nothing is inserted, so there is no capacity check and no veto, and the map-update phase is the
 // fit pass (op_fit) at the final pose. Nothing writes to the map.
+// k_register_frame<OdometryFitParams>: the odometry statement with the fit pass at the final pose in front of the map
+// update, and one grid barrier between them (op_fit reads the table op_map_add writes).
 template <class Params>
 __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
     constexpr bool LOCALIZE = std::is_same<Params, LocalizeParams>::value;
+    constexpr bool ODOMETRY_FIT = std::is_same<Params, OdometryFitParams>::value;
     __shared__ Shared sh;
     Grid g;
     g.init(P.sc.bar);
@@ -325,6 +334,14 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
         op_fit(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part);
         kb_mark(0x700u);
     } else {
+        if constexpr (ODOMETRY_FIT) {
+            // the fit at the final pose, with this frame's (3 sigma, sigma), against the map before local_map_.Update
+            // (after it, the frame's own points would be in the map). Stamps: the pass including the barrier behind it.
+            if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[35] = globaltimer_ns();
+            op_fit(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part);
+            g.sync();
+            if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[36] = globaltimer_ns();
+        }
         // local_map_.Update(frame_downsample, new_pose) (KissICP.cpp:61)
         op_map_add(g, sh, P.m, fr.ds1, n_ds, true, new_pose, P.ws.tp, P.ws.next, P.ws.touched, P.sc.profile ? &P.res->t_ns[8] : nullptr);
         kb_mark(0x700u);
@@ -334,7 +351,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
     g.sync();
     kb_mark(0x900u);
     KB_STAMP(5);
-    if constexpr (LOCALIZE) {
+    if constexpr (LOCALIZE || ODOMETRY_FIT) {
         if (blockIdx.x == gridDim.x - 1) fit_finish(P.fit, n_src);
     }
     if (book) {
@@ -359,3 +376,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
 const void *localize_kernel();
 cudaError_t localize_watchdog_init(unsigned *d_host_words, const unsigned init[8]);
 cudaError_t localize_watchdog_rearm();
+// defined in odometry_fit.cu, likewise: k_register_frame<OdometryFitParams> and its copies of the watchdog words
+const void *odometry_fit_kernel();
+cudaError_t odometry_fit_watchdog_init(unsigned *d_host_words, const unsigned init[8]);
+cudaError_t odometry_fit_watchdog_rearm();

@@ -12,6 +12,10 @@ Two execution modes:
 localizer exists the map's mutators raise MapInUseError. Build a prior map with existing calls, for example a
 VoxelHashMap with a large max_distance and ``vmap.update(frame_downsample, pose)`` per scan of an odometry run, or
 ``vmap.load(...)`` from a state_dict (INTEGRATION.md section 4).
+
+``KissICP(config, report_fit=True)`` is an odometry pipeline that also reports, in ``last_fit`` and
+``register_frames(..., return_fits=True)``, how well each scan fit the map it was registered in: the pipeline's own map
+before the scan's ``local_map.update``. Poses, thresholds and the map are the same as without it.
 """
 from __future__ import annotations
 
@@ -34,7 +38,7 @@ from .voxelization import voxel_down_sample
 STATE_FORMAT_VERSION = 1  # of KissICP.state_dict()
 MAP_KEYS = ("voxels", "counts", "points")  # the map's part of an odometry state_dict()
 
-# the fit of a localized scan at its final pose (kb_fit): correspondences closer than 3 sigma, source points,
+# the fit of a scan at its final pose (kb_fit): correspondences closer than 3 sigma, source points,
 # sqrt(sum |r|^2 / n_correspondences) (NaN without correspondences), and the 6x6 information matrix J^T W J
 Fit = namedtuple("Fit", ["n_correspondences", "n_source", "rmse", "information"])
 
@@ -104,7 +108,8 @@ class _PipelineThreshold:
 
 
 class KissICP:
-    def __init__(self, config: KISSConfig | None = None, fused: bool = True, prior_map: VoxelHashMap | None = None):
+    def __init__(self, config: KISSConfig | None = None, fused: bool = True, prior_map: VoxelHashMap | None = None,
+                 report_fit: bool = False):
         if prior_map is not None and not isinstance(prior_map, VoxelHashMap):
             raise TypeError(f"prior_map must be a VoxelHashMap, not {type(prior_map).__name__}")
         self.config = config if config is not None else load_config()
@@ -112,6 +117,7 @@ class KissICP:
             self.config.mapping.voxel_size = float(self.config.data.max_range / 100.0)
         self.fused = bool(fused) and self.config.adaptive_threshold.fixed_threshold is None
         self.localizer = prior_map is not None
+        self._report_fit = self.localizer or bool(report_fit)  # (a localizer always reports)
         self._h = None
         if self.localizer:
             self._check_prior(prior_map)
@@ -136,6 +142,8 @@ class KissICP:
                 N.check(N.lib().kb_pipeline_create(C.byref(c), C.byref(self._h)))
                 self.local_map = VoxelHashMap(c.voxel_size, c.max_range, c.max_points_per_voxel,
                                               _borrowed=N.lib().kb_pipeline_voxel_map(self._h), _owner=self)
+                if self._report_fit:
+                    N.check(N.lib().kb_pipeline_set_fit_reporting(self._h, 1))
             self.adaptive_threshold = _PipelineThreshold(self)
         else:
             self._last_pose = np.eye(4)
@@ -192,10 +200,20 @@ class KissICP:
             N.check(N.lib().kb_pipeline_set_delta(self._h, N.ptr(N.mat4_arg(T))))
 
     @property
+    def report_fit(self) -> bool:
+        """whether every scan gets a fit (a localizer, or KissICP(config, report_fit=True))"""
+        return self._report_fit
+
+    def _check_reports_fits(self):
+        if not self._report_fit:
+            raise ValueError("fits are computed by localizers and by odometry pipelines that report them: "
+                             "KissICP(config, prior_map=...) or KissICP(config, report_fit=True)")
+
+    @property
     def last_fit(self) -> Fit:
-        """the fit of the last scan of a localizer at its final pose (zeros before the first scan)"""
-        if not self.localizer:
-            raise ValueError("fits are computed by localizers only: KissICP(config, prior_map=...)")
+        """the fit of the last scan at its final pose (zeros before the first scan): against the prior map of a
+        localizer, or against the map of an odometry pipeline with report_fit=True before the scan's update"""
+        self._check_reports_fits()
         if not self.fused:
             return self._last_fit
         f = N.Fit()
@@ -282,10 +300,10 @@ class KissICP:
         Same results as K ``register_frame`` calls; the frames are queued on the device (copy of frame k+1
         overlaps the registration of frame k, results are read behind the queue). ``frames`` is a sequence of
         (N_k,3) arrays, all float64 or all float32; ``timestamps`` a matching sequence (or None).
-        ``return_fits`` (localizers only) -> (poses, fits): a Fit of arrays, one entry per frame."""
+        ``return_fits`` (localizers and report_fit=True only) -> (poses, fits): a Fit of arrays, one entry per frame."""
         K = len(frames)
-        if return_fits and not self.localizer:
-            raise ValueError("fits are computed by localizers only: KissICP(config, prior_map=...)")
+        if return_fits:
+            self._check_reports_fits()
         if timestamps is None:
             timestamps = [np.empty(0)] * K
         if len(timestamps) != K:
@@ -342,9 +360,9 @@ class KissICP:
         )
         model_deviation = np.linalg.inv(initial_guess) @ new_pose
         self.adaptive_threshold.update_model_deviation(model_deviation)
-        if self.localizer:  # no local_map.update: the fit at the final pose instead
+        if self._report_fit:  # against the map the scan was registered in: before local_map.update adds it
             self._last_fit = self._fit_modular(source, new_pose, sigma)
-        else:
+        if not self.localizer:  # (a localizer has no local_map.update)
             self.local_map.update(frame_downsample, new_pose)
         self._last_delta = np.linalg.inv(self._last_pose) @ new_pose
         self._last_pose = new_pose
