@@ -708,17 +708,14 @@ struct kb_pipeline {
     // a localizer (kb_pipeline_create_localizer): `map` is the prior map, borrowed and never written
     bool localizer = false;
     bool fit_reporting = false;  // an odometry pipeline that reports fits (kb_pipeline_set_fit_reporting)
-    // a pipeline that reports fits computes one per frame, into fit_dev[0] (blocking calls) or fit_dev[1 + k % Q_DEPTH]
-    // (queued frame k)
+    // a pipeline that reports fits computes one per frame, into fit_dev[k % Q_DEPTH] (frame k of a call)
     bool reports_fits() const { return localizer || fit_reporting; }
     DBuf<double> fit_part;           // [FIT_VALS][grid] per-CTA partials of the fit pass
-    DBuf<FitResult> fit_dev;         // [1 + Q_DEPTH]
-    PinBuf<FitResult> fit_host;      // [1 + Q_DEPTH] copies
+    DBuf<FitResult> fit_dev;         // [Q_DEPTH]
+    PinBuf<FitResult> fit_host;      // [Q_DEPTH] copies
     FitResult last_fit{};
     Work ws;
     DBuf<PipeState> d_state;
-    DBuf<FrameResult> d_res;
-    PinBuf<FrameResult> h_res;
     FrameResult last{};
     bool has_last = false;
     long long next_id = 0;  // id of the next frame to register (Workspace::fr[id & 1] holds its front end)
@@ -728,7 +725,8 @@ struct kb_pipeline {
     std::vector<kb_frame_stats> history;
     std::vector<std::array<double, 20>> history_stamps;  // the frames' %globaltimer stamps, ns modulo 2^40 (profiling on)
     size_t history_cap = 0;
-    // frame queue of kb_pipeline_register_frames: frame k+1 is copied in while frame k is registered
+    // frame queue of every registration call (a blocking call is a queue of one frame): frame k+1 is copied in while
+    // frame k is registered
     static constexpr int Q_DEPTH = 4;  // frame k registering, k+1 being prefetched by the same launch, k+2 / k+3 copying
     struct Slot {
         DBuf<double> in, ts;  // device copy of one queued frame
@@ -1749,12 +1747,9 @@ static int pipeline_push_state(kb_pipeline *p, const SE3 &pose, const SE3 &delta
     return p->ex->sync();
 }
 
-// the pipeline's device state and result buffers; the state of a new sequence (identity pose and delta, the initial threshold)
+// the pipeline's device state; the state of a new sequence (identity pose and delta, the initial threshold)
 static int pipeline_init_state(kb_pipeline *p) {
     CK(p->d_state.alloc(1));
-    CK(p->d_res.alloc(1));
-    CK(cudaMemsetAsync(p->d_res.p, 0, sizeof(FrameResult), p->ex->stream));  // (fields a launch does not write are read back too)
-    CK(p->h_res.alloc(1));
     std::memset(&p->last, 0, sizeof(p->last));
     se3_to_matrix(se3_identity(), p->last.pose);
     se3_to_matrix(se3_identity(), p->last.delta);
@@ -1766,9 +1761,9 @@ static int pipeline_init_state(kb_pipeline *p) {
 // the buffers of a pipeline that reports fits (on the pipeline's device); the last fit becomes all zero
 static int pipeline_alloc_fit(kb_pipeline *p) {
     RET(p->fit_part.ensure(static_cast<size_t>(FIT_VALS) * p->ex->grid));
-    CK(p->fit_dev.alloc(1 + kb_pipeline::Q_DEPTH));
-    CK(cudaMemsetAsync(p->fit_dev.p, 0, sizeof(FitResult) * (1 + kb_pipeline::Q_DEPTH), p->ex->stream));
-    CK(p->fit_host.alloc(1 + kb_pipeline::Q_DEPTH));
+    CK(p->fit_dev.alloc(kb_pipeline::Q_DEPTH));
+    CK(cudaMemsetAsync(p->fit_dev.p, 0, sizeof(FitResult) * kb_pipeline::Q_DEPTH, p->ex->stream));
+    CK(p->fit_host.alloc(kb_pipeline::Q_DEPTH));
     p->last_fit = FitResult{};
     return KB_OK;
 }
@@ -1860,7 +1855,7 @@ static size_t pipeline_extra(const kb_pipeline *p, size_t n) {
 // `next_xyz` (may be null): the frame after this one, already on the device, no timestamps -> its front end is prefetched
 // `fit` (pipelines that report fits only): where the frame's fit goes
 static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, size_t n, const double *d_ts, size_t n_ts,
-                           bool in_f32, FrameResult *res, FitResult *fit, const double *next_xyz = nullptr, size_t next_n = 0) {
+                           bool in_f32, FrameResult *res, FitResult *fit, const double *next_xyz, size_t next_n) {
     Exec &ex = *p->ex;
     FrameParams P;
     P.m = p->map->view();
@@ -1950,7 +1945,7 @@ static void fit_to_abi(const FitResult &f, kb_fit *out) {
 
 enum Taken { TAKEN_ABSORBED, TAKEN_VETOED, TAKEN_SKIPPED };
 
-// take over the result `r` of frame `id` (n points in), blocking or queued, once its launch has ended:
+// take over the result `r` of frame `id` (n points in) once its launch has ended:
 // - vetoed: the table was too small and the frame modified nothing; the frames queued behind it are skipped on the
 //   device. When they have ended, the table is grown for the frame's now known voxel count and the veto is cleared:
 //   the frame can be replayed.
@@ -1963,7 +1958,7 @@ static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long
     if (r.map_status & ST_NEED_GROW) {
         *taken = TAKEN_VETOED;
         RET(p->ex->sync());
-        if (p->res_stream.p) CK(cudaStreamSynchronize(p->res_stream.p));
+        CK(cudaStreamSynchronize(p->res_stream.p));
         ++p->grow_retries;
         p->map->h_counters[C_STATUS] = 0;
         CK(cudaMemsetAsync(&p->d_state.p->vetoed, 0, sizeof(int), p->ex->stream));
@@ -1984,33 +1979,7 @@ static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long
     return KB_OK;
 }
 
-// blocking RegisterFrame on device-resident input
-static int pipeline_run(kb_pipeline *p, const double *d_xyz, size_t n, const double *d_ts, size_t n_ts, bool in_f32 = false) {
-    Exec &ex = *p->ex;
-    if (!p->localizer) RET(p->map->ensure_capacity(pipeline_extra(p, n)));
-    const long long id = p->next_id++;
-    for (int attempt = 0; attempt < 3; ++attempt) {
-        {
-            StallTrace t("blocking: launch");
-            RET(pipeline_launch(p, id, d_xyz, n, d_ts, n_ts, in_f32, p->d_res.p, p->fit_dev.p));
-        }
-        {
-            StallTrace t("blocking: result D2H enqueue");
-            CK(cudaMemcpyAsync(p->h_res.p, p->d_res.p, sizeof(FrameResult), cudaMemcpyDeviceToHost, ex.stream));
-            if (p->reports_fits()) CK(cudaMemcpyAsync(p->fit_host.p, p->fit_dev.p, sizeof(FitResult), cudaMemcpyDeviceToHost, ex.stream));
-        }
-        {
-            StallTrace t("blocking: stream sync");
-            RET(ex.sync());
-        }
-        Taken taken;
-        RET(take_result(p, *p->h_res.p, n, id, 0, nullptr, nullptr, &taken));
-        if (taken == TAKEN_ABSORBED) return KB_OK;
-        if (taken == TAKEN_SKIPPED) return fail(KB_ERR_CUDA, "the frame was skipped behind a vetoed one (internal error)");
-    }
-    return fail(KB_ERR_CUDA, "voxel table could not be grown (internal capacity bug)");
-}
-
+// ---- registration through the frame queue: a sequence, or one frame for a blocking call -----------------------
 static int pipeline_check(kb_pipeline *p, const void *xyz, size_t n, const void *ts, size_t n_ts, bool *use_ts) {
     if (!p || (!xyz && n) || (!ts && n_ts)) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (n >= (size_t(1) << 30)) return fail(KB_ERR_INVALID_ARG, "frame too large");
@@ -2021,41 +1990,6 @@ static int pipeline_check(kb_pipeline *p, const void *xyz, size_t n, const void 
     return KB_OK;
 }
 
-// the common part of kb_pipeline_register_frame[_f32|_dev]: checks, device, workspace sizing. A frame on the host
-// (elem: bytes per coordinate) and its timestamps are copied into the workspace; elem = 0: both are on the device.
-// *n_ts_used: the timestamps the frame is deskewed with (0: none).
-static int pipeline_stage(kb_pipeline *p, const void *xyz, size_t n, const double *ts, size_t n_ts, size_t elem,
-                          size_t *n_ts_used) {
-    bool use_ts;
-    RET(pipeline_check(p, xyz, n, ts, n_ts, &use_ts));
-    CK(cudaSetDevice(p->ex->device));
-    *n_ts_used = use_ts ? n_ts : 0;
-    RET(p->ws.ensure(std::max(n, *n_ts_used)));
-    RET(p->ws.ensure_pipeline(std::max(n, *n_ts_used)));
-    if (elem) {
-        StallTrace t("blocking: H2D enqueue");
-        if (n) CK(cudaMemcpyAsync(p->ws.in.p, xyz, n * 3 * elem, cudaMemcpyHostToDevice, p->ex->stream));
-        if (use_ts) CK(cudaMemcpyAsync(p->ws.ts.p, ts, n_ts * 8, cudaMemcpyHostToDevice, p->ex->stream));
-    }
-    return KB_OK;
-}
-int kb_pipeline_register_frame(kb_pipeline *p, const double *xyz, size_t n, const double *timestamps, size_t n_timestamps) {
-    size_t nt;
-    RET(pipeline_stage(p, xyz, n, timestamps, n_timestamps, sizeof(double), &nt));
-    return pipeline_run(p, p->ws.in.p, n, p->ws.ts.p, nt);
-}
-int kb_pipeline_register_frame_f32(kb_pipeline *p, const float *xyz, size_t n, const double *timestamps, size_t n_timestamps) {
-    size_t nt;
-    RET(pipeline_stage(p, xyz, n, timestamps, n_timestamps, sizeof(float), &nt));  // half the bytes of the f64 path
-    return pipeline_run(p, p->ws.in.p, n, p->ws.ts.p, nt, true);
-}
-int kb_pipeline_register_frame_dev(kb_pipeline *p, const double *d_xyz, size_t n, const double *d_timestamps,
-                                   size_t n_timestamps) {
-    size_t nt;
-    RET(pipeline_stage(p, d_xyz, n, d_timestamps, n_timestamps, 0, &nt));
-    return pipeline_run(p, d_xyz, n, d_timestamps, nt);
-}
-// ---- queued registration of a whole sequence ------------------------------------------------------------------
 static int queue_init(kb_pipeline *p, size_t max_n, bool any_ts, bool device_input) {
     if (!p->q_res_dev.p) {  // (made last: a failed first call is redone whole)
         CK(p->copy_stream.create());
@@ -2103,7 +2037,8 @@ static const char *const kNoFits =
     "fits are computed by localizers (kb_pipeline_create_localizer) and by odometry pipelines with fit reporting on "
     "(kb_pipeline_set_fit_reporting)";
 
-// kb_pipeline_register_frames[_fit]; fits_out (pipelines that report fits only, may be NULL) receives one fit per frame
+// kb_pipeline_register_frames[_fit] and, with count = 1, kb_pipeline_register_frame[_f32|_dev]; fits_out (pipelines
+// that report fits only, may be NULL) receives one fit per frame
 static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
                            const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out) {
     if (!p || (count && (!xyz || !n))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
@@ -2151,7 +2086,7 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
         return KB_OK;
     };
     auto take = [&](size_t k, Taken *taken) {  // the result of frame k, once its launch and read-back have ended
-        return take_result(p, p->q_res.p[k % D], n[k], id0 + static_cast<long long>(k), 1 + k % D,
+        return take_result(p, p->q_res.p[k % D], n[k], id0 + static_cast<long long>(k), k % D,
                            poses_out ? poses_out + 16 * k : nullptr, fits_out ? fits_out + k : nullptr, taken);
     };
     auto run = [&]() -> int {
@@ -2180,7 +2115,7 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
             {
                 StallTrace t("queue: launch");
                 RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32, p->q_res_dev.p + k % D,
-                                    p->reports_fits() ? p->fit_dev.p + 1 + k % D : nullptr, d_next, prefetch ? n[k + 1] : 0));
+                                    p->reports_fits() ? p->fit_dev.p + k % D : nullptr, d_next, prefetch ? n[k + 1] : 0));
                 CK(cudaEventRecord(s.done.p, ex.stream));
                 // result read-back on its own stream: neither the next kernel nor the next H2D waits for it (letting
                 // the kernel write to mapped host memory instead was slower)
@@ -2188,7 +2123,7 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
                 CK(cudaMemcpyAsync(p->q_res.p + k % D, p->q_res_dev.p + k % D, sizeof(FrameResult), cudaMemcpyDeviceToHost,
                                    p->res_stream.p));
                 if (p->reports_fits())
-                    CK(cudaMemcpyAsync(p->fit_host.p + 1 + k % D, p->fit_dev.p + 1 + k % D, sizeof(FitResult),
+                    CK(cudaMemcpyAsync(p->fit_host.p + k % D, p->fit_dev.p + k % D, sizeof(FitResult),
                                        cudaMemcpyDeviceToHost, p->res_stream.p));
                 CK(cudaEventRecord(s.read.p, p->res_stream.p));
             }
@@ -2244,6 +2179,20 @@ int kb_pipeline_register_frames_fit(kb_pipeline *p, const void *const *xyz, cons
                                     const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out) {
     if (p && fits_out && !p->reports_fits()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
     return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out);
+}
+// a blocking call is a queue of one frame: there is no frame after it, so its front end runs in its own launch
+int kb_pipeline_register_frame(kb_pipeline *p, const double *xyz, size_t n, const double *timestamps, size_t n_timestamps) {
+    const void *x = xyz;
+    return register_frames(p, &x, &n, &timestamps, &n_timestamps, 1, KB_FRAMES_HOST_F64, nullptr, nullptr);
+}
+int kb_pipeline_register_frame_f32(kb_pipeline *p, const float *xyz, size_t n, const double *timestamps, size_t n_timestamps) {
+    const void *x = xyz;
+    return register_frames(p, &x, &n, &timestamps, &n_timestamps, 1, KB_FRAMES_HOST_F32, nullptr, nullptr);
+}
+int kb_pipeline_register_frame_dev(kb_pipeline *p, const double *d_xyz, size_t n, const double *d_timestamps,
+                                   size_t n_timestamps) {
+    const void *x = d_xyz;
+    return register_frames(p, &x, &n, &d_timestamps, &n_timestamps, 1, KB_FRAMES_DEVICE_F64, nullptr, nullptr);
 }
 int kb_pipeline_last_fit(const kb_pipeline *p, kb_fit *out) {
     if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
