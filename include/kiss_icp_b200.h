@@ -329,6 +329,38 @@ int kb_pipeline_set_fit_reporting(kb_pipeline *p, int enabled);
 /* *out = 1 if the pipeline reports fits (a localizer, or fit reporting on), else 0; KB_ERR_INVALID_ARG for NULL */
 int kb_pipeline_fit_reporting(const kb_pipeline *p, int *out);
 
+/* ---- plane constraints: which directions a registration pins down ---------------------------
+ * No reference counterpart. For every correspondence of the fit (source point p = pose * s, nearest map neighbour q
+ * closer than max_correspondence_distance) whose voxel (q's own) holds m >= 3 points: the voxel's mean and covariance
+ * C (1/m), n = a unit eigenvector of C's smallest eigenvalue l0 (l0 <= l1 <= l2), planarity a = (l1 - l0) / l2 (0 when
+ * l2 = 0), residual e = n.(p - q) and Jacobian J = [n^T, (p x n)^T] in the tangent order (translation, rotation) of
+ * kb_fit.JTJ. The information matrix is a sum of rank-one terms a J^T J: a direction no plane faces has no
+ * information. Bit-identical from run to run for a given grid size (kb_set_grid_blocks). */
+typedef struct kb_constraints {
+    int n_planes;                   /* correspondences whose map voxel holds >= 3 points                */
+    double weight_sum;              /* sum of planarity weights a_i                                     */
+    double sum_sq_plane_residual;   /* sum a_i e_i^2                                                    */
+    double information[36];         /* sum a_i J_i^T J_i, row-major, symmetric, (translation, rotation) */
+} kb_constraints;
+/* one source (host xyz[n][3]) at one pose against a map. Read-only: allowed while localizers hold the map.
+ * KB_ERR_INVALID_ARG for a NULL argument, KB_ERR_NOT_SE3 for a pose outside SE(3); n = 0 or an empty map gives zeros. */
+int kb_registration_constraints(kb_registration *reg, const double *xyz, size_t n, const kb_map *map,
+                                const double pose[16], double max_correspondence_distance, kb_constraints *out);
+/* Plane-constraint reporting (off when a pipeline is created): every registered frame also gets a kb_constraints, of
+ * the fit's correspondences (3 sigma at the final pose, against the map the fit is against: for odometry, before the
+ * frame's own update). Needs a pipeline that reports fits (a localizer, or kb_pipeline_set_fit_reporting on), else
+ * KB_ERR_INVALID_ARG and nothing changes. Enabling allocates its buffers and zeroes the last result, enabling again is a
+ * no-op, 0 releases them. While it is on, kb_pipeline_set_fit_reporting(p, 0) is KB_ERR_INVALID_ARG. Poses, fits and
+ * the map are bit for bit those of reporting off; the frames run a kernel of their own. */
+int kb_pipeline_set_constraint_reporting(kb_pipeline *p, int enabled);
+/* the plane constraints of the last frame (zeros before the first); KB_ERR_INVALID_ARG when reporting is off */
+int kb_pipeline_last_constraints(const kb_pipeline *p, kb_constraints *out);
+/* kb_pipeline_register_frames_fit with one kb_constraints per frame in constraints_out[count] (may be NULL; non-NULL
+ * without constraint reporting is KB_ERR_INVALID_ARG). A frame vetoed for table capacity gets its replay's. */
+int kb_pipeline_register_frames_constraints(kb_pipeline *p, const void *const *xyz, const size_t *n,
+                                            const double *const *timestamps, const size_t *n_timestamps, size_t count,
+                                            int layout, double *poses_out, kb_fit *fits_out, kb_constraints *constraints_out);
+
 /* ---- relocalization: a global pose search in a bounded region ----------------------------
  * No reference counterpart. Finds a scan's pose in a map without an initial pose: every hypothesis of a grid in x, y
  * and yaw around a centre is scored on the device, the best peaks are refined with kb_registration_align_batch, and

@@ -19,6 +19,9 @@ int kb_debug_barrier_ns(int iters, double *ns_per_barrier);
 /* host evaluation of the ICP loop's structured (Schur complement) solve vs the pivoted LDL^T it falls back to, on the
  * same 16 accumulators {sum w, sum w*s (3), lower triangle of sum w*hat(s)^T*hat(s) (6), JTr (6)} */
 int kb_debug_icp_schur(const double acc[16], double x_schur[6], double x_ldlt[6], int *used_schur);
+/* host evaluation of the symmetric 3x3 eigen-solver of the plane constraints (cyclic Jacobi): c = (xx, xy, xz, yy, yz, zz),
+ * eigenvalues ascending, eigenvectors[3 k .. 3 k + 2] = unit eigenvector of eigenvalues[k] */
+int kb_debug_sym3_eig(const double c[6], double eigenvalues[3], double eigenvectors[9]);
 /* host evaluation of the latency-optimised (reciprocal / sincos) ICP solve step the kernels run:
  * x = LDLT solve, T = exp(x) * exp(b) */
 int kb_debug_icp_solve_fast(const double A[36], const double b[6], double x_fast[6], double T_fast[16]);

@@ -41,12 +41,13 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/api.cu, csrc/localize.cu, csrc/odometry_fit.cu, csrc/probe.cu and csrc/relocalize.cu
+    """Compile csrc/api.cu, csrc/localize.cu, csrc/odometry_fit.cu, csrc/constraints.cu, csrc/probe.cu and csrc/relocalize.cu
     -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in sources())
     if force or stale:
         cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH,
-               *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "odometry_fit.cu", "probe.cu", "relocalize.cu"))]
+               *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "odometry_fit.cu", "constraints.cu", "probe.cu",
+                                                       "relocalize.cu"))]
         if verbose:
             print(" ".join(cmd))
         env = dict(os.environ)
@@ -92,6 +93,11 @@ class PipelineState(C.Structure):
 class Fit(C.Structure):
     """kb_fit: the fit of one localized frame at its final pose"""
     _fields_ = [("n_correspondences", i32), ("n_source", i32), ("sum_sq_residual", dbl), ("JTJ", dbl * 36)]
+
+
+class Constraints(C.Structure):
+    """kb_constraints: the plane constraints of one source at one pose"""
+    _fields_ = [("n_planes", i32), ("weight_sum", dbl), ("sum_sq_plane_residual", dbl), ("information", dbl * 36)]
 
 
 class RelocSearch(C.Structure):
@@ -203,6 +209,11 @@ SIGNATURES = {
     "kb_reloc_hypotheses": (i32, [C.POINTER(RelocSearch), vp, sz, C.POINTER(sz)]),
     "kb_relocalize": (i32, [vp, vp, sz, vp, C.POINTER(RelocSearch), C.POINTER(RelocResult), vp, vp, vp]),
     "kb_debug_reloc_score_ms": (i32, [vp, C.POINTER(C.c_float)]),
+    "kb_registration_constraints": (i32, [vp, vp, sz, vp, vp, dbl, C.POINTER(Constraints)]),
+    "kb_pipeline_set_constraint_reporting": (i32, [vp, i32]),
+    "kb_pipeline_last_constraints": (i32, [vp, C.POINTER(Constraints)]),
+    "kb_pipeline_register_frames_constraints": (i32, [vp, vp, vp, vp, vp, sz, i32, vp, vp, vp]),
+    "kb_debug_sym3_eig": (i32, [vp, vp, vp]),
 }
 
 

@@ -92,6 +92,7 @@ int watchdog_init(int device) {
     CK(cudaMemcpyToSymbol(g_kb_wd, init, sizeof(init)));
     CK(localize_watchdog_init(d, init));  // the localizer kernel's module has its own copies
     CK(odometry_fit_watchdog_init(d, init));  // and so has the fit-reporting odometry kernel's
+    CK(constraints_watchdog_init(d, init));   // and the module of the plane-constraint kernels
     g_wd[device].host = h;
     return KB_OK;
 }
@@ -115,6 +116,7 @@ int watchdog_check(int device) {
     cudaMemcpyToSymbol(g_kb_wd, &zero, sizeof(zero));  // re-arm
     localize_watchdog_rearm();
     odometry_fit_watchdog_rearm();
+    constraints_watchdog_rearm();
     static const char *names[] = {"?", "grid barrier", "ICP gather", "ICP result record", "ICP team gather", "NN bulk copy"};
     std::string marks;
     unsigned m[256];
@@ -686,6 +688,8 @@ struct kb_registration {
     DBuf<int> biout;
     DBuf<double> rgrid;   // kb_relocalize: rotations [n_yaw][9], then xs [Nx], ys [Ny]
     DBuf<int> rscore;     // kb_relocalize: scores [H]
+    DBuf<double> plane_part;      // kb_registration_constraints: [PLANE_VALS][grid] per-CTA partials
+    DBuf<PlaneResult> plane_res;  // and the result
     Event rev[2];  // around the last k_reloc_score (kb_debug_reloc_score_ms), on the device of that call
 };
 
@@ -714,6 +718,13 @@ struct kb_pipeline {
     DBuf<FitResult> fit_dev;         // [Q_DEPTH]
     PinBuf<FitResult> fit_host;      // [Q_DEPTH] copies
     FitResult last_fit{};
+    // a pipeline that reports fits may also report plane constraints (kb_pipeline_set_constraint_reporting): one result
+    // per frame into plane_dev[k % Q_DEPTH], next to the fit
+    bool constraint_reporting = false;
+    DBuf<double> plane_part;          // [PLANE_VALS][grid] per-CTA partials of the plane pass
+    DBuf<PlaneResult> plane_dev;      // [Q_DEPTH]
+    PinBuf<PlaneResult> plane_host;   // [Q_DEPTH] copies
+    PlaneResult last_planes{};
     Work ws;
     DBuf<PipeState> d_state;
     FrameResult last{};
@@ -1169,6 +1180,44 @@ int kb_registration_align_points_to_map(kb_registration *reg, const double *xyz,
     CK(cudaMemcpyAsync(&it, reg->iout.p, sizeof(int), cudaMemcpyDeviceToHost, map->ex->stream));
     RET(map->ex->sync());
     reg->last_iters = it;
+    return KB_OK;
+}
+// the upper triangle of the plane information matrix expanded to the symmetric 6x6
+static void planes_to_abi(const PlaneResult &r, kb_constraints *out) {
+    out->n_planes = r.n_planes;
+    out->weight_sum = r.weight_sum;
+    out->sum_sq_plane_residual = r.sse;
+    for (int i = 0, k = 0; i < 6; ++i)
+        for (int j = i; j < 6; ++j, ++k) out->information[6 * i + j] = out->information[6 * j + i] = r.info[k];
+}
+int kb_registration_constraints(kb_registration *reg, const double *xyz, size_t n, const kb_map *cmap, const double pose[16],
+                                double max_correspondence_distance, kb_constraints *out) {
+    kb_map *map = const_cast<kb_map *>(cmap);
+    if (!reg || !map || (!xyz && n) || !pose || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    SE3 T;
+    if (!se3_from_matrix(pose, &T)) return fail(KB_ERR_NOT_SE3, "pose is not in SE(3)");
+    if (n > static_cast<size_t>(INT_MAX)) return fail(KB_ERR_INVALID_ARG, "more than 2^31 - 1 source points");
+    *out = kb_constraints{};
+    if (n == 0) return KB_OK;
+    Exec &ex = *map->ex;
+    CK(cudaSetDevice(ex.device));
+    RET(reg->ws.src.ensure(3 * n));
+    RET(reg->plane_part.ensure(static_cast<size_t>(PLANE_VALS) * ex.grid));
+    RET(reg->plane_res.ensure(1));
+    CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
+    ConstraintsParams P{};
+    P.m = map->view();
+    P.sc = ex.sc;
+    P.src = reg->ws.src.p;
+    P.n = static_cast<int>(n);
+    P.pose = T;
+    P.max_dist = max_correspondence_distance;
+    P.planes = PlaneOut{reg->plane_part.p, reg->plane_res.p};
+    RET(ex.coop_raw(constraints_kernel(), &P, 0, true));
+    PlaneResult r;
+    CK(cudaMemcpyAsync(&r, reg->plane_res.p, sizeof(r), cudaMemcpyDeviceToHost, ex.stream));
+    RET(ex.sync());
+    planes_to_abi(r, out);
     return KB_OK;
 }
 int kb_registration_last_iterations(const kb_registration *reg, int *out) {
@@ -1772,6 +1821,20 @@ static void pipeline_free_fit(kb_pipeline *p) {
     p->fit_dev = DBuf<FitResult>{};
     p->fit_host = PinBuf<FitResult>{};
 }
+// likewise for the plane constraints
+static int pipeline_alloc_planes(kb_pipeline *p) {
+    RET(p->plane_part.ensure(static_cast<size_t>(PLANE_VALS) * p->ex->grid));
+    CK(p->plane_dev.alloc(kb_pipeline::Q_DEPTH));
+    CK(cudaMemsetAsync(p->plane_dev.p, 0, sizeof(PlaneResult) * kb_pipeline::Q_DEPTH, p->ex->stream));
+    CK(p->plane_host.alloc(kb_pipeline::Q_DEPTH));
+    p->last_planes = PlaneResult{};
+    return KB_OK;
+}
+static void pipeline_free_planes(kb_pipeline *p) {
+    p->plane_part = DBuf<double>{};
+    p->plane_dev = DBuf<PlaneResult>{};
+    p->plane_host = PinBuf<PlaneResult>{};
+}
 
 int kb_pipeline_create(const kb_config *cfg, kb_pipeline **out) {
     if (!cfg || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
@@ -1853,9 +1916,11 @@ static size_t pipeline_extra(const kb_pipeline *p, size_t n) {
 
 // enqueue one RegisterFrame on the pipeline's stream; the result goes to `res` (device-visible memory)
 // `next_xyz` (may be null): the frame after this one, already on the device, no timestamps -> its front end is prefetched
-// `fit` (pipelines that report fits only): where the frame's fit goes
+// `fit` (pipelines that report fits only): where the frame's fit goes; `planes` (pipelines that report plane
+// constraints only): where its plane constraints go
 static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, size_t n, const double *d_ts, size_t n_ts,
-                           bool in_f32, FrameResult *res, FitResult *fit, const double *next_xyz, size_t next_n) {
+                           bool in_f32, FrameResult *res, FitResult *fit, PlaneResult *planes, const double *next_xyz,
+                           size_t next_n) {
     Exec &ex = *p->ex;
     FrameParams P;
     P.m = p->map->view();
@@ -1885,6 +1950,20 @@ static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, si
     P.tag_base = ex.next_tag_base();
     P.in_f32 = in_f32 ? 1 : 0;
     const size_t smem = std::max<size_t>(QC_BYTES, ex.icp_smem);
+    if (p->constraint_reporting) {  // (a localizer, or fit reporting on)
+        if (p->localizer) {
+            LocalizeConstraintParams L;
+            static_cast<FrameParams &>(L) = P;
+            L.fit = FitOut{p->fit_part.p, fit};
+            L.planes = PlaneOut{p->plane_part.p, planes};
+            return ex.coop_raw(localize_constraints_kernel(), &L, smem, true);
+        }
+        OdometryConstraintParams F;
+        static_cast<FrameParams &>(F) = P;
+        F.fit = FitOut{p->fit_part.p, fit};
+        F.planes = PlaneOut{p->plane_part.p, planes};
+        return ex.coop_raw(odometry_constraints_kernel(), &F, smem, true);
+    }
     if (p->localizer) {
         LocalizeParams L;
         static_cast<FrameParams &>(L) = P;
@@ -1951,9 +2030,10 @@ enum Taken { TAKEN_ABSORBED, TAKEN_VETOED, TAKEN_SKIPPED };
 //   the frame can be replayed.
 // - skipped: the frame did not run.
 // - absorbed: pipeline_absorb; the pose goes to pose_out, and the fit of a pipeline that reports fits (pinned copy
-//   `fit_slot`) becomes the last one and goes to fit_out (either may be null).
+//   `fit_slot`) becomes the last one and goes to fit_out (either may be null); so do its plane constraints when it
+//   reports them (constraints_out).
 static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long id, size_t fit_slot, double *pose_out,
-                       kb_fit *fit_out, Taken *taken) {
+                       kb_fit *fit_out, kb_constraints *constraints_out, Taken *taken) {
     RET(watchdog_check(p->ex->device));  // (a spin loop that gave up invalidates the launch)
     if (r.map_status & ST_NEED_GROW) {
         *taken = TAKEN_VETOED;
@@ -1975,6 +2055,10 @@ static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long
     if (p->reports_fits()) {
         p->last_fit = p->fit_host.p[fit_slot];
         if (fit_out) fit_to_abi(p->last_fit, fit_out);
+    }
+    if (p->constraint_reporting) {
+        p->last_planes = p->plane_host.p[fit_slot];
+        if (constraints_out) planes_to_abi(p->last_planes, constraints_out);
     }
     return KB_OK;
 }
@@ -2037,10 +2121,15 @@ static const char *const kNoFits =
     "fits are computed by localizers (kb_pipeline_create_localizer) and by odometry pipelines with fit reporting on "
     "(kb_pipeline_set_fit_reporting)";
 
-// kb_pipeline_register_frames[_fit] and, with count = 1, kb_pipeline_register_frame[_f32|_dev]; fits_out (pipelines
-// that report fits only, may be NULL) receives one fit per frame
+static const char *const kNoConstraints =
+    "plane constraints are reported by pipelines with kb_pipeline_set_constraint_reporting on";
+
+// kb_pipeline_register_frames[_fit|_constraints] and, with count = 1, kb_pipeline_register_frame[_f32|_dev]; fits_out
+// (pipelines that report fits only, may be NULL) receives one fit per frame, constraints_out (pipelines that report
+// plane constraints only, may be NULL) one kb_constraints per frame
 static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
-                           const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out) {
+                           const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out,
+                           kb_constraints *constraints_out) {
     if (!p || (count && (!xyz || !n))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (layout != KB_FRAMES_HOST_F64 && layout != KB_FRAMES_HOST_F32 && layout != KB_FRAMES_DEVICE_F64)
         return fail(KB_ERR_INVALID_ARG, "unknown frame layout %d", layout);
@@ -2087,7 +2176,8 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
     };
     auto take = [&](size_t k, Taken *taken) {  // the result of frame k, once its launch and read-back have ended
         return take_result(p, p->q_res.p[k % D], n[k], id0 + static_cast<long long>(k), k % D,
-                           poses_out ? poses_out + 16 * k : nullptr, fits_out ? fits_out + k : nullptr, taken);
+                           poses_out ? poses_out + 16 * k : nullptr, fits_out ? fits_out + k : nullptr,
+                           constraints_out ? constraints_out + k : nullptr, taken);
     };
     auto run = [&]() -> int {
     while (next_absorb < valid) {
@@ -2115,7 +2205,8 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
             {
                 StallTrace t("queue: launch");
                 RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32, p->q_res_dev.p + k % D,
-                                    p->reports_fits() ? p->fit_dev.p + k % D : nullptr, d_next, prefetch ? n[k + 1] : 0));
+                                    p->reports_fits() ? p->fit_dev.p + k % D : nullptr,
+                                    p->constraint_reporting ? p->plane_dev.p + k % D : nullptr, d_next, prefetch ? n[k + 1] : 0));
                 CK(cudaEventRecord(s.done.p, ex.stream));
                 // result read-back on its own stream: neither the next kernel nor the next H2D waits for it (letting
                 // the kernel write to mapped host memory instead was slower)
@@ -2124,6 +2215,9 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
                                    p->res_stream.p));
                 if (p->reports_fits())
                     CK(cudaMemcpyAsync(p->fit_host.p + k % D, p->fit_dev.p + k % D, sizeof(FitResult),
+                                       cudaMemcpyDeviceToHost, p->res_stream.p));
+                if (p->constraint_reporting)
+                    CK(cudaMemcpyAsync(p->plane_host.p + k % D, p->plane_dev.p + k % D, sizeof(PlaneResult),
                                        cudaMemcpyDeviceToHost, p->res_stream.p));
                 CK(cudaEventRecord(s.read.p, p->res_stream.p));
             }
@@ -2173,26 +2267,33 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
 }
 int kb_pipeline_register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
                                 const size_t *n_timestamps, size_t count, int layout, double *poses_out) {
-    return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, nullptr);
+    return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, nullptr, nullptr);
 }
 int kb_pipeline_register_frames_fit(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
                                     const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out) {
     if (p && fits_out && !p->reports_fits()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
-    return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out);
+    return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out, nullptr);
+}
+int kb_pipeline_register_frames_constraints(kb_pipeline *p, const void *const *xyz, const size_t *n,
+                                            const double *const *timestamps, const size_t *n_timestamps, size_t count,
+                                            int layout, double *poses_out, kb_fit *fits_out, kb_constraints *constraints_out) {
+    if (p && fits_out && !p->reports_fits()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
+    if (p && constraints_out && !p->constraint_reporting) return fail(KB_ERR_INVALID_ARG, "%s", kNoConstraints);
+    return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out, constraints_out);
 }
 // a blocking call is a queue of one frame: there is no frame after it, so its front end runs in its own launch
 int kb_pipeline_register_frame(kb_pipeline *p, const double *xyz, size_t n, const double *timestamps, size_t n_timestamps) {
     const void *x = xyz;
-    return register_frames(p, &x, &n, &timestamps, &n_timestamps, 1, KB_FRAMES_HOST_F64, nullptr, nullptr);
+    return register_frames(p, &x, &n, &timestamps, &n_timestamps, 1, KB_FRAMES_HOST_F64, nullptr, nullptr, nullptr);
 }
 int kb_pipeline_register_frame_f32(kb_pipeline *p, const float *xyz, size_t n, const double *timestamps, size_t n_timestamps) {
     const void *x = xyz;
-    return register_frames(p, &x, &n, &timestamps, &n_timestamps, 1, KB_FRAMES_HOST_F32, nullptr, nullptr);
+    return register_frames(p, &x, &n, &timestamps, &n_timestamps, 1, KB_FRAMES_HOST_F32, nullptr, nullptr, nullptr);
 }
 int kb_pipeline_register_frame_dev(kb_pipeline *p, const double *d_xyz, size_t n, const double *d_timestamps,
                                    size_t n_timestamps) {
     const void *x = d_xyz;
-    return register_frames(p, &x, &n, &d_timestamps, &n_timestamps, 1, KB_FRAMES_DEVICE_F64, nullptr, nullptr);
+    return register_frames(p, &x, &n, &d_timestamps, &n_timestamps, 1, KB_FRAMES_DEVICE_F64, nullptr, nullptr, nullptr);
 }
 int kb_pipeline_last_fit(const kb_pipeline *p, kb_fit *out) {
     if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
@@ -2203,6 +2304,8 @@ int kb_pipeline_last_fit(const kb_pipeline *p, kb_fit *out) {
 int kb_pipeline_set_fit_reporting(kb_pipeline *p, int enabled) {
     if (!p) return fail(KB_ERR_INVALID_ARG, "p == NULL");
     if (p->localizer) return enabled ? KB_OK : fail(KB_ERR_INVALID_ARG, "a localizer always reports fits");
+    if (!enabled && p->constraint_reporting)
+        return fail(KB_ERR_INVALID_ARG, "plane constraint reporting needs the fits: turn it off first");
     if (!enabled) {
         p->fit_reporting = false;
         pipeline_free_fit(p);  // (no launch of this pipeline is in flight between calls)
@@ -2216,6 +2319,32 @@ int kb_pipeline_set_fit_reporting(kb_pipeline *p, int enabled) {
         return st;
     }
     p->fit_reporting = true;
+    return KB_OK;
+}
+int kb_pipeline_set_constraint_reporting(kb_pipeline *p, int enabled) {
+    if (!p) return fail(KB_ERR_INVALID_ARG, "p == NULL");
+    if (!enabled) {
+        p->constraint_reporting = false;
+        pipeline_free_planes(p);  // (no launch of this pipeline is in flight between calls)
+        return KB_OK;
+    }
+    if (!p->reports_fits())
+        return fail(KB_ERR_INVALID_ARG, "plane constraints are reported next to the fit: a localizer, or an odometry pipeline "
+                                        "with kb_pipeline_set_fit_reporting on");
+    if (p->constraint_reporting) return KB_OK;
+    CK(cudaSetDevice(p->ex->device));
+    const int st = pipeline_alloc_planes(p);
+    if (st != KB_OK) {
+        pipeline_free_planes(p);
+        return st;
+    }
+    p->constraint_reporting = true;
+    return KB_OK;
+}
+int kb_pipeline_last_constraints(const kb_pipeline *p, kb_constraints *out) {
+    if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (!p->constraint_reporting) return fail(KB_ERR_INVALID_ARG, "%s", kNoConstraints);
+    planes_to_abi(p->last_planes, out);
     return KB_OK;
 }
 int kb_pipeline_fit_reporting(const kb_pipeline *p, int *out) {
@@ -2366,6 +2495,17 @@ int kb_debug_icp_solve_fast(const double A[36], const double b[6], double x_fast
     if (!A || !b || !x_fast || !T_fast) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     ldlt6_solve_fast(A, b, x_fast);
     se3_to_matrix(se3_mul_fast(se3_exp_fast(x_fast), se3_exp(b)), T_fast);
+    return KB_OK;
+}
+int kb_debug_sym3_eig(const double c[6], double eigenvalues[3], double eigenvectors[9]) {
+    if (!c || !eigenvalues || !eigenvectors) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    V3 v[3];
+    sym3_eig(c, eigenvalues, v);
+    for (int k = 0; k < 3; ++k) {
+        eigenvectors[3 * k] = v[k].x;
+        eigenvectors[3 * k + 1] = v[k].y;
+        eigenvectors[3 * k + 2] = v[k].z;
+    }
     return KB_OK;
 }
 int kb_debug_icp_schur(const double acc[16], double x_schur[6], double x_ldlt[6], int *used_schur) {

@@ -1,7 +1,7 @@
 // KissICP::RegisterFrame as one persistent kernel (k_register_frame) and what it works on. A header of its own:
-// the odometry instantiation is compiled with the other kernels (api.cu), the localizer's and the fit-reporting
-// odometry's each in a translation unit of its own (localize.cu, odometry_fit.cu), so that none changes the code
-// generated for another.
+// the odometry instantiation is compiled with the other kernels (api.cu), the localizer's, the fit-reporting
+// odometry's and the two plane-constraint-reporting ones each in a translation unit of their own (localize.cu,
+// odometry_fit.cu, constraints.cu), so that none changes the code generated for another.
 #pragma once
 
 #include <type_traits>
@@ -191,6 +191,167 @@ __device__ __forceinline__ void fit_finish(const FitOut &fit, int n_src) {
     }
 }
 
+// ---- the plane constraints of a frame (kb_registration_constraints, kb_pipeline_set_constraint_reporting) ------------
+// For every correspondence of the fit (nearest neighbour q closer than max_dist to p = pose * s) with at least 3 points in
+// q's own voxel: mean and covariance C of the voxel's points (two passes), n = the eigenvector of C's smallest
+// eigenvalue, planarity a = (l1 - l0) / l2 (0 when l2 = 0), e = n.(p - q), J = [n, p x n]. Accumulated: the count,
+// sum a, sum a e^2 and the 21 entries of sum a J^T J on and above the diagonal (row-major). Same split and order as the
+// fit: a lane sums its warp's correspondences in order, the warps are added in warp order, the CTA partials in CTA order.
+constexpr int PLANE_VALS = 3 + 21;  // count, sum a, sum a e^2, upper triangle of sum a J^T J
+struct PlaneResult {
+    double info[21];  // upper triangle, row-major: (0,0), (0,1), ..., (0,5), (1,1), ..., (5,5)
+    double weight_sum, sse;
+    int n_planes, pad;
+};
+struct PlaneOut {
+    double *part;      // [PLANE_VALS][grid] per-CTA partials (value-major)
+    PlaneResult *res;  // this frame's result
+};
+// a localizer / a fit-reporting odometry pipeline that also reports plane constraints
+struct LocalizeConstraintParams : FrameParams {
+    FitOut fit;
+    PlaneOut planes;
+};
+struct OdometryConstraintParams : FrameParams {
+    FitOut fit;
+    PlaneOut planes;
+};
+// the stand-alone pass (k_constraints): one source at one pose
+struct ConstraintsParams {
+    MapView m;
+    Scratch sc;
+    const double *src;
+    int n;
+    SE3 pose;
+    double max_dist;
+    PlaneOut planes;
+};
+
+__device__ __forceinline__ double warp_sum(double v) {  // fixed butterfly: every lane ends with the same bits
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+    return v;
+}
+
+// the plane term of one correspondence (p, q) for this lane's value (lane < PLANE_VALS; warp-uniform arguments)
+__device__ __forceinline__ double plane_term(const MapView &m, const V3 &p, const V3 &q, int lane, int ji, int jj) {
+    const int3 v = point_to_voxel(q.x, q.y, q.z, m.vdiv);
+    int cnt = 0;
+    const int slot = map_find(m, v.x, v.y, v.z, &cnt);  // q is stored in this voxel: found
+    if (slot < 0 || cnt < 3) return 0.0;
+    const double *blk = m.points + static_cast<size_t>(slot) * m.cap * 3;
+    double sx = 0.0, sy = 0.0, sz = 0.0;
+    for (int k = lane; k < cnt; k += 32) {
+        sx += blk[3 * k];
+        sy += blk[3 * k + 1];
+        sz += blk[3 * k + 2];
+    }
+    const double inv_m = 1.0 / static_cast<double>(cnt);
+    const V3 mu{warp_sum(sx) * inv_m, warp_sum(sy) * inv_m, warp_sum(sz) * inv_m};
+    double c[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int k = lane; k < cnt; k += 32) {  // (the block is L1-hot from the first pass)
+        const V3 d = V3{blk[3 * k], blk[3 * k + 1], blk[3 * k + 2]} - mu;
+        c[0] += d.x * d.x;
+        c[1] += d.x * d.y;
+        c[2] += d.x * d.z;
+        c[3] += d.y * d.y;
+        c[4] += d.y * d.z;
+        c[5] += d.z * d.z;
+    }
+#pragma unroll
+    for (int i = 0; i < 6; ++i) c[i] = warp_sum(c[i]) * inv_m;
+    double lam[3];
+    V3 ev[3];
+    sym3_eig(c, lam, ev);  // every lane solves the same system (uniform: no broadcast needed)
+    const double a = lam[2] > 0.0 ? (lam[1] - lam[0]) / lam[2] : 0.0;
+    const V3 n = ev[0];
+    const V3 r = p - q;
+    const double e = (n.x * r.x + n.y * r.y) + n.z * r.z;
+    const V3 pn = cross(p, n);
+    const double J[6] = {n.x, n.y, n.z, pn.x, pn.y, pn.z};
+    double Ji = 0.0, Jj = 0.0;
+#pragma unroll
+    for (int i = 0; i < 6; ++i) {
+        Ji = (ji == i) ? J[i] : Ji;
+        Jj = (jj == i) ? J[i] : Jj;
+    }
+    if (lane == 0) return 1.0;
+    if (lane == 1) return a;
+    if (lane == 2) return a * (e * e);
+    return a * (Ji * Jj);
+}
+
+// the fit (FIT: op_fit's values into fit_part, the same operations in the same order) and the plane constraints of
+// the same correspondences into plane_part, from one nearest-neighbour search per source point. The caller provides the
+// grid barrier behind it.
+template <bool FIT>
+__device__ __noinline__ void op_fit_planes(Shared &sh, const MapView &m, const double *src, int n, const SE3 &pose,
+                                           double max_dist, double kscale, double *fit_part, double *plane_part) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int G = static_cast<int>(gridDim.x);
+    // this lane's Jacobian pair (lanes 3..23: the upper triangle, row-major)
+    int ji = 0, jj = 0;
+    for (int t = lane - 3, row = 0; t >= 0 && row < 6; t -= 6 - row, ++row)
+        if (t < 6 - row) {
+            ji = row;
+            jj = row + t;
+        }
+    double acc = 0.0, sse = 0.0, pacc = 0.0;
+    int corr = 0;
+    for (int qi = static_cast<int>(blockIdx.x) + G * warp; qi < n; qi += G * NWARPS) {
+        const V3 p = se3_act(pose, V3{src[3 * qi], src[3 * qi + 1], src[3 * qi + 2]});
+        const NNResult r = nn_search_warp(m, p, lane, sh.wnn[warp]);
+        if (r.d < max_dist) {
+            if constexpr (FIT) {
+                acc += icp_term(lane, p, r.p, kscale);
+                sse += sqnorm(p - r.p);
+                ++corr;
+            }
+            pacc += plane_term(m, p, r.p, lane, ji, jj);
+        }
+    }
+    // (chunk_pref is free here: the ICP loop and the front end are done)
+    double(*pw)[PLANE_VALS] = reinterpret_cast<double(*)[PLANE_VALS]>(sh.chunk_pref);
+    if constexpr (FIT) {
+        if (lane < NACC) sh.warp_d[warp][lane] = acc;
+        if (lane == NACC) sh.warp_d[warp][NACC] = static_cast<double>(corr);
+        if (lane == NACC + 1) sh.warp_d[warp][NACC + 1] = sse;
+    }
+    if (lane < PLANE_VALS) pw[warp][lane] = pacc;
+    __syncthreads();
+    if constexpr (FIT) {
+        if (threadIdx.x < FIT_VALS) {
+            double v = 0.0;
+            for (int w = 0; w < NWARPS; ++w) v += sh.warp_d[w][threadIdx.x];
+            fit_part[threadIdx.x * G + static_cast<int>(blockIdx.x)] = v;
+        }
+    }
+    const int t = static_cast<int>(threadIdx.x) - 32;
+    if (t >= 0 && t < PLANE_VALS) {
+        double v = 0.0;
+        for (int w = 0; w < NWARPS; ++w) v += pw[w][t];
+        plane_part[t * G + static_cast<int>(blockIdx.x)] = v;
+    }
+}
+
+// after the barrier behind op_fit_planes: one CTA adds the partials in CTA order (threads 32..55, next to fit_finish's)
+__device__ __forceinline__ void planes_finish(const PlaneOut &pl) {
+    const int G = static_cast<int>(gridDim.x);
+    const int t = static_cast<int>(threadIdx.x) - 32;
+    if (t >= 0 && t < PLANE_VALS) {
+        double v = 0.0;
+        for (int c = 0; c < G; ++c) v += __ldcg(&pl.part[t * G + c]);
+        if (t == 0)
+            pl.res->n_planes = static_cast<int>(v);
+        else if (t == 1)
+            pl.res->weight_sum = v;
+        else if (t == 2)
+            pl.res->sse = v;
+        else
+            pl.res->info[t - 3] = v;
+    }
+}
+
 // ---- KissICP::RegisterFrame (pipeline/KissICP.cpp:35-68) as ONE persistent kernel ----------
 //   [front end of this frame, unless a previous launch prefetched it]
 //   capacity check | fill pass (all CTAs) | ICP iterations on the team  ||  front end of the NEXT frame on the rest
@@ -200,10 +361,16 @@ __device__ __forceinline__ void fit_finish(const FitOut &fit, int n_src) {
 // fit pass (op_fit) at the final pose. Nothing writes to the map.
 // k_register_frame<OdometryFitParams>: the odometry statement with the fit pass at the final pose in front of the map
 // update, and one grid barrier between them (op_fit reads the table op_map_add writes).
+// k_register_frame<LocalizeConstraintParams> / <OdometryConstraintParams>: the same, with op_fit_planes in place of
+// op_fit (the same fit, plus the plane constraints of its correspondences) and planes_finish next to fit_finish.
 template <class Params>
 __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
-    constexpr bool LOCALIZE = std::is_same<Params, LocalizeParams>::value;
-    constexpr bool ODOMETRY_FIT = std::is_same<Params, OdometryFitParams>::value;
+    constexpr bool PLANES = std::is_same<Params, LocalizeConstraintParams>::value ||
+                            std::is_same<Params, OdometryConstraintParams>::value;
+    constexpr bool LOCALIZE = std::is_same<Params, LocalizeParams>::value ||
+                              std::is_same<Params, LocalizeConstraintParams>::value;
+    constexpr bool ODOMETRY_FIT = std::is_same<Params, OdometryFitParams>::value ||
+                                  std::is_same<Params, OdometryConstraintParams>::value;
     __shared__ Shared sh;
     Grid g;
     g.init(P.sc.bar);
@@ -331,14 +498,20 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
     }
     if constexpr (LOCALIZE) {
         // the fit at the final pose, with this frame's (3 sigma, sigma)
-        op_fit(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part);
+        if constexpr (PLANES)
+            op_fit_planes<true>(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part, P.planes.part);
+        else
+            op_fit(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part);
         kb_mark(0x700u);
     } else {
         if constexpr (ODOMETRY_FIT) {
             // the fit at the final pose, with this frame's (3 sigma, sigma), against the map before local_map_.Update
             // (after it, the frame's own points would be in the map). Stamps: the pass including the barrier behind it.
             if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[35] = globaltimer_ns();
-            op_fit(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part);
+            if constexpr (PLANES)
+                op_fit_planes<true>(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part, P.planes.part);
+            else
+                op_fit(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part);
             g.sync();
             if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[36] = globaltimer_ns();
         }
@@ -353,6 +526,9 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
     KB_STAMP(5);
     if constexpr (LOCALIZE || ODOMETRY_FIT) {
         if (blockIdx.x == gridDim.x - 1) fit_finish(P.fit, n_src);
+    }
+    if constexpr (PLANES) {
+        if (blockIdx.x == gridDim.x - 1) planes_finish(P.planes);
     }
     if (book) {
         P.st->model_sse = sse;
@@ -380,3 +556,10 @@ cudaError_t localize_watchdog_rearm();
 const void *odometry_fit_kernel();
 cudaError_t odometry_fit_watchdog_init(unsigned *d_host_words, const unsigned init[8]);
 cudaError_t odometry_fit_watchdog_rearm();
+// defined in constraints.cu, likewise: k_register_frame<LocalizeConstraintParams> / <OdometryConstraintParams>, the
+// stand-alone k_constraints (takes a ConstraintsParams) and the module's copies of the watchdog words
+const void *localize_constraints_kernel();
+const void *odometry_constraints_kernel();
+const void *constraints_kernel();
+cudaError_t constraints_watchdog_init(unsigned *d_host_words, const unsigned init[8]);
+cudaError_t constraints_watchdog_rearm();

@@ -559,4 +559,60 @@ KB_HD bool icp_solve_schur(const double acc[16], double dx[6]) {
     return true;
 }
 
+// ---- symmetric 3x3 eigen-decomposition (the plane fit of a voxel: kb_registration_constraints) ----------------------
+// Cyclic Jacobi. A closed-form (trigonometric) solver loses its eigenvectors when eigenvalues nearly coincide, which is
+// exactly what collinear and blob-like voxels produce; Jacobi rotations keep V orthonormal to a few ulps and resolve
+// repeated and zero eigenvalues. One rotation (P, Q) zeroes a[P][Q] (Numerical Recipes' stable form, tau = s / (1 + c)).
+template <int P, int Q>
+KB_HD void sym3_rotate(double (&a)[3][3], double (&v)[3][3]) {
+    constexpr int R = 3 - P - Q;
+    const double apq = a[P][Q];
+    if (apq == 0.0) return;
+    const double theta = (a[Q][Q] - a[P][P]) / (2.0 * apq);
+    double t = 1.0 / (fabs(theta) + sqrt(1.0 + theta * theta));  // theta^2 overflows -> t = 0: a[P][Q] is negligible
+    if (theta < 0.0) t = -t;
+    const double c = 1.0 / sqrt(t * t + 1.0), s = t * c, tau = s / (1.0 + c);
+    a[P][P] -= t * apq;
+    a[Q][Q] += t * apq;
+    a[P][Q] = a[Q][P] = 0.0;
+    const double arp = a[R][P], arq = a[R][Q];
+    a[R][P] = a[P][R] = arp - s * (arq + tau * arp);
+    a[R][Q] = a[Q][R] = arq + s * (arp - tau * arq);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const double vp = v[k][P], vq = v[k][Q];
+        v[k][P] = vp - s * (vq + tau * vp);
+        v[k][Q] = vq + s * (vp - tau * vq);
+    }
+}
+
+// c = the 6 unique entries (xx, xy, xz, yy, yz, zz). lam: eigenvalues ascending; vec[k] = unit eigenvector of lam[k].
+// At most 16 sweeps (a 3x3 converges quadratically in 4-6); a sweep ends the loop when the off-diagonal part is below
+// 1e-36 of the squared Frobenius norm, i.e. below rounding.
+KB_HD void sym3_eig(const double c[6], double lam[3], V3 vec[3]) {
+    double a[3][3] = {{c[0], c[1], c[2]}, {c[1], c[3], c[4]}, {c[2], c[4], c[5]}};
+    double v[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
+    for (int sweep = 0; sweep < 16; ++sweep) {
+        const double off = (a[0][1] * a[0][1] + a[0][2] * a[0][2]) + a[1][2] * a[1][2];
+        const double diag = (a[0][0] * a[0][0] + a[1][1] * a[1][1]) + a[2][2] * a[2][2];
+        if (!(off > 1e-36 * (diag + 2.0 * off))) break;
+        sym3_rotate<0, 1>(a, v);
+        sym3_rotate<0, 2>(a, v);
+        sym3_rotate<1, 2>(a, v);
+    }
+    double l[3] = {a[0][0], a[1][1], a[2][2]};
+    int o[3] = {0, 1, 2};
+    // three compare-exchanges (ascending, stable)
+    if (l[o[1]] < l[o[0]]) { const int t = o[0]; o[0] = o[1]; o[1] = t; }
+    if (l[o[2]] < l[o[1]]) { const int t = o[1]; o[1] = o[2]; o[2] = t; }
+    if (l[o[1]] < l[o[0]]) { const int t = o[0]; o[0] = o[1]; o[1] = t; }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        // (selects instead of indexing with o[k]: the arrays stay in registers)
+        const int j = o[k];
+        lam[k] = j == 0 ? l[0] : (j == 1 ? l[1] : l[2]);
+        vec[k] = j == 0 ? V3{v[0][0], v[1][0], v[2][0]} : (j == 1 ? V3{v[0][1], v[1][1], v[2][1]} : V3{v[0][2], v[1][2], v[2][2]});
+    }
+}
+
 }  // namespace kb

@@ -16,6 +16,10 @@ VoxelHashMap with a large max_distance and ``vmap.update(frame_downsample, pose)
 ``KissICP(config, report_fit=True)`` is an odometry pipeline that also reports, in ``last_fit`` and
 ``register_frames(..., return_fits=True)``, how well each scan fit the map it was registered in: the pipeline's own map
 before the scan's ``local_map.update``. Poses, thresholds and the map are the same as without it.
+
+``report_constraints=True`` (a localizer, or odometry, where it turns fit reporting on too) also reports, in
+``last_constraints`` and ``register_frames(..., return_constraints=True)``, the plane constraints of each scan's fit
+(constraints.Constraints): which directions the scan pins down. Poses, fits and the map are the same as without it.
 """
 from __future__ import annotations
 
@@ -28,6 +32,7 @@ import numpy as np
 
 from . import _native as N
 from .config import KISSConfig, load_config
+from .constraints import Constraints, _constraints_of, _from_struct, _from_structs
 from .mapping import VoxelHashMap, check_value, get_voxel_hash_map
 from .preprocess import Preprocessor, get_preprocessor
 from .registration import get_registration
@@ -109,7 +114,7 @@ class _PipelineThreshold:
 
 class KissICP:
     def __init__(self, config: KISSConfig | None = None, fused: bool = True, prior_map: VoxelHashMap | None = None,
-                 report_fit: bool = False):
+                 report_fit: bool = False, report_constraints: bool = False):
         if prior_map is not None and not isinstance(prior_map, VoxelHashMap):
             raise TypeError(f"prior_map must be a VoxelHashMap, not {type(prior_map).__name__}")
         self.config = config if config is not None else load_config()
@@ -117,7 +122,9 @@ class KissICP:
             self.config.mapping.voxel_size = float(self.config.data.max_range / 100.0)
         self.fused = bool(fused) and self.config.adaptive_threshold.fixed_threshold is None
         self.localizer = prior_map is not None
-        self._report_fit = self.localizer or bool(report_fit)  # (a localizer always reports)
+        self._report_constraints = bool(report_constraints)
+        # (a localizer always reports fits; plane constraints are reported next to the fit)
+        self._report_fit = self.localizer or bool(report_fit) or self._report_constraints
         self._h = None
         if self.localizer:
             self._check_prior(prior_map)
@@ -144,6 +151,8 @@ class KissICP:
                                               _borrowed=N.lib().kb_pipeline_voxel_map(self._h), _owner=self)
                 if self._report_fit:
                     N.check(N.lib().kb_pipeline_set_fit_reporting(self._h, 1))
+            if self._report_constraints:
+                N.check(N.lib().kb_pipeline_set_constraint_reporting(self._h, 1))
             self.adaptive_threshold = _PipelineThreshold(self)
         else:
             self._last_pose = np.eye(4)
@@ -153,6 +162,7 @@ class KissICP:
             self.registration = get_registration(self.config)
             self.local_map = prior_map if self.localizer else get_voxel_hash_map(self.config)
             self._last_fit = _fit_of(0, 0, 0.0, np.zeros(36))
+            self._last_constraints = _constraints_of(0, 0.0, 0.0, np.zeros(36))
 
     def _check_prior(self, prior_map):
         vs, mp = N.dbl(0), N.u32(0)
@@ -219,6 +229,26 @@ class KissICP:
         f = N.Fit()
         N.check(N.lib().kb_pipeline_last_fit(self._h, C.byref(f)))
         return _fit_of(f.n_correspondences, f.n_source, f.sum_sq_residual, np.array(f.JTJ[:]))
+
+    @property
+    def report_constraints(self) -> bool:
+        """whether every scan gets plane constraints (KissICP(config, report_constraints=True))"""
+        return self._report_constraints
+
+    def _check_reports_constraints(self):
+        if not self._report_constraints:
+            raise ValueError("plane constraints are reported by pipelines created with report_constraints=True")
+
+    @property
+    def last_constraints(self) -> Constraints:
+        """the plane constraints of the last scan's fit (zeros before the first scan), against the map the fit is
+        against"""
+        self._check_reports_constraints()
+        if not self.fused:
+            return self._last_constraints
+        c = N.Constraints()
+        N.check(N.lib().kb_pipeline_last_constraints(self._h, C.byref(c)))
+        return _from_struct(c)
 
     def _sigma_next(self):
         s = N.dbl(0)
@@ -294,41 +324,53 @@ class KissICP:
         N.check(N.lib().kb_pipeline_last_clouds(self._h, N.ptr(pre), a.value, N.ptr(src), b.value))
         return pre, src
 
-    def register_frames(self, frames, timestamps=None, return_fits: bool = False):
+    def register_frames(self, frames, timestamps=None, return_fits: bool = False, return_constraints: bool = False):
         """Register a whole sequence (the dataset loop of python/kiss_icp/pipeline.py:106-112) -> poses (K,4,4).
 
         Same results as K ``register_frame`` calls; the frames are queued on the device (copy of frame k+1
         overlaps the registration of frame k, results are read behind the queue). ``frames`` is a sequence of
         (N_k,3) arrays, all float64 or all float32; ``timestamps`` a matching sequence (or None).
-        ``return_fits`` (localizers and report_fit=True only) -> (poses, fits): a Fit of arrays, one entry per frame."""
+        ``return_fits`` (localizers and report_fit=True only) -> (poses, fits): a Fit of arrays, one entry per frame.
+        ``return_constraints`` (report_constraints=True only) appends a Constraints of arrays: (poses, [fits,] constraints)."""
         K = len(frames)
         if return_fits:
             self._check_reports_fits()
+        if return_constraints:
+            self._check_reports_constraints()
         if timestamps is None:
             timestamps = [np.empty(0)] * K
         if len(timestamps) != K:
             raise ValueError("frames and timestamps differ in length")
         if not self.fused:
             poses = np.empty((K, 4, 4))
-            fits = []
+            fits, cons = [], []
             for k in range(K):
                 self._register_frame_modular(frames[k], timestamps[k])
                 poses[k] = self._last_pose
                 if return_fits:
                     fits.append(self._last_fit)
-            if not return_fits:
-                return poses
-            return poses, _fit_of([f.n_correspondences for f in fits], [f.n_source for f in fits],
-                                  [f.rmse ** 2 * f.n_correspondences if f.n_correspondences else 0.0 for f in fits],
-                                  np.array([f.information for f in fits]).reshape(-1, 36))
+                if return_constraints:
+                    cons.append(self._last_constraints)
+            out = [poses]
+            if return_fits:
+                out.append(_fit_of([f.n_correspondences for f in fits], [f.n_source for f in fits],
+                                   [f.rmse ** 2 * f.n_correspondences if f.n_correspondences else 0.0 for f in fits],
+                                   np.array([f.information for f in fits]).reshape(-1, 36)))
+            if return_constraints:
+                out.append(_constraints_of([c.n_planes for c in cons], [c.weight_sum for c in cons],
+                                           [c.plane_rmse ** 2 * c.weight_sum if c.weight_sum > 0 else 0.0 for c in cons],
+                                           np.array([c.information for c in cons]).reshape(-1, 36)))
+            return out[0] if len(out) == 1 else tuple(out)
         arrs = [np.asarray(f) for f in frames]
         f32 = K > 0 and all(a.dtype == np.float32 and a.ndim == 2 and a.shape[1] == 3 for a in arrs)
         pts = [np.ascontiguousarray(a) for a in arrs] if f32 else [N.points_arg(a) for a in arrs]
         ts = [np.ascontiguousarray(np.asarray(t).ravel(), dtype=np.float64) for t in timestamps]
         return self._register_frames_raw([N.ptr(a) for a in pts], [len(a) for a in pts], [N.ptr(t) for t in ts],
-                                         [len(t) for t in ts], 1 if f32 else 0, return_fits=return_fits)
+                                         [len(t) for t in ts], 1 if f32 else 0, return_fits=return_fits,
+                                         return_constraints=return_constraints)
 
-    def _register_frames_raw(self, xyz_ptrs, sizes, ts_ptrs, ts_sizes, layout, return_fits: bool = False):
+    def _register_frames_raw(self, xyz_ptrs, sizes, ts_ptrs, ts_sizes, layout, return_fits: bool = False,
+                             return_constraints: bool = False):
         """raw-pointer form (host or device addresses): layout 0 host f64, 1 host f32, 2 device f64"""
         K = len(xyz_ptrs)
         as_vp = lambda v: v if isinstance(v, C.c_void_p) else C.c_void_p(int(v) if v else None)
@@ -337,6 +379,16 @@ class KissICP:
         n = (N.sz * K)(*sizes)
         nt = (N.sz * K)(*ts_sizes)
         poses = np.empty((K, 4, 4))
+        if return_constraints:
+            fits = (N.Fit * K)() if return_fits else None
+            cons = (N.Constraints * K)()
+            N.check(N.lib().kb_pipeline_register_frames_constraints(self._h, X, n, T, nt, K, int(layout), N.ptr(poses),
+                                                                    fits, cons))
+            if not return_fits:
+                return poses, _from_structs(cons)
+            return poses, _fit_of([f.n_correspondences for f in fits], [f.n_source for f in fits],
+                                  [f.sum_sq_residual for f in fits], np.array([f.JTJ[:] for f in fits]).reshape(-1, 36)), \
+                _from_structs(cons)
         if not return_fits:
             N.check(N.lib().kb_pipeline_register_frames(self._h, X, n, T, nt, K, int(layout), N.ptr(poses)))
             return poses
@@ -362,6 +414,8 @@ class KissICP:
         self.adaptive_threshold.update_model_deviation(model_deviation)
         if self._report_fit:  # against the map the scan was registered in: before local_map.update adds it
             self._last_fit = self._fit_modular(source, new_pose, sigma)
+        if self._report_constraints:
+            self._last_constraints = self.registration.constraints(source, self.local_map, new_pose, 3 * sigma)
         if not self.localizer:  # (a localizer has no local_map.update)
             self.local_map.update(frame_downsample, new_pose)
         self._last_delta = np.linalg.inv(self._last_pose) @ new_pose

@@ -8,6 +8,7 @@ import numpy as np
 
 from . import _native as N
 from .config import KISSConfig
+from .constraints import Constraints, _from_struct
 from .mapping import VoxelHashMap
 from .relocalization import RelocalizationResult, RelocalizationSearch, relocalize
 
@@ -75,6 +76,17 @@ class Registration:
         N.check(N.lib().kb_registration_align_points_to_map(self._h, N.ptr(pts), len(pts), voxel_map._h, N.ptr(g),
                                                             float(max_correspondance_distance), float(kernel), N.ptr(out)))
         return out
+
+    def constraints(self, points, voxel_map: VoxelHashMap, pose, max_correspondance_distance: float) -> Constraints:
+        """The plane constraints (constraints.Constraints) of ``points`` mapped by ``pose`` against ``voxel_map``, for
+        the correspondences closer than ``max_correspondance_distance``: those of the fit. Read-only, so it works on a
+        localizer's prior map. ValueError for a pose outside SE(3)."""
+        pts = N.points_arg(points)
+        T = N.mat4_arg(pose)
+        c = N.Constraints()
+        N.check(N.lib().kb_registration_constraints(self._h, N.ptr(pts), len(pts), voxel_map._h, N.ptr(T),
+                                                    float(max_correspondance_distance), C.byref(c)))
+        return _from_struct(c)
 
     def align_points_to_map_batch(self, points, voxel_map: VoxelHashMap, initial_guesses, max_correspondance_distance,
                                   kernel, ranges=None, return_inliers: bool = False):
