@@ -415,6 +415,90 @@ typedef struct kb_reloc_result {
 int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_map *map, const kb_reloc_search *search,
                   kb_reloc_result *out, double *candidates, int *candidate_scores, int *scores);
 
+/* ---- place recognition: relocalization without any pose, loop-closure candidates -----------------------------
+ * No reference counterpart. A database holds the Scan Context descriptor (Kim & Kim, IROS 2018) of a cloud at each
+ * keyframe pose of a mapping run. A query cloud is compared with every entry at every cyclic shift on the device; the
+ * best entries, rotated by their shift, are initial guesses for kb_registration_align_batch.
+ * Parameters: 1 <= n_rings <= 64, 3 <= n_sectors <= 720, n_rings n_sectors <= 4096, max_radius finite and > 0, z_offset
+ * finite (defaults 20, 60, 80.0, 2.0).
+ * Descriptor D[r][k] of a cloud in its sensor frame (bit for bit; the device rounds like the host, without FMA):
+ *   a point with x = y = 0 is skipped; d2 = x*x + y*y;
+ *   ring r: b_r <= d2 < b_{r+1} with b_i = (i * (max_radius / n_rings))^2 for i < n_rings and b_{n_rings} =
+ *     max_radius * max_radius (computed on the host); a point with d2 >= b_{n_rings} is skipped;
+ *   sector k: u_k x p >= 0 and u_{k+1} x p < 0 with u x p = u.x*y - u.y*x, u_k = (cos t_k, sin t_k) from std::cos /
+ *     std::sin on the host, t_k = -pi + k * (2 pi / n_sectors), u_{n_sectors} = u_0. Exactly one k passes for every point
+ *     (a point no k passes, possible only for subnormal x and y, is skipped);
+ *   D[r][k] = max(0, the largest z + z_offset of the cell's points); an empty cell is 0.
+ * Distance of a query Q to an entry C: norm_k = sqrt(sum_r D[r][k]^2) (ring order); column k is nonempty when norm_k > 0,
+ *   its unit column is D[.][k] / norm_k (zeros when empty). For shift s in [0, n_sectors):
+ *   dot_k = sum_r q[r][k] c[r][(k + s) mod n_sectors] (ring order, from 0), S_s = sum_k dot_k (k order, from 0),
+ *   m_s = the k where both columns are nonempty, d_s = 1 - S_s / m_s (1 when m_s = 0).
+ *   The entry's distance is min_s d_s, its shift the smallest s attaining it.
+ * Heading: shift s means the query's column k matches the entry's column k + s: a cloud rotated by Rz(j D), D = 2 pi /
+ *   n_sectors, against the unrotated one gives s = (n_sectors - j) mod n_sectors. The query's pose guess from entry i is
+ *   T_i Rz(s D), Rz = [c -s 0; s c 0; 0 0 1] from std::cos / std::sin of yaw = s D:
+ *   guess[r][c] = (T_i[r][0] Rz[0][c] + T_i[r][1] Rz[1][c]) + T_i[r][2] Rz[2][c] for c < 3, guess[r][3] = T_i[r][3].
+ * Candidates: the searched entries by (distance ascending, entry ascending); walking that order an entry is taken unless
+ *   its keyframe's xy is closer than `separation` to a candidate already taken (0 takes everything); at most top_k
+ *   (1..256). max_entry < 0 searches every entry, otherwise entries [0, min(max_entry, N)) (a loop-closure query:
+ *   only entries older than the recent ones); an empty range is KB_ERR_INVALID_ARG.
+ * Every argument that needs no handle is checked first; without a device the calls then return KB_ERR_NO_DEVICE. A
+ * non-finite point is KB_ERR_INVALID_ARG, a pose outside SE(3) KB_ERR_NOT_SE3. On error nothing is written. */
+typedef struct kb_place_params {
+    int n_rings, n_sectors;
+    double max_radius, z_offset;
+} kb_place_params;
+void kb_place_params_default(kb_place_params *p); /* 20, 60, 80.0, 2.0; needs no device */
+typedef struct kb_place_db kb_place_db;
+/* a database on the calling thread's device (kb_set_device) */
+int kb_place_db_create(const kb_place_params *p, kb_place_db **out);
+int kb_place_db_destroy(kb_place_db *db);
+int kb_place_db_size(const kb_place_db *db, size_t *out);
+/* the descriptor of xyz[n] into out[n_rings][n_sectors]; nothing is added. n = 0 gives zeros. */
+int kb_place_descriptor(kb_place_db *db, const double *xyz, size_t n, double *out);
+/* append the descriptor of xyz[n] (the cloud in its sensor frame) with the keyframe pose (row-major SE(3)); *index (may
+ * be NULL) = its entry. At most 2^24 entries. Earlier entries are unchanged when the storage grows. */
+int kb_place_db_add(kb_place_db *db, const double *xyz, size_t n, const double pose[16], size_t *index);
+/* two-call like kb_map_pointcloud: *n_out = N; descriptors (double[N][n_rings][n_sectors]) and poses (double[N][16])
+ * both NULL or cap 0 only query it; cap < N is KB_ERR_CAPACITY, with *n_out = N written (the one output written on that
+ * error) and nothing else. Either array may be NULL when cap >= N. */
+int kb_place_db_dump(const kb_place_db *db, double *descriptors, double *poses, size_t cap, size_t *n_out);
+/* replace the entries by n dumped ones, all or nothing: KB_ERR_INVALID_ARG for a negative or non-finite descriptor value
+ * or n > 2^24, KB_ERR_NOT_SE3 for a pose outside SE(3); the database is unchanged on error */
+int kb_place_db_load(kb_place_db *db, const double *descriptors, const double *poses, size_t n);
+typedef struct kb_place_match {
+    int entry, shift;
+    double yaw, distance; /* yaw = shift 2 pi / n_sectors */
+    double guess[16];     /* T_entry Rz(yaw), row-major */
+} kb_place_match;
+/* the candidates of the query cloud xyz[n] into out[top_k], *n_out = their count. entry_distances / entry_shifts (may be
+ * NULL) receive every searched entry's distance and shift, in entry order. */
+int kb_place_query(kb_place_db *db, const double *xyz, size_t n, int max_entry, double separation, int top_k,
+                   kb_place_match *out, size_t *n_out, double *entry_distances, int *entry_shifts);
+typedef struct kb_place_search {
+    int top_k, max_entry;   /* as kb_place_query */
+    double separation;      /* metres, >= 0: of the candidate walk and of the runner-up */
+    double max_correspondence_distance, kernel_scale; /* of the refinement */
+} kb_place_search;
+typedef struct kb_place_result {
+    double pose[16];  /* the winner, refined, row-major */
+    int inliers, iterations, rank; /* its inliers, ICP iterations and index among the candidates */
+    int n_source, n_entries, n_candidates;  /* source points, entries searched, candidates refined */
+    double runner_up_pose[16];  /* all zero when there is no runner-up */
+    int runner_up_inliers;      /* -1 when there is none */
+} kb_place_result;
+/* Relocalize without any pose: the candidates of the descriptor cloud desc_xyz[n_desc] (kb_place_query with s's top_k,
+ * max_entry and separation), then kb_registration_align_batch of the source src_xyz[n_src] from every candidate's guess
+ * with s's thresholds, inliers on: each refined pose, iteration count and inlier count is bit for bit that call's.
+ * Winner: the most inliers, ties to the lower rank. Runner-up: the best other candidate whose refined pose is farther
+ * from the winner's than `separation` in xy or 2 sector widths in rotation angle (the rule of kb_relocalize).
+ * candidates (kb_place_match[top_k], may be NULL) receives the first n_candidates matches. db, map and reg must be on
+ * one device. Only reads the map: allowed while localizers hold it. KB_ERR_INVALID_ARG as kb_place_query, for n_src = 0
+ * and for an empty map. */
+int kb_place_relocalize(kb_registration *reg, kb_place_db *db, const double *desc_xyz, size_t n_desc,
+                        const double *src_xyz, size_t n_src, const kb_map *map, const kb_place_search *s,
+                        kb_place_result *out, kb_place_match *candidates);
+
 #ifdef __cplusplus
 }
 #endif

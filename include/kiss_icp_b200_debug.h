@@ -42,6 +42,8 @@ int kb_debug_fast_rcp_dev(const double *x, size_t n, double *out);
 /* device time [ms] of the coarse score (k_reloc_score) of the last kb_relocalize on this handle, from CUDA events recorded
  * around its launch; KB_ERR_INVALID_ARG before the first call */
 int kb_debug_reloc_score_ms(const kb_registration *reg, float *ms);
+/* time of the last k_place_distance launch of a kb_place_query or kb_place_relocalize on db [ms] (CUDA events) */
+int kb_debug_place_distance_ms(const kb_place_db *db, float *ms);
 /* work done by the ICP loop of the last RegisterFrame: GetClosestNeighbor calls (iterations x
  * source points) and map points examined — the inputs of the algorithmic-bytes formula */
 int kb_pipeline_last_icp_work(const kb_pipeline *p, double *queries, double *candidates);

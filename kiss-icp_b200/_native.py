@@ -41,13 +41,13 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/api.cu, csrc/localize.cu, csrc/odometry_fit.cu, csrc/constraints.cu, csrc/probe.cu and csrc/relocalize.cu
-    -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
+    """Compile csrc/api.cu, csrc/localize.cu, csrc/odometry_fit.cu, csrc/constraints.cu, csrc/probe.cu, csrc/relocalize.cu
+    and csrc/places.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in sources())
     if force or stale:
         cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH,
                *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "odometry_fit.cu", "constraints.cu", "probe.cu",
-                                                       "relocalize.cu"))]
+                                                       "relocalize.cu", "places.cu"))]
         if verbose:
             print(" ".join(cmd))
         env = dict(os.environ)
@@ -111,6 +111,28 @@ class RelocResult(C.Structure):
     _fields_ = [("pose", dbl * 16), ("inliers", i32), ("iterations", i32), ("rank", i32), ("n_source", i32),
                 ("n_hypotheses", i32), ("n_peaks", i32), ("n_candidates", i32), ("runner_up_pose", dbl * 16),
                 ("runner_up_inliers", i32)]
+
+
+class PlaceParams(C.Structure):
+    """kb_place_params: the Scan Context grid"""
+    _fields_ = [("n_rings", i32), ("n_sectors", i32), ("max_radius", dbl), ("z_offset", dbl)]
+
+
+class PlaceMatch(C.Structure):
+    """kb_place_match: one candidate of a place query"""
+    _fields_ = [("entry", i32), ("shift", i32), ("yaw", dbl), ("distance", dbl), ("guess", dbl * 16)]
+
+
+class PlaceSearch(C.Structure):
+    """kb_place_search: the query and refinement of kb_place_relocalize"""
+    _fields_ = [("top_k", i32), ("max_entry", i32), ("separation", dbl), ("max_correspondence_distance", dbl),
+                ("kernel_scale", dbl)]
+
+
+class PlaceResult(C.Structure):
+    """kb_place_result"""
+    _fields_ = [("pose", dbl * 16), ("inliers", i32), ("iterations", i32), ("rank", i32), ("n_source", i32),
+                ("n_entries", i32), ("n_candidates", i32), ("runner_up_pose", dbl * 16), ("runner_up_inliers", i32)]
 
 
 # every exported symbol of include/kiss_icp_b200.h: name -> (restype, argtypes)
@@ -214,6 +236,17 @@ SIGNATURES = {
     "kb_pipeline_last_constraints": (i32, [vp, C.POINTER(Constraints)]),
     "kb_pipeline_register_frames_constraints": (i32, [vp, vp, vp, vp, vp, sz, i32, vp, vp, vp]),
     "kb_debug_sym3_eig": (i32, [vp, vp, vp]),
+    "kb_place_params_default": (None, [C.POINTER(PlaceParams)]),
+    "kb_place_db_create": (i32, [C.POINTER(PlaceParams), C.POINTER(vp)]),
+    "kb_place_db_destroy": (i32, [vp]),
+    "kb_place_db_size": (i32, [vp, C.POINTER(sz)]),
+    "kb_place_descriptor": (i32, [vp, vp, sz, vp]),
+    "kb_place_db_add": (i32, [vp, vp, sz, vp, C.POINTER(sz)]),
+    "kb_place_db_dump": (i32, [vp, vp, vp, sz, C.POINTER(sz)]),
+    "kb_place_db_load": (i32, [vp, vp, vp, sz]),
+    "kb_place_query": (i32, [vp, vp, sz, i32, dbl, i32, vp, C.POINTER(sz), vp, vp]),
+    "kb_place_relocalize": (i32, [vp, vp, vp, sz, vp, sz, vp, C.POINTER(PlaceSearch), C.POINTER(PlaceResult), vp]),
+    "kb_debug_place_distance_ms": (i32, [vp, C.POINTER(C.c_float)]),
 }
 
 

@@ -34,6 +34,7 @@ from . import _native as N
 from .config import KISSConfig, load_config
 from .constraints import Constraints, _constraints_of, _from_struct, _from_structs
 from .mapping import VoxelHashMap, check_value, get_voxel_hash_map
+from .places import PlaceDatabase, PlaceRelocalizationResult
 from .preprocess import Preprocessor, get_preprocessor
 from .registration import get_registration
 from .relocalization import RelocalizationResult, RelocalizationSearch
@@ -444,11 +445,7 @@ class KissICP:
             raise ValueError("relocalization needs a prior map: KissICP(config, prior_map=...)")
         if not isinstance(search, RelocalizationSearch):
             raise TypeError(f"search must be a RelocalizationSearch, not {type(search).__name__}")
-        if getattr(self, "_reloc", None) is None:
-            c = self.config
-            self._reloc = (Preprocessor(c.data.max_range, c.data.min_range, False, c.registration.max_num_threads),
-                           self.registration if not self.fused else get_registration(c))
-        pre, reg = self._reloc
+        pre, reg = self._relocalizer()
         frame = pre.preprocess(frame, np.empty(0), np.eye(4))
         source, _ = self.voxelize(frame)
         sigma = self._sigma_next() if self.fused else self.adaptive_threshold.get_threshold()
@@ -457,6 +454,38 @@ class KissICP:
         self.last_pose = result.pose
         self.last_delta = np.eye(4)
         return result
+
+    def relocalize_by_place(self, frame, places: PlaceDatabase, top_k: int = 8,
+                            separation: float = 3.0) -> PlaceRelocalizationResult:
+        """Find the localizer's pose in its prior map from one scan without any pose, through the place database
+        ``places`` built from the same run as the map, and continue the track from there.
+
+        The scan is preprocessed as relocalize() does (without deskewing). The preprocessed frame is the descriptor
+        cloud, the source is built from it by voxelize(). Registration.relocalize_in_places refines the top_k
+        candidates with the thresholds of the pipeline's current sigma (3 sigma, sigma). Then last_pose is the winner
+        and last_delta the identity; the adaptive threshold's state is unchanged. Returns the
+        PlaceRelocalizationResult; accepting it is the caller's decision."""
+        if not self.localizer:
+            raise ValueError("relocalization needs a prior map: KissICP(config, prior_map=...)")
+        if not isinstance(places, PlaceDatabase):
+            raise TypeError(f"places must be a PlaceDatabase, not {type(places).__name__}")
+        pre, reg = self._relocalizer()
+        frame = pre.preprocess(frame, np.empty(0), np.eye(4))
+        source, _ = self.voxelize(frame)
+        sigma = self._sigma_next() if self.fused else self.adaptive_threshold.get_threshold()
+        result = reg.relocalize_in_places(frame, source, self.local_map, places, top_k=top_k, separation=separation,
+                                          max_correspondence_distance=3 * sigma, kernel_scale=sigma)
+        self.last_pose = result.pose
+        self.last_delta = np.eye(4)
+        return result
+
+    def _relocalizer(self):
+        """(the preprocessor without deskewing, a registration) of the relocalization calls"""
+        if getattr(self, "_reloc", None) is None:
+            c = self.config
+            self._reloc = (Preprocessor(c.data.max_range, c.data.min_range, False, c.registration.max_num_threads),
+                           self.registration if not self.fused else get_registration(c))
+        return self._reloc
 
     # -- checkpoint / restore -----------------------------------------------------------------------
     def state_dict(self):

@@ -10,6 +10,7 @@ from . import _native as N
 from .config import KISSConfig
 from .constraints import Constraints, _from_struct
 from .mapping import VoxelHashMap
+from .places import PlaceDatabase, PlaceRelocalizationResult, relocalize_in_places
 from .relocalization import RelocalizationResult, RelocalizationSearch, relocalize
 
 
@@ -173,6 +174,18 @@ class Registration:
         return_scores, the (n_yaw, Ny, Nx) coarse scores. Only reads the map. Accepting the result is the caller's
         decision. kb_relocalize in include/kiss_icp_b200.h states every rule."""
         return relocalize(self._h, source, voxel_map, search, return_scores)
+
+    def relocalize_in_places(self, descriptor_points, source, voxel_map: VoxelHashMap, places: PlaceDatabase, top_k=8,
+                             separation=3.0, max_correspondence_distance=3.0, kernel_scale=1.0,
+                             max_entry=-1) -> PlaceRelocalizationResult:
+        """Find the pose of ``source`` (N, 3) in ``voxel_map`` without any pose: the top_k candidates of
+        ``descriptor_points`` (the preprocessed frame the entries of ``places`` describe) among the database's entries,
+        no two closer than ``separation`` metres, refined from their guesses with align_points_to_map_batch (bit for
+        bit that call's poses, iterations and inliers); the candidate with the most inliers wins. Only reads the map.
+        Accepting the result is the caller's decision. kb_place_relocalize in include/kiss_icp_b200.h states every
+        rule."""
+        return relocalize_in_places(self._h, descriptor_points, source, voxel_map, places, top_k, separation,
+                                    max_correspondence_distance, kernel_scale, max_entry)
 
     @property
     def last_iterations(self) -> int:
