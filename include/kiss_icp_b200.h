@@ -499,6 +499,62 @@ int kb_place_relocalize(kb_registration *reg, kb_place_db *db, const double *des
                         const double *src_xyz, size_t n_src, const kb_map *map, const kb_place_search *s,
                         kb_place_result *out, kb_place_match *candidates);
 
+/* ---- pose graph: loop closure --------------------------------------------------------------------------------------
+ * No reference counterpart. Nodes are poses T_i (row-major SE(3)); a fixed node does not move. An edge
+ * e = (i, j, Z, Omega, c) has the residual r_e = Log(Z^-1 T_i^-1 T_j) in R^6, in the tangent order (translation,
+ * rotation) of the library, s_e = r_e^T Omega r_e, and the cost F = 1/2 sum_e rho_e(s_e) with rho(s) = s for c = 0 and
+ * the Cauchy loss rho(s) = c^2 log(1 + s / c^2) for c > 0; w_e = rho'(s_e).
+ * kb_pose_graph_optimize moves the free nodes by right perturbation, T_i <- T_i Exp(d_i), with Levenberg-Marquardt on
+ * IRLS weights and exact Jacobians (dr/dd_j = J_r^-1(r), dr/dd_i = -J_r^-1(r) Ad(T_j^-1 T_i)):
+ *   H = sum J^T w Omega J, g = sum J^T w Omega r over the free nodes; (H + lambda diag H) d = -g is solved by PCG
+ *   preconditioned by the exact inverse of M, the block-tridiagonal part of the damped system (the edges with
+ *   |i - j| = 1 in full, every other edge's two diagonal blocks, the damping), which block cyclic reduction factors once
+ *   per step. PCG stops at |r_k| <= cg_tolerance |g| or after max_cg_iterations.
+ *   An accepted step (lower F) divides lambda by 10, a rejected one (including a non-finite F) multiplies it by 10.
+ *   Stop: an accepted step lowers F by at most function_tolerance F; max |d| <= parameter_tolerance; lambda > 1e12; or
+ *   max_iterations steps (accepted and rejected both count).
+ * One cooperative launch per call, on the graph's device and stream. The results are bit-identical from run to run for a
+ * given grid size (kb_set_grid_blocks caps it at optimize time): every sum is formed in a fixed order.
+ * The graph lives on the host. Its device buffers are allocated at the first optimize on the device and stream the
+ * creating thread had selected (kb_set_device / kb_set_stream), kept for later calls and released by destroy. Nodes and
+ * edges may be added after an optimize; the next one starts from the current poses.
+ * Every argument is checked before any work and nothing is written on error: KB_ERR_NOT_SE3 for a pose or measurement
+ * outside SE(3) (non-finite included); KB_ERR_INVALID_ARG for a NULL argument, i == j, a node that does not exist,
+ * information that is not exactly symmetric, not finite or not positive definite, a negative or non-finite
+ * robust_scale, more than 2^22 nodes or 2^24 edges, options out of range, and at optimize a free node that no path of
+ * edges connects to a fixed node. Without a device, optimize returns KB_ERR_NO_DEVICE after these checks. */
+typedef struct kb_pose_graph kb_pose_graph;
+int kb_pose_graph_create(kb_pose_graph **out); /* host-side; needs no device */
+int kb_pose_graph_destroy(kb_pose_graph *g);
+/* *index (may be NULL) = the new node's index */
+int kb_pose_graph_add_node(kb_pose_graph *g, const double pose[16], int fixed, size_t *index);
+/* information: row-major 6x6 in the tangent order; robust_scale: c (0 = squared loss). *index may be NULL. */
+int kb_pose_graph_add_edge(kb_pose_graph *g, size_t i, size_t j, const double measurement[16],
+                           const double information[36], double robust_scale, size_t *index);
+int kb_pose_graph_size(const kb_pose_graph *g, size_t *n_nodes, size_t *n_edges);
+/* two-call: *n_out = N; poses (double[N][16]) NULL or cap 0 only queries it, cap < N is KB_ERR_CAPACITY (with *n_out) */
+int kb_pose_graph_poses(const kb_pose_graph *g, double *poses, size_t cap, size_t *n_out);
+typedef struct kb_pose_graph_options {
+    int max_iterations;          /* [0, 10^6] */
+    double function_tolerance;   /* >= 0 */
+    double parameter_tolerance;  /* >= 0 */
+    double initial_lambda;       /* (0, 1e12] */
+    int max_cg_iterations;       /* [1, 10^6] */
+    double cg_tolerance;         /* [0, 1) */
+} kb_pose_graph_options;
+/* 100, 1e-12, 1e-10, 1e-4, 100, 1e-10; needs no device */
+void kb_pose_graph_options_default(kb_pose_graph_options *o);
+enum { KB_PG_FUNCTION_TOLERANCE = 0, KB_PG_PARAMETER_TOLERANCE = 1, KB_PG_MAX_ITERATIONS = 2, KB_PG_NO_DECREASE = 3 };
+typedef struct kb_pose_graph_report {
+    int iterations, accepted, cg_iterations; /* LM steps (accepted and rejected), accepted ones, PCG iterations in all */
+    int termination;                         /* KB_PG_* */
+    double initial_cost, final_cost, lambda; /* F at the start and at the returned poses, the last lambda */
+} kb_pose_graph_report;
+/* o may be NULL (the defaults). edge_chi2 / edge_weight (double[E], may be NULL) receive s_e and w_e at the returned
+ * poses. */
+int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *o, kb_pose_graph_report *out,
+                           double *edge_chi2, double *edge_weight);
+
 #ifdef __cplusplus
 }
 #endif

@@ -44,6 +44,11 @@ int kb_debug_fast_rcp_dev(const double *x, size_t n, double *out);
 int kb_debug_reloc_score_ms(const kb_registration *reg, float *ms);
 /* time of the last k_place_distance launch of a kb_place_query or kb_place_relocalize on db [ms] (CUDA events) */
 int kb_debug_place_distance_ms(const kb_place_db *db, float *ms);
+/* time of the last kb_pose_graph_optimize launch on g [ms] (CUDA events); KB_ERR_INVALID_ARG before the first */
+int kb_debug_pose_graph_ms(const kb_pose_graph *g, float *ms);
+/* host evaluation of the pose graph's Jacobian pieces: Ad(T) of a row-major SE(3) and J_r^-1(x), row-major 6x6 */
+int kb_debug_se3_adjoint(const double T[16], double A[36]);
+int kb_debug_se3_right_jacobian_inverse(const double x[6], double J[36]);
 /* work done by the ICP loop of the last RegisterFrame: GetClosestNeighbor calls (iterations x
  * source points) and map points examined — the inputs of the algorithmic-bytes formula */
 int kb_pipeline_last_icp_work(const kb_pipeline *p, double *queries, double *candidates);

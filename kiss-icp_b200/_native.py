@@ -41,13 +41,13 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/api.cu, csrc/localize.cu, csrc/odometry_fit.cu, csrc/constraints.cu, csrc/probe.cu, csrc/relocalize.cu
-    and csrc/places.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
+    """Compile csrc/api.cu, csrc/localize.cu, csrc/odometry_fit.cu, csrc/constraints.cu, csrc/probe.cu, csrc/relocalize.cu,
+    csrc/places.cu and csrc/pose_graph.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in sources())
     if force or stale:
         cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH,
                *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "odometry_fit.cu", "constraints.cu", "probe.cu",
-                                                       "relocalize.cu", "places.cu"))]
+                                                       "relocalize.cu", "places.cu", "pose_graph.cu"))]
         if verbose:
             print(" ".join(cmd))
         env = dict(os.environ)
@@ -133,6 +133,18 @@ class PlaceResult(C.Structure):
     """kb_place_result"""
     _fields_ = [("pose", dbl * 16), ("inliers", i32), ("iterations", i32), ("rank", i32), ("n_source", i32),
                 ("n_entries", i32), ("n_candidates", i32), ("runner_up_pose", dbl * 16), ("runner_up_inliers", i32)]
+
+
+class PoseGraphOptions(C.Structure):
+    """kb_pose_graph_options"""
+    _fields_ = [("max_iterations", i32), ("function_tolerance", dbl), ("parameter_tolerance", dbl),
+                ("initial_lambda", dbl), ("max_cg_iterations", i32), ("cg_tolerance", dbl)]
+
+
+class PoseGraphReport(C.Structure):
+    """kb_pose_graph_report"""
+    _fields_ = [("iterations", i32), ("accepted", i32), ("cg_iterations", i32), ("termination", i32),
+                ("initial_cost", dbl), ("final_cost", dbl), ("lambda_", dbl)]
 
 
 # every exported symbol of include/kiss_icp_b200.h: name -> (restype, argtypes)
@@ -247,6 +259,17 @@ SIGNATURES = {
     "kb_place_query": (i32, [vp, vp, sz, i32, dbl, i32, vp, C.POINTER(sz), vp, vp]),
     "kb_place_relocalize": (i32, [vp, vp, vp, sz, vp, sz, vp, C.POINTER(PlaceSearch), C.POINTER(PlaceResult), vp]),
     "kb_debug_place_distance_ms": (i32, [vp, C.POINTER(C.c_float)]),
+    "kb_pose_graph_create": (i32, [C.POINTER(vp)]),
+    "kb_pose_graph_destroy": (i32, [vp]),
+    "kb_pose_graph_add_node": (i32, [vp, vp, i32, C.POINTER(sz)]),
+    "kb_pose_graph_add_edge": (i32, [vp, sz, sz, vp, vp, dbl, C.POINTER(sz)]),
+    "kb_pose_graph_size": (i32, [vp, C.POINTER(sz), C.POINTER(sz)]),
+    "kb_pose_graph_poses": (i32, [vp, vp, sz, C.POINTER(sz)]),
+    "kb_pose_graph_options_default": (None, [C.POINTER(PoseGraphOptions)]),
+    "kb_pose_graph_optimize": (i32, [vp, C.POINTER(PoseGraphOptions), C.POINTER(PoseGraphReport), vp, vp]),
+    "kb_debug_pose_graph_ms": (i32, [vp, C.POINTER(C.c_float)]),
+    "kb_debug_se3_adjoint": (i32, [vp, vp]),
+    "kb_debug_se3_right_jacobian_inverse": (i32, [vp, vp]),
 }
 
 

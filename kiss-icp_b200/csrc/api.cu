@@ -28,6 +28,7 @@
 #include "kernels.cuh"
 #include "probe.cuh"
 #include "places.cuh"
+#include "pose_graph.cuh"
 #include "relocalize.cuh"
 
 using namespace kb;
@@ -94,6 +95,7 @@ int watchdog_init(int device) {
     CK(localize_watchdog_init(d, init));  // the localizer kernel's module has its own copies
     CK(odometry_fit_watchdog_init(d, init));  // and so has the fit-reporting odometry kernel's
     CK(constraints_watchdog_init(d, init));   // and the module of the plane-constraint kernels
+    CK(pose_graph_watchdog_init(d, init));    // and the pose-graph optimizer's
     g_wd[device].host = h;
     return KB_OK;
 }
@@ -118,6 +120,7 @@ int watchdog_check(int device) {
     localize_watchdog_rearm();
     odometry_fit_watchdog_rearm();
     constraints_watchdog_rearm();
+    pose_graph_watchdog_rearm();
     static const char *names[] = {"?", "grid barrier", "ICP gather", "ICP result record", "ICP team gather", "NN bulk copy"};
     std::string marks;
     unsigned m[256];
@@ -301,13 +304,14 @@ struct Exec {
         scratch_mem.push_back(std::move(b));
         return KB_OK;
     }
-    int init() {
+    // on `dev`, on `user_stream` (nullptr: a stream of its own)
+    int init(int dev, cudaStream_t user_stream) {
         RET(require_device());
-        device = tl_device;
+        device = dev;
         CK(cudaSetDevice(device));
         RET(watchdog_init(device));
-        if (tl_user_stream) {
-            stream = tl_user_stream;
+        if (user_stream) {
+            stream = user_stream;
         } else {
             CK(own_stream.create());
             stream = own_stream.p;
@@ -397,9 +401,10 @@ struct Exec {
 };
 
 
-int make_exec(std::shared_ptr<Exec> *out) {
+// on the calling thread's device and stream (kb_set_device / kb_set_stream) unless given others
+int make_exec(std::shared_ptr<Exec> *out, int device = tl_device, cudaStream_t user_stream = tl_user_stream) {
     auto e = std::make_shared<Exec>();
-    RET(e->init());
+    RET(e->init(device, user_stream));
     *out = e;
     return KB_OK;
 }
@@ -1981,6 +1986,325 @@ int kb_place_relocalize(kb_registration *reg, kb_place_db *db, const double *des
     }
     *out = r;
     if (candidates) std::copy(m.begin(), m.end(), candidates);
+    return KB_OK;
+}
+
+// ------------------------------------------------------------------------------- Pose graph
+// The graph lives on the host (kb_pose_graph_* in the header state the problem and the method; pose_graph.cu has the
+// kernel). Edges are immutable, so an optimize uploads only those added since the last one; the poses, the fixed flags
+// and the incidence lists are uploaded every time.
+struct kb_pose_graph {
+    int device = 0;                  // of the creating thread: where the buffers go at the first optimize
+    cudaStream_t user_stream = nullptr;
+    std::vector<double> mat;         // [N][16] the poses as given or as last optimized (fixed nodes: as given, bit for bit)
+    std::vector<SE3> pose;           // [N] the same poses as the optimizer carries them
+    std::vector<int> fixed;          // [N]
+    std::vector<int> ij;             // [E][2]
+    std::vector<double> meas_inv;    // [E][8] Z^-1
+    std::vector<double> info;        // [E][36]
+    std::vector<double> robust;      // [E]
+    std::shared_ptr<Exec> ex;
+    size_t uploaded = 0;             // edges on the device
+    DBuf<double> pose_d, cand, hd, grad, D, U, UL, vec, part;
+    DBuf<double> meas_d, info_d, rob_d, e_s, e_w, e_jj, e_ii, e_ad, e_g;
+    DBuf<int> fixed_d, inc_ptr, inc, ij_d, flag;
+    DBuf<kb_pose_graph_report> report;
+    Event ev[2];                     // around the last launch (kb_debug_pose_graph_ms)
+    size_t n() const { return fixed.size(); }
+    size_t m() const { return robust.size(); }
+};
+
+static constexpr size_t kPoseGraphMaxNodes = size_t(1) << 22, kPoseGraphMaxEdges = size_t(1) << 24;
+
+static int pg_se3_arg(const double M[16], const char *what, SE3 *out) {
+    if (!M) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    for (int k = 0; k < 16; ++k)
+        if (!std::isfinite(M[k])) return fail(KB_ERR_NOT_SE3, "%s is not finite", what);
+    if (!se3_from_matrix(M, out)) return fail(KB_ERR_NOT_SE3, "%s is not in SE(3)", what);
+    return KB_OK;
+}
+
+static int pg_options_check(const kb_pose_graph_options &o) {
+    if (o.max_iterations < 0 || o.max_iterations > 1000000) return fail(KB_ERR_INVALID_ARG, "max_iterations must be in [0, 10^6]");
+    if (!(o.function_tolerance >= 0.0) || !std::isfinite(o.function_tolerance))
+        return fail(KB_ERR_INVALID_ARG, "function_tolerance must be finite and >= 0");
+    if (!(o.parameter_tolerance >= 0.0) || !std::isfinite(o.parameter_tolerance))
+        return fail(KB_ERR_INVALID_ARG, "parameter_tolerance must be finite and >= 0");
+    if (!(o.initial_lambda > 0.0 && o.initial_lambda <= 1e12)) return fail(KB_ERR_INVALID_ARG, "initial_lambda must be in (0, 1e12]");
+    if (o.max_cg_iterations < 1 || o.max_cg_iterations > 1000000) return fail(KB_ERR_INVALID_ARG, "max_cg_iterations must be in [1, 10^6]");
+    if (!(o.cg_tolerance >= 0.0 && o.cg_tolerance < 1.0)) return fail(KB_ERR_INVALID_ARG, "cg_tolerance must be in [0, 1)");
+    return KB_OK;
+}
+
+// every free node reaches a fixed node through edges (the gauge): union-find over the edges
+static int pg_gauge_check(const kb_pose_graph &g) {
+    const size_t N = g.n();
+    std::vector<size_t> parent(N);
+    std::iota(parent.begin(), parent.end(), size_t(0));
+    auto root = [&](size_t a) {
+        while (parent[a] != a) a = parent[a] = parent[parent[a]];
+        return a;
+    };
+    for (size_t e = 0; e < g.m(); ++e) {
+        const size_t a = root(static_cast<size_t>(g.ij[2 * e])), b = root(static_cast<size_t>(g.ij[2 * e + 1]));
+        if (a != b) parent[std::max(a, b)] = std::min(a, b);
+    }
+    std::vector<char> grounded(N, 0);
+    for (size_t k = 0; k < N; ++k)
+        if (g.fixed[k]) grounded[root(k)] = 1;
+    for (size_t k = 0; k < N; ++k)
+        if (!grounded[root(k)])
+            return fail(KB_ERR_INVALID_ARG, "node %zu is free and no path of edges connects it to a fixed node (the gauge is free)", k);
+    return KB_OK;
+}
+
+// device buffers for the graph as it is now; edge buffers that had to grow are uploaded again from edge 0
+static int pg_reserve(kb_pose_graph *g, int grid) {
+    const size_t N = std::max<size_t>(g->n(), 1), E = std::max<size_t>(g->m(), 1);
+    RET(g->pose_d.ensure(8 * N));
+    RET(g->cand.ensure(8 * N));
+    RET(g->hd.ensure(36 * N));
+    RET(g->D.ensure(36 * N));
+    RET(g->U.ensure(36 * N));
+    RET(g->UL.ensure(36 * N));
+    RET(g->grad.ensure(6 * N));
+    RET(g->vec.ensure(6 * 6 * N));
+    RET(g->fixed_d.ensure(N));
+    RET(g->inc_ptr.ensure(N + 1));
+    RET(g->inc.ensure(2 * E));
+    RET(g->part.ensure(4 * static_cast<size_t>(grid)));
+    if (g->flag.n == 0) {
+        CK(g->flag.alloc(1));
+        CK(cudaMemsetAsync(g->flag.p, 0, sizeof(int), g->ex->stream));
+    }
+    RET(g->report.ensure(1));
+    if (2 * E > g->ij_d.n || 8 * E > g->meas_d.n || 36 * E > g->info_d.n || E > g->rob_d.n) g->uploaded = 0;
+    RET(g->ij_d.ensure(2 * E));
+    RET(g->meas_d.ensure(8 * E));
+    RET(g->info_d.ensure(36 * E));
+    RET(g->rob_d.ensure(E));
+    RET(g->e_s.ensure(E));
+    RET(g->e_w.ensure(E));
+    RET(g->e_jj.ensure(36 * E));
+    RET(g->e_ii.ensure(36 * E));
+    RET(g->e_ad.ensure(36 * E));
+    RET(g->e_g.ensure(6 * E));
+    return KB_OK;
+}
+
+void kb_pose_graph_options_default(kb_pose_graph_options *o) {
+    if (o) *o = kb_pose_graph_options{100, 1e-12, 1e-10, 1e-4, 100, 1e-10};
+}
+int kb_pose_graph_create(kb_pose_graph **out) {
+    if (!out) return fail(KB_ERR_INVALID_ARG, "out == NULL");
+    auto g = std::make_unique<kb_pose_graph>();
+    g->device = tl_device;
+    g->user_stream = tl_user_stream;
+    *out = g.release();
+    return KB_OK;
+}
+int kb_pose_graph_destroy(kb_pose_graph *g) {
+    delete g;
+    return KB_OK;
+}
+int kb_pose_graph_add_node(kb_pose_graph *g, const double pose[16], int fixed, size_t *index) {
+    if (!g) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    SE3 T;
+    RET(pg_se3_arg(pose, "pose", &T));
+    if (g->n() >= kPoseGraphMaxNodes) return fail(KB_ERR_INVALID_ARG, "the graph holds 2^22 nodes");
+    g->mat.insert(g->mat.end(), pose, pose + 16);
+    g->pose.push_back(T);
+    g->fixed.push_back(fixed ? 1 : 0);
+    if (index) *index = g->n() - 1;
+    return KB_OK;
+}
+int kb_pose_graph_add_edge(kb_pose_graph *g, size_t i, size_t j, const double measurement[16], const double information[36],
+                           double robust_scale, size_t *index) {
+    if (!g || !information) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    SE3 Z;
+    RET(pg_se3_arg(measurement, "measurement", &Z));
+    if (i == j) return fail(KB_ERR_INVALID_ARG, "an edge joins two different nodes (i == j == %zu)", i);
+    if (i >= g->n() || j >= g->n()) return fail(KB_ERR_INVALID_ARG, "node %zu does not exist (%zu nodes)", std::max(i, j), g->n());
+    for (int k = 0; k < 36; ++k)
+        if (!std::isfinite(information[k])) return fail(KB_ERR_INVALID_ARG, "information is not finite");
+    for (int a = 0; a < 6; ++a)
+        for (int b = 0; b < a; ++b)
+            if (information[6 * a + b] != information[6 * b + a]) return fail(KB_ERR_INVALID_ARG, "information is not symmetric");
+    double L[36] = {};
+    for (int c = 0; c < 6; ++c) {  // Cholesky: positive definite
+        double d = information[7 * c];
+        for (int k = 0; k < c; ++k) d -= L[6 * c + k] * L[6 * c + k];
+        if (!(d > 0.0)) return fail(KB_ERR_INVALID_ARG, "information is not positive definite");
+        L[7 * c] = std::sqrt(d);
+        for (int r = c + 1; r < 6; ++r) {
+            double s = information[6 * r + c];
+            for (int k = 0; k < c; ++k) s -= L[6 * r + k] * L[6 * c + k];
+            L[6 * r + c] = s / L[7 * c];
+        }
+    }
+    if (!(robust_scale >= 0.0) || !std::isfinite(robust_scale)) return fail(KB_ERR_INVALID_ARG, "robust_scale must be finite and >= 0");
+    if (g->m() >= kPoseGraphMaxEdges) return fail(KB_ERR_INVALID_ARG, "the graph holds 2^24 edges");
+    const SE3 Zi = se3_inverse(Z);
+    const double zi[8] = {Zi.q.x, Zi.q.y, Zi.q.z, Zi.q.w, Zi.t.x, Zi.t.y, Zi.t.z, 0.0};
+    g->ij.push_back(static_cast<int>(i));
+    g->ij.push_back(static_cast<int>(j));
+    g->meas_inv.insert(g->meas_inv.end(), zi, zi + 8);
+    g->info.insert(g->info.end(), information, information + 36);
+    g->robust.push_back(robust_scale);
+    if (index) *index = g->m() - 1;
+    return KB_OK;
+}
+int kb_pose_graph_size(const kb_pose_graph *g, size_t *n_nodes, size_t *n_edges) {
+    if (!g || !n_nodes || !n_edges) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *n_nodes = g->n();
+    *n_edges = g->m();
+    return KB_OK;
+}
+int kb_pose_graph_poses(const kb_pose_graph *g, double *poses, size_t cap, size_t *n_out) {
+    if (!g || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *n_out = g->n();
+    if (!poses || cap == 0) return KB_OK;
+    if (cap < g->n()) return fail(KB_ERR_CAPACITY, "buffer too small (%zu < %zu poses)", cap, g->n());
+    std::copy(g->mat.begin(), g->mat.end(), poses);
+    return KB_OK;
+}
+int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_pose_graph_report *out, double *edge_chi2,
+                           double *edge_weight) {
+    if (!g || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    kb_pose_graph_options o;
+    kb_pose_graph_options_default(&o);
+    if (opt) o = *opt;
+    RET(pg_options_check(o));
+    RET(pg_gauge_check(*g));
+    RET(require_device());
+    if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
+    Exec &ex = *g->ex;
+    CK(cudaSetDevice(ex.device));
+    const size_t N = g->n(), E = g->m();
+    int co_resident = 0;
+    CK(pose_graph_max_grid(ex.sms, &co_resident));
+    const int cap = std::min(tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : ex.sms, co_resident);
+    const size_t items = std::max<size_t>(std::max(N, E), 1);
+    const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>((items + POSE_GRAPH_BLOCK - 1) / POSE_GRAPH_BLOCK, cap)));
+    RET(pg_reserve(g, grid));
+    // nodes, incidence lists (each node's edges ascending: the order its blocks are summed in), new edges
+    std::vector<double> pq(8 * N);
+    for (size_t k = 0; k < N; ++k) {
+        const SE3 &T = g->pose[k];
+        const double v[8] = {T.q.x, T.q.y, T.q.z, T.q.w, T.t.x, T.t.y, T.t.z, 0.0};
+        std::copy(v, v + 8, &pq[8 * k]);
+    }
+    std::vector<int> inc_ptr(N + 1, 0), inc(2 * E);
+    for (size_t e = 0; e < 2 * E; ++e) ++inc_ptr[static_cast<size_t>(g->ij[e]) + 1];
+    for (size_t k = 0; k < N; ++k) inc_ptr[k + 1] += inc_ptr[k];
+    {
+        std::vector<int> at(inc_ptr.begin(), inc_ptr.end() - 1);
+        for (size_t e = 0; e < E; ++e) {
+            inc[at[g->ij[2 * e]]++] = static_cast<int>(e);
+            inc[at[g->ij[2 * e + 1]]++] = static_cast<int>(e);
+        }
+    }
+    cudaStream_t s = ex.stream;
+    if (N) {
+        CK(cudaMemcpyAsync(g->pose_d.p, pq.data(), 8 * N * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->fixed_d.p, g->fixed.data(), N * sizeof(int), cudaMemcpyHostToDevice, s));
+    }
+    CK(cudaMemcpyAsync(g->inc_ptr.p, inc_ptr.data(), (N + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (E) CK(cudaMemcpyAsync(g->inc.p, inc.data(), 2 * E * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (E > g->uploaded) {
+        const size_t a = g->uploaded, n = E - a;
+        CK(cudaMemcpyAsync(g->ij_d.p + 2 * a, &g->ij[2 * a], 2 * n * sizeof(int), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->meas_d.p + 8 * a, &g->meas_inv[8 * a], 8 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->info_d.p + 36 * a, &g->info[36 * a], 36 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->rob_d.p + a, &g->robust[a], n * sizeof(double), cudaMemcpyHostToDevice, s));
+    }
+    PoseGraphParams P{};
+    P.bar = ex.sc.bar;
+    P.n_nodes = static_cast<int>(N);
+    P.n_edges = static_cast<int>(E);
+    P.pose = g->pose_d.p;
+    P.cand = g->cand.p;
+    P.fixed = g->fixed_d.p;
+    P.inc_ptr = g->inc_ptr.p;
+    P.inc = g->inc.p;
+    P.ij = g->ij_d.p;
+    P.meas_inv = g->meas_d.p;
+    P.info = g->info_d.p;
+    P.robust = g->rob_d.p;
+    P.e_s = g->e_s.p;
+    P.e_w = g->e_w.p;
+    P.e_jj = g->e_jj.p;
+    P.e_ii = g->e_ii.p;
+    P.e_ad = g->e_ad.p;
+    P.e_g = g->e_g.p;
+    P.hd = g->hd.p;
+    P.g = g->grad.p;
+    P.D = g->D.p;
+    P.U = g->U.p;
+    P.UL = g->UL.p;
+    const size_t V = 6 * std::max<size_t>(N, 1);
+    P.x = g->vec.p;
+    P.r = P.x + V;
+    P.z = P.r + V;
+    P.p = P.z + V;
+    P.q = P.p + V;
+    P.y = P.q + V;
+    P.part = g->part.p;
+    P.flag = g->flag.p;
+    P.report = g->report.p;
+    P.max_iterations = o.max_iterations;
+    P.max_cg_iterations = o.max_cg_iterations;
+    P.function_tolerance = o.function_tolerance;
+    P.parameter_tolerance = o.parameter_tolerance;
+    P.initial_lambda = o.initial_lambda;
+    P.cg_tolerance = o.cg_tolerance;
+    if (g->ev[1].device != ex.device) {  // (ev[1] is made last: both exist on that device)
+        CK(g->ev[0].create(cudaEventDefault));
+        CK(g->ev[1].create(cudaEventDefault));
+    }
+    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
+    ex.bar_dirty = true;
+    CK(cudaEventRecord(g->ev[0].p, s));
+    CK(pose_graph_launch(P, grid, s));
+    ++ex.launches;
+    CK(cudaEventRecord(g->ev[1].p, s));
+    kb_pose_graph_report rep{};
+    CK(cudaMemcpyAsync(&rep, g->report.p, sizeof(rep), cudaMemcpyDeviceToHost, s));
+    if (N) CK(cudaMemcpyAsync(pq.data(), g->pose_d.p, 8 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
+    std::vector<double> chi2(edge_chi2 ? E : 0), weight(edge_weight ? E : 0);
+    if (edge_chi2 && E) CK(cudaMemcpyAsync(chi2.data(), g->e_s.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (edge_weight && E) CK(cudaMemcpyAsync(weight.data(), g->e_w.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
+    RET(ex.sync());
+    g->uploaded = E;
+    for (size_t k = 0; k < N; ++k) {
+        if (g->fixed[k]) continue;
+        const double *v = &pq[8 * k];
+        g->pose[k] = SE3{{v[0], v[1], v[2], v[3]}, {v[4], v[5], v[6]}};
+        se3_to_matrix(g->pose[k], &g->mat[16 * k]);
+    }
+    *out = rep;
+    std::copy(chi2.begin(), chi2.end(), edge_chi2 ? edge_chi2 : chi2.data());
+    std::copy(weight.begin(), weight.end(), edge_weight ? edge_weight : weight.data());
+    return KB_OK;
+}
+
+int kb_debug_pose_graph_ms(const kb_pose_graph *g, float *ms) {
+    if (!g || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (!g->ev[1].p) return fail(KB_ERR_INVALID_ARG, "no optimize has run on this graph");
+    CK(cudaSetDevice(g->ex->device));
+    CK(cudaEventElapsedTime(ms, g->ev[0].p, g->ev[1].p));
+    return KB_OK;
+}
+int kb_debug_se3_adjoint(const double T[16], double A[36]) {
+    if (!A) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    SE3 X;
+    RET(pg_se3_arg(T, "T", &X));
+    se3_adjoint(X, A);
+    return KB_OK;
+}
+int kb_debug_se3_right_jacobian_inverse(const double x[6], double J[36]) {
+    if (!x || !J) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    se3_right_jacobian_inverse(x, J);
     return KB_OK;
 }
 

@@ -1,0 +1,688 @@
+// The pose-graph optimizer (kb_pose_graph_optimize in api.cu): Levenberg-Marquardt with IRLS weights, the damped normal
+// equations solved by PCG with the exact inverse of their block-tridiagonal part, applied by block cyclic reduction.
+// The whole optimization is one persistent cooperative launch on the Grid barrier of device_ops.cuh. Like localize.cu,
+// the unit compiles the header in a namespace of its own (and so has its own copies of the device watchdog's words,
+// which api.cu sets and re-arms through the functions at the end), and a kernel here changes no code generated for the
+// kernels of the other units.
+//
+// Determinism: every sum is formed in a fixed order. A node's blocks add their edges' contributions in ascending edge
+// order; every dot product and the cost are summed per thread over its grid-stride items, then by a fixed tree in the
+// CTA, then over the CTAs in index order. No floating-point atomics: a result depends on the grid size only.
+#define kb kb_pg
+#include "device_ops.cuh"
+#undef kb
+
+#include <algorithm>
+
+#include "pose_graph.cuh"
+
+namespace kb_pg {
+
+constexpr int PB = POSE_GRAPH_BLOCK;
+
+__device__ __forceinline__ SE3 ld_pose(const double *p) { return SE3{{p[0], p[1], p[2], p[3]}, {p[4], p[5], p[6]}}; }
+__device__ __forceinline__ void st_pose(double *p, const SE3 &T) {
+    p[0] = T.q.x;
+    p[1] = T.q.y;
+    p[2] = T.q.z;
+    p[3] = T.q.w;
+    p[4] = T.t.x;
+    p[5] = T.t.y;
+    p[6] = T.t.z;
+    p[7] = 0.0;
+}
+
+// y = A v, A^T v, A 6x6 row-major
+__device__ __forceinline__ void mv6(const double *A, const double v[6], double y[6]) {
+#pragma unroll
+    for (int a = 0; a < 6; ++a) {
+        double s = 0.0;
+#pragma unroll
+        for (int b = 0; b < 6; ++b) s = s + A[6 * a + b] * v[b];
+        y[a] = s;
+    }
+}
+__device__ __forceinline__ void mtv6(const double *A, const double v[6], double y[6]) {
+#pragma unroll
+    for (int a = 0; a < 6; ++a) {
+        double s = 0.0;
+#pragma unroll
+        for (int b = 0; b < 6; ++b) s = s + A[6 * b + a] * v[b];
+        y[a] = s;
+    }
+}
+
+struct Red {
+    double *part;  // [2][2][grid]
+    int seq;       // which half the next reduction uses (the same in every thread)
+};
+
+// sum (or max, MAX) of v[K] over every thread of the grid, in a fixed order; the result is in every thread. One grid
+// barrier. Consecutive reductions alternate between two halves of the partials: a CTA may start the next reduction
+// while another still reads this one's.
+template <int K, bool MAX = false>
+__device__ void grid_reduce(Grid &g, Red &rd, const double (&v)[K], double (&out)[K], double *s_red, double *s_out) {
+    const int t = threadIdx.x;
+#pragma unroll
+    for (int k = 0; k < K; ++k) s_red[k * PB + t] = v[k];
+    __syncthreads();
+    for (int w = PB / 2; w > 0; w >>= 1) {
+        if (t < w)
+#pragma unroll
+            for (int k = 0; k < K; ++k)
+                s_red[k * PB + t] = MAX ? fmax(s_red[k * PB + t], s_red[k * PB + t + w]) : s_red[k * PB + t] + s_red[k * PB + t + w];
+        __syncthreads();
+    }
+    double *part = rd.part + static_cast<size_t>(rd.seq & 1) * 2 * gridDim.x;
+    ++rd.seq;
+    if (t == 0)
+#pragma unroll
+        for (int k = 0; k < K; ++k) part[k * gridDim.x + blockIdx.x] = s_red[k * PB];
+    g.sync();
+    if (t == 0)
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            double s = 0.0;  // (the maxima are of absolute values)
+            for (unsigned b = 0; b < gridDim.x; ++b) {
+                const double u = __ldcg(&part[k * gridDim.x + b]);
+                s = MAX ? fmax(s, u) : s + u;
+            }
+            s_out[k] = s;
+        }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < K; ++k) out[k] = s_out[k];
+    __syncthreads();
+}
+
+// r_e = Log(Z^-1 T_i^-1 T_j), s_e = r^T Omega r, rho(s_e) and w_e = rho'(s_e)
+struct EdgeEval {
+    SE3 Ti, Tj;
+    double r[6], s, rho, w;
+};
+__device__ __forceinline__ EdgeEval edge_eval(const PoseGraphParams &P, const double *poses, int e) {
+    EdgeEval v;
+    const int i = P.ij[2 * e], j = P.ij[2 * e + 1];
+    v.Ti = ld_pose(poses + 8 * static_cast<size_t>(i));
+    v.Tj = ld_pose(poses + 8 * static_cast<size_t>(j));
+    const SE3 E = se3_mul(ld_pose(P.meas_inv + 8 * static_cast<size_t>(e)), se3_mul(se3_inverse(v.Ti), v.Tj));
+    se3_log(E, v.r);
+    double Or[6];
+    mv6(P.info + 36 * static_cast<size_t>(e), v.r, Or);
+    double s = 0.0;
+#pragma unroll
+    for (int a = 0; a < 6; ++a) s = s + v.r[a] * Or[a];
+    v.s = s;
+    const double c = P.robust[e];
+    if (c > 0.0) {
+        const double c2 = c * c;
+        v.rho = c2 * log1p(s / c2);
+        v.w = 1.0 / (1.0 + s / c2);
+    } else {
+        v.rho = s;
+        v.w = 1.0;
+    }
+    return v;
+}
+
+// the edge's part of the linearization: B = J_r^-1(r), A = -B Ad(T_j^-1 T_i), W = w Omega.
+// Bt W B and At W A = Ad^T (Bt W B) Ad are formed on the upper triangle and mirrored (exactly symmetric);
+// At W B = -Ad^T (Bt W B) is applied from these two where it is needed.
+// Returns rho(s_e).
+__device__ __noinline__ double edge_linearize(const PoseGraphParams &P, const double *poses, int e) {
+    const EdgeEval v = edge_eval(P, poses, e);
+    P.e_s[e] = v.s;
+    P.e_w[e] = v.w;
+    const double *Om = P.info + 36 * static_cast<size_t>(e);
+    double *Ejj = P.e_jj + 36 * static_cast<size_t>(e);
+    double *Eii = P.e_ii + 36 * static_cast<size_t>(e);
+    double *Ad = P.e_ad + 36 * static_cast<size_t>(e);
+    {
+        double J[36];
+        se3_right_jacobian_inverse(v.r, J);
+        double Or[6], gj[6];
+        mv6(Om, v.r, Or);
+        mtv6(J, Or, gj);
+#pragma unroll
+        for (int a = 0; a < 6; ++a) P.e_g[6 * static_cast<size_t>(e) + a] = v.w * gj[a];
+#pragma unroll
+        for (int b = 0; b < 6; ++b) {
+            double col[6], x[6];
+#pragma unroll
+            for (int k = 0; k < 6; ++k) col[k] = J[6 * k + b];
+            mv6(Om, col, x);  // Omega J[:, b]
+#pragma unroll
+            for (int a = 0; a <= b; ++a) {
+                double s = 0.0;
+#pragma unroll
+                for (int m = 0; m < 6; ++m) s = s + J[6 * m + a] * x[m];
+                Ejj[6 * a + b] = Ejj[6 * b + a] = v.w * s;
+            }
+        }
+    }
+    double A[36];
+    se3_adjoint(se3_mul(se3_inverse(v.Tj), v.Ti), A);
+#pragma unroll
+    for (int k = 0; k < 36; ++k) Ad[k] = A[k];
+#pragma unroll
+    for (int b = 0; b < 6; ++b) {
+        double col[6], y[6];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) col[k] = A[6 * k + b];
+        mv6(Ejj, col, y);  // Ejj Ad[:, b]
+#pragma unroll
+        for (int a = 0; a <= b; ++a) {
+            double s = 0.0;
+#pragma unroll
+            for (int m = 0; m < 6; ++m) s = s + A[6 * m + a] * y[m];
+            Eii[6 * a + b] = Eii[6 * b + a] = s;
+        }
+    }
+    return v.rho;
+}
+
+// in place: the inverse of the SPD 6x6 at M (Cholesky); false when a pivot is not positive and finite
+__device__ __noinline__ bool inv6_spd(double *M) {
+    double L[6][6];
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+#pragma unroll
+        for (int j = 0; j < 6; ++j) L[i][j] = j <= i ? M[6 * i + j] : 0.0;
+    bool ok = true;
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+        double d = L[j][j];
+#pragma unroll
+        for (int k = 0; k < j; ++k) d = d - L[j][k] * L[j][k];
+        ok = ok && d > 0.0 && d < INFINITY;
+        const double l = sqrt(fmax(d, 1e-300));
+        const double il = 1.0 / l;
+        L[j][j] = l;
+#pragma unroll
+        for (int i = j + 1; i < 6; ++i) {
+            double s = L[i][j];
+#pragma unroll
+            for (int k = 0; k < j; ++k) s = s - L[i][k] * L[j][k];
+            L[i][j] = s * il;
+        }
+    }
+    // X = L^-1 (lower), M^-1 = X^T X
+    double X[6][6];
+#pragma unroll
+    for (int c = 0; c < 6; ++c)
+#pragma unroll
+        for (int i = 0; i < 6; ++i) {
+            if (i < c) {
+                X[i][c] = 0.0;
+                continue;
+            }
+            double s = i == c ? 1.0 : 0.0;
+#pragma unroll
+            for (int k = c; k < i; ++k) s = s - L[i][k] * X[k][c];
+            X[i][c] = s / L[i][i];
+        }
+#pragma unroll
+    for (int a = 0; a < 6; ++a)
+#pragma unroll
+        for (int b = a; b < 6; ++b) {
+            double s = 0.0;
+#pragma unroll
+            for (int k = b; k < 6; ++k) s = s + X[k][a] * X[k][b];
+            M[6 * a + b] = M[6 * b + a] = s;
+        }
+    return ok;
+}
+
+// the products of the reduction, column by column through 6-vectors: D -= X^T Y X, D -= X Y X^T, U = -X Y Z
+__device__ __noinline__ void sub_xt_y_x(double *D, const double *X, const double *Y) {
+#pragma unroll 1
+    for (int b = 0; b < 6; ++b) {
+        double col[6], t[6];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) col[k] = X[6 * k + b];
+        mv6(Y, col, t);
+#pragma unroll
+        for (int a = 0; a < 6; ++a) {
+            double s = 0.0;
+#pragma unroll
+            for (int m = 0; m < 6; ++m) s = s + X[6 * m + a] * t[m];
+            D[6 * a + b] = D[6 * a + b] - s;
+        }
+    }
+}
+__device__ __noinline__ void sub_x_y_xt(double *D, const double *X, const double *Y) {
+#pragma unroll 1
+    for (int b = 0; b < 6; ++b) {
+        double col[6], t[6];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) col[k] = X[6 * b + k];
+        mv6(Y, col, t);
+#pragma unroll
+        for (int a = 0; a < 6; ++a) {
+            double s = 0.0;
+#pragma unroll
+            for (int m = 0; m < 6; ++m) s = s + X[6 * a + m] * t[m];
+            D[6 * a + b] = D[6 * a + b] - s;
+        }
+    }
+}
+__device__ __noinline__ void set_neg_x_y_z(double *U, const double *X, const double *Y, const double *Z) {
+#pragma unroll 1
+    for (int b = 0; b < 6; ++b) {
+        double col[6], t[6];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) col[k] = Z[6 * k + b];
+        mv6(Y, col, t);
+#pragma unroll
+        for (int a = 0; a < 6; ++a) {
+            double s = 0.0;
+#pragma unroll
+            for (int m = 0; m < 6; ++m) s = s + X[6 * a + m] * t[m];
+            U[6 * a + b] = -s;
+        }
+    }
+}
+
+// (H + lambda diag H) v at free node k; fixed nodes are identity rows
+__device__ __noinline__ void matvec_node(const PoseGraphParams &P, int k, double lambda, const double *v, double *out) {
+    double y[6];
+    const double *vk = v + 6 * static_cast<size_t>(k);
+    if (P.fixed[k]) {
+#pragma unroll
+        for (int a = 0; a < 6; ++a) out[6 * static_cast<size_t>(k) + a] = vk[a];
+        return;
+    }
+    const double *H = P.hd + 36 * static_cast<size_t>(k);
+    double vv[6];
+#pragma unroll
+    for (int a = 0; a < 6; ++a) vv[a] = vk[a];
+    mv6(H, vv, y);
+#pragma unroll
+    for (int a = 0; a < 6; ++a) y[a] = y[a] + (lambda * H[7 * a]) * vv[a];
+    for (int t = P.inc_ptr[k]; t < P.inc_ptr[k + 1]; ++t) {
+        const int e = P.inc[t];
+        const int i = P.ij[2 * e], j = P.ij[2 * e + 1];
+        const int o = i == k ? j : i;
+        if (P.fixed[o]) continue;
+        double vo[6], u[6], w[6];
+#pragma unroll
+        for (int a = 0; a < 6; ++a) vo[a] = v[6 * static_cast<size_t>(o) + a];
+        const double *Ejj = P.e_jj + 36 * static_cast<size_t>(e), *Ad = P.e_ad + 36 * static_cast<size_t>(e);
+        if (i == k) {  // (At W B) v_j = -Ad^T (Ejj v_j)
+            mv6(Ejj, vo, u);
+            mtv6(Ad, u, w);
+        } else {  // (At W B)^T v_i = -Ejj (Ad v_i)
+            mv6(Ad, vo, u);
+            mv6(Ejj, u, w);
+        }
+#pragma unroll
+        for (int a = 0; a < 6; ++a) y[a] = y[a] - w[a];
+    }
+#pragma unroll
+    for (int a = 0; a < 6; ++a) out[6 * static_cast<size_t>(k) + a] = y[a];
+}
+
+// diagonal block, gradient, damped M diagonal block and chain coupling of node k
+__device__ __noinline__ void assemble_node(const PoseGraphParams &P, int k, double lambda) {
+    const int N = P.n_nodes;
+    double *Hk = P.hd + 36 * static_cast<size_t>(k), *Dk = P.D + 36 * static_cast<size_t>(k);
+    double *Uk = P.U + 36 * static_cast<size_t>(k), *gk = P.g + 6 * static_cast<size_t>(k);
+    if (P.fixed[k]) {
+#pragma unroll
+        for (int a = 0; a < 36; ++a) {
+            Hk[a] = 0.0;
+            Dk[a] = a % 7 == 0 ? 1.0 : 0.0;
+            Uk[a] = 0.0;
+        }
+#pragma unroll
+        for (int a = 0; a < 6; ++a) gk[a] = 0.0;
+        return;
+    }
+    double g[6] = {0, 0, 0, 0, 0, 0};
+#pragma unroll
+    for (int a = 0; a < 36; ++a) Hk[a] = 0.0;
+    for (int t = P.inc_ptr[k]; t < P.inc_ptr[k + 1]; ++t) {
+        const int e = P.inc[t];
+        const bool is_i = P.ij[2 * e] == k;
+        const double *E = (is_i ? P.e_ii : P.e_jj) + 36 * static_cast<size_t>(e);
+#pragma unroll 6
+        for (int a = 0; a < 36; ++a) Hk[a] = Hk[a] + E[a];
+        const double *gj = P.e_g + 6 * static_cast<size_t>(e);
+        double gg[6], u[6];
+#pragma unroll
+        for (int a = 0; a < 6; ++a) gg[a] = gj[a];
+        if (is_i) {  // At W r = -Ad^T (Bt W r)
+            mtv6(P.e_ad + 36 * static_cast<size_t>(e), gg, u);
+#pragma unroll
+            for (int a = 0; a < 6; ++a) g[a] = g[a] - u[a];
+        } else {
+#pragma unroll
+            for (int a = 0; a < 6; ++a) g[a] = g[a] + gg[a];
+        }
+    }
+#pragma unroll
+    for (int a = 0; a < 6; ++a) gk[a] = g[a];
+#pragma unroll
+    for (int a = 0; a < 36; ++a) Dk[a] = a % 7 == 0 ? Hk[a] + lambda * Hk[a] : Hk[a];
+    // block (k, k + 1) of the chain: the edges between k and k + 1, in full
+#pragma unroll
+    for (int a = 0; a < 36; ++a) Uk[a] = 0.0;
+    if (k + 1 >= N || P.fixed[k + 1]) return;
+    for (int t = P.inc_ptr[k]; t < P.inc_ptr[k + 1]; ++t) {
+        const int e = P.inc[t];
+        const int i = P.ij[2 * e], j = P.ij[2 * e + 1];
+        if ((i == k ? j : i) != k + 1) continue;
+        const double *Ejj = P.e_jj + 36 * static_cast<size_t>(e), *Ad = P.e_ad + 36 * static_cast<size_t>(e);
+#pragma unroll 1
+        for (int a = 0; a < 6; ++a)
+#pragma unroll
+            for (int b = 0; b < 6; ++b) {
+                double s = 0.0;
+                if (i == k) {  // At W B = -Ad^T Ejj
+#pragma unroll
+                    for (int m = 0; m < 6; ++m) s = s + Ad[6 * m + a] * Ejj[6 * m + b];
+                } else {  // (At W B)^T = -Ejj Ad
+#pragma unroll
+                    for (int m = 0; m < 6; ++m) s = s + Ejj[6 * a + m] * Ad[6 * m + b];
+                }
+                Uk[6 * a + b] = Uk[6 * a + b] - s;
+            }
+    }
+}
+
+struct PgShared {
+    double red[2 * PB];
+    double out[2];
+};
+
+// Block cyclic reduction of M (in place). Level s = 1, 2, 4, ...: the nodes that are odd multiples of s are eliminated
+// (D becomes D^-1; UL keeps the coupling from the left neighbour k - s), then every even multiple k of s takes
+// D_k -= U_{k-s}^T D_{k-s}^-1 U_{k-s} + UL_{k+s} D_{k+s}^-1 UL_{k+s}^T and couples to k + 2s by
+// -UL_{k+s} D_{k+s}^-1 U_{k+s}. Node 0 is left; it is inverted last. A block that is not SPD (rounding on a nearly
+// singular system) sets *flag = mark; marks grow from call to call, so the flag is never reset while a CTA reads it.
+__device__ void bcr_factor(Grid &g, const PoseGraphParams &P, int mark, long long gt, long long gs) {
+    const long long N = P.n_nodes;
+    for (long long s = 1; s < N; s *= 2) {
+        for (long long m = gt; s * (2 * m + 1) < N; m += gs) {
+            const long long k = s * (2 * m + 1);
+            if (!inv6_spd(P.D + 36 * k)) *P.flag = mark;
+            const double *src = P.U + 36 * (k - s);
+            double *dst = P.UL + 36 * k;
+#pragma unroll 6
+            for (int a = 0; a < 36; ++a) dst[a] = src[a];
+        }
+        g.sync();
+        for (long long m = gt; 2 * s * m < N; m += gs) {
+            const long long k = 2 * s * m;
+            double *Dk = P.D + 36 * k, *Uk = P.U + 36 * k;
+            if (k >= s) sub_xt_y_x(Dk, P.U + 36 * (k - s), P.D + 36 * (k - s));
+            if (k + s < N) {
+                const long long o = k + s;
+                sub_x_y_xt(Dk, P.UL + 36 * o, P.D + 36 * o);
+                set_neg_x_y_z(Uk, P.UL + 36 * o, P.D + 36 * o, P.U + 36 * o);
+            } else {
+#pragma unroll 6
+                for (int a = 0; a < 36; ++a) Uk[a] = 0.0;
+            }
+        }
+        g.sync();
+    }
+    if (gt == 0 && !inv6_spd(P.D)) *P.flag = mark;
+    g.sync();
+}
+
+// z = M^-1 r with the factors of bcr_factor (y: workspace)
+__device__ void bcr_solve(Grid &g, const PoseGraphParams &P, long long gt, long long gs) {
+    const long long N = P.n_nodes;
+    for (long long k = gt; k < N; k += gs)
+#pragma unroll
+        for (int a = 0; a < 6; ++a) P.y[6 * k + a] = P.r[6 * k + a];
+    g.sync();
+    long long top = 1;
+    for (long long s = 1; s < N; s *= 2) {
+        for (long long m = gt; 2 * s * m < N; m += gs) {
+            const long long k = 2 * s * m;
+            double yk[6], t[6], u[6], w[6];
+#pragma unroll
+            for (int a = 0; a < 6; ++a) yk[a] = P.y[6 * k + a];
+            if (k >= s) {
+                const long long o = k - s;
+#pragma unroll
+                for (int a = 0; a < 6; ++a) t[a] = P.y[6 * o + a];
+                mv6(P.D + 36 * o, t, u);
+                mtv6(P.U + 36 * o, u, w);
+#pragma unroll
+                for (int a = 0; a < 6; ++a) yk[a] = yk[a] - w[a];
+            }
+            if (k + s < N) {
+                const long long o = k + s;
+#pragma unroll
+                for (int a = 0; a < 6; ++a) t[a] = P.y[6 * o + a];
+                mv6(P.D + 36 * o, t, u);
+                mv6(P.UL + 36 * o, u, w);
+#pragma unroll
+                for (int a = 0; a < 6; ++a) yk[a] = yk[a] - w[a];
+            }
+#pragma unroll
+            for (int a = 0; a < 6; ++a) P.y[6 * k + a] = yk[a];
+        }
+        g.sync();
+        top = s;
+    }
+    if (gt == 0) {
+        double t[6], u[6];
+#pragma unroll
+        for (int a = 0; a < 6; ++a) t[a] = P.y[a];
+        mv6(P.D, t, u);
+#pragma unroll
+        for (int a = 0; a < 6; ++a) P.z[a] = u[a];
+    }
+    g.sync();
+    if (N < 2) return;
+    for (long long s = top; s >= 1; s /= 2) {
+        for (long long m = gt; s * (2 * m + 1) < N; m += gs) {
+            const long long k = s * (2 * m + 1);
+            double b[6], t[6], u[6];
+#pragma unroll
+            for (int a = 0; a < 6; ++a) {
+                b[a] = P.y[6 * k + a];
+                t[a] = P.z[6 * (k - s) + a];
+            }
+            mtv6(P.UL + 36 * k, t, u);
+#pragma unroll
+            for (int a = 0; a < 6; ++a) b[a] = b[a] - u[a];
+            if (k + s < N) {
+#pragma unroll
+                for (int a = 0; a < 6; ++a) t[a] = P.z[6 * (k + s) + a];
+                mv6(P.U + 36 * k, t, u);
+#pragma unroll
+                for (int a = 0; a < 6; ++a) b[a] = b[a] - u[a];
+            }
+            mv6(P.D + 36 * k, b, u);
+#pragma unroll
+            for (int a = 0; a < 6; ++a) P.z[6 * k + a] = u[a];
+        }
+        g.sync();
+    }
+}
+
+// 1/2 sum_e rho(s_e) at `poses`; with `linearize` also every edge's linearization
+__device__ double edges_pass(Grid &g, Red &rd, PgShared &sh, const PoseGraphParams &P, const double *poses, bool linearize,
+                             long long gt, long long gs) {
+    double c[1] = {0.0}, out[1];
+    for (long long e = gt; e < P.n_edges; e += gs)
+        c[0] = c[0] + (linearize ? edge_linearize(P, poses, static_cast<int>(e)) : edge_eval(P, poses, static_cast<int>(e)).rho);
+    grid_reduce<1>(g, rd, c, out, sh.red, sh.out);
+    return 0.5 * out[0];
+}
+
+enum { T_FUNCTION = KB_PG_FUNCTION_TOLERANCE, T_STEP = KB_PG_PARAMETER_TOLERANCE, T_MAX = KB_PG_MAX_ITERATIONS,
+       T_NO_DECREASE = KB_PG_NO_DECREASE };
+
+__global__ void __launch_bounds__(PB, 1) k_pose_graph(const PoseGraphParams P) {
+    __shared__ PgShared sh;
+    Grid g;
+    g.init(P.bar);
+    Red rd{P.part, 0};
+    const long long gt = static_cast<long long>(blockIdx.x) * PB + threadIdx.x, gs = static_cast<long long>(gridDim.x) * PB;
+    const long long N = P.n_nodes;
+    double *cur = P.pose, *cand = P.cand;
+    double F = edges_pass(g, rd, sh, P, cur, true, gt, gs);
+    const double F0 = F;
+    double lambda = P.initial_lambda;
+    int iterations = 0, accepted = 0, cg_total = 0, term = T_MAX;
+    while (iterations < P.max_iterations) {
+        for (long long k = gt; k < N; k += gs) assemble_node(P, static_cast<int>(k), lambda);
+        g.sync();
+        bcr_factor(g, P, iterations + 1, gt, gs);
+        const bool factored = *reinterpret_cast<volatile int *>(P.flag) != iterations + 1;  // (written before the last barrier)
+        double step = 0.0;
+        if (factored) {
+            // PCG on (H + lambda diag H) x = -g from x = 0
+            for (long long k = gt; k < N; k += gs)
+#pragma unroll
+                for (int a = 0; a < 6; ++a) {
+                    P.x[6 * k + a] = 0.0;
+                    P.r[6 * k + a] = -P.g[6 * k + a];
+                }
+            g.sync();
+            bcr_solve(g, P, gt, gs);
+            double v[2] = {0.0, 0.0}, o[2];
+            for (long long k = gt; k < N; k += gs)
+#pragma unroll
+                for (int a = 0; a < 6; ++a) {
+                    const double r = P.r[6 * k + a], z = P.z[6 * k + a];
+                    P.p[6 * k + a] = z;
+                    v[0] = v[0] + r * z;
+                    v[1] = v[1] + r * r;
+                }
+            grid_reduce<2>(g, rd, v, o, sh.red, sh.out);
+            double rz = o[0];
+            const double rr0 = o[1];
+            const double stop = P.cg_tolerance * P.cg_tolerance * rr0;
+            for (int it = 0; it < P.max_cg_iterations && rr0 > 0.0; ++it) {
+                double pq[1] = {0.0}, opq[1];
+                for (long long k = gt; k < N; k += gs) {
+                    matvec_node(P, static_cast<int>(k), lambda, P.p, P.q);
+#pragma unroll
+                    for (int a = 0; a < 6; ++a) pq[0] = pq[0] + P.p[6 * k + a] * P.q[6 * k + a];
+                }
+                grid_reduce<1>(g, rd, pq, opq, sh.red, sh.out);
+                ++cg_total;
+                if (!(opq[0] > 0.0) || !(rz > 0.0)) break;
+                const double alpha = rz / opq[0];
+                double rr[1] = {0.0}, orr[1];
+                for (long long k = gt; k < N; k += gs)
+#pragma unroll
+                    for (int a = 0; a < 6; ++a) {
+                        P.x[6 * k + a] = P.x[6 * k + a] + alpha * P.p[6 * k + a];
+                        const double r = P.r[6 * k + a] - alpha * P.q[6 * k + a];
+                        P.r[6 * k + a] = r;
+                        rr[0] = rr[0] + r * r;
+                    }
+                grid_reduce<1>(g, rd, rr, orr, sh.red, sh.out);
+                if (orr[0] <= stop) break;
+                bcr_solve(g, P, gt, gs);
+                double rz1[1] = {0.0}, orz[1];
+                for (long long k = gt; k < N; k += gs)
+#pragma unroll
+                    for (int a = 0; a < 6; ++a) rz1[0] = rz1[0] + P.r[6 * k + a] * P.z[6 * k + a];
+                grid_reduce<1>(g, rd, rz1, orz, sh.red, sh.out);
+                const double beta = orz[0] / rz;
+                rz = orz[0];
+                for (long long k = gt; k < N; k += gs)
+#pragma unroll
+                    for (int a = 0; a < 6; ++a) P.p[6 * k + a] = P.z[6 * k + a] + beta * P.p[6 * k + a];
+                g.sync();
+            }
+            // candidate T_k Exp(x_k), and max |x|
+            double mx[1] = {0.0}, omx[1];
+            for (long long k = gt; k < N; k += gs) {
+                const double *src = cur + 8 * k;
+                double *dst = cand + 8 * k;
+                if (P.fixed[k]) {
+#pragma unroll
+                    for (int a = 0; a < 8; ++a) dst[a] = src[a];
+                    continue;
+                }
+                double d[6];
+#pragma unroll
+                for (int a = 0; a < 6; ++a) {
+                    d[a] = P.x[6 * k + a];
+                    mx[0] = fmax(mx[0], fabs(d[a]));
+                }
+                st_pose(dst, se3_mul(ld_pose(src), se3_exp(d)));
+            }
+            grid_reduce<1, true>(g, rd, mx, omx, sh.red, sh.out);
+            step = omx[0];
+        }
+        ++iterations;
+        const double Fc = factored ? edges_pass(g, rd, sh, P, cand, false, gt, gs) : NAN;
+        if (Fc < F) {  // (false for a non-finite cost)
+            double *t = cur;
+            cur = cand;
+            cand = t;
+            const double F_old = F;
+            F = Fc;
+            lambda = lambda / 10.0;
+            ++accepted;
+            edges_pass(g, rd, sh, P, cur, true, gt, gs);
+            if (F_old - F <= P.function_tolerance * F_old) {
+                term = T_FUNCTION;
+                break;
+            }
+        } else {
+            lambda = lambda * 10.0;
+            if (lambda > 1e12) {
+                term = T_NO_DECREASE;
+                break;
+            }
+        }
+        if (factored && step <= P.parameter_tolerance) {
+            term = T_STEP;
+            break;
+        }
+    }
+    if (cur != P.pose) {
+        for (long long k = gt; k < N; k += gs)
+#pragma unroll
+            for (int a = 0; a < 8; ++a) P.pose[8 * k + a] = cur[8 * k + a];
+    }
+    if (gt == 0) {
+        kb_pose_graph_report r;
+        r.iterations = iterations;
+        r.accepted = accepted;
+        r.cg_iterations = cg_total;
+        r.termination = term;
+        r.initial_cost = F0;
+        r.final_cost = F;
+        r.lambda = lambda;
+        *P.report = r;
+    }
+}
+
+}  // namespace kb_pg
+
+cudaError_t pose_graph_max_grid(int sms, int *out) {
+    int per_sm = 0;
+    const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kb_pg::k_pose_graph, POSE_GRAPH_BLOCK, 0);
+    *out = per_sm * sms;
+    return e;
+}
+
+cudaError_t pose_graph_launch(const PoseGraphParams &P, int grid, cudaStream_t s) {
+    void *args[] = {const_cast<PoseGraphParams *>(&P)};
+    return cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(&kb_pg::k_pose_graph), dim3(grid),
+                                       dim3(POSE_GRAPH_BLOCK), args, 0, s);
+}
+
+cudaError_t pose_graph_watchdog_init(unsigned *d_host_words, const unsigned init[8]) {
+    cudaError_t e = cudaMemcpyToSymbol(kb_pg::g_kb_wd_host, &d_host_words, sizeof(d_host_words));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(kb_pg::g_kb_wd, init, 8 * sizeof(unsigned));
+    return e;
+}
+
+cudaError_t pose_graph_watchdog_rearm() {
+    const unsigned zero = 0;
+    return cudaMemcpyToSymbol(kb_pg::g_kb_wd, &zero, sizeof(zero));
+}

@@ -559,6 +559,88 @@ KB_HD bool icp_solve_schur(const double acc[16], double dx[6]) {
     return true;
 }
 
+// ---- Jacobians of the pose graph (kb_pose_graph_optimize) -------------------------------------------------------------
+// Tangent order (translation, rotation), as se3_exp / se3_log; 6x6 matrices row-major.
+// Ad(T) = [R, hat(t) R; 0, R]: T Exp(x) T^-1 = Exp(Ad(T) x).
+KB_HD void se3_adjoint(const SE3 &T, double A[36]) {
+    const M3 R = q_to_matrix(T.q);
+    const double th[3][3] = {{0.0, -T.t.z, T.t.y}, {T.t.z, 0.0, -T.t.x}, {-T.t.y, T.t.x, 0.0}};
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            A[6 * i + j] = R.m[i][j];
+            A[6 * i + j + 3] = (th[i][0] * R.m[0][j] + th[i][1] * R.m[1][j]) + th[i][2] * R.m[2][j];
+            A[6 * (i + 3) + j] = 0.0;
+            A[6 * (i + 3) + j + 3] = R.m[i][j];
+        }
+}
+
+KB_HD void m3_mul(const double a[3][3], const double b[3][3], double c[3][3]) {
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) c[i][j] = (a[i][0] * b[0][j] + a[i][1] * b[1][j]) + a[i][2] * b[2][j];
+}
+
+// J_r^-1(x): Log(Exp(x) Exp(d)) = x + J_r^-1(x) d + O(|d|^2). J_r^-1(x) = J_l^-1(-x), with (rho, phi) = -x,
+//   J_l^-1 = [S, -S Q S; 0, S],  S = I - hat(phi)/2 + c hat(phi)^2,  c = 1/t^2 - (1 + cos t) / (2 t sin t),  t = |phi|,
+//   Q = hat(rho)/2 + c1 (P Rh + Rh P + P Rh P) + c2 (P P Rh + Rh P P - 3 P Rh P) + c3 (P Rh P P + P P Rh P),
+//   P = hat(phi), Rh = hat(rho), c1 = (t - sin t)/t^3, c2 = (t^2 + 2 cos t - 2)/(2 t^4), c3 = (2 t - 3 sin t + t cos t)/(2 t^5)
+//   (Barfoot, State Estimation for Robotics, 7.1.5). Below t = 0.1 the coefficients are their Taylor series to t^4: the
+//   closed forms cancel there, and the series' truncation is below 1e-13 relative.
+KB_HD void se3_right_jacobian_inverse(const double x[6], double J[36]) {
+    const double rho[3] = {-x[0], -x[1], -x[2]}, phi[3] = {-x[3], -x[4], -x[5]};
+    const double t2 = (phi[0] * phi[0] + phi[1] * phi[1]) + phi[2] * phi[2];
+    double c, c1, c2, c3;
+    if (t2 < 1e-2) {
+        const double t4 = t2 * t2;
+        c = (1.0 / 12.0 + t2 / 720.0) + t4 / 30240.0;
+        c1 = (1.0 / 6.0 - t2 / 120.0) + t4 / 5040.0;
+        c2 = (1.0 / 24.0 - t2 / 720.0) + t4 / 40320.0;
+        c3 = (1.0 / 120.0 - t2 / 2520.0) + t4 / 120960.0;
+    } else {
+        const double t = sqrt(t2), st = sin(t), ct = cos(t);
+        c = 1.0 / t2 - (1.0 + ct) / (2.0 * t * st);
+        c1 = (t - st) / (t2 * t);
+        c2 = ((t2 + 2.0 * ct) - 2.0) / (2.0 * t2 * t2);
+        c3 = ((2.0 * t - 3.0 * st) + t * ct) / (2.0 * t2 * t2 * t);
+    }
+    const double P[3][3] = {{0.0, -phi[2], phi[1]}, {phi[2], 0.0, -phi[0]}, {-phi[1], phi[0], 0.0}};
+    const double Rh[3][3] = {{0.0, -rho[2], rho[1]}, {rho[2], 0.0, -rho[0]}, {-rho[1], rho[0], 0.0}};
+    double PP[3][3], PR[3][3], RP[3][3], PRP[3][3], PPR[3][3], RPP[3][3], PRPP[3][3], PPRP[3][3];
+    m3_mul(P, P, PP);
+    m3_mul(P, Rh, PR);
+    m3_mul(Rh, P, RP);
+    m3_mul(PR, P, PRP);
+    m3_mul(PP, Rh, PPR);
+    m3_mul(RP, P, RPP);
+    m3_mul(PRP, P, PRPP);
+    m3_mul(PP, RP, PPRP);
+    double S[3][3], Q[3][3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            S[i][j] = ((i == j ? 1.0 : 0.0) - 0.5 * P[i][j]) + c * PP[i][j];
+            Q[i][j] = ((0.5 * Rh[i][j] + c1 * ((PR[i][j] + RP[i][j]) + PRP[i][j])) +
+                       c2 * ((PPR[i][j] + RPP[i][j]) - 3.0 * PRP[i][j])) +
+                      c3 * (PRPP[i][j] + PPRP[i][j]);
+        }
+    double SQ[3][3], SQS[3][3];
+    m3_mul(S, Q, SQ);
+    m3_mul(SQ, S, SQS);
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            J[6 * i + j] = S[i][j];
+            J[6 * i + j + 3] = -SQS[i][j];
+            J[6 * (i + 3) + j] = 0.0;
+            J[6 * (i + 3) + j + 3] = S[i][j];
+        }
+}
+
 // ---- symmetric 3x3 eigen-decomposition (the plane fit of a voxel: kb_registration_constraints) ----------------------
 // Cyclic Jacobi. A closed-form (trigonometric) solver loses its eigenvectors when eigenvalues nearly coincide, which is
 // exactly what collinear and blob-like voxels produce; Jacobi rotations keep V orthonormal to a few ulps and resolve
