@@ -555,6 +555,42 @@ typedef struct kb_pose_graph_report {
 int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *o, kb_pose_graph_report *out,
                            double *edge_chi2, double *edge_weight);
 
+/* ---- pose graph: marginal covariances -------------------------------------------------------------------------------
+ * How well each pose is known, at the graph's current poses (as added, or as the last optimize left them):
+ *   H = sum_e J_e^T w_e Omega_e J_e over the free nodes, with the optimizer's exact Jacobians
+ *   (dr/dd_j = J_r^-1(r), dr/dd_i = -J_r^-1(r) Ad(T_j^-1 T_i)) and w_e = rho'(s_e) at those poses; no damping. An edge
+ *   with one fixed node adds only the free node's diagonal block, an edge between two fixed nodes nothing; parallel
+ *   edges between one pair add up in ascending edge order.
+ *   Sigma = H^-1, in the tangent space of the right perturbation T_k Exp(d_k), order (translation, rotation). A fixed
+ *   node's rows and columns are exactly 0.
+ * Sigma is the Gauss-Newton (Laplace) approximation at those poses. It is not rescaled by the residuals: Omega is taken
+ * as the measurement's true information.
+ * Method: H = P L L^T P^T, a sparse block Cholesky factorization with a nested-dissection order P (George), computed on
+ * the device (one cooperative launch); Sigma_ij = sum_m X_i[m]^T X_j[m] with X_k = L^-1 P^T E_k, which is non-zero only
+ * on the elimination-tree path from k's column to its root, summed over the common part of the two paths (Sigma_ij = 0
+ * when the two lie in different trees). Every value is formed by one thread in a fixed order: the results are
+ * bit-identical from run to run and for every grid size, and a diagonal block is exactly symmetric.
+ * The symbolic analysis is cached for the graph's size, the numeric factor until the next add_node, add_edge or
+ * optimize; neither changes what optimize computes.
+ * Checked before any device work, writing nothing on error: KB_ERR_INVALID_ARG for NULL with n > 0, a node that does
+ * not exist, a free node that no path of edges connects to a fixed node, and (after the factorization) an H that is not
+ * positive definite at the current poses; then KB_ERR_NO_DEVICE without a device. n == 0 does nothing. */
+/* cov: double[n][36], the row-major 6x6 Sigma_kk of each nodes[t] */
+int kb_pose_graph_marginals(kb_pose_graph *g, const size_t *nodes, size_t n, double *cov);
+/* pairs: size_t[n][2]; cov: double[n][144], the row-major 12x12 [[Sigma_ii, Sigma_ij], [Sigma_ji, Sigma_jj]] of each
+ * pair (any pair: i == j, and nodes that share no edge) */
+int kb_pose_graph_joint_marginals(kb_pose_graph *g, const size_t *pairs, size_t n, double *cov);
+struct kb_pose_graph_factor_info {
+    size_t free_nodes;
+    size_t h_blocks;      /* 6x6 blocks of H's lower triangle, diagonal included */
+    size_t l_blocks;      /* 6x6 blocks of L, diagonal included */
+    size_t etree_height;  /* columns on the longest leaf-to-root path of the elimination tree */
+    double flops;         /* of one numeric factorization: 2*6^3 per block update, 6^3 per block solve, 6^3/3 per pivot */
+};
+/* the symbolic analysis of the graph as it is now; host-side, needs no device (the struct shares the function's
+ * name: C and C++ refer to it as struct kb_pose_graph_factor_info) */
+int kb_pose_graph_factor_info(kb_pose_graph *g, struct kb_pose_graph_factor_info *out);
+
 #ifdef __cplusplus
 }
 #endif

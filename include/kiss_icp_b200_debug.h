@@ -49,6 +49,15 @@ int kb_debug_pose_graph_ms(const kb_pose_graph *g, float *ms);
 /* host evaluation of the pose graph's Jacobian pieces: Ad(T) of a row-major SE(3) and J_r^-1(x), row-major 6x6 */
 int kb_debug_se3_adjoint(const double T[16], double A[36]);
 int kb_debug_se3_right_jacobian_inverse(const double x[6], double J[36]);
+/* the symbolic analysis of kb_pose_graph_marginals (host-side, needs no device), two-call: *n_free = the free nodes;
+ * with cap >= n_free, each of these that is not NULL receives per position p of the elimination order: order[p] = the
+ * node, parent[p] = the position of its elimination-tree parent (-1: a root), col_blocks[p] = the blocks of L's column
+ * p, diagonal included. cap < n_free is KB_ERR_CAPACITY. */
+int kb_debug_pose_graph_symbolic(kb_pose_graph *g, size_t cap, size_t *n_free, size_t *order, long long *parent,
+                                 size_t *col_blocks);
+/* ms[0]: the last numeric factorization launch of kb_pose_graph_marginals / _joint_marginals on g (0 when every node is
+ * fixed), ms[1]: the last marginal solve launch [ms] (CUDA events); KB_ERR_INVALID_ARG before the first */
+int kb_debug_pose_graph_cov_ms(const kb_pose_graph *g, float ms[2]);
 /* work done by the ICP loop of the last RegisterFrame: GetClosestNeighbor calls (iterations x
  * source points) and map points examined — the inputs of the algorithmic-bytes formula */
 int kb_pipeline_last_icp_work(const kb_pipeline *p, double *queries, double *candidates);

@@ -42,12 +42,14 @@ def sources():
 
 def build(force: bool = False, verbose: bool = False) -> str:
     """Compile csrc/api.cu, csrc/localize.cu, csrc/odometry_fit.cu, csrc/constraints.cu, csrc/probe.cu, csrc/relocalize.cu,
-    csrc/places.cu and csrc/pose_graph.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
+    csrc/places.cu, csrc/pose_graph.cu and csrc/pose_graph_cov.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to
+    date."""
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in sources())
     if force or stale:
         cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH,
                *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "odometry_fit.cu", "constraints.cu", "probe.cu",
-                                                       "relocalize.cu", "places.cu", "pose_graph.cu"))]
+                                                       "relocalize.cu", "places.cu", "pose_graph.cu",
+                                                       "pose_graph_cov.cu"))]
         if verbose:
             print(" ".join(cmd))
         env = dict(os.environ)
@@ -145,6 +147,11 @@ class PoseGraphReport(C.Structure):
     """kb_pose_graph_report"""
     _fields_ = [("iterations", i32), ("accepted", i32), ("cg_iterations", i32), ("termination", i32),
                 ("initial_cost", dbl), ("final_cost", dbl), ("lambda_", dbl)]
+
+
+class PoseGraphFactorInfo(C.Structure):
+    """kb_pose_graph_factor_info"""
+    _fields_ = [("free_nodes", sz), ("h_blocks", sz), ("l_blocks", sz), ("etree_height", sz), ("flops", dbl)]
 
 
 # every exported symbol of include/kiss_icp_b200.h: name -> (restype, argtypes)
@@ -270,6 +277,11 @@ SIGNATURES = {
     "kb_debug_pose_graph_ms": (i32, [vp, C.POINTER(C.c_float)]),
     "kb_debug_se3_adjoint": (i32, [vp, vp]),
     "kb_debug_se3_right_jacobian_inverse": (i32, [vp, vp]),
+    "kb_pose_graph_marginals": (i32, [vp, vp, sz, vp]),
+    "kb_pose_graph_joint_marginals": (i32, [vp, vp, sz, vp]),
+    "kb_pose_graph_factor_info": (i32, [vp, C.POINTER(PoseGraphFactorInfo)]),
+    "kb_debug_pose_graph_symbolic": (i32, [vp, sz, C.POINTER(sz), vp, vp, vp]),
+    "kb_debug_pose_graph_cov_ms": (i32, [vp, vp]),
 }
 
 

@@ -29,6 +29,7 @@
 #include "probe.cuh"
 #include "places.cuh"
 #include "pose_graph.cuh"
+#include "pose_graph_cov.cuh"
 #include "relocalize.cuh"
 
 using namespace kb;
@@ -96,6 +97,7 @@ int watchdog_init(int device) {
     CK(odometry_fit_watchdog_init(d, init));  // and so has the fit-reporting odometry kernel's
     CK(constraints_watchdog_init(d, init));   // and the module of the plane-constraint kernels
     CK(pose_graph_watchdog_init(d, init));    // and the pose-graph optimizer's
+    CK(pgc_watchdog_init(d, init));           // and the pose-graph covariance's
     g_wd[device].host = h;
     return KB_OK;
 }
@@ -121,6 +123,7 @@ int watchdog_check(int device) {
     odometry_fit_watchdog_rearm();
     constraints_watchdog_rearm();
     pose_graph_watchdog_rearm();
+    pgc_watchdog_rearm();
     static const char *names[] = {"?", "grid barrier", "ICP gather", "ICP result record", "ICP team gather", "NN bulk copy"};
     std::string marks;
     unsigned m[256];
@@ -2010,6 +2013,15 @@ struct kb_pose_graph {
     DBuf<int> fixed_d, inc_ptr, inc, ij_d, flag;
     DBuf<kb_pose_graph_report> report;
     Event ev[2];                     // around the last launch (kb_debug_pose_graph_ms)
+    // the covariance (kb_pose_graph_marginals & co.): the symbolic analysis for (N, E), its copy on the device, the
+    // numeric factor at the current poses (valid until the next add_node, add_edge or optimize) and the solves
+    PgcSymbolic sym;
+    int sym_dev_n = -1, sym_dev_e = -1;  // the graph the device copy of `sym` was made for
+    bool factored = false;
+    DBuf<int> s_order, s_pos, s_parent, s_col_slot, s_lev_ptr, s_colptr, s_brow, s_bcol, s_hptr, s_hedge, s_uptr, s_upd;
+    DBuf<int> cov_flag, cov_req, cov_path;
+    DBuf<double> Lx, cov_X, cov_out;
+    Event cev[4];                    // around the last factorization and the last marginal solves (kb_debug_pose_graph_cov_ms)
     size_t n() const { return fixed.size(); }
     size_t m() const { return robust.size(); }
 };
@@ -2092,6 +2104,80 @@ static int pg_reserve(kb_pose_graph *g, int grid) {
     return KB_OK;
 }
 
+// the graph's current state on the device: poses, fixed flags, incidence lists (each node's edges ascending: the order
+// its blocks are summed in) and the edges added since the last upload; *P_out gets the graph's buffers, *pq_out the
+// poses as uploaded. g->uploaded is advanced by the caller once the stream has run.
+static int pg_upload(kb_pose_graph *g, std::vector<double> *pq_out, PoseGraphParams *P_out) {
+    const size_t N = g->n(), E = g->m();
+    std::vector<double> &pq = *pq_out;
+    pq.assign(8 * N, 0.0);
+    for (size_t k = 0; k < N; ++k) {
+        const SE3 &T = g->pose[k];
+        const double v[8] = {T.q.x, T.q.y, T.q.z, T.q.w, T.t.x, T.t.y, T.t.z, 0.0};
+        std::copy(v, v + 8, &pq[8 * k]);
+    }
+    std::vector<int> inc_ptr(N + 1, 0), inc(2 * E);
+    for (size_t e = 0; e < 2 * E; ++e) ++inc_ptr[static_cast<size_t>(g->ij[e]) + 1];
+    for (size_t k = 0; k < N; ++k) inc_ptr[k + 1] += inc_ptr[k];
+    {
+        std::vector<int> at(inc_ptr.begin(), inc_ptr.end() - 1);
+        for (size_t e = 0; e < E; ++e) {
+            inc[at[g->ij[2 * e]]++] = static_cast<int>(e);
+            inc[at[g->ij[2 * e + 1]]++] = static_cast<int>(e);
+        }
+    }
+    cudaStream_t s = g->ex->stream;
+    if (N) {
+        CK(cudaMemcpyAsync(g->pose_d.p, pq.data(), 8 * N * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->fixed_d.p, g->fixed.data(), N * sizeof(int), cudaMemcpyHostToDevice, s));
+    }
+    CK(cudaMemcpyAsync(g->inc_ptr.p, inc_ptr.data(), (N + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (E) CK(cudaMemcpyAsync(g->inc.p, inc.data(), 2 * E * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (E > g->uploaded) {
+        const size_t a = g->uploaded, n = E - a;
+        CK(cudaMemcpyAsync(g->ij_d.p + 2 * a, &g->ij[2 * a], 2 * n * sizeof(int), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->meas_d.p + 8 * a, &g->meas_inv[8 * a], 8 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->info_d.p + 36 * a, &g->info[36 * a], 36 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->rob_d.p + a, &g->robust[a], n * sizeof(double), cudaMemcpyHostToDevice, s));
+    }
+    PoseGraphParams &P = *P_out;
+    P = PoseGraphParams{};
+    P.bar = g->ex->sc.bar;
+    P.n_nodes = static_cast<int>(N);
+    P.n_edges = static_cast<int>(E);
+    P.pose = g->pose_d.p;
+    P.cand = g->cand.p;
+    P.fixed = g->fixed_d.p;
+    P.inc_ptr = g->inc_ptr.p;
+    P.inc = g->inc.p;
+    P.ij = g->ij_d.p;
+    P.meas_inv = g->meas_d.p;
+    P.info = g->info_d.p;
+    P.robust = g->rob_d.p;
+    P.e_s = g->e_s.p;
+    P.e_w = g->e_w.p;
+    P.e_jj = g->e_jj.p;
+    P.e_ii = g->e_ii.p;
+    P.e_ad = g->e_ad.p;
+    P.e_g = g->e_g.p;
+    P.hd = g->hd.p;
+    P.g = g->grad.p;
+    P.D = g->D.p;
+    P.U = g->U.p;
+    P.UL = g->UL.p;
+    const size_t V = 6 * std::max<size_t>(N, 1);
+    P.x = g->vec.p;
+    P.r = P.x + V;
+    P.z = P.r + V;
+    P.p = P.z + V;
+    P.q = P.p + V;
+    P.y = P.q + V;
+    P.part = g->part.p;
+    P.flag = g->flag.p;
+    P.report = g->report.p;
+    return KB_OK;
+}
+
 void kb_pose_graph_options_default(kb_pose_graph_options *o) {
     if (o) *o = kb_pose_graph_options{100, 1e-12, 1e-10, 1e-4, 100, 1e-10};
 }
@@ -2115,6 +2201,7 @@ int kb_pose_graph_add_node(kb_pose_graph *g, const double pose[16], int fixed, s
     g->mat.insert(g->mat.end(), pose, pose + 16);
     g->pose.push_back(T);
     g->fixed.push_back(fixed ? 1 : 0);
+    g->factored = false;
     if (index) *index = g->n() - 1;
     return KB_OK;
 }
@@ -2151,6 +2238,7 @@ int kb_pose_graph_add_edge(kb_pose_graph *g, size_t i, size_t j, const double me
     g->meas_inv.insert(g->meas_inv.end(), zi, zi + 8);
     g->info.insert(g->info.end(), information, information + 36);
     g->robust.push_back(robust_scale);
+    g->factored = false;
     if (index) *index = g->m() - 1;
     return KB_OK;
 }
@@ -2187,71 +2275,10 @@ int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, k
     const size_t items = std::max<size_t>(std::max(N, E), 1);
     const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>((items + POSE_GRAPH_BLOCK - 1) / POSE_GRAPH_BLOCK, cap)));
     RET(pg_reserve(g, grid));
-    // nodes, incidence lists (each node's edges ascending: the order its blocks are summed in), new edges
-    std::vector<double> pq(8 * N);
-    for (size_t k = 0; k < N; ++k) {
-        const SE3 &T = g->pose[k];
-        const double v[8] = {T.q.x, T.q.y, T.q.z, T.q.w, T.t.x, T.t.y, T.t.z, 0.0};
-        std::copy(v, v + 8, &pq[8 * k]);
-    }
-    std::vector<int> inc_ptr(N + 1, 0), inc(2 * E);
-    for (size_t e = 0; e < 2 * E; ++e) ++inc_ptr[static_cast<size_t>(g->ij[e]) + 1];
-    for (size_t k = 0; k < N; ++k) inc_ptr[k + 1] += inc_ptr[k];
-    {
-        std::vector<int> at(inc_ptr.begin(), inc_ptr.end() - 1);
-        for (size_t e = 0; e < E; ++e) {
-            inc[at[g->ij[2 * e]]++] = static_cast<int>(e);
-            inc[at[g->ij[2 * e + 1]]++] = static_cast<int>(e);
-        }
-    }
+    std::vector<double> pq;
+    PoseGraphParams P;
+    RET(pg_upload(g, &pq, &P));
     cudaStream_t s = ex.stream;
-    if (N) {
-        CK(cudaMemcpyAsync(g->pose_d.p, pq.data(), 8 * N * sizeof(double), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(g->fixed_d.p, g->fixed.data(), N * sizeof(int), cudaMemcpyHostToDevice, s));
-    }
-    CK(cudaMemcpyAsync(g->inc_ptr.p, inc_ptr.data(), (N + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (E) CK(cudaMemcpyAsync(g->inc.p, inc.data(), 2 * E * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (E > g->uploaded) {
-        const size_t a = g->uploaded, n = E - a;
-        CK(cudaMemcpyAsync(g->ij_d.p + 2 * a, &g->ij[2 * a], 2 * n * sizeof(int), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(g->meas_d.p + 8 * a, &g->meas_inv[8 * a], 8 * n * sizeof(double), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(g->info_d.p + 36 * a, &g->info[36 * a], 36 * n * sizeof(double), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(g->rob_d.p + a, &g->robust[a], n * sizeof(double), cudaMemcpyHostToDevice, s));
-    }
-    PoseGraphParams P{};
-    P.bar = ex.sc.bar;
-    P.n_nodes = static_cast<int>(N);
-    P.n_edges = static_cast<int>(E);
-    P.pose = g->pose_d.p;
-    P.cand = g->cand.p;
-    P.fixed = g->fixed_d.p;
-    P.inc_ptr = g->inc_ptr.p;
-    P.inc = g->inc.p;
-    P.ij = g->ij_d.p;
-    P.meas_inv = g->meas_d.p;
-    P.info = g->info_d.p;
-    P.robust = g->rob_d.p;
-    P.e_s = g->e_s.p;
-    P.e_w = g->e_w.p;
-    P.e_jj = g->e_jj.p;
-    P.e_ii = g->e_ii.p;
-    P.e_ad = g->e_ad.p;
-    P.e_g = g->e_g.p;
-    P.hd = g->hd.p;
-    P.g = g->grad.p;
-    P.D = g->D.p;
-    P.U = g->U.p;
-    P.UL = g->UL.p;
-    const size_t V = 6 * std::max<size_t>(N, 1);
-    P.x = g->vec.p;
-    P.r = P.x + V;
-    P.z = P.r + V;
-    P.p = P.z + V;
-    P.q = P.p + V;
-    P.y = P.q + V;
-    P.part = g->part.p;
-    P.flag = g->flag.p;
-    P.report = g->report.p;
     P.max_iterations = o.max_iterations;
     P.max_cg_iterations = o.max_cg_iterations;
     P.function_tolerance = o.function_tolerance;
@@ -2264,6 +2291,7 @@ int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, k
     }
     CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
     ex.bar_dirty = true;
+    g->factored = false;  // (the poses move)
     CK(cudaEventRecord(g->ev[0].p, s));
     CK(pose_graph_launch(P, grid, s));
     ++ex.launches;
@@ -2305,6 +2333,224 @@ int kb_debug_se3_adjoint(const double T[16], double A[36]) {
 int kb_debug_se3_right_jacobian_inverse(const double x[6], double J[36]) {
     if (!x || !J) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     se3_right_jacobian_inverse(x, J);
+    return KB_OK;
+}
+
+// ------------------------------------------------------------------------------- Pose graph: marginal covariances
+// The symbolic analysis (pgc_symbolic, host) is cached for (N, E): nodes and edges are only ever added. The numeric
+// factor is cached until the next add_node, add_edge or optimize, so marginals and joint marginals taken one after the
+// other factor once.
+static int pg_symbolic(kb_pose_graph *g) {
+    const int N = static_cast<int>(g->n()), E = static_cast<int>(g->m());
+    if (g->sym.n_nodes == N && g->sym.n_edges == E) return KB_OK;
+    g->factored = false;
+    pgc_symbolic(N, g->fixed.data(), E, g->ij.data(), &g->sym);
+    if (g->sym.uptr.size() == 1 && g->sym.uptr[0] < 0) {
+        g->sym.n_nodes = -1;  // (analysed again at the next call, and refused again)
+        return fail(KB_ERR_INVALID_ARG, "the factorization of this graph needs more than 2^30 block updates");
+    }
+    return KB_OK;
+}
+
+// the requested nodes exist, and every free node is tied to a fixed one (otherwise H is singular)
+static int pg_cov_check(const kb_pose_graph *g, const size_t *nodes, size_t n_idx) {
+    if (!nodes) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n_idx > (size_t(1) << 30)) return fail(KB_ERR_INVALID_ARG, "more than 2^29 requests in one call");
+    for (size_t t = 0; t < n_idx; ++t)
+        if (nodes[t] >= g->n()) return fail(KB_ERR_INVALID_ARG, "node %zu does not exist (%zu nodes)", nodes[t], g->n());
+    return pg_gauge_check(*g);
+}
+
+static int pg_put(DBuf<int> &d, const std::vector<int> &h, cudaStream_t s) {
+    RET(d.ensure(std::max<size_t>(h.size(), 1)));
+    if (!h.empty()) CK(cudaMemcpyAsync(d.p, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    return KB_OK;
+}
+
+// the numeric factor of H at the current poses (one cooperative launch), unless the cached one is still valid
+static int pg_factor(kb_pose_graph *g) {
+    RET(pg_symbolic(g));
+    if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
+    Exec &ex = *g->ex;
+    CK(cudaSetDevice(ex.device));
+    if (g->cev[3].device != ex.device) {  // (cev[3] is made last: all four exist on that device)
+        for (Event &e : g->cev) CK(e.create(cudaEventDefault));
+    }
+    const PgcSymbolic &S = g->sym;
+    if (g->factored || S.nf == 0) {
+        g->factored = true;
+        return KB_OK;
+    }
+    int co_resident = 0;
+    CK(pgc_factor_max_grid(ex.sms, &co_resident));
+    const int cap = std::min(tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : ex.sms, co_resident);
+    const size_t items = std::max({g->n(), g->m(), S.blocks(), size_t(1)});
+    const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>((items + PGC_BLOCK - 1) / PGC_BLOCK, cap)));
+    RET(pg_reserve(g, grid));
+    std::vector<double> pq;
+    PgcFactorParams F{};
+    RET(pg_upload(g, &pq, &F.P));
+    cudaStream_t s = ex.stream;
+    if (g->sym_dev_n != S.n_nodes || g->sym_dev_e != S.n_edges) {
+        RET(pg_put(g->s_order, S.order, s));
+        RET(pg_put(g->s_pos, S.pos, s));
+        RET(pg_put(g->s_parent, S.parent, s));
+        RET(pg_put(g->s_col_slot, S.col_slot, s));
+        RET(pg_put(g->s_lev_ptr, S.lev_ptr, s));
+        RET(pg_put(g->s_colptr, S.colptr, s));
+        RET(pg_put(g->s_brow, S.brow, s));
+        RET(pg_put(g->s_bcol, S.bcol, s));
+        RET(pg_put(g->s_hptr, S.hptr, s));
+        RET(pg_put(g->s_hedge, S.hedge, s));
+        RET(pg_put(g->s_uptr, S.uptr, s));
+        RET(pg_put(g->s_upd, S.upd, s));
+        g->sym_dev_n = S.n_nodes;
+        g->sym_dev_e = S.n_edges;
+    }
+    RET(g->Lx.ensure(36 * S.blocks()));
+    RET(g->cov_flag.ensure(1));
+    CK(cudaMemsetAsync(g->cov_flag.p, 0, sizeof(int), s));
+    F.nf = S.nf;
+    F.levels = S.levels();
+    F.n_blocks = static_cast<int>(S.blocks());
+    F.order = g->s_order.p;
+    F.lev_ptr = g->s_lev_ptr.p;
+    F.colptr = g->s_colptr.p;
+    F.brow = g->s_brow.p;
+    F.bcol = g->s_bcol.p;
+    F.hptr = g->s_hptr.p;
+    F.hedge = g->s_hedge.p;
+    F.uptr = g->s_uptr.p;
+    F.upd = g->s_upd.p;
+    F.Lx = g->Lx.p;
+    F.flag = g->cov_flag.p;
+    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
+    ex.bar_dirty = true;
+    CK(cudaEventRecord(g->cev[0].p, s));
+    CK(pgc_factor_launch(F, grid, s));
+    ++ex.launches;
+    CK(cudaEventRecord(g->cev[1].p, s));
+    int flag = 0;
+    CK(cudaMemcpyAsync(&flag, g->cov_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+    RET(ex.sync());
+    g->uploaded = g->m();
+    if (flag) return fail(KB_ERR_INVALID_ARG, "H is not positive definite at the current poses");
+    g->factored = true;
+    return KB_OK;
+}
+
+// req[2 n]: node pairs; out: n blocks of 36 (marginals) or 144 (joint) doubles
+static int pg_cov_solve(kb_pose_graph *g, const std::vector<int> &req, int joint, std::vector<double> *out) {
+    const PgcSymbolic &S = g->sym;
+    const size_t n = req.size() / 2, per = joint ? 144 : 36;
+    out->assign(n * per, 0.0);
+    if (S.nf == 0) return KB_OK;  // (every node is fixed)
+    Exec &ex = *g->ex;
+    cudaStream_t s = ex.stream;
+    const size_t H = static_cast<size_t>(S.levels());
+    const size_t group_bytes = 2 * H * (36 * sizeof(double) + sizeof(int));
+    // at most 4 CTAs per SM, and at most 1 GB of solve scratch
+    const int sm_cap = tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : 4 * ex.sms;
+    const size_t mem_cap = std::max<size_t>(1, (size_t(1) << 30) / (group_bytes * PGC_GROUPS));
+    const int grid = static_cast<int>(std::max<size_t>(1, std::min({(n + PGC_GROUPS - 1) / PGC_GROUPS, static_cast<size_t>(sm_cap), mem_cap})));
+    const size_t groups = static_cast<size_t>(grid) * PGC_GROUPS;
+    RET(g->cov_X.ensure(groups * 2 * H * 36));
+    RET(g->cov_path.ensure(groups * 2 * H));
+    RET(g->cov_req.ensure(2 * n));
+    RET(g->cov_out.ensure(n * per));
+    CK(cudaMemcpyAsync(g->cov_req.p, req.data(), 2 * n * sizeof(int), cudaMemcpyHostToDevice, s));
+    PgcMarginalParams M{};
+    M.Lx = g->Lx.p;
+    M.colptr = g->s_colptr.p;
+    M.brow = g->s_brow.p;
+    M.col_slot = g->s_col_slot.p;
+    M.parent = g->s_parent.p;
+    M.pos = g->s_pos.p;
+    M.req = g->cov_req.p;
+    M.n = static_cast<int>(n);
+    M.joint = joint;
+    M.max_path = static_cast<int>(H);
+    M.X = g->cov_X.p;
+    M.path = g->cov_path.p;
+    M.out = g->cov_out.p;
+    CK(cudaEventRecord(g->cev[2].p, s));
+    CK(pgc_marginals_launch(M, grid, s));
+    ++ex.launches;
+    CK(cudaEventRecord(g->cev[3].p, s));
+    CK(cudaMemcpyAsync(out->data(), g->cov_out.p, n * per * sizeof(double), cudaMemcpyDeviceToHost, s));
+    return ex.sync();
+}
+
+int kb_pose_graph_marginals(kb_pose_graph *g, const size_t *nodes, size_t n, double *cov) {
+    if (!g) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n == 0) return KB_OK;
+    if (!cov) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(pg_cov_check(g, nodes, n));
+    RET(require_device());
+    RET(pg_factor(g));
+    std::vector<int> req(2 * n);
+    for (size_t t = 0; t < n; ++t) req[2 * t] = req[2 * t + 1] = static_cast<int>(nodes[t]);
+    std::vector<double> out;
+    RET(pg_cov_solve(g, req, 0, &out));
+    std::copy(out.begin(), out.end(), cov);
+    return KB_OK;
+}
+int kb_pose_graph_joint_marginals(kb_pose_graph *g, const size_t *pairs, size_t n, double *cov) {
+    if (!g) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n == 0) return KB_OK;
+    if (!cov) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n > (size_t(1) << 29)) return fail(KB_ERR_INVALID_ARG, "more than 2^29 requests in one call");
+    RET(pg_cov_check(g, pairs, 2 * n));
+    RET(require_device());
+    RET(pg_factor(g));
+    std::vector<int> req(2 * n);
+    for (size_t t = 0; t < 2 * n; ++t) req[t] = static_cast<int>(pairs[t]);
+    std::vector<double> out;
+    RET(pg_cov_solve(g, req, 1, &out));
+    std::copy(out.begin(), out.end(), cov);
+    return KB_OK;
+}
+int kb_pose_graph_factor_info(kb_pose_graph *g, struct kb_pose_graph_factor_info *out) {
+    if (!g || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(pg_symbolic(g));
+    const PgcSymbolic &S = g->sym;
+    struct kb_pose_graph_factor_info r {};
+    r.free_nodes = static_cast<size_t>(S.nf);
+    r.h_blocks = S.h_blocks;
+    r.l_blocks = S.blocks();
+    r.etree_height = S.nf ? static_cast<size_t>(S.levels()) : 0;
+    r.flops = S.flops;
+    *out = r;
+    return KB_OK;
+}
+int kb_debug_pose_graph_symbolic(kb_pose_graph *g, size_t cap, size_t *n_free, size_t *order, long long *parent,
+                                 size_t *col_blocks) {
+    if (!g || !n_free) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(pg_symbolic(g));
+    const PgcSymbolic &S = g->sym;
+    const size_t nf = static_cast<size_t>(S.nf);
+    *n_free = nf;
+    if (!order && !parent && !col_blocks) return KB_OK;
+    if (cap < nf) return fail(KB_ERR_CAPACITY, "buffer too small (%zu < %zu free nodes)", cap, nf);
+    for (size_t p = 0; p < nf; ++p) {
+        if (order) order[p] = static_cast<size_t>(S.order[p]);
+        if (parent) parent[p] = S.parent[p];
+        if (col_blocks) col_blocks[p] = static_cast<size_t>(S.colptr[S.col_slot[p] + 1] - S.colptr[S.col_slot[p]]);
+    }
+    return KB_OK;
+}
+int kb_debug_pose_graph_cov_ms(const kb_pose_graph *g, float ms[2]) {
+    if (!g || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (!g->cev[3].p || !g->ex) return fail(KB_ERR_INVALID_ARG, "no marginals have been computed on this graph");
+    CK(cudaSetDevice(g->ex->device));
+    float f = 0.0f, m = 0.0f;
+    if (cudaEventQuery(g->cev[1].p) == cudaSuccess && cudaEventElapsedTime(&f, g->cev[0].p, g->cev[1].p) != cudaSuccess) {
+        cudaGetLastError();
+        f = 0.0f;  // (no factorization was launched: every node is fixed)
+    }
+    CK(cudaEventElapsedTime(&m, g->cev[2].p, g->cev[3].p));
+    ms[0] = f;
+    ms[1] = m;
     return KB_OK;
 }
 

@@ -20,7 +20,8 @@ namespace kb_pg {
 
 constexpr int PB = POSE_GRAPH_BLOCK;
 
-__device__ __forceinline__ SE3 ld_pose(const double *p) { return SE3{{p[0], p[1], p[2], p[3]}, {p[4], p[5], p[6]}}; }
+#include "pose_graph_edges.cuh"
+
 __device__ __forceinline__ void st_pose(double *p, const SE3 &T) {
     p[0] = T.q.x;
     p[1] = T.q.y;
@@ -30,26 +31,6 @@ __device__ __forceinline__ void st_pose(double *p, const SE3 &T) {
     p[5] = T.t.y;
     p[6] = T.t.z;
     p[7] = 0.0;
-}
-
-// y = A v, A^T v, A 6x6 row-major
-__device__ __forceinline__ void mv6(const double *A, const double v[6], double y[6]) {
-#pragma unroll
-    for (int a = 0; a < 6; ++a) {
-        double s = 0.0;
-#pragma unroll
-        for (int b = 0; b < 6; ++b) s = s + A[6 * a + b] * v[b];
-        y[a] = s;
-    }
-}
-__device__ __forceinline__ void mtv6(const double *A, const double v[6], double y[6]) {
-#pragma unroll
-    for (int a = 0; a < 6; ++a) {
-        double s = 0.0;
-#pragma unroll
-        for (int b = 0; b < 6; ++b) s = s + A[6 * b + a] * v[b];
-        y[a] = s;
-    }
 }
 
 struct Red {
@@ -93,92 +74,6 @@ __device__ void grid_reduce(Grid &g, Red &rd, const double (&v)[K], double (&out
 #pragma unroll
     for (int k = 0; k < K; ++k) out[k] = s_out[k];
     __syncthreads();
-}
-
-// r_e = Log(Z^-1 T_i^-1 T_j), s_e = r^T Omega r, rho(s_e) and w_e = rho'(s_e)
-struct EdgeEval {
-    SE3 Ti, Tj;
-    double r[6], s, rho, w;
-};
-__device__ __forceinline__ EdgeEval edge_eval(const PoseGraphParams &P, const double *poses, int e) {
-    EdgeEval v;
-    const int i = P.ij[2 * e], j = P.ij[2 * e + 1];
-    v.Ti = ld_pose(poses + 8 * static_cast<size_t>(i));
-    v.Tj = ld_pose(poses + 8 * static_cast<size_t>(j));
-    const SE3 E = se3_mul(ld_pose(P.meas_inv + 8 * static_cast<size_t>(e)), se3_mul(se3_inverse(v.Ti), v.Tj));
-    se3_log(E, v.r);
-    double Or[6];
-    mv6(P.info + 36 * static_cast<size_t>(e), v.r, Or);
-    double s = 0.0;
-#pragma unroll
-    for (int a = 0; a < 6; ++a) s = s + v.r[a] * Or[a];
-    v.s = s;
-    const double c = P.robust[e];
-    if (c > 0.0) {
-        const double c2 = c * c;
-        v.rho = c2 * log1p(s / c2);
-        v.w = 1.0 / (1.0 + s / c2);
-    } else {
-        v.rho = s;
-        v.w = 1.0;
-    }
-    return v;
-}
-
-// the edge's part of the linearization: B = J_r^-1(r), A = -B Ad(T_j^-1 T_i), W = w Omega.
-// Bt W B and At W A = Ad^T (Bt W B) Ad are formed on the upper triangle and mirrored (exactly symmetric);
-// At W B = -Ad^T (Bt W B) is applied from these two where it is needed.
-// Returns rho(s_e).
-__device__ __noinline__ double edge_linearize(const PoseGraphParams &P, const double *poses, int e) {
-    const EdgeEval v = edge_eval(P, poses, e);
-    P.e_s[e] = v.s;
-    P.e_w[e] = v.w;
-    const double *Om = P.info + 36 * static_cast<size_t>(e);
-    double *Ejj = P.e_jj + 36 * static_cast<size_t>(e);
-    double *Eii = P.e_ii + 36 * static_cast<size_t>(e);
-    double *Ad = P.e_ad + 36 * static_cast<size_t>(e);
-    {
-        double J[36];
-        se3_right_jacobian_inverse(v.r, J);
-        double Or[6], gj[6];
-        mv6(Om, v.r, Or);
-        mtv6(J, Or, gj);
-#pragma unroll
-        for (int a = 0; a < 6; ++a) P.e_g[6 * static_cast<size_t>(e) + a] = v.w * gj[a];
-#pragma unroll
-        for (int b = 0; b < 6; ++b) {
-            double col[6], x[6];
-#pragma unroll
-            for (int k = 0; k < 6; ++k) col[k] = J[6 * k + b];
-            mv6(Om, col, x);  // Omega J[:, b]
-#pragma unroll
-            for (int a = 0; a <= b; ++a) {
-                double s = 0.0;
-#pragma unroll
-                for (int m = 0; m < 6; ++m) s = s + J[6 * m + a] * x[m];
-                Ejj[6 * a + b] = Ejj[6 * b + a] = v.w * s;
-            }
-        }
-    }
-    double A[36];
-    se3_adjoint(se3_mul(se3_inverse(v.Tj), v.Ti), A);
-#pragma unroll
-    for (int k = 0; k < 36; ++k) Ad[k] = A[k];
-#pragma unroll
-    for (int b = 0; b < 6; ++b) {
-        double col[6], y[6];
-#pragma unroll
-        for (int k = 0; k < 6; ++k) col[k] = A[6 * k + b];
-        mv6(Ejj, col, y);  // Ejj Ad[:, b]
-#pragma unroll
-        for (int a = 0; a <= b; ++a) {
-            double s = 0.0;
-#pragma unroll
-            for (int m = 0; m < 6; ++m) s = s + A[6 * m + a] * y[m];
-            Eii[6 * a + b] = Eii[6 * b + a] = s;
-        }
-    }
-    return v.rho;
 }
 
 // in place: the inverse of the SPD 6x6 at M (Cholesky); false when a pivot is not positive and finite
@@ -320,74 +215,6 @@ __device__ __noinline__ void matvec_node(const PoseGraphParams &P, int k, double
     }
 #pragma unroll
     for (int a = 0; a < 6; ++a) out[6 * static_cast<size_t>(k) + a] = y[a];
-}
-
-// diagonal block, gradient, damped M diagonal block and chain coupling of node k
-__device__ __noinline__ void assemble_node(const PoseGraphParams &P, int k, double lambda) {
-    const int N = P.n_nodes;
-    double *Hk = P.hd + 36 * static_cast<size_t>(k), *Dk = P.D + 36 * static_cast<size_t>(k);
-    double *Uk = P.U + 36 * static_cast<size_t>(k), *gk = P.g + 6 * static_cast<size_t>(k);
-    if (P.fixed[k]) {
-#pragma unroll
-        for (int a = 0; a < 36; ++a) {
-            Hk[a] = 0.0;
-            Dk[a] = a % 7 == 0 ? 1.0 : 0.0;
-            Uk[a] = 0.0;
-        }
-#pragma unroll
-        for (int a = 0; a < 6; ++a) gk[a] = 0.0;
-        return;
-    }
-    double g[6] = {0, 0, 0, 0, 0, 0};
-#pragma unroll
-    for (int a = 0; a < 36; ++a) Hk[a] = 0.0;
-    for (int t = P.inc_ptr[k]; t < P.inc_ptr[k + 1]; ++t) {
-        const int e = P.inc[t];
-        const bool is_i = P.ij[2 * e] == k;
-        const double *E = (is_i ? P.e_ii : P.e_jj) + 36 * static_cast<size_t>(e);
-#pragma unroll 6
-        for (int a = 0; a < 36; ++a) Hk[a] = Hk[a] + E[a];
-        const double *gj = P.e_g + 6 * static_cast<size_t>(e);
-        double gg[6], u[6];
-#pragma unroll
-        for (int a = 0; a < 6; ++a) gg[a] = gj[a];
-        if (is_i) {  // At W r = -Ad^T (Bt W r)
-            mtv6(P.e_ad + 36 * static_cast<size_t>(e), gg, u);
-#pragma unroll
-            for (int a = 0; a < 6; ++a) g[a] = g[a] - u[a];
-        } else {
-#pragma unroll
-            for (int a = 0; a < 6; ++a) g[a] = g[a] + gg[a];
-        }
-    }
-#pragma unroll
-    for (int a = 0; a < 6; ++a) gk[a] = g[a];
-#pragma unroll
-    for (int a = 0; a < 36; ++a) Dk[a] = a % 7 == 0 ? Hk[a] + lambda * Hk[a] : Hk[a];
-    // block (k, k + 1) of the chain: the edges between k and k + 1, in full
-#pragma unroll
-    for (int a = 0; a < 36; ++a) Uk[a] = 0.0;
-    if (k + 1 >= N || P.fixed[k + 1]) return;
-    for (int t = P.inc_ptr[k]; t < P.inc_ptr[k + 1]; ++t) {
-        const int e = P.inc[t];
-        const int i = P.ij[2 * e], j = P.ij[2 * e + 1];
-        if ((i == k ? j : i) != k + 1) continue;
-        const double *Ejj = P.e_jj + 36 * static_cast<size_t>(e), *Ad = P.e_ad + 36 * static_cast<size_t>(e);
-#pragma unroll 1
-        for (int a = 0; a < 6; ++a)
-#pragma unroll
-            for (int b = 0; b < 6; ++b) {
-                double s = 0.0;
-                if (i == k) {  // At W B = -Ad^T Ejj
-#pragma unroll
-                    for (int m = 0; m < 6; ++m) s = s + Ad[6 * m + a] * Ejj[6 * m + b];
-                } else {  // (At W B)^T = -Ejj Ad
-#pragma unroll
-                    for (int m = 0; m < 6; ++m) s = s + Ejj[6 * a + m] * Ad[6 * m + b];
-                }
-                Uk[6 * a + b] = Uk[6 * a + b] - s;
-            }
-    }
 }
 
 struct PgShared {

@@ -5,6 +5,8 @@ No reference counterpart. Nodes are poses, some of them fixed; an edge (i, j, Z,
 with the information Omega (6x6, tangent order translation then rotation) and an optional Cauchy scale c. optimize()
 runs Levenberg-Marquardt on the device, in one launch, and leaves the result in ``poses``; nodes and edges may be
 added afterwards and optimize() called again (the online use of loop closure: loop_closure.LoopCloser).
+marginal_covariances() and joint_marginal_covariances() say how well the poses are known: blocks of H^-1 at the
+current poses, from a sparse block Cholesky factorization on the device.
 """
 from __future__ import annotations
 
@@ -58,6 +60,47 @@ class PoseGraphReport:
     lambda_: float
     chi2: np.ndarray | None = None
     weight: np.ndarray | None = None
+
+
+@dataclass
+class PoseGraphFactorInfo:
+    """kb_pose_graph_factor_info: free_nodes; h_blocks / l_blocks: 6x6 blocks of H's lower triangle and of its
+    Cholesky factor L (diagonals included); etree_height: columns on the longest leaf-to-root path of the elimination
+    tree (the length of a marginal's solve); flops of one numeric factorization"""
+    free_nodes: int
+    h_blocks: int
+    l_blocks: int
+    etree_height: int
+    flops: float
+
+
+def _nodes_arg(nodes, shape_tail, what):
+    a = np.asarray(nodes)
+    if a.size and a.dtype.kind not in "iu":
+        raise ValueError(f"{what} must be node indices (integers)")
+    if a.size == 0:
+        return np.empty((0,) + shape_tail, dtype=np.uint64)
+    if a.ndim != 1 + len(shape_tail) or a.shape[1:] != shape_tail:
+        raise ValueError(f"{what} must have the shape (n,) + {shape_tail}, not {a.shape}")
+    if a.size and a.min() < 0:
+        raise ValueError(f"{what}: node {int(a.min())} does not exist")
+    return np.ascontiguousarray(a, dtype=np.uint64)
+
+
+def _adjoint(T):
+    """Ad(T) in the tangent order (translation, rotation)"""
+    R, t = T[:3, :3], T[:3, 3]
+    A = np.zeros((6, 6))
+    A[:3, :3] = A[3:, 3:] = R
+    A[:3, 3:] = np.array([[0.0, -t[2], t[1]], [t[2], 0.0, -t[0]], [-t[1], t[0], 0.0]]) @ R
+    return A
+
+
+def _inverse(T):
+    out = np.eye(4)
+    out[:3, :3] = T[:3, :3].T
+    out[:3, 3] = -T[:3, :3].T @ T[:3, 3]
+    return out
 
 
 def _index(v, name):
@@ -135,6 +178,49 @@ class PoseGraph:
         return PoseGraphReport(iterations=r.iterations, accepted=r.accepted, cg_iterations=r.cg_iterations,
                                termination=TERMINATIONS[r.termination], initial_cost=r.initial_cost,
                                final_cost=r.final_cost, lambda_=r.lambda_, chi2=chi2, weight=weight)
+
+    def marginal_covariances(self, nodes=None) -> np.ndarray:
+        """the (n, 6, 6) marginal covariances Sigma_kk of ``nodes`` (None: every node) at the current poses: blocks of
+        H^-1, tangent order (translation, rotation) of the right perturbation T_k Exp(d_k); zero for a fixed node. The
+        Gauss-Newton approximation, not rescaled by the residuals (kb_pose_graph_marginals states it in full).
+        ValueError for a node that does not exist or a free node no path of edges connects to a fixed node."""
+        idx = np.arange(len(self), dtype=np.uint64) if nodes is None else _nodes_arg(nodes, (), "nodes")
+        out = np.empty((len(idx), 6, 6))
+        if len(idx):
+            check_value(N.lib().kb_pose_graph_marginals(self._h, N.ptr(idx), len(idx), N.ptr(out)))
+        return out
+
+    def joint_marginal_covariances(self, pairs) -> np.ndarray:
+        """the (n, 12, 12) joint covariances [[Sigma_ii, Sigma_ij], [Sigma_ji, Sigma_jj]] of the node pairs (n, 2);
+        any pair, i == j and nodes that share no edge included"""
+        idx = _nodes_arg(pairs, (2,), "pairs")
+        out = np.empty((len(idx), 12, 12))
+        if len(idx):
+            check_value(N.lib().kb_pose_graph_joint_marginals(self._h, N.ptr(idx), len(idx), N.ptr(out)))
+        return out
+
+    def relative_covariance(self, i: int, j: int) -> np.ndarray:
+        """the first-order (6, 6) covariance of T_i^-1 T_j, in the tangent space of its right perturbation:
+        A Sigma_ii A^T - A Sigma_ij - Sigma_ji A^T + Sigma_jj with A = Ad(T_j^-1 T_i) (the optimizer's Jacobians at a
+        zero residual), from the joint block"""
+        J = self.joint_marginal_covariances([(i, j)])[0]
+        P = self.poses
+        A = _adjoint(_inverse(P[j]) @ P[i])
+        Sii, Sij, Sji, Sjj = J[:6, :6], J[:6, 6:], J[6:, :6], J[6:, 6:]
+        return A @ Sii @ A.T - A @ Sij - Sji @ A.T + Sjj
+
+    def factor_info(self) -> PoseGraphFactorInfo:
+        """the size of the covariance's factorization for the graph as it is now (host-side: needs no device)"""
+        r = N.PoseGraphFactorInfo()
+        N.check(N.lib().kb_pose_graph_factor_info(self._h, C.byref(r)))
+        return PoseGraphFactorInfo(free_nodes=r.free_nodes, h_blocks=r.h_blocks, l_blocks=r.l_blocks,
+                                   etree_height=r.etree_height, flops=r.flops)
+
+    def covariance_kernel_ms(self) -> tuple[float, float]:
+        """device time [ms] of the last numeric factorization and of the last marginal solves (CUDA events)"""
+        ms = (C.c_float * 2)()
+        N.check(N.lib().kb_debug_pose_graph_cov_ms(self._h, ms))
+        return float(ms[0]), float(ms[1])
 
     def kernel_ms(self) -> float:
         """device time of the last optimize() [ms] (CUDA events)"""
