@@ -591,6 +591,67 @@ struct kb_pose_graph_factor_info {
  * name: C and C++ refer to it as struct kb_pose_graph_factor_info) */
 int kb_pose_graph_factor_info(kb_pose_graph *g, struct kb_pose_graph_factor_info *out);
 
+/* ---- free space: removing moving objects from a map ----------------------------------------------------------------
+ * No reference counterpart. A map keeps everything the sensor ever hit, including a car that drove past or was parked
+ * and left. The scans of a run that saw through such a place are evidence that it is free; this call counts that
+ * evidence for every map point and removes the points it outweighs.
+ * Inputs: a map and S scans; scan s is points p in its sensor frame and a pose T_s (world <- sensor, row-major SE(3)).
+ * Rays: each point gives a ray from o = t_s to e = T_s p, computed exactly as kb_map_update_pose transforms points (the
+ *   same device function); L = |e - o|, d = (e - o) / L, each component divided by L.
+ * Planes: a voxel is planar when it holds m >= 3 points and its planarity a >= min_planarity, with the mean, the
+ *   covariance C (1/m), n (the unit eigenvector of C's smallest eigenvalue) and a = (l1 - l0) / l2 (0 when l2 = 0) of the
+ *   plane constraints above.
+ * Passes, per map point m: a ray passes m when all of these hold (rays with L = 0 pass nothing):
+ *   1. u = (m - o).d lies in [0, L - end_margin];
+ *   2. r = |m - o - u d| <= pass_radius;
+ *   3. if m's voxel is planar, |n.d| >= sin(min_incidence).
+ *   Rule 3 keeps the ground and walls: a ray that ends on m's own plane at least end_margin beyond m, at an angle alpha to
+ *   that plane, has r >= end_margin sin(alpha) at m. So when sin(min_incidence) > pass_radius / end_margin, a planar
+ *   surface is never passed by the rays that graze it; only rays steeper than min_incidence can pass its points, and
+ *   those end far from it. The defaults meet this condition with a factor of 2 for noise.
+ * Hits, per map voxel V: the rays whose endpoint e falls in V (the hot path's FP64 point_to_voxel; a zero-length ray
+ *   too). Hits protect thin static objects (poles, box edges): rays skim past their edges, but every scan that sees them
+ *   ends many rays in their voxels.
+ * Removed: a map point m is removed when passes(m) >= min_passes and passes(m) >= ratio * hits(V(m)) (in double).
+ * Parameters are checked on the host before any device call: KB_ERR_INVALID_ARG for a non-finite value,
+ * pass_radius <= 0, end_margin < 0, min_incidence outside [0, pi/2], min_planarity outside [0, 1], min_passes = 0 or
+ * ratio < 0. */
+typedef struct kb_free_space_params {
+    double pass_radius;    /* epsilon [m] */
+    double end_margin;     /* delta [m] */
+    double min_incidence;  /* theta_min [rad] */
+    double min_planarity;  /* a_min */
+    unsigned min_passes;
+    double ratio;
+} kb_free_space_params;
+/* pass_radius 0.1 v, end_margin 2.0 v, min_incidence asin(2 pass_radius / end_margin), min_planarity 0.3, min_passes 20,
+ * ratio 0.1 for voxel size v (chosen from measurements: DESIGN.md §4.13); needs no device */
+void kb_free_space_params_default(kb_free_space_params *p, double voxel_size);
+typedef struct kb_free_space_report {
+    unsigned long long rays, scans;                   /* the input */
+    unsigned long long points, voxels;                /* of the map */
+    unsigned long long points_removed, voxels_removed; /* voxels that lose every point */
+    unsigned long long ray_point_tests;               /* (ray, point) pairs the counting tested exactly */
+} kb_free_space_report;
+/* Count the free-space evidence of scans xyz[offset[s] .. offset[s + 1]) at poses[s][16] (s < n_scans) for map.
+ * passes (unsigned[kb_map_num_points]) and hits (unsigned[kb_map_num_voxels]) may each be NULL; both are in dump order
+ * (kb_map_dump: voxels ascending, points in per-voxel insertion order). out, when not NULL, receives the kept points
+ * through kb_map_load_dev's path, in per-voxel insertion order; voxels that lose every point disappear. out must be
+ * another map with map's voxel_size and max_points_per_voxel, on map's device, that no localizer reads; else
+ * KB_ERR_INVALID_ARG and nothing changes. report may be NULL.
+ * map is only read: the call works while localizers read it. Device memory is bounded by the map and the largest chunk
+ * of scans (up to 2^22 rays, or one larger scan), not by n_scans. The counts are integers: they do not depend on
+ * kb_set_grid_blocks, the ray bin size, the order of the scans or how they are split over calls (two calls over a
+ * split of the scans sum to one call's counts).
+ * Every argument is checked before any work and nothing is written on error: KB_ERR_INVALID_ARG for the parameters
+ * above, NULL p, NULL xyz / offset / poses where needed, an offset that is not a non-decreasing partition of
+ * [0, n_points], a non-finite point, an endpoint whose voxel coordinate would not fit in an int, or n_points >= 2^32;
+ * KB_ERR_NOT_SE3 for a pose outside SE(3). Without a device the call then returns KB_ERR_NO_DEVICE; a NULL map is
+ * KB_ERR_INVALID_ARG after that. */
+int kb_map_free_space(const kb_map *map, const double *xyz, size_t n_points, const size_t *offset, size_t n_scans,
+                      const double *poses, const kb_free_space_params *p, unsigned *passes, unsigned *hits, kb_map *out,
+                      kb_free_space_report *report);
+
 #ifdef __cplusplus
 }
 #endif

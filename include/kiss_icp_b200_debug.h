@@ -58,6 +58,12 @@ int kb_debug_pose_graph_symbolic(kb_pose_graph *g, size_t cap, size_t *n_free, s
 /* ms[0]: the last numeric factorization launch of kb_pose_graph_marginals / _joint_marginals on g (0 when every node is
  * fixed), ms[1]: the last marginal solve launch [ms] (CUDA events); KB_ERR_INVALID_ARG before the first */
 int kb_debug_pose_graph_cov_ms(const kb_pose_graph *g, float ms[2]);
+/* the angular size [rad] of the ray bins of kb_map_free_space calls on this thread: 0 = the default (1 degree), else
+ * within [0.002, pi] (KB_ERR_INVALID_ARG otherwise). The counts do not depend on it; the time does. */
+int kb_debug_free_space_bin_size(double radians);
+/* ms[0..2]: planes, bin index, counting of the last kb_map_free_space on this thread [ms] (CUDA events, summed over the
+ * chunks of scans); KB_ERR_INVALID_ARG before the first */
+int kb_debug_free_space_ms(float ms[3]);
 /* work done by the ICP loop of the last RegisterFrame: GetClosestNeighbor calls (iterations x
  * source points) and map points examined — the inputs of the algorithmic-bytes formula */
 int kb_pipeline_last_icp_work(const kb_pipeline *p, double *queries, double *candidates);

@@ -4,6 +4,7 @@ hand-written CUDA kernels reached through the C-ABI of include/kiss_icp_b200.h; 
 is the host-side mirror of the reference interface. No CPU fallback."""
 from .config import KISSConfig, load_config  # noqa: F401
 from .constraints import Constraints, covariance, degeneracy  # noqa: F401
+from .free_space import FreeSpace, FreeSpaceParams  # noqa: F401
 from .kiss_icp import KissICP  # noqa: F401
 from .mapping import VoxelHashMap, get_voxel_hash_map  # noqa: F401
 from .places import PlaceDatabase, PlaceDescriptorParams, PlaceMatch, PlaceRelocalizationResult  # noqa: F401

@@ -42,14 +42,14 @@ def sources():
 
 def build(force: bool = False, verbose: bool = False) -> str:
     """Compile csrc/api.cu, csrc/localize.cu, csrc/odometry_fit.cu, csrc/constraints.cu, csrc/probe.cu, csrc/relocalize.cu,
-    csrc/places.cu, csrc/pose_graph.cu and csrc/pose_graph_cov.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to
-    date."""
+    csrc/places.cu, csrc/pose_graph.cu, csrc/pose_graph_cov.cu and csrc/free_space.cu -> libkiss_icp_b200.so (sm_90a).
+    No-op when up to date."""
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in sources())
     if force or stale:
         cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH,
                *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "odometry_fit.cu", "constraints.cu", "probe.cu",
                                                        "relocalize.cu", "places.cu", "pose_graph.cu",
-                                                       "pose_graph_cov.cu"))]
+                                                       "pose_graph_cov.cu", "free_space.cu"))]
         if verbose:
             print(" ".join(cmd))
         env = dict(os.environ)
@@ -147,6 +147,18 @@ class PoseGraphReport(C.Structure):
     """kb_pose_graph_report"""
     _fields_ = [("iterations", i32), ("accepted", i32), ("cg_iterations", i32), ("termination", i32),
                 ("initial_cost", dbl), ("final_cost", dbl), ("lambda_", dbl)]
+
+
+class FreeSpaceParams(C.Structure):
+    """kb_free_space_params"""
+    _fields_ = [("pass_radius", dbl), ("end_margin", dbl), ("min_incidence", dbl), ("min_planarity", dbl),
+                ("min_passes", u32), ("ratio", dbl)]
+
+
+class FreeSpaceReport(C.Structure):
+    """kb_free_space_report"""
+    _fields_ = [(f, C.c_ulonglong) for f in ("rays", "scans", "points", "voxels", "points_removed", "voxels_removed",
+                                             "ray_point_tests")]
 
 
 class PoseGraphFactorInfo(C.Structure):
@@ -282,6 +294,11 @@ SIGNATURES = {
     "kb_pose_graph_factor_info": (i32, [vp, C.POINTER(PoseGraphFactorInfo)]),
     "kb_debug_pose_graph_symbolic": (i32, [vp, sz, C.POINTER(sz), vp, vp, vp]),
     "kb_debug_pose_graph_cov_ms": (i32, [vp, vp]),
+    "kb_free_space_params_default": (None, [C.POINTER(FreeSpaceParams), dbl]),
+    "kb_map_free_space": (i32, [vp, vp, sz, vp, sz, vp, C.POINTER(FreeSpaceParams), vp, vp, vp,
+                                C.POINTER(FreeSpaceReport)]),
+    "kb_debug_free_space_bin_size": (i32, [dbl]),
+    "kb_debug_free_space_ms": (i32, [vp]),
 }
 
 

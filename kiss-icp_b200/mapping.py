@@ -144,6 +144,23 @@ class VoxelHashMap:
             raise ValueError("expected voxels (V, 3), counts (V,) and points (P, 3)")
         self._mutated(N.lib().kb_map_load(self._h, N.ptr(vox), N.ptr(cnt), N.ptr(pts), len(vox), len(pts)), check_value)
 
+    def free_space(self, scans, poses, params=None):
+        """Count the free-space evidence of the scans (a list of (N_s, 3) arrays in their sensor frames) at poses
+        (S, 4, 4, world <- sensor) for this map -> FreeSpace (passes, hits, removed, report), aligned with dump().
+        Only reads the map: it works while localizers use it. params: a FreeSpaceParams (None: the defaults)."""
+        from . import free_space
+        return free_space.count(self, scans, poses, params)
+
+    def cleaned(self, scans, poses, params=None):
+        """-> (VoxelHashMap, FreeSpace): a new map with this one's voxel size, maximum distance and points per voxel that
+        holds the points free_space() does not remove, in per-voxel insertion order. This map is unchanged."""
+        from . import free_space
+        vs, md, mp = N.dbl(0), N.dbl(0), N.u32(0)
+        N.check(N.lib().kb_map_params(self._h, C.byref(vs), C.byref(md), C.byref(mp)))
+        out = VoxelHashMap(vs.value, md.value, mp.value)
+        fs = free_space.count(self, scans, poses, params, out=out)
+        return out, fs
+
     def closest_neighbors(self, queries):
         """batched VoxelHashMap::GetClosestNeighbor (VoxelHashMap.cpp:46-70)."""
         q = N.points_arg(queries)

@@ -40,8 +40,15 @@ class SyntheticLidar:
 
     def __init__(self, seed=0, beams=64, cols=1024, elev_deg=(-24.8, 2.0), max_ray=120.0, noise=0.02,
                  stamps="none", speed=10.0, hz=10.0, loop_radius=150.0, sensor_height=1.73, n_boxes=260,
-                 device="cpu"):
+                 device="cpu", movers=None):
+        """movers: moving boxes (none by default). Each is (size, s0, lateral, speed) or (size, s0, lateral, speed,
+        "cross"), with size = (sx, sy, sz) [m] of an axis-aligned box standing on the ground, and t = scan index / hz:
+        along the road its centre is at arclength s0 + speed t of the loop, `lateral` metres to the left of it (a
+        negative speed drives the other way); a crossing box stays at arclength s0 and moves across the road, its
+        centre at lateral + speed t."""
         self.seed, self.beams, self.cols = int(seed), int(beams), int(cols)
+        self.hz = float(hz)
+        self.movers = [tuple(m) for m in movers] if movers else []
         self.max_ray, self.noise, self.stamps = float(max_ray), float(noise), stamps
         self.device = torch.device(device)
         self.sensor_height = sensor_height
@@ -124,8 +131,22 @@ class SyntheticLidar:
         return T
 
     # -- ray casting -------------------------------------------------------------------
-    def _cast(self, origins, dirs):
-        """origins/dirs (N,3) world frame -> range (N,), inf where nothing is hit."""
+    def mover_boxes(self, k: float):
+        """(lo, hi) (M, 3) of the moving boxes at scan index k"""
+        lo, hi = np.zeros((len(self.movers), 3)), np.zeros((len(self.movers), 3))
+        t = k / self.hz
+        for i, m in enumerate(self.movers):
+            size, s0, lat, v = np.asarray(m[0], dtype=np.float64), float(m[1]), float(m[2]), float(m[3])
+            cross = len(m) > 4 and m[4] == "cross"
+            s = s0 if cross else s0 + v * t
+            off = lat + v * t if cross else lat
+            c = self._xy(s) + self._normal(s) * off
+            lo[i] = [c[0] - size[0] / 2, c[1] - size[1] / 2, 0.0]
+            hi[i] = [c[0] + size[0] / 2, c[1] + size[1] / 2, size[2]]
+        return lo, hi
+
+    def _cast(self, origins, dirs, k=None):
+        """origins/dirs (N,3) world frame -> range (N,), inf where nothing is hit. k: also the movers at scan k."""
         big = float("inf")
         dz = dirs[:, 2]
         t = torch.where(dz < -1e-9, -origins[:, 2] / dz, torch.full_like(dz, big))
@@ -134,6 +155,10 @@ class SyntheticLidar:
         near = ((self.box_lo[:, 0] - c[0]).clamp(min=0) + (c[0] - self.box_hi[:, 0]).clamp(min=0)) ** 2 + \
                ((self.box_lo[:, 1] - c[1]).clamp(min=0) + (c[1] - self.box_hi[:, 1]).clamp(min=0)) ** 2 < (self.max_ray + 5) ** 2
         lo, hi = self.box_lo[near], self.box_hi[near]
+        if k is not None and self.movers:
+            mlo, mhi = self.mover_boxes(k)
+            lo = torch.cat([lo, torch.tensor(mlo, dtype=torch.float64, device=self.device)])
+            hi = torch.cat([hi, torch.tensor(mhi, dtype=torch.float64, device=self.device)])
         inv = 1.0 / torch.where(dirs.abs() < 1e-12, torch.full_like(dirs, 1e-12), dirs)
         chunk = 16
         for b in range(0, lo.shape[0], chunk):
@@ -152,7 +177,13 @@ class SyntheticLidar:
         pts, ts = self.scan_torch(k)
         return pts.cpu().numpy(), ts.cpu().numpy()
 
-    def scan_torch(self, k: int):
+    def scan_with_movers(self, k: int):
+        """scan(k) and a (N,) bool mask of the returned points that hit a moving box: the same rays cast without the
+        movers end farther (or nowhere)."""
+        pts, ts, mask = self.scan_torch(k, mover_mask=True)
+        return pts.cpu().numpy(), ts.cpu().numpy(), mask.cpu().numpy()
+
+    def scan_torch(self, k: int, mover_mask: bool = False):
         g = torch.Generator(device="cpu")
         g.manual_seed(self.seed * 1_000_003 + int(k))
         n = self.dirs.shape[0]
@@ -182,7 +213,7 @@ class SyntheticLidar:
             Rt = torch.tensor(T[:3, :3], dtype=torch.float64, device=self.device)
             origins = torch.tensor(T[:3, 3], dtype=torch.float64, device=self.device).expand(n, 3)
             dirs_w = self.dirs @ Rt.T
-        rng_ = self._cast(origins, dirs_w)
+        rng_ = self._cast(origins, dirs_w, k) if self.movers else self._cast(origins, dirs_w)
         noise = torch.randn(n, generator=g, dtype=torch.float64).to(self.device) * self.noise
         valid = rng_ < self.max_ray
         r = (rng_ + noise)[valid]
@@ -192,6 +223,9 @@ class SyntheticLidar:
             ts = col.to(torch.float64) / self.cols
         else:
             ts = torch.empty(0, dtype=torch.float64, device=self.device)
+        if mover_mask:
+            static = self._cast(origins, dirs_w) if self.movers else rng_
+            return pts, ts, (rng_ < static)[valid]
         return pts, ts
 
 
