@@ -41,15 +41,10 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/api.cu, csrc/localize.cu, csrc/odometry_fit.cu, csrc/constraints.cu, csrc/probe.cu, csrc/relocalize.cu,
-    csrc/places.cu, csrc/pose_graph.cu, csrc/pose_graph_cov.cu and csrc/free_space.cu -> libkiss_icp_b200.so (sm_90a).
-    No-op when up to date."""
+    """Compile every csrc/*.cu -> libkiss_icp_b200.so (sm_90a). No-op when up to date."""
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in sources())
     if force or stale:
-        cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH,
-               *(os.path.join(CSRC, f) for f in ("api.cu", "localize.cu", "odometry_fit.cu", "constraints.cu", "probe.cu",
-                                                       "relocalize.cu", "places.cu", "pose_graph.cu",
-                                                       "pose_graph_cov.cu", "free_space.cu"))]
+        cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH, *(s for s in sources() if s.endswith(".cu"))]
         if verbose:
             print(" ".join(cmd))
         env = dict(os.environ)

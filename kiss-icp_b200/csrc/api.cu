@@ -1,7 +1,8 @@
-// Host side of the C-ABI (include/kiss_icp_b200.h). Thin: argument checks, H2D/D2H copies,
-// capacity management of the HBM voxel table, and ONE cooperative launch per call.
-// There is no CPU fallback anywhere in this file: without a CUDA device every compute entry
-// point returns KB_ERR_NO_DEVICE.
+// Host side of the C-ABI (include/kiss_icp_b200.h) for the kernels of the core device module (kernels.cuh): the map,
+// registration, align-batch, grid relocalization, the pipeline, preprocessing, threshold, downsample and the probes of
+// these kernels. Thin: argument checks, H2D/D2H copies, capacity management of the HBM voxel table, and ONE cooperative
+// launch per call. There is no CPU fallback anywhere in this file: without a CUDA device every compute entry point
+// returns KB_ERR_NO_DEVICE. Places, the pose graph and free space have host files of their own (api_*.cu).
 #include <cuda_runtime.h>
 
 #include <cub/device/device_scan.cuh>
@@ -9,15 +10,10 @@
 
 #include <algorithm>
 #include <array>
-#include <atomic>
-#include <chrono>
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
-#include <mutex>
 #include <numeric>
 #include <string>
 #include <utility>
@@ -25,394 +21,19 @@
 
 #include "../../include/kiss_icp_b200.h"
 #include "../../include/kiss_icp_b200_debug.h"
-#include "free_space.cuh"
+#include "api.cuh"
 #include "kernels.cuh"
 #include "probe.cuh"
-#include "places.cuh"
-#include "pose_graph.cuh"
-#include "pose_graph_cov.cuh"
 #include "relocalize.cuh"
 
 using namespace kb;
+using namespace kb_host;
+
+// this module's hooks for host.cu: its copies of the watchdog's words, and where k_register_frame leaves its phase marks
+cudaError_t core_watchdog(unsigned *d_host_words, const unsigned *init) { return kb::watchdog_arm(d_host_words, init); }
+const void *phase_marks_symbol() { return reinterpret_cast<const void *>(&kb::g_kb_marks); }
 
 namespace {
-
-thread_local std::string tl_err;
-thread_local int tl_device = 0;
-thread_local cudaStream_t tl_user_stream = nullptr;
-thread_local int tl_grid_blocks = 0;
-
-int fail(int status, const char *fmt, ...) {
-    char buf[4096];  // (room for the per-CTA phase marks of the hang reports)
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof(buf), fmt, ap);
-    va_end(ap);
-    tl_err = buf;
-    return status;
-}
-
-#define CK(call)                                                                              \
-    do {                                                                                      \
-        cudaError_t e_ = (call);                                                              \
-        if (e_ != cudaSuccess) return fail(KB_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(e_)); \
-    } while (0)
-#define RET(call)              \
-    do {                       \
-        int s_ = (call);       \
-        if (s_ != KB_OK) return s_; \
-    } while (0)
-
-int device_count() {
-    int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess) {
-        cudaGetLastError();
-        return 0;
-    }
-    return n;
-}
-int require_device() {
-    return device_count() > 0 ? KB_OK : fail(KB_ERR_NO_DEVICE, "no CUDA device visible (this library has no CPU fallback)");
-}
-
-// the device watchdog's report (device_ops.cuh): mapped host words per device, checked after every synchronisation
-struct WatchdogHost {
-    unsigned *host = nullptr;  // [0] flag [1] code [2] block [3] thread [4] a [5] b
-};
-WatchdogHost g_wd[64];
-int watchdog_init(int device) {
-    static std::mutex mu;
-    std::lock_guard<std::mutex> lock(mu);
-    if (device < 0 || device >= 64 || g_wd[device].host) return KB_OK;
-    unsigned *h = nullptr, *d = nullptr;
-    CK(cudaHostAlloc(&h, 8 * sizeof(unsigned), cudaHostAllocMapped));
-    std::memset(h, 0, 8 * sizeof(unsigned));
-    CK(cudaHostGetDevicePointer(&d, h, 0));
-    CK(cudaMemcpyToSymbol(g_kb_wd_host, &d, sizeof(d)));
-    // give up after 2^24 polls (of the order of 10 s, below the host's 30 s deadline). 2^22 (a second or two) fired once in
-    // ~40 full-file test runs at the FIRST grid barrier of a launch; whether that was a stall or a deadlock is not known.
-    unsigned init[8] = {0, 0, 0, 0, 0, 0, 0, 24};
-    if (const char *e = std::getenv("KB_WATCHDOG_SHIFT")) init[7] = static_cast<unsigned>(std::max(10, std::min(std::atoi(e), 31)));
-    CK(cudaMemcpyToSymbol(g_kb_wd, init, sizeof(init)));
-    CK(localize_watchdog_init(d, init));  // the localizer kernel's module has its own copies
-    CK(odometry_fit_watchdog_init(d, init));  // and so has the fit-reporting odometry kernel's
-    CK(constraints_watchdog_init(d, init));   // and the module of the plane-constraint kernels
-    CK(pose_graph_watchdog_init(d, init));    // and the pose-graph optimizer's
-    CK(pgc_watchdog_init(d, init));           // and the pose-graph covariance's
-    g_wd[device].host = h;
-    return KB_OK;
-}
-// where every CTA of the last k_register_frame was (g_kb_marks)
-std::string format_marks(const unsigned m[256]) {
-    std::string out = "phase marks per CTA:";
-    char buf[16];
-    for (int i = 0; i < 160; ++i) {
-        std::snprintf(buf, sizeof(buf), " %x", m[i]);
-        out += buf;
-    }
-    return out;
-}
-// after a synchronisation: did a spin loop of the last launches give up?
-int watchdog_check(int device) {
-    unsigned *h = (device >= 0 && device < 64) ? g_wd[device].host : nullptr;
-    if (!h || !*reinterpret_cast<volatile unsigned *>(h)) return KB_OK;
-    const unsigned code = h[1], block = h[2], thread = h[3], a = h[4], b = h[5];
-    h[0] = 0;
-    unsigned zero = 0;
-    cudaMemcpyToSymbol(g_kb_wd, &zero, sizeof(zero));  // re-arm
-    localize_watchdog_rearm();
-    odometry_fit_watchdog_rearm();
-    constraints_watchdog_rearm();
-    pose_graph_watchdog_rearm();
-    pgc_watchdog_rearm();
-    static const char *names[] = {"?", "grid barrier", "ICP gather", "ICP result record", "ICP team gather", "NN bulk copy"};
-    std::string marks;
-    unsigned m[256];
-    if (cudaMemcpyFromSymbol(m, g_kb_marks, sizeof(m)) == cudaSuccess) marks = "; " + format_marks(m);  // (the launch has ended: a plain copy)
-    cudaGetLastError();
-    return fail(KB_ERR_CUDA, "device watchdog: a kernel gave up waiting at the %s (block %u, thread %u, a=%u, b=%u; grid barrier: a = target, b = counter); "
-                             "the results of that launch are invalid%s",
-                names[code < 6 ? code : 0], block, thread, a, b, marks.c_str());
-}
-
-bool g_stuck[64];
-void device_stuck(int device) {
-    if (device >= 0 && device < 64) g_stuck[device] = true;
-}
-// a launch on this device (-1: any device) never ended
-bool device_is_stuck(int device) {
-    if (device < 0) {
-        for (bool b : g_stuck)
-            if (b) return true;
-        return false;
-    }
-    return device < 64 && g_stuck[device];
-}
-std::string phase_marks(int device) {
-    // the compute stream is stuck: read the marks on a stream of their own (bounded wait, the copy engine is free)
-    unsigned marks[256];
-    cudaStream_t side = nullptr;
-    if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&side, cudaStreamNonBlocking) != cudaSuccess) return "";
-    std::string out;
-    if (cudaMemcpyFromSymbolAsync(marks, g_kb_marks, sizeof(marks), 0, cudaMemcpyDeviceToHost, side) == cudaSuccess) {
-        const auto t0 = std::chrono::steady_clock::now();
-        cudaError_t q;
-        while ((q = cudaStreamQuery(side)) == cudaErrorNotReady &&
-               std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() < 5.0) {
-        }
-        out = q == cudaSuccess ? format_marks(marks) : "(phase marks unreadable)";
-    }
-    return out;  // (the side stream is leaked with the rest of the stuck context)
-}
-
-// Owner of one CUDA resource: device or pinned memory, an event, a stream. It records the device the resource was
-// created on and releases it when it goes, unless a launch on that device never ended: cudaFree & co. would block
-// forever then, so the resource is leaked with the stuck context. (The release calls find the resource's device from
-// the handle: they do not depend on the current device.)
-template <class H, cudaError_t (*Release)(H)>
-struct Owned {
-    H p = nullptr;
-    int device = -1;  // where p was created
-    Owned() = default;
-    Owned(Owned &&o) noexcept { *this = std::move(o); }
-    Owned &operator=(Owned &&o) noexcept {  // (o releases what this owned)
-        std::swap(p, o.p);
-        std::swap(device, o.device);
-        return *this;
-    }
-    ~Owned() {
-        if (p && !device_is_stuck(device)) Release(p);
-    }
-
-  protected:
-    // release what this owns, then own what create(&handle) makes on the current device (nothing when it fails)
-    template <class Create>
-    cudaError_t make(Create create) {
-        *this = Owned{};
-        const cudaError_t e = create(&p);
-        if (e == cudaSuccess)
-            cudaGetDevice(&device);
-        else
-            p = nullptr;
-        return e;
-    }
-};
-struct Event : Owned<cudaEvent_t, cudaEventDestroy> {
-    cudaError_t create(unsigned flags) { return make([&](cudaEvent_t *e) { return cudaEventCreateWithFlags(e, flags); }); }
-};
-struct Stream : Owned<cudaStream_t, cudaStreamDestroy> {
-    cudaError_t create() { return make([](cudaStream_t *s) { return cudaStreamCreateWithFlags(s, cudaStreamNonBlocking); }); }
-};
-
-template <class T>
-cudaError_t free_device(T *p) { return cudaFree(p); }
-template <class T>
-cudaError_t free_pinned(T *p) { return cudaFreeHost(p); }
-
-// an array of n T in device memory, or in pinned host memory (Pinned)
-template <class T, bool Pinned>
-struct Buffer : Owned<T *, Pinned ? &free_pinned<T> : &free_device<T>> {
-    size_t n = 0;
-    Buffer() = default;
-    Buffer(Buffer &&o) noexcept { *this = std::move(o); }
-    Buffer &operator=(Buffer &&o) noexcept {
-        Buffer::Owned::operator=(std::move(o));
-        std::swap(n, o.n);
-        return *this;
-    }
-    // exactly `count` elements; what the buffer held is released first
-    cudaError_t alloc(size_t count) {
-        const cudaError_t e = this->make([&](T **q) {
-            return Pinned ? cudaHostAlloc(q, count * sizeof(T), cudaHostAllocDefault) : cudaMalloc(q, count * sizeof(T));
-        });
-        n = e == cudaSuccess ? count : 0;
-        return e;
-    }
-    // at least `count` elements. Grown with 25% headroom: scan sizes jitter from frame to frame and a
-    // cudaFree/cudaMalloc pair per new maximum would put milliseconds of allocator time on the hot path
-    int ensure(size_t count) {
-        if (count <= n) return KB_OK;
-        const size_t want = std::max<size_t>(count + count / 4, 1024);
-        const cudaError_t e = alloc(want);
-        if (e != cudaSuccess)
-            return fail(KB_ERR_CUDA, "%s of %zu bytes failed: %s", Pinned ? "cudaHostAlloc" : "cudaMalloc", want * sizeof(T),
-                        cudaGetErrorString(e));
-        return KB_OK;
-    }
-};
-template <class T>
-using DBuf = Buffer<T, false>;
-template <class T>
-using PinBuf = Buffer<T, true>;
-
-// KB_TRACE_STALLS=<ms>: report host-side API calls of the frame paths that block longer than <ms> (diagnostic)
-struct StallTrace {
-    const char *what;
-    std::chrono::steady_clock::time_point t0;
-    static double limit_ms() {
-        static const double v = [] {
-            const char *e = std::getenv("KB_TRACE_STALLS");
-            return e ? std::atof(e) : 0.0;
-        }();
-        return v;
-    }
-    explicit StallTrace(const char *w) : what(w) {
-        if (limit_ms() > 0.0) t0 = std::chrono::steady_clock::now();
-    }
-    ~StallTrace() {
-        if (limit_ms() > 0.0) {
-            const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-            if (ms > limit_ms()) std::fprintf(stderr, "[kb stall] %s took %.1f ms\n", what, ms);
-        }
-    }
-};
-
-size_t pow2_at_least(size_t v) {
-    size_t p = 1;
-    while (p < v) p <<= 1;
-    return p;
-}
-
-// execution context: device, stream, persistent-grid size and the cross-CTA scratch
-struct Exec {
-    int device = 0;
-    cudaStream_t stream = nullptr;
-    Stream own_stream;  // (none when the calling thread set a stream: kb_set_stream)
-    int grid = 0;
-    int sms = 0;  // multiprocessors of the device
-    Scratch sc{};  // all pointers null, profiling off
-    TeamScratch team{};  // ll / out (qrec belongs to the caller's workspace)
-    size_t icp_smem = 96 * 1024;  // dynamic shared memory of the ICP kernels: candidate coordinates of the team's source points (KB_ICP_SMEM_KB)
-    int icp_team_q = TQ_PER_CTA;  // source points per CTA of the ICP team (KB_ICP_TEAM_Q; 0 = whole-grid ICP loop)
-    unsigned tag_seq = 0;  // launch sequence number of the tagged ICP protocol
-    unsigned long long launches = 0;
-    bool bar_dirty = true;  // the barrier words may be non-zero (a kernel without Grid::finish() ran last)
-    std::vector<const void *> smem_opted;  // kernels opted in to > 48 KB of dynamic shared memory on THIS context's device
-    unsigned next_tag_base() { return (++tag_seq) << 13; }  // 8192 epochs per launch
-    // a launch that uses more epochs (k_icp_batch) takes as many consecutive 8192-epoch blocks as it needs
-    unsigned reserve_tags(size_t epochs) {
-        const unsigned first = tag_seq + 1;
-        tag_seq += static_cast<unsigned>((epochs + 8191) / 8192);
-        return first << 13;
-    }
-    DBuf<uint4> batch_ll;  // all-gather regions of k_icp_batch's slots (allocated by the first batch call)
-    std::vector<DBuf<char>> scratch_mem;  // what sc and team point to
-
-    // `view` = a scratch array of `count` elements that lives as long as this context, zeroed on its stream when `zero`
-    template <class T>
-    int scratch(T *&view, size_t count, bool zero) {
-        DBuf<char> b;
-        CK(b.alloc(count * sizeof(T)));
-        if (zero) CK(cudaMemsetAsync(b.p, 0, count * sizeof(T), stream));
-        view = reinterpret_cast<T *>(b.p);
-        scratch_mem.push_back(std::move(b));
-        return KB_OK;
-    }
-    // on `dev`, on `user_stream` (nullptr: a stream of its own)
-    int init(int dev, cudaStream_t user_stream) {
-        RET(require_device());
-        device = dev;
-        CK(cudaSetDevice(device));
-        RET(watchdog_init(device));
-        if (user_stream) {
-            stream = user_stream;
-        } else {
-            CK(own_stream.create());
-            stream = own_stream.p;
-        }
-        int coop = 0;
-        CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-        CK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
-        if (!coop) return fail(KB_ERR_CUDA, "device does not support cooperative launch");
-        grid = tl_grid_blocks > 0 ? std::min(tl_grid_blocks, sms) : sms;
-        grid = std::min(grid, 256);  // the two-level gather tree of the ICP loop handles up to 16 x 16 CTAs
-        RET(scratch(sc.bar, BAR_WORDS, true));
-        RET(scratch(sc.blk_d, 2 * grid * NPART, false));
-        RET(scratch(sc.blk_i, 2 * grid, false));
-        RET(scratch(sc.ll_part, NPART * grid, true));
-        RET(scratch(sc.ll_res, LL_RES, true));
-        RET(scratch(sc.ll_group, NPART * 16, true));
-        RET(scratch(team.ll, 2 * NPART * TEAM_MAX * TEAM_MAX, true));  // 11 MB: one copy of the partials per reader
-        RET(scratch(team.out, 16, false));
-        RET(scratch(sc.dbg, 64 + 4 * grid, true));
-        if (const char *e = std::getenv("KB_ICP_TEAM_Q")) icp_team_q = std::max(0, std::min(std::atoi(e), TQ_MAX));
-        if (const char *e = std::getenv("KB_ICP_SMEM_KB")) icp_smem = static_cast<size_t>(std::max(60, std::min(std::atoi(e), 180))) * 1024;
-        team.smem_bytes = static_cast<int>(icp_smem);
-        team.radius_frac = 0.2;
-        if (const char *e = std::getenv("KB_ICP_RADIUS")) team.radius_frac = std::max(0.01, std::min(std::atof(e), 0.45));
-        return KB_OK;
-    }
-    // opt in to > 48 KB of dynamic shared memory, once per kernel AND device (the attribute is per device)
-    int opt_in_smem(const void *k, size_t bytes) {
-        if (bytes <= 48 * 1024 || std::find(smem_opted.begin(), smem_opted.end(), k) != smem_opted.end()) return KB_OK;
-        CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
-        smem_opted.push_back(k);
-        return KB_OK;
-    }
-    template <class P>
-    int coop(void (*kern)(P), const P &p, size_t smem = 0, bool self_reset = false) {
-        return coop_raw(reinterpret_cast<const void *>(kern), const_cast<P *>(&p), smem, self_reset);
-    }
-    // `kern` takes one parameter struct, `param` points to it (a kernel of another device module: localize_kernel())
-    int coop_raw(const void *kern, void *param, size_t smem, bool self_reset) {
-        CK(cudaSetDevice(device));
-        RET(opt_in_smem(kern, smem));
-        if (!self_reset || bar_dirty)  // kernels that end with Grid::finish() leave the barrier words zeroed themselves
-            CK(cudaMemsetAsync(sc.bar, 0, BAR_WORDS * sizeof(unsigned), stream));
-        bar_dirty = !self_reset;
-        void *args[] = {param};
-        CK(cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(BLOCK), args, smem, stream));
-        ++launches;
-        return KB_OK;
-    }
-    template <class A, class B>
-    int coop(void (*kern)(A, B), const A &a, const B &b) {
-        CK(cudaSetDevice(device));
-        CK(cudaMemsetAsync(sc.bar, 0, BAR_WORDS * sizeof(unsigned), stream));
-        bar_dirty = true;
-        void *args[] = {const_cast<A *>(&a), const_cast<B *>(&b)};
-        CK(cudaLaunchCooperativeKernel(reinterpret_cast<const void *>(kern), dim3(grid), dim3(BLOCK), args, 0, stream));
-        ++launches;
-        return KB_OK;
-    }
-    // wait for the stream with a deadline (KB_SYNC_TIMEOUT_S, default 30 s; 0 = wait forever): a launch that never
-    // ends is reported as KB_ERR_CUDA instead of hanging the caller (the device watchdog should have fired long before)
-    int sync() {
-        RET(wait_deadline([&] { return cudaStreamQuery(stream); }, "stream"));
-        return watchdog_check(device);
-    }
-    template <class Q>
-    int wait_deadline(Q query, const char *what) {
-        static const double limit_s = [] {
-            const char *e = std::getenv("KB_SYNC_TIMEOUT_S");
-            return e ? std::atof(e) : 30.0;
-        }();
-        const auto t0 = std::chrono::steady_clock::now();
-        for (unsigned spins = 0;; ++spins) {
-            const cudaError_t e = query();
-            if (e == cudaSuccess) return KB_OK;
-            if (e != cudaErrorNotReady) return fail(KB_ERR_CUDA, "%s wait failed: %s", what, cudaGetErrorString(e));
-            if ((spins & 0x3ff) == 0x3ff && limit_s > 0.0 &&
-                std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() > limit_s) {
-                const int wd = watchdog_check(device);
-                device_stuck(device);
-                if (wd != KB_OK) return wd;
-                return fail(KB_ERR_CUDA, "the device did not finish the %s within %.0f s (launch %llu): giving up; %s", what, limit_s, launches,
-                            phase_marks(device).c_str());
-            }
-        }
-    }
-};
-
-
-// on the calling thread's device and stream (kb_set_device / kb_set_stream) unless given others
-int make_exec(std::shared_ptr<Exec> *out, int device = tl_device, cudaStream_t user_stream = tl_user_stream) {
-    auto e = std::make_shared<Exec>();
-    RET(e->init(device, user_stream));
-    *out = e;
-    return KB_OK;
-}
-
 // per-call workspace sized by the largest cloud seen
 struct Work {
     DBuf<double> in, ts, tmp, pre, ds1, src, work, tp;
@@ -684,6 +305,15 @@ struct kb_map {
     }
 };
 
+// what the host-only subsystems (api.cuh) use of a map
+Exec &kb_host::map_exec(const kb_map *map) { return *map->ex; }
+MapView kb_host::map_view(const kb_map *map) { return map->view(); }
+int kb_host::map_pull_live(kb_map *map, int *live) { return map->pull_live(live); }
+int kb_host::map_load(kb_map *map, const int *d_vox, const int *d_cnt, const long long *d_off, const double *d_pts, size_t nv,
+                      size_t np) {
+    return map->load(d_vox, d_cnt, d_off, d_pts, nv, np);
+}
+
 struct kb_registration {
     int max_iter;
     double conv;
@@ -796,25 +426,13 @@ int run_downsample(Exec &ex, Work &ws, const double *d_in, size_t n, double v1, 
 }
 }  // namespace
 
-extern "C" {
+int kb_host::map_in_use(const kb_map *map) {
+    const int r = map->readers.load();
+    if (r) return fail(KB_ERR_INVALID_ARG, "the map is in use by %d localizer%s: it cannot be changed or destroyed", r, r == 1 ? "" : "s");
+    return KB_OK;
+}
 
-const char *kb_last_error(void) { return tl_err.c_str(); }
-const char *kb_version(void) { return "kiss_icp_b200 0.1 (sm_90a)"; }
-int kb_device_count(void) { return device_count(); }
-int kb_set_device(int device) {
-    if (device < 0 || device >= device_count()) return fail(KB_ERR_INVALID_ARG, "device %d out of range", device);
-    tl_device = device;
-    return KB_OK;
-}
-int kb_set_stream(void *cuda_stream) {
-    tl_user_stream = static_cast<cudaStream_t>(cuda_stream);
-    return KB_OK;
-}
-int kb_set_grid_blocks(int blocks) {
-    if (blocks < 0) return fail(KB_ERR_INVALID_ARG, "blocks < 0");
-    tl_grid_blocks = blocks;
-    return KB_OK;
-}
+extern "C" {
 
 // ------------------------------------------------------------------------------- VoxelHashMap
 static int map_create_impl(double voxel_size, double max_distance, unsigned cap, std::shared_ptr<Exec> ex, kb_map **out) {
@@ -836,12 +454,6 @@ static int map_create_impl(double voxel_size, double max_distance, unsigned cap,
 }
 int kb_map_create(double voxel_size, double max_distance, unsigned max_points_per_voxel, kb_map **out) {
     return map_create_impl(voxel_size, max_distance, max_points_per_voxel, nullptr, out);
-}
-// every call that changes or frees a map fails while localizers read it (kb_pipeline_create_localizer)
-static int map_in_use(const kb_map *map) {
-    const int r = map->readers.load();
-    if (r) return fail(KB_ERR_INVALID_ARG, "the map is in use by %d localizer%s: it cannot be changed or destroyed", r, r == 1 ? "" : "s");
-    return KB_OK;
 }
 int kb_map_destroy(kb_map *map) {
     if (map && !map->borrowed) {
@@ -1534,17 +1146,12 @@ int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_ma
         return fail(KB_ERR_INVALID_ARG, "%zu source points x top_k %d refinements exceed 2^31 - 1 points", n, search->top_k);
     RET(require_device());
     if (!reg || !map) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    // every voxel coordinate must fit in an int: |(R_h p + t_h)_c| <= |p| (1 + 1e-6: R within SE(3)'s tolerance) + |t_h|_max
-    double pmax = 0.0;
-    for (size_t i = 0; i < n; ++i) {
-        const double r = std::sqrt(xyz[3 * i] * xyz[3 * i] + xyz[3 * i + 1] * xyz[3 * i + 1] + xyz[3 * i + 2] * xyz[3 * i + 2]);
-        if (!std::isfinite(r)) return fail(KB_ERR_INVALID_ARG, "source point %zu is not finite", i);
-        pmax = std::max(pmax, r);
-    }
     const double tmax = std::max({std::fabs(g.xs.front()), std::fabs(g.xs.back()), std::fabs(g.ys.front()),
                                   std::fabs(g.ys.back()), std::fabs(g.tz)});
-    const double reach = (pmax * (1.0 + 1e-6) + tmax) / map->voxel_size + 1.0;
-    if (!(reach < 2147483000.0))
+    double reach;
+    size_t bad;
+    if (!voxel_reach(xyz, n, tmax, map->voxel_size, &reach, &bad)) return fail(KB_ERR_INVALID_ARG, "source point %zu is not finite", bad);
+    if (!(reach < kIntReach))
         return fail(KB_ERR_INVALID_ARG, "a hypothesis maps source points to voxel coordinates beyond the int range (%.3g)", reach);
     Exec &ex = *map->ex;
     CK(cudaSetDevice(ex.device));
@@ -1559,16 +1166,13 @@ int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_ma
     RET(reg->ws.src.ensure(3 * n));
     RET(reg->rgrid.ensure(grid.size()));
     RET(reg->rscore.ensure(g.H));
-    if (reg->rev[1].device != ex.device) {  // (rev[1] is made last: both exist on that device)
-        CK(reg->rev[0].create(cudaEventDefault));
-        CK(reg->rev[1].create(cudaEventDefault));
-    }
+    RET(events_on(reg->rev, ex.device));
     CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
     CK(cudaMemcpyAsync(reg->rgrid.p, grid.data(), grid.size() * sizeof(double), cudaMemcpyHostToDevice, ex.stream));
     const MapView mv = map->view();
     const double *d_rot = reg->rgrid.p, *d_xs = d_rot + g.rot.size(), *d_ys = d_xs + g.nx;
     CK(cudaEventRecord(reg->rev[0].p, ex.stream));
-    CK(reloc_score(&mv, sizeof(mv), reg->ws.src.p, static_cast<int>(n), d_rot, g.n_yaw, d_xs, g.nx, d_ys, g.ny, g.tz,
+    CK(reloc_score(mv, reg->ws.src.p, static_cast<int>(n), d_rot, g.n_yaw, d_xs, g.nx, d_ys, g.ny, g.tz,
                    reg->rscore.p, ex.sms, ex.stream));
     ++ex.launches;
     CK(cudaEventRecord(reg->rev[1].p, ex.stream));
@@ -1586,27 +1190,17 @@ int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_ma
         if (!se3_from_matrix(&cand[16 * c], &guesses[c])) return fail(KB_ERR_NOT_SE3, "candidate %zu is not in SE(3)", c);
     }
 
-    // 4. refinement: align_batch of the source from every candidate, inliers on
-    const std::vector<size_t> off(K, 0), cnt(K, n);
-    const std::vector<double> md(K, search->max_correspondence_distance), ks(K, search->kernel_scale);
-    RET(reg->bpose.ensure(16 * K));
-    RET(reg->biout.ensure(2 * K));
-    RET(align_batch_run(reg, map, reg->ws.src.p, off.data(), cnt.data(), K, guesses, md.data(), ks.data(), reg->bpose.p,
-                        reg->biout.p, reg->biout.p + K));
-    std::vector<double> refined(16 * K);
-    std::vector<int> io(2 * K);  // iterations [K], inliers [K]
-    CK(cudaMemcpyAsync(refined.data(), reg->bpose.p, 16 * K * sizeof(double), cudaMemcpyDeviceToHost, ex.stream));
-    CK(cudaMemcpyAsync(io.data(), reg->biout.p, 2 * K * sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
-    RET(ex.sync());
-
-    // 5. winner and runner-up
+    // 4-5. refinement, winner and runner-up
+    std::vector<double> refined;
+    std::vector<int> its, inl;
     size_t w;
     long long ru;
-    reloc_winner(refined.data(), io.data() + K, K, 2.0 * search->step, 2.0 * search->yaw_step, &w, &ru);
+    RET(refine_candidates(reg, map, nullptr, n, guesses, search->max_correspondence_distance, search->kernel_scale,
+                          2.0 * search->step, 2.0 * search->yaw_step, &refined, &its, &inl, &w, &ru));
     kb_reloc_result r{};
     std::memcpy(r.pose, &refined[16 * w], sizeof(r.pose));
-    r.inliers = io[K + w];
-    r.iterations = io[w];
+    r.inliers = inl[w];
+    r.iterations = its[w];
     r.rank = static_cast<int>(w);
     r.n_source = static_cast<int>(n);
     r.n_hypotheses = static_cast<int>(g.H);
@@ -1615,943 +1209,13 @@ int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_ma
     r.runner_up_inliers = -1;
     if (ru >= 0) {
         std::memcpy(r.runner_up_pose, &refined[16 * ru], sizeof(r.runner_up_pose));
-        r.runner_up_inliers = io[K + ru];
+        r.runner_up_inliers = inl[ru];
     }
     *out = r;
     if (candidates) std::memcpy(candidates, cand.data(), cand.size() * sizeof(double));
     if (candidate_scores)
         for (size_t c = 0; c < K; ++c) candidate_scores[c] = sc[peaks[c]];
     if (scores) std::memcpy(scores, sc.data(), g.H * sizeof(int));
-    return KB_OK;
-}
-
-// ------------------------------------------------------------------------------- Place recognition
-// A database of Scan Context descriptors (places.cu has the kernels). The device holds every entry's raw descriptor (for
-// kb_place_db_dump), unit columns and nonempty mask; the keyframe poses stay on the host, where the candidate walk runs.
-struct kb_place_db {
-    std::shared_ptr<Exec> ex;
-    kb_place_params prm;
-    size_t n = 0, cap = 0;          // entries, and entries the storage holds
-    DBuf<double> geom;              // ring boundaries [n_rings + 1], then sector directions [n_sectors + 1][2]
-    DBuf<double> raw, unit;         // [cap][n_rings][n_sectors], [cap][n_sectors][n_rings]
-    DBuf<unsigned char> mask;       // [cap][n_sectors]
-    std::vector<double> poses;      // [n][16]
-    DBuf<double> pts;               // the cloud being described
-    DBuf<double> q_raw, q_unit;     // a query's descriptor
-    DBuf<unsigned char> q_mask;
-    DBuf<double> dist;              // [entries searched] of the last query
-    DBuf<int> shift;
-    Event ev[2];                    // around the last k_place_distance (kb_debug_place_distance_ms)
-    size_t cells() const { return static_cast<size_t>(prm.n_rings) * prm.n_sectors; }
-};
-
-static constexpr size_t kPlaceMaxEntries = size_t(1) << 24;
-static constexpr double kPi = 3.141592653589793;
-
-static int place_params_check(const kb_place_params *p) {
-    if (!p) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (p->n_rings < 1 || p->n_rings > 64) return fail(KB_ERR_INVALID_ARG, "n_rings must be in [1, 64]");
-    if (p->n_sectors < 3 || p->n_sectors > 720) return fail(KB_ERR_INVALID_ARG, "n_sectors must be in [3, 720]");
-    if (p->n_rings * p->n_sectors > 4096) return fail(KB_ERR_INVALID_ARG, "n_rings * n_sectors must be <= 4096");
-    if (!(p->max_radius > 0.0) || !std::isfinite(p->max_radius)) return fail(KB_ERR_INVALID_ARG, "max_radius must be finite and > 0");
-    if (!std::isfinite(p->z_offset)) return fail(KB_ERR_INVALID_ARG, "z_offset must be finite");
-    return KB_OK;
-}
-static double place_sector_width(const kb_place_params &p) { return (2.0 * kPi) / p.n_sectors; }
-static int points_finite(const double *xyz, size_t n, const char *what) {
-    if (!xyz && n) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (n > static_cast<size_t>(INT_MAX)) return fail(KB_ERR_INVALID_ARG, "%s: more than 2^31 - 1 points", what);
-    for (size_t i = 0; i < 3 * n; ++i)
-        if (!std::isfinite(xyz[i])) return fail(KB_ERR_INVALID_ARG, "%s: point %zu is not finite", what, i / 3);
-    return KB_OK;
-}
-// the descriptor of the host cloud xyz[n] into raw / unit / mask (device, one entry's room) on the database's stream
-static int place_describe(kb_place_db *db, const double *xyz, size_t n, double *raw, double *unit, unsigned char *mask) {
-    Exec &ex = *db->ex;
-    CK(cudaSetDevice(ex.device));
-    const int R = db->prm.n_rings, S = db->prm.n_sectors;
-    CK(cudaMemsetAsync(raw, 0, db->cells() * sizeof(double), ex.stream));
-    if (n) {
-        RET(db->pts.ensure(3 * n));
-        CK(cudaMemcpyAsync(db->pts.p, xyz, n * 3 * sizeof(double), cudaMemcpyHostToDevice, ex.stream));
-        CK(place_descriptor(db->pts.p, static_cast<int>(n), db->geom.p, db->geom.p + R + 1, R, S, db->prm.z_offset,
-                            reinterpret_cast<unsigned long long *>(raw), ex.sms, ex.stream));
-        ++ex.launches;
-    }
-    CK(place_columns(raw, 1, R, S, unit, mask, ex.stream));
-    ++ex.launches;
-    return KB_OK;
-}
-// storage for at least `need` entries; the first db->n are copied into the new allocation
-static int place_reserve(kb_place_db *db, size_t need) {
-    if (need <= db->cap) return KB_OK;
-    size_t cap = std::max<size_t>(db->cap, 256);
-    while (cap < need) cap *= 2;
-    cap = std::min(cap, kPlaceMaxEntries);
-    const size_t C = db->cells(), S = static_cast<size_t>(db->prm.n_sectors);
-    DBuf<double> raw, unit;
-    DBuf<unsigned char> mask;
-    cudaError_t e;
-    if ((e = raw.alloc(cap * C)) != cudaSuccess || (e = unit.alloc(cap * C)) != cudaSuccess || (e = mask.alloc(cap * S)) != cudaSuccess)
-        return fail(KB_ERR_CUDA, "place database storage (%zu entries): %s", cap, cudaGetErrorString(e));
-    Exec &ex = *db->ex;
-    if (db->n) {
-        CK(cudaMemcpyAsync(raw.p, db->raw.p, db->n * C * sizeof(double), cudaMemcpyDeviceToDevice, ex.stream));
-        CK(cudaMemcpyAsync(unit.p, db->unit.p, db->n * C * sizeof(double), cudaMemcpyDeviceToDevice, ex.stream));
-        CK(cudaMemcpyAsync(mask.p, db->mask.p, db->n * S, cudaMemcpyDeviceToDevice, ex.stream));
-    }
-    RET(ex.sync());  // (the old storage is released below)
-    db->raw = std::move(raw);
-    db->unit = std::move(unit);
-    db->mask = std::move(mask);
-    db->cap = cap;
-    return KB_OK;
-}
-// the arguments of a query that need no handle
-static int place_query_check(const double *xyz, size_t n, double separation, int top_k) {
-    RET(points_finite(xyz, n, "query cloud"));
-    if (top_k < 1 || top_k > 256) return fail(KB_ERR_INVALID_ARG, "top_k must be in [1, 256]");
-    if (!(separation >= 0.0) || !std::isfinite(separation)) return fail(KB_ERR_INVALID_ARG, "separation must be finite and >= 0");
-    return KB_OK;
-}
-// the query of xyz[n] against entries [0, M): every entry's distance and shift, then the candidate walk
-static int place_search(kb_place_db *db, const double *xyz, size_t n, int max_entry, double separation, int top_k,
-                 std::vector<kb_place_match> *matches, std::vector<double> *dist, std::vector<int> *shift) {
-    const size_t M = max_entry < 0 ? db->n : std::min(static_cast<size_t>(max_entry), db->n);
-    if (M == 0) return fail(KB_ERR_INVALID_ARG, "no entry to search (%zu entries, max_entry %d)", db->n, max_entry);
-    Exec &ex = *db->ex;
-    const int R = db->prm.n_rings, S = db->prm.n_sectors;
-    RET(db->q_raw.ensure(db->cells()));
-    RET(db->q_unit.ensure(db->cells()));
-    RET(db->q_mask.ensure(S));
-    RET(db->dist.ensure(M));
-    RET(db->shift.ensure(M));
-    RET(place_describe(db, xyz, n, db->q_raw.p, db->q_unit.p, db->q_mask.p));
-    if (db->ev[1].device != ex.device) {  // (ev[1] is made last: both exist on that device)
-        CK(db->ev[0].create(cudaEventDefault));
-        CK(db->ev[1].create(cudaEventDefault));
-    }
-    CK(cudaEventRecord(db->ev[0].p, ex.stream));
-    CK(place_distance(db->q_unit.p, db->q_mask.p, db->unit.p, db->mask.p, static_cast<int>(M), R, S, db->dist.p,
-                      db->shift.p, ex.grid, ex.stream));
-    ++ex.launches;
-    CK(cudaEventRecord(db->ev[1].p, ex.stream));
-    dist->resize(M);
-    shift->resize(M);
-    CK(cudaMemcpyAsync(dist->data(), db->dist.p, M * sizeof(double), cudaMemcpyDeviceToHost, ex.stream));
-    CK(cudaMemcpyAsync(shift->data(), db->shift.p, M * sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
-    RET(ex.sync());
-    std::vector<int> order(M);
-    for (size_t i = 0; i < M; ++i) order[i] = static_cast<int>(i);
-    std::sort(order.begin(), order.end(), [&](int a, int b) { return (*dist)[a] != (*dist)[b] ? (*dist)[a] < (*dist)[b] : a < b; });
-    const double width = place_sector_width(db->prm);
-    matches->clear();
-    for (size_t o = 0; o < M && matches->size() < static_cast<size_t>(top_k); ++o) {
-        const int i = order[o];
-        const double *T = &db->poses[16 * static_cast<size_t>(i)];
-        bool near = false;
-        for (const kb_place_match &c : *matches) {
-            const double *U = &db->poses[16 * static_cast<size_t>(c.entry)];
-            if (std::hypot(T[3] - U[3], T[7] - U[7]) < separation) {
-                near = true;
-                break;
-            }
-        }
-        if (near) continue;
-        kb_place_match m{};
-        m.entry = i;
-        m.shift = (*shift)[i];
-        m.yaw = m.shift * width;
-        m.distance = (*dist)[i];
-        const double cs = std::cos(m.yaw), sn = std::sin(m.yaw);
-        const double Rz[9] = {cs, -sn, 0.0, sn, cs, 0.0, 0.0, 0.0, 1.0};
-        for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) m.guess[4 * r + c] = (T[4 * r] * Rz[c] + T[4 * r + 1] * Rz[3 + c]) + T[4 * r + 2] * Rz[6 + c];
-            m.guess[4 * r + 3] = T[4 * r + 3];
-        }
-        for (int c = 0; c < 4; ++c) m.guess[12 + c] = T[12 + c];
-        matches->push_back(m);
-    }
-    return KB_OK;
-}
-
-void kb_place_params_default(kb_place_params *p) {
-    if (p) *p = kb_place_params{20, 60, 80.0, 2.0};
-}
-int kb_place_db_create(const kb_place_params *p, kb_place_db **out) {
-    RET(place_params_check(p));
-    if (!out) return fail(KB_ERR_INVALID_ARG, "out == NULL");
-    RET(require_device());
-    auto db = std::make_unique<kb_place_db>();
-    db->prm = *p;
-    RET(make_exec(&db->ex));
-    const int R = p->n_rings, S = p->n_sectors;
-    std::vector<double> geom(R + 1 + 2 * (S + 1));
-    const double w = p->max_radius / R;
-    for (int i = 0; i < R; ++i) {
-        const double ri = i * w;
-        geom[i] = ri * ri;
-    }
-    geom[R] = p->max_radius * p->max_radius;
-    const double width = place_sector_width(*p);
-    for (int k = 0; k < S; ++k) {
-        const double th = -kPi + k * width;
-        geom[R + 1 + 2 * k] = std::cos(th);
-        geom[R + 1 + 2 * k + 1] = std::sin(th);
-    }
-    geom[R + 1 + 2 * S] = geom[R + 1];
-    geom[R + 1 + 2 * S + 1] = geom[R + 2];
-    CK(db->geom.alloc(geom.size()));
-    CK(cudaMemcpyAsync(db->geom.p, geom.data(), geom.size() * sizeof(double), cudaMemcpyHostToDevice, db->ex->stream));
-    RET(place_reserve(db.get(), 1));
-    *out = db.release();
-    return KB_OK;
-}
-int kb_place_db_destroy(kb_place_db *db) {
-    delete db;
-    return KB_OK;
-}
-int kb_place_db_size(const kb_place_db *db, size_t *out) {
-    if (!db || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    *out = db->n;
-    return KB_OK;
-}
-int kb_place_descriptor(kb_place_db *db, const double *xyz, size_t n, double *out) {
-    RET(points_finite(xyz, n, "cloud"));
-    if (!out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    RET(require_device());
-    if (!db) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    CK(cudaSetDevice(db->ex->device));  // (the buffers below belong to the database's device)
-    RET(db->q_raw.ensure(db->cells()));
-    RET(db->q_unit.ensure(db->cells()));
-    RET(db->q_mask.ensure(db->prm.n_sectors));
-    RET(place_describe(db, xyz, n, db->q_raw.p, db->q_unit.p, db->q_mask.p));
-    std::vector<double> d(db->cells());
-    CK(cudaMemcpyAsync(d.data(), db->q_raw.p, d.size() * sizeof(double), cudaMemcpyDeviceToHost, db->ex->stream));
-    RET(db->ex->sync());
-    std::memcpy(out, d.data(), d.size() * sizeof(double));
-    return KB_OK;
-}
-int kb_place_db_add(kb_place_db *db, const double *xyz, size_t n, const double pose[16], size_t *index) {
-    RET(points_finite(xyz, n, "cloud"));
-    if (!pose) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    for (int i = 0; i < 16; ++i)
-        if (!std::isfinite(pose[i])) return fail(KB_ERR_INVALID_ARG, "pose is not finite");
-    SE3 T;
-    if (!se3_from_matrix(pose, &T)) return fail(KB_ERR_NOT_SE3, "pose is not in SE(3)");
-    RET(require_device());
-    if (!db) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    CK(cudaSetDevice(db->ex->device));  // (growth allocates on the database's device)
-    if (db->n >= kPlaceMaxEntries) return fail(KB_ERR_CAPACITY, "the database holds 2^24 entries");
-    RET(place_reserve(db, db->n + 1));
-    const size_t C = db->cells();
-    RET(place_describe(db, xyz, n, db->raw.p + db->n * C, db->unit.p + db->n * C, db->mask.p + db->n * db->prm.n_sectors));
-    RET(db->ex->sync());
-    db->poses.insert(db->poses.end(), pose, pose + 16);
-    if (index) *index = db->n;
-    ++db->n;
-    return KB_OK;
-}
-int kb_place_db_dump(const kb_place_db *cdb, double *descriptors, double *poses, size_t cap, size_t *n_out) {
-    kb_place_db *db = const_cast<kb_place_db *>(cdb);
-    if (!db || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    const size_t N = db->n;
-    if ((!descriptors && !poses) || cap == 0) {
-        *n_out = N;
-        return KB_OK;
-    }
-    if (cap < N) {
-        *n_out = N;
-        return fail(KB_ERR_CAPACITY, "buffers too small (%zu < %zu entries)", cap, N);
-    }
-    if (descriptors && N) {
-        CK(cudaSetDevice(db->ex->device));
-        CK(cudaMemcpyAsync(descriptors, db->raw.p, N * db->cells() * sizeof(double), cudaMemcpyDeviceToHost, db->ex->stream));
-        RET(db->ex->sync());
-    }
-    if (poses && N) std::memcpy(poses, db->poses.data(), N * 16 * sizeof(double));
-    *n_out = N;
-    return KB_OK;
-}
-int kb_place_db_load(kb_place_db *db, const double *descriptors, const double *poses, size_t n) {
-    if (n > kPlaceMaxEntries) return fail(KB_ERR_INVALID_ARG, "%zu entries: at most 2^24", n);
-    if (n && (!poses || !descriptors)) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    for (size_t i = 0; i < n; ++i) {
-        for (int j = 0; j < 16; ++j)
-            if (!std::isfinite(poses[16 * i + j])) return fail(KB_ERR_INVALID_ARG, "pose %zu is not finite", i);
-        SE3 T;
-        if (!se3_from_matrix(poses + 16 * i, &T)) return fail(KB_ERR_NOT_SE3, "pose %zu is not in SE(3)", i);
-    }
-    RET(require_device());
-    if (!db) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    CK(cudaSetDevice(db->ex->device));  // (the new storage is allocated on the database's device)
-    const size_t C = db->cells();
-    for (size_t i = 0; i < n * C; ++i)
-        if (!(descriptors[i] >= 0.0) || !std::isfinite(descriptors[i]))
-            return fail(KB_ERR_INVALID_ARG, "descriptor %zu: value %zu is negative or not finite", i / C, i % C);
-    // into new storage: the database changes only once everything has succeeded
-    kb_place_db next;
-    next.ex = db->ex;
-    next.prm = db->prm;
-    RET(place_reserve(&next, std::max<size_t>(n, 1)));
-    Exec &ex = *db->ex;
-    if (n) {
-        CK(cudaMemcpyAsync(next.raw.p, descriptors, n * C * sizeof(double), cudaMemcpyHostToDevice, ex.stream));
-        CK(place_columns(next.raw.p, n, db->prm.n_rings, db->prm.n_sectors, next.unit.p, next.mask.p, ex.stream));
-        ++ex.launches;
-    }
-    RET(ex.sync());
-    db->raw = std::move(next.raw);
-    db->unit = std::move(next.unit);
-    db->mask = std::move(next.mask);
-    db->cap = next.cap;
-    db->n = n;
-    db->poses.assign(poses, poses + 16 * n);
-    return KB_OK;
-}
-int kb_place_query(kb_place_db *db, const double *xyz, size_t n, int max_entry, double separation, int top_k,
-                   kb_place_match *out, size_t *n_out, double *entry_distances, int *entry_shifts) {
-    RET(place_query_check(xyz, n, separation, top_k));
-    if (!out || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    RET(require_device());
-    if (!db) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    CK(cudaSetDevice(db->ex->device));  // (the query's buffers belong to the database's device)
-    std::vector<kb_place_match> m;
-    std::vector<double> dist;
-    std::vector<int> shift;
-    RET(place_search(db, xyz, n, max_entry, separation, top_k, &m, &dist, &shift));
-    std::copy(m.begin(), m.end(), out);
-    *n_out = m.size();
-    if (entry_distances) std::copy(dist.begin(), dist.end(), entry_distances);
-    if (entry_shifts) std::copy(shift.begin(), shift.end(), entry_shifts);
-    return KB_OK;
-}
-int kb_place_relocalize(kb_registration *reg, kb_place_db *db, const double *desc_xyz, size_t n_desc,
-                        const double *src_xyz, size_t n_src, const kb_map *cmap, const kb_place_search *s,
-                        kb_place_result *out, kb_place_match *candidates) {
-    kb_map *map = const_cast<kb_map *>(cmap);
-    if (!s || !out || !src_xyz) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    RET(place_query_check(desc_xyz, n_desc, s->separation, s->top_k));
-    if (n_src == 0) return fail(KB_ERR_INVALID_ARG, "empty source");
-    RET(points_finite(src_xyz, n_src, "source"));
-    if (n_src * static_cast<size_t>(s->top_k) > static_cast<size_t>(INT_MAX))
-        return fail(KB_ERR_INVALID_ARG, "%zu source points x top_k %d refinements exceed 2^31 - 1 points", n_src, s->top_k);
-    RET(require_device());
-    if (!reg || !db || !map) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (db->ex->device != map->ex->device) return fail(KB_ERR_INVALID_ARG, "the database and the map are on different devices");
-    Exec &ex = *map->ex;
-    CK(cudaSetDevice(ex.device));
-    int live = 0;
-    RET(map->pull_live(&live));
-    if (live == 0) return fail(KB_ERR_INVALID_ARG, "the map is empty");
-
-    // 1. candidates
-    std::vector<kb_place_match> m;
-    std::vector<double> dist;
-    std::vector<int> shift;
-    RET(place_search(db, desc_xyz, n_desc, s->max_entry, s->separation, s->top_k, &m, &dist, &shift));
-    const size_t K = m.size();
-    std::vector<SE3> guesses(K);
-    for (size_t c = 0; c < K; ++c)
-        if (!se3_from_matrix(m[c].guess, &guesses[c])) return fail(KB_ERR_NOT_SE3, "candidate %zu is not in SE(3)", c);
-
-    // 2. refinement: align_batch of the source from every candidate, inliers on
-    CK(cudaSetDevice(ex.device));
-    RET(reg->ws.src.ensure(3 * n_src));
-    CK(cudaMemcpyAsync(reg->ws.src.p, src_xyz, n_src * 24, cudaMemcpyHostToDevice, ex.stream));
-    const std::vector<size_t> off(K, 0), cnt(K, n_src);
-    const std::vector<double> md(K, s->max_correspondence_distance), ks(K, s->kernel_scale);
-    RET(reg->bpose.ensure(16 * K));
-    RET(reg->biout.ensure(2 * K));
-    RET(align_batch_run(reg, map, reg->ws.src.p, off.data(), cnt.data(), K, guesses, md.data(), ks.data(), reg->bpose.p,
-                        reg->biout.p, reg->biout.p + K));
-    std::vector<double> refined(16 * K);
-    std::vector<int> io(2 * K);  // iterations [K], inliers [K]
-    CK(cudaMemcpyAsync(refined.data(), reg->bpose.p, 16 * K * sizeof(double), cudaMemcpyDeviceToHost, ex.stream));
-    CK(cudaMemcpyAsync(io.data(), reg->biout.p, 2 * K * sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
-    RET(ex.sync());
-
-    // 3. winner and runner-up
-    size_t w;
-    long long ru;
-    reloc_winner(refined.data(), io.data() + K, K, s->separation, 2.0 * place_sector_width(db->prm), &w, &ru);
-    kb_place_result r{};
-    std::memcpy(r.pose, &refined[16 * w], sizeof(r.pose));
-    r.inliers = io[K + w];
-    r.iterations = io[w];
-    r.rank = static_cast<int>(w);
-    r.n_source = static_cast<int>(n_src);
-    r.n_entries = static_cast<int>(dist.size());
-    r.n_candidates = static_cast<int>(K);
-    r.runner_up_inliers = -1;
-    if (ru >= 0) {
-        std::memcpy(r.runner_up_pose, &refined[16 * ru], sizeof(r.runner_up_pose));
-        r.runner_up_inliers = io[K + ru];
-    }
-    *out = r;
-    if (candidates) std::copy(m.begin(), m.end(), candidates);
-    return KB_OK;
-}
-
-// ------------------------------------------------------------------------------- Pose graph
-// The graph lives on the host (kb_pose_graph_* in the header state the problem and the method; pose_graph.cu has the
-// kernel). Edges are immutable, so an optimize uploads only those added since the last one; the poses, the fixed flags
-// and the incidence lists are uploaded every time.
-struct kb_pose_graph {
-    int device = 0;                  // of the creating thread: where the buffers go at the first optimize
-    cudaStream_t user_stream = nullptr;
-    std::vector<double> mat;         // [N][16] the poses as given or as last optimized (fixed nodes: as given, bit for bit)
-    std::vector<SE3> pose;           // [N] the same poses as the optimizer carries them
-    std::vector<int> fixed;          // [N]
-    std::vector<int> ij;             // [E][2]
-    std::vector<double> meas_inv;    // [E][8] Z^-1
-    std::vector<double> info;        // [E][36]
-    std::vector<double> robust;      // [E]
-    std::shared_ptr<Exec> ex;
-    size_t uploaded = 0;             // edges on the device
-    DBuf<double> pose_d, cand, hd, grad, D, U, UL, vec, part;
-    DBuf<double> meas_d, info_d, rob_d, e_s, e_w, e_jj, e_ii, e_ad, e_g;
-    DBuf<int> fixed_d, inc_ptr, inc, ij_d, flag;
-    DBuf<kb_pose_graph_report> report;
-    Event ev[2];                     // around the last launch (kb_debug_pose_graph_ms)
-    // the covariance (kb_pose_graph_marginals & co.): the symbolic analysis for (N, E), its copy on the device, the
-    // numeric factor at the current poses (valid until the next add_node, add_edge or optimize) and the solves
-    PgcSymbolic sym;
-    int sym_dev_n = -1, sym_dev_e = -1;  // the graph the device copy of `sym` was made for
-    bool factored = false;
-    DBuf<int> s_order, s_pos, s_parent, s_col_slot, s_lev_ptr, s_colptr, s_brow, s_bcol, s_hptr, s_hedge, s_uptr, s_upd;
-    DBuf<int> cov_flag, cov_req, cov_path;
-    DBuf<double> Lx, cov_X, cov_out;
-    Event cev[4];                    // around the last factorization and the last marginal solves (kb_debug_pose_graph_cov_ms)
-    size_t n() const { return fixed.size(); }
-    size_t m() const { return robust.size(); }
-};
-
-static constexpr size_t kPoseGraphMaxNodes = size_t(1) << 22, kPoseGraphMaxEdges = size_t(1) << 24;
-
-static int pg_se3_arg(const double M[16], const char *what, SE3 *out) {
-    if (!M) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    for (int k = 0; k < 16; ++k)
-        if (!std::isfinite(M[k])) return fail(KB_ERR_NOT_SE3, "%s is not finite", what);
-    if (!se3_from_matrix(M, out)) return fail(KB_ERR_NOT_SE3, "%s is not in SE(3)", what);
-    return KB_OK;
-}
-
-static int pg_options_check(const kb_pose_graph_options &o) {
-    if (o.max_iterations < 0 || o.max_iterations > 1000000) return fail(KB_ERR_INVALID_ARG, "max_iterations must be in [0, 10^6]");
-    if (!(o.function_tolerance >= 0.0) || !std::isfinite(o.function_tolerance))
-        return fail(KB_ERR_INVALID_ARG, "function_tolerance must be finite and >= 0");
-    if (!(o.parameter_tolerance >= 0.0) || !std::isfinite(o.parameter_tolerance))
-        return fail(KB_ERR_INVALID_ARG, "parameter_tolerance must be finite and >= 0");
-    if (!(o.initial_lambda > 0.0 && o.initial_lambda <= 1e12)) return fail(KB_ERR_INVALID_ARG, "initial_lambda must be in (0, 1e12]");
-    if (o.max_cg_iterations < 1 || o.max_cg_iterations > 1000000) return fail(KB_ERR_INVALID_ARG, "max_cg_iterations must be in [1, 10^6]");
-    if (!(o.cg_tolerance >= 0.0 && o.cg_tolerance < 1.0)) return fail(KB_ERR_INVALID_ARG, "cg_tolerance must be in [0, 1)");
-    return KB_OK;
-}
-
-// every free node reaches a fixed node through edges (the gauge): union-find over the edges
-static int pg_gauge_check(const kb_pose_graph &g) {
-    const size_t N = g.n();
-    std::vector<size_t> parent(N);
-    std::iota(parent.begin(), parent.end(), size_t(0));
-    auto root = [&](size_t a) {
-        while (parent[a] != a) a = parent[a] = parent[parent[a]];
-        return a;
-    };
-    for (size_t e = 0; e < g.m(); ++e) {
-        const size_t a = root(static_cast<size_t>(g.ij[2 * e])), b = root(static_cast<size_t>(g.ij[2 * e + 1]));
-        if (a != b) parent[std::max(a, b)] = std::min(a, b);
-    }
-    std::vector<char> grounded(N, 0);
-    for (size_t k = 0; k < N; ++k)
-        if (g.fixed[k]) grounded[root(k)] = 1;
-    for (size_t k = 0; k < N; ++k)
-        if (!grounded[root(k)])
-            return fail(KB_ERR_INVALID_ARG, "node %zu is free and no path of edges connects it to a fixed node (the gauge is free)", k);
-    return KB_OK;
-}
-
-// device buffers for the graph as it is now; edge buffers that had to grow are uploaded again from edge 0
-static int pg_reserve(kb_pose_graph *g, int grid) {
-    const size_t N = std::max<size_t>(g->n(), 1), E = std::max<size_t>(g->m(), 1);
-    RET(g->pose_d.ensure(8 * N));
-    RET(g->cand.ensure(8 * N));
-    RET(g->hd.ensure(36 * N));
-    RET(g->D.ensure(36 * N));
-    RET(g->U.ensure(36 * N));
-    RET(g->UL.ensure(36 * N));
-    RET(g->grad.ensure(6 * N));
-    RET(g->vec.ensure(6 * 6 * N));
-    RET(g->fixed_d.ensure(N));
-    RET(g->inc_ptr.ensure(N + 1));
-    RET(g->inc.ensure(2 * E));
-    RET(g->part.ensure(4 * static_cast<size_t>(grid)));
-    if (g->flag.n == 0) {
-        CK(g->flag.alloc(1));
-        CK(cudaMemsetAsync(g->flag.p, 0, sizeof(int), g->ex->stream));
-    }
-    RET(g->report.ensure(1));
-    if (2 * E > g->ij_d.n || 8 * E > g->meas_d.n || 36 * E > g->info_d.n || E > g->rob_d.n) g->uploaded = 0;
-    RET(g->ij_d.ensure(2 * E));
-    RET(g->meas_d.ensure(8 * E));
-    RET(g->info_d.ensure(36 * E));
-    RET(g->rob_d.ensure(E));
-    RET(g->e_s.ensure(E));
-    RET(g->e_w.ensure(E));
-    RET(g->e_jj.ensure(36 * E));
-    RET(g->e_ii.ensure(36 * E));
-    RET(g->e_ad.ensure(36 * E));
-    RET(g->e_g.ensure(6 * E));
-    return KB_OK;
-}
-
-// the graph's current state on the device: poses, fixed flags, incidence lists (each node's edges ascending: the order
-// its blocks are summed in) and the edges added since the last upload; *P_out gets the graph's buffers, *pq_out the
-// poses as uploaded. g->uploaded is advanced by the caller once the stream has run.
-static int pg_upload(kb_pose_graph *g, std::vector<double> *pq_out, PoseGraphParams *P_out) {
-    const size_t N = g->n(), E = g->m();
-    std::vector<double> &pq = *pq_out;
-    pq.assign(8 * N, 0.0);
-    for (size_t k = 0; k < N; ++k) {
-        const SE3 &T = g->pose[k];
-        const double v[8] = {T.q.x, T.q.y, T.q.z, T.q.w, T.t.x, T.t.y, T.t.z, 0.0};
-        std::copy(v, v + 8, &pq[8 * k]);
-    }
-    std::vector<int> inc_ptr(N + 1, 0), inc(2 * E);
-    for (size_t e = 0; e < 2 * E; ++e) ++inc_ptr[static_cast<size_t>(g->ij[e]) + 1];
-    for (size_t k = 0; k < N; ++k) inc_ptr[k + 1] += inc_ptr[k];
-    {
-        std::vector<int> at(inc_ptr.begin(), inc_ptr.end() - 1);
-        for (size_t e = 0; e < E; ++e) {
-            inc[at[g->ij[2 * e]]++] = static_cast<int>(e);
-            inc[at[g->ij[2 * e + 1]]++] = static_cast<int>(e);
-        }
-    }
-    cudaStream_t s = g->ex->stream;
-    if (N) {
-        CK(cudaMemcpyAsync(g->pose_d.p, pq.data(), 8 * N * sizeof(double), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(g->fixed_d.p, g->fixed.data(), N * sizeof(int), cudaMemcpyHostToDevice, s));
-    }
-    CK(cudaMemcpyAsync(g->inc_ptr.p, inc_ptr.data(), (N + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (E) CK(cudaMemcpyAsync(g->inc.p, inc.data(), 2 * E * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (E > g->uploaded) {
-        const size_t a = g->uploaded, n = E - a;
-        CK(cudaMemcpyAsync(g->ij_d.p + 2 * a, &g->ij[2 * a], 2 * n * sizeof(int), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(g->meas_d.p + 8 * a, &g->meas_inv[8 * a], 8 * n * sizeof(double), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(g->info_d.p + 36 * a, &g->info[36 * a], 36 * n * sizeof(double), cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(g->rob_d.p + a, &g->robust[a], n * sizeof(double), cudaMemcpyHostToDevice, s));
-    }
-    PoseGraphParams &P = *P_out;
-    P = PoseGraphParams{};
-    P.bar = g->ex->sc.bar;
-    P.n_nodes = static_cast<int>(N);
-    P.n_edges = static_cast<int>(E);
-    P.pose = g->pose_d.p;
-    P.cand = g->cand.p;
-    P.fixed = g->fixed_d.p;
-    P.inc_ptr = g->inc_ptr.p;
-    P.inc = g->inc.p;
-    P.ij = g->ij_d.p;
-    P.meas_inv = g->meas_d.p;
-    P.info = g->info_d.p;
-    P.robust = g->rob_d.p;
-    P.e_s = g->e_s.p;
-    P.e_w = g->e_w.p;
-    P.e_jj = g->e_jj.p;
-    P.e_ii = g->e_ii.p;
-    P.e_ad = g->e_ad.p;
-    P.e_g = g->e_g.p;
-    P.hd = g->hd.p;
-    P.g = g->grad.p;
-    P.D = g->D.p;
-    P.U = g->U.p;
-    P.UL = g->UL.p;
-    const size_t V = 6 * std::max<size_t>(N, 1);
-    P.x = g->vec.p;
-    P.r = P.x + V;
-    P.z = P.r + V;
-    P.p = P.z + V;
-    P.q = P.p + V;
-    P.y = P.q + V;
-    P.part = g->part.p;
-    P.flag = g->flag.p;
-    P.report = g->report.p;
-    return KB_OK;
-}
-
-void kb_pose_graph_options_default(kb_pose_graph_options *o) {
-    if (o) *o = kb_pose_graph_options{100, 1e-12, 1e-10, 1e-4, 100, 1e-10};
-}
-int kb_pose_graph_create(kb_pose_graph **out) {
-    if (!out) return fail(KB_ERR_INVALID_ARG, "out == NULL");
-    auto g = std::make_unique<kb_pose_graph>();
-    g->device = tl_device;
-    g->user_stream = tl_user_stream;
-    *out = g.release();
-    return KB_OK;
-}
-int kb_pose_graph_destroy(kb_pose_graph *g) {
-    delete g;
-    return KB_OK;
-}
-int kb_pose_graph_add_node(kb_pose_graph *g, const double pose[16], int fixed, size_t *index) {
-    if (!g) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    SE3 T;
-    RET(pg_se3_arg(pose, "pose", &T));
-    if (g->n() >= kPoseGraphMaxNodes) return fail(KB_ERR_INVALID_ARG, "the graph holds 2^22 nodes");
-    g->mat.insert(g->mat.end(), pose, pose + 16);
-    g->pose.push_back(T);
-    g->fixed.push_back(fixed ? 1 : 0);
-    g->factored = false;
-    if (index) *index = g->n() - 1;
-    return KB_OK;
-}
-int kb_pose_graph_add_edge(kb_pose_graph *g, size_t i, size_t j, const double measurement[16], const double information[36],
-                           double robust_scale, size_t *index) {
-    if (!g || !information) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    SE3 Z;
-    RET(pg_se3_arg(measurement, "measurement", &Z));
-    if (i == j) return fail(KB_ERR_INVALID_ARG, "an edge joins two different nodes (i == j == %zu)", i);
-    if (i >= g->n() || j >= g->n()) return fail(KB_ERR_INVALID_ARG, "node %zu does not exist (%zu nodes)", std::max(i, j), g->n());
-    for (int k = 0; k < 36; ++k)
-        if (!std::isfinite(information[k])) return fail(KB_ERR_INVALID_ARG, "information is not finite");
-    for (int a = 0; a < 6; ++a)
-        for (int b = 0; b < a; ++b)
-            if (information[6 * a + b] != information[6 * b + a]) return fail(KB_ERR_INVALID_ARG, "information is not symmetric");
-    double L[36] = {};
-    for (int c = 0; c < 6; ++c) {  // Cholesky: positive definite
-        double d = information[7 * c];
-        for (int k = 0; k < c; ++k) d -= L[6 * c + k] * L[6 * c + k];
-        if (!(d > 0.0)) return fail(KB_ERR_INVALID_ARG, "information is not positive definite");
-        L[7 * c] = std::sqrt(d);
-        for (int r = c + 1; r < 6; ++r) {
-            double s = information[6 * r + c];
-            for (int k = 0; k < c; ++k) s -= L[6 * r + k] * L[6 * c + k];
-            L[6 * r + c] = s / L[7 * c];
-        }
-    }
-    if (!(robust_scale >= 0.0) || !std::isfinite(robust_scale)) return fail(KB_ERR_INVALID_ARG, "robust_scale must be finite and >= 0");
-    if (g->m() >= kPoseGraphMaxEdges) return fail(KB_ERR_INVALID_ARG, "the graph holds 2^24 edges");
-    const SE3 Zi = se3_inverse(Z);
-    const double zi[8] = {Zi.q.x, Zi.q.y, Zi.q.z, Zi.q.w, Zi.t.x, Zi.t.y, Zi.t.z, 0.0};
-    g->ij.push_back(static_cast<int>(i));
-    g->ij.push_back(static_cast<int>(j));
-    g->meas_inv.insert(g->meas_inv.end(), zi, zi + 8);
-    g->info.insert(g->info.end(), information, information + 36);
-    g->robust.push_back(robust_scale);
-    g->factored = false;
-    if (index) *index = g->m() - 1;
-    return KB_OK;
-}
-int kb_pose_graph_size(const kb_pose_graph *g, size_t *n_nodes, size_t *n_edges) {
-    if (!g || !n_nodes || !n_edges) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    *n_nodes = g->n();
-    *n_edges = g->m();
-    return KB_OK;
-}
-int kb_pose_graph_poses(const kb_pose_graph *g, double *poses, size_t cap, size_t *n_out) {
-    if (!g || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    *n_out = g->n();
-    if (!poses || cap == 0) return KB_OK;
-    if (cap < g->n()) return fail(KB_ERR_CAPACITY, "buffer too small (%zu < %zu poses)", cap, g->n());
-    std::copy(g->mat.begin(), g->mat.end(), poses);
-    return KB_OK;
-}
-int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_pose_graph_report *out, double *edge_chi2,
-                           double *edge_weight) {
-    if (!g || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    kb_pose_graph_options o;
-    kb_pose_graph_options_default(&o);
-    if (opt) o = *opt;
-    RET(pg_options_check(o));
-    RET(pg_gauge_check(*g));
-    RET(require_device());
-    if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
-    Exec &ex = *g->ex;
-    CK(cudaSetDevice(ex.device));
-    const size_t N = g->n(), E = g->m();
-    int co_resident = 0;
-    CK(pose_graph_max_grid(ex.sms, &co_resident));
-    const int cap = std::min(tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : ex.sms, co_resident);
-    const size_t items = std::max<size_t>(std::max(N, E), 1);
-    const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>((items + POSE_GRAPH_BLOCK - 1) / POSE_GRAPH_BLOCK, cap)));
-    RET(pg_reserve(g, grid));
-    std::vector<double> pq;
-    PoseGraphParams P;
-    RET(pg_upload(g, &pq, &P));
-    cudaStream_t s = ex.stream;
-    P.max_iterations = o.max_iterations;
-    P.max_cg_iterations = o.max_cg_iterations;
-    P.function_tolerance = o.function_tolerance;
-    P.parameter_tolerance = o.parameter_tolerance;
-    P.initial_lambda = o.initial_lambda;
-    P.cg_tolerance = o.cg_tolerance;
-    if (g->ev[1].device != ex.device) {  // (ev[1] is made last: both exist on that device)
-        CK(g->ev[0].create(cudaEventDefault));
-        CK(g->ev[1].create(cudaEventDefault));
-    }
-    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
-    ex.bar_dirty = true;
-    g->factored = false;  // (the poses move)
-    CK(cudaEventRecord(g->ev[0].p, s));
-    CK(pose_graph_launch(P, grid, s));
-    ++ex.launches;
-    CK(cudaEventRecord(g->ev[1].p, s));
-    kb_pose_graph_report rep{};
-    CK(cudaMemcpyAsync(&rep, g->report.p, sizeof(rep), cudaMemcpyDeviceToHost, s));
-    if (N) CK(cudaMemcpyAsync(pq.data(), g->pose_d.p, 8 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
-    std::vector<double> chi2(edge_chi2 ? E : 0), weight(edge_weight ? E : 0);
-    if (edge_chi2 && E) CK(cudaMemcpyAsync(chi2.data(), g->e_s.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
-    if (edge_weight && E) CK(cudaMemcpyAsync(weight.data(), g->e_w.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
-    RET(ex.sync());
-    g->uploaded = E;
-    for (size_t k = 0; k < N; ++k) {
-        if (g->fixed[k]) continue;
-        const double *v = &pq[8 * k];
-        g->pose[k] = SE3{{v[0], v[1], v[2], v[3]}, {v[4], v[5], v[6]}};
-        se3_to_matrix(g->pose[k], &g->mat[16 * k]);
-    }
-    *out = rep;
-    std::copy(chi2.begin(), chi2.end(), edge_chi2 ? edge_chi2 : chi2.data());
-    std::copy(weight.begin(), weight.end(), edge_weight ? edge_weight : weight.data());
-    return KB_OK;
-}
-
-int kb_debug_pose_graph_ms(const kb_pose_graph *g, float *ms) {
-    if (!g || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (!g->ev[1].p) return fail(KB_ERR_INVALID_ARG, "no optimize has run on this graph");
-    CK(cudaSetDevice(g->ex->device));
-    CK(cudaEventElapsedTime(ms, g->ev[0].p, g->ev[1].p));
-    return KB_OK;
-}
-int kb_debug_se3_adjoint(const double T[16], double A[36]) {
-    if (!A) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    SE3 X;
-    RET(pg_se3_arg(T, "T", &X));
-    se3_adjoint(X, A);
-    return KB_OK;
-}
-int kb_debug_se3_right_jacobian_inverse(const double x[6], double J[36]) {
-    if (!x || !J) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    se3_right_jacobian_inverse(x, J);
-    return KB_OK;
-}
-
-// ------------------------------------------------------------------------------- Pose graph: marginal covariances
-// The symbolic analysis (pgc_symbolic, host) is cached for (N, E): nodes and edges are only ever added. The numeric
-// factor is cached until the next add_node, add_edge or optimize, so marginals and joint marginals taken one after the
-// other factor once.
-static int pg_symbolic(kb_pose_graph *g) {
-    const int N = static_cast<int>(g->n()), E = static_cast<int>(g->m());
-    if (g->sym.n_nodes == N && g->sym.n_edges == E) return KB_OK;
-    g->factored = false;
-    pgc_symbolic(N, g->fixed.data(), E, g->ij.data(), &g->sym);
-    if (g->sym.uptr.size() == 1 && g->sym.uptr[0] < 0) {
-        g->sym.n_nodes = -1;  // (analysed again at the next call, and refused again)
-        return fail(KB_ERR_INVALID_ARG, "the factorization of this graph needs more than 2^30 block updates");
-    }
-    return KB_OK;
-}
-
-// the requested nodes exist, and every free node is tied to a fixed one (otherwise H is singular)
-static int pg_cov_check(const kb_pose_graph *g, const size_t *nodes, size_t n_idx) {
-    if (!nodes) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (n_idx > (size_t(1) << 30)) return fail(KB_ERR_INVALID_ARG, "more than 2^29 requests in one call");
-    for (size_t t = 0; t < n_idx; ++t)
-        if (nodes[t] >= g->n()) return fail(KB_ERR_INVALID_ARG, "node %zu does not exist (%zu nodes)", nodes[t], g->n());
-    return pg_gauge_check(*g);
-}
-
-static int pg_put(DBuf<int> &d, const std::vector<int> &h, cudaStream_t s) {
-    RET(d.ensure(std::max<size_t>(h.size(), 1)));
-    if (!h.empty()) CK(cudaMemcpyAsync(d.p, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-    return KB_OK;
-}
-
-// the numeric factor of H at the current poses (one cooperative launch), unless the cached one is still valid
-static int pg_factor(kb_pose_graph *g) {
-    RET(pg_symbolic(g));
-    if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
-    Exec &ex = *g->ex;
-    CK(cudaSetDevice(ex.device));
-    if (g->cev[3].device != ex.device) {  // (cev[3] is made last: all four exist on that device)
-        for (Event &e : g->cev) CK(e.create(cudaEventDefault));
-    }
-    const PgcSymbolic &S = g->sym;
-    if (g->factored || S.nf == 0) {
-        g->factored = true;
-        return KB_OK;
-    }
-    int co_resident = 0;
-    CK(pgc_factor_max_grid(ex.sms, &co_resident));
-    const int cap = std::min(tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : ex.sms, co_resident);
-    const size_t items = std::max({g->n(), g->m(), S.blocks(), size_t(1)});
-    const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>((items + PGC_BLOCK - 1) / PGC_BLOCK, cap)));
-    RET(pg_reserve(g, grid));
-    std::vector<double> pq;
-    PgcFactorParams F{};
-    RET(pg_upload(g, &pq, &F.P));
-    cudaStream_t s = ex.stream;
-    if (g->sym_dev_n != S.n_nodes || g->sym_dev_e != S.n_edges) {
-        RET(pg_put(g->s_order, S.order, s));
-        RET(pg_put(g->s_pos, S.pos, s));
-        RET(pg_put(g->s_parent, S.parent, s));
-        RET(pg_put(g->s_col_slot, S.col_slot, s));
-        RET(pg_put(g->s_lev_ptr, S.lev_ptr, s));
-        RET(pg_put(g->s_colptr, S.colptr, s));
-        RET(pg_put(g->s_brow, S.brow, s));
-        RET(pg_put(g->s_bcol, S.bcol, s));
-        RET(pg_put(g->s_hptr, S.hptr, s));
-        RET(pg_put(g->s_hedge, S.hedge, s));
-        RET(pg_put(g->s_uptr, S.uptr, s));
-        RET(pg_put(g->s_upd, S.upd, s));
-        g->sym_dev_n = S.n_nodes;
-        g->sym_dev_e = S.n_edges;
-    }
-    RET(g->Lx.ensure(36 * S.blocks()));
-    RET(g->cov_flag.ensure(1));
-    CK(cudaMemsetAsync(g->cov_flag.p, 0, sizeof(int), s));
-    F.nf = S.nf;
-    F.levels = S.levels();
-    F.n_blocks = static_cast<int>(S.blocks());
-    F.order = g->s_order.p;
-    F.lev_ptr = g->s_lev_ptr.p;
-    F.colptr = g->s_colptr.p;
-    F.brow = g->s_brow.p;
-    F.bcol = g->s_bcol.p;
-    F.hptr = g->s_hptr.p;
-    F.hedge = g->s_hedge.p;
-    F.uptr = g->s_uptr.p;
-    F.upd = g->s_upd.p;
-    F.Lx = g->Lx.p;
-    F.flag = g->cov_flag.p;
-    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
-    ex.bar_dirty = true;
-    CK(cudaEventRecord(g->cev[0].p, s));
-    CK(pgc_factor_launch(F, grid, s));
-    ++ex.launches;
-    CK(cudaEventRecord(g->cev[1].p, s));
-    int flag = 0;
-    CK(cudaMemcpyAsync(&flag, g->cov_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-    RET(ex.sync());
-    g->uploaded = g->m();
-    if (flag) return fail(KB_ERR_INVALID_ARG, "H is not positive definite at the current poses");
-    g->factored = true;
-    return KB_OK;
-}
-
-// req[2 n]: node pairs; out: n blocks of 36 (marginals) or 144 (joint) doubles
-static int pg_cov_solve(kb_pose_graph *g, const std::vector<int> &req, int joint, std::vector<double> *out) {
-    const PgcSymbolic &S = g->sym;
-    const size_t n = req.size() / 2, per = joint ? 144 : 36;
-    out->assign(n * per, 0.0);
-    if (S.nf == 0) return KB_OK;  // (every node is fixed)
-    Exec &ex = *g->ex;
-    cudaStream_t s = ex.stream;
-    const size_t H = static_cast<size_t>(S.levels());
-    const size_t group_bytes = 2 * H * (36 * sizeof(double) + sizeof(int));
-    // at most 4 CTAs per SM, and at most 1 GB of solve scratch
-    const int sm_cap = tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : 4 * ex.sms;
-    const size_t mem_cap = std::max<size_t>(1, (size_t(1) << 30) / (group_bytes * PGC_GROUPS));
-    const int grid = static_cast<int>(std::max<size_t>(1, std::min({(n + PGC_GROUPS - 1) / PGC_GROUPS, static_cast<size_t>(sm_cap), mem_cap})));
-    const size_t groups = static_cast<size_t>(grid) * PGC_GROUPS;
-    RET(g->cov_X.ensure(groups * 2 * H * 36));
-    RET(g->cov_path.ensure(groups * 2 * H));
-    RET(g->cov_req.ensure(2 * n));
-    RET(g->cov_out.ensure(n * per));
-    CK(cudaMemcpyAsync(g->cov_req.p, req.data(), 2 * n * sizeof(int), cudaMemcpyHostToDevice, s));
-    PgcMarginalParams M{};
-    M.Lx = g->Lx.p;
-    M.colptr = g->s_colptr.p;
-    M.brow = g->s_brow.p;
-    M.col_slot = g->s_col_slot.p;
-    M.parent = g->s_parent.p;
-    M.pos = g->s_pos.p;
-    M.req = g->cov_req.p;
-    M.n = static_cast<int>(n);
-    M.joint = joint;
-    M.max_path = static_cast<int>(H);
-    M.X = g->cov_X.p;
-    M.path = g->cov_path.p;
-    M.out = g->cov_out.p;
-    CK(cudaEventRecord(g->cev[2].p, s));
-    CK(pgc_marginals_launch(M, grid, s));
-    ++ex.launches;
-    CK(cudaEventRecord(g->cev[3].p, s));
-    CK(cudaMemcpyAsync(out->data(), g->cov_out.p, n * per * sizeof(double), cudaMemcpyDeviceToHost, s));
-    return ex.sync();
-}
-
-int kb_pose_graph_marginals(kb_pose_graph *g, const size_t *nodes, size_t n, double *cov) {
-    if (!g) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (n == 0) return KB_OK;
-    if (!cov) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    RET(pg_cov_check(g, nodes, n));
-    RET(require_device());
-    RET(pg_factor(g));
-    std::vector<int> req(2 * n);
-    for (size_t t = 0; t < n; ++t) req[2 * t] = req[2 * t + 1] = static_cast<int>(nodes[t]);
-    std::vector<double> out;
-    RET(pg_cov_solve(g, req, 0, &out));
-    std::copy(out.begin(), out.end(), cov);
-    return KB_OK;
-}
-int kb_pose_graph_joint_marginals(kb_pose_graph *g, const size_t *pairs, size_t n, double *cov) {
-    if (!g) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (n == 0) return KB_OK;
-    if (!cov) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (n > (size_t(1) << 29)) return fail(KB_ERR_INVALID_ARG, "more than 2^29 requests in one call");
-    RET(pg_cov_check(g, pairs, 2 * n));
-    RET(require_device());
-    RET(pg_factor(g));
-    std::vector<int> req(2 * n);
-    for (size_t t = 0; t < 2 * n; ++t) req[t] = static_cast<int>(pairs[t]);
-    std::vector<double> out;
-    RET(pg_cov_solve(g, req, 1, &out));
-    std::copy(out.begin(), out.end(), cov);
-    return KB_OK;
-}
-int kb_pose_graph_factor_info(kb_pose_graph *g, struct kb_pose_graph_factor_info *out) {
-    if (!g || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    RET(pg_symbolic(g));
-    const PgcSymbolic &S = g->sym;
-    struct kb_pose_graph_factor_info r {};
-    r.free_nodes = static_cast<size_t>(S.nf);
-    r.h_blocks = S.h_blocks;
-    r.l_blocks = S.blocks();
-    r.etree_height = S.nf ? static_cast<size_t>(S.levels()) : 0;
-    r.flops = S.flops;
-    *out = r;
-    return KB_OK;
-}
-int kb_debug_pose_graph_symbolic(kb_pose_graph *g, size_t cap, size_t *n_free, size_t *order, long long *parent,
-                                 size_t *col_blocks) {
-    if (!g || !n_free) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    RET(pg_symbolic(g));
-    const PgcSymbolic &S = g->sym;
-    const size_t nf = static_cast<size_t>(S.nf);
-    *n_free = nf;
-    if (!order && !parent && !col_blocks) return KB_OK;
-    if (cap < nf) return fail(KB_ERR_CAPACITY, "buffer too small (%zu < %zu free nodes)", cap, nf);
-    for (size_t p = 0; p < nf; ++p) {
-        if (order) order[p] = static_cast<size_t>(S.order[p]);
-        if (parent) parent[p] = S.parent[p];
-        if (col_blocks) col_blocks[p] = static_cast<size_t>(S.colptr[S.col_slot[p] + 1] - S.colptr[S.col_slot[p]]);
-    }
-    return KB_OK;
-}
-int kb_debug_pose_graph_cov_ms(const kb_pose_graph *g, float ms[2]) {
-    if (!g || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (!g->cev[3].p || !g->ex) return fail(KB_ERR_INVALID_ARG, "no marginals have been computed on this graph");
-    CK(cudaSetDevice(g->ex->device));
-    float f = 0.0f, m = 0.0f;
-    if (cudaEventQuery(g->cev[1].p) == cudaSuccess && cudaEventElapsedTime(&f, g->cev[0].p, g->cev[1].p) != cudaSuccess) {
-        cudaGetLastError();
-        f = 0.0f;  // (no factorization was launched: every node is fixed)
-    }
-    CK(cudaEventElapsedTime(&m, g->cev[2].p, g->cev[3].p));
-    ms[0] = f;
-    ms[1] = m;
     return KB_OK;
 }
 
@@ -3488,8 +2152,7 @@ int kb_debug_nn_reuse(const kb_map *map, const double *pf, const double *p, size
     RET(d_or.ensure(n));
     CK(cudaMemcpyAsync(d_pf.p, pf, 24 * n, cudaMemcpyHostToDevice, ex.stream));
     CK(cudaMemcpyAsync(d_p.p, p, 24 * n, cudaMemcpyHostToDevice, ex.stream));
-    const MapView mv = map->view();
-    CK(probe_nn_reuse(&mv, sizeof(mv), d_pf.p, d_p.p, static_cast<int>(n), path, ex.team.radius_frac, ex.team.smem_bytes,
+    CK(probe_nn_reuse(map->view(), d_pf.p, d_p.p, static_cast<int>(n), path, ex.team.radius_frac, ex.team.smem_bytes,
                       ex.icp_team_q, d_op.p, d_od.p, d_or.p, ex.stream));
     ++ex.launches;
     CK(cudaMemcpyAsync(out_points, d_op.p, 24 * n, cudaMemcpyDeviceToHost, ex.stream));
@@ -3547,13 +2210,6 @@ int kb_debug_reloc_score_ms(const kb_registration *reg, float *ms) {
     if (reg->rev[1].device < 0) return fail(KB_ERR_INVALID_ARG, "no kb_relocalize call on this handle yet");
     CK(cudaSetDevice(reg->rev[1].device));
     CK(cudaEventElapsedTime(ms, reg->rev[0].p, reg->rev[1].p));
-    return KB_OK;
-}
-int kb_debug_place_distance_ms(const kb_place_db *db, float *ms) {
-    if (!db || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (db->ev[1].device < 0) return fail(KB_ERR_INVALID_ARG, "no query on this database yet");
-    CK(cudaSetDevice(db->ev[1].device));
-    CK(cudaEventElapsedTime(ms, db->ev[0].p, db->ev[1].p));
     return KB_OK;
 }
 int kb_debug_barrier_ns(int iters, double *ns_per_barrier) {
@@ -3614,7 +2270,6 @@ int kb_pipeline_last_profile(const kb_pipeline *p, double *us, int n) {
     for (int i = 0; i < n && i < 6; ++i) us[i] = (static_cast<double>(p->last.t_ns[i + 1]) - static_cast<double>(p->last.t_ns[i])) * 1e-3;
     return KB_OK;
 }
-int kb_any_device_stuck(void) { return device_is_stuck(-1) ? 1 : 0; }
 int kb_pipeline_set_profiling(kb_pipeline *p, int enabled) {
     if (!p) return fail(KB_ERR_INVALID_ARG, "p == NULL");
     p->ex->sc.profile = enabled;  // 1: all stamps (incl. one per ICP iteration, ~1 us each); 2: phase boundaries only
@@ -3651,142 +2306,45 @@ int kb_pipeline_launch_count(const kb_pipeline *p, unsigned long long *out) {
     return KB_OK;
 }
 
-// ------------------------------------------------------------------------------- free space
-namespace {
-thread_local double tl_fs_bin_size = 0.0;  // kb_debug_free_space_bin_size (0: the default)
-thread_local float tl_fs_ms[3];
-thread_local bool tl_fs_timed = false;
-}  // namespace
-void kb_free_space_params_default(kb_free_space_params *p, double voxel_size) {
-    if (!p) return;
-    // measured on the KITTI-shape run with moving boxes (DESIGN.md §4.13)
-    p->pass_radius = 0.1 * voxel_size;
-    p->end_margin = 2.0 * voxel_size;
-    p->min_incidence = std::asin(std::min(1.0, 2.0 * p->pass_radius / p->end_margin));
-    p->min_planarity = 0.3;
-    p->min_passes = 20;
-    p->ratio = 0.1;
-}
-static int free_space_params_check(const kb_free_space_params *p) {
-    if (!p) return fail(KB_ERR_INVALID_ARG, "NULL params");
-    if (!std::isfinite(p->pass_radius) || !(p->pass_radius > 0.0)) return fail(KB_ERR_INVALID_ARG, "pass_radius must be finite and > 0");
-    if (!std::isfinite(p->end_margin) || !(p->end_margin >= 0.0)) return fail(KB_ERR_INVALID_ARG, "end_margin must be finite and >= 0");
-    if (!(p->min_incidence >= 0.0 && p->min_incidence <= kPi / 2))
-        return fail(KB_ERR_INVALID_ARG, "min_incidence must be in [0, pi/2]");
-    if (!(p->min_planarity >= 0.0 && p->min_planarity <= 1.0)) return fail(KB_ERR_INVALID_ARG, "min_planarity must be in [0, 1]");
-    if (p->min_passes == 0) return fail(KB_ERR_INVALID_ARG, "min_passes must be >= 1");
-    if (!std::isfinite(p->ratio) || !(p->ratio >= 0.0)) return fail(KB_ERR_INVALID_ARG, "ratio must be finite and >= 0");
-    return KB_OK;
-}
-int kb_map_free_space(const kb_map *cmap, const double *xyz, size_t n_points, const size_t *offset, size_t n_scans,
-                      const double *poses, const kb_free_space_params *p, unsigned *passes, unsigned *hits, kb_map *out,
-                      kb_free_space_report *report) {
-    kb_map *map = const_cast<kb_map *>(cmap);
-    RET(free_space_params_check(p));
-    if (n_points >= (size_t(1) << 32)) return fail(KB_ERR_INVALID_ARG, "%zu rays: at most 2^32 - 1", n_points);
-    if (n_points && !xyz) return fail(KB_ERR_INVALID_ARG, "NULL xyz");
-    if (n_scans && (!offset || !poses)) return fail(KB_ERR_INVALID_ARG, "NULL offset or poses");
-    if (!n_scans && n_points) return fail(KB_ERR_INVALID_ARG, "%zu points but no scan", n_points);
-    if (n_scans) {
-        if (offset[0] != 0 || offset[n_scans] != n_points)
-            return fail(KB_ERR_INVALID_ARG, "offset must start at 0 and end at n_points (%zu)", n_points);
-        for (size_t s = 0; s < n_scans; ++s)
-            if (offset[s + 1] < offset[s]) return fail(KB_ERR_INVALID_ARG, "offset decreases at scan %zu", s);
-    }
-    std::vector<double> se3(7 * n_scans);
-    for (size_t s = 0; s < n_scans; ++s) {
-        SE3 T;
-        if (!se3_from_matrix(poses + 16 * s, &T) || !std::isfinite(T.t.x) || !std::isfinite(T.t.y) || !std::isfinite(T.t.z))
-            return fail(KB_ERR_NOT_SE3, "pose %zu is not in SE(3)", s);
-        const double q[7] = {T.q.x, T.q.y, T.q.z, T.q.w, T.t.x, T.t.y, T.t.z};
-        std::memcpy(&se3[7 * s], q, sizeof(q));
-        // every endpoint's voxel coordinate must fit in an int: |e_c| <= |p| (1 + 1e-6) + |t|
-        double pmax = 0.0;
-        for (size_t i = offset[s]; i < offset[s + 1]; ++i) {
-            const double r = std::sqrt(xyz[3 * i] * xyz[3 * i] + xyz[3 * i + 1] * xyz[3 * i + 1] + xyz[3 * i + 2] * xyz[3 * i + 2]);
-            if (!std::isfinite(r)) return fail(KB_ERR_INVALID_ARG, "point %zu is not finite", i);
-            pmax = std::max(pmax, r);
+}  // extern "C"
+
+bool kb_host::voxel_reach(const double *xyz, size_t n, double tmax, double voxel_size, double *reach, size_t *bad) {
+    double pmax = 0.0;
+    for (size_t i = 0; i < n; ++i) {
+        const double r = std::sqrt(xyz[3 * i] * xyz[3 * i] + xyz[3 * i + 1] * xyz[3 * i + 1] + xyz[3 * i + 2] * xyz[3 * i + 2]);
+        if (!std::isfinite(r)) {
+            *bad = i;
+            return false;
         }
-        const double tmax = std::max({std::fabs(T.t.x), std::fabs(T.t.y), std::fabs(T.t.z)});
-        if (map && !((pmax * (1.0 + 1e-6) + tmax) / map->voxel_size + 1.0 < 2147483000.0))
-            return fail(KB_ERR_INVALID_ARG, "scan %zu reaches voxel coordinates beyond the int range", s);
+        pmax = std::max(pmax, r);
     }
-    RET(require_device());
-    if (!map) return fail(KB_ERR_INVALID_ARG, "NULL map");
-    if (out) {
-        if (out == map) return fail(KB_ERR_INVALID_ARG, "out must be another map than the input");
-        if (out->voxel_size != map->voxel_size || out->cap != map->cap)
-            return fail(KB_ERR_INVALID_ARG, "out must have the input's voxel_size and max_points_per_voxel");
-        if (out->ex->device != map->ex->device) return fail(KB_ERR_INVALID_ARG, "out must be on the input's device");
-        RET(map_in_use(out));
-    }
-    Exec &ex = *map->ex;
-    CK(cudaSetDevice(ex.device));
-    size_t nv = 0, np = 0;
-    RET(kb_map_dump(map, nullptr, nullptr, nullptr, 0, 0, &nv, &np));
-    std::vector<int> vox(3 * nv), cnt(nv);
-    std::vector<double> pts(3 * np);
-    if (nv) RET(kb_map_dump(map, vox.data(), cnt.data(), pts.data(), nv, np, &nv, &np));
-    std::vector<unsigned> h_passes(np), h_hits(nv);
-    const MapView mv = map->view();
-    FsInput in;
-    in.map_view = &mv;
-    in.view_bytes = sizeof(mv);
-    in.voxels = vox.data();
-    in.counts = cnt.data();
-    in.points = pts.data();
-    in.n_voxels = nv;
-    in.n_points = np;
-    in.xyz = xyz;
-    in.offset = offset;
-    in.n_scans = n_scans;
-    in.poses = se3.data();
-    in.pose_bytes = sizeof(SE3);
-    in.rule = FsRule{p->pass_radius, p->end_margin, std::sin(p->min_incidence), p->min_planarity, p->min_passes, p->ratio};
-    in.bin_size = tl_fs_bin_size > 0.0 ? tl_fs_bin_size : fs_default_bin_size();
-    in.max_ctas = tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : ex.sms;
-    in.want_kept = out != nullptr;
-    FsOutput res{};
-    res.passes = h_passes.data();
-    res.hits = h_hits.data();
-    StallTrace trace("free space");
-    const cudaError_t e = fs_run(in, &res, ex.stream);
-    ex.launches += 4 + 2 * n_scans;
-    if (e != cudaSuccess) {
-        fs_release(&res);
-        return fail(KB_ERR_CUDA, "free-space counting failed: %s", cudaGetErrorString(e));
-    }
-    if (out) {
-        const int st = out->load(res.kept_vox, res.kept_cnt, res.kept_off, res.kept_pts, res.kept_voxels, res.kept_points);
-        fs_release(&res);
-        RET(st);
-    }
-    std::memcpy(tl_fs_ms, res.ms, sizeof(tl_fs_ms));
-    tl_fs_timed = true;
-    if (passes && np) std::memcpy(passes, h_passes.data(), np * sizeof(unsigned));
-    if (hits && nv) std::memcpy(hits, h_hits.data(), nv * sizeof(unsigned));
-    if (report) {
-        report->rays = n_points;
-        report->scans = n_scans;
-        report->points = np;
-        report->voxels = nv;
-        report->points_removed = res.points_removed;
-        report->voxels_removed = res.voxels_removed;
-        report->ray_point_tests = res.tests;
-    }
-    return KB_OK;
-}
-int kb_debug_free_space_bin_size(double radians) {
-    if (radians != 0.0 && !(radians >= 0.002 && radians <= kPi))
-        return fail(KB_ERR_INVALID_ARG, "bin size must be 0 or within [0.002, pi]");
-    tl_fs_bin_size = radians;
-    return KB_OK;
-}
-int kb_debug_free_space_ms(float ms[3]) {
-    if (!ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (!tl_fs_timed) return fail(KB_ERR_INVALID_ARG, "no kb_map_free_space call on this thread yet");
-    std::memcpy(ms, tl_fs_ms, sizeof(tl_fs_ms));
-    return KB_OK;
+    *reach = (pmax * (1.0 + 1e-6) + tmax) / voxel_size + 1.0;
+    return true;
 }
 
-}  // extern "C"
+int kb_host::refine_candidates(kb_registration *reg, kb_map *map, const double *xyz, size_t n,
+                               const std::vector<SE3> &guesses, double max_dist, double kscale, double max_xy, double max_angle, std::vector<double> *refined,
+                      std::vector<int> *iterations, std::vector<int> *inliers, size_t *winner, long long *runner_up) {
+    Exec &ex = *map->ex;
+    CK(cudaSetDevice(ex.device));
+    const size_t K = guesses.size();
+    if (xyz) {
+        RET(reg->ws.src.ensure(3 * n));
+        CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
+    }
+    const std::vector<size_t> off(K, 0), cnt(K, n);
+    const std::vector<double> md(K, max_dist), ks(K, kscale);
+    RET(reg->bpose.ensure(16 * K));
+    RET(reg->biout.ensure(2 * K));
+    RET(align_batch_run(reg, map, reg->ws.src.p, off.data(), cnt.data(), K, guesses, md.data(), ks.data(), reg->bpose.p,
+                        reg->biout.p, reg->biout.p + K));
+    refined->resize(16 * K);
+    std::vector<int> io(2 * K);  // iterations [K], inliers [K]
+    CK(cudaMemcpyAsync(refined->data(), reg->bpose.p, 16 * K * sizeof(double), cudaMemcpyDeviceToHost, ex.stream));
+    CK(cudaMemcpyAsync(io.data(), reg->biout.p, 2 * K * sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
+    RET(ex.sync());
+    iterations->assign(io.begin(), io.begin() + K);
+    inliers->assign(io.begin() + K, io.end());
+    reloc_winner(refined->data(), inliers->data(), K, max_xy, max_angle, winner, runner_up);
+    return KB_OK;
+}

@@ -1,0 +1,572 @@
+// Host side of the pose graph and its marginal covariances (kb_pose_graph_* and their kb_debug_* calls). The kernels
+// are in pose_graph.cu and pose_graph_cov.cu.
+#include <algorithm>
+#include <cmath>
+#include <memory>
+#include <numeric>
+#include <vector>
+
+#include "../../include/kiss_icp_b200.h"
+#include "../../include/kiss_icp_b200_debug.h"
+#include "host.cuh"
+#include "pose_graph.cuh"
+#include "pose_graph_cov.cuh"
+#include "se3.cuh"
+
+using namespace kb;
+using namespace kb_host;
+
+extern "C" {
+
+// The graph lives on the host (kb_pose_graph_* in the header state the problem and the method; pose_graph.cu has the
+// kernel). Edges are immutable, so an optimize uploads only those added since the last one; the poses, the fixed flags
+// and the incidence lists are uploaded every time.
+struct kb_pose_graph {
+    int device = 0;                  // of the creating thread: where the buffers go at the first optimize
+    cudaStream_t user_stream = nullptr;
+    std::vector<double> mat;         // [N][16] the poses as given or as last optimized (fixed nodes: as given, bit for bit)
+    std::vector<SE3> pose;           // [N] the same poses as the optimizer carries them
+    std::vector<int> fixed;          // [N]
+    std::vector<int> ij;             // [E][2]
+    std::vector<double> meas_inv;    // [E][8] Z^-1
+    std::vector<double> info;        // [E][36]
+    std::vector<double> robust;      // [E]
+    std::shared_ptr<Exec> ex;
+    size_t uploaded = 0;             // edges on the device
+    DBuf<double> pose_d, cand, hd, grad, D, U, UL, vec, part;
+    DBuf<double> meas_d, info_d, rob_d, e_s, e_w, e_jj, e_ii, e_ad, e_g;
+    DBuf<int> fixed_d, inc_ptr, inc, ij_d, flag;
+    DBuf<kb_pose_graph_report> report;
+    Event ev[2];                     // around the last launch (kb_debug_pose_graph_ms)
+    // the covariance (kb_pose_graph_marginals & co.): the symbolic analysis for (N, E), its copy on the device, the
+    // numeric factor at the current poses (valid until the next add_node, add_edge or optimize) and the solves
+    PgcSymbolic sym;
+    int sym_dev_n = -1, sym_dev_e = -1;  // the graph the device copy of `sym` was made for
+    bool factored = false;
+    DBuf<int> s_order, s_pos, s_parent, s_col_slot, s_lev_ptr, s_colptr, s_brow, s_bcol, s_hptr, s_hedge, s_uptr, s_upd;
+    DBuf<int> cov_flag, cov_req, cov_path;
+    DBuf<double> Lx, cov_X, cov_out;
+    Event cev[4];                    // around the last factorization and the last marginal solves (kb_debug_pose_graph_cov_ms)
+    size_t n() const { return fixed.size(); }
+    size_t m() const { return robust.size(); }
+};
+
+static constexpr size_t kPoseGraphMaxNodes = size_t(1) << 22, kPoseGraphMaxEdges = size_t(1) << 24;
+
+static int pg_se3_arg(const double M[16], const char *what, SE3 *out) {
+    if (!M) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    for (int k = 0; k < 16; ++k)
+        if (!std::isfinite(M[k])) return fail(KB_ERR_NOT_SE3, "%s is not finite", what);
+    if (!se3_from_matrix(M, out)) return fail(KB_ERR_NOT_SE3, "%s is not in SE(3)", what);
+    return KB_OK;
+}
+
+static int pg_options_check(const kb_pose_graph_options &o) {
+    if (o.max_iterations < 0 || o.max_iterations > 1000000) return fail(KB_ERR_INVALID_ARG, "max_iterations must be in [0, 10^6]");
+    if (!(o.function_tolerance >= 0.0) || !std::isfinite(o.function_tolerance))
+        return fail(KB_ERR_INVALID_ARG, "function_tolerance must be finite and >= 0");
+    if (!(o.parameter_tolerance >= 0.0) || !std::isfinite(o.parameter_tolerance))
+        return fail(KB_ERR_INVALID_ARG, "parameter_tolerance must be finite and >= 0");
+    if (!(o.initial_lambda > 0.0 && o.initial_lambda <= 1e12)) return fail(KB_ERR_INVALID_ARG, "initial_lambda must be in (0, 1e12]");
+    if (o.max_cg_iterations < 1 || o.max_cg_iterations > 1000000) return fail(KB_ERR_INVALID_ARG, "max_cg_iterations must be in [1, 10^6]");
+    if (!(o.cg_tolerance >= 0.0 && o.cg_tolerance < 1.0)) return fail(KB_ERR_INVALID_ARG, "cg_tolerance must be in [0, 1)");
+    return KB_OK;
+}
+
+// every free node reaches a fixed node through edges (the gauge): union-find over the edges
+static int pg_gauge_check(const kb_pose_graph &g) {
+    const size_t N = g.n();
+    std::vector<size_t> parent(N);
+    std::iota(parent.begin(), parent.end(), size_t(0));
+    auto root = [&](size_t a) {
+        while (parent[a] != a) a = parent[a] = parent[parent[a]];
+        return a;
+    };
+    for (size_t e = 0; e < g.m(); ++e) {
+        const size_t a = root(static_cast<size_t>(g.ij[2 * e])), b = root(static_cast<size_t>(g.ij[2 * e + 1]));
+        if (a != b) parent[std::max(a, b)] = std::min(a, b);
+    }
+    std::vector<char> grounded(N, 0);
+    for (size_t k = 0; k < N; ++k)
+        if (g.fixed[k]) grounded[root(k)] = 1;
+    for (size_t k = 0; k < N; ++k)
+        if (!grounded[root(k)])
+            return fail(KB_ERR_INVALID_ARG, "node %zu is free and no path of edges connects it to a fixed node (the gauge is free)", k);
+    return KB_OK;
+}
+
+// device buffers for the graph as it is now; edge buffers that had to grow are uploaded again from edge 0
+static int pg_reserve(kb_pose_graph *g, int grid) {
+    const size_t N = std::max<size_t>(g->n(), 1), E = std::max<size_t>(g->m(), 1);
+    RET(g->pose_d.ensure(8 * N));
+    RET(g->cand.ensure(8 * N));
+    RET(g->hd.ensure(36 * N));
+    RET(g->D.ensure(36 * N));
+    RET(g->U.ensure(36 * N));
+    RET(g->UL.ensure(36 * N));
+    RET(g->grad.ensure(6 * N));
+    RET(g->vec.ensure(6 * 6 * N));
+    RET(g->fixed_d.ensure(N));
+    RET(g->inc_ptr.ensure(N + 1));
+    RET(g->inc.ensure(2 * E));
+    RET(g->part.ensure(4 * static_cast<size_t>(grid)));
+    if (g->flag.n == 0) {
+        CK(g->flag.alloc(1));
+        CK(cudaMemsetAsync(g->flag.p, 0, sizeof(int), g->ex->stream));
+    }
+    RET(g->report.ensure(1));
+    if (2 * E > g->ij_d.n || 8 * E > g->meas_d.n || 36 * E > g->info_d.n || E > g->rob_d.n) g->uploaded = 0;
+    RET(g->ij_d.ensure(2 * E));
+    RET(g->meas_d.ensure(8 * E));
+    RET(g->info_d.ensure(36 * E));
+    RET(g->rob_d.ensure(E));
+    RET(g->e_s.ensure(E));
+    RET(g->e_w.ensure(E));
+    RET(g->e_jj.ensure(36 * E));
+    RET(g->e_ii.ensure(36 * E));
+    RET(g->e_ad.ensure(36 * E));
+    RET(g->e_g.ensure(6 * E));
+    return KB_OK;
+}
+
+// the graph's current state on the device: poses, fixed flags, incidence lists (each node's edges ascending: the order
+// its blocks are summed in) and the edges added since the last upload; *P_out gets the graph's buffers, *pq_out the
+// poses as uploaded. g->uploaded is advanced by the caller once the stream has run.
+static int pg_upload(kb_pose_graph *g, std::vector<double> *pq_out, PoseGraphParams *P_out) {
+    const size_t N = g->n(), E = g->m();
+    std::vector<double> &pq = *pq_out;
+    pq.assign(8 * N, 0.0);
+    for (size_t k = 0; k < N; ++k) {
+        const SE3 &T = g->pose[k];
+        const double v[8] = {T.q.x, T.q.y, T.q.z, T.q.w, T.t.x, T.t.y, T.t.z, 0.0};
+        std::copy(v, v + 8, &pq[8 * k]);
+    }
+    std::vector<int> inc_ptr(N + 1, 0), inc(2 * E);
+    for (size_t e = 0; e < 2 * E; ++e) ++inc_ptr[static_cast<size_t>(g->ij[e]) + 1];
+    for (size_t k = 0; k < N; ++k) inc_ptr[k + 1] += inc_ptr[k];
+    {
+        std::vector<int> at(inc_ptr.begin(), inc_ptr.end() - 1);
+        for (size_t e = 0; e < E; ++e) {
+            inc[at[g->ij[2 * e]]++] = static_cast<int>(e);
+            inc[at[g->ij[2 * e + 1]]++] = static_cast<int>(e);
+        }
+    }
+    cudaStream_t s = g->ex->stream;
+    if (N) {
+        CK(cudaMemcpyAsync(g->pose_d.p, pq.data(), 8 * N * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->fixed_d.p, g->fixed.data(), N * sizeof(int), cudaMemcpyHostToDevice, s));
+    }
+    CK(cudaMemcpyAsync(g->inc_ptr.p, inc_ptr.data(), (N + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (E) CK(cudaMemcpyAsync(g->inc.p, inc.data(), 2 * E * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (E > g->uploaded) {
+        const size_t a = g->uploaded, n = E - a;
+        CK(cudaMemcpyAsync(g->ij_d.p + 2 * a, &g->ij[2 * a], 2 * n * sizeof(int), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->meas_d.p + 8 * a, &g->meas_inv[8 * a], 8 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->info_d.p + 36 * a, &g->info[36 * a], 36 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->rob_d.p + a, &g->robust[a], n * sizeof(double), cudaMemcpyHostToDevice, s));
+    }
+    PoseGraphParams &P = *P_out;
+    P = PoseGraphParams{};
+    P.bar = g->ex->sc.bar;
+    P.n_nodes = static_cast<int>(N);
+    P.n_edges = static_cast<int>(E);
+    P.pose = g->pose_d.p;
+    P.cand = g->cand.p;
+    P.fixed = g->fixed_d.p;
+    P.inc_ptr = g->inc_ptr.p;
+    P.inc = g->inc.p;
+    P.ij = g->ij_d.p;
+    P.meas_inv = g->meas_d.p;
+    P.info = g->info_d.p;
+    P.robust = g->rob_d.p;
+    P.e_s = g->e_s.p;
+    P.e_w = g->e_w.p;
+    P.e_jj = g->e_jj.p;
+    P.e_ii = g->e_ii.p;
+    P.e_ad = g->e_ad.p;
+    P.e_g = g->e_g.p;
+    P.hd = g->hd.p;
+    P.g = g->grad.p;
+    P.D = g->D.p;
+    P.U = g->U.p;
+    P.UL = g->UL.p;
+    const size_t V = 6 * std::max<size_t>(N, 1);
+    P.x = g->vec.p;
+    P.r = P.x + V;
+    P.z = P.r + V;
+    P.p = P.z + V;
+    P.q = P.p + V;
+    P.y = P.q + V;
+    P.part = g->part.p;
+    P.flag = g->flag.p;
+    P.report = g->report.p;
+    return KB_OK;
+}
+
+void kb_pose_graph_options_default(kb_pose_graph_options *o) {
+    if (o) *o = kb_pose_graph_options{100, 1e-12, 1e-10, 1e-4, 100, 1e-10};
+}
+int kb_pose_graph_create(kb_pose_graph **out) {
+    if (!out) return fail(KB_ERR_INVALID_ARG, "out == NULL");
+    auto g = std::make_unique<kb_pose_graph>();
+    g->device = tl_device;
+    g->user_stream = tl_user_stream;
+    *out = g.release();
+    return KB_OK;
+}
+int kb_pose_graph_destroy(kb_pose_graph *g) {
+    delete g;
+    return KB_OK;
+}
+int kb_pose_graph_add_node(kb_pose_graph *g, const double pose[16], int fixed, size_t *index) {
+    if (!g) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    SE3 T;
+    RET(pg_se3_arg(pose, "pose", &T));
+    if (g->n() >= kPoseGraphMaxNodes) return fail(KB_ERR_INVALID_ARG, "the graph holds 2^22 nodes");
+    g->mat.insert(g->mat.end(), pose, pose + 16);
+    g->pose.push_back(T);
+    g->fixed.push_back(fixed ? 1 : 0);
+    g->factored = false;
+    if (index) *index = g->n() - 1;
+    return KB_OK;
+}
+int kb_pose_graph_add_edge(kb_pose_graph *g, size_t i, size_t j, const double measurement[16], const double information[36],
+                           double robust_scale, size_t *index) {
+    if (!g || !information) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    SE3 Z;
+    RET(pg_se3_arg(measurement, "measurement", &Z));
+    if (i == j) return fail(KB_ERR_INVALID_ARG, "an edge joins two different nodes (i == j == %zu)", i);
+    if (i >= g->n() || j >= g->n()) return fail(KB_ERR_INVALID_ARG, "node %zu does not exist (%zu nodes)", std::max(i, j), g->n());
+    for (int k = 0; k < 36; ++k)
+        if (!std::isfinite(information[k])) return fail(KB_ERR_INVALID_ARG, "information is not finite");
+    for (int a = 0; a < 6; ++a)
+        for (int b = 0; b < a; ++b)
+            if (information[6 * a + b] != information[6 * b + a]) return fail(KB_ERR_INVALID_ARG, "information is not symmetric");
+    double L[36] = {};
+    for (int c = 0; c < 6; ++c) {  // Cholesky: positive definite
+        double d = information[7 * c];
+        for (int k = 0; k < c; ++k) d -= L[6 * c + k] * L[6 * c + k];
+        if (!(d > 0.0)) return fail(KB_ERR_INVALID_ARG, "information is not positive definite");
+        L[7 * c] = std::sqrt(d);
+        for (int r = c + 1; r < 6; ++r) {
+            double s = information[6 * r + c];
+            for (int k = 0; k < c; ++k) s -= L[6 * r + k] * L[6 * c + k];
+            L[6 * r + c] = s / L[7 * c];
+        }
+    }
+    if (!(robust_scale >= 0.0) || !std::isfinite(robust_scale)) return fail(KB_ERR_INVALID_ARG, "robust_scale must be finite and >= 0");
+    if (g->m() >= kPoseGraphMaxEdges) return fail(KB_ERR_INVALID_ARG, "the graph holds 2^24 edges");
+    const SE3 Zi = se3_inverse(Z);
+    const double zi[8] = {Zi.q.x, Zi.q.y, Zi.q.z, Zi.q.w, Zi.t.x, Zi.t.y, Zi.t.z, 0.0};
+    g->ij.push_back(static_cast<int>(i));
+    g->ij.push_back(static_cast<int>(j));
+    g->meas_inv.insert(g->meas_inv.end(), zi, zi + 8);
+    g->info.insert(g->info.end(), information, information + 36);
+    g->robust.push_back(robust_scale);
+    g->factored = false;
+    if (index) *index = g->m() - 1;
+    return KB_OK;
+}
+int kb_pose_graph_size(const kb_pose_graph *g, size_t *n_nodes, size_t *n_edges) {
+    if (!g || !n_nodes || !n_edges) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *n_nodes = g->n();
+    *n_edges = g->m();
+    return KB_OK;
+}
+int kb_pose_graph_poses(const kb_pose_graph *g, double *poses, size_t cap, size_t *n_out) {
+    if (!g || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *n_out = g->n();
+    if (!poses || cap == 0) return KB_OK;
+    if (cap < g->n()) return fail(KB_ERR_CAPACITY, "buffer too small (%zu < %zu poses)", cap, g->n());
+    std::copy(g->mat.begin(), g->mat.end(), poses);
+    return KB_OK;
+}
+int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_pose_graph_report *out, double *edge_chi2,
+                           double *edge_weight) {
+    if (!g || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    kb_pose_graph_options o;
+    kb_pose_graph_options_default(&o);
+    if (opt) o = *opt;
+    RET(pg_options_check(o));
+    RET(pg_gauge_check(*g));
+    RET(require_device());
+    if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
+    Exec &ex = *g->ex;
+    CK(cudaSetDevice(ex.device));
+    const size_t N = g->n(), E = g->m();
+    int co_resident = 0;
+    CK(pose_graph_max_grid(ex.sms, &co_resident));
+    const int cap = std::min(tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : ex.sms, co_resident);
+    const size_t items = std::max<size_t>(std::max(N, E), 1);
+    const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>((items + POSE_GRAPH_BLOCK - 1) / POSE_GRAPH_BLOCK, cap)));
+    RET(pg_reserve(g, grid));
+    std::vector<double> pq;
+    PoseGraphParams P;
+    RET(pg_upload(g, &pq, &P));
+    cudaStream_t s = ex.stream;
+    P.max_iterations = o.max_iterations;
+    P.max_cg_iterations = o.max_cg_iterations;
+    P.function_tolerance = o.function_tolerance;
+    P.parameter_tolerance = o.parameter_tolerance;
+    P.initial_lambda = o.initial_lambda;
+    P.cg_tolerance = o.cg_tolerance;
+    RET(events_on(g->ev, ex.device));
+    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
+    ex.bar_dirty = true;
+    g->factored = false;  // (the poses move)
+    CK(cudaEventRecord(g->ev[0].p, s));
+    CK(pose_graph_launch(P, grid, s));
+    ++ex.launches;
+    CK(cudaEventRecord(g->ev[1].p, s));
+    kb_pose_graph_report rep{};
+    CK(cudaMemcpyAsync(&rep, g->report.p, sizeof(rep), cudaMemcpyDeviceToHost, s));
+    if (N) CK(cudaMemcpyAsync(pq.data(), g->pose_d.p, 8 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
+    std::vector<double> chi2(edge_chi2 ? E : 0), weight(edge_weight ? E : 0);
+    if (edge_chi2 && E) CK(cudaMemcpyAsync(chi2.data(), g->e_s.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (edge_weight && E) CK(cudaMemcpyAsync(weight.data(), g->e_w.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
+    RET(ex.sync());
+    g->uploaded = E;
+    for (size_t k = 0; k < N; ++k) {
+        if (g->fixed[k]) continue;
+        const double *v = &pq[8 * k];
+        g->pose[k] = SE3{{v[0], v[1], v[2], v[3]}, {v[4], v[5], v[6]}};
+        se3_to_matrix(g->pose[k], &g->mat[16 * k]);
+    }
+    *out = rep;
+    std::copy(chi2.begin(), chi2.end(), edge_chi2 ? edge_chi2 : chi2.data());
+    std::copy(weight.begin(), weight.end(), edge_weight ? edge_weight : weight.data());
+    return KB_OK;
+}
+
+int kb_debug_pose_graph_ms(const kb_pose_graph *g, float *ms) {
+    if (!g || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (!g->ev[1].p) return fail(KB_ERR_INVALID_ARG, "no optimize has run on this graph");
+    CK(cudaSetDevice(g->ex->device));
+    CK(cudaEventElapsedTime(ms, g->ev[0].p, g->ev[1].p));
+    return KB_OK;
+}
+int kb_debug_se3_adjoint(const double T[16], double A[36]) {
+    if (!A) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    SE3 X;
+    RET(pg_se3_arg(T, "T", &X));
+    se3_adjoint(X, A);
+    return KB_OK;
+}
+int kb_debug_se3_right_jacobian_inverse(const double x[6], double J[36]) {
+    if (!x || !J) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    se3_right_jacobian_inverse(x, J);
+    return KB_OK;
+}
+
+// ------------------------------------------------------------------------------- Pose graph: marginal covariances
+// The symbolic analysis (pgc_symbolic, host) is cached for (N, E): nodes and edges are only ever added. The numeric
+// factor is cached until the next add_node, add_edge or optimize, so marginals and joint marginals taken one after the
+// other factor once.
+static int pg_symbolic(kb_pose_graph *g) {
+    const int N = static_cast<int>(g->n()), E = static_cast<int>(g->m());
+    if (g->sym.n_nodes == N && g->sym.n_edges == E) return KB_OK;
+    g->factored = false;
+    pgc_symbolic(N, g->fixed.data(), E, g->ij.data(), &g->sym);
+    if (g->sym.uptr.size() == 1 && g->sym.uptr[0] < 0) {
+        g->sym.n_nodes = -1;  // (analysed again at the next call, and refused again)
+        return fail(KB_ERR_INVALID_ARG, "the factorization of this graph needs more than 2^30 block updates");
+    }
+    return KB_OK;
+}
+
+// the requested nodes exist, and every free node is tied to a fixed one (otherwise H is singular)
+static int pg_cov_check(const kb_pose_graph *g, const size_t *nodes, size_t n_idx) {
+    if (!nodes) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n_idx > (size_t(1) << 30)) return fail(KB_ERR_INVALID_ARG, "more than 2^29 requests in one call");
+    for (size_t t = 0; t < n_idx; ++t)
+        if (nodes[t] >= g->n()) return fail(KB_ERR_INVALID_ARG, "node %zu does not exist (%zu nodes)", nodes[t], g->n());
+    return pg_gauge_check(*g);
+}
+
+static int pg_put(DBuf<int> &d, const std::vector<int> &h, cudaStream_t s) {
+    RET(d.ensure(std::max<size_t>(h.size(), 1)));
+    if (!h.empty()) CK(cudaMemcpyAsync(d.p, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    return KB_OK;
+}
+
+// the numeric factor of H at the current poses (one cooperative launch), unless the cached one is still valid
+static int pg_factor(kb_pose_graph *g) {
+    RET(pg_symbolic(g));
+    if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
+    Exec &ex = *g->ex;
+    CK(cudaSetDevice(ex.device));
+    RET(events_on(g->cev, ex.device));
+    const PgcSymbolic &S = g->sym;
+    if (g->factored || S.nf == 0) {
+        g->factored = true;
+        return KB_OK;
+    }
+    int co_resident = 0;
+    CK(pgc_factor_max_grid(ex.sms, &co_resident));
+    const int cap = std::min(tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : ex.sms, co_resident);
+    const size_t items = std::max({g->n(), g->m(), S.blocks(), size_t(1)});
+    const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>((items + PGC_BLOCK - 1) / PGC_BLOCK, cap)));
+    RET(pg_reserve(g, grid));
+    std::vector<double> pq;
+    PgcFactorParams F{};
+    RET(pg_upload(g, &pq, &F.P));
+    cudaStream_t s = ex.stream;
+    if (g->sym_dev_n != S.n_nodes || g->sym_dev_e != S.n_edges) {
+        RET(pg_put(g->s_order, S.order, s));
+        RET(pg_put(g->s_pos, S.pos, s));
+        RET(pg_put(g->s_parent, S.parent, s));
+        RET(pg_put(g->s_col_slot, S.col_slot, s));
+        RET(pg_put(g->s_lev_ptr, S.lev_ptr, s));
+        RET(pg_put(g->s_colptr, S.colptr, s));
+        RET(pg_put(g->s_brow, S.brow, s));
+        RET(pg_put(g->s_bcol, S.bcol, s));
+        RET(pg_put(g->s_hptr, S.hptr, s));
+        RET(pg_put(g->s_hedge, S.hedge, s));
+        RET(pg_put(g->s_uptr, S.uptr, s));
+        RET(pg_put(g->s_upd, S.upd, s));
+        g->sym_dev_n = S.n_nodes;
+        g->sym_dev_e = S.n_edges;
+    }
+    RET(g->Lx.ensure(36 * S.blocks()));
+    RET(g->cov_flag.ensure(1));
+    CK(cudaMemsetAsync(g->cov_flag.p, 0, sizeof(int), s));
+    F.nf = S.nf;
+    F.levels = S.levels();
+    F.n_blocks = static_cast<int>(S.blocks());
+    F.order = g->s_order.p;
+    F.lev_ptr = g->s_lev_ptr.p;
+    F.colptr = g->s_colptr.p;
+    F.brow = g->s_brow.p;
+    F.bcol = g->s_bcol.p;
+    F.hptr = g->s_hptr.p;
+    F.hedge = g->s_hedge.p;
+    F.uptr = g->s_uptr.p;
+    F.upd = g->s_upd.p;
+    F.Lx = g->Lx.p;
+    F.flag = g->cov_flag.p;
+    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
+    ex.bar_dirty = true;
+    CK(cudaEventRecord(g->cev[0].p, s));
+    CK(pgc_factor_launch(F, grid, s));
+    ++ex.launches;
+    CK(cudaEventRecord(g->cev[1].p, s));
+    int flag = 0;
+    CK(cudaMemcpyAsync(&flag, g->cov_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+    RET(ex.sync());
+    g->uploaded = g->m();
+    if (flag) return fail(KB_ERR_INVALID_ARG, "H is not positive definite at the current poses");
+    g->factored = true;
+    return KB_OK;
+}
+
+// req[2 n]: node pairs; cov: n blocks of 36 (marginals) or 144 (joint) doubles. Factors first (pg_factor)
+static int pg_cov_solve(kb_pose_graph *g, const std::vector<int> &req, int joint, double *cov) {
+    RET(require_device());
+    RET(pg_factor(g));
+    const PgcSymbolic &S = g->sym;
+    const size_t n = req.size() / 2, per = joint ? 144 : 36;
+    std::vector<double> out(n * per, 0.0);
+    if (S.nf == 0) {  // (every node is fixed)
+        std::copy(out.begin(), out.end(), cov);
+        return KB_OK;
+    }
+    Exec &ex = *g->ex;
+    cudaStream_t s = ex.stream;
+    const size_t H = static_cast<size_t>(S.levels());
+    const size_t group_bytes = 2 * H * (36 * sizeof(double) + sizeof(int));
+    // at most 4 CTAs per SM, and at most 1 GB of solve scratch
+    const int sm_cap = tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : 4 * ex.sms;
+    const size_t mem_cap = std::max<size_t>(1, (size_t(1) << 30) / (group_bytes * PGC_GROUPS));
+    const int grid = static_cast<int>(std::max<size_t>(1, std::min({(n + PGC_GROUPS - 1) / PGC_GROUPS, static_cast<size_t>(sm_cap), mem_cap})));
+    const size_t groups = static_cast<size_t>(grid) * PGC_GROUPS;
+    RET(g->cov_X.ensure(groups * 2 * H * 36));
+    RET(g->cov_path.ensure(groups * 2 * H));
+    RET(g->cov_req.ensure(2 * n));
+    RET(g->cov_out.ensure(n * per));
+    CK(cudaMemcpyAsync(g->cov_req.p, req.data(), 2 * n * sizeof(int), cudaMemcpyHostToDevice, s));
+    PgcMarginalParams M{};
+    M.Lx = g->Lx.p;
+    M.colptr = g->s_colptr.p;
+    M.brow = g->s_brow.p;
+    M.col_slot = g->s_col_slot.p;
+    M.parent = g->s_parent.p;
+    M.pos = g->s_pos.p;
+    M.req = g->cov_req.p;
+    M.n = static_cast<int>(n);
+    M.joint = joint;
+    M.max_path = static_cast<int>(H);
+    M.X = g->cov_X.p;
+    M.path = g->cov_path.p;
+    M.out = g->cov_out.p;
+    CK(cudaEventRecord(g->cev[2].p, s));
+    CK(pgc_marginals_launch(M, grid, s));
+    ++ex.launches;
+    CK(cudaEventRecord(g->cev[3].p, s));
+    CK(cudaMemcpyAsync(out.data(), g->cov_out.p, n * per * sizeof(double), cudaMemcpyDeviceToHost, s));
+    RET(ex.sync());
+    std::copy(out.begin(), out.end(), cov);
+    return KB_OK;
+}
+
+int kb_pose_graph_marginals(kb_pose_graph *g, const size_t *nodes, size_t n, double *cov) {
+    if (!g) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n == 0) return KB_OK;
+    if (!cov) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(pg_cov_check(g, nodes, n));
+    std::vector<int> req(2 * n);
+    for (size_t t = 0; t < n; ++t) req[2 * t] = req[2 * t + 1] = static_cast<int>(nodes[t]);
+    return pg_cov_solve(g, req, 0, cov);
+}
+int kb_pose_graph_joint_marginals(kb_pose_graph *g, const size_t *pairs, size_t n, double *cov) {
+    if (!g) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n == 0) return KB_OK;
+    if (!cov) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n > (size_t(1) << 29)) return fail(KB_ERR_INVALID_ARG, "more than 2^29 requests in one call");
+    RET(pg_cov_check(g, pairs, 2 * n));
+    return pg_cov_solve(g, std::vector<int>(pairs, pairs + 2 * n), 1, cov);
+}
+int kb_pose_graph_factor_info(kb_pose_graph *g, struct kb_pose_graph_factor_info *out) {
+    if (!g || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(pg_symbolic(g));
+    const PgcSymbolic &S = g->sym;
+    struct kb_pose_graph_factor_info r {};
+    r.free_nodes = static_cast<size_t>(S.nf);
+    r.h_blocks = S.h_blocks;
+    r.l_blocks = S.blocks();
+    r.etree_height = S.nf ? static_cast<size_t>(S.levels()) : 0;
+    r.flops = S.flops;
+    *out = r;
+    return KB_OK;
+}
+int kb_debug_pose_graph_symbolic(kb_pose_graph *g, size_t cap, size_t *n_free, size_t *order, long long *parent,
+                                 size_t *col_blocks) {
+    if (!g || !n_free) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(pg_symbolic(g));
+    const PgcSymbolic &S = g->sym;
+    const size_t nf = static_cast<size_t>(S.nf);
+    *n_free = nf;
+    if (!order && !parent && !col_blocks) return KB_OK;
+    if (cap < nf) return fail(KB_ERR_CAPACITY, "buffer too small (%zu < %zu free nodes)", cap, nf);
+    for (size_t p = 0; p < nf; ++p) {
+        if (order) order[p] = static_cast<size_t>(S.order[p]);
+        if (parent) parent[p] = S.parent[p];
+        if (col_blocks) col_blocks[p] = static_cast<size_t>(S.colptr[S.col_slot[p] + 1] - S.colptr[S.col_slot[p]]);
+    }
+    return KB_OK;
+}
+int kb_debug_pose_graph_cov_ms(const kb_pose_graph *g, float ms[2]) {
+    if (!g || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (!g->cev[3].p || !g->ex) return fail(KB_ERR_INVALID_ARG, "no marginals have been computed on this graph");
+    CK(cudaSetDevice(g->ex->device));
+    float f = 0.0f, m = 0.0f;
+    if (cudaEventQuery(g->cev[1].p) == cudaSuccess && cudaEventElapsedTime(&f, g->cev[0].p, g->cev[1].p) != cudaSuccess) {
+        cudaGetLastError();
+        f = 0.0f;  // (no factorization was launched: every node is fixed)
+    }
+    CK(cudaEventElapsedTime(&m, g->cev[2].p, g->cev[3].p));
+    ms[0] = f;
+    ms[1] = m;
+    return KB_OK;
+}
+
+}  // extern "C"

@@ -1,7 +1,7 @@
 // The kernels that report plane constraints (frame.cuh: op_fit_planes), in a translation unit of their own, for the
 // reason localize.cu gives: inside another device module further instantiations would change the code the compiler
 // generates for the kernels every other pipeline runs. Like localize.cu, it compiles the headers in a namespace of its
-// own and has its own copies of the device watchdog's words, which api.cu sets and re-arms through the functions below.
+// own and has its own copies of the device watchdog's words, which host.cu arms through constraints_watchdog.
 //   k_register_frame<LocalizeConstraintParams>  a localizer with plane reporting on
 //   k_register_frame<OdometryConstraintParams>  an odometry pipeline with fit and plane reporting on
 //   k_constraints                               kb_registration_constraints: the same pass for one source at one pose
@@ -33,13 +33,4 @@ const void *odometry_constraints_kernel() {
 }
 const void *constraints_kernel() { return reinterpret_cast<const void *>(&kb_constraints::k_constraints); }
 
-cudaError_t constraints_watchdog_init(unsigned *d_host_words, const unsigned init[8]) {
-    cudaError_t e = cudaMemcpyToSymbol(kb_constraints::g_kb_wd_host, &d_host_words, sizeof(d_host_words));
-    if (e == cudaSuccess) e = cudaMemcpyToSymbol(kb_constraints::g_kb_wd, init, 8 * sizeof(unsigned));
-    return e;
-}
-
-cudaError_t constraints_watchdog_rearm() {
-    const unsigned zero = 0;
-    return cudaMemcpyToSymbol(kb_constraints::g_kb_wd, &zero, sizeof(zero));
-}
+cudaError_t constraints_watchdog(unsigned *d_host_words, const unsigned *init) { return kb_constraints::watchdog_arm(d_host_words, init); }

@@ -26,68 +26,13 @@
 
 namespace kb {
 
+using namespace kb_types;  // the types this module shares with the others and with the host (types.cuh)
+
 constexpr int KB_EMPTY = -1;
 constexpr int KB_TOMB = -2;
 constexpr unsigned FULL = 0xffffffffu;
-constexpr int BLOCK = 512;  // threads per CTA of every cooperative kernel
 constexpr int NWARPS = BLOCK / 32;
-constexpr int NACC = 16;  // unique accumulators of the 6x6 normal equations (see icp_accumulate)
-constexpr int NPART = NACC + 5;  // per-CTA partial: accumulators, #correspondences, #candidate points, cache hits/fills/overflows
 constexpr int DS_MAX_CHUNKS = 4096;  // downsample: 32-bucket chunks up to 131072 buckets (a 65k-point scan), coarser beyond
-constexpr int BAR_ARRIVE = 32, BAR_TEAM = 64, BAR_TICKET = 96, BAR_WORDS = 128;  // word offsets inside Scratch::bar (one 128-byte line each)
-constexpr int LL_RES = 16;        // est(7) + done flag, final pose(7), spare      // est(7) t_icp(7) final(7) conv cand_total query_total ...
-
-enum Counter { C_LIVE = 0, C_TOMB = 1, C_POINTS = 2, C_STATUS = 3, C_TOUCHED = 4, C_NCOUNTERS = 8 };
-enum StatusBit { ST_TABLE_FULL = 1, ST_NEED_GROW = 2, ST_SKIPPED = 4,
-                 // k_map_load's validation (set only in a table that is being loaded; the host discards it then)
-                 ST_LOAD_DUPLICATE = 8, ST_LOAD_COUNT = 16, ST_LOAD_NONFINITE = 32, ST_LOAD_OUTSIDE = 64 };
-
-// core/VoxelUtils.hpp:33-37 — FP64 DIVISION then floor then int cast (bit-exact with the CPU).
-// A DDIV is a long dependent instruction sequence; when voxel_size is an exact power of two (1.0, 0.5, 2.0 ...:
-// the reference defaults) x / v == x * (1/v) EXACTLY, so the division is replaced by a multiply.
-struct VoxelDiv {
-    double v, inv;
-    bool pow2;
-};
-__host__ __device__ __forceinline__ VoxelDiv make_voxel_div(double voxel_size) {
-    VoxelDiv d;
-    d.v = voxel_size;
-    unsigned long long bits;
-    memcpy(&bits, &voxel_size, 8);
-    const unsigned long long expo = (bits >> 52) & 0x7ffULL;
-    // normal power of two whose reciprocal is also a normal power of two
-    d.pow2 = (bits & 0x000fffffffffffffULL) == 0 && expo > 2 && expo < 2044 && voxel_size > 0.0;
-    d.inv = d.pow2 ? 1.0 / voxel_size : 0.0;
-    return d;
-}
-
-struct MapView {
-    int4 *slots;      // [capacity]
-    double *points;   // [capacity][cap][3]
-    int *head;        // [capacity] overflow list head of the pending-insert set (-1 when idle)
-    int *pcount;      // [capacity] size of the pending-insert set (0 when idle)
-    int *pending;     // [capacity][32] input indices of the pending-insert set
-    int *counters;    // [C_NCOUNTERS]
-    unsigned mask;    // capacity - 1 (capacity is a power of two)
-    int cap;          // max_points_per_voxel
-    double voxel_size;
-    double max_distance;
-    double map_resolution;  // sqrt(voxel_size^2 / max_points_per_voxel)  VoxelHashMap.cpp:98
-    VoxelDiv vdiv;          // voxel_size as a divisor (exact multiply when it is a power of two)
-};
-
-// cross-CTA scratch, sized by the grid
-struct Scratch {
-    unsigned *bar;  // [0] grid barrier counter, [BAR_ARRIVE] CTAs that left the kernel (Grid::finish), [BAR_TEAM] barrier counter of the front-end team: one 128-B
-                    // line each (arrival atomics must not fight the epoch pollers); zeroed before each launch
-    double *blk_d;  // [2][NPART][grid] doubles (ping-pong by ICP iteration parity; value-major so the reduce is coalesced)
-    uint4 *ll_part;   // [NPART][grid] epoch-tagged partial systems, one 16-B chunk per value and CTA
-    uint4 *ll_res;    // [LL_RES] epoch-tagged result record published by the coordinator
-    uint4 *ll_group;  // [NPART][16] epoch-tagged group partials (second level of the gather tree)
-    int *blk_i;     // [grid] ints
-    unsigned long long *dbg;  // [64 + 4*grid] timestamps (profiling aid)
-    int profile;              // 0: no in-kernel timestamps at all (%globaltimer reads cost ~1 us each on the critical path)
-};
 
 // ------------------------------------------------------------------------------------------
 // grid barrier (all CTAs co-resident: cooperative launch)
@@ -156,6 +101,19 @@ __device__ __forceinline__ void kb_mark(unsigned code) {
     if (threadIdx.x == 0) *reinterpret_cast<volatile unsigned *>(&g_kb_marks[blockIdx.x & 255]) = code;
 }
 enum WatchdogCode { WD_GRID_BARRIER = 1, WD_ICP_GATHER16 = 2, WD_ICP_RESULT = 3, WD_TEAM_GATHER = 4, WD_NN_BULK = 5 };
+
+// host side: every module that includes this header has its own copies of the words above and exports this function
+// for them (host.cu lists the modules). With d_host_words it arms them (g_kb_wd = init[8]); without, it re-arms them
+// after a report (clears the abort flag).
+inline cudaError_t watchdog_arm(unsigned *d_host_words, const unsigned *init) {
+    if (!d_host_words) {
+        const unsigned zero = 0;
+        return cudaMemcpyToSymbol(g_kb_wd, &zero, sizeof(zero));
+    }
+    cudaError_t e = cudaMemcpyToSymbol(g_kb_wd_host, &d_host_words, sizeof(d_host_words));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_kb_wd, init, 8 * sizeof(unsigned));
+    return e;
+}
 
 __device__ __noinline__ bool kb_spin_giveup(unsigned spins, int code, unsigned a, unsigned b) {
     if (*reinterpret_cast<volatile unsigned *>(&g_kb_wd[0]) != 0u) return true;  // somebody gave up: everybody leaves
@@ -421,7 +379,6 @@ struct WarpNN {
 // AlignPointsToMap and ICP steps shrink geometrically, so after the first iterations a query
 // costs no global memory traffic at all: ~30-cycle LDS instead of ~300-cycle L2 round trips,
 // and ~10-40 candidates instead of the 135-300 of the full 27-voxel neighbourhood.
-constexpr int QC_MAX = 64;   // cached candidates per query
 constexpr int QC_SLOTS = 2;  // cached queries per warp
 constexpr double QC_RADIUS = 0.2;  // R / voxel_size of the whole-grid ICP loop's cache
 struct QCache {

@@ -548,18 +548,11 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
 }  // namespace kb
 
 // defined in localize.cu, the localizer's device module: its k_register_frame<LocalizeParams> (takes a LocalizeParams)
-// and its copies of the watchdog words
 const void *localize_kernel();
-cudaError_t localize_watchdog_init(unsigned *d_host_words, const unsigned init[8]);
-cudaError_t localize_watchdog_rearm();
-// defined in odometry_fit.cu, likewise: k_register_frame<OdometryFitParams> and its copies of the watchdog words
+// defined in odometry_fit.cu, likewise: k_register_frame<OdometryFitParams>
 const void *odometry_fit_kernel();
-cudaError_t odometry_fit_watchdog_init(unsigned *d_host_words, const unsigned init[8]);
-cudaError_t odometry_fit_watchdog_rearm();
-// defined in constraints.cu, likewise: k_register_frame<LocalizeConstraintParams> / <OdometryConstraintParams>, the
-// stand-alone k_constraints (takes a ConstraintsParams) and the module's copies of the watchdog words
+// defined in constraints.cu, likewise: k_register_frame<LocalizeConstraintParams> / <OdometryConstraintParams> and the
+// stand-alone k_constraints (takes a ConstraintsParams)
 const void *localize_constraints_kernel();
 const void *odometry_constraints_kernel();
 const void *constraints_kernel();
-cudaError_t constraints_watchdog_init(unsigned *d_host_words, const unsigned init[8]);
-cudaError_t constraints_watchdog_rearm();

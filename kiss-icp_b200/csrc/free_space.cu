@@ -1,4 +1,4 @@
-// Free-space evidence of a voxel map (kb_map_free_space in api.cu), in a translation unit of its own for the reason
+// Free-space evidence of a voxel map (kb_map_free_space in api_free_space.cu), in a translation unit of its own for the reason
 // relocalize.cu gives: the headers are compiled here in a namespace of their own, so no kernel of another module changes.
 //   k_fs_planes   the plane of every voxel (include/kiss_icp_b200.h, "free space")
 //   k_fs_index    slot -> dump index of every voxel (the endpoint lookup goes through the map's own table)
@@ -91,7 +91,7 @@ struct RayParams {
     unsigned n;
     const unsigned *off;        // [ns + 1] chunk-local offsets
     int ns;
-    const double *pose;         // [ns][7]
+    const double *pose;         // [ns][7] q(4) t(3): the SE3 of each scan
     Bins b;
     unsigned *bin_cnt;          // [ns][ne * na]
     unsigned long long *lmax;   // [ns] bits of the longest ray
@@ -301,20 +301,7 @@ __global__ void k_fs_compact(const double *pts, const int *vox, const unsigned *
     }
 }
 
-// device memory released at scope exit
-struct Mem {
-    std::vector<void *> ptrs;
-    template <class T>
-    cudaError_t get(T **p, size_t count) {
-        *p = nullptr;
-        const cudaError_t e = cudaMalloc(reinterpret_cast<void **>(p), std::max<size_t>(count, 1) * sizeof(T));
-        if (e == cudaSuccess) ptrs.push_back(*p);
-        return e;
-    }
-    ~Mem() {
-        for (void *p : ptrs) cudaFree(p);
-    }
-};
+static_assert(sizeof(SE3) == 7 * sizeof(double), "RayParams::pose is an array of SE3");
 
 int blocks_for(size_t n, int max_ctas) {
     return static_cast<int>(std::max<size_t>(1, std::min<size_t>((n + FS_THREADS - 1) / FS_THREADS, static_cast<size_t>(max_ctas))));
@@ -324,80 +311,69 @@ int blocks_for(size_t n, int max_ctas) {
 
 double fs_default_bin_size() { return 1.0 * 3.141592653589793 / 180.0; }
 
-#define FS_CK(call)                          \
-    do {                                     \
-        const cudaError_t e_ = (call);       \
-        if (e_ != cudaSuccess) return e_;    \
-    } while (0)
+cudaError_t free_space_watchdog(unsigned *d_host_words, const unsigned *init) { return kb_fs::watchdog_arm(d_host_words, init); }
 
-cudaError_t fs_run(const FsInput &in, FsOutput *out, cudaStream_t s) {
+int fs_run(const FsInput &in, FsOutput *out, kb_host::Exec &ex) {
     using namespace kb_fs;
-    if (in.view_bytes != sizeof(MapView) || in.pose_bytes != sizeof(SE3)) return cudaErrorInvalidValue;
-    MapView m;
-    std::memcpy(&m, in.map_view, sizeof(MapView));
+    using namespace kb_host;
+    const MapView &m = in.m;
+    const cudaStream_t s = ex.stream;
     out->points_removed = out->voxels_removed = out->tests = 0;
-    out->kept_vox = out->kept_cnt = nullptr;
-    out->kept_off = nullptr;
-    out->kept_pts = nullptr;
     out->kept_voxels = out->kept_points = 0;
     out->ms[0] = out->ms[1] = out->ms[2] = 0.0f;
     const size_t V = in.n_voxels, P = in.n_points;
     const int nv = static_cast<int>(V);
     const int G = std::max(in.max_ctas, 1) * 4;  // CTAs of the grid-stride launches
-    Mem mem;
-    cudaEvent_t ev[2];
-    FS_CK(cudaEventCreate(&ev[0]));
-    FS_CK(cudaEventCreate(&ev[1]));
-    struct EvGuard {
-        cudaEvent_t *e;
-        ~EvGuard() { cudaEventDestroy(e[0]); cudaEventDestroy(e[1]); }
-    } evg{ev};
-    auto timed = [&](int phase) -> cudaError_t {  // add the time between ev[0] and ev[1] to ms[phase]
-        FS_CK(cudaEventRecord(ev[1], s));
-        FS_CK(cudaEventSynchronize(ev[1]));
+    auto get = [](auto &buf, size_t count) { return buf.alloc(std::max<size_t>(count, 1)); };  // (call-local buffers)
+    Event ev[2];
+    CK(ev[0].create(cudaEventDefault));
+    CK(ev[1].create(cudaEventDefault));
+    auto timed = [&](int phase) -> int {  // add the time between ev[0] and ev[1] to ms[phase]
+        CK(cudaEventRecord(ev[1].p, s));
+        RET(ex.wait_deadline([&] { return cudaEventQuery(ev[1].p); }, "free-space counting"));
         float t = 0.0f;
-        FS_CK(cudaEventElapsedTime(&t, ev[0], ev[1]));
+        CK(cudaEventElapsedTime(&t, ev[0].p, ev[1].p));
         out->ms[phase] += t;
-        return cudaSuccess;
+        return KB_OK;
     };
 
     // the map in dump layout, its planes and the slot -> dump index of its table
-    int *d_vox, *d_cnt, *slot2dump;
-    long long *d_voff;
-    double *d_pts;
-    double4 *d_plane;
-    unsigned *d_passes, *d_hits;
-    unsigned long long *d_tot;  // [0] tests, [1] points removed, [2] voxels removed
+    DBuf<int> d_vox, d_cnt, slot2dump;
+    DBuf<long long> d_voff;
+    DBuf<double> d_pts;
+    DBuf<double4> d_plane;
+    DBuf<unsigned> d_passes, d_hits;
+    DBuf<unsigned long long> d_tot;  // [0] tests, [1] points removed, [2] voxels removed
     std::vector<long long> voff(V);
     long long acc = 0;
     for (size_t r = 0; r < V; ++r) {
         voff[r] = acc;
         acc += in.counts[r];
     }
-    FS_CK(mem.get(&d_vox, 3 * V));
-    FS_CK(mem.get(&d_cnt, V));
-    FS_CK(mem.get(&d_voff, V));
-    FS_CK(mem.get(&d_pts, 3 * P));
-    FS_CK(mem.get(&d_plane, V));
-    FS_CK(mem.get(&d_passes, P));
-    FS_CK(mem.get(&d_hits, V));
-    FS_CK(mem.get(&d_tot, 3));
-    FS_CK(mem.get(&slot2dump, static_cast<size_t>(m.mask) + 1));
-    FS_CK(cudaMemcpyAsync(d_vox, in.voxels, 3 * V * sizeof(int), cudaMemcpyHostToDevice, s));
-    FS_CK(cudaMemcpyAsync(d_cnt, in.counts, V * sizeof(int), cudaMemcpyHostToDevice, s));
-    FS_CK(cudaMemcpyAsync(d_voff, voff.data(), V * sizeof(long long), cudaMemcpyHostToDevice, s));
-    FS_CK(cudaMemcpyAsync(d_pts, in.points, 3 * P * sizeof(double), cudaMemcpyHostToDevice, s));
-    FS_CK(cudaMemsetAsync(d_passes, 0, std::max<size_t>(P, 1) * sizeof(unsigned), s));
-    FS_CK(cudaMemsetAsync(d_hits, 0, std::max<size_t>(V, 1) * sizeof(unsigned), s));
-    FS_CK(cudaMemsetAsync(d_tot, 0, 3 * sizeof(unsigned long long), s));
-    FS_CK(cudaMemsetAsync(slot2dump, 0xff, (static_cast<size_t>(m.mask) + 1) * sizeof(int), s));
-    FS_CK(cudaEventRecord(ev[0], s));
+    CK(get(d_vox, 3 * V));
+    CK(get(d_cnt, V));
+    CK(get(d_voff, V));
+    CK(get(d_pts, 3 * P));
+    CK(get(d_plane, V));
+    CK(get(d_passes, P));
+    CK(get(d_hits, V));
+    CK(get(d_tot, 3));
+    CK(get(slot2dump, static_cast<size_t>(m.mask) + 1));
+    CK(cudaMemcpyAsync(d_vox.p, in.voxels, 3 * V * sizeof(int), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_cnt.p, in.counts, V * sizeof(int), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_voff.p, voff.data(), V * sizeof(long long), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d_pts.p, in.points, 3 * P * sizeof(double), cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync(d_passes.p, 0, std::max<size_t>(P, 1) * sizeof(unsigned), s));
+    CK(cudaMemsetAsync(d_hits.p, 0, std::max<size_t>(V, 1) * sizeof(unsigned), s));
+    CK(cudaMemsetAsync(d_tot.p, 0, 3 * sizeof(unsigned long long), s));
+    CK(cudaMemsetAsync(slot2dump.p, 0xff, (static_cast<size_t>(m.mask) + 1) * sizeof(int), s));
+    CK(cudaEventRecord(ev[0].p, s));
     if (V) {
-        k_fs_planes<<<blocks_for(V, G), FS_THREADS, 0, s>>>(d_pts, d_voff, d_cnt, nv, in.rule.a_min, d_plane);
-        k_fs_index<<<blocks_for(V, G), FS_THREADS, 0, s>>>(m, d_vox, nv, slot2dump);
-        FS_CK(cudaGetLastError());
+        k_fs_planes<<<blocks_for(V, G), FS_THREADS, 0, s>>>(d_pts.p, d_voff.p, d_cnt.p, nv, in.rule.a_min, d_plane.p);
+        k_fs_index<<<blocks_for(V, G), FS_THREADS, 0, s>>>(m, d_vox.p, nv, slot2dump.p);
+        CK(cudaGetLastError());
     }
-    FS_CK(timed(0));
+    RET(timed(0));
 
     // the bins and the chunks: at most 2^22 rays (or one scan, if larger) and 2^24 bins per chunk
     Bins b;
@@ -411,26 +387,26 @@ cudaError_t fs_run(const FsInput &in, FsOutput *out, cudaStream_t s) {
     size_t largest = 0;
     for (size_t k = 0; k < in.n_scans; ++k) largest = std::max(largest, in.offset[k + 1] - in.offset[k]);
     const size_t ray_cap = std::max(max_rays, largest);
-    double *d_xyz, *d_pose;
-    unsigned *d_off, *d_bcnt, *d_bstart, *d_nsel;
-    unsigned long long *d_lmax;
-    double4 *d_ray, *d_sorted;
-    int *d_rbin, *d_sel;
-    FS_CK(mem.get(&d_xyz, 3 * ray_cap));
-    FS_CK(mem.get(&d_pose, 7 * max_scans));
-    FS_CK(mem.get(&d_off, max_scans + 1));
-    FS_CK(mem.get(&d_bcnt, max_scans * nb + 1));
-    FS_CK(mem.get(&d_bstart, max_scans * nb + 1));
-    FS_CK(mem.get(&d_lmax, max_scans));
-    FS_CK(mem.get(&d_ray, ray_cap));
-    FS_CK(mem.get(&d_sorted, ray_cap));
-    FS_CK(mem.get(&d_rbin, ray_cap));
-    FS_CK(mem.get(&d_sel, V));
-    FS_CK(mem.get(&d_nsel, 1));
-    void *d_tmp = nullptr;
+    DBuf<double> d_xyz, d_pose;
+    DBuf<unsigned> d_off, d_bcnt, d_bstart, d_nsel;
+    DBuf<unsigned long long> d_lmax;
+    DBuf<double4> d_ray, d_sorted;
+    DBuf<int> d_rbin, d_sel;
+    CK(get(d_xyz, 3 * ray_cap));
+    CK(get(d_pose, 7 * max_scans));
+    CK(get(d_off, max_scans + 1));
+    CK(get(d_bcnt, max_scans * nb + 1));
+    CK(get(d_bstart, max_scans * nb + 1));
+    CK(get(d_lmax, max_scans));
+    CK(get(d_ray, ray_cap));
+    CK(get(d_sorted, ray_cap));
+    CK(get(d_rbin, ray_cap));
+    CK(get(d_sel, V));
+    CK(get(d_nsel, 1));
+    DBuf<char> d_tmp;
     size_t tmp_bytes = 0;
-    FS_CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_bcnt, d_bstart, static_cast<int>(max_scans * nb + 1), s));
-    FS_CK(mem.get(reinterpret_cast<char **>(&d_tmp), tmp_bytes));
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_bcnt.p, d_bstart.p, static_cast<int>(max_scans * nb + 1), s));
+    CK(get(d_tmp, tmp_bytes));
 
     std::vector<unsigned> off;
     std::vector<unsigned long long> lmax;
@@ -441,132 +417,122 @@ cudaError_t fs_run(const FsInput &in, FsOutput *out, cudaStream_t s) {
         const size_t base = in.offset[s0], n = in.offset[s1] - base;
         off.resize(ns + 1);
         for (int k = 0; k <= ns; ++k) off[k] = static_cast<unsigned>(in.offset[s0 + k] - base);
-        if (n) FS_CK(cudaMemcpyAsync(d_xyz, in.xyz + 3 * base, 3 * n * sizeof(double), cudaMemcpyHostToDevice, s));
-        FS_CK(cudaMemcpyAsync(d_pose, in.poses + 7 * s0, 7 * ns * sizeof(double), cudaMemcpyHostToDevice, s));
-        FS_CK(cudaMemcpyAsync(d_off, off.data(), (ns + 1) * sizeof(unsigned), cudaMemcpyHostToDevice, s));
+        if (n) CK(cudaMemcpyAsync(d_xyz.p, in.xyz + 3 * base, 3 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_pose.p, in.poses + s0, ns * sizeof(SE3), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_off.p, off.data(), (ns + 1) * sizeof(unsigned), cudaMemcpyHostToDevice, s));
         const int nbins = static_cast<int>(ns * nb + 1);
-        FS_CK(cudaMemsetAsync(d_bcnt, 0, nbins * sizeof(unsigned), s));
-        FS_CK(cudaMemsetAsync(d_lmax, 0, ns * sizeof(unsigned long long), s));
+        CK(cudaMemsetAsync(d_bcnt.p, 0, nbins * sizeof(unsigned), s));
+        CK(cudaMemsetAsync(d_lmax.p, 0, ns * sizeof(unsigned long long), s));
         // the bin index of the chunk's rays: histogram (and the hits), scan, scatter
-        FS_CK(cudaEventRecord(ev[0], s));
+        CK(cudaEventRecord(ev[0].p, s));
         if (n) {
             RayParams R;
             R.m = m;
-            R.slot2dump = slot2dump;
-            R.hits = d_hits;
-            R.xyz = d_xyz;
+            R.slot2dump = slot2dump.p;
+            R.hits = d_hits.p;
+            R.xyz = d_xyz.p;
             R.n = static_cast<unsigned>(n);
-            R.off = d_off;
+            R.off = d_off.p;
             R.ns = ns;
-            R.pose = d_pose;
+            R.pose = d_pose.p;
             R.b = b;
-            R.bin_cnt = d_bcnt;
-            R.lmax = d_lmax;
-            R.ray = d_ray;
-            R.rbin = d_rbin;
+            R.bin_cnt = d_bcnt.p;
+            R.lmax = d_lmax.p;
+            R.ray = d_ray.p;
+            R.rbin = d_rbin.p;
             k_fs_rays<<<blocks_for(n, G), FS_THREADS, 0, s>>>(R);
-            FS_CK(cudaGetLastError());
+            CK(cudaGetLastError());
         }
-        FS_CK(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_bcnt, d_bstart, nbins, s));
-        FS_CK(cudaMemsetAsync(d_bcnt, 0, nbins * sizeof(unsigned), s));
+        CK(cub::DeviceScan::ExclusiveSum(d_tmp.p, tmp_bytes, d_bcnt.p, d_bstart.p, nbins, s));
+        CK(cudaMemsetAsync(d_bcnt.p, 0, nbins * sizeof(unsigned), s));
         if (n) {
-            k_fs_scatter<<<blocks_for(n, G), FS_THREADS, 0, s>>>(d_ray, d_rbin, static_cast<unsigned>(n), d_bstart, d_bcnt, d_sorted);
-            FS_CK(cudaGetLastError());
+            k_fs_scatter<<<blocks_for(n, G), FS_THREADS, 0, s>>>(d_ray.p, d_rbin.p, static_cast<unsigned>(n), d_bstart.p, d_bcnt.p, d_sorted.p);
+            CK(cudaGetLastError());
         }
         lmax.resize(ns);
-        FS_CK(cudaMemcpyAsync(lmax.data(), d_lmax, ns * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-        FS_CK(timed(1));
+        CK(cudaMemcpyAsync(lmax.data(), d_lmax.p, ns * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+        RET(timed(1));
         // the counting, scan by scan
-        FS_CK(cudaEventRecord(ev[0], s));
+        CK(cudaEventRecord(ev[0].p, s));
         for (int k = 0; k < ns && V; ++k) {
             double L;
             std::memcpy(&L, &lmax[k], sizeof(L));
             if (!(L > in.rule.delta)) continue;  // no ray of the scan passes anything
-            const double *q = in.poses + 7 * (s0 + k);
-            const V3 o{q[4], q[5], q[6]};
+            const V3 o = in.poses[s0 + k].t;
             const double reach = (L + in.rule.eps) * (1.0 + 1e-9) + 1e-3 * m.voxel_size;
-            FS_CK(cudaMemsetAsync(d_nsel, 0, sizeof(unsigned), s));
-            k_fs_select<<<blocks_for(V, G), FS_THREADS, 0, s>>>(d_vox, nv, m.voxel_size, o, reach, d_sel, d_nsel);
+            CK(cudaMemsetAsync(d_nsel.p, 0, sizeof(unsigned), s));
+            k_fs_select<<<blocks_for(V, G), FS_THREADS, 0, s>>>(d_vox.p, nv, m.voxel_size, o, reach, d_sel.p, d_nsel.p);
             CountParams C;
-            C.pts = d_pts;
-            C.voff = d_voff;
-            C.cnt = d_cnt;
-            C.plane = d_plane;
-            C.sel = d_sel;
-            C.nsel = d_nsel;
-            C.ray = d_sorted;
-            C.bin_start = d_bstart + k * nb;
+            C.pts = d_pts.p;
+            C.voff = d_voff.p;
+            C.cnt = d_cnt.p;
+            C.plane = d_plane.p;
+            C.sel = d_sel.p;
+            C.nsel = d_nsel.p;
+            C.ray = d_sorted.p;
+            C.bin_start = d_bstart.p + k * nb;
             C.b = b;
             C.o = o;
             C.lmax = L;
             C.eps = in.rule.eps;
             C.delta = in.rule.delta;
             C.sin_min = in.rule.sin_min;
-            C.passes = d_passes;
-            C.tests = d_tot;
+            C.passes = d_passes.p;
+            C.tests = d_tot.p;
             k_fs_count<<<blocks_for(32 * V, G), FS_THREADS, 0, s>>>(C);
-            FS_CK(cudaGetLastError());
+            CK(cudaGetLastError());
         }
-        FS_CK(timed(2));
+        RET(timed(2));
         s0 = s1;
     }
 
     // the removal rule and the kept points
     if (V) {
-        int *kcnt, *kflag, *kvi;
-        long long *koff;
-        FS_CK(mem.get(&kcnt, V));
-        FS_CK(mem.get(&kflag, V));
-        FS_CK(mem.get(&kvi, V));
-        FS_CK(mem.get(&koff, V));
-        k_fs_keep<<<blocks_for(V, G), FS_THREADS, 0, s>>>(d_passes, d_hits, d_voff, d_cnt, nv, in.rule.min_passes,
-                                                            in.rule.ratio, kcnt, kflag, d_tot + 1);
-        FS_CK(cudaGetLastError());
+        DBuf<int> kcnt, kflag, kvi;
+        DBuf<long long> koff;
+        CK(get(kcnt, V));
+        CK(get(kflag, V));
+        CK(get(kvi, V));
+        CK(get(koff, V));
+        k_fs_keep<<<blocks_for(V, G), FS_THREADS, 0, s>>>(d_passes.p, d_hits.p, d_voff.p, d_cnt.p, nv, in.rule.min_passes,
+                                                            in.rule.ratio, kcnt.p, kflag.p, d_tot.p + 1);
+        CK(cudaGetLastError());
         if (in.want_kept) {
             size_t b1 = 0, b2 = 0;
-            FS_CK(cub::DeviceScan::ExclusiveScan(nullptr, b1, kcnt, koff, ::cuda::std::plus<>{}, 0LL, nv, s));
-            FS_CK(cub::DeviceScan::ExclusiveSum(nullptr, b2, kflag, kvi, nv, s));
-            char *t;
-            FS_CK(mem.get(&t, std::max(b1, b2)));
-            FS_CK(cub::DeviceScan::ExclusiveScan(t, b1, kcnt, koff, ::cuda::std::plus<>{}, 0LL, nv, s));
-            FS_CK(cub::DeviceScan::ExclusiveSum(t, b2, kflag, kvi, nv, s));
+            CK(cub::DeviceScan::ExclusiveScan(nullptr, b1, kcnt.p, koff.p, ::cuda::std::plus<>{}, 0LL, nv, s));
+            CK(cub::DeviceScan::ExclusiveSum(nullptr, b2, kflag.p, kvi.p, nv, s));
+            DBuf<char> t;
+            CK(get(t, std::max(b1, b2)));
+            CK(cub::DeviceScan::ExclusiveScan(t.p, b1, kcnt.p, koff.p, ::cuda::std::plus<>{}, 0LL, nv, s));
+            CK(cub::DeviceScan::ExclusiveSum(t.p, b2, kflag.p, kvi.p, nv, s));
             long long last_off;
             int last_cnt, last_vi, last_flag;
-            FS_CK(cudaMemcpyAsync(&last_off, koff + V - 1, sizeof(last_off), cudaMemcpyDeviceToHost, s));
-            FS_CK(cudaMemcpyAsync(&last_cnt, kcnt + V - 1, sizeof(last_cnt), cudaMemcpyDeviceToHost, s));
-            FS_CK(cudaMemcpyAsync(&last_vi, kvi + V - 1, sizeof(last_vi), cudaMemcpyDeviceToHost, s));
-            FS_CK(cudaMemcpyAsync(&last_flag, kflag + V - 1, sizeof(last_flag), cudaMemcpyDeviceToHost, s));
-            FS_CK(cudaStreamSynchronize(s));
+            CK(cudaMemcpyAsync(&last_off, koff.p + V - 1, sizeof(last_off), cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(&last_cnt, kcnt.p + V - 1, sizeof(last_cnt), cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(&last_vi, kvi.p + V - 1, sizeof(last_vi), cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(&last_flag, kflag.p + V - 1, sizeof(last_flag), cudaMemcpyDeviceToHost, s));
+            RET(ex.sync());
             const size_t kv = static_cast<size_t>(last_vi + last_flag), kp = static_cast<size_t>(last_off + last_cnt);
-            FS_CK(cudaMalloc(&out->kept_vox, std::max<size_t>(3 * kv, 1) * sizeof(int)));
-            FS_CK(cudaMalloc(&out->kept_cnt, std::max<size_t>(kv, 1) * sizeof(int)));
-            FS_CK(cudaMalloc(&out->kept_off, std::max<size_t>(kv, 1) * sizeof(long long)));
-            FS_CK(cudaMalloc(&out->kept_pts, std::max<size_t>(3 * kp, 1) * sizeof(double)));
+            CK(get(out->kept_vox, 3 * kv));
+            CK(get(out->kept_cnt, kv));
+            CK(get(out->kept_off, kv));
+            CK(get(out->kept_pts, 3 * kp));
             out->kept_voxels = kv;
             out->kept_points = kp;
-            k_fs_compact<<<blocks_for(V, G), FS_THREADS, 0, s>>>(d_pts, d_vox, d_passes, d_hits, d_voff, d_cnt, nv,
-                                                                  in.rule.min_passes, in.rule.ratio, kcnt, koff, kvi,
-                                                                  out->kept_vox, out->kept_cnt, out->kept_off, out->kept_pts);
-            FS_CK(cudaGetLastError());
+            k_fs_compact<<<blocks_for(V, G), FS_THREADS, 0, s>>>(d_pts.p, d_vox.p, d_passes.p, d_hits.p, d_voff.p, d_cnt.p, nv,
+                                                                  in.rule.min_passes, in.rule.ratio, kcnt.p, koff.p, kvi.p,
+                                                                  out->kept_vox.p, out->kept_cnt.p, out->kept_off.p, out->kept_pts.p);
+            CK(cudaGetLastError());
         }
     }
     unsigned long long tot[3];
-    FS_CK(cudaMemcpyAsync(tot, d_tot, sizeof(tot), cudaMemcpyDeviceToHost, s));
-    if (out->passes && P) FS_CK(cudaMemcpyAsync(out->passes, d_passes, P * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
-    if (out->hits && V) FS_CK(cudaMemcpyAsync(out->hits, d_hits, V * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
-    FS_CK(cudaStreamSynchronize(s));
+    CK(cudaMemcpyAsync(tot, d_tot.p, sizeof(tot), cudaMemcpyDeviceToHost, s));
+    if (out->passes && P) CK(cudaMemcpyAsync(out->passes, d_passes.p, P * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+    if (out->hits && V) CK(cudaMemcpyAsync(out->hits, d_hits.p, V * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+    RET(ex.sync());
     out->tests = tot[0];
     out->points_removed = tot[1];
     out->voxels_removed = tot[2];
-    return cudaSuccess;
+    return KB_OK;
 }
 
-void fs_release(FsOutput *out) {
-    cudaFree(out->kept_vox);
-    cudaFree(out->kept_cnt);
-    cudaFree(out->kept_off);
-    cudaFree(out->kept_pts);
-    out->kept_vox = out->kept_cnt = nullptr;
-    out->kept_off = nullptr;
-    out->kept_pts = nullptr;
-}

@@ -22,28 +22,10 @@
 
 namespace kb {
 
-constexpr int TEAM_MAX = 96;    // CTAs of an ICP team (the gathered partials, 21 x TEAM_MAX doubles, fit the 16 KB reduction scratch)
 static_assert(NPART * TEAM_MAX * 8 <= DS_MAX_CHUNKS * 4, "the gathered partials live in Shared::chunk_pref");
-constexpr int TQ_LANES = 4;     // lanes that share one source point in the list walk
-constexpr int TQ_PER_WARP = 32 / TQ_LANES;
-constexpr int TQ_PER_CTA = 80;  // source points per team CTA by default (10 warps; H100 A/B in DESIGN.md section 6)
-constexpr int TQ_MAX = 120;     // upper bound of source points per team CTA (warps 0..14; the solver is thread 511)
 constexpr int TRED_STRIDE = NACC + 1;  // row of the per-point reduction scratch: 16 entries + the gate flag (odd: conflict-free)
 static_assert(TQ_MAX * TRED_STRIDE * 8 <= DS_MAX_CHUNKS * 4, "the reduction scratch lives in Shared::chunk_pref");
 
-// Output of the fill pass for one source point (global memory): the list holds POINT INDICES (slot * cap + k) in the
-// reference's visiting order (voxel_shifts order, then insertion order) around the voxel where it was made, so for a
-// point in that voxel the first strict minimum over the list is the reference's answer, ties included (in another
-// voxel a tie is searched again: team_list_nn).
-struct QList {
-    int count;      // >= 0: idx[0..count) valid; -1: not cacheable (too many candidates / max_points_per_voxel > 32)
-    int full;       // points of the whole 27-voxel neighbourhood (bookkeeping of algorithmic bytes)
-    int vx, vy, vz; // voxel at fill time
-    int pad[3];
-    double pf[3];   // position at fill time (= initial_guess * source point)
-    int idx[QC_MAX];
-    int tail[2];    // 320 bytes
-};
 static_assert(sizeof(QList) % 16 == 0 && sizeof(QList) == sizeof(QListRaw), "QList records are 16-byte aligned; Shared::rlist holds one per warp");
 
 // A source point inside its team CTA (shared memory): state + where its candidate COORDINATES are. A warp owns 8
@@ -93,14 +75,6 @@ __device__ __forceinline__ unsigned tq_coord_addr(unsigned coords_base, int K, i
 __device__ __forceinline__ double *tq_coord(const TeamSmem &ts, int li, int k) {
     return ts.coords + (static_cast<size_t>(li / TQ_PER_WARP) * (ts.K >> 2) + (k >> 2)) * 96 + ((4 * (li & (TQ_PER_WARP - 1)) + k) & 31);
 }
-
-struct TeamScratch {
-    uint4 *ll;        // [2][TEAM_MAX readers][TEAM_MAX members][NPART] epoch-tagged partial systems, ping-pong by iteration parity
-    double *out;      // [16] result record: pose(7) iters cand_total query_total cache_stats(3)
-    QList *qrec;      // [n] per source point, written by the fill pass
-    int smem_bytes;   // dynamic shared memory of the launch
-    double radius_frac;  // R / voxel_size: a list stays exact while its point has moved by <= R (shorter lists for smaller R)
-};
 
 // team size for n source points at q_per_cta points per CTA; 0 when the lists would not fit in shared memory
 __host__ __device__ __forceinline__ int icp_team_size(int n, int q_per_cta, int grid, int smem_bytes) {

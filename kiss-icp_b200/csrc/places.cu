@@ -1,5 +1,5 @@
 // Place recognition: the Scan Context descriptor of a cloud and its distance to every entry of a database at every
-// cyclic shift (the kb_place_* calls in api.cu), in a translation unit of its own: a kernel added to api.cu's device
+// cyclic shift (the kb_place_* calls in api_places.cu), in a translation unit of its own: a kernel added to api.cu's device
 // module changes the code the compiler generates for the kernels already there. These kernels use none of the hot
 // path's device code.
 #include <algorithm>

@@ -1,4 +1,4 @@
-// Launchers of the place-recognition kernels (places.cu, the kb_place_* calls in api.cu). All pointers are device
+// Launchers of the place-recognition kernels (places.cu, the kb_place_* calls in api_places.cu). All pointers are device
 // pointers; every launch is asynchronous on `s`.
 #pragma once
 

@@ -1,8 +1,8 @@
-// The pose-graph optimizer (kb_pose_graph_optimize in api.cu): Levenberg-Marquardt with IRLS weights, the damped normal
+// The pose-graph optimizer (kb_pose_graph_optimize in api_pose_graph.cu): Levenberg-Marquardt with IRLS weights, the damped normal
 // equations solved by PCG with the exact inverse of their block-tridiagonal part, applied by block cyclic reduction.
 // The whole optimization is one persistent cooperative launch on the Grid barrier of device_ops.cuh. Like localize.cu,
 // the unit compiles the header in a namespace of its own (and so has its own copies of the device watchdog's words,
-// which api.cu sets and re-arms through the functions at the end), and a kernel here changes no code generated for the
+// which host.cu arms through pose_graph_watchdog), and a kernel here changes no code generated for the
 // kernels of the other units.
 //
 // Determinism: every sum is formed in a fixed order. A node's blocks add their edges' contributions in ascending edge
@@ -503,13 +503,4 @@ cudaError_t pose_graph_launch(const PoseGraphParams &P, int grid, cudaStream_t s
                                        dim3(POSE_GRAPH_BLOCK), args, 0, s);
 }
 
-cudaError_t pose_graph_watchdog_init(unsigned *d_host_words, const unsigned init[8]) {
-    cudaError_t e = cudaMemcpyToSymbol(kb_pg::g_kb_wd_host, &d_host_words, sizeof(d_host_words));
-    if (e == cudaSuccess) e = cudaMemcpyToSymbol(kb_pg::g_kb_wd, init, 8 * sizeof(unsigned));
-    return e;
-}
-
-cudaError_t pose_graph_watchdog_rearm() {
-    const unsigned zero = 0;
-    return cudaMemcpyToSymbol(kb_pg::g_kb_wd, &zero, sizeof(zero));
-}
+cudaError_t pose_graph_watchdog(unsigned *d_host_words, const unsigned *init) { return kb_pg::watchdog_arm(d_host_words, init); }

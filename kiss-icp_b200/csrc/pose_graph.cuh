@@ -1,4 +1,4 @@
-// Launcher of the pose-graph optimizer (pose_graph.cu, kb_pose_graph_optimize in api.cu). All pointers are device
+// Launcher of the pose-graph optimizer (pose_graph.cu, kb_pose_graph_optimize in api_pose_graph.cu). All pointers are device
 // pointers; the launch is asynchronous on the caller's stream.
 #pragma once
 
@@ -38,6 +38,3 @@ cudaError_t pose_graph_launch(const PoseGraphParams &P, int grid, cudaStream_t s
 // the most CTAs of the optimizer kernel that are co-resident on a device with `sms` multiprocessors
 cudaError_t pose_graph_max_grid(int sms, int *out);
 constexpr int POSE_GRAPH_BLOCK = 256;  // threads per CTA
-// the module's copies of the device watchdog's words (device_ops.cuh), set and re-armed by api.cu
-cudaError_t pose_graph_watchdog_init(unsigned *d_host_words, const unsigned init[8]);
-cudaError_t pose_graph_watchdog_rearm();

@@ -1,9 +1,9 @@
-// Marginal covariances of a pose graph (kb_pose_graph_marginals & co. in api.cu): H = P L L^T P^T over the free nodes,
+// Marginal covariances of a pose graph (kb_pose_graph_marginals & co. in api_pose_graph.cu): H = P L L^T P^T over the free nodes,
 // a sparse block Cholesky factorization in a nested-dissection order, and Sigma_ij = X_i^T X_j with X_k = L^-1 P^T E_k
 // solved along the elimination-tree path of k. The symbolic analysis is host code (pgc_symbolic); the factorization is
 // one persistent cooperative launch on the Grid barrier of device_ops.cuh, the marginals one ordinary launch.
 //
-// A translation unit of its own, with its own copies of the watchdog's words (set and re-armed by api.cu), so that the
+// A translation unit of its own, with its own copies of the watchdog's words (armed by host.cu), so that the
 // optimizer's kernel compiles exactly as before (DESIGN §4.6); the device code both need is pose_graph_edges.cuh.
 //
 // Determinism: every value is formed by one thread in a fixed order (a block's updates in ascending column order, a
@@ -611,13 +611,4 @@ cudaError_t pgc_marginals_launch(const PgcMarginalParams &P, int grid, cudaStrea
     return cudaGetLastError();
 }
 
-cudaError_t pgc_watchdog_init(unsigned *d_host_words, const unsigned init[8]) {
-    cudaError_t e = cudaMemcpyToSymbol(kb_pgc::g_kb_wd_host, &d_host_words, sizeof(d_host_words));
-    if (e == cudaSuccess) e = cudaMemcpyToSymbol(kb_pgc::g_kb_wd, init, 8 * sizeof(unsigned));
-    return e;
-}
-
-cudaError_t pgc_watchdog_rearm() {
-    const unsigned zero = 0;
-    return cudaMemcpyToSymbol(kb_pgc::g_kb_wd, &zero, sizeof(zero));
-}
+cudaError_t pose_graph_cov_watchdog(unsigned *d_host_words, const unsigned *init) { return kb_pgc::watchdog_arm(d_host_words, init); }

@@ -1,4 +1,4 @@
-// Marginal covariances of a pose graph (pose_graph_cov.cu, kb_pose_graph_marginals & co. in api.cu): the symbolic
+// Marginal covariances of a pose graph (pose_graph_cov.cu, kb_pose_graph_marginals & co. in api_pose_graph.cu): the symbolic
 // analysis on the host, the launchers of the numeric factorization and of the marginal solves. All pointers of the
 // parameter structs are device pointers; launches are asynchronous on the caller's stream.
 #pragma once
@@ -57,6 +57,3 @@ constexpr int PGC_GROUPS = PGC_SOLVE_BLOCK / 8;
 cudaError_t pgc_factor_max_grid(int sms, int *out);
 cudaError_t pgc_factor_launch(const PgcFactorParams &P, int grid, cudaStream_t s);
 cudaError_t pgc_marginals_launch(const PgcMarginalParams &P, int grid, cudaStream_t s);
-// the module's copies of the device watchdog's words (device_ops.cuh), set and re-armed by api.cu
-cudaError_t pgc_watchdog_init(unsigned *d_host_words, const unsigned init[8]);
-cudaError_t pgc_watchdog_rearm();

@@ -6,7 +6,6 @@
 #undef kb
 
 #include <algorithm>
-#include <cstring>
 
 #include "probe.cuh"
 
@@ -127,14 +126,13 @@ unsigned blocks_for(int n, int per_block) { return static_cast<unsigned>((n + pe
 
 }  // namespace kb_probe
 
-cudaError_t probe_nn_reuse(const void *map_view, size_t view_bytes, const double *pf, const double *p, int n, int path,
+cudaError_t probe_watchdog(unsigned *d_host_words, const unsigned *init) { return kb_probe::watchdog_arm(d_host_words, init); }
+
+cudaError_t probe_nn_reuse(const kb_types::MapView &m, const double *pf, const double *p, int n, int path,
                            double radius_frac, int smem_bytes, int team_q, double *out_points, double *out_dist,
                            int *out_reused, cudaStream_t s) {
     using namespace kb_probe;
-    if (view_bytes != sizeof(MapView)) return cudaErrorInvalidValue;
     if (n <= 0) return cudaSuccess;
-    MapView m;
-    std::memcpy(&m, map_view, sizeof(m));
     if (path == 0) {
         const int qmax = team_q > 0 ? team_q : TQ_PER_CTA;  // (KB_ICP_TEAM_Q=0 runs no team: the default team's lists)
         cudaError_t e = cudaFuncSetAttribute(reinterpret_cast<const void *>(&k_probe_team),

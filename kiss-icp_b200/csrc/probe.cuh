@@ -8,10 +8,11 @@
 
 #include <cstddef>
 
-// map_view points to api.cu's MapView (view_bytes = its size; probe.cu checks that its own copy has the same layout).
+#include "types.cuh"
+
 // path 0: the team's candidate list made at pf[i], then its answer at p[i]; path 1: the whole-grid loop's cache.
 // radius_frac, smem_bytes and team_q are the team's R / voxel_size, dynamic shared memory and source points per CTA.
-cudaError_t probe_nn_reuse(const void *map_view, size_t view_bytes, const double *pf, const double *p, int n, int path,
+cudaError_t probe_nn_reuse(const kb_types::MapView &m, const double *pf, const double *p, int n, int path,
                            double radius_frac, int smem_bytes, int team_q, double *out_points, double *out_dist,
                            int *out_reused, cudaStream_t s);
 // the ICP team's solver step on n systems of 16 accumulators: dx[6], used_schur, est = q(4) t(3), converged

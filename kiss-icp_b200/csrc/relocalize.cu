@@ -6,7 +6,6 @@
 #undef kb
 
 #include <algorithm>
-#include <cstring>
 
 #include "relocalize.cuh"
 
@@ -88,14 +87,15 @@ __global__ void __launch_bounds__(RS_THREADS) k_reloc_score(const RelocScorePara
 
 }  // namespace kb_reloc
 
-cudaError_t reloc_score(const void *map_view, size_t view_bytes, const double *src, int n, const double *rot, int n_yaw,
+cudaError_t relocalize_watchdog(unsigned *d_host_words, const unsigned *init) { return kb_reloc::watchdog_arm(d_host_words, init); }
+
+cudaError_t reloc_score(const kb_types::MapView &m, const double *src, int n, const double *rot, int n_yaw,
                         const double *xs, int nx, const double *ys, int ny, double tz, int *scores, int sms,
                         cudaStream_t s) {
     using namespace kb_reloc;
-    if (view_bytes != sizeof(MapView)) return cudaErrorInvalidValue;
     if (n <= 0 || n_yaw <= 0 || nx <= 0 || ny <= 0) return cudaErrorInvalidValue;
     RelocScoreParams P;
-    std::memcpy(&P.m, map_view, sizeof(MapView));
+    P.m = m;
     P.src = src;
     P.n = n;
     P.rot = rot;

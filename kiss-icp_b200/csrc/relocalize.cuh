@@ -6,10 +6,11 @@
 
 #include <cstddef>
 
-// map_view points to api.cu's MapView (view_bytes = its size; relocalize.cu checks that its own copy has the same
-// layout). Hypothesis h = (k * ny + jj) * nx + ii scores the n source points under rotation rot[9 k ..] (row-major) and
+#include "types.cuh"
+
+// Hypothesis h = (k * ny + jj) * nx + ii scores the n source points under rotation rot[9 k ..] (row-major) and
 // translation (xs[ii], ys[jj], tz): scores[h] = the points whose voxel the map holds. As many CTAs as fit on the
 // device's `sms` multiprocessors at once, at most one per work item.
-cudaError_t reloc_score(const void *map_view, size_t view_bytes, const double *src, int n, const double *rot, int n_yaw,
+cudaError_t reloc_score(const kb_types::MapView &m, const double *src, int n, const double *rot, int n_yaw,
                         const double *xs, int nx, const double *ys, int ny, double tz, int *scores, int sms,
                         cudaStream_t s);

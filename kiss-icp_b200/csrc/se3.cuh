@@ -14,13 +14,16 @@
 #include <cfloat>
 #include <cmath>
 
+#include "types.cuh"
+
 #define KB_HD __host__ __device__ __forceinline__
 
 namespace kb {
 
-struct V3 {
-    double x, y, z;
-};
+using kb_types::Q4;
+using kb_types::SE3;
+using kb_types::V3;
+
 KB_HD V3 operator+(const V3 &a, const V3 &b) { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
 KB_HD V3 operator-(const V3 &a, const V3 &b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
 KB_HD V3 operator*(double s, const V3 &a) { return {s * a.x, s * a.y, s * a.z}; }
@@ -53,14 +56,6 @@ KB_HD V3 correct_kitti_point(const V3 &pt, double sn, double cs) {
               (r20 * pt.x + r21 * pt.y) + r22 * pt.z};
 }
 
-struct Q4 {
-    double x, y, z, w;
-};
-
-struct SE3 {
-    Q4 q;
-    V3 t;
-};
 KB_HD SE3 se3_identity() { return SE3{{0, 0, 0, 1}, {0, 0, 0}}; }
 
 constexpr double kEps = 1e-10;  // Sophus::Constants<double>::epsilon()
