@@ -554,6 +554,27 @@ typedef struct kb_pose_graph_report {
  * poses. */
 int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *o, kb_pose_graph_report *out,
                            double *edge_chi2, double *edge_weight);
+/* The same problem and the same Levenberg-Marquardt as kb_pose_graph_optimize (cost, IRLS weights, exact Jacobians,
+ * right perturbation, lambda schedule, the four stopping rules and their order, fixed nodes returned bit for bit), with
+ * every step solved exactly: (H + lambda diag H) d = -g by P L L^T P^T, the sparse block Cholesky factorization of
+ * kb_pose_graph_marginals applied to the damped system (its symbolic analysis; damping changes only diagonal blocks),
+ * then a forward and a backward block substitution. A pivot that is not positive and finite rejects the step like a
+ * non-finite F (lambda x 10); it is not an error. Each step is one factorization; report.iterations counts them and
+ * report.cg_iterations is 0. max_cg_iterations and cg_tolerance are checked as by kb_pose_graph_optimize and otherwise
+ * ignored.
+ * Where it pays: on graphs with loops, whose edges reach far back in node index, PCG's block-tridiagonal preconditioner
+ * covers little of H and a step takes many PCG iterations; the exact step takes one factorization. On a pure chain PCG
+ * is exact in one iteration and needs fewer grid barriers.
+ * One cooperative launch per call. The results are bit-identical from run to run and for every grid size: the factor
+ * and the solves are formed in a fixed order, and the cost is summed over fixed chunks of edges, then the chunks in
+ * index order. The symbolic analysis stays cached for the graph's size; the numeric factor the call leaves behind is of
+ * the damped system, so the next kb_pose_graph_marginals factors H again at the new poses. kb_debug_pose_graph_ms
+ * times this call's launch as it times kb_pose_graph_optimize's.
+ * Checked before any work, in the order of kb_pose_graph_optimize and with its codes, writing nothing on error; in
+ * addition KB_ERR_INVALID_ARG for a graph whose factorization needs more than 2^30 block updates (as the marginals).
+ * Without a device, KB_ERR_NO_DEVICE after these checks. */
+int kb_pose_graph_optimize_direct(kb_pose_graph *g, const kb_pose_graph_options *o, kb_pose_graph_report *out,
+                                  double *edge_chi2, double *edge_weight);
 
 /* ---- pose graph: marginal covariances -------------------------------------------------------------------------------
  * How well each pose is known, at the graph's current poses (as added, or as the last optimize left them):

@@ -44,7 +44,8 @@ int kb_debug_fast_rcp_dev(const double *x, size_t n, double *out);
 int kb_debug_reloc_score_ms(const kb_registration *reg, float *ms);
 /* time of the last k_place_distance launch of a kb_place_query or kb_place_relocalize on db [ms] (CUDA events) */
 int kb_debug_place_distance_ms(const kb_place_db *db, float *ms);
-/* time of the last kb_pose_graph_optimize launch on g [ms] (CUDA events); KB_ERR_INVALID_ARG before the first */
+/* time of the last kb_pose_graph_optimize or kb_pose_graph_optimize_direct launch on g [ms] (CUDA events);
+ * KB_ERR_INVALID_ARG before the first */
 int kb_debug_pose_graph_ms(const kb_pose_graph *g, float *ms);
 /* host evaluation of the pose graph's Jacobian pieces: Ad(T) of a row-major SE(3) and J_r^-1(x), row-major 6x6 */
 int kb_debug_se3_adjoint(const double T[16], double A[36]);
@@ -55,6 +56,12 @@ int kb_debug_se3_right_jacobian_inverse(const double x[6], double J[36]);
  * p, diagonal included. cap < n_free is KB_ERR_CAPACITY. */
 int kb_debug_pose_graph_symbolic(kb_pose_graph *g, size_t cap, size_t *n_free, size_t *order, long long *parent,
                                  size_t *col_blocks);
+/* the row index of kb_pose_graph_optimize_direct's forward substitution (host-side, needs no device), two-call:
+ * *n_off = the off-diagonal blocks of L; with cap >= n_off, each of col_pairs and row_pairs (long long[n_off][2]) that
+ * is not NULL receives (row, column) positions: col_pairs of L's off-diagonal blocks as L stores them (by column in
+ * the level schedule, rows ascending), row_pairs of the row index's entries in its order (by row, columns ascending;
+ * row -1 where an entry names a block of another row). cap < n_off is KB_ERR_CAPACITY. */
+int kb_debug_pose_graph_rows(kb_pose_graph *g, size_t cap, size_t *n_off, long long *col_pairs, long long *row_pairs);
 /* ms[0]: the last numeric factorization launch of kb_pose_graph_marginals / _joint_marginals on g (0 when every node is
  * fixed), ms[1]: the last marginal solve launch [ms] (CUDA events); KB_ERR_INVALID_ARG before the first */
 int kb_debug_pose_graph_cov_ms(const kb_pose_graph *g, float ms[2]);

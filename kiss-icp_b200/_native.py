@@ -281,6 +281,7 @@ SIGNATURES = {
     "kb_pose_graph_poses": (i32, [vp, vp, sz, C.POINTER(sz)]),
     "kb_pose_graph_options_default": (None, [C.POINTER(PoseGraphOptions)]),
     "kb_pose_graph_optimize": (i32, [vp, C.POINTER(PoseGraphOptions), C.POINTER(PoseGraphReport), vp, vp]),
+    "kb_pose_graph_optimize_direct": (i32, [vp, C.POINTER(PoseGraphOptions), C.POINTER(PoseGraphReport), vp, vp]),
     "kb_debug_pose_graph_ms": (i32, [vp, C.POINTER(C.c_float)]),
     "kb_debug_se3_adjoint": (i32, [vp, vp]),
     "kb_debug_se3_right_jacobian_inverse": (i32, [vp, vp]),
@@ -288,6 +289,7 @@ SIGNATURES = {
     "kb_pose_graph_joint_marginals": (i32, [vp, vp, sz, vp]),
     "kb_pose_graph_factor_info": (i32, [vp, C.POINTER(PoseGraphFactorInfo)]),
     "kb_debug_pose_graph_symbolic": (i32, [vp, sz, C.POINTER(sz), vp, vp, vp]),
+    "kb_debug_pose_graph_rows": (i32, [vp, sz, C.POINTER(sz), vp, vp]),
     "kb_debug_pose_graph_cov_ms": (i32, [vp, vp]),
     "kb_free_space_params_default": (None, [C.POINTER(FreeSpaceParams), dbl]),
     "kb_map_free_space": (i32, [vp, vp, sz, vp, sz, vp, C.POINTER(FreeSpaceParams), vp, vp, vp,

@@ -1,7 +1,8 @@
 // Host side of the pose graph and its marginal covariances (kb_pose_graph_* and their kb_debug_* calls). The kernels
-// are in pose_graph.cu and pose_graph_cov.cu.
+// are in pose_graph.cu, pose_graph_cov.cu and pose_graph_direct.cu.
 #include <algorithm>
 #include <cmath>
+#include <functional>
 #include <memory>
 #include <numeric>
 #include <vector>
@@ -44,8 +45,10 @@ struct kb_pose_graph {
     int sym_dev_n = -1, sym_dev_e = -1;  // the graph the device copy of `sym` was made for
     bool factored = false;
     DBuf<int> s_order, s_pos, s_parent, s_col_slot, s_lev_ptr, s_colptr, s_brow, s_bcol, s_hptr, s_hedge, s_uptr, s_upd;
+    DBuf<int> s_rptr, s_rblk;
     DBuf<int> cov_flag, cov_req, cov_path;
     DBuf<double> Lx, cov_X, cov_out;
+    DBuf<double> dir_val, dir_chunk;  // kb_pose_graph_optimize_direct: per edge and node values, their chunk partials
     Event cev[4];                    // around the last factorization and the last marginal solves (kb_debug_pose_graph_cov_ms)
     size_t n() const { return fixed.size(); }
     size_t m() const { return robust.size(); }
@@ -203,6 +206,63 @@ static int pg_upload(kb_pose_graph *g, std::vector<double> *pq_out, PoseGraphPar
     return KB_OK;
 }
 
+// the options of an optimize call, checked; the defaults for NULL
+static int pg_options(const kb_pose_graph_options *opt, kb_pose_graph_options *o) {
+    kb_pose_graph_options_default(o);
+    if (opt) *o = *opt;
+    return pg_options_check(*o);
+}
+static void pg_set_options(const kb_pose_graph_options &o, PoseGraphParams *P) {
+    P->max_iterations = o.max_iterations;
+    P->max_cg_iterations = o.max_cg_iterations;
+    P->function_tolerance = o.function_tolerance;
+    P->parameter_tolerance = o.parameter_tolerance;
+    P->initial_lambda = o.initial_lambda;
+    P->cg_tolerance = o.cg_tolerance;
+}
+
+// CTAs of an optimizer launch: one per PB items (nodes, edges, blocks of L), within kb_set_grid_blocks, the SMs and
+// the kernel's co-resident CTAs
+static int pg_grid(const Exec &ex, int co_resident, size_t items, int PB) {
+    const int cap = std::min(tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : ex.sms, co_resident);
+    return static_cast<int>(std::max<size_t>(1, std::min<size_t>((std::max<size_t>(items, 1) + PB - 1) / PB, cap)));
+}
+
+// One optimizer launch between the graph's events (kb_debug_pose_graph_ms), then its result: the report, the free
+// nodes' poses (pq: the poses as uploaded) and s_e, w_e. Nothing is written to the caller's buffers on error.
+static int pg_run(kb_pose_graph *g, std::vector<double> &pq, const std::function<cudaError_t(cudaStream_t)> &launch,
+                  kb_pose_graph_report *out, double *edge_chi2, double *edge_weight) {
+    Exec &ex = *g->ex;
+    const size_t N = g->n(), E = g->m();
+    cudaStream_t s = ex.stream;
+    RET(events_on(g->ev, ex.device));
+    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
+    ex.bar_dirty = true;
+    g->factored = false;  // (the poses move)
+    CK(cudaEventRecord(g->ev[0].p, s));
+    CK(launch(s));
+    ++ex.launches;
+    CK(cudaEventRecord(g->ev[1].p, s));
+    kb_pose_graph_report rep{};
+    CK(cudaMemcpyAsync(&rep, g->report.p, sizeof(rep), cudaMemcpyDeviceToHost, s));
+    if (N) CK(cudaMemcpyAsync(pq.data(), g->pose_d.p, 8 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
+    std::vector<double> chi2(edge_chi2 ? E : 0), weight(edge_weight ? E : 0);
+    if (edge_chi2 && E) CK(cudaMemcpyAsync(chi2.data(), g->e_s.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (edge_weight && E) CK(cudaMemcpyAsync(weight.data(), g->e_w.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
+    RET(ex.sync());
+    g->uploaded = E;
+    for (size_t k = 0; k < N; ++k) {
+        if (g->fixed[k]) continue;
+        const double *v = &pq[8 * k];
+        g->pose[k] = SE3{{v[0], v[1], v[2], v[3]}, {v[4], v[5], v[6]}};
+        se3_to_matrix(g->pose[k], &g->mat[16 * k]);
+    }
+    *out = rep;
+    std::copy(chi2.begin(), chi2.end(), edge_chi2 ? edge_chi2 : chi2.data());
+    std::copy(weight.begin(), weight.end(), edge_weight ? edge_weight : weight.data());
+    return KB_OK;
+}
+
 void kb_pose_graph_options_default(kb_pose_graph_options *o) {
     if (o) *o = kb_pose_graph_options{100, 1e-12, 1e-10, 1e-4, 100, 1e-10};
 }
@@ -285,57 +345,80 @@ int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, k
                            double *edge_weight) {
     if (!g || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     kb_pose_graph_options o;
-    kb_pose_graph_options_default(&o);
-    if (opt) o = *opt;
-    RET(pg_options_check(o));
+    RET(pg_options(opt, &o));
     RET(pg_gauge_check(*g));
     RET(require_device());
     if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
     Exec &ex = *g->ex;
     CK(cudaSetDevice(ex.device));
-    const size_t N = g->n(), E = g->m();
     int co_resident = 0;
     CK(pose_graph_max_grid(ex.sms, &co_resident));
-    const int cap = std::min(tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : ex.sms, co_resident);
-    const size_t items = std::max<size_t>(std::max(N, E), 1);
-    const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>((items + POSE_GRAPH_BLOCK - 1) / POSE_GRAPH_BLOCK, cap)));
+    const int grid = pg_grid(ex, co_resident, std::max(g->n(), g->m()), POSE_GRAPH_BLOCK);
     RET(pg_reserve(g, grid));
     std::vector<double> pq;
     PoseGraphParams P;
     RET(pg_upload(g, &pq, &P));
-    cudaStream_t s = ex.stream;
-    P.max_iterations = o.max_iterations;
-    P.max_cg_iterations = o.max_cg_iterations;
-    P.function_tolerance = o.function_tolerance;
-    P.parameter_tolerance = o.parameter_tolerance;
-    P.initial_lambda = o.initial_lambda;
-    P.cg_tolerance = o.cg_tolerance;
-    RET(events_on(g->ev, ex.device));
-    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
-    ex.bar_dirty = true;
-    g->factored = false;  // (the poses move)
-    CK(cudaEventRecord(g->ev[0].p, s));
-    CK(pose_graph_launch(P, grid, s));
-    ++ex.launches;
-    CK(cudaEventRecord(g->ev[1].p, s));
-    kb_pose_graph_report rep{};
-    CK(cudaMemcpyAsync(&rep, g->report.p, sizeof(rep), cudaMemcpyDeviceToHost, s));
-    if (N) CK(cudaMemcpyAsync(pq.data(), g->pose_d.p, 8 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
-    std::vector<double> chi2(edge_chi2 ? E : 0), weight(edge_weight ? E : 0);
-    if (edge_chi2 && E) CK(cudaMemcpyAsync(chi2.data(), g->e_s.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
-    if (edge_weight && E) CK(cudaMemcpyAsync(weight.data(), g->e_w.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
-    RET(ex.sync());
-    g->uploaded = E;
-    for (size_t k = 0; k < N; ++k) {
-        if (g->fixed[k]) continue;
-        const double *v = &pq[8 * k];
-        g->pose[k] = SE3{{v[0], v[1], v[2], v[3]}, {v[4], v[5], v[6]}};
-        se3_to_matrix(g->pose[k], &g->mat[16 * k]);
-    }
-    *out = rep;
-    std::copy(chi2.begin(), chi2.end(), edge_chi2 ? edge_chi2 : chi2.data());
-    std::copy(weight.begin(), weight.end(), edge_weight ? edge_weight : weight.data());
-    return KB_OK;
+    pg_set_options(o, &P);
+    return pg_run(g, pq, [&](cudaStream_t s) { return pose_graph_launch(P, grid, s); }, out, edge_chi2, edge_weight);
+}
+
+static int pg_symbolic(kb_pose_graph *g);
+static int pg_sym_upload(kb_pose_graph *g);
+
+int kb_pose_graph_optimize_direct(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_pose_graph_report *out,
+                                  double *edge_chi2, double *edge_weight) {
+    if (!g || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    kb_pose_graph_options o;
+    RET(pg_options(opt, &o));
+    RET(pg_gauge_check(*g));
+    RET(pg_symbolic(g));  // (refuses a graph whose factorization needs more than 2^30 block updates)
+    RET(require_device());
+    if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
+    Exec &ex = *g->ex;
+    CK(cudaSetDevice(ex.device));
+    const PgcSymbolic &S = g->sym;
+    const size_t N = g->n(), E = g->m();
+    int co_resident = 0;
+    CK(pgc_optimize_max_grid(ex.sms, &co_resident));
+    const int grid = pg_grid(ex, co_resident, std::max({N, E, S.blocks()}), PGC_BLOCK);
+    RET(pg_reserve(g, grid));
+    PgcOptimizeParams O{};
+    std::vector<double> pq;
+    RET(pg_upload(g, &pq, &O.F.P));
+    pg_set_options(o, &O.F.P);
+    RET(pg_sym_upload(g));
+    const size_t V = std::max({N, E, size_t(1)});
+    RET(g->Lx.ensure(std::max<size_t>(36 * S.blocks(), 1)));
+    RET(g->cov_flag.ensure(1));
+    RET(g->dir_val.ensure(2 * V));
+    RET(g->dir_chunk.ensure(2 * ((V + PGC_CHUNK - 1) / PGC_CHUNK)));
+    CK(cudaMemsetAsync(g->cov_flag.p, 0, sizeof(int), ex.stream));
+    PgcFactorParams &F = O.F;
+    F.nf = S.nf;
+    F.levels = S.levels();
+    F.n_blocks = static_cast<int>(S.blocks());
+    F.order = g->s_order.p;
+    F.lev_ptr = g->s_lev_ptr.p;
+    F.colptr = g->s_colptr.p;
+    F.brow = g->s_brow.p;
+    F.bcol = g->s_bcol.p;
+    F.hptr = g->s_hptr.p;
+    F.hedge = g->s_hedge.p;
+    F.uptr = g->s_uptr.p;
+    F.upd = g->s_upd.p;
+    F.Lx = g->Lx.p;
+    F.flag = g->cov_flag.p;
+    O.Fd = F;
+    O.Fd.P.hd = F.P.D;
+    O.rptr = g->s_rptr.p;
+    O.rblk = g->s_rblk.p;
+    O.pos = g->s_pos.p;
+    O.y = F.P.x;  // (6 N doubles of the PCG vectors: nf <= N)
+    O.val = g->dir_val.p;
+    O.chunk = g->dir_chunk.p;
+    O.stride = static_cast<int>(V);
+    // (Lx now holds the damped system's factor: the marginals factor H again)
+    return pg_run(g, pq, [&](cudaStream_t s) { return pgc_optimize_launch(O, grid, s); }, out, edge_chi2, edge_weight);
 }
 
 int kb_debug_pose_graph_ms(const kb_pose_graph *g, float *ms) {
@@ -389,6 +472,30 @@ static int pg_put(DBuf<int> &d, const std::vector<int> &h, cudaStream_t s) {
     return KB_OK;
 }
 
+// the device copy of the symbolic analysis, uploaded once per analysis (on the graph's stream)
+static int pg_sym_upload(kb_pose_graph *g) {
+    const PgcSymbolic &S = g->sym;
+    if (g->sym_dev_n == S.n_nodes && g->sym_dev_e == S.n_edges) return KB_OK;
+    cudaStream_t s = g->ex->stream;
+    RET(pg_put(g->s_order, S.order, s));
+    RET(pg_put(g->s_pos, S.pos, s));
+    RET(pg_put(g->s_parent, S.parent, s));
+    RET(pg_put(g->s_col_slot, S.col_slot, s));
+    RET(pg_put(g->s_lev_ptr, S.lev_ptr, s));
+    RET(pg_put(g->s_colptr, S.colptr, s));
+    RET(pg_put(g->s_brow, S.brow, s));
+    RET(pg_put(g->s_bcol, S.bcol, s));
+    RET(pg_put(g->s_hptr, S.hptr, s));
+    RET(pg_put(g->s_hedge, S.hedge, s));
+    RET(pg_put(g->s_uptr, S.uptr, s));
+    RET(pg_put(g->s_upd, S.upd, s));
+    RET(pg_put(g->s_rptr, S.rptr, s));
+    RET(pg_put(g->s_rblk, S.rblk, s));
+    g->sym_dev_n = S.n_nodes;
+    g->sym_dev_e = S.n_edges;
+    return KB_OK;
+}
+
 // the numeric factor of H at the current poses (one cooperative launch), unless the cached one is still valid
 static int pg_factor(kb_pose_graph *g) {
     RET(pg_symbolic(g));
@@ -403,30 +510,13 @@ static int pg_factor(kb_pose_graph *g) {
     }
     int co_resident = 0;
     CK(pgc_factor_max_grid(ex.sms, &co_resident));
-    const int cap = std::min(tl_grid_blocks > 0 ? std::min(tl_grid_blocks, ex.sms) : ex.sms, co_resident);
-    const size_t items = std::max({g->n(), g->m(), S.blocks(), size_t(1)});
-    const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>((items + PGC_BLOCK - 1) / PGC_BLOCK, cap)));
+    const int grid = pg_grid(ex, co_resident, std::max({g->n(), g->m(), S.blocks()}), PGC_BLOCK);
     RET(pg_reserve(g, grid));
     std::vector<double> pq;
     PgcFactorParams F{};
     RET(pg_upload(g, &pq, &F.P));
     cudaStream_t s = ex.stream;
-    if (g->sym_dev_n != S.n_nodes || g->sym_dev_e != S.n_edges) {
-        RET(pg_put(g->s_order, S.order, s));
-        RET(pg_put(g->s_pos, S.pos, s));
-        RET(pg_put(g->s_parent, S.parent, s));
-        RET(pg_put(g->s_col_slot, S.col_slot, s));
-        RET(pg_put(g->s_lev_ptr, S.lev_ptr, s));
-        RET(pg_put(g->s_colptr, S.colptr, s));
-        RET(pg_put(g->s_brow, S.brow, s));
-        RET(pg_put(g->s_bcol, S.bcol, s));
-        RET(pg_put(g->s_hptr, S.hptr, s));
-        RET(pg_put(g->s_hedge, S.hedge, s));
-        RET(pg_put(g->s_uptr, S.uptr, s));
-        RET(pg_put(g->s_upd, S.upd, s));
-        g->sym_dev_n = S.n_nodes;
-        g->sym_dev_e = S.n_edges;
-    }
+    RET(pg_sym_upload(g));
     RET(g->Lx.ensure(36 * S.blocks()));
     RET(g->cov_flag.ensure(1));
     CK(cudaMemsetAsync(g->cov_flag.p, 0, sizeof(int), s));
@@ -552,6 +642,32 @@ int kb_debug_pose_graph_symbolic(kb_pose_graph *g, size_t cap, size_t *n_free, s
         if (parent) parent[p] = S.parent[p];
         if (col_blocks) col_blocks[p] = static_cast<size_t>(S.colptr[S.col_slot[p] + 1] - S.colptr[S.col_slot[p]]);
     }
+    return KB_OK;
+}
+int kb_debug_pose_graph_rows(kb_pose_graph *g, size_t cap, size_t *n_off, long long *col_pairs, long long *row_pairs) {
+    if (!g || !n_off) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(pg_symbolic(g));
+    const PgcSymbolic &S = g->sym;
+    const size_t n = S.rblk.size();
+    *n_off = n;
+    if (!col_pairs && !row_pairs) return KB_OK;
+    if (cap < n) return fail(KB_ERR_CAPACITY, "buffer too small (%zu < %zu off-diagonal blocks)", cap, n);
+    if (col_pairs) {
+        size_t t = 0;
+        for (size_t b = 0; b < S.blocks(); ++b)
+            if (S.brow[b] != S.bcol[b]) {
+                col_pairs[2 * t] = S.brow[b];
+                col_pairs[2 * t + 1] = S.bcol[b];
+                ++t;
+            }
+    }
+    if (row_pairs)
+        for (int j = 0; j < S.nf; ++j)
+            for (int t = S.rptr[j]; t < S.rptr[j + 1]; ++t) {
+                const int b = S.rblk[t];
+                row_pairs[2 * t] = S.brow[b] == j ? j : -1;  // (-1: the block is not in the row it is listed in)
+                row_pairs[2 * t + 1] = S.bcol[b];
+            }
     return KB_OK;
 }
 int kb_debug_pose_graph_cov_ms(const kb_pose_graph *g, float ms[2]) {

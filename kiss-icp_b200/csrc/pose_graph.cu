@@ -22,17 +22,6 @@ constexpr int PB = POSE_GRAPH_BLOCK;
 
 #include "pose_graph_edges.cuh"
 
-__device__ __forceinline__ void st_pose(double *p, const SE3 &T) {
-    p[0] = T.q.x;
-    p[1] = T.q.y;
-    p[2] = T.q.z;
-    p[3] = T.q.w;
-    p[4] = T.t.x;
-    p[5] = T.t.y;
-    p[6] = T.t.z;
-    p[7] = 0.0;
-}
-
 struct Red {
     double *part;  // [2][2][grid]
     int seq;       // which half the next reduction uses (the same in every thread)

@@ -4,7 +4,9 @@
 // one persistent cooperative launch on the Grid barrier of device_ops.cuh, the marginals one ordinary launch.
 //
 // A translation unit of its own, with its own copies of the watchdog's words (armed by host.cu), so that the
-// optimizer's kernel compiles exactly as before (DESIGN §4.6); the device code both need is pose_graph_edges.cuh.
+// optimizer's kernel compiles exactly as before (DESIGN §4.6); the device code both need is pose_graph_edges.cuh. The
+// factorization's device functions are pose_graph_factor.cuh, which the exact-step optimizer (pose_graph_direct.cu)
+// compiles too.
 //
 // Determinism: every value is formed by one thread in a fixed order (a block's updates in ascending column order, a
 // marginal's sum in path order), so the factor and the covariances are bit-identical from run to run and for every
@@ -73,6 +75,7 @@ void pgc_symbolic(int N, const int *fixed, int E, const int *ij, PgcSymbolic *S)
         S->colptr.assign(1, 0);
         S->hptr.assign(1, 0);
         S->uptr.assign(1, 0);
+        S->rptr.assign(1, 0);
         return;
     }
     // the block graph of the free nodes
@@ -271,6 +274,19 @@ void pgc_symbolic(int N, const int *fixed, int E, const int *ij, PgcSymbolic *S)
             S->bcol[b] = j;
         }
     }
+    // the row index (the transpose of the column structure): row j's blocks L_jk, k < j, by ascending k
+    S->rptr.assign(nf + 1, 0);
+    for (int b = 0; b < nb; ++b)
+        if (S->brow[b] != S->bcol[b]) ++S->rptr[S->brow[b] + 1];
+    for (int j = 0; j < nf; ++j) S->rptr[j + 1] += S->rptr[j];
+    S->rblk.resize(S->rptr[nf]);
+    {
+        std::vector<int> at(S->rptr.begin(), S->rptr.end() - 1);
+        for (int k = 0; k < nf; ++k) {
+            const int s = S->col_slot[k];
+            for (int b = S->colptr[s] + 1; b < S->colptr[s + 1]; ++b) S->rblk[at[S->brow[b]]++] = b;
+        }
+    }
     // the block (i, j), i >= j, of L (it exists for every pair this is asked for)
     auto find = [&](int i, int j) {
         const int s = S->col_slot[j];
@@ -333,119 +349,7 @@ void pgc_symbolic(int N, const int *fixed, int E, const int *ij, PgcSymbolic *S)
 namespace kb_pgc {
 
 #include "pose_graph_edges.cuh"
-
-// H's block b: a node's diagonal block as assemble_node left it, or the sum over the edges between the two nodes of
-// At W B = -Ad^T Ejj (the row is the edge's i) or (At W B)^T = -Ejj Ad, in ascending edge order (assemble_node's
-// formula for the chain's blocks)
-__device__ __noinline__ void gather_block(const PgcFactorParams &F, int b) {
-    double *X = F.Lx + 36 * static_cast<size_t>(b);
-    const int i = F.brow[b], j = F.bcol[b];
-    if (i == j) {
-        const double *Hd = F.P.hd + 36 * static_cast<size_t>(F.order[j]);
-#pragma unroll 6
-        for (int a = 0; a < 36; ++a) X[a] = Hd[a];
-        return;
-    }
-    const int ni = F.order[i];
-    double U[36];
-#pragma unroll
-    for (int a = 0; a < 36; ++a) U[a] = 0.0;
-    for (int t = F.hptr[b]; t < F.hptr[b + 1]; ++t) {
-        const int e = F.hedge[t];
-        const bool row_is_i = F.P.ij[2 * e] == ni;
-        const double *Ejj = F.P.e_jj + 36 * static_cast<size_t>(e), *Ad = F.P.e_ad + 36 * static_cast<size_t>(e);
-#pragma unroll 1
-        for (int a = 0; a < 6; ++a)
-#pragma unroll
-            for (int c = 0; c < 6; ++c) {
-                double s = 0.0;
-                if (row_is_i) {
-#pragma unroll
-                    for (int m = 0; m < 6; ++m) s = s + Ad[6 * m + a] * Ejj[6 * m + c];
-                } else {
-#pragma unroll
-                    for (int m = 0; m < 6; ++m) s = s + Ejj[6 * a + m] * Ad[6 * m + c];
-                }
-                U[6 * a + c] = U[6 * a + c] - s;
-            }
-    }
-#pragma unroll
-    for (int a = 0; a < 36; ++a) X[a] = U[a];
-}
-
-// A'_ij = A_ij - sum_k L_ik L_jk^T over the block's update list, in list order (ascending k)
-__device__ __noinline__ void update_block(const PgcFactorParams &F, int b) {
-    double X[36];
-    double *dst = F.Lx + 36 * static_cast<size_t>(b);
-#pragma unroll
-    for (int a = 0; a < 36; ++a) X[a] = dst[a];
-    for (int t = F.uptr[b]; t < F.uptr[b + 1]; ++t) {
-        const double *Li = F.Lx + 36 * static_cast<size_t>(F.upd[2 * t]);
-        const double *Lj = F.Lx + 36 * static_cast<size_t>(F.upd[2 * t + 1]);
-#pragma unroll 1
-        for (int a = 0; a < 6; ++a) {
-            double li[6];
-#pragma unroll
-            for (int m = 0; m < 6; ++m) li[m] = Li[6 * a + m];
-#pragma unroll
-            for (int c = 0; c < 6; ++c) {
-                double s = 0.0;
-#pragma unroll
-                for (int m = 0; m < 6; ++m) s = s + li[m] * Lj[6 * c + m];
-                X[6 * a + c] = X[6 * a + c] - s;
-            }
-        }
-    }
-#pragma unroll
-    for (int a = 0; a < 36; ++a) dst[a] = X[a];
-}
-
-// the column of slot s: L_jj = chol(A'_jj) (lower, zeros above), then L_ij = A'_ij L_jj^-T for its other blocks
-__device__ __noinline__ void factor_column(const PgcFactorParams &F, int s) {
-    const int b0 = F.colptr[s];
-    double *D = F.Lx + 36 * static_cast<size_t>(b0);
-    double L[36];
-#pragma unroll
-    for (int a = 0; a < 36; ++a) L[a] = D[a];
-    bool ok = true;
-#pragma unroll
-    for (int j = 0; j < 6; ++j) {
-        double d = L[7 * j];
-#pragma unroll
-        for (int k = 0; k < j; ++k) d = d - L[6 * j + k] * L[6 * j + k];
-        ok = ok && d > 0.0 && d < INFINITY;
-        const double l = sqrt(fmax(d, 1e-300));
-        L[7 * j] = l;
-#pragma unroll
-        for (int i = j + 1; i < 6; ++i) {
-            double v = L[6 * i + j];
-#pragma unroll
-            for (int k = 0; k < j; ++k) v = v - L[6 * i + k] * L[6 * j + k];
-            L[6 * i + j] = v / l;
-        }
-#pragma unroll
-        for (int i = 0; i < j; ++i) L[6 * i + j] = 0.0;
-    }
-    if (!ok) *F.flag = 1;
-#pragma unroll
-    for (int a = 0; a < 36; ++a) D[a] = L[a];
-    for (int b = b0 + 1; b < F.colptr[s + 1]; ++b) {
-        double *X = F.Lx + 36 * static_cast<size_t>(b);
-#pragma unroll 1
-        for (int a = 0; a < 6; ++a) {  // row a: x L^T = row, forward substitution
-            double x[6];
-#pragma unroll
-            for (int c = 0; c < 6; ++c) {
-                double v = X[6 * a + c];
-#pragma unroll
-                for (int k = 0; k < c; ++k) v = v - L[6 * c + k] * x[k];
-                x[c] = v / L[7 * c];
-            }
-#pragma unroll
-            for (int c = 0; c < 6; ++c) X[6 * a + c] = x[c];
-        }
-    }
-}
+#include "pose_graph_factor.cuh"
 
 // Linearize every edge at the current poses, assemble H's blocks (lambda 0), then the levels of the elimination tree
 // from the leaves up: every block of the level's columns takes its updates, then every column its pivot and solves.

@@ -25,6 +25,7 @@ struct PgcSymbolic {
     std::vector<int> brow, bcol;     // [blocks] row and column position of each block
     std::vector<int> hptr, hedge;    // [blocks + 1], edges between the two nodes of an off-diagonal block, ascending
     std::vector<int> uptr, upd;      // [blocks + 1], [2 updates]: (block of L_ik, block of L_jk), k ascending
+    std::vector<int> rptr, rblk;     // [nf + 1], [off-diagonal blocks]: the row index, the blocks L_jk of row j, k ascending
     size_t h_blocks = 0;             // blocks of H's lower triangle (diagonal included)
     double flops = 0.0;              // of one numeric factorization (2 * 6^3 per update, 6^3 per solve, 6^3 / 3 per pivot)
     int levels() const { return static_cast<int>(lev_ptr.size()) - 1; }
@@ -51,9 +52,24 @@ struct PgcMarginalParams {
     int *path;           // [groups][2][max_path] their positions
     double *out;
 };
+// One kb_pose_graph_optimize_direct call: Levenberg-Marquardt with the step solved exactly through the factorization
+// of the damped system (pose_graph_direct.cu, k_pgc_optimize).
+struct PgcOptimizeParams {
+    PgcFactorParams F;   // F.P: the graph, its workspace and the options; F.flag: a pivot of this step was not positive
+    PgcFactorParams Fd;  // the same, but Fd.P.hd = F.P.D: the damped diagonal blocks are what gather_block reads
+    const int *rptr, *rblk;  // the row index (PgcSymbolic)
+    const int *pos;          // [N] the position of each node (-1: fixed)
+    double *y;               // [nf][6] by position: -g, then L^-1 P^T (-g), then the step
+    double *val;             // [2][V] per edge rho(s_e), per node max |step| (V = max(N, E, 1))
+    double *chunk;           // [2][ceil(V / PGC_CHUNK)] their sums and maxima over fixed chunks
+    int stride;              // V
+};
 constexpr int PGC_BLOCK = 256;       // threads per CTA of the factorization
 constexpr int PGC_SOLVE_BLOCK = 128;  // threads per CTA of the marginal solves: 16 groups of 8 lanes, 6 of them busy
 constexpr int PGC_GROUPS = PGC_SOLVE_BLOCK / 8;
+constexpr int PGC_CHUNK = 1024;       // items per partial of the optimizer's cost and step: one warp, 32 per lane
 cudaError_t pgc_factor_max_grid(int sms, int *out);
 cudaError_t pgc_factor_launch(const PgcFactorParams &P, int grid, cudaStream_t s);
 cudaError_t pgc_marginals_launch(const PgcMarginalParams &P, int grid, cudaStream_t s);
+cudaError_t pgc_optimize_max_grid(int sms, int *out);
+cudaError_t pgc_optimize_launch(const PgcOptimizeParams &P, int grid, cudaStream_t s);

@@ -1,9 +1,20 @@
-// Device code of the pose graph that both the optimizer (pose_graph.cu) and the covariance (pose_graph_cov.cu) run: the
-// pose layout, the 6x6 helpers, one edge's linearization and the gather of a node's diagonal block. Each unit includes
-// this inside its own namespace, after device_ops.cuh, so each module has its own copies (DESIGN §4.6: a kernel of one
-// unit changes no code generated for another's).
+// Device code of the pose graph that both optimizers (pose_graph.cu, pose_graph_direct.cu) and the covariance
+// (pose_graph_cov.cu) run: the pose layout, the 6x6 helpers, one edge's linearization and the gather of a node's
+// diagonal block. Each unit includes this inside its own namespace, after device_ops.cuh, so each module has its own
+// copies (DESIGN §4.6: a kernel of one unit changes no code generated for another's).
 
 __device__ __forceinline__ SE3 ld_pose(const double *p) { return SE3{{p[0], p[1], p[2], p[3]}, {p[4], p[5], p[6]}}; }
+
+__device__ __forceinline__ void st_pose(double *p, const SE3 &T) {
+    p[0] = T.q.x;
+    p[1] = T.q.y;
+    p[2] = T.q.z;
+    p[3] = T.q.w;
+    p[4] = T.t.x;
+    p[5] = T.t.y;
+    p[6] = T.t.z;
+    p[7] = 0.0;
+}
 
 // y = A v, A^T v, A 6x6 row-major
 __device__ __forceinline__ void mv6(const double *A, const double v[6], double y[6]) {

@@ -166,7 +166,8 @@ class LoopCloser:
         return loop
 
     def optimize(self, options: PoseGraphOptions | None = None) -> PoseGraphReport:
-        """optimize the keyframe graph from its current poses (PoseGraph.optimize)"""
+        """optimize the keyframe graph from its current poses (PoseGraph.optimize; options.linear_solver="cholesky"
+        solves every step exactly, which pays on graphs with loops)"""
         return self._graph.optimize(options)
 
     # -- corrected products -----------------------------------------------------------------------------------------

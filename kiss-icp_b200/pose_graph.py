@@ -3,8 +3,9 @@ problem, the method and every rule).
 
 No reference counterpart. Nodes are poses, some of them fixed; an edge (i, j, Z, Omega, c) asks T_i^-1 T_j to equal Z,
 with the information Omega (6x6, tangent order translation then rotation) and an optional Cauchy scale c. optimize()
-runs Levenberg-Marquardt on the device, in one launch, and leaves the result in ``poses``; nodes and edges may be
-added afterwards and optimize() called again (the online use of loop closure: loop_closure.LoopCloser).
+runs Levenberg-Marquardt on the device, in one launch, and leaves the result in ``poses``; each step is solved by PCG
+or, with PoseGraphOptions(linear_solver="cholesky"), exactly by a sparse block Cholesky factorization. Nodes and edges
+may be added afterwards and optimize() called again (the online use of loop closure: loop_closure.LoopCloser).
 marginal_covariances() and joint_marginal_covariances() say how well the poses are known: blocks of H^-1 at the
 current poses, from a sparse block Cholesky factorization on the device.
 """
@@ -20,19 +21,30 @@ from . import _native as N
 from .mapping import check_value
 
 TERMINATIONS = ("function_tolerance", "parameter_tolerance", "max_iterations", "no_decrease")
+LINEAR_SOLVERS = {"pcg": "kb_pose_graph_optimize", "cholesky": "kb_pose_graph_optimize_direct"}
 
 
 @dataclass
 class PoseGraphOptions:
     """kb_pose_graph_options: max_iterations [0, 10^6] (LM steps, accepted and rejected), function_tolerance >= 0,
     parameter_tolerance >= 0 (of max |step|), initial_lambda (0, 1e12], max_cg_iterations [1, 10^6] (per step),
-    cg_tolerance [0, 1) (of |r| / |g|)"""
+    cg_tolerance [0, 1) (of |r| / |g|); and how each step is solved, linear_solver: "pcg" (kb_pose_graph_optimize:
+    PCG with a block-tridiagonal preconditioner, exact in one iteration on a chain) or "cholesky"
+    (kb_pose_graph_optimize_direct: the sparse block Cholesky factorization of the damped system, exact on any graph;
+    max_cg_iterations and cg_tolerance are checked but unused). Not part of the C struct."""
     max_iterations: int = 100
     function_tolerance: float = 1e-12
     parameter_tolerance: float = 1e-10
     initial_lambda: float = 1e-4
     max_cg_iterations: int = 100
     cg_tolerance: float = 1e-10
+    linear_solver: str = "pcg"
+
+    def _solver(self):
+        """the C entry point of linear_solver"""
+        if self.linear_solver not in LINEAR_SOLVERS:
+            raise ValueError(f"linear_solver = {self.linear_solver!r}: one of {LINEAR_SOLVERS}")
+        return LINEAR_SOLVERS[self.linear_solver]
 
     def _struct(self):
         o = N.PoseGraphOptions()
@@ -48,7 +60,8 @@ class PoseGraphOptions:
 
 @dataclass
 class PoseGraphReport:
-    """iterations: LM steps (accepted and rejected); accepted; cg_iterations: PCG iterations in all; termination: one of
+    """iterations: LM steps (accepted and rejected); accepted; cg_iterations: PCG iterations in all (0 with
+    linear_solver "cholesky", whose every step is one factorization); termination: one of
     TERMINATIONS; initial_cost / final_cost: F = 1/2 sum rho(s_e) at the start and at the returned poses; lambda_: the
     last damping. chi2 / weight: every edge's s_e and w_e at the returned poses (optimize(return_edges=True))."""
     iterations: int
@@ -165,16 +178,17 @@ class PoseGraph:
         return out
 
     def optimize(self, options: PoseGraphOptions | None = None, return_edges: bool = False) -> PoseGraphReport:
-        """optimize the free nodes from their current poses. ValueError for a rejected argument (among them a free
-        node that no path of edges connects to a fixed node)."""
-        o = (PoseGraphOptions() if options is None else options)._struct()
+        """optimize the free nodes from their current poses, each step solved as options.linear_solver says.
+        ValueError for a rejected argument (among them a free node that no path of edges connects to a fixed node)."""
+        options = PoseGraphOptions() if options is None else options
+        solve = getattr(N.lib(), options._solver())
+        o = options._struct()
         r = N.PoseGraphReport()
         m = self.n_edges
         chi2 = np.empty(m) if return_edges else None
         weight = np.empty(m) if return_edges else None
-        check_value(N.lib().kb_pose_graph_optimize(self._h, C.byref(o), C.byref(r),
-                                                   N.ptr(chi2) if chi2 is not None else None,
-                                                   N.ptr(weight) if weight is not None else None))
+        check_value(solve(self._h, C.byref(o), C.byref(r), N.ptr(chi2) if chi2 is not None else None,
+                          N.ptr(weight) if weight is not None else None))
         return PoseGraphReport(iterations=r.iterations, accepted=r.accepted, cg_iterations=r.cg_iterations,
                                termination=TERMINATIONS[r.termination], initial_cost=r.initial_cost,
                                final_cost=r.final_cost, lambda_=r.lambda_, chi2=chi2, weight=weight)
@@ -223,7 +237,7 @@ class PoseGraph:
         return float(ms[0]), float(ms[1])
 
     def kernel_ms(self) -> float:
-        """device time of the last optimize() [ms] (CUDA events)"""
+        """device time of the last optimize() [ms] (CUDA events), whichever linear_solver it used"""
         ms = C.c_float(0.0)
         N.check(N.lib().kb_debug_pose_graph_ms(self._h, C.byref(ms)))
         return float(ms.value)
