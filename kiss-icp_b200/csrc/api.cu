@@ -432,6 +432,18 @@ int kb_host::map_in_use(const kb_map *map) {
     return KB_OK;
 }
 
+// The direct entry points take points as the pipeline's crop leaves them: finite, with voxel coordinates that fit in an
+// int after a translation of at most tmax. The pipeline itself keeps accepting any point, as the reference crops it;
+// here the reference would give a NaN point a voxel of its own (floor(NaN) -> INT_MIN on x86) and the device voxel 0.
+static int check_points(const double *xyz, size_t n, double tmax, double voxel_size, const char *what) {
+    double reach;
+    size_t bad;
+    if (!voxel_reach(xyz, n, tmax, voxel_size, &reach, &bad)) return fail(KB_ERR_INVALID_ARG, "%s %zu is not finite", what, bad);
+    if (!(reach < kIntReach)) return fail(KB_ERR_INVALID_ARG, "%ss reach voxel coordinates beyond the int range (%.3g)", what, reach);
+    return KB_OK;
+}
+static double t_norm(const SE3 &T) { return std::sqrt(T.t.x * T.t.x + T.t.y * T.t.y + T.t.z * T.t.z); }
+
 extern "C" {
 
 // ------------------------------------------------------------------------------- VoxelHashMap
@@ -478,6 +490,9 @@ int kb_map_empty(const kb_map *map, int *out_is_empty) {
 int kb_map_update_origin(kb_map *map, const double *xyz, size_t n, const double origin[3]) {
     if (!map || (!xyz && n) || !origin) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     RET(map_in_use(map));
+    if (!std::isfinite(origin[0]) || !std::isfinite(origin[1]) || !std::isfinite(origin[2]))
+        return fail(KB_ERR_INVALID_ARG, "origin is not finite");
+    RET(check_points(xyz, n, 0.0, map->voxel_size, "point"));
     return map->update_host(xyz, n, false, se3_identity(), true, true, V3{origin[0], origin[1], origin[2]});
 }
 int kb_map_update_pose(kb_map *map, const double *xyz, size_t n, const double pose[16]) {
@@ -485,11 +500,13 @@ int kb_map_update_pose(kb_map *map, const double *xyz, size_t n, const double po
     RET(map_in_use(map));
     SE3 T;
     if (!se3_from_matrix(pose, &T)) return fail(KB_ERR_NOT_SE3, "pose is not in SE(3)");
+    RET(check_points(xyz, n, t_norm(T), map->voxel_size, "point"));
     return map->update_host(xyz, n, true, T, true, true, T.t);
 }
 int kb_map_add_points(kb_map *map, const double *xyz, size_t n) {
     if (!map || (!xyz && n)) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     RET(map_in_use(map));
+    RET(check_points(xyz, n, 0.0, map->voxel_size, "point"));
     return map->update_host(xyz, n, false, se3_identity(), true, false, V3{0, 0, 0});
 }
 int kb_map_remove_far(kb_map *map, const double origin[3]) {
@@ -694,6 +711,7 @@ int kb_map_closest_neighbors_dev(const kb_map *cmap, const double *d_queries, si
 int kb_map_closest_neighbors(const kb_map *cmap, const double *queries, size_t n, double *out_points, double *out_dist) {
     kb_map *map = const_cast<kb_map *>(cmap);
     if (!map || (n && (!queries || !out_points || !out_dist))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(check_points(queries, n, 0.0, map->voxel_size, "query"));
     CK(cudaSetDevice(map->ex->device));
     const size_t chunk = size_t(1) << 22;
     for (size_t off = 0; off < n; off += chunk) {
@@ -796,6 +814,7 @@ int kb_registration_align_points_to_map(kb_registration *reg, const double *xyz,
     if (!reg || !map || (!xyz && n) || !initial_guess || !out_pose) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     SE3 g;
     if (!se3_from_matrix(initial_guess, &g)) return fail(KB_ERR_NOT_SE3, "initial_guess is not in SE(3)");
+    RET(check_points(xyz, n, t_norm(g), map->voxel_size, "source point"));
     RET(registration_run(reg, xyz, n, map, g, max_correspondence_distance, kernel_scale, false));
     int it = 0;
     CK(cudaMemcpyAsync(out_pose, reg->out.p, 16 * sizeof(double), cudaMemcpyDeviceToHost, map->ex->stream));
@@ -852,6 +871,7 @@ int kb_registration_build_system(kb_registration *reg, const double *xyz, size_t
                                  int *n_correspondences) {
     kb_map *map = const_cast<kb_map *>(cmap);
     if (!reg || !map || (!xyz && n) || !JTJ || !JTr) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(check_points(xyz, n, 0.0, map->voxel_size, "point"));
     RET(registration_run(reg, xyz, n, map, se3_identity(), max_correspondence_distance, kernel_scale, true));
     double sys[NACC];
     int nc = 0;
@@ -1334,6 +1354,8 @@ int kb_threshold_set_state(kb_threshold *th, double model_sse, int num_samples) 
 int kb_voxel_down_sample(const double *xyz, size_t n, double voxel_size, double *out_xyz, size_t capacity, size_t *n_out) {
     if ((!xyz && n) || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (n >= (size_t(1) << 30)) return fail(KB_ERR_INVALID_ARG, "frame too large");
+    if (!(voxel_size > 0.0) || !std::isfinite(voxel_size)) return fail(KB_ERR_INVALID_ARG, "voxel_size must be finite and > 0");
+    RET(check_points(xyz, n, 0.0, voxel_size, "point"));
     DefaultCtx *c;
     RET(default_ctx(&c));
     Exec &ex = *c->ex;

@@ -426,6 +426,36 @@ struct Shared {
 // `in` is double[n][3], or float[n][3] when in_f32 (KITTI .bin / PointCloud2 payloads are float32; the reference
 // widens them on the host — python/kiss_icp/datasets/kitti.py:66, ros/src/Utils.hpp:198-208 — here the H2D copy
 // is half the size and the exact float->double widening happens on the device)
+// std::minmax_element's scan as libstdc++ states it: the first pair seeds (min, max), then each later pair's smaller
+// element is offered as min and its larger as max, an odd last element to min and else to max. Every test is `<`,
+// which is false on NaN: a leading NaN stays min, a NaN offered as max takes it until a later max candidate does, and
+// an element paired with a NaN is offered to one role only. Serial, for stamps that hold a NaN.
+__device__ __noinline__ void minmax_element_serial(const double *t, int n, double *mn, double *mx) {
+    double lo = t[0], hi = t[0];
+    int i = 1;
+    if (n > 1) {
+        if (t[1] < t[0]) lo = t[1];
+        else hi = t[1];
+        i = 2;
+    }
+    for (; i + 1 < n; i += 2) {
+        const double a = t[i], b = t[i + 1];
+        if (b < a) {
+            if (b < lo) lo = b;
+            if (!(a < hi)) hi = a;
+        } else {
+            if (a < lo) lo = a;
+            if (!(b < hi)) hi = b;
+        }
+    }
+    if (i < n) {
+        if (t[i] < lo) lo = t[i];
+        else if (!(t[i] < hi)) hi = t[i];
+    }
+    *mn = lo;
+    *mx = hi;
+}
+
 __device__ __forceinline__ V3 pre_load(const double *in, long long i, bool in_f32) {
     if (in_f32) {
         const float *f = reinterpret_cast<const float *>(in);
@@ -439,37 +469,47 @@ __device__ __noinline__ void op_preprocess(Grid &g, const Scratch &sc, Shared &s
                               double *tmp, double *out, int *out_n, bool in_f32 = false) {
     const bool do_deskew = deskew && n_ts > 0;
     if (do_deskew) {
-        // std::minmax_element over ALL stamps (Preprocessing.cpp:62-64)
+        // std::minmax_element over ALL stamps (Preprocessing.cpp:62-64): without NaN, the plain min and max. fmin/fmax
+        // skip NaN, so a NaN stamp instead marks its block's max slot with NaN and the scan is repeated in order.
         double mn = DBL_MAX, mx = -DBL_MAX;
+        bool has_nan = false;
         for (int i = static_cast<unsigned>(g.rank) * BLOCK + threadIdx.x; i < n_ts; i += static_cast<unsigned>(g.size) * BLOCK) {
             const double t = ts[i];
             mn = fmin(mn, t);
             mx = fmax(mx, t);
+            has_nan |= isnan(t);
         }
         for (int o = 16; o > 0; o >>= 1) {
             mn = fmin(mn, __shfl_xor_sync(FULL, mn, o));
             mx = fmax(mx, __shfl_xor_sync(FULL, mx, o));
         }
+        if (__any_sync(FULL, has_nan)) mx = __longlong_as_double(0x7ff8000000000000LL);
         if ((threadIdx.x & 31) == 0) {
             sh.warp_d[threadIdx.x >> 5][0] = mn;
             sh.warp_d[threadIdx.x >> 5][1] = mx;
         }
         __syncthreads();
         if (threadIdx.x == 0) {
+            bool marked = isnan(mx);
             for (int w = 1; w < NWARPS; ++w) {
                 mn = fmin(mn, sh.warp_d[w][0]);
                 mx = fmax(mx, sh.warp_d[w][1]);
+                marked |= isnan(sh.warp_d[w][1]);
             }
             sc.blk_d[2 * static_cast<unsigned>(g.rank)] = mn;
-            sc.blk_d[2 * static_cast<unsigned>(g.rank) + 1] = mx;
+            sc.blk_d[2 * static_cast<unsigned>(g.rank) + 1] = marked ? __longlong_as_double(0x7ff8000000000000LL) : mx;
         }
         g.sync();
         if (threadIdx.x == 0) {
             double a = DBL_MAX, b = -DBL_MAX;
+            bool marked = false;
             for (unsigned i = 0; i < static_cast<unsigned>(g.size); ++i) {
                 a = fmin(a, __ldcg(&sc.blk_d[2 * i]));
-                b = fmax(b, __ldcg(&sc.blk_d[2 * i + 1]));
+                const double bi = __ldcg(&sc.blk_d[2 * i + 1]);
+                b = fmax(b, bi);
+                marked |= isnan(bi);
             }
+            if (marked) minmax_element_serial(ts, n_ts, &a, &b);
             sh.mm[0] = a;
             sh.mm[1] = b;
             se3_log(motion, sh.omega);  // relative_motion.log()  (:68)

@@ -59,6 +59,7 @@ KB_HD V3 correct_kitti_point(const V3 &pt, double sn, double cs) {
 KB_HD SE3 se3_identity() { return SE3{{0, 0, 0, 1}, {0, 0, 0}}; }
 
 constexpr double kEps = 1e-10;  // Sophus::Constants<double>::epsilon()
+constexpr double kSchurNoise = 0x1p-42;  // 1024 DBL_EPSILON: icp_solve_schur's floor under cancellation
 
 KB_HD Q4 q_normalized(const Q4 &q) {
     const double len = sqrt(((q.x * q.x + q.y * q.y) + q.z * q.z) + q.w * q.w);
@@ -540,7 +541,14 @@ KB_HD bool icp_solve_schur(const double acc[16], double dx[6]) {
     const double c22 = s00 * s11 - s10 * s10;
     const double det = s00 * c00 + s10 * c01 + s20 * c02;
     const double scale = (fabs(s00) + fabs(s11) + fabs(s22)) * (1.0 / 3.0);
-    if (!(fabs(det) > 1e-9 * scale * scale * scale) || !(scale > 0.0)) return false;
+    // S is C minus terms as large as C. Where they cancel in exact arithmetic (one correspondence, coincident points,
+    // points on one line) what is left is their rounding, ~eps tr(C), and the relative test above compares that noise
+    // with itself. So S, and det S against scale^2, must also stand above kSchurNoise tr(C)/3: 1024 eps, 30x the
+    // rounding measured on 2000 sequentially summed correspondences (DESIGN.md, "Degenerate systems").
+    const double noise = kSchurNoise * (((acc[4] + acc[6]) + acc[9]) * (1.0 / 3.0));
+    if (!(fabs(det) > 1e-9 * scale * scale * scale) || !(scale > 0.0) || !(scale > noise) ||
+        !(fabs(det) > noise * scale * scale))
+        return false;
     const double inv_det = fast_rcp(det);
     const V3 x2{(c00 * b.x + c01 * b.y + c02 * b.z) * inv_det, (c01 * b.x + c11 * b.y + c12 * b.z) * inv_det,
                 (c02 * b.x + c12 * b.y + c22 * b.z) * inv_det};

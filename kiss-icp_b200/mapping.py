@@ -82,19 +82,20 @@ class VoxelHashMap:
 
     def update(self, points: np.ndarray, pose: np.ndarray = np.eye(4)):
         """points + (4,4) pose  -> VoxelHashMap::Update(points, pose)   (VoxelHashMap.cpp:89-95)
-        points + (3,) origin    -> VoxelHashMap::Update(points, origin) (VoxelHashMap.cpp:83-87)"""
+        points + (3,) origin    -> VoxelHashMap::Update(points, origin) (VoxelHashMap.cpp:83-87)
+        ValueError for a non-finite point or origin, or a point whose voxel coordinates do not fit in an int."""
         pts = N.points_arg(points)
         x = np.ascontiguousarray(pose, dtype=np.float64)
         if x.shape == (4, 4):
-            self._mutated(N.lib().kb_map_update_pose(self._h, N.ptr(pts), len(pts), N.ptr(x)))
+            self._mutated(N.lib().kb_map_update_pose(self._h, N.ptr(pts), len(pts), N.ptr(x)), check_value)
         elif x.shape == (3,):
-            self._mutated(N.lib().kb_map_update_origin(self._h, N.ptr(pts), len(pts), N.ptr(x)))
+            self._mutated(N.lib().kb_map_update_origin(self._h, N.ptr(pts), len(pts), N.ptr(x)), check_value)
         else:
             raise TypeError("_update(): incompatible function arguments (pose (4,4) or origin (3,))")
 
     def add_points(self, points):
         pts = N.points_arg(points)
-        self._mutated(N.lib().kb_map_add_points(self._h, N.ptr(pts), len(pts)))
+        self._mutated(N.lib().kb_map_add_points(self._h, N.ptr(pts), len(pts)), check_value)
 
     def remove_far_away_points(self, origin):
         o = np.ascontiguousarray(origin, dtype=np.float64).reshape(3)
@@ -162,9 +163,10 @@ class VoxelHashMap:
         return out, fs
 
     def closest_neighbors(self, queries):
-        """batched VoxelHashMap::GetClosestNeighbor (VoxelHashMap.cpp:46-70)."""
+        """batched VoxelHashMap::GetClosestNeighbor (VoxelHashMap.cpp:46-70). ValueError for a non-finite query or
+        one whose voxel coordinates do not fit in an int."""
         q = N.points_arg(queries)
         outp = np.empty_like(q)
         outd = np.empty(len(q))
-        N.check(N.lib().kb_map_closest_neighbors(self._h, N.ptr(q), len(q), N.ptr(outp), N.ptr(outd)))
+        check_value(N.lib().kb_map_closest_neighbors(self._h, N.ptr(q), len(q), N.ptr(outp), N.ptr(outd)))
         return outp, outd

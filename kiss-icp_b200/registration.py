@@ -9,7 +9,7 @@ import numpy as np
 from . import _native as N
 from .config import KISSConfig
 from .constraints import Constraints, _from_struct
-from .mapping import VoxelHashMap
+from .mapping import VoxelHashMap, check_value
 from .places import PlaceDatabase, PlaceRelocalizationResult, relocalize_in_places
 from .relocalization import RelocalizationResult, RelocalizationSearch, relocalize
 
@@ -74,8 +74,8 @@ class Registration:
         pts = N.points_arg(points)
         g = N.mat4_arg(initial_guess)
         out = np.empty((4, 4))
-        N.check(N.lib().kb_registration_align_points_to_map(self._h, N.ptr(pts), len(pts), voxel_map._h, N.ptr(g),
-                                                            float(max_correspondance_distance), float(kernel), N.ptr(out)))
+        check_value(N.lib().kb_registration_align_points_to_map(self._h, N.ptr(pts), len(pts), voxel_map._h, N.ptr(g),
+                                                                float(max_correspondance_distance), float(kernel), N.ptr(out)))
         return out
 
     def constraints(self, points, voxel_map: VoxelHashMap, pose, max_correspondance_distance: float) -> Constraints:
@@ -199,7 +199,7 @@ class Registration:
         JTJ = np.empty((6, 6))
         JTr = np.empty(6)
         nc = N.i32(0)
-        N.check(N.lib().kb_registration_build_system(self._h, N.ptr(pts), len(pts), voxel_map._h,
-                                                     float(max_correspondance_distance), float(kernel), N.ptr(JTJ),
-                                                     N.ptr(JTr), C.byref(nc)))
+        check_value(N.lib().kb_registration_build_system(self._h, N.ptr(pts), len(pts), voxel_map._h,
+                                                         float(max_correspondance_distance), float(kernel), N.ptr(JTJ),
+                                                         N.ptr(JTr), C.byref(nc)))
         return JTJ, JTr, nc.value
