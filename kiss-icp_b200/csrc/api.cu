@@ -351,20 +351,51 @@ struct kb_pipeline {
     kb_map *map = nullptr;
     // a localizer (kb_pipeline_create_localizer): `map` is the prior map, borrowed and never written
     bool localizer = false;
-    bool fit_reporting = false;  // an odometry pipeline that reports fits (kb_pipeline_set_fit_reporting)
-    // a pipeline that reports fits computes one per frame, into fit_dev[k % Q_DEPTH] (frame k of a call)
-    bool reports_fits() const { return localizer || fit_reporting; }
-    DBuf<double> fit_part;           // [FIT_VALS][grid] per-CTA partials of the fit pass
-    DBuf<FitResult> fit_dev;         // [Q_DEPTH]
-    PinBuf<FitResult> fit_host;      // [Q_DEPTH] copies
-    FitResult last_fit{};
-    // a pipeline that reports fits may also report plane constraints (kb_pipeline_set_constraint_reporting): one result
-    // per frame into plane_dev[k % Q_DEPTH], next to the fit
-    bool constraint_reporting = false;
-    DBuf<double> plane_part;          // [PLANE_VALS][grid] per-CTA partials of the plane pass
-    DBuf<PlaneResult> plane_dev;      // [Q_DEPTH]
-    PinBuf<PlaneResult> plane_host;   // [Q_DEPTH] copies
-    PlaneResult last_planes{};
+    static constexpr int Q_DEPTH = 4;  // frame k registering, k+1 being prefetched by the same launch, k+2 / k+3 copying
+    // one kind of per-frame report (T: FitResult, PlaneResult), reported exactly while its buffers exist: the per-CTA
+    // partials of its pass, frame k's result in dev[k % Q_DEPTH] (frame k of a call), its pinned copy in
+    // host[k % Q_DEPTH] and the last result taken
+    template <class T>
+    struct Report {
+        DBuf<double> part;  // [vals][grid]
+        DBuf<T> dev;
+        PinBuf<T> host;
+        T last{};
+        bool on() const { return dev.p != nullptr; }
+        // on: allocated on ex's device for `vals` values per CTA, the last result all zero (nothing is kept when an
+        // allocation fails); off: released (no launch of the pipeline is in flight between calls)
+        int set(bool enabled, size_t vals, const Exec &ex) {
+            if (enabled && on()) return KB_OK;
+            *this = Report{};
+            if (!enabled) return KB_OK;
+            const int st = [&]() -> int {
+                CK(cudaSetDevice(ex.device));
+                RET(part.ensure(vals * static_cast<size_t>(ex.grid)));
+                CK(dev.alloc(Q_DEPTH));
+                CK(cudaMemsetAsync(dev.p, 0, sizeof(T) * Q_DEPTH, ex.stream));
+                CK(host.alloc(Q_DEPTH));
+                return KB_OK;
+            }();
+            if (st != KB_OK) *this = Report{};
+            return st;
+        }
+        // queue slot s (nothing while the report is off): the frame's result to its pinned copy, on `stream`
+        cudaError_t read_back(size_t s, cudaStream_t stream) {
+            return on() ? cudaMemcpyAsync(host.p + s, dev.p + s, sizeof(T), cudaMemcpyDeviceToHost, stream) : cudaSuccess;
+        }
+        // queue slot s once its copy has ended (nothing while the report is off): the frame's result becomes the last one
+        // and goes to `out` (may be null)
+        template <class Out>
+        void take(size_t s, Out *out, void (*to_abi)(const T &, Out *)) {
+            if (!on()) return;
+            last = host.p[s];
+            if (out) to_abi(last, out);
+        }
+    };
+    // a localizer, or an odometry pipeline with kb_pipeline_set_fit_reporting on, reports fits; either may also report
+    // plane constraints (kb_pipeline_set_constraint_reporting)
+    Report<FitResult> fit;
+    Report<PlaneResult> planes;
     Work ws;
     DBuf<PipeState> d_state;
     FrameResult last{};
@@ -378,7 +409,6 @@ struct kb_pipeline {
     size_t history_cap = 0;
     // frame queue of every registration call (a blocking call is a queue of one frame): frame k+1 is copied in while
     // frame k is registered
-    static constexpr int Q_DEPTH = 4;  // frame k registering, k+1 being prefetched by the same launch, k+2 / k+3 copying
     struct Slot {
         DBuf<double> in, ts;  // device copy of one queued frame
         PinBuf<unsigned char> pin_xyz, pin_ts;  // staging, used only when the caller's memory is pageable
@@ -1442,35 +1472,6 @@ static int pipeline_init_state(kb_pipeline *p) {
     return pipeline_push_state(p, se3_identity(), se3_identity(), p->last.model_sse, 1);
 }
 
-// the buffers of a pipeline that reports fits (on the pipeline's device); the last fit becomes all zero
-static int pipeline_alloc_fit(kb_pipeline *p) {
-    RET(p->fit_part.ensure(static_cast<size_t>(FIT_VALS) * p->ex->grid));
-    CK(p->fit_dev.alloc(kb_pipeline::Q_DEPTH));
-    CK(cudaMemsetAsync(p->fit_dev.p, 0, sizeof(FitResult) * kb_pipeline::Q_DEPTH, p->ex->stream));
-    CK(p->fit_host.alloc(kb_pipeline::Q_DEPTH));
-    p->last_fit = FitResult{};
-    return KB_OK;
-}
-static void pipeline_free_fit(kb_pipeline *p) {
-    p->fit_part = DBuf<double>{};
-    p->fit_dev = DBuf<FitResult>{};
-    p->fit_host = PinBuf<FitResult>{};
-}
-// likewise for the plane constraints
-static int pipeline_alloc_planes(kb_pipeline *p) {
-    RET(p->plane_part.ensure(static_cast<size_t>(PLANE_VALS) * p->ex->grid));
-    CK(p->plane_dev.alloc(kb_pipeline::Q_DEPTH));
-    CK(cudaMemsetAsync(p->plane_dev.p, 0, sizeof(PlaneResult) * kb_pipeline::Q_DEPTH, p->ex->stream));
-    CK(p->plane_host.alloc(kb_pipeline::Q_DEPTH));
-    p->last_planes = PlaneResult{};
-    return KB_OK;
-}
-static void pipeline_free_planes(kb_pipeline *p) {
-    p->plane_part = DBuf<double>{};
-    p->plane_dev = DBuf<PlaneResult>{};
-    p->plane_host = PinBuf<PlaneResult>{};
-}
-
 int kb_pipeline_create(const kb_config *cfg, kb_pipeline **out) {
     if (!cfg || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (cfg->max_num_iterations > 8000) return fail(KB_ERR_INVALID_ARG, "max_num_iterations > 8000 is not supported");
@@ -1521,7 +1522,7 @@ int kb_pipeline_create_localizer(const kb_config *cfg, const kb_map *cprior, kb_
     // everything queued on the map before (a load, updates, asynchronous queries) is complete before a frame reads it
     RET(prior->ex->sync());
     CK(cudaSetDevice(p->ex->device));
-    RET(pipeline_alloc_fit(p.get()));
+    RET(p->fit.set(true, FIT_VALS, *p->ex));
     RET(pipeline_init_state(p.get()));
     prior->readers.fetch_add(1);
     *out = p.release();
@@ -1549,13 +1550,11 @@ static size_t pipeline_extra(const kb_pipeline *p, size_t n) {
     return std::min(extra, n);
 }
 
-// enqueue one RegisterFrame on the pipeline's stream; the result goes to `res` (device-visible memory)
+// enqueue one RegisterFrame on the pipeline's stream; the result, and the reports the pipeline computes, go to queue
+// slot `slot` on the device
 // `next_xyz` (may be null): the frame after this one, already on the device, no timestamps -> its front end is prefetched
-// `fit` (pipelines that report fits only): where the frame's fit goes; `planes` (pipelines that report plane
-// constraints only): where its plane constraints go
 static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, size_t n, const double *d_ts, size_t n_ts,
-                           bool in_f32, FrameResult *res, FitResult *fit, PlaneResult *planes, const double *next_xyz,
-                           size_t next_n) {
+                           bool in_f32, size_t slot, const double *next_xyz, size_t next_n) {
     Exec &ex = *p->ex;
     FrameParams P;
     P.m = p->map->view();
@@ -1569,7 +1568,7 @@ static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, si
     P.next_in_f32 = in_f32 ? 1 : 0;
     P.ws = p->ws.view();
     P.st = p->d_state.p;
-    P.res = res;
+    P.res = p->q_res_dev.p + slot;
     P.in = d_xyz;
     P.ts = d_ts;
     P.n = static_cast<int>(n);
@@ -1585,33 +1584,12 @@ static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, si
     P.tag_base = ex.next_tag_base();
     P.in_f32 = in_f32 ? 1 : 0;
     const size_t smem = std::max<size_t>(QC_BYTES, ex.icp_smem);
-    if (p->constraint_reporting) {  // (a localizer, or fit reporting on)
-        if (p->localizer) {
-            LocalizeConstraintParams L;
-            static_cast<FrameParams &>(L) = P;
-            L.fit = FitOut{p->fit_part.p, fit};
-            L.planes = PlaneOut{p->plane_part.p, planes};
-            return ex.coop_raw(localize_constraints_kernel(), &L, smem, true);
-        }
-        OdometryConstraintParams F;
-        static_cast<FrameParams &>(F) = P;
-        F.fit = FitOut{p->fit_part.p, fit};
-        F.planes = PlaneOut{p->plane_part.p, planes};
-        return ex.coop_raw(odometry_constraints_kernel(), &F, smem, true);
-    }
-    if (p->localizer) {
-        LocalizeParams L;
-        static_cast<FrameParams &>(L) = P;
-        L.fit = FitOut{p->fit_part.p, fit};
-        return ex.coop_raw(localize_kernel(), &L, smem, true);
-    }
-    if (p->fit_reporting) {
-        OdometryFitParams F;
-        static_cast<FrameParams &>(F) = P;
-        F.fit = FitOut{p->fit_part.p, fit};
-        return ex.coop_raw(odometry_fit_kernel(), &F, smem, true);
-    }
-    return ex.coop(k_register_frame<FrameParams>, P, smem, true);
+    if (!p->fit.on()) return ex.coop(k_register_frame<FrameParams>, P, smem, true);
+    ReportParams R{};
+    static_cast<FrameParams &>(R) = P;
+    R.fit = FitOut{p->fit.part.p, p->fit.dev.p + slot};
+    if (p->planes.on()) R.planes = PlaneOut{p->planes.part.p, p->planes.dev.p + slot};
+    return ex.coop_raw(report_kernel(p->localizer, p->planes.on()), &R, smem, true);
 }
 
 // take over the result of a frame that ran (not vetoed): host mirror of the counters, history
@@ -1664,10 +1642,9 @@ enum Taken { TAKEN_ABSORBED, TAKEN_VETOED, TAKEN_SKIPPED };
 //   device. When they have ended, the table is grown for the frame's now known voxel count and the veto is cleared:
 //   the frame can be replayed.
 // - skipped: the frame did not run.
-// - absorbed: pipeline_absorb; the pose goes to pose_out, and the fit of a pipeline that reports fits (pinned copy
-//   `fit_slot`) becomes the last one and goes to fit_out (either may be null); so do its plane constraints when it
-//   reports them (constraints_out).
-static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long id, size_t fit_slot, double *pose_out,
+// - absorbed: pipeline_absorb; the pose goes to pose_out, and each report the pipeline computes (pinned copy `slot`)
+//   becomes the last one and goes to fit_out / constraints_out (any of them may be null).
+static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long id, size_t slot, double *pose_out,
                        kb_fit *fit_out, kb_constraints *constraints_out, Taken *taken) {
     RET(watchdog_check(p->ex->device));  // (a spin loop that gave up invalidates the launch)
     if (r.map_status & ST_NEED_GROW) {
@@ -1687,14 +1664,8 @@ static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long
     p->next_id = id + 1;
     RET(pipeline_absorb(p, r, n, id));
     if (pose_out) std::memcpy(pose_out, r.pose, sizeof(double) * 16);
-    if (p->reports_fits()) {
-        p->last_fit = p->fit_host.p[fit_slot];
-        if (fit_out) fit_to_abi(p->last_fit, fit_out);
-    }
-    if (p->constraint_reporting) {
-        p->last_planes = p->plane_host.p[fit_slot];
-        if (constraints_out) planes_to_abi(p->last_planes, constraints_out);
-    }
+    p->fit.take(slot, fit_out, fit_to_abi);
+    p->planes.take(slot, constraints_out, planes_to_abi);
     return KB_OK;
 }
 
@@ -1839,21 +1810,16 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
             }
             {
                 StallTrace t("queue: launch");
-                RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32, p->q_res_dev.p + k % D,
-                                    p->reports_fits() ? p->fit_dev.p + k % D : nullptr,
-                                    p->constraint_reporting ? p->plane_dev.p + k % D : nullptr, d_next, prefetch ? n[k + 1] : 0));
+                RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32, k % D, d_next,
+                                    prefetch ? n[k + 1] : 0));
                 CK(cudaEventRecord(s.done.p, ex.stream));
                 // result read-back on its own stream: neither the next kernel nor the next H2D waits for it (letting
                 // the kernel write to mapped host memory instead was slower)
                 CK(cudaStreamWaitEvent(p->res_stream.p, s.done.p, 0));
                 CK(cudaMemcpyAsync(p->q_res.p + k % D, p->q_res_dev.p + k % D, sizeof(FrameResult), cudaMemcpyDeviceToHost,
                                    p->res_stream.p));
-                if (p->reports_fits())
-                    CK(cudaMemcpyAsync(p->fit_host.p + k % D, p->fit_dev.p + k % D, sizeof(FitResult),
-                                       cudaMemcpyDeviceToHost, p->res_stream.p));
-                if (p->constraint_reporting)
-                    CK(cudaMemcpyAsync(p->plane_host.p + k % D, p->plane_dev.p + k % D, sizeof(PlaneResult),
-                                       cudaMemcpyDeviceToHost, p->res_stream.p));
+                CK(p->fit.read_back(k % D, p->res_stream.p));
+                CK(p->planes.read_back(k % D, p->res_stream.p));
                 CK(cudaEventRecord(s.read.p, p->res_stream.p));
             }
             ++next_submit;
@@ -1906,14 +1872,14 @@ int kb_pipeline_register_frames(kb_pipeline *p, const void *const *xyz, const si
 }
 int kb_pipeline_register_frames_fit(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
                                     const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out) {
-    if (p && fits_out && !p->reports_fits()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
+    if (p && fits_out && !p->fit.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
     return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out, nullptr);
 }
 int kb_pipeline_register_frames_constraints(kb_pipeline *p, const void *const *xyz, const size_t *n,
                                             const double *const *timestamps, const size_t *n_timestamps, size_t count,
                                             int layout, double *poses_out, kb_fit *fits_out, kb_constraints *constraints_out) {
-    if (p && fits_out && !p->reports_fits()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
-    if (p && constraints_out && !p->constraint_reporting) return fail(KB_ERR_INVALID_ARG, "%s", kNoConstraints);
+    if (p && fits_out && !p->fit.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
+    if (p && constraints_out && !p->planes.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoConstraints);
     return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out, constraints_out);
 }
 // a blocking call is a queue of one frame: there is no frame after it, so its front end runs in its own launch
@@ -1932,59 +1898,33 @@ int kb_pipeline_register_frame_dev(kb_pipeline *p, const double *d_xyz, size_t n
 }
 int kb_pipeline_last_fit(const kb_pipeline *p, kb_fit *out) {
     if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (!p->reports_fits()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
-    fit_to_abi(p->last_fit, out);
+    if (!p->fit.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
+    fit_to_abi(p->fit.last, out);
     return KB_OK;
 }
 int kb_pipeline_set_fit_reporting(kb_pipeline *p, int enabled) {
     if (!p) return fail(KB_ERR_INVALID_ARG, "p == NULL");
     if (p->localizer) return enabled ? KB_OK : fail(KB_ERR_INVALID_ARG, "a localizer always reports fits");
-    if (!enabled && p->constraint_reporting)
+    if (!enabled && p->planes.on())
         return fail(KB_ERR_INVALID_ARG, "plane constraint reporting needs the fits: turn it off first");
-    if (!enabled) {
-        p->fit_reporting = false;
-        pipeline_free_fit(p);  // (no launch of this pipeline is in flight between calls)
-        return KB_OK;
-    }
-    if (p->fit_reporting) return KB_OK;
-    CK(cudaSetDevice(p->ex->device));
-    const int st = pipeline_alloc_fit(p);
-    if (st != KB_OK) {
-        pipeline_free_fit(p);
-        return st;
-    }
-    p->fit_reporting = true;
-    return KB_OK;
+    return p->fit.set(enabled, FIT_VALS, *p->ex);
 }
 int kb_pipeline_set_constraint_reporting(kb_pipeline *p, int enabled) {
     if (!p) return fail(KB_ERR_INVALID_ARG, "p == NULL");
-    if (!enabled) {
-        p->constraint_reporting = false;
-        pipeline_free_planes(p);  // (no launch of this pipeline is in flight between calls)
-        return KB_OK;
-    }
-    if (!p->reports_fits())
+    if (enabled && !p->fit.on())
         return fail(KB_ERR_INVALID_ARG, "plane constraints are reported next to the fit: a localizer, or an odometry pipeline "
                                         "with kb_pipeline_set_fit_reporting on");
-    if (p->constraint_reporting) return KB_OK;
-    CK(cudaSetDevice(p->ex->device));
-    const int st = pipeline_alloc_planes(p);
-    if (st != KB_OK) {
-        pipeline_free_planes(p);
-        return st;
-    }
-    p->constraint_reporting = true;
-    return KB_OK;
+    return p->planes.set(enabled, PLANE_VALS, *p->ex);
 }
 int kb_pipeline_last_constraints(const kb_pipeline *p, kb_constraints *out) {
     if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    if (!p->constraint_reporting) return fail(KB_ERR_INVALID_ARG, "%s", kNoConstraints);
-    planes_to_abi(p->last_planes, out);
+    if (!p->planes.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoConstraints);
+    planes_to_abi(p->planes.last, out);
     return KB_OK;
 }
 int kb_pipeline_fit_reporting(const kb_pipeline *p, int *out) {
     if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    *out = p->reports_fits() ? 1 : 0;
+    *out = p->fit.on() ? 1 : 0;
     return KB_OK;
 }
 

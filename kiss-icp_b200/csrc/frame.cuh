@@ -1,7 +1,6 @@
 // KissICP::RegisterFrame as one persistent kernel (k_register_frame) and what it works on. A header of its own:
-// the odometry instantiation is compiled with the other kernels (api.cu), the localizer's, the fit-reporting
-// odometry's and the two plane-constraint-reporting ones each in a translation unit of their own (localize.cu,
-// odometry_fit.cu, constraints.cu), so that none changes the code generated for another.
+// the odometry instantiation is compiled with the other kernels (api.cu), the four that report fits and plane
+// constraints in a translation unit of their own (report.cu), so that they change no code generated for the first.
 #pragma once
 
 #include <type_traits>
@@ -124,7 +123,7 @@ __device__ __noinline__ void op_front(Grid &g, const Scratch &sc, Shared &sh, co
     op_downsample(g, sc, sh, fr.ds1, n_ds, voxel_size * 1.5, ws.ds2, fr.src, &fr.cnt[2], t_ns ? &t_ns[16] : nullptr, true);
 }
 
-// ---- the fit of a frame (k_register_frame<LocalizeParams> / <OdometryFitParams>, kb_pipeline_last_fit) --------------
+// ---- the fit of a frame (a reporting k_register_frame, kb_pipeline_last_fit) ---------------------------------------
 // DataAssociation + BuildLinearSystem (Registration.cpp:60-121) of the source mapped by the final pose, formed the way
 // kb_registration_build_system forms them (nn_search_warp, icp_term, expanded by icp_expand on the host), plus the
 // unweighted sum of |r|^2. Deterministic for a grid size: point qi -> CTA qi % G, warp (qi / G) % NWARPS, a lane sums
@@ -139,43 +138,8 @@ struct FitOut {
     double *part;    // [FIT_VALS][grid] per-CTA partials (value-major)
     FitResult *res;  // this frame's fit
 };
-struct LocalizeParams : FrameParams {
-    FitOut fit;
-};
-// an odometry pipeline that reports fits (kb_pipeline_set_fit_reporting): the odometry statement, plus the fit
-// against the map as this frame's ICP saw it, i.e. before the frame's own points are inserted
-struct OdometryFitParams : FrameParams {
-    FitOut fit;
-};
 
-// this CTA's partials of the fit: part[v][cta]. The caller provides the grid barrier behind it.
-__device__ __noinline__ void op_fit(Shared &sh, const MapView &m, const double *src, int n, const SE3 &pose,
-                                    double max_dist, double kscale, double *part) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int G = static_cast<int>(gridDim.x);
-    double acc = 0.0, sse = 0.0;  // lane l < 16 owns accumulator l; r is warp-uniform, so is sse
-    int corr = 0;
-    for (int qi = static_cast<int>(blockIdx.x) + G * warp; qi < n; qi += G * NWARPS) {
-        const V3 p = se3_act(pose, V3{src[3 * qi], src[3 * qi + 1], src[3 * qi + 2]});
-        const NNResult r = nn_search_warp(m, p, lane, sh.wnn[warp]);
-        if (r.d < max_dist) {
-            acc += icp_term(lane, p, r.p, kscale);
-            sse += sqnorm(p - r.p);
-            ++corr;
-        }
-    }
-    if (lane < NACC) sh.warp_d[warp][lane] = acc;
-    if (lane == NACC) sh.warp_d[warp][NACC] = static_cast<double>(corr);
-    if (lane == NACC + 1) sh.warp_d[warp][NACC + 1] = sse;
-    __syncthreads();
-    if (threadIdx.x < FIT_VALS) {
-        double v = 0.0;
-        for (int w = 0; w < NWARPS; ++w) v += sh.warp_d[w][threadIdx.x];
-        part[threadIdx.x * G + static_cast<int>(blockIdx.x)] = v;
-    }
-}
-
-// after the barrier behind op_fit: one CTA adds the partials in CTA order
+// after the barrier behind op_fit_planes: one CTA adds the partials in CTA order
 __device__ __forceinline__ void fit_finish(const FitOut &fit, int n_src) {
     const int G = static_cast<int>(gridDim.x);
     if (threadIdx.x < FIT_VALS) {
@@ -207,12 +171,9 @@ struct PlaneOut {
     double *part;      // [PLANE_VALS][grid] per-CTA partials (value-major)
     PlaneResult *res;  // this frame's result
 };
-// a localizer / a fit-reporting odometry pipeline that also reports plane constraints
-struct LocalizeConstraintParams : FrameParams {
-    FitOut fit;
-    PlaneOut planes;
-};
-struct OdometryConstraintParams : FrameParams {
+// a pipeline that reports fits (a localizer, or an odometry pipeline with kb_pipeline_set_fit_reporting on), and plane
+// constraints when it has kb_pipeline_set_constraint_reporting on (`planes` is not used otherwise)
+struct ReportParams : FrameParams {
     FitOut fit;
     PlaneOut planes;
 };
@@ -281,10 +242,10 @@ __device__ __forceinline__ double plane_term(const MapView &m, const V3 &p, cons
     return a * (Ji * Jj);
 }
 
-// the fit (FIT: op_fit's values into fit_part, the same operations in the same order) and the plane constraints of
-// the same correspondences into plane_part, from one nearest-neighbour search per source point. The caller provides the
-// grid barrier behind it.
-template <bool FIT>
+// this CTA's partials of the fit (FIT: into fit_part[v][cta]) and of the plane constraints of the same correspondences
+// (PLANES: into plane_part[v][cta]), from one nearest-neighbour search per source point. The caller provides the grid
+// barrier behind it.
+template <bool FIT, bool PLANES>
 __device__ __noinline__ void op_fit_planes(Shared &sh, const MapView &m, const double *src, int n, const SE3 &pose,
                                            double max_dist, double kscale, double *fit_part, double *plane_part) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -296,7 +257,7 @@ __device__ __noinline__ void op_fit_planes(Shared &sh, const MapView &m, const d
             ji = row;
             jj = row + t;
         }
-    double acc = 0.0, sse = 0.0, pacc = 0.0;
+    double acc = 0.0, sse = 0.0, pacc = 0.0;  // lane l < 16 owns accumulator l; r is warp-uniform, so is sse
     int corr = 0;
     for (int qi = static_cast<int>(blockIdx.x) + G * warp; qi < n; qi += G * NWARPS) {
         const V3 p = se3_act(pose, V3{src[3 * qi], src[3 * qi + 1], src[3 * qi + 2]});
@@ -307,7 +268,7 @@ __device__ __noinline__ void op_fit_planes(Shared &sh, const MapView &m, const d
                 sse += sqnorm(p - r.p);
                 ++corr;
             }
-            pacc += plane_term(m, p, r.p, lane, ji, jj);
+            if constexpr (PLANES) pacc += plane_term(m, p, r.p, lane, ji, jj);
         }
     }
     // (chunk_pref is free here: the ICP loop and the front end are done)
@@ -317,7 +278,9 @@ __device__ __noinline__ void op_fit_planes(Shared &sh, const MapView &m, const d
         if (lane == NACC) sh.warp_d[warp][NACC] = static_cast<double>(corr);
         if (lane == NACC + 1) sh.warp_d[warp][NACC + 1] = sse;
     }
-    if (lane < PLANE_VALS) pw[warp][lane] = pacc;
+    if constexpr (PLANES) {
+        if (lane < PLANE_VALS) pw[warp][lane] = pacc;
+    }
     __syncthreads();
     if constexpr (FIT) {
         if (threadIdx.x < FIT_VALS) {
@@ -326,11 +289,13 @@ __device__ __noinline__ void op_fit_planes(Shared &sh, const MapView &m, const d
             fit_part[threadIdx.x * G + static_cast<int>(blockIdx.x)] = v;
         }
     }
-    const int t = static_cast<int>(threadIdx.x) - 32;
-    if (t >= 0 && t < PLANE_VALS) {
-        double v = 0.0;
-        for (int w = 0; w < NWARPS; ++w) v += pw[w][t];
-        plane_part[t * G + static_cast<int>(blockIdx.x)] = v;
+    if constexpr (PLANES) {
+        const int t = static_cast<int>(threadIdx.x) - 32;
+        if (t >= 0 && t < PLANE_VALS) {
+            double v = 0.0;
+            for (int w = 0; w < NWARPS; ++w) v += pw[w][t];
+            plane_part[t * G + static_cast<int>(blockIdx.x)] = v;
+        }
     }
 }
 
@@ -356,21 +321,16 @@ __device__ __forceinline__ void planes_finish(const PlaneOut &pl) {
 //   [front end of this frame, unless a previous launch prefetched it]
 //   capacity check | fill pass (all CTAs) | ICP iterations on the team  ||  front end of the NEXT frame on the rest
 //   map update (all CTAs) | epilogue
-// k_register_frame<LocalizeParams> (a localizer): the same statement against a read-only prior map, without local_map_.Update
-// (KissICP.cpp:61). Nothing is inserted, so there is no capacity check and no veto, and the map-update phase is the
-// fit pass (op_fit) at the final pose. Nothing writes to the map.
-// k_register_frame<OdometryFitParams>: the odometry statement with the fit pass at the final pose in front of the map
-// update, and one grid barrier between them (op_fit reads the table op_map_add writes).
-// k_register_frame<LocalizeConstraintParams> / <OdometryConstraintParams>: the same, with op_fit_planes in place of
-// op_fit (the same fit, plus the plane constraints of its correspondences) and planes_finish next to fit_finish.
-template <class Params>
+// Params = ReportParams: the fit pass (op_fit_planes) at the final pose, with PLANES the plane constraints of its
+// correspondences too, and fit_finish / planes_finish after the last barrier.
+// LOCALIZE (a localizer): the same statement against a read-only prior map, without local_map_.Update (KissICP.cpp:61).
+// Nothing is inserted, so there is no capacity check and no veto, and the map-update phase is the fit pass. Nothing
+// writes to the map. Otherwise (odometry) the fit pass runs in front of the map update, with one grid barrier between
+// them (op_fit_planes reads the table op_map_add writes).
+template <class Params, bool LOCALIZE = false, bool PLANES = false>
 __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
-    constexpr bool PLANES = std::is_same<Params, LocalizeConstraintParams>::value ||
-                            std::is_same<Params, OdometryConstraintParams>::value;
-    constexpr bool LOCALIZE = std::is_same<Params, LocalizeParams>::value ||
-                              std::is_same<Params, LocalizeConstraintParams>::value;
-    constexpr bool ODOMETRY_FIT = std::is_same<Params, OdometryFitParams>::value ||
-                                  std::is_same<Params, OdometryConstraintParams>::value;
+    constexpr bool FIT = std::is_same<Params, ReportParams>::value;
+    static_assert(FIT || (!LOCALIZE && !PLANES), "a localizer, and plane reporting, need the fit's ReportParams");
     __shared__ Shared sh;
     Grid g;
     g.init(P.sc.bar);
@@ -496,25 +456,20 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
         r->cache_stats[1] = cs1;
         r->cache_stats[2] = cs2;
     }
-    if constexpr (LOCALIZE) {
-        // the fit at the final pose, with this frame's (3 sigma, sigma)
-        if constexpr (PLANES)
-            op_fit_planes<true>(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part, P.planes.part);
-        else
-            op_fit(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part);
-        kb_mark(0x700u);
-    } else {
-        if constexpr (ODOMETRY_FIT) {
-            // the fit at the final pose, with this frame's (3 sigma, sigma), against the map before local_map_.Update
-            // (after it, the frame's own points would be in the map). Stamps: the pass including the barrier behind it.
-            if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[35] = globaltimer_ns();
-            if constexpr (PLANES)
-                op_fit_planes<true>(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part, P.planes.part);
-            else
-                op_fit(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part);
+    if constexpr (FIT) {
+        // the fit at the final pose, with this frame's (3 sigma, sigma); an odometry pipeline's against the map before
+        // local_map_.Update (after it, the frame's own points would be in the map). Odometry stamps: the pass including
+        // the barrier behind it.
+        if (!LOCALIZE && P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[35] = globaltimer_ns();
+        op_fit_planes<true, PLANES>(sh, P.m, fr.src, n_src, new_pose, 3.0 * sigma, sigma, P.fit.part, P.planes.part);
+        if constexpr (!LOCALIZE) {
             g.sync();
             if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[36] = globaltimer_ns();
         }
+    }
+    if constexpr (LOCALIZE) {
+        kb_mark(0x700u);
+    } else {
         // local_map_.Update(frame_downsample, new_pose) (KissICP.cpp:61)
         op_map_add(g, sh, P.m, fr.ds1, n_ds, true, new_pose, P.ws.tp, P.ws.next, P.ws.touched, P.sc.profile ? &P.res->t_ns[8] : nullptr);
         kb_mark(0x700u);
@@ -524,7 +479,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
     g.sync();
     kb_mark(0x900u);
     KB_STAMP(5);
-    if constexpr (LOCALIZE || ODOMETRY_FIT) {
+    if constexpr (FIT) {
         if (blockIdx.x == gridDim.x - 1) fit_finish(P.fit, n_src);
     }
     if constexpr (PLANES) {
@@ -547,12 +502,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
 
 }  // namespace kb
 
-// defined in localize.cu, the localizer's device module: its k_register_frame<LocalizeParams> (takes a LocalizeParams)
-const void *localize_kernel();
-// defined in odometry_fit.cu, likewise: k_register_frame<OdometryFitParams>
-const void *odometry_fit_kernel();
-// defined in constraints.cu, likewise: k_register_frame<LocalizeConstraintParams> / <OdometryConstraintParams> and the
-// stand-alone k_constraints (takes a ConstraintsParams)
-const void *localize_constraints_kernel();
-const void *odometry_constraints_kernel();
+// defined in report.cu, the reporting device module: k_register_frame<ReportParams, localizer, planes> (takes a
+// ReportParams) and the stand-alone k_constraints (takes a ConstraintsParams)
+const void *report_kernel(bool localizer, bool planes);
 const void *constraints_kernel();

@@ -10,8 +10,8 @@
 // every device module that includes device_ops.cuh, by the function that sets its own copies of the watchdog's words
 // (device_ops.cuh: watchdog_arm), named after its file; and where api.cu's module keeps its phase marks (g_kb_marks)
 using WatchdogArm = cudaError_t(unsigned *d_host_words, const unsigned *init);
-WatchdogArm core_watchdog, localize_watchdog, odometry_fit_watchdog, constraints_watchdog, relocalize_watchdog, probe_watchdog,
-    pose_graph_watchdog, pose_graph_cov_watchdog, pose_graph_direct_watchdog, free_space_watchdog;
+WatchdogArm core_watchdog, report_watchdog, relocalize_watchdog, probe_watchdog, pose_graph_watchdog, pose_graph_cov_watchdog,
+    pose_graph_direct_watchdog, free_space_watchdog;
 const void *phase_marks_symbol();
 #pragma GCC visibility pop
 
@@ -43,9 +43,8 @@ int device_count() {
     return n;
 }
 
-WatchdogArm *const kWatchdogs[] = {core_watchdog,        localize_watchdog,   odometry_fit_watchdog,
-                                   constraints_watchdog, relocalize_watchdog, probe_watchdog,
-                                   pose_graph_watchdog,  pose_graph_cov_watchdog, pose_graph_direct_watchdog,
+WatchdogArm *const kWatchdogs[] = {core_watchdog,           report_watchdog,            relocalize_watchdog, probe_watchdog,
+                                   pose_graph_watchdog,     pose_graph_cov_watchdog,    pose_graph_direct_watchdog,
                                    free_space_watchdog};
 
 // the device watchdog's report (device_ops.cuh): mapped host words per device, checked after every synchronisation

@@ -217,7 +217,7 @@ struct Exec {
     int coop(void (*kern)(P), const P &p, size_t smem = 0, bool self_reset = false) {
         return coop_raw(reinterpret_cast<const void *>(kern), const_cast<P *>(&p), smem, self_reset);
     }
-    // `kern` takes one parameter struct, `param` points to it (a kernel of another device module: localize_kernel())
+    // `kern` takes one parameter struct, `param` points to it (a kernel of another device module: report_kernel())
     int coop_raw(const void *kern, void *param, size_t smem, bool self_reset) {
         CK(cudaSetDevice(device));
         RET(opt_in_smem(kern, smem));

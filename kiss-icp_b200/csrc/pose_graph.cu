@@ -1,6 +1,6 @@
 // The pose-graph optimizer (kb_pose_graph_optimize in api_pose_graph.cu): Levenberg-Marquardt with IRLS weights, the damped normal
 // equations solved by PCG with the exact inverse of their block-tridiagonal part, applied by block cyclic reduction.
-// The whole optimization is one persistent cooperative launch on the Grid barrier of device_ops.cuh. Like localize.cu,
+// The whole optimization is one persistent cooperative launch on the Grid barrier of device_ops.cuh. Like report.cu,
 // the unit compiles the header in a namespace of its own (and so has its own copies of the device watchdog's words,
 // which host.cu arms through pose_graph_watchdog), and a kernel here changes no code generated for the
 // kernels of the other units.

@@ -1,6 +1,6 @@
 // Device probes: small kernels that run the ICP loop's own device functions — the candidate-list reuse of both ICP paths,
 // the solver step, the exp and the reciprocal — on inputs a test chooses. The headers are compiled here in a namespace
-// of their own, like localize.cu, so that these kernels change no production kernel's code.
+// of their own, like report.cu, so that these kernels change no production kernel's code.
 #define kb kb_probe
 #include "icp_team.cuh"
 #undef kb

@@ -1,5 +1,5 @@
 // The relocalization's coarse score, k_reloc_score (kb_relocalize in api.cu), in a translation unit of its own. The
-// headers are compiled here in a namespace of their own, like localize.cu and probe.cu: a kernel added to api.cu's device
+// headers are compiled here in a namespace of their own, like report.cu and probe.cu: a kernel added to api.cu's device
 // module changes the code the compiler generates for the kernels already there.
 #define kb kb_reloc
 #include "device_ops.cuh"

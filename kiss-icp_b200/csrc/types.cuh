@@ -1,5 +1,5 @@
 // The plain data types that cross device-module boundaries: the map's view, the cross-CTA scratch, the ICP team's
-// scratch and the SE(3) structs. Every device module compiles device_ops.cuh in a namespace of its own (localize.cu);
+// scratch and the SE(3) structs. Every device module compiles device_ops.cuh in a namespace of its own (report.cu);
 // these live in kb_types, which that renaming leaves alone, and device_ops.cuh, icp_team.cuh and se3.cuh bring them
 // into each module's namespace. So a MapView or an SE3 is one type in every module and in the host code that passes
 // it between them. No __device__ variable and no non-inline function may go here.

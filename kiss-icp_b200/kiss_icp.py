@@ -59,6 +59,12 @@ def _fit_of(n_corr, n_src, sse, JTJ):
     return Fit(n.astype(np.int64), np.asarray(n_src, dtype=np.int64), rmse, np.asarray(JTJ, dtype=np.float64).reshape(-1, 6, 6))
 
 
+def _fits_from_structs(fs) -> Fit:
+    """a Fit of arrays from an array of kb_fit"""
+    return _fit_of([f.n_correspondences for f in fs], [f.n_source for f in fs], [f.sum_sq_residual for f in fs],
+                   np.array([f.JTJ[:] for f in fs]).reshape(-1, 36))
+
+
 def se3_params_from_matrix(T) -> np.ndarray:
     """4x4 SE(3) -> {qx,qy,qz,qw,tx,ty,tz}, the quaternion exactly as the library computes it from a matrix
     (Eigen's Quaterniond(Matrix3d); se3.cuh q_from_matrix, same operations in the same order)"""
@@ -380,23 +386,16 @@ class KissICP:
         n = (N.sz * K)(*sizes)
         nt = (N.sz * K)(*ts_sizes)
         poses = np.empty((K, 4, 4))
+        fits = (N.Fit * K)() if return_fits else None
+        cons = (N.Constraints * K)() if return_constraints else None
+        N.check(N.lib().kb_pipeline_register_frames_constraints(self._h, X, n, T, nt, K, int(layout), N.ptr(poses), fits,
+                                                                cons))
+        out = [poses]
+        if return_fits:
+            out.append(_fits_from_structs(fits))
         if return_constraints:
-            fits = (N.Fit * K)() if return_fits else None
-            cons = (N.Constraints * K)()
-            N.check(N.lib().kb_pipeline_register_frames_constraints(self._h, X, n, T, nt, K, int(layout), N.ptr(poses),
-                                                                    fits, cons))
-            if not return_fits:
-                return poses, _from_structs(cons)
-            return poses, _fit_of([f.n_correspondences for f in fits], [f.n_source for f in fits],
-                                  [f.sum_sq_residual for f in fits], np.array([f.JTJ[:] for f in fits]).reshape(-1, 36)), \
-                _from_structs(cons)
-        if not return_fits:
-            N.check(N.lib().kb_pipeline_register_frames(self._h, X, n, T, nt, K, int(layout), N.ptr(poses)))
-            return poses
-        fits = (N.Fit * K)()
-        N.check(N.lib().kb_pipeline_register_frames_fit(self._h, X, n, T, nt, K, int(layout), N.ptr(poses), fits))
-        return poses, _fit_of([f.n_correspondences for f in fits], [f.n_source for f in fits],
-                              [f.sum_sq_residual for f in fits], np.array([f.JTJ[:] for f in fits]).reshape(-1, 36))
+            out.append(_from_structs(cons))
+        return out[0] if len(out) == 1 else tuple(out)
 
     def _register_frame_modular(self, frame, timestamps):
         # python/kiss_icp/kiss_icp.py:43-75, line for line, on the per-module device API
