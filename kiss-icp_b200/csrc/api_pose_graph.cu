@@ -2,7 +2,6 @@
 // are in pose_graph.cu, pose_graph_cov.cu and pose_graph_direct.cu.
 #include <algorithm>
 #include <cmath>
-#include <functional>
 #include <memory>
 #include <numeric>
 #include <vector>
@@ -228,41 +227,6 @@ static int pg_grid(const Exec &ex, int co_resident, size_t items, int PB) {
     return static_cast<int>(std::max<size_t>(1, std::min<size_t>((std::max<size_t>(items, 1) + PB - 1) / PB, cap)));
 }
 
-// One optimizer launch between the graph's events (kb_debug_pose_graph_ms), then its result: the report, the free
-// nodes' poses (pq: the poses as uploaded) and s_e, w_e. Nothing is written to the caller's buffers on error.
-static int pg_run(kb_pose_graph *g, std::vector<double> &pq, const std::function<cudaError_t(cudaStream_t)> &launch,
-                  kb_pose_graph_report *out, double *edge_chi2, double *edge_weight) {
-    Exec &ex = *g->ex;
-    const size_t N = g->n(), E = g->m();
-    cudaStream_t s = ex.stream;
-    RET(events_on(g->ev, ex.device));
-    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
-    ex.bar_dirty = true;
-    g->factored = false;  // (the poses move)
-    CK(cudaEventRecord(g->ev[0].p, s));
-    CK(launch(s));
-    ++ex.launches;
-    CK(cudaEventRecord(g->ev[1].p, s));
-    kb_pose_graph_report rep{};
-    CK(cudaMemcpyAsync(&rep, g->report.p, sizeof(rep), cudaMemcpyDeviceToHost, s));
-    if (N) CK(cudaMemcpyAsync(pq.data(), g->pose_d.p, 8 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
-    std::vector<double> chi2(edge_chi2 ? E : 0), weight(edge_weight ? E : 0);
-    if (edge_chi2 && E) CK(cudaMemcpyAsync(chi2.data(), g->e_s.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
-    if (edge_weight && E) CK(cudaMemcpyAsync(weight.data(), g->e_w.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
-    RET(ex.sync());
-    g->uploaded = E;
-    for (size_t k = 0; k < N; ++k) {
-        if (g->fixed[k]) continue;
-        const double *v = &pq[8 * k];
-        g->pose[k] = SE3{{v[0], v[1], v[2], v[3]}, {v[4], v[5], v[6]}};
-        se3_to_matrix(g->pose[k], &g->mat[16 * k]);
-    }
-    *out = rep;
-    std::copy(chi2.begin(), chi2.end(), edge_chi2 ? edge_chi2 : chi2.data());
-    std::copy(weight.begin(), weight.end(), edge_weight ? edge_weight : weight.data());
-    return KB_OK;
-}
-
 void kb_pose_graph_options_default(kb_pose_graph_options *o) {
     if (o) *o = kb_pose_graph_options{100, 1e-12, 1e-10, 1e-4, 100, 1e-10};
 }
@@ -341,37 +305,19 @@ int kb_pose_graph_poses(const kb_pose_graph *g, double *poses, size_t cap, size_
     std::copy(g->mat.begin(), g->mat.end(), poses);
     return KB_OK;
 }
-int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_pose_graph_report *out, double *edge_chi2,
-                           double *edge_weight) {
-    if (!g || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
-    kb_pose_graph_options o;
-    RET(pg_options(opt, &o));
-    RET(pg_gauge_check(*g));
-    RET(require_device());
-    if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
-    Exec &ex = *g->ex;
-    CK(cudaSetDevice(ex.device));
-    int co_resident = 0;
-    CK(pose_graph_max_grid(ex.sms, &co_resident));
-    const int grid = pg_grid(ex, co_resident, std::max(g->n(), g->m()), POSE_GRAPH_BLOCK);
-    RET(pg_reserve(g, grid));
-    std::vector<double> pq;
-    PoseGraphParams P;
-    RET(pg_upload(g, &pq, &P));
-    pg_set_options(o, &P);
-    return pg_run(g, pq, [&](cudaStream_t s) { return pose_graph_launch(P, grid, s); }, out, edge_chi2, edge_weight);
-}
-
 static int pg_symbolic(kb_pose_graph *g);
 static int pg_sym_upload(kb_pose_graph *g);
 
-int kb_pose_graph_optimize_direct(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_pose_graph_report *out,
-                                  double *edge_chi2, double *edge_weight) {
+// One optimizer launch between the graph's events (kb_debug_pose_graph_ms): PCG (k_pose_graph) or, `direct`, exact
+// steps (k_pgc_optimize). Then its result: the report, the free nodes' poses and s_e, w_e. Nothing is written to the
+// caller's buffers on error.
+static int pg_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_pose_graph_report *out, double *edge_chi2,
+                       double *edge_weight, bool direct) {
     if (!g || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     kb_pose_graph_options o;
     RET(pg_options(opt, &o));
     RET(pg_gauge_check(*g));
-    RET(pg_symbolic(g));  // (refuses a graph whose factorization needs more than 2^30 block updates)
+    if (direct) RET(pg_symbolic(g));  // (refuses a graph whose factorization needs more than 2^30 block updates)
     RET(require_device());
     if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
     Exec &ex = *g->ex;
@@ -379,46 +325,83 @@ int kb_pose_graph_optimize_direct(kb_pose_graph *g, const kb_pose_graph_options 
     const PgcSymbolic &S = g->sym;
     const size_t N = g->n(), E = g->m();
     int co_resident = 0;
-    CK(pgc_optimize_max_grid(ex.sms, &co_resident));
-    const int grid = pg_grid(ex, co_resident, std::max({N, E, S.blocks()}), PGC_BLOCK);
+    CK(direct ? pgc_optimize_max_grid(ex.sms, &co_resident) : pose_graph_max_grid(ex.sms, &co_resident));
+    const int grid = direct ? pg_grid(ex, co_resident, std::max({N, E, S.blocks()}), PGC_BLOCK)
+                            : pg_grid(ex, co_resident, std::max(N, E), POSE_GRAPH_BLOCK);
     RET(pg_reserve(g, grid));
     PgcOptimizeParams O{};
     std::vector<double> pq;
     RET(pg_upload(g, &pq, &O.F.P));
     pg_set_options(o, &O.F.P);
-    RET(pg_sym_upload(g));
-    const size_t V = std::max({N, E, size_t(1)});
-    RET(g->Lx.ensure(std::max<size_t>(36 * S.blocks(), 1)));
-    RET(g->cov_flag.ensure(1));
-    RET(g->dir_val.ensure(2 * V));
-    RET(g->dir_chunk.ensure(2 * ((V + PGC_CHUNK - 1) / PGC_CHUNK)));
-    CK(cudaMemsetAsync(g->cov_flag.p, 0, sizeof(int), ex.stream));
-    PgcFactorParams &F = O.F;
-    F.nf = S.nf;
-    F.levels = S.levels();
-    F.n_blocks = static_cast<int>(S.blocks());
-    F.order = g->s_order.p;
-    F.lev_ptr = g->s_lev_ptr.p;
-    F.colptr = g->s_colptr.p;
-    F.brow = g->s_brow.p;
-    F.bcol = g->s_bcol.p;
-    F.hptr = g->s_hptr.p;
-    F.hedge = g->s_hedge.p;
-    F.uptr = g->s_uptr.p;
-    F.upd = g->s_upd.p;
-    F.Lx = g->Lx.p;
-    F.flag = g->cov_flag.p;
-    O.Fd = F;
-    O.Fd.P.hd = F.P.D;
-    O.rptr = g->s_rptr.p;
-    O.rblk = g->s_rblk.p;
-    O.pos = g->s_pos.p;
-    O.y = F.P.x;  // (6 N doubles of the PCG vectors: nf <= N)
-    O.val = g->dir_val.p;
-    O.chunk = g->dir_chunk.p;
-    O.stride = static_cast<int>(V);
-    // (Lx now holds the damped system's factor: the marginals factor H again)
-    return pg_run(g, pq, [&](cudaStream_t s) { return pgc_optimize_launch(O, grid, s); }, out, edge_chi2, edge_weight);
+    cudaStream_t s = ex.stream;
+    if (direct) {
+        RET(pg_sym_upload(g));
+        const size_t V = std::max({N, E, size_t(1)});
+        RET(g->Lx.ensure(std::max<size_t>(36 * S.blocks(), 1)));
+        RET(g->cov_flag.ensure(1));
+        RET(g->dir_val.ensure(2 * V));
+        RET(g->dir_chunk.ensure(2 * ((V + PGC_CHUNK - 1) / PGC_CHUNK)));
+        CK(cudaMemsetAsync(g->cov_flag.p, 0, sizeof(int), s));
+        PgcFactorParams &F = O.F;
+        F.nf = S.nf;
+        F.levels = S.levels();
+        F.n_blocks = static_cast<int>(S.blocks());
+        F.order = g->s_order.p;
+        F.lev_ptr = g->s_lev_ptr.p;
+        F.colptr = g->s_colptr.p;
+        F.brow = g->s_brow.p;
+        F.bcol = g->s_bcol.p;
+        F.hptr = g->s_hptr.p;
+        F.hedge = g->s_hedge.p;
+        F.uptr = g->s_uptr.p;
+        F.upd = g->s_upd.p;
+        F.Lx = g->Lx.p;
+        F.flag = g->cov_flag.p;
+        O.Fd = F;
+        O.Fd.P.hd = F.P.D;
+        O.rptr = g->s_rptr.p;
+        O.rblk = g->s_rblk.p;
+        O.pos = g->s_pos.p;
+        O.y = F.P.x;  // (6 N doubles of the PCG vectors: nf <= N)
+        O.val = g->dir_val.p;
+        O.chunk = g->dir_chunk.p;
+        O.stride = static_cast<int>(V);
+    }
+    RET(events_on(g->ev, ex.device));
+    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
+    ex.bar_dirty = true;
+    g->factored = false;  // (the poses move; after the direct solver Lx holds the damped system's factor)
+    CK(cudaEventRecord(g->ev[0].p, s));
+    CK(direct ? pgc_optimize_launch(O, grid, s) : pose_graph_launch(O.F.P, grid, s));
+    ++ex.launches;
+    CK(cudaEventRecord(g->ev[1].p, s));
+    kb_pose_graph_report rep{};
+    CK(cudaMemcpyAsync(&rep, g->report.p, sizeof(rep), cudaMemcpyDeviceToHost, s));
+    if (N) CK(cudaMemcpyAsync(pq.data(), g->pose_d.p, 8 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
+    std::vector<double> chi2(edge_chi2 ? E : 0), weight(edge_weight ? E : 0);
+    if (edge_chi2 && E) CK(cudaMemcpyAsync(chi2.data(), g->e_s.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (edge_weight && E) CK(cudaMemcpyAsync(weight.data(), g->e_w.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
+    RET(ex.sync());
+    g->uploaded = E;
+    for (size_t k = 0; k < N; ++k) {
+        if (g->fixed[k]) continue;
+        const double *v = &pq[8 * k];
+        g->pose[k] = SE3{{v[0], v[1], v[2], v[3]}, {v[4], v[5], v[6]}};
+        se3_to_matrix(g->pose[k], &g->mat[16 * k]);
+    }
+    *out = rep;
+    std::copy(chi2.begin(), chi2.end(), edge_chi2 ? edge_chi2 : chi2.data());
+    std::copy(weight.begin(), weight.end(), edge_weight ? edge_weight : weight.data());
+    return KB_OK;
+}
+
+int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_pose_graph_report *out, double *edge_chi2,
+                           double *edge_weight) {
+    return pg_optimize(g, opt, out, edge_chi2, edge_weight, false);
+}
+int kb_pose_graph_optimize_direct(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_pose_graph_report *out,
+                                  double *edge_chi2, double *edge_weight) {
+    return pg_optimize(g, opt, out, edge_chi2, edge_weight, true);
 }
 
 int kb_debug_pose_graph_ms(const kb_pose_graph *g, float *ms) {

@@ -1,5 +1,6 @@
 // The pose-graph optimizer (kb_pose_graph_optimize in api_pose_graph.cu): Levenberg-Marquardt with IRLS weights, the damped normal
 // equations solved by PCG with the exact inverse of their block-tridiagonal part, applied by block cyclic reduction.
+// The LM loop is lm_optimize (pose_graph_edges.cuh), shared with pose_graph_direct.cu; this unit supplies its solve.
 // The whole optimization is one persistent cooperative launch on the Grid barrier of device_ops.cuh. Like report.cu,
 // the unit compiles the header in a namespace of its own (and so has its own copies of the device watchdog's words,
 // which host.cu arms through pose_graph_watchdog), and a kernel here changes no code generated for the
@@ -332,149 +333,97 @@ __device__ double edges_pass(Grid &g, Red &rd, PgShared &sh, const PoseGraphPara
     return 0.5 * out[0];
 }
 
-enum { T_FUNCTION = KB_PG_FUNCTION_TOLERANCE, T_STEP = KB_PG_PARAMETER_TOLERANCE, T_MAX = KB_PG_MAX_ITERATIONS,
-       T_NO_DECREASE = KB_PG_NO_DECREASE };
+// The PCG solve of lm_optimize (pose_graph_edges.cuh): every sum by grid_reduce
+struct PcgSolve {
+    Grid &g;
+    const PoseGraphParams &P;
+    PgShared &sh;
+    Red rd;
+    long long gt, gs;
+    int cg_iterations;
+
+    __device__ double linearize(const double *poses) { return edges_pass(g, rd, sh, P, poses, true, gt, gs); }
+    __device__ void relinearize(const double *poses) { edges_pass(g, rd, sh, P, poses, true, gt, gs); }
+
+    __device__ bool step(double lambda, int iteration, const double *cur, double *cand, double &max_d, double &Fc) {
+        const long long N = P.n_nodes;
+        for (long long k = gt; k < N; k += gs) assemble_node(P, static_cast<int>(k), lambda);
+        g.sync();
+        bcr_factor(g, P, iteration + 1, gt, gs);
+        if (*reinterpret_cast<volatile int *>(P.flag) == iteration + 1) return false;  // (written before the last barrier)
+        // PCG on (H + lambda diag H) x = -g from x = 0
+        for (long long k = gt; k < N; k += gs)
+#pragma unroll
+            for (int a = 0; a < 6; ++a) {
+                P.x[6 * k + a] = 0.0;
+                P.r[6 * k + a] = -P.g[6 * k + a];
+            }
+        g.sync();
+        bcr_solve(g, P, gt, gs);
+        double v[2] = {0.0, 0.0}, o[2];
+        for (long long k = gt; k < N; k += gs)
+#pragma unroll
+            for (int a = 0; a < 6; ++a) {
+                const double r = P.r[6 * k + a], z = P.z[6 * k + a];
+                P.p[6 * k + a] = z;
+                v[0] = v[0] + r * z;
+                v[1] = v[1] + r * r;
+            }
+        grid_reduce<2>(g, rd, v, o, sh.red, sh.out);
+        double rz = o[0];
+        const double rr0 = o[1];
+        const double stop = P.cg_tolerance * P.cg_tolerance * rr0;
+        for (int it = 0; it < P.max_cg_iterations && rr0 > 0.0; ++it) {
+            double pq[1] = {0.0}, opq[1];
+            for (long long k = gt; k < N; k += gs) {
+                matvec_node(P, static_cast<int>(k), lambda, P.p, P.q);
+#pragma unroll
+                for (int a = 0; a < 6; ++a) pq[0] = pq[0] + P.p[6 * k + a] * P.q[6 * k + a];
+            }
+            grid_reduce<1>(g, rd, pq, opq, sh.red, sh.out);
+            ++cg_iterations;
+            if (!(opq[0] > 0.0) || !(rz > 0.0)) break;
+            const double alpha = rz / opq[0];
+            double rr[1] = {0.0}, orr[1];
+            for (long long k = gt; k < N; k += gs)
+#pragma unroll
+                for (int a = 0; a < 6; ++a) {
+                    P.x[6 * k + a] = P.x[6 * k + a] + alpha * P.p[6 * k + a];
+                    const double r = P.r[6 * k + a] - alpha * P.q[6 * k + a];
+                    P.r[6 * k + a] = r;
+                    rr[0] = rr[0] + r * r;
+                }
+            grid_reduce<1>(g, rd, rr, orr, sh.red, sh.out);
+            if (orr[0] <= stop) break;
+            bcr_solve(g, P, gt, gs);
+            double rz1[1] = {0.0}, orz[1];
+            for (long long k = gt; k < N; k += gs)
+#pragma unroll
+                for (int a = 0; a < 6; ++a) rz1[0] = rz1[0] + P.r[6 * k + a] * P.z[6 * k + a];
+            grid_reduce<1>(g, rd, rz1, orz, sh.red, sh.out);
+            const double beta = orz[0] / rz;
+            rz = orz[0];
+            for (long long k = gt; k < N; k += gs)
+#pragma unroll
+                for (int a = 0; a < 6; ++a) P.p[6 * k + a] = P.z[6 * k + a] + beta * P.p[6 * k + a];
+            g.sync();
+        }
+        double mx[1] = {0.0}, omx[1];
+        for (long long k = gt; k < N; k += gs) mx[0] = fmax(mx[0], candidate_pose(P, cur, cand, k, P.x + 6 * k));
+        grid_reduce<1, true>(g, rd, mx, omx, sh.red, sh.out);
+        max_d = omx[0];
+        Fc = edges_pass(g, rd, sh, P, cand, false, gt, gs);
+        return true;
+    }
+};
 
 __global__ void __launch_bounds__(PB, 1) k_pose_graph(const PoseGraphParams P) {
     __shared__ PgShared sh;
     Grid g;
     g.init(P.bar);
-    Red rd{P.part, 0};
-    const long long gt = static_cast<long long>(blockIdx.x) * PB + threadIdx.x, gs = static_cast<long long>(gridDim.x) * PB;
-    const long long N = P.n_nodes;
-    double *cur = P.pose, *cand = P.cand;
-    double F = edges_pass(g, rd, sh, P, cur, true, gt, gs);
-    const double F0 = F;
-    double lambda = P.initial_lambda;
-    int iterations = 0, accepted = 0, cg_total = 0, term = T_MAX;
-    while (iterations < P.max_iterations) {
-        for (long long k = gt; k < N; k += gs) assemble_node(P, static_cast<int>(k), lambda);
-        g.sync();
-        bcr_factor(g, P, iterations + 1, gt, gs);
-        const bool factored = *reinterpret_cast<volatile int *>(P.flag) != iterations + 1;  // (written before the last barrier)
-        double step = 0.0;
-        if (factored) {
-            // PCG on (H + lambda diag H) x = -g from x = 0
-            for (long long k = gt; k < N; k += gs)
-#pragma unroll
-                for (int a = 0; a < 6; ++a) {
-                    P.x[6 * k + a] = 0.0;
-                    P.r[6 * k + a] = -P.g[6 * k + a];
-                }
-            g.sync();
-            bcr_solve(g, P, gt, gs);
-            double v[2] = {0.0, 0.0}, o[2];
-            for (long long k = gt; k < N; k += gs)
-#pragma unroll
-                for (int a = 0; a < 6; ++a) {
-                    const double r = P.r[6 * k + a], z = P.z[6 * k + a];
-                    P.p[6 * k + a] = z;
-                    v[0] = v[0] + r * z;
-                    v[1] = v[1] + r * r;
-                }
-            grid_reduce<2>(g, rd, v, o, sh.red, sh.out);
-            double rz = o[0];
-            const double rr0 = o[1];
-            const double stop = P.cg_tolerance * P.cg_tolerance * rr0;
-            for (int it = 0; it < P.max_cg_iterations && rr0 > 0.0; ++it) {
-                double pq[1] = {0.0}, opq[1];
-                for (long long k = gt; k < N; k += gs) {
-                    matvec_node(P, static_cast<int>(k), lambda, P.p, P.q);
-#pragma unroll
-                    for (int a = 0; a < 6; ++a) pq[0] = pq[0] + P.p[6 * k + a] * P.q[6 * k + a];
-                }
-                grid_reduce<1>(g, rd, pq, opq, sh.red, sh.out);
-                ++cg_total;
-                if (!(opq[0] > 0.0) || !(rz > 0.0)) break;
-                const double alpha = rz / opq[0];
-                double rr[1] = {0.0}, orr[1];
-                for (long long k = gt; k < N; k += gs)
-#pragma unroll
-                    for (int a = 0; a < 6; ++a) {
-                        P.x[6 * k + a] = P.x[6 * k + a] + alpha * P.p[6 * k + a];
-                        const double r = P.r[6 * k + a] - alpha * P.q[6 * k + a];
-                        P.r[6 * k + a] = r;
-                        rr[0] = rr[0] + r * r;
-                    }
-                grid_reduce<1>(g, rd, rr, orr, sh.red, sh.out);
-                if (orr[0] <= stop) break;
-                bcr_solve(g, P, gt, gs);
-                double rz1[1] = {0.0}, orz[1];
-                for (long long k = gt; k < N; k += gs)
-#pragma unroll
-                    for (int a = 0; a < 6; ++a) rz1[0] = rz1[0] + P.r[6 * k + a] * P.z[6 * k + a];
-                grid_reduce<1>(g, rd, rz1, orz, sh.red, sh.out);
-                const double beta = orz[0] / rz;
-                rz = orz[0];
-                for (long long k = gt; k < N; k += gs)
-#pragma unroll
-                    for (int a = 0; a < 6; ++a) P.p[6 * k + a] = P.z[6 * k + a] + beta * P.p[6 * k + a];
-                g.sync();
-            }
-            // candidate T_k Exp(x_k), and max |x|
-            double mx[1] = {0.0}, omx[1];
-            for (long long k = gt; k < N; k += gs) {
-                const double *src = cur + 8 * k;
-                double *dst = cand + 8 * k;
-                if (P.fixed[k]) {
-#pragma unroll
-                    for (int a = 0; a < 8; ++a) dst[a] = src[a];
-                    continue;
-                }
-                double d[6];
-#pragma unroll
-                for (int a = 0; a < 6; ++a) {
-                    d[a] = P.x[6 * k + a];
-                    mx[0] = fmax(mx[0], fabs(d[a]));
-                }
-                st_pose(dst, se3_mul(ld_pose(src), se3_exp(d)));
-            }
-            grid_reduce<1, true>(g, rd, mx, omx, sh.red, sh.out);
-            step = omx[0];
-        }
-        ++iterations;
-        const double Fc = factored ? edges_pass(g, rd, sh, P, cand, false, gt, gs) : NAN;
-        if (Fc < F) {  // (false for a non-finite cost)
-            double *t = cur;
-            cur = cand;
-            cand = t;
-            const double F_old = F;
-            F = Fc;
-            lambda = lambda / 10.0;
-            ++accepted;
-            edges_pass(g, rd, sh, P, cur, true, gt, gs);
-            if (F_old - F <= P.function_tolerance * F_old) {
-                term = T_FUNCTION;
-                break;
-            }
-        } else {
-            lambda = lambda * 10.0;
-            if (lambda > 1e12) {
-                term = T_NO_DECREASE;
-                break;
-            }
-        }
-        if (factored && step <= P.parameter_tolerance) {
-            term = T_STEP;
-            break;
-        }
-    }
-    if (cur != P.pose) {
-        for (long long k = gt; k < N; k += gs)
-#pragma unroll
-            for (int a = 0; a < 8; ++a) P.pose[8 * k + a] = cur[8 * k + a];
-    }
-    if (gt == 0) {
-        kb_pose_graph_report r;
-        r.iterations = iterations;
-        r.accepted = accepted;
-        r.cg_iterations = cg_total;
-        r.termination = term;
-        r.initial_cost = F0;
-        r.final_cost = F;
-        r.lambda = lambda;
-        *P.report = r;
-    }
+    PcgSolve S{g, P, sh, {P.part, 0}, static_cast<long long>(blockIdx.x) * PB + threadIdx.x,
+               static_cast<long long>(gridDim.x) * PB, 0};
+    lm_optimize(P, S);
 }
 
 }  // namespace kb_pg

@@ -351,8 +351,8 @@ namespace kb_pgc {
 #include "pose_graph_edges.cuh"
 #include "pose_graph_factor.cuh"
 
-// Linearize every edge at the current poses, assemble H's blocks (lambda 0), then the levels of the elimination tree
-// from the leaves up: every block of the level's columns takes its updates, then every column its pivot and solves.
+// Linearize every edge at the current poses, assemble H's blocks (lambda 0), gather them into L's, then factor them
+// level by level.
 __global__ void __launch_bounds__(PGC_BLOCK, 1) k_pgc_factor(const PgcFactorParams F) {
     Grid g;
     g.init(F.P.bar);
@@ -363,15 +363,7 @@ __global__ void __launch_bounds__(PGC_BLOCK, 1) k_pgc_factor(const PgcFactorPara
     g.sync();
     for (int b = gt; b < F.n_blocks; b += gs) gather_block(F, b);
     g.sync();
-    for (int l = 0; l < F.levels; ++l) {
-        const int s0 = F.lev_ptr[l], s1 = F.lev_ptr[l + 1];
-        if (l > 0) {  // (the leaves have no updates)
-            for (int b = F.colptr[s0] + gt; b < F.colptr[s1]; b += gs) update_block(F, b);
-            g.sync();
-        }
-        for (int s = s0 + gt; s < s1; s += gs) factor_column(F, s);
-        if (l + 1 < F.levels) g.sync();
-    }
+    factor_levels(g, F, gt, gs);
 }
 
 // Column c of X = L^-1 P^T E (E: the node's six unit columns), along the path `path` (n positions, ascending) from the

@@ -1,5 +1,5 @@
 // The pose-graph optimizer with exact steps (kb_pose_graph_optimize_direct in api_pose_graph.cu): the
-// Levenberg-Marquardt of k_pose_graph (pose_graph.cu), each step's damped system H + lambda diag H factored by the sparse
+// Levenberg-Marquardt of lm_optimize (pose_graph_edges.cuh), each step's damped system H + lambda diag H factored by the sparse
 // block Cholesky factorization of the covariance (pose_graph_cov.cu: its symbolic analysis, and the device functions of
 // pose_graph_factor.cuh), then solved by a forward and a backward block substitution over the level schedule. One
 // persistent cooperative launch on the Grid barrier of device_ops.cuh.
@@ -140,122 +140,71 @@ __device__ __noinline__ void backward_column(const PgcOptimizeParams &O, int s) 
     for (int a = 0; a < 6; ++a) yj[a] = v[a];
 }
 
-// Per LM step: assemble H + lambda diag H, gather it into L's blocks and factor it level by level (k_pgc_factor's
-// functions), the forward sweep from the leaves up and the backward sweep from the roots down, the candidate
-// T_k Exp(d_k) and its cost; acceptance, lambda and the stopping rules are k_pose_graph's, in its order.
-__global__ void __launch_bounds__(PGC_BLOCK, 1) k_pgc_optimize(const PgcOptimizeParams O) {
-    __shared__ double s_out[2];
-    const PgcFactorParams &F = O.F;
-    const PoseGraphParams &P = F.P;
-    Grid g;
-    g.init(P.bar);
-    const int gt = blockIdx.x * PGC_BLOCK + threadIdx.x, gs = gridDim.x * PGC_BLOCK;
-    const int N = P.n_nodes, E = P.n_edges;
-    double *cur = P.pose, *cand = P.cand;
-    double red[2];
-    for (int e = gt; e < E; e += gs) O.val[e] = edge_linearize(P, cur, e);
-    reduce_chunks(g, O, E, 0, s_out, red);
-    double Fx = 0.5 * red[0];
-    const double F0 = Fx;
-    double lambda = P.initial_lambda;
-    int iterations = 0, accepted = 0, term = KB_PG_MAX_ITERATIONS;
-    while (iterations < P.max_iterations) {
+// The exact solve of lm_optimize (pose_graph_edges.cuh): per step, assemble H + lambda diag H, gather it into L's
+// blocks and factor it level by level (k_pgc_factor's functions), the forward sweep from the leaves up and the
+// backward sweep from the roots down, the candidate and its cost. Every sum by reduce_chunks.
+struct DirectSolve {
+    Grid &g;
+    const PgcOptimizeParams &O;
+    double *s_out;
+    int gt, gs;
+    static constexpr int cg_iterations = 0;
+
+    __device__ double linearize(const double *poses) {
+        const PoseGraphParams &P = O.F.P;
+        for (int e = gt; e < P.n_edges; e += gs) O.val[e] = edge_linearize(P, poses, e);
+        double red[2];
+        reduce_chunks(g, O, P.n_edges, 0, s_out, red);
+        return 0.5 * red[0];
+    }
+    __device__ void relinearize(const double *poses) {
+        for (int e = gt; e < O.F.P.n_edges; e += gs) edge_linearize(O.F.P, poses, e);
+        g.sync();
+    }
+
+    __device__ bool step(double lambda, int, const double *cur, double *cand, double &max_d, double &Fc) {
+        const PgcFactorParams &F = O.F;
+        const PoseGraphParams &P = F.P;
+        const int N = P.n_nodes, E = P.n_edges;
         if (gt == 0) *F.flag = 0;  // (every CTA read the last step's flag before a barrier that follows)
         for (int k = gt; k < N; k += gs) assemble_node(P, k, lambda);
         g.sync();
         for (int b = gt; b < F.n_blocks; b += gs) gather_block(O.Fd, b);
         g.sync();
-        for (int l = 0; l < F.levels; ++l) {
-            const int s0 = F.lev_ptr[l], s1 = F.lev_ptr[l + 1];
-            if (l > 0) {
-                for (int b = F.colptr[s0] + gt; b < F.colptr[s1]; b += gs) update_block(F, b);
-                g.sync();
-            }
-            for (int s = s0 + gt; s < s1; s += gs) factor_column(F, s);
-            g.sync();
-        }
-        const bool factored = *reinterpret_cast<volatile int *>(F.flag) == 0;
-        double step = 0.0, Fc = NAN;
-        if (factored) {
-            for (int l = 0; l < F.levels; ++l) {
-                for (int s = F.lev_ptr[l] + gt; s < F.lev_ptr[l + 1]; s += gs) forward_column(O, s);
-                g.sync();
-            }
-            for (int l = F.levels - 1; l >= 0; --l) {
-                for (int s = F.lev_ptr[l] + gt; s < F.lev_ptr[l + 1]; s += gs) backward_column(O, s);
-                g.sync();
-            }
-            // candidate T_k Exp(d_k), and max |d_k| per node
-            for (int k = gt; k < N; k += gs) {
-                const double *src = cur + 8 * static_cast<size_t>(k);
-                double *dst = cand + 8 * static_cast<size_t>(k);
-                double mx = 0.0;
-                if (P.fixed[k]) {
-#pragma unroll
-                    for (int a = 0; a < 8; ++a) dst[a] = src[a];
-                } else {
-                    const double *y = O.y + 6 * static_cast<size_t>(O.pos[k]);
-                    double d[6];
-#pragma unroll
-                    for (int a = 0; a < 6; ++a) {
-                        d[a] = y[a];
-                        mx = fmax(mx, fabs(d[a]));
-                    }
-                    st_pose(dst, se3_mul(ld_pose(src), se3_exp(d)));
-                }
-                O.val[O.stride + k] = mx;
-            }
-            g.sync();
-            for (int e = gt; e < E; e += gs) O.val[e] = edge_eval(P, cand, e).rho;
-            reduce_chunks(g, O, E, N, s_out, red);
-            Fc = 0.5 * red[0];
-            step = red[1];
-        } else {
+        factor_levels(g, F, gt, gs);
+        if (F.levels > 0) g.sync();  // (after the last level)
+        if (*reinterpret_cast<volatile int *>(F.flag) != 0) {
             g.sync();  // (every CTA has read the flag before the next step clears it)
+            return false;
         }
-        ++iterations;
-        if (Fc < Fx) {  // (false for a non-finite cost)
-            double *t = cur;
-            cur = cand;
-            cand = t;
-            const double F_old = Fx;
-            Fx = Fc;
-            lambda = lambda / 10.0;
-            ++accepted;
-            for (int e = gt; e < E; e += gs) edge_linearize(P, cur, e);
+        for (int l = 0; l < F.levels; ++l) {
+            for (int s = F.lev_ptr[l] + gt; s < F.lev_ptr[l + 1]; s += gs) forward_column(O, s);
             g.sync();
-            if (F_old - Fx <= P.function_tolerance * F_old) {
-                term = KB_PG_FUNCTION_TOLERANCE;
-                break;
-            }
-        } else {
-            lambda = lambda * 10.0;
-            if (lambda > 1e12) {
-                term = KB_PG_NO_DECREASE;
-                break;
-            }
         }
-        if (factored && step <= P.parameter_tolerance) {
-            term = KB_PG_PARAMETER_TOLERANCE;
-            break;
+        for (int l = F.levels - 1; l >= 0; --l) {
+            for (int s = F.lev_ptr[l] + gt; s < F.lev_ptr[l + 1]; s += gs) backward_column(O, s);
+            g.sync();
         }
-    }
-    if (cur != P.pose) {
+        // (a fixed node's position is -1: its d is not read)
         for (int k = gt; k < N; k += gs)
-#pragma unroll
-            for (int a = 0; a < 8; ++a) P.pose[8 * static_cast<size_t>(k) + a] = cur[8 * static_cast<size_t>(k) + a];
+            O.val[O.stride + k] = candidate_pose(P, cur, cand, k, O.y + 6 * static_cast<size_t>(max(O.pos[k], 0)));
+        g.sync();
+        for (int e = gt; e < E; e += gs) O.val[e] = edge_eval(P, cand, e).rho;
+        double red[2];
+        reduce_chunks(g, O, E, N, s_out, red);
+        Fc = 0.5 * red[0];
+        max_d = red[1];
+        return true;
     }
-    if (gt == 0) {
-        kb_pose_graph_report r;
-        r.iterations = iterations;
-        r.accepted = accepted;
-        r.cg_iterations = 0;
-        r.termination = term;
-        r.initial_cost = F0;
-        r.final_cost = Fx;
-        r.lambda = lambda;
-        *P.report = r;
-    }
+};
+
+__global__ void __launch_bounds__(PGC_BLOCK, 1) k_pgc_optimize(const PgcOptimizeParams O) {
+    __shared__ double s_out[2];
+    Grid g;
+    g.init(O.F.P.bar);
+    DirectSolve S{g, O, s_out, static_cast<int>(blockIdx.x * PGC_BLOCK + threadIdx.x),
+                  static_cast<int>(gridDim.x * PGC_BLOCK)};
+    lm_optimize(O.F.P, S);
 }
 
 }  // namespace kb_pgd

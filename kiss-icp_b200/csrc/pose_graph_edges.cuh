@@ -1,7 +1,8 @@
 // Device code of the pose graph that both optimizers (pose_graph.cu, pose_graph_direct.cu) and the covariance
-// (pose_graph_cov.cu) run: the pose layout, the 6x6 helpers, one edge's linearization and the gather of a node's
-// diagonal block. Each unit includes this inside its own namespace, after device_ops.cuh, so each module has its own
-// copies (DESIGN §4.6: a kernel of one unit changes no code generated for another's).
+// (pose_graph_cov.cu) run: the pose layout, the 6x6 helpers, one edge's linearization, the gather of a node's
+// diagonal block, and the Levenberg-Marquardt loop with its candidate step. Each unit includes this inside its own
+// namespace, after device_ops.cuh, so each module has its own copies (DESIGN §4.6: a kernel of one unit changes no
+// code generated for another's).
 
 __device__ __forceinline__ SE3 ld_pose(const double *p) { return SE3{{p[0], p[1], p[2], p[3]}, {p[4], p[5], p[6]}}; }
 
@@ -187,5 +188,89 @@ __device__ __noinline__ void assemble_node(const PoseGraphParams &P, int k, doub
                 }
                 Uk[6 * a + b] = Uk[6 * a + b] - s;
             }
+    }
+}
+
+// the candidate T_k Exp(d) of node k, from cur into cand; a fixed node's 8 doubles are copied as they are (d unread).
+// Returns max |d| (0 for a fixed node).
+__device__ __forceinline__ double candidate_pose(const PoseGraphParams &P, const double *cur, double *cand, long long k,
+                                                 const double *d) {
+    const double *src = cur + 8 * k;
+    double *dst = cand + 8 * k;
+    if (P.fixed[k]) {
+#pragma unroll
+        for (int a = 0; a < 8; ++a) dst[a] = src[a];
+        return 0.0;
+    }
+    double t[6], mx = 0.0;
+#pragma unroll
+    for (int a = 0; a < 6; ++a) {
+        t[a] = d[a];
+        mx = fmax(mx, fabs(t[a]));
+    }
+    st_pose(dst, se3_mul(ld_pose(src), se3_exp(t)));
+    return mx;
+}
+
+// Levenberg-Marquardt on the graph of P, both optimizers' loop: the lambda schedule, acceptance, the stopping rules in
+// their order, the poses back in P.pose and the report. The solver S runs every grid-wide part, with its own sums and
+// barriers:
+//   double S.linearize(poses): every edge's linearization at `poses`; returns the cost there
+//   void S.relinearize(poses): the same after an accepted step, the cost unused
+//   bool S.step(lambda, iteration, cur, cand, max_d, Fc): assemble (H + lambda diag H) at the linearization, solve it
+//     for d, write the candidate T_k Exp(d_k) of every node into cand (candidate_pose), max_d = max |d|, Fc = the cost
+//     at cand; false when the system did not factor (max_d and Fc left as they are)
+//   S.cg_iterations: PCG iterations in all; S.gt, S.gs: the thread's grid-stride start and stride of S.step's node loop
+template <class Solver>
+__device__ void lm_optimize(const PoseGraphParams &P, Solver &S) {
+    double *cur = P.pose, *cand = P.cand;
+    double F = S.linearize(cur);
+    const double F0 = F;
+    double lambda = P.initial_lambda;
+    int iterations = 0, accepted = 0, term = KB_PG_MAX_ITERATIONS;
+    while (iterations < P.max_iterations) {
+        double step = 0.0, Fc = NAN;
+        const bool factored = S.step(lambda, iterations, cur, cand, step, Fc);
+        ++iterations;
+        if (Fc < F) {  // (false for a non-finite cost)
+            double *t = cur;
+            cur = cand;
+            cand = t;
+            const double F_old = F;
+            F = Fc;
+            lambda = lambda / 10.0;
+            ++accepted;
+            S.relinearize(cur);
+            if (F_old - F <= P.function_tolerance * F_old) {
+                term = KB_PG_FUNCTION_TOLERANCE;
+                break;
+            }
+        } else {
+            lambda = lambda * 10.0;
+            if (lambda > 1e12) {
+                term = KB_PG_NO_DECREASE;
+                break;
+            }
+        }
+        if (factored && step <= P.parameter_tolerance) {
+            term = KB_PG_PARAMETER_TOLERANCE;
+            break;
+        }
+    }
+    if (cur != P.pose) {  // (each node's candidate was written by this thread)
+        for (long long k = S.gt; k < P.n_nodes; k += S.gs)
+#pragma unroll
+            for (int a = 0; a < 8; ++a) P.pose[8 * k + a] = cur[8 * k + a];
+    }
+    if (S.gt == 0) {
+        kb_pose_graph_report r;
+        r.iterations = iterations;
+        r.accepted = accepted;
+        r.cg_iterations = S.cg_iterations;
+        r.termination = term;
+        r.initial_cost = F0;
+        r.final_cost = F;
+        r.lambda = lambda;
+        *P.report = r;
     }
 }

@@ -115,3 +115,17 @@ __device__ __noinline__ void factor_column(const PgcFactorParams &F, int s) {
         }
     }
 }
+
+// The levels of the elimination tree from the leaves up: every block of a level's columns takes its updates (the leaves
+// have none), then every column its pivot and solves. A grid barrier between levels; none after the last.
+__device__ void factor_levels(Grid &g, const PgcFactorParams &F, int gt, int gs) {
+    for (int l = 0; l < F.levels; ++l) {
+        const int s0 = F.lev_ptr[l], s1 = F.lev_ptr[l + 1];
+        if (l > 0) {
+            for (int b = F.colptr[s0] + gt; b < F.colptr[s1]; b += gs) update_block(F, b);
+            g.sync();
+        }
+        for (int s = s0 + gt; s < s1; s += gs) factor_column(F, s);
+        if (l + 1 < F.levels) g.sync();
+    }
+}
