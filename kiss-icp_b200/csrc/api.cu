@@ -318,9 +318,11 @@ struct kb_registration {
     int max_iter;
     double conv;
     int threads;
-    Work ws;
-    DBuf<double> out;  // pose[16] + sys[NACC]
-    DBuf<int> iout;    // iters, ncorr
+    DBuf<double> src;   // [n][3] the source of the last call
+    DBuf<double> work;  // [n][3] source in the map frame (ICP iterate of the whole-grid loop)
+    DBuf<QList> qrec;   // per source point: candidate lists of the ICP team
+    DBuf<double> pose;  // [16] kb_registration_align_points_to_map's result
+    DBuf<int> iters;    // and its iterations
     int last_iters = 0;
     DBuf<BatchHyp> bhyp;  // kb_registration_align_batch: team hypotheses, then all hypotheses (inlier pass)
     DBuf<unsigned> bctl;
@@ -328,8 +330,9 @@ struct kb_registration {
     DBuf<int> biout;
     DBuf<double> rgrid;   // kb_relocalize: rotations [n_yaw][9], then xs [Nx], ys [Ny]
     DBuf<int> rscore;     // kb_relocalize: scores [H]
-    DBuf<double> plane_part;      // kb_registration_constraints: [PLANE_VALS][grid] per-CTA partials
-    DBuf<PlaneResult> plane_res;  // and the result
+    DBuf<double> part;         // k_pose_pass (build_system, constraints): [FIT_VALS or PLANE_VALS][grid] per-CTA partials
+    DBuf<FitResult> fit;       // and its result: the fit
+    DBuf<PlaneResult> planes;  // or the plane constraints
     Event rev[2];  // around the last k_reloc_score (kb_debug_reloc_score_ms), on the device of that call
 };
 
@@ -795,15 +798,14 @@ int kb_registration_destroy(kb_registration *reg) {
     delete reg;
     return KB_OK;
 }
-// one k_icp launch: AlignPointsToMap of the n points at d_src into out_pose / out_iters, or (system_only) one
-// BuildLinearSystem pass at the identity into reg->out[16..] and the correspondence count into reg->iout[1]
+// one k_icp launch: AlignPointsToMap of the n points at d_src into out_pose / out_iters
 static int icp_launch(kb_registration *reg, Exec &ex, const MapView &m, const double *d_src, int n, const SE3 &guess,
-                      double max_dist, double kscale, double *out_pose, int *out_iters, bool system_only = false) {
+                      double max_dist, double kscale, double *out_pose, int *out_iters) {
     IcpParams P{};
     P.m = m;
     P.sc = ex.sc;
     P.src = d_src;
-    P.work = reg->ws.work.p;
+    P.work = reg->work.p;
     P.n = n;
     P.guess = guess;
     P.max_dist = max_dist;
@@ -812,30 +814,24 @@ static int icp_launch(kb_registration *reg, Exec &ex, const MapView &m, const do
     P.conv = reg->conv;
     P.out_pose = out_pose;
     P.out_iters = out_iters;
-    if (system_only) {
-        P.system_only = 1;
-        P.out_sys = reg->out.p + 16;
-        P.out_ncorr = reg->iout.p + 1;
-    }
-    P.use_qcache = system_only ? 0 : 1;
     P.tag_base = ex.next_tag_base();
     P.team = ex.team;
-    P.team.qrec = reg->ws.qrec.p;
+    P.team.qrec = reg->qrec.p;
     P.icp_team_q = ex.icp_team_q;
-    return ex.coop(k_icp, P, system_only ? 0 : std::max<size_t>(QC_BYTES, ex.icp_smem));
+    return ex.coop(k_icp, P, std::max<size_t>(QC_BYTES, ex.icp_smem));
 }
 static int registration_run(kb_registration *reg, const double *xyz, size_t n, kb_map *map, const SE3 &guess,
-                            double max_dist, double kscale, bool system_only) {
+                            double max_dist, double kscale) {
     Exec &ex = *map->ex;
     CK(cudaSetDevice(ex.device));
-    RET(reg->ws.src.ensure(3 * std::max<size_t>(n, 1)));
-    RET(reg->ws.work.ensure(3 * std::max<size_t>(n, 1)));
-    RET(reg->out.ensure(16 + NACC));
-    RET(reg->iout.ensure(2));
-    RET(reg->ws.qrec.ensure(std::max<size_t>(n, 1)));
-    if (n) CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
-    return icp_launch(reg, ex, map->view(), reg->ws.src.p, static_cast<int>(n), guess, max_dist, kscale, reg->out.p,
-                      reg->iout.p, system_only);
+    RET(reg->src.ensure(3 * std::max<size_t>(n, 1)));
+    RET(reg->work.ensure(3 * std::max<size_t>(n, 1)));
+    RET(reg->pose.ensure(16));
+    RET(reg->iters.ensure(1));
+    RET(reg->qrec.ensure(std::max<size_t>(n, 1)));
+    if (n) CK(cudaMemcpyAsync(reg->src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
+    return icp_launch(reg, ex, map->view(), reg->src.p, static_cast<int>(n), guess, max_dist, kscale, reg->pose.p,
+                      reg->iters.p);
 }
 int kb_registration_align_points_to_map(kb_registration *reg, const double *xyz, size_t n, const kb_map *cmap,
                                         const double initial_guess[16], double max_correspondence_distance,
@@ -845,13 +841,36 @@ int kb_registration_align_points_to_map(kb_registration *reg, const double *xyz,
     SE3 g;
     if (!se3_from_matrix(initial_guess, &g)) return fail(KB_ERR_NOT_SE3, "initial_guess is not in SE(3)");
     RET(check_points(xyz, n, t_norm(g), map->voxel_size, "source point"));
-    RET(registration_run(reg, xyz, n, map, g, max_correspondence_distance, kernel_scale, false));
+    RET(registration_run(reg, xyz, n, map, g, max_correspondence_distance, kernel_scale));
     int it = 0;
-    CK(cudaMemcpyAsync(out_pose, reg->out.p, 16 * sizeof(double), cudaMemcpyDeviceToHost, map->ex->stream));
-    CK(cudaMemcpyAsync(&it, reg->iout.p, sizeof(int), cudaMemcpyDeviceToHost, map->ex->stream));
+    CK(cudaMemcpyAsync(out_pose, reg->pose.p, 16 * sizeof(double), cudaMemcpyDeviceToHost, map->ex->stream));
+    CK(cudaMemcpyAsync(&it, reg->iters.p, sizeof(int), cudaMemcpyDeviceToHost, map->ex->stream));
     RET(map->ex->sync());
     reg->last_iters = it;
     return KB_OK;
+}
+// one k_pose_pass launch: the fit (into reg->fit) or the plane constraints (into reg->planes) of the n points at xyz
+// mapped by `pose`
+static int pose_pass(kb_registration *reg, kb_map *map, const double *xyz, size_t n, const SE3 &pose, double max_dist,
+                     double kscale, bool fit) {
+    Exec &ex = *map->ex;
+    CK(cudaSetDevice(ex.device));
+    RET(reg->src.ensure(3 * std::max<size_t>(n, 1)));
+    RET(reg->part.ensure(static_cast<size_t>(std::max(FIT_VALS, PLANE_VALS)) * ex.grid));
+    RET(reg->fit.ensure(1));
+    RET(reg->planes.ensure(1));
+    if (n) CK(cudaMemcpyAsync(reg->src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
+    PosePassParams P{};
+    P.m = map->view();
+    P.sc = ex.sc;
+    P.src = reg->src.p;
+    P.n = static_cast<int>(n);
+    P.pose = pose;
+    P.max_dist = max_dist;
+    P.kscale = kscale;
+    P.fit = FitOut{reg->part.p, reg->fit.p};
+    P.planes = PlaneOut{reg->part.p, reg->planes.p};
+    return ex.coop_raw(pose_pass_kernel(fit), &P, 0, true);
 }
 // the upper triangle of the plane information matrix expanded to the symmetric 6x6
 static void planes_to_abi(const PlaneResult &r, kb_constraints *out) {
@@ -870,24 +889,10 @@ int kb_registration_constraints(kb_registration *reg, const double *xyz, size_t 
     if (n > static_cast<size_t>(INT_MAX)) return fail(KB_ERR_INVALID_ARG, "more than 2^31 - 1 source points");
     *out = kb_constraints{};
     if (n == 0) return KB_OK;
-    Exec &ex = *map->ex;
-    CK(cudaSetDevice(ex.device));
-    RET(reg->ws.src.ensure(3 * n));
-    RET(reg->plane_part.ensure(static_cast<size_t>(PLANE_VALS) * ex.grid));
-    RET(reg->plane_res.ensure(1));
-    CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
-    ConstraintsParams P{};
-    P.m = map->view();
-    P.sc = ex.sc;
-    P.src = reg->ws.src.p;
-    P.n = static_cast<int>(n);
-    P.pose = T;
-    P.max_dist = max_correspondence_distance;
-    P.planes = PlaneOut{reg->plane_part.p, reg->plane_res.p};
-    RET(ex.coop_raw(constraints_kernel(), &P, 0, true));
+    RET(pose_pass(reg, map, xyz, n, T, max_correspondence_distance, 0.0, false));
     PlaneResult r;
-    CK(cudaMemcpyAsync(&r, reg->plane_res.p, sizeof(r), cudaMemcpyDeviceToHost, ex.stream));
-    RET(ex.sync());
+    CK(cudaMemcpyAsync(&r, reg->planes.p, sizeof(r), cudaMemcpyDeviceToHost, map->ex->stream));
+    RET(map->ex->sync());
     planes_to_abi(r, out);
     return KB_OK;
 }
@@ -902,14 +907,12 @@ int kb_registration_build_system(kb_registration *reg, const double *xyz, size_t
     kb_map *map = const_cast<kb_map *>(cmap);
     if (!reg || !map || (!xyz && n) || !JTJ || !JTr) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     RET(check_points(xyz, n, 0.0, map->voxel_size, "point"));
-    RET(registration_run(reg, xyz, n, map, se3_identity(), max_correspondence_distance, kernel_scale, true));
-    double sys[NACC];
-    int nc = 0;
-    CK(cudaMemcpyAsync(sys, reg->out.p + 16, sizeof(sys), cudaMemcpyDeviceToHost, map->ex->stream));
-    CK(cudaMemcpyAsync(&nc, reg->iout.p + 1, sizeof(int), cudaMemcpyDeviceToHost, map->ex->stream));
+    RET(pose_pass(reg, map, xyz, n, se3_identity(), max_correspondence_distance, kernel_scale, true));
+    FitResult f;
+    CK(cudaMemcpyAsync(&f, reg->fit.p, sizeof(f), cudaMemcpyDeviceToHost, map->ex->stream));
     RET(map->ex->sync());
-    icp_expand(sys, JTJ, JTr);
-    if (n_correspondences) *n_correspondences = nc;
+    icp_expand(f.acc, JTJ, JTr);
+    if (n_correspondences) *n_correspondences = f.n_corr;
     return KB_OK;
 }
 
@@ -970,8 +973,8 @@ static int align_batch_run(kb_registration *reg, kb_map *map, const double *d_xy
     }
     RET(reg->bhyp.ensure(hyp.size()));
     CK(cudaMemcpyAsync(reg->bhyp.p, hyp.data(), hyp.size() * sizeof(BatchHyp), cudaMemcpyHostToDevice, ex.stream));
-    RET(reg->ws.qrec.ensure(std::max<size_t>(n_single, static_cast<size_t>(n_team))));
-    if (!single.empty()) RET(reg->ws.work.ensure(3 * n_single));
+    RET(reg->qrec.ensure(std::max<size_t>(n_single, static_cast<size_t>(n_team))));
+    if (!single.empty()) RET(reg->work.ensure(3 * n_single));
     for (size_t b : single)
         RET(icp_launch(reg, ex, mv, d_xyz + 3 * offset[b], static_cast<int>(count[b]), g[b], max_dist[b], kscale[b],
                        d_poses + 16 * b, d_iters + b));
@@ -989,7 +992,7 @@ static int align_batch_run(kb_registration *reg, kb_map *map, const double *d_xy
         P.sc.profile = 0;  // (the profiling stamps belong to single launches)
         P.team = ex.team;
         P.team.ll = ex.batch_ll.p;
-        P.team.qrec = reg->ws.qrec.p;
+        P.team.qrec = reg->qrec.p;
         P.src = d_xyz;
         P.hyp = reg->bhyp.p;
         P.nh = nh;
@@ -1026,11 +1029,11 @@ int kb_registration_align_batch(kb_registration *reg, const double *xyz, size_t 
     if (B == 0) return KB_OK;
     Exec &ex = *map->ex;
     CK(cudaSetDevice(ex.device));
-    RET(reg->ws.src.ensure(3 * std::max<size_t>(n_points, 1)));
+    RET(reg->src.ensure(3 * std::max<size_t>(n_points, 1)));
     RET(reg->bpose.ensure(16 * B));
     RET(reg->biout.ensure(2 * B));
-    if (n_points) CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n_points * 24, cudaMemcpyHostToDevice, ex.stream));
-    RET(align_batch_run(reg, map, reg->ws.src.p, offset, count, B, g, max_correspondence_distance, kernel_scale, reg->bpose.p,
+    if (n_points) CK(cudaMemcpyAsync(reg->src.p, xyz, n_points * 24, cudaMemcpyHostToDevice, ex.stream));
+    RET(align_batch_run(reg, map, reg->src.p, offset, count, B, g, max_correspondence_distance, kernel_scale, reg->bpose.p,
                         reg->biout.p, inliers ? reg->biout.p + B : nullptr));
     CK(cudaMemcpyAsync(poses, reg->bpose.p, 16 * B * sizeof(double), cudaMemcpyDeviceToHost, ex.stream));
     CK(cudaMemcpyAsync(iterations, reg->biout.p, B * sizeof(int), cudaMemcpyDeviceToHost, ex.stream));
@@ -1213,16 +1216,16 @@ int kb_relocalize(kb_registration *reg, const double *xyz, size_t n, const kb_ma
     std::vector<double> grid(g.rot);
     grid.insert(grid.end(), g.xs.begin(), g.xs.end());
     grid.insert(grid.end(), g.ys.begin(), g.ys.end());
-    RET(reg->ws.src.ensure(3 * n));
+    RET(reg->src.ensure(3 * n));
     RET(reg->rgrid.ensure(grid.size()));
     RET(reg->rscore.ensure(g.H));
     RET(events_on(reg->rev, ex.device));
-    CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
+    CK(cudaMemcpyAsync(reg->src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
     CK(cudaMemcpyAsync(reg->rgrid.p, grid.data(), grid.size() * sizeof(double), cudaMemcpyHostToDevice, ex.stream));
     const MapView mv = map->view();
     const double *d_rot = reg->rgrid.p, *d_xs = d_rot + g.rot.size(), *d_ys = d_xs + g.nx;
     CK(cudaEventRecord(reg->rev[0].p, ex.stream));
-    CK(reloc_score(mv, reg->ws.src.p, static_cast<int>(n), d_rot, g.n_yaw, d_xs, g.nx, d_ys, g.ny, g.tz,
+    CK(reloc_score(mv, reg->src.p, static_cast<int>(n), d_rot, g.n_yaw, d_xs, g.nx, d_ys, g.ny, g.tz,
                    reg->rscore.p, ex.sms, ex.stream));
     ++ex.launches;
     CK(cudaEventRecord(reg->rev[1].p, ex.stream));
@@ -1580,7 +1583,6 @@ static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, si
     P.max_iter = p->cfg.max_num_iterations;
     P.conv = p->cfg.convergence_criterion;
     P.min_motion_th = p->cfg.min_motion_th;
-    P.use_qcache = 1;
     P.tag_base = ex.next_tag_base();
     P.in_f32 = in_f32 ? 1 : 0;
     const size_t smem = std::max<size_t>(QC_BYTES, ex.icp_smem);
@@ -2291,14 +2293,14 @@ int kb_host::refine_candidates(kb_registration *reg, kb_map *map, const double *
     CK(cudaSetDevice(ex.device));
     const size_t K = guesses.size();
     if (xyz) {
-        RET(reg->ws.src.ensure(3 * n));
-        CK(cudaMemcpyAsync(reg->ws.src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
+        RET(reg->src.ensure(3 * n));
+        CK(cudaMemcpyAsync(reg->src.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
     }
     const std::vector<size_t> off(K, 0), cnt(K, n);
     const std::vector<double> md(K, max_dist), ks(K, kscale);
     RET(reg->bpose.ensure(16 * K));
     RET(reg->biout.ensure(2 * K));
-    RET(align_batch_run(reg, map, reg->ws.src.p, off.data(), cnt.data(), K, guesses, md.data(), ks.data(), reg->bpose.p,
+    RET(align_batch_run(reg, map, reg->src.p, off.data(), cnt.data(), K, guesses, md.data(), ks.data(), reg->bpose.p,
                         reg->biout.p, reg->biout.p + K));
     refined->resize(16 * K);
     std::vector<int> io(2 * K);  // iterations [K], inliers [K]

@@ -80,7 +80,6 @@ struct FrameParams {
     double max_range, min_range, voxel_size;
     int max_iter;
     double conv, min_motion_th;
-    int use_qcache;
     int icp_team_q;  // source points per CTA of the ICP team; 0: whole-grid loop (op_icp)
     unsigned tag_base;
 };
@@ -123,11 +122,11 @@ __device__ __noinline__ void op_front(Grid &g, const Scratch &sc, Shared &sh, co
     op_downsample(g, sc, sh, fr.ds1, n_ds, voxel_size * 1.5, ws.ds2, fr.src, &fr.cnt[2], t_ns ? &t_ns[16] : nullptr, true);
 }
 
-// ---- the fit of a frame (a reporting k_register_frame, kb_pipeline_last_fit) ---------------------------------------
-// DataAssociation + BuildLinearSystem (Registration.cpp:60-121) of the source mapped by the final pose, formed the way
-// kb_registration_build_system forms them (nn_search_warp, icp_term, expanded by icp_expand on the host), plus the
-// unweighted sum of |r|^2. Deterministic for a grid size: point qi -> CTA qi % G, warp (qi / G) % NWARPS, a lane sums
-// its warp's points in order, the warps of a CTA are added in warp order and the CTA partials in CTA order.
+// ---- the fit of a source at one pose (a reporting k_register_frame, kb_registration_build_system) ---------------------
+// DataAssociation + BuildLinearSystem (Registration.cpp:60-121) of the source mapped by the pose (nn_search_warp,
+// icp_term, expanded by icp_expand on the host), plus the unweighted sum of |r|^2. Deterministic for a grid size: point
+// qi -> CTA qi % G, warp (qi / G) % NWARPS, a lane sums its warp's points in order, the warps of a CTA are added in warp
+// order and the CTA partials in CTA order.
 constexpr int FIT_VALS = NACC + 2;  // accumulators, correspondences, sum of squared residuals
 struct FitResult {
     double acc[NACC];  // Geman-McClure-weighted accumulators of J^T W J and J^T W r (icp_term's layout)
@@ -177,14 +176,15 @@ struct ReportParams : FrameParams {
     FitOut fit;
     PlaneOut planes;
 };
-// the stand-alone pass (k_constraints): one source at one pose
-struct ConstraintsParams {
+// the stand-alone pass (k_pose_pass): one source at one pose, the fit or the plane constraints
+struct PosePassParams {
     MapView m;
     Scratch sc;
     const double *src;
     int n;
     SE3 pose;
-    double max_dist;
+    double max_dist, kscale;
+    FitOut fit;
     PlaneOut planes;
 };
 
@@ -415,7 +415,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
         __syncthreads();
     } else {
         op_icp(g, P.sc, sh, P.m, fr.src, P.ws.work, n_src, guess, 3.0 * sigma, sigma, P.max_iter, P.conv,
-               P.use_qcache ? reinterpret_cast<QCache *>(kb_dyn_smem) : nullptr, P.tag_base);
+               reinterpret_cast<QCache *>(kb_dyn_smem), P.tag_base);
         // Without ICP (empty map, max_iter <= 0) op_icp has no grid-wide rendezvous, and with a prefetched front end
         // (the replay of a vetoed first frame) neither has anything above. Every CTA must have read the state the
         // decisions above depend on (vetoed, the map counters) before any CTA starts the map update, which changes it.
@@ -503,6 +503,6 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
 }  // namespace kb
 
 // defined in report.cu, the reporting device module: k_register_frame<ReportParams, localizer, planes> (takes a
-// ReportParams) and the stand-alone k_constraints (takes a ConstraintsParams)
+// ReportParams) and the stand-alone k_pose_pass with the fit or with the plane constraints (takes a PosePassParams)
 const void *report_kernel(bool localizer, bool planes);
-const void *constraints_kernel();
+const void *pose_pass_kernel(bool fit);

@@ -73,33 +73,17 @@ struct IcpParams {
     double conv;
     double *out_pose;  // [16] row-major
     int *out_iters;
-    // build-system-only mode (one pass, no solve): out_sys[NACC], out_ncorr
-    int system_only;
-    double *out_sys;
-    int *out_ncorr;
-    int use_qcache;
     unsigned tag_base;
     TeamScratch team;
     int icp_team_q;  // source points per CTA of the ICP team; 0: whole-grid loop
 };
+// AlignPointsToMap (Registration.cpp:138-167) on a team of CTAs, or on the whole grid when icp_team_plan gives none
 __global__ void __launch_bounds__(BLOCK, 1) k_icp(const IcpParams P) {
     __shared__ Shared sh;
     Grid g;
     g.init(P.sc.bar);
-    if (P.system_only) {
-        icp_queries(P.sc, sh, P.m, P.src, P.work, P.n, se3_identity(), P.max_dist, P.kscale, P.tag_base + 1u, false);
-        icp_gather(P.sc, sh, P.tag_base + 1u, icp_group_size());
-        if (blockIdx.x == 0) {
-            if (threadIdx.x == 0) {
-                for (int i = 0; i < NACC; ++i) P.out_sys[i] = sh.red[i];
-                *P.out_ncorr = static_cast<int>(sh.red[NACC]);
-            }
-        }
-        return;
-    }
-    const int T = P.use_qcache ? icp_team_plan(P.m, __ldcg(&P.m.counters[C_LIVE]), P.max_iter, P.icp_team_q, P.n,
-                                               static_cast<int>(gridDim.x), P.team.smem_bytes)
-                               : 0;
+    const int T = icp_team_plan(P.m, __ldcg(&P.m.counters[C_LIVE]), P.max_iter, P.icp_team_q, P.n,
+                                static_cast<int>(gridDim.x), P.team.smem_bytes);
     if (T > 0) {
         icp_fill_pass(g, sh, P.m, P.src, P.n, P.guess, P.team.qrec, P.team.radius_frac, P.sc.bar + BAR_TICKET);
         g.sync();
@@ -108,7 +92,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_icp(const IcpParams P) {
                     kb_dyn_smem, T, P.tag_base);
     } else {
         op_icp(g, P.sc, sh, P.m, P.src, P.work, P.n, P.guess, P.max_dist, P.kscale, P.max_iter, P.conv,
-               P.use_qcache ? reinterpret_cast<QCache *>(kb_dyn_smem) : nullptr, P.tag_base);
+               reinterpret_cast<QCache *>(kb_dyn_smem), P.tag_base);
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         se3_to_matrix(sh.result, P.out_pose);

@@ -6,7 +6,8 @@
 // device watchdog's words (device_ops.cuh), which host.cu arms with the others through report_watchdog.
 //   k_register_frame<ReportParams, localizer, planes>  a localizer, or an odometry pipeline with fit reporting on,
 //                                                      with or without plane reporting
-//   k_constraints                                      kb_registration_constraints: the plane pass for one source at
+//   k_pose_pass<true, false>                           kb_registration_build_system: the fit of one source at one pose
+//   k_pose_pass<false, true>                           kb_registration_constraints: the plane pass for one source at
 //                                                      one pose
 #define kb kb_report
 #include "frame.cuh"
@@ -19,15 +20,21 @@ template __global__ void k_register_frame<ReportParams, true, false>(const Repor
 template __global__ void k_register_frame<ReportParams, true, true>(const ReportParams P);
 
 // cooperative: the pass, one grid barrier, the partials added by the last CTA (as in the pipeline kernels)
-__global__ void __launch_bounds__(BLOCK, 1) k_constraints(const ConstraintsParams P) {
+template <bool FIT, bool PLANES>
+__global__ void __launch_bounds__(BLOCK, 1) k_pose_pass(const PosePassParams P) {
     __shared__ Shared sh;
     Grid g;
     g.init(P.sc.bar);
-    op_fit_planes<false, true>(sh, P.m, P.src, P.n, P.pose, P.max_dist, 0.0, nullptr, P.planes.part);
+    op_fit_planes<FIT, PLANES>(sh, P.m, P.src, P.n, P.pose, P.max_dist, P.kscale, P.fit.part, P.planes.part);
     g.sync();
-    if (blockIdx.x == gridDim.x - 1) planes_finish(P.planes);
+    if (blockIdx.x == gridDim.x - 1) {
+        if constexpr (FIT) fit_finish(P.fit, P.n);
+        if constexpr (PLANES) planes_finish(P.planes);
+    }
     g.finish();
 }
+template __global__ void k_pose_pass<true, false>(const PosePassParams P);
+template __global__ void k_pose_pass<false, true>(const PosePassParams P);
 }  // namespace kb_report
 
 const void *report_kernel(bool localizer, bool planes) {
@@ -40,6 +47,10 @@ const void *report_kernel(bool localizer, bool planes) {
          reinterpret_cast<const void *>(&k_register_frame<ReportParams, true, true>)}};
     return kernels[localizer][planes];
 }
-const void *constraints_kernel() { return reinterpret_cast<const void *>(&kb_report::k_constraints); }
+const void *pose_pass_kernel(bool fit) {
+    using kb_report::k_pose_pass;
+    return fit ? reinterpret_cast<const void *>(&k_pose_pass<true, false>)
+               : reinterpret_cast<const void *>(&k_pose_pass<false, true>);
+}
 
 cudaError_t report_watchdog(unsigned *d_host_words, const unsigned *init) { return kb_report::watchdog_arm(d_host_words, init); }
