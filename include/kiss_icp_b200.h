@@ -502,11 +502,22 @@ int kb_place_relocalize(kb_registration *reg, kb_place_db *db, const double *des
 /* ---- pose graph: loop closure --------------------------------------------------------------------------------------
  * No reference counterpart. Nodes are poses T_i (row-major SE(3)); a fixed node does not move. An edge
  * e = (i, j, Z, Omega, c) has the residual r_e = Log(Z^-1 T_i^-1 T_j) in R^6, in the tangent order (translation,
- * rotation) of the library, s_e = r_e^T Omega r_e, and the cost F = 1/2 sum_e rho_e(s_e) with rho(s) = s for c = 0 and
- * the Cauchy loss rho(s) = c^2 log(1 + s / c^2) for c > 0; w_e = rho'(s_e).
+ * rotation) of the library, s_e = r_e^T Omega r_e, and the cost F = 1/2 (sum_e rho_e(s_e) + sum_p rho_p(s_p)) with
+ * rho(s) = s for c = 0 and the Cauchy loss rho(s) = c^2 log(1 + s / c^2) for c > 0; w_e = rho'(s_e).
+ * A prior p is a unary factor on one node k, with its own Omega and Cauchy scale c, s_p = r_p^T Omega r_p and
+ * w_p = rho'(s_p) as for edges. Two kinds (kb_pose_graph_add_pose_prior, kb_pose_graph_add_position_prior):
+ *   pose prior (k, Z, Omega 6x6, c): r_p = Log(Z^-1 T_k), dr/dd_k = J_r^-1(r_p);
+ *   position prior (k, p, lever arm l in the body frame, Omega 3x3 in the world frame, c): r_p = R_k l + t_k - p in
+ *   R^3, dr/dd_k = [R_k, -R_k [l]x], e.g. a GNSS antenna l away from the body origin.
+ * A prior adds only to its node's diagonal block and gradient, after the node's edges (and nothing on a fixed node, whose
+ * prior adds a constant to F). The gauge: every connected component of free nodes must hold a fixed node or a node with
+ * a prior, so a graph with priors needs no fixed node. Position priors fix a component's rotation only through at least
+ * 3 non-collinear antenna positions; on fewer, the damped steps still solve, but kb_pose_graph_marginals reports H as
+ * not positive definite. A graph without priors computes exactly what it computed before priors existed.
  * kb_pose_graph_optimize moves the free nodes by right perturbation, T_i <- T_i Exp(d_i), with Levenberg-Marquardt on
  * IRLS weights and exact Jacobians (dr/dd_j = J_r^-1(r), dr/dd_i = -J_r^-1(r) Ad(T_j^-1 T_i)):
- *   H = sum J^T w Omega J, g = sum J^T w Omega r over the free nodes; (H + lambda diag H) d = -g is solved by PCG
+ *   H = sum J^T w Omega J, g = sum J^T w Omega r over the free nodes (edges, then priors); (H + lambda diag H) d = -g
+ *   is solved by PCG
  *   preconditioned by the exact inverse of M, the block-tridiagonal part of the damped system (the edges with
  *   |i - j| = 1 in full, every other edge's two diagonal blocks, the damping), which block cyclic reduction factors once
  *   per step. PCG stops at |r_k| <= cg_tolerance |g| or after max_cg_iterations.
@@ -521,8 +532,9 @@ int kb_place_relocalize(kb_registration *reg, kb_place_db *db, const double *des
  * Every argument is checked before any work and nothing is written on error: KB_ERR_NOT_SE3 for a pose or measurement
  * outside SE(3) (non-finite included); KB_ERR_INVALID_ARG for a NULL argument, i == j, a node that does not exist,
  * information that is not exactly symmetric, not finite or not positive definite, a negative or non-finite
- * robust_scale, more than 2^22 nodes or 2^24 edges, options out of range, and at optimize a free node that no path of
- * edges connects to a fixed node. Without a device, optimize returns KB_ERR_NO_DEVICE after these checks. */
+ * robust_scale, more than 2^22 nodes, 2^24 edges or 2^24 priors, a non-finite prior position or lever arm, options out
+ * of range, and at optimize a free node that no path of edges connects to a fixed node or a prior. Without a device,
+ * optimize returns KB_ERR_NO_DEVICE after these checks. */
 typedef struct kb_pose_graph kb_pose_graph;
 int kb_pose_graph_create(kb_pose_graph **out); /* host-side; needs no device */
 int kb_pose_graph_destroy(kb_pose_graph *g);
@@ -531,6 +543,17 @@ int kb_pose_graph_add_node(kb_pose_graph *g, const double pose[16], int fixed, s
 /* information: row-major 6x6 in the tangent order; robust_scale: c (0 = squared loss). *index may be NULL. */
 int kb_pose_graph_add_edge(kb_pose_graph *g, size_t i, size_t j, const double measurement[16],
                            const double information[36], double robust_scale, size_t *index);
+/* Priors of both kinds share one index space, in the order they are added; *index (may be NULL) = the new prior's.
+ * pose: row-major SE(3) Z; information: row-major 6x6 in the tangent order; robust_scale: c (0 = squared loss). */
+int kb_pose_graph_add_pose_prior(kb_pose_graph *g, size_t k, const double pose[16], const double information[36],
+                                 double robust_scale, size_t *index);
+/* position: p in the world frame; lever_arm: l in node k's body frame; information: row-major 3x3 in the world frame */
+int kb_pose_graph_add_position_prior(kb_pose_graph *g, size_t k, const double position[3], const double lever_arm[3],
+                                     const double information[9], double robust_scale, size_t *index);
+int kb_pose_graph_num_priors(const kb_pose_graph *g, size_t *n);
+/* s_p and w_p of every prior at the graph's current poses; host-side, needs no device. Two-call: *n_out = P; chi2 and
+ * weight (double[P], either may be NULL) both NULL or cap 0 only queries it, cap < P is KB_ERR_CAPACITY (with *n_out) */
+int kb_pose_graph_prior_chi2(const kb_pose_graph *g, double *chi2, double *weight, size_t cap, size_t *n_out);
 int kb_pose_graph_size(const kb_pose_graph *g, size_t *n_nodes, size_t *n_edges);
 /* two-call: *n_out = N; poses (double[N][16]) NULL or cap 0 only queries it, cap < N is KB_ERR_CAPACITY (with *n_out) */
 int kb_pose_graph_poses(const kb_pose_graph *g, double *poses, size_t cap, size_t *n_out);
@@ -566,8 +589,8 @@ int kb_pose_graph_optimize(kb_pose_graph *g, const kb_pose_graph_options *o, kb_
  * covers little of H and a step takes many PCG iterations; the exact step takes one factorization. On a pure chain PCG
  * is exact in one iteration and needs fewer grid barriers.
  * One cooperative launch per call. The results are bit-identical from run to run and for every grid size: the factor
- * and the solves are formed in a fixed order, and the cost is summed over fixed chunks of edges, then the chunks in
- * index order. The symbolic analysis stays cached for the graph's size; the numeric factor the call leaves behind is of
+ * and the solves are formed in a fixed order, and the cost is summed over fixed chunks of factors (the edges, then the
+ * priors), then the chunks in index order. The symbolic analysis stays cached for the graph's size; the numeric factor the call leaves behind is of
  * the damped system, so the next kb_pose_graph_marginals factors H again at the new poses. kb_debug_pose_graph_ms
  * times this call's launch as it times kb_pose_graph_optimize's.
  * Checked before any work, in the order of kb_pose_graph_optimize and with its codes, writing nothing on error; in
@@ -581,7 +604,8 @@ int kb_pose_graph_optimize_direct(kb_pose_graph *g, const kb_pose_graph_options 
  *   H = sum_e J_e^T w_e Omega_e J_e over the free nodes, with the optimizer's exact Jacobians
  *   (dr/dd_j = J_r^-1(r), dr/dd_i = -J_r^-1(r) Ad(T_j^-1 T_i)) and w_e = rho'(s_e) at those poses; no damping. An edge
  *   with one fixed node adds only the free node's diagonal block, an edge between two fixed nodes nothing; parallel
- *   edges between one pair add up in ascending edge order.
+ *   edges between one pair add up in ascending edge order. Priors add J^T w Omega J to their free node's diagonal
+ *   block, after its edges.
  *   Sigma = H^-1, in the tangent space of the right perturbation T_k Exp(d_k), order (translation, rotation). A fixed
  *   node's rows and columns are exactly 0.
  * Sigma is the Gauss-Newton (Laplace) approximation at those poses. It is not rescaled by the residuals: Omega is taken
@@ -591,11 +615,11 @@ int kb_pose_graph_optimize_direct(kb_pose_graph *g, const kb_pose_graph_options 
  * on the elimination-tree path from k's column to its root, summed over the common part of the two paths (Sigma_ij = 0
  * when the two lie in different trees). Every value is formed by one thread in a fixed order: the results are
  * bit-identical from run to run and for every grid size, and a diagonal block is exactly symmetric.
- * The symbolic analysis is cached for the graph's size, the numeric factor until the next add_node, add_edge or
- * optimize; neither changes what optimize computes.
+ * The symbolic analysis is cached for the graph's size, the numeric factor until the next add_node, add_edge,
+ * add_*_prior or optimize; neither changes what optimize computes.
  * Checked before any device work, writing nothing on error: KB_ERR_INVALID_ARG for NULL with n > 0, a node that does
- * not exist, a free node that no path of edges connects to a fixed node, and (after the factorization) an H that is not
- * positive definite at the current poses; then KB_ERR_NO_DEVICE without a device. n == 0 does nothing. */
+ * not exist, a free node that no path of edges connects to a fixed node or a prior, and (after the factorization) an H
+ * that is not positive definite at the current poses; then KB_ERR_NO_DEVICE without a device. n == 0 does nothing. */
 /* cov: double[n][36], the row-major 6x6 Sigma_kk of each nodes[t] */
 int kb_pose_graph_marginals(kb_pose_graph *g, const size_t *nodes, size_t n, double *cov);
 /* pairs: size_t[n][2]; cov: double[n][144], the row-major 12x12 [[Sigma_ii, Sigma_ij], [Sigma_ji, Sigma_jj]] of each

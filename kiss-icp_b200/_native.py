@@ -277,6 +277,10 @@ SIGNATURES = {
     "kb_pose_graph_destroy": (i32, [vp]),
     "kb_pose_graph_add_node": (i32, [vp, vp, i32, C.POINTER(sz)]),
     "kb_pose_graph_add_edge": (i32, [vp, sz, sz, vp, vp, dbl, C.POINTER(sz)]),
+    "kb_pose_graph_add_pose_prior": (i32, [vp, sz, vp, vp, dbl, C.POINTER(sz)]),
+    "kb_pose_graph_add_position_prior": (i32, [vp, sz, vp, vp, vp, dbl, C.POINTER(sz)]),
+    "kb_pose_graph_num_priors": (i32, [vp, C.POINTER(sz)]),
+    "kb_pose_graph_prior_chi2": (i32, [vp, vp, vp, sz, C.POINTER(sz)]),
     "kb_pose_graph_size": (i32, [vp, C.POINTER(sz), C.POINTER(sz)]),
     "kb_pose_graph_poses": (i32, [vp, vp, sz, C.POINTER(sz)]),
     "kb_pose_graph_options_default": (None, [C.POINTER(PoseGraphOptions)]),

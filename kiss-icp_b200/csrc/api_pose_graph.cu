@@ -13,14 +13,18 @@
 #include "pose_graph_cov.cuh"
 #include "se3.cuh"
 
+namespace kb {
+#include "pose_graph_priors.cuh"
+}  // namespace kb
+
 using namespace kb;
 using namespace kb_host;
 
 extern "C" {
 
 // The graph lives on the host (kb_pose_graph_* in the header state the problem and the method; pose_graph.cu has the
-// kernel). Edges are immutable, so an optimize uploads only those added since the last one; the poses, the fixed flags
-// and the incidence lists are uploaded every time.
+// kernel). Edges and priors are immutable, so an optimize uploads only those added since the last one; the poses, the
+// fixed flags and the incidence lists (of edges and of priors) are uploaded every time.
 struct kb_pose_graph {
     int device = 0;                  // of the creating thread: where the buffers go at the first optimize
     cudaStream_t user_stream = nullptr;
@@ -31,15 +35,23 @@ struct kb_pose_graph {
     std::vector<double> meas_inv;    // [E][8] Z^-1
     std::vector<double> info;        // [E][36]
     std::vector<double> robust;      // [E]
+    std::vector<int> p_node_kind;    // [P][2] priors: node, PG_POSE_PRIOR or PG_POSITION_PRIOR
+    std::vector<double> p_meas;      // [P][8] Z^-1 as q(4) t(3), or p(3) l(3)
+    std::vector<double> p_info;      // [P][36] (a position prior's 3x3 in the top-left corner)
+    std::vector<double> p_robust;    // [P]
     std::shared_ptr<Exec> ex;
     size_t uploaded = 0;             // edges on the device
+    size_t p_uploaded = 0;           // priors on the device
     DBuf<double> pose_d, cand, hd, grad, D, U, UL, vec, part;
     DBuf<double> meas_d, info_d, rob_d, e_s, e_w, e_jj, e_ii, e_ad, e_g;
     DBuf<int> fixed_d, inc_ptr, inc, ij_d, flag;
+    DBuf<double> p_meas_d, p_info_d, p_rob_d, p_s, p_w, p_h, p_g;
+    DBuf<int> p_nk_d, pinc_ptr, pinc;
     DBuf<kb_pose_graph_report> report;
     Event ev[2];                     // around the last launch (kb_debug_pose_graph_ms)
     // the covariance (kb_pose_graph_marginals & co.): the symbolic analysis for (N, E), its copy on the device, the
-    // numeric factor at the current poses (valid until the next add_node, add_edge or optimize) and the solves
+    // numeric factor at the current poses (valid until the next add_node, add_edge, add_*_prior or optimize) and the
+    // solves
     PgcSymbolic sym;
     int sym_dev_n = -1, sym_dev_e = -1;  // the graph the device copy of `sym` was made for
     bool factored = false;
@@ -51,9 +63,11 @@ struct kb_pose_graph {
     Event cev[4];                    // around the last factorization and the last marginal solves (kb_debug_pose_graph_cov_ms)
     size_t n() const { return fixed.size(); }
     size_t m() const { return robust.size(); }
+    size_t np() const { return p_robust.size(); }
 };
 
 static constexpr size_t kPoseGraphMaxNodes = size_t(1) << 22, kPoseGraphMaxEdges = size_t(1) << 24;
+static constexpr size_t kPoseGraphMaxPriors = size_t(1) << 24;
 
 static int pg_se3_arg(const double M[16], const char *what, SE3 *out) {
     if (!M) return fail(KB_ERR_INVALID_ARG, "NULL argument");
@@ -75,7 +89,35 @@ static int pg_options_check(const kb_pose_graph_options &o) {
     return KB_OK;
 }
 
-// every free node reaches a fixed node through edges (the gauge): union-find over the edges
+// information (n x n, row-major): finite, exactly symmetric and positive definite (Cholesky)
+static int pg_information_check(const double *information, int n) {
+    for (int k = 0; k < n * n; ++k)
+        if (!std::isfinite(information[k])) return fail(KB_ERR_INVALID_ARG, "information is not finite");
+    for (int a = 0; a < n; ++a)
+        for (int b = 0; b < a; ++b)
+            if (information[n * a + b] != information[n * b + a]) return fail(KB_ERR_INVALID_ARG, "information is not symmetric");
+    double L[36] = {};
+    for (int c = 0; c < n; ++c) {
+        double d = information[(n + 1) * c];
+        for (int k = 0; k < c; ++k) d -= L[n * c + k] * L[n * c + k];
+        if (!(d > 0.0)) return fail(KB_ERR_INVALID_ARG, "information is not positive definite");
+        L[(n + 1) * c] = std::sqrt(d);
+        for (int r = c + 1; r < n; ++r) {
+            double s = information[n * r + c];
+            for (int k = 0; k < c; ++k) s -= L[n * r + k] * L[n * c + k];
+            L[n * r + c] = s / L[(n + 1) * c];
+        }
+    }
+    return KB_OK;
+}
+
+static int pg_robust_check(double robust_scale) {
+    if (!(robust_scale >= 0.0) || !std::isfinite(robust_scale)) return fail(KB_ERR_INVALID_ARG, "robust_scale must be finite and >= 0");
+    return KB_OK;
+}
+
+// every connected component of free nodes holds a fixed node or a node with a prior (the gauge): union-find over the
+// edges
 static int pg_gauge_check(const kb_pose_graph &g) {
     const size_t N = g.n();
     std::vector<size_t> parent(N);
@@ -91,9 +133,11 @@ static int pg_gauge_check(const kb_pose_graph &g) {
     std::vector<char> grounded(N, 0);
     for (size_t k = 0; k < N; ++k)
         if (g.fixed[k]) grounded[root(k)] = 1;
+    for (size_t p = 0; p < g.np(); ++p) grounded[root(static_cast<size_t>(g.p_node_kind[2 * p]))] = 1;
     for (size_t k = 0; k < N; ++k)
         if (!grounded[root(k)])
-            return fail(KB_ERR_INVALID_ARG, "node %zu is free and no path of edges connects it to a fixed node (the gauge is free)", k);
+            return fail(KB_ERR_INVALID_ARG,
+                        "node %zu is free and no path of edges connects it to a fixed node or a prior (the gauge is free)", k);
     return KB_OK;
 }
 
@@ -128,14 +172,27 @@ static int pg_reserve(kb_pose_graph *g, int grid) {
     RET(g->e_ii.ensure(36 * E));
     RET(g->e_ad.ensure(36 * E));
     RET(g->e_g.ensure(6 * E));
+    const size_t Pr = std::max<size_t>(g->np(), 1);
+    RET(g->pinc_ptr.ensure(N + 1));
+    RET(g->pinc.ensure(Pr));
+    if (2 * Pr > g->p_nk_d.n || 8 * Pr > g->p_meas_d.n || 36 * Pr > g->p_info_d.n || Pr > g->p_rob_d.n) g->p_uploaded = 0;
+    RET(g->p_nk_d.ensure(2 * Pr));
+    RET(g->p_meas_d.ensure(8 * Pr));
+    RET(g->p_info_d.ensure(36 * Pr));
+    RET(g->p_rob_d.ensure(Pr));
+    RET(g->p_s.ensure(Pr));
+    RET(g->p_w.ensure(Pr));
+    RET(g->p_h.ensure(36 * Pr));
+    RET(g->p_g.ensure(6 * Pr));
     return KB_OK;
 }
 
-// the graph's current state on the device: poses, fixed flags, incidence lists (each node's edges ascending: the order
-// its blocks are summed in) and the edges added since the last upload; *P_out gets the graph's buffers, *pq_out the
-// poses as uploaded. g->uploaded is advanced by the caller once the stream has run.
+// the graph's current state on the device: poses, fixed flags, incidence lists (each node's edges ascending, then its
+// priors ascending: the order its blocks are summed in) and the edges and priors added since the last upload; *P_out
+// gets the graph's buffers, *pq_out the poses as uploaded. g->uploaded and g->p_uploaded are advanced by the caller
+// once the stream has run (pg_uploaded).
 static int pg_upload(kb_pose_graph *g, std::vector<double> *pq_out, PoseGraphParams *P_out) {
-    const size_t N = g->n(), E = g->m();
+    const size_t N = g->n(), E = g->m(), Pr = g->np();
     std::vector<double> &pq = *pq_out;
     pq.assign(8 * N, 0.0);
     for (size_t k = 0; k < N; ++k) {
@@ -153,6 +210,13 @@ static int pg_upload(kb_pose_graph *g, std::vector<double> *pq_out, PoseGraphPar
             inc[at[g->ij[2 * e + 1]]++] = static_cast<int>(e);
         }
     }
+    std::vector<int> pinc_ptr(N + 1, 0), pinc(Pr);
+    for (size_t p = 0; p < Pr; ++p) ++pinc_ptr[static_cast<size_t>(g->p_node_kind[2 * p]) + 1];
+    for (size_t k = 0; k < N; ++k) pinc_ptr[k + 1] += pinc_ptr[k];
+    {
+        std::vector<int> at(pinc_ptr.begin(), pinc_ptr.end() - 1);
+        for (size_t p = 0; p < Pr; ++p) pinc[at[g->p_node_kind[2 * p]]++] = static_cast<int>(p);
+    }
     cudaStream_t s = g->ex->stream;
     if (N) {
         CK(cudaMemcpyAsync(g->pose_d.p, pq.data(), 8 * N * sizeof(double), cudaMemcpyHostToDevice, s));
@@ -166,6 +230,15 @@ static int pg_upload(kb_pose_graph *g, std::vector<double> *pq_out, PoseGraphPar
         CK(cudaMemcpyAsync(g->meas_d.p + 8 * a, &g->meas_inv[8 * a], 8 * n * sizeof(double), cudaMemcpyHostToDevice, s));
         CK(cudaMemcpyAsync(g->info_d.p + 36 * a, &g->info[36 * a], 36 * n * sizeof(double), cudaMemcpyHostToDevice, s));
         CK(cudaMemcpyAsync(g->rob_d.p + a, &g->robust[a], n * sizeof(double), cudaMemcpyHostToDevice, s));
+    }
+    CK(cudaMemcpyAsync(g->pinc_ptr.p, pinc_ptr.data(), (N + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (Pr) CK(cudaMemcpyAsync(g->pinc.p, pinc.data(), Pr * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (Pr > g->p_uploaded) {
+        const size_t a = g->p_uploaded, n = Pr - a;
+        CK(cudaMemcpyAsync(g->p_nk_d.p + 2 * a, &g->p_node_kind[2 * a], 2 * n * sizeof(int), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->p_meas_d.p + 8 * a, &g->p_meas[8 * a], 8 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->p_info_d.p + 36 * a, &g->p_info[36 * a], 36 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(g->p_rob_d.p + a, &g->p_robust[a], n * sizeof(double), cudaMemcpyHostToDevice, s));
     }
     PoseGraphParams &P = *P_out;
     P = PoseGraphParams{};
@@ -187,6 +260,17 @@ static int pg_upload(kb_pose_graph *g, std::vector<double> *pq_out, PoseGraphPar
     P.e_ii = g->e_ii.p;
     P.e_ad = g->e_ad.p;
     P.e_g = g->e_g.p;
+    P.n_priors = static_cast<int>(Pr);
+    P.p_node_kind = g->p_nk_d.p;
+    P.p_meas = g->p_meas_d.p;
+    P.p_info = g->p_info_d.p;
+    P.p_robust = g->p_rob_d.p;
+    P.pinc_ptr = g->pinc_ptr.p;
+    P.pinc = g->pinc.p;
+    P.p_s = g->p_s.p;
+    P.p_w = g->p_w.p;
+    P.p_h = g->p_h.p;
+    P.p_g = g->p_g.p;
     P.hd = g->hd.p;
     P.g = g->grad.p;
     P.D = g->D.p;
@@ -203,6 +287,11 @@ static int pg_upload(kb_pose_graph *g, std::vector<double> *pq_out, PoseGraphPar
     P.flag = g->flag.p;
     P.report = g->report.p;
     return KB_OK;
+}
+// what pg_upload sent is on the device (after the stream ran)
+static void pg_uploaded(kb_pose_graph *g) {
+    g->uploaded = g->m();
+    g->p_uploaded = g->np();
 }
 
 // the options of an optimize call, checked; the defaults for NULL
@@ -261,24 +350,8 @@ int kb_pose_graph_add_edge(kb_pose_graph *g, size_t i, size_t j, const double me
     RET(pg_se3_arg(measurement, "measurement", &Z));
     if (i == j) return fail(KB_ERR_INVALID_ARG, "an edge joins two different nodes (i == j == %zu)", i);
     if (i >= g->n() || j >= g->n()) return fail(KB_ERR_INVALID_ARG, "node %zu does not exist (%zu nodes)", std::max(i, j), g->n());
-    for (int k = 0; k < 36; ++k)
-        if (!std::isfinite(information[k])) return fail(KB_ERR_INVALID_ARG, "information is not finite");
-    for (int a = 0; a < 6; ++a)
-        for (int b = 0; b < a; ++b)
-            if (information[6 * a + b] != information[6 * b + a]) return fail(KB_ERR_INVALID_ARG, "information is not symmetric");
-    double L[36] = {};
-    for (int c = 0; c < 6; ++c) {  // Cholesky: positive definite
-        double d = information[7 * c];
-        for (int k = 0; k < c; ++k) d -= L[6 * c + k] * L[6 * c + k];
-        if (!(d > 0.0)) return fail(KB_ERR_INVALID_ARG, "information is not positive definite");
-        L[7 * c] = std::sqrt(d);
-        for (int r = c + 1; r < 6; ++r) {
-            double s = information[6 * r + c];
-            for (int k = 0; k < c; ++k) s -= L[6 * r + k] * L[6 * c + k];
-            L[6 * r + c] = s / L[7 * c];
-        }
-    }
-    if (!(robust_scale >= 0.0) || !std::isfinite(robust_scale)) return fail(KB_ERR_INVALID_ARG, "robust_scale must be finite and >= 0");
+    RET(pg_information_check(information, 6));
+    RET(pg_robust_check(robust_scale));
     if (g->m() >= kPoseGraphMaxEdges) return fail(KB_ERR_INVALID_ARG, "the graph holds 2^24 edges");
     const SE3 Zi = se3_inverse(Z);
     const double zi[8] = {Zi.q.x, Zi.q.y, Zi.q.z, Zi.q.w, Zi.t.x, Zi.t.y, Zi.t.z, 0.0};
@@ -289,6 +362,69 @@ int kb_pose_graph_add_edge(kb_pose_graph *g, size_t i, size_t j, const double me
     g->robust.push_back(robust_scale);
     g->factored = false;
     if (index) *index = g->m() - 1;
+    return KB_OK;
+}
+// a prior of either kind on node k, its arguments checked by the caller
+static void pg_push_prior(kb_pose_graph *g, size_t k, int kind, const double meas[8], const double info[36],
+                          double robust_scale, size_t *index) {
+    g->p_node_kind.push_back(static_cast<int>(k));
+    g->p_node_kind.push_back(kind);
+    g->p_meas.insert(g->p_meas.end(), meas, meas + 8);
+    g->p_info.insert(g->p_info.end(), info, info + 36);
+    g->p_robust.push_back(robust_scale);
+    g->factored = false;
+    if (index) *index = g->np() - 1;
+}
+int kb_pose_graph_add_pose_prior(kb_pose_graph *g, size_t k, const double pose[16], const double information[36],
+                                 double robust_scale, size_t *index) {
+    if (!g || !information) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    SE3 Z;
+    RET(pg_se3_arg(pose, "pose", &Z));
+    if (k >= g->n()) return fail(KB_ERR_INVALID_ARG, "node %zu does not exist (%zu nodes)", k, g->n());
+    RET(pg_information_check(information, 6));
+    RET(pg_robust_check(robust_scale));
+    if (g->np() >= kPoseGraphMaxPriors) return fail(KB_ERR_INVALID_ARG, "the graph holds 2^24 priors");
+    const SE3 Zi = se3_inverse(Z);
+    const double zi[8] = {Zi.q.x, Zi.q.y, Zi.q.z, Zi.q.w, Zi.t.x, Zi.t.y, Zi.t.z, 0.0};
+    pg_push_prior(g, k, PG_POSE_PRIOR, zi, information, robust_scale, index);
+    return KB_OK;
+}
+int kb_pose_graph_add_position_prior(kb_pose_graph *g, size_t k, const double position[3], const double lever_arm[3],
+                                     const double information[9], double robust_scale, size_t *index) {
+    if (!g || !position || !lever_arm || !information) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (k >= g->n()) return fail(KB_ERR_INVALID_ARG, "node %zu does not exist (%zu nodes)", k, g->n());
+    for (int a = 0; a < 3; ++a)
+        if (!std::isfinite(position[a]) || !std::isfinite(lever_arm[a]))
+            return fail(KB_ERR_INVALID_ARG, "position and lever_arm must be finite");
+    RET(pg_information_check(information, 3));
+    RET(pg_robust_check(robust_scale));
+    if (g->np() >= kPoseGraphMaxPriors) return fail(KB_ERR_INVALID_ARG, "the graph holds 2^24 priors");
+    const double m[8] = {position[0], position[1], position[2], lever_arm[0], lever_arm[1], lever_arm[2], 0.0, 0.0};
+    double info[36] = {};
+    for (int a = 0; a < 3; ++a)
+        for (int b = 0; b < 3; ++b) info[6 * a + b] = information[3 * a + b];
+    pg_push_prior(g, k, PG_POSITION_PRIOR, m, info, robust_scale, index);
+    return KB_OK;
+}
+int kb_pose_graph_num_priors(const kb_pose_graph *g, size_t *n) {
+    if (!g || !n) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *n = g->np();
+    return KB_OK;
+}
+int kb_pose_graph_prior_chi2(const kb_pose_graph *g, double *chi2, double *weight, size_t cap, size_t *n_out) {
+    if (!g || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    const size_t Pr = g->np();
+    *n_out = Pr;
+    if ((!chi2 && !weight) || cap == 0) return KB_OK;
+    if (cap < Pr) return fail(KB_ERR_CAPACITY, "buffer too small (%zu < %zu priors)", cap, Pr);
+    for (size_t p = 0; p < Pr; ++p) {
+        double r[6], rho, w;
+        const double s = prior_residual(g->p_node_kind[2 * p + 1], &g->p_meas[8 * p], &g->p_info[36 * p],
+                                        g->pose[g->p_node_kind[2 * p]], r);
+        robust_loss(s, g->p_robust[p], &rho, &w);
+        if (chi2) chi2[p] = s;
+        if (weight) weight[p] = w;
+    }
     return KB_OK;
 }
 int kb_pose_graph_size(const kb_pose_graph *g, size_t *n_nodes, size_t *n_edges) {
@@ -323,11 +459,11 @@ static int pg_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_po
     Exec &ex = *g->ex;
     CK(cudaSetDevice(ex.device));
     const PgcSymbolic &S = g->sym;
-    const size_t N = g->n(), E = g->m();
+    const size_t N = g->n(), E = g->m(), NF = E + g->np();  // (NF: the factors, edges and priors)
     int co_resident = 0;
     CK(direct ? pgc_optimize_max_grid(ex.sms, &co_resident) : pose_graph_max_grid(ex.sms, &co_resident));
-    const int grid = direct ? pg_grid(ex, co_resident, std::max({N, E, S.blocks()}), PGC_BLOCK)
-                            : pg_grid(ex, co_resident, std::max(N, E), POSE_GRAPH_BLOCK);
+    const int grid = direct ? pg_grid(ex, co_resident, std::max({N, NF, S.blocks()}), PGC_BLOCK)
+                            : pg_grid(ex, co_resident, std::max(N, NF), POSE_GRAPH_BLOCK);
     RET(pg_reserve(g, grid));
     PgcOptimizeParams O{};
     std::vector<double> pq;
@@ -336,7 +472,7 @@ static int pg_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_po
     cudaStream_t s = ex.stream;
     if (direct) {
         RET(pg_sym_upload(g));
-        const size_t V = std::max({N, E, size_t(1)});
+        const size_t V = std::max({N, NF, size_t(1)});
         RET(g->Lx.ensure(std::max<size_t>(36 * S.blocks(), 1)));
         RET(g->cov_flag.ensure(1));
         RET(g->dir_val.ensure(2 * V));
@@ -382,7 +518,7 @@ static int pg_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_po
     if (edge_chi2 && E) CK(cudaMemcpyAsync(chi2.data(), g->e_s.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
     if (edge_weight && E) CK(cudaMemcpyAsync(weight.data(), g->e_w.p, E * sizeof(double), cudaMemcpyDeviceToHost, s));
     RET(ex.sync());
-    g->uploaded = E;
+    pg_uploaded(g);
     for (size_t k = 0; k < N; ++k) {
         if (g->fixed[k]) continue;
         const double *v = &pq[8 * k];
@@ -425,9 +561,9 @@ int kb_debug_se3_right_jacobian_inverse(const double x[6], double J[36]) {
 }
 
 // ------------------------------------------------------------------------------- Pose graph: marginal covariances
-// The symbolic analysis (pgc_symbolic, host) is cached for (N, E): nodes and edges are only ever added. The numeric
-// factor is cached until the next add_node, add_edge or optimize, so marginals and joint marginals taken one after the
-// other factor once.
+// The symbolic analysis (pgc_symbolic, host) is cached for (N, E): nodes and edges are only ever added, and a prior adds
+// no off-diagonal block. The numeric factor is cached until the next add_node, add_edge, add_*_prior or optimize, so
+// marginals and joint marginals taken one after the other factor once.
 static int pg_symbolic(kb_pose_graph *g) {
     const int N = static_cast<int>(g->n()), E = static_cast<int>(g->m());
     if (g->sym.n_nodes == N && g->sym.n_edges == E) return KB_OK;
@@ -440,7 +576,7 @@ static int pg_symbolic(kb_pose_graph *g) {
     return KB_OK;
 }
 
-// the requested nodes exist, and every free node is tied to a fixed one (otherwise H is singular)
+// the requested nodes exist, and every free node is tied to a fixed node or a prior (otherwise H is singular)
 static int pg_cov_check(const kb_pose_graph *g, const size_t *nodes, size_t n_idx) {
     if (!nodes) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (n_idx > (size_t(1) << 30)) return fail(KB_ERR_INVALID_ARG, "more than 2^29 requests in one call");
@@ -493,7 +629,7 @@ static int pg_factor(kb_pose_graph *g) {
     }
     int co_resident = 0;
     CK(pgc_factor_max_grid(ex.sms, &co_resident));
-    const int grid = pg_grid(ex, co_resident, std::max({g->n(), g->m(), S.blocks()}), PGC_BLOCK);
+    const int grid = pg_grid(ex, co_resident, std::max({g->n(), g->m() + g->np(), S.blocks()}), PGC_BLOCK);
     RET(pg_reserve(g, grid));
     std::vector<double> pq;
     PgcFactorParams F{};
@@ -526,7 +662,7 @@ static int pg_factor(kb_pose_graph *g) {
     int flag = 0;
     CK(cudaMemcpyAsync(&flag, g->cov_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
     RET(ex.sync());
-    g->uploaded = g->m();
+    pg_uploaded(g);
     if (flag) return fail(KB_ERR_INVALID_ARG, "H is not positive definite at the current poses");
     g->factored = true;
     return KB_OK;

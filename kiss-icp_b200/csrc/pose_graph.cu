@@ -7,7 +7,7 @@
 // kernels of the other units.
 //
 // Determinism: every sum is formed in a fixed order. A node's blocks add their edges' contributions in ascending edge
-// order; every dot product and the cost are summed per thread over its grid-stride items, then by a fixed tree in the
+// order, then its priors in ascending prior order; every dot product and the cost are summed per thread over its grid-stride items, then by a fixed tree in the
 // CTA, then over the CTAs in index order. No floating-point atomics: a result depends on the grid size only.
 #define kb kb_pg
 #include "device_ops.cuh"
@@ -323,12 +323,13 @@ __device__ void bcr_solve(Grid &g, const PoseGraphParams &P, long long gt, long 
     }
 }
 
-// 1/2 sum_e rho(s_e) at `poses`; with `linearize` also every edge's linearization
-__device__ double edges_pass(Grid &g, Red &rd, PgShared &sh, const PoseGraphParams &P, const double *poses, bool linearize,
-                             long long gt, long long gs) {
+// 1/2 sum_f rho(s_f) over the factors (the edges, then the priors) at `poses`; with `linearize` also every factor's
+// linearization
+__device__ double factors_pass(Grid &g, Red &rd, PgShared &sh, const PoseGraphParams &P, const double *poses, bool linearize,
+                               long long gt, long long gs) {
     double c[1] = {0.0}, out[1];
-    for (long long e = gt; e < P.n_edges; e += gs)
-        c[0] = c[0] + (linearize ? edge_linearize(P, poses, static_cast<int>(e)) : edge_eval(P, poses, static_cast<int>(e)).rho);
+    for (long long f = gt; f < P.n_edges + P.n_priors; f += gs)
+        c[0] = c[0] + (linearize ? factor_linearize(P, poses, static_cast<int>(f)) : factor_rho(P, poses, static_cast<int>(f)));
     grid_reduce<1>(g, rd, c, out, sh.red, sh.out);
     return 0.5 * out[0];
 }
@@ -342,8 +343,8 @@ struct PcgSolve {
     long long gt, gs;
     int cg_iterations;
 
-    __device__ double linearize(const double *poses) { return edges_pass(g, rd, sh, P, poses, true, gt, gs); }
-    __device__ void relinearize(const double *poses) { edges_pass(g, rd, sh, P, poses, true, gt, gs); }
+    __device__ double linearize(const double *poses) { return factors_pass(g, rd, sh, P, poses, true, gt, gs); }
+    __device__ void relinearize(const double *poses) { factors_pass(g, rd, sh, P, poses, true, gt, gs); }
 
     __device__ bool step(double lambda, int iteration, const double *cur, double *cand, double &max_d, double &Fc) {
         const long long N = P.n_nodes;
@@ -412,7 +413,7 @@ struct PcgSolve {
         for (long long k = gt; k < N; k += gs) mx[0] = fmax(mx[0], candidate_pose(P, cur, cand, k, P.x + 6 * k));
         grid_reduce<1, true>(g, rd, mx, omx, sh.red, sh.out);
         max_d = omx[0];
-        Fc = edges_pass(g, rd, sh, P, cand, false, gt, gs);
+        Fc = factors_pass(g, rd, sh, P, cand, false, gt, gs);
         return true;
     }
 };

@@ -351,13 +351,13 @@ namespace kb_pgc {
 #include "pose_graph_edges.cuh"
 #include "pose_graph_factor.cuh"
 
-// Linearize every edge at the current poses, assemble H's blocks (lambda 0), gather them into L's, then factor them
+// Linearize every factor (the edges, then the priors) at the current poses, assemble H's blocks (lambda 0), gather them into L's, then factor them
 // level by level.
 __global__ void __launch_bounds__(PGC_BLOCK, 1) k_pgc_factor(const PgcFactorParams F) {
     Grid g;
     g.init(F.P.bar);
     const int gt = blockIdx.x * PGC_BLOCK + threadIdx.x, gs = gridDim.x * PGC_BLOCK;
-    for (int e = gt; e < F.P.n_edges; e += gs) edge_linearize(F.P, F.P.pose, e);
+    for (int f = gt; f < F.P.n_edges + F.P.n_priors; f += gs) factor_linearize(F.P, F.P.pose, f);
     g.sync();
     for (int k = gt; k < F.P.n_nodes; k += gs) assemble_node(F.P, k, 0.0);
     g.sync();

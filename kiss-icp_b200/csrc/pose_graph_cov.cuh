@@ -36,7 +36,7 @@ struct PgcSymbolic {
 void pgc_symbolic(int N, const int *fixed, int E, const int *ij, PgcSymbolic *out);
 
 struct PgcFactorParams {
-    PoseGraphParams P;  // the graph, the edge linearization and the node diagonal blocks (lambda 0)
+    PoseGraphParams P;  // the graph, the factors' linearization and the node diagonal blocks (lambda 0)
     int nf, levels, n_blocks;
     const int *order, *lev_ptr, *colptr, *brow, *bcol, *hptr, *hedge, *uptr, *upd;
     double *Lx;   // [blocks][36] H's blocks, then L's
@@ -60,7 +60,7 @@ struct PgcOptimizeParams {
     const int *rptr, *rblk;  // the row index (PgcSymbolic)
     const int *pos;          // [N] the position of each node (-1: fixed)
     double *y;               // [nf][6] by position: -g, then L^-1 P^T (-g), then the step
-    double *val;             // [2][V] per edge rho(s_e), per node max |step| (V = max(N, E, 1))
+    double *val;             // [2][V] per factor rho(s_f), per node max |step| (V = max(N, E + n_priors, 1))
     double *chunk;           // [2][ceil(V / PGC_CHUNK)] their sums and maxima over fixed chunks
     int stride;              // V
 };

@@ -9,8 +9,8 @@
 // the machine code ptxas generates for k_pgc_factor (DESIGN §4.6, §4.14).
 //
 // Determinism: the factor is formed as k_pgc_factor forms it; every column of the two substitutions is solved by one
-// thread in a fixed order; a node's gradient sums its edges in ascending order; the cost and max |d| are folded over
-// fixed chunks of edges and nodes, then over the chunks in index order (the max is exact in any order). No
+// thread in a fixed order; a node's gradient sums its edges in ascending order, then its priors; the cost and max |d|
+// are folded over fixed chunks of factors (the edges, then the priors) and nodes, then over the chunks in index order (the max is exact in any order). No
 // floating-point atomics: the results are bit-identical from run to run and for every grid size.
 #define kb kb_pgd
 #include "device_ops.cuh"
@@ -152,20 +152,20 @@ struct DirectSolve {
 
     __device__ double linearize(const double *poses) {
         const PoseGraphParams &P = O.F.P;
-        for (int e = gt; e < P.n_edges; e += gs) O.val[e] = edge_linearize(P, poses, e);
+        for (int f = gt; f < P.n_edges + P.n_priors; f += gs) O.val[f] = factor_linearize(P, poses, f);
         double red[2];
-        reduce_chunks(g, O, P.n_edges, 0, s_out, red);
+        reduce_chunks(g, O, P.n_edges + P.n_priors, 0, s_out, red);
         return 0.5 * red[0];
     }
     __device__ void relinearize(const double *poses) {
-        for (int e = gt; e < O.F.P.n_edges; e += gs) edge_linearize(O.F.P, poses, e);
+        for (int f = gt; f < O.F.P.n_edges + O.F.P.n_priors; f += gs) factor_linearize(O.F.P, poses, f);
         g.sync();
     }
 
     __device__ bool step(double lambda, int, const double *cur, double *cand, double &max_d, double &Fc) {
         const PgcFactorParams &F = O.F;
         const PoseGraphParams &P = F.P;
-        const int N = P.n_nodes, E = P.n_edges;
+        const int N = P.n_nodes, NF = P.n_edges + P.n_priors;
         if (gt == 0) *F.flag = 0;  // (every CTA read the last step's flag before a barrier that follows)
         for (int k = gt; k < N; k += gs) assemble_node(P, k, lambda);
         g.sync();
@@ -189,9 +189,9 @@ struct DirectSolve {
         for (int k = gt; k < N; k += gs)
             O.val[O.stride + k] = candidate_pose(P, cur, cand, k, O.y + 6 * static_cast<size_t>(max(O.pos[k], 0)));
         g.sync();
-        for (int e = gt; e < E; e += gs) O.val[e] = edge_eval(P, cand, e).rho;
+        for (int f = gt; f < NF; f += gs) O.val[f] = factor_rho(P, cand, f);
         double red[2];
-        reduce_chunks(g, O, E, N, s_out, red);
+        reduce_chunks(g, O, NF, N, s_out, red);
         Fc = 0.5 * red[0];
         max_d = red[1];
         return true;

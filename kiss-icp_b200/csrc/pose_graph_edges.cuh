@@ -1,8 +1,10 @@
 // Device code of the pose graph that both optimizers (pose_graph.cu, pose_graph_direct.cu) and the covariance
-// (pose_graph_cov.cu) run: the pose layout, the 6x6 helpers, one edge's linearization, the gather of a node's
-// diagonal block, and the Levenberg-Marquardt loop with its candidate step. Each unit includes this inside its own
-// namespace, after device_ops.cuh, so each module has its own copies (DESIGN §4.6: a kernel of one unit changes no
-// code generated for another's).
+// (pose_graph_cov.cu) run: the pose layout, the 6x6 helpers, one factor's linearization (an edge or a prior), the
+// gather of a node's diagonal block, and the Levenberg-Marquardt loop with its candidate step. Each unit includes this
+// inside its own namespace, after device_ops.cuh, so each module has its own copies (DESIGN §4.6: a kernel of one unit
+// changes no code generated for another's).
+
+#include "pose_graph_priors.cuh"
 
 __device__ __forceinline__ SE3 ld_pose(const double *p) { return SE3{{p[0], p[1], p[2], p[3]}, {p[4], p[5], p[6]}}; }
 
@@ -55,16 +57,32 @@ __device__ __forceinline__ EdgeEval edge_eval(const PoseGraphParams &P, const do
 #pragma unroll
     for (int a = 0; a < 6; ++a) s = s + v.r[a] * Or[a];
     v.s = s;
-    const double c = P.robust[e];
-    if (c > 0.0) {
-        const double c2 = c * c;
-        v.rho = c2 * log1p(s / c2);
-        v.w = 1.0 / (1.0 + s / c2);
-    } else {
-        v.rho = s;
-        v.w = 1.0;
-    }
+    robust_loss(s, P.robust[e], &v.rho, &v.w);
     return v;
+}
+
+// H = J^T W J (formed on the upper triangle and mirrored: exactly symmetric) and g = J^T W r, W = w Omega
+__device__ __forceinline__ void weighted_normal(const double *J, const double *Om, const double r[6], double w, double *H,
+                                                double *g) {
+    double Or[6], gj[6];
+    mv6(Om, r, Or);
+    mtv6(J, Or, gj);
+#pragma unroll
+    for (int a = 0; a < 6; ++a) g[a] = w * gj[a];
+#pragma unroll
+    for (int b = 0; b < 6; ++b) {
+        double col[6], x[6];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) col[k] = J[6 * k + b];
+        mv6(Om, col, x);  // Omega J[:, b]
+#pragma unroll
+        for (int a = 0; a <= b; ++a) {
+            double s = 0.0;
+#pragma unroll
+            for (int m = 0; m < 6; ++m) s = s + J[6 * m + a] * x[m];
+            H[6 * a + b] = H[6 * b + a] = w * s;
+        }
+    }
 }
 
 // the edge's part of the linearization: B = J_r^-1(r), A = -B Ad(T_j^-1 T_i), W = w Omega.
@@ -82,25 +100,7 @@ __device__ __noinline__ double edge_linearize(const PoseGraphParams &P, const do
     {
         double J[36];
         se3_right_jacobian_inverse(v.r, J);
-        double Or[6], gj[6];
-        mv6(Om, v.r, Or);
-        mtv6(J, Or, gj);
-#pragma unroll
-        for (int a = 0; a < 6; ++a) P.e_g[6 * static_cast<size_t>(e) + a] = v.w * gj[a];
-#pragma unroll
-        for (int b = 0; b < 6; ++b) {
-            double col[6], x[6];
-#pragma unroll
-            for (int k = 0; k < 6; ++k) col[k] = J[6 * k + b];
-            mv6(Om, col, x);  // Omega J[:, b]
-#pragma unroll
-            for (int a = 0; a <= b; ++a) {
-                double s = 0.0;
-#pragma unroll
-                for (int m = 0; m < 6; ++m) s = s + J[6 * m + a] * x[m];
-                Ejj[6 * a + b] = Ejj[6 * b + a] = v.w * s;
-            }
-        }
+        weighted_normal(J, Om, v.r, v.w, Ejj, P.e_g + 6 * static_cast<size_t>(e));
     }
     double A[36];
     se3_adjoint(se3_mul(se3_inverse(v.Tj), v.Ti), A);
@@ -121,6 +121,41 @@ __device__ __noinline__ double edge_linearize(const PoseGraphParams &P, const do
         }
     }
     return v.rho;
+}
+
+// prior p at `poses`: r_p and s_p (prior_residual), rho(s_p) and w_p = rho'(s_p)
+struct PriorEval {
+    SE3 T;
+    double r[6], s, rho, w;
+};
+__device__ __forceinline__ PriorEval prior_eval(const PoseGraphParams &P, const double *poses, int p) {
+    PriorEval v;
+    v.T = ld_pose(poses + 8 * static_cast<size_t>(P.p_node_kind[2 * p]));
+    v.s = prior_residual(P.p_node_kind[2 * p + 1], P.p_meas + 8 * static_cast<size_t>(p), P.p_info + 36 * static_cast<size_t>(p),
+                         v.T, v.r);
+    robust_loss(v.s, P.p_robust[p], &v.rho, &v.w);
+    return v;
+}
+
+// the prior's linearization: Jt W J and Jt W r (J = prior_jacobian, W = w Omega). Returns rho(s_p).
+__device__ __noinline__ double prior_linearize(const PoseGraphParams &P, const double *poses, int p) {
+    const PriorEval v = prior_eval(P, poses, p);
+    P.p_s[p] = v.s;
+    P.p_w[p] = v.w;
+    double J[36];
+    prior_jacobian(P.p_node_kind[2 * p + 1], P.p_meas + 8 * static_cast<size_t>(p), v.T, v.r, J);
+    weighted_normal(J, P.p_info + 36 * static_cast<size_t>(p), v.r, v.w, P.p_h + 36 * static_cast<size_t>(p),
+                    P.p_g + 6 * static_cast<size_t>(p));
+    return v.rho;
+}
+
+// factor f of the loops over E + n_priors: edge f, or prior f - E. Its rho at `poses`, and the same with its
+// linearization.
+__device__ __forceinline__ double factor_rho(const PoseGraphParams &P, const double *poses, int f) {
+    return f < P.n_edges ? edge_eval(P, poses, f).rho : prior_eval(P, poses, f - P.n_edges).rho;
+}
+__device__ __forceinline__ double factor_linearize(const PoseGraphParams &P, const double *poses, int f) {
+    return f < P.n_edges ? edge_linearize(P, poses, f) : prior_linearize(P, poses, f - P.n_edges);
 }
 
 // diagonal block, gradient, damped M diagonal block and chain coupling of node k
@@ -160,6 +195,14 @@ __device__ __noinline__ void assemble_node(const PoseGraphParams &P, int k, doub
 #pragma unroll
             for (int a = 0; a < 6; ++a) g[a] = g[a] + gg[a];
         }
+    }
+    for (int t = P.pinc_ptr[k]; t < P.pinc_ptr[k + 1]; ++t) {  // the node's priors, after its edges
+        const int p = P.pinc[t];
+        const double *Hp = P.p_h + 36 * static_cast<size_t>(p), *gp = P.p_g + 6 * static_cast<size_t>(p);
+#pragma unroll 6
+        for (int a = 0; a < 36; ++a) Hk[a] = Hk[a] + Hp[a];
+#pragma unroll
+        for (int a = 0; a < 6; ++a) g[a] = g[a] + gp[a];
     }
 #pragma unroll
     for (int a = 0; a < 6; ++a) gk[a] = g[a];
@@ -215,7 +258,7 @@ __device__ __forceinline__ double candidate_pose(const PoseGraphParams &P, const
 // Levenberg-Marquardt on the graph of P, both optimizers' loop: the lambda schedule, acceptance, the stopping rules in
 // their order, the poses back in P.pose and the report. The solver S runs every grid-wide part, with its own sums and
 // barriers:
-//   double S.linearize(poses): every edge's linearization at `poses`; returns the cost there
+//   double S.linearize(poses): every factor's linearization at `poses` (factor_linearize); returns the cost there
 //   void S.relinearize(poses): the same after an accepted step, the cost unused
 //   bool S.step(lambda, iteration, cur, cand, max_d, Fc): assemble (H + lambda diag H) at the linearization, solve it
 //     for d, write the candidate T_k Exp(d_k) of every node into cand (candidate_pose), max_d = max |d|, Fc = the cost

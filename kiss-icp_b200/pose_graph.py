@@ -6,6 +6,8 @@ with the information Omega (6x6, tangent order translation then rotation) and an
 runs Levenberg-Marquardt on the device, in one launch, and leaves the result in ``poses``; each step is solved by PCG
 or, with PoseGraphOptions(linear_solver="cholesky"), exactly by a sparse block Cholesky factorization. Nodes and edges
 may be added afterwards and optimize() called again (the online use of loop closure: loop_closure.LoopCloser).
+Priors anchor nodes to absolute measurements: add_pose_prior() (a surveyed or relocalized pose) and
+add_position_prior() (a GNSS antenna position through a lever arm); a graph with priors needs no fixed node.
 marginal_covariances() and joint_marginal_covariances() say how well the poses are known: blocks of H^-1 at the
 current poses, from a sparse block Cholesky factorization on the device.
 """
@@ -155,6 +157,51 @@ class PoseGraph:
                                                    float(robust_scale), C.byref(idx)))
         return idx.value
 
+    def add_pose_prior(self, k: int, pose, information, robust_scale: float = 0.0) -> int:
+        """the prior T_k = pose (4x4, world frame): residual Log(pose^-1 T_k), ``information`` 6x6 (symmetric positive
+        definite, tangent order translation then rotation), Cauchy scale (0: squared loss). Returns its index among
+        the priors of both kinds."""
+        Z = N.mat4_arg(pose)
+        Om = np.ascontiguousarray(information, dtype=np.float64)
+        if Om.shape != (6, 6):
+            raise ValueError(f"information must be 6x6, not {Om.shape}")
+        idx = N.sz(0)
+        check_value(N.lib().kb_pose_graph_add_pose_prior(self._h, _index(k, "k"), N.ptr(Z), N.ptr(Om),
+                                                         float(robust_scale), C.byref(idx)))
+        return idx.value
+
+    def add_position_prior(self, k: int, position, information, lever_arm=(0.0, 0.0, 0.0),
+                           robust_scale: float = 0.0) -> int:
+        """the prior R_k lever_arm + t_k = position: a point ``lever_arm`` (3,) of node k's body frame, e.g. a GNSS
+        antenna, measured at ``position`` (3,) in the world frame, with ``information`` 3x3 in the world frame and a
+        Cauchy scale (0: squared loss). Returns its index among the priors of both kinds."""
+        p = np.ascontiguousarray(position, dtype=np.float64)
+        arm = np.ascontiguousarray(lever_arm, dtype=np.float64)
+        Om = np.ascontiguousarray(information, dtype=np.float64)
+        if p.shape != (3,) or arm.shape != (3,):
+            raise ValueError(f"position and lever_arm must have the shape (3,), not {p.shape} and {arm.shape}")
+        if Om.shape != (3, 3):
+            raise ValueError(f"information must be 3x3, not {Om.shape}")
+        idx = N.sz(0)
+        check_value(N.lib().kb_pose_graph_add_position_prior(self._h, _index(k, "k"), N.ptr(p), N.ptr(arm), N.ptr(Om),
+                                                             float(robust_scale), C.byref(idx)))
+        return idx.value
+
+    @property
+    def n_priors(self) -> int:
+        n = N.sz(0)
+        N.check(N.lib().kb_pose_graph_num_priors(self._h, C.byref(n)))
+        return n.value
+
+    def prior_residuals(self) -> tuple[np.ndarray, np.ndarray]:
+        """(chi2, weight): every prior's s_p = r^T Omega r and Cauchy weight w_p at the current poses (host-side)"""
+        n = self.n_priors
+        chi2, weight = np.empty(n), np.empty(n)
+        got = N.sz(0)
+        if n:
+            N.check(N.lib().kb_pose_graph_prior_chi2(self._h, N.ptr(chi2), N.ptr(weight), n, C.byref(got)))
+        return chi2, weight
+
     def _size(self):
         n, m = N.sz(0), N.sz(0)
         N.check(N.lib().kb_pose_graph_size(self._h, C.byref(n), C.byref(m)))
@@ -179,7 +226,9 @@ class PoseGraph:
 
     def optimize(self, options: PoseGraphOptions | None = None, return_edges: bool = False) -> PoseGraphReport:
         """optimize the free nodes from their current poses, each step solved as options.linear_solver says.
-        ValueError for a rejected argument (among them a free node that no path of edges connects to a fixed node)."""
+        ValueError for a rejected argument, among them a free node that no path of edges connects to a fixed node or
+        to a node with a prior (the gauge: every connected component needs one; with priors, no node need be
+        fixed)."""
         options = PoseGraphOptions() if options is None else options
         solve = getattr(N.lib(), options._solver())
         o = options._struct()
@@ -197,7 +246,9 @@ class PoseGraph:
         """the (n, 6, 6) marginal covariances Sigma_kk of ``nodes`` (None: every node) at the current poses: blocks of
         H^-1, tangent order (translation, rotation) of the right perturbation T_k Exp(d_k); zero for a fixed node. The
         Gauss-Newton approximation, not rescaled by the residuals (kb_pose_graph_marginals states it in full).
-        ValueError for a node that does not exist or a free node no path of edges connects to a fixed node."""
+        ValueError for a node that does not exist, a free node no path of edges connects to a fixed node or to a node
+        with a prior, or an H that is not positive definite (e.g. a component held only by position priors at fewer
+        than 3 non-collinear antenna positions, which leave a rotation free)."""
         idx = np.arange(len(self), dtype=np.uint64) if nodes is None else _nodes_arg(nodes, (), "nodes")
         out = np.empty((len(idx), 6, 6))
         if len(idx):
