@@ -361,6 +361,48 @@ int kb_pipeline_register_frames_constraints(kb_pipeline *p, const void *const *x
                                             const double *const *timestamps, const size_t *n_timestamps, size_t count,
                                             int layout, double *poses_out, kb_fit *fits_out, kb_constraints *constraints_out);
 
+/* ---- degeneracy-aware ICP: hold the prediction along directions a scan does not constrain ----------------
+ * No reference counterpart. In a tunnel, a corridor or open ground with one wall, point-to-point ICP has no information
+ * along the free axis and drags the pose toward the previous scan's ring pattern. With a degeneracy ratio rho in
+ * (0, 1), every frame first runs the plane pass of kb_registration_constraints at its initial guess G = last_pose *
+ * last_delta with the frame's own 3 sigma, but with the lever about the guess's position c = G.t:
+ * J_c = [n^T, ((p - c) x n)^T], H_c = sum a J_c^T J_c (= A^T H A, A = [[I, [c]x], [0, I]]). Its translation block and
+ * its rotation block are eigen-decomposed separately (3x3 Jacobi, ascending); in each block an axis with
+ * l_k < rho * l_max is held, except that nothing is held in a block with l_max <= 0 or in a frame without a plane term.
+ * P = blockdiag(V_t M_t V_t^T, V_r M_r V_r^T), M = 0 on held axes and 1 elsewhere. Every ICP step dx (tangent order
+ * translation, rotation, about the map origin) becomes A P A^-1 dx before Exp and before the convergence test, so
+ * held directions keep the prediction (the constant-velocity model). A frame that holds nothing runs the plain ICP
+ * loop: its result is bit for bit that of rho = 0. No pipeline state is added: checkpoints are unchanged.
+ * Recommended: rho = 0.02 (both synthetic test streams, which are well conditioned, stay above it in both blocks;
+ * DESIGN.md section 4.16). The frames run a kernel of their own with one more pass and grid barrier before ICP. */
+typedef struct kb_degeneracy {
+    int n_planes;                       /* plane terms of the pass at the guess (0: nothing held)                 */
+    double weight_sum;                  /* sum of their planarity weights                                         */
+    double translation_eigenvalues[3];  /* of H_c[:3, :3], ascending                                              */
+    double translation_axes[9];         /* row-major, column k = unit axis of eigenvalue k (sign arbitrary)       */
+    double rotation_eigenvalues[3];     /* of H_c[3:, 3:], ascending                                              */
+    double rotation_axes[9];            /* likewise, rotation axes through c                                      */
+    int translation_held[3];            /* 1: axis k was held                                                     */
+    int rotation_held[3];
+} kb_degeneracy;
+/* Set the degeneracy ratio (0 when a pipeline is created: off). ratio > 0 needs a pipeline that reports fits (a
+ * localizer, or kb_pipeline_set_fit_reporting on), else KB_ERR_INVALID_ARG. NaN, negative and >= 1 values are
+ * KB_ERR_INVALID_ARG. On error nothing changes. A ratio > 0 allocates the per-frame results (zeroed; KB_ERR_CUDA if
+ * that fails, and the mode stays off), changing it keeps them, 0 releases them. While it is on,
+ * kb_pipeline_set_fit_reporting(p, 0) is KB_ERR_INVALID_ARG. */
+int kb_pipeline_set_degeneracy_ratio(kb_pipeline *p, double ratio);
+/* the pipeline's degeneracy ratio (0: off); KB_ERR_INVALID_ARG for NULL */
+int kb_pipeline_degeneracy_ratio(const kb_pipeline *p, double *out);
+/* the degeneracy result of the last frame (zeros before the first); KB_ERR_INVALID_ARG when the mode is off */
+int kb_pipeline_last_degeneracy(const kb_pipeline *p, kb_degeneracy *out);
+/* kb_pipeline_register_frames_constraints with one kb_degeneracy per frame in degeneracy_out[count] (may be NULL;
+ * non-NULL with the mode off is KB_ERR_INVALID_ARG), read behind the queue like the fits. A frame vetoed for table
+ * capacity gets its replay's. */
+int kb_pipeline_register_frames_degeneracy(kb_pipeline *p, const void *const *xyz, const size_t *n,
+                                           const double *const *timestamps, const size_t *n_timestamps, size_t count,
+                                           int layout, double *poses_out, kb_fit *fits_out, kb_constraints *constraints_out,
+                                           kb_degeneracy *degeneracy_out);
+
 /* ---- relocalization: a global pose search in a bounded region ----------------------------
  * No reference counterpart. Finds a scan's pose in a map without an initial pose: every hypothesis of a grid in x, y
  * and yaw around a centre is scored on the device, the best peaks are refined with kb_registration_align_batch, and

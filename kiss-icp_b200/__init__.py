@@ -3,7 +3,7 @@ path behind the reference's own Python surface (python/kiss_icp/*.py). The compu
 hand-written CUDA kernels reached through the C-ABI of include/kiss_icp_b200.h; this package
 is the host-side mirror of the reference interface. No CPU fallback."""
 from .config import KISSConfig, load_config  # noqa: F401
-from .constraints import Constraints, covariance, degeneracy  # noqa: F401
+from .constraints import RECOMMENDED_DEGENERACY_RATIO, Constraints, ScanDegeneracy, covariance, degeneracy  # noqa: F401
 from .free_space import FreeSpace, FreeSpaceParams  # noqa: F401
 from .kiss_icp import KissICP  # noqa: F401
 from .mapping import VoxelHashMap, get_voxel_hash_map  # noqa: F401

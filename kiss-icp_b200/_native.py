@@ -97,6 +97,13 @@ class Constraints(C.Structure):
     _fields_ = [("n_planes", i32), ("weight_sum", dbl), ("sum_sq_plane_residual", dbl), ("information", dbl * 36)]
 
 
+class Degeneracy(C.Structure):
+    """kb_degeneracy: the degeneracy-aware ICP's eigen-decomposition of one frame"""
+    _fields_ = [("n_planes", i32), ("weight_sum", dbl), ("translation_eigenvalues", dbl * 3),
+                ("translation_axes", dbl * 9), ("rotation_eigenvalues", dbl * 3), ("rotation_axes", dbl * 9),
+                ("translation_held", i32 * 3), ("rotation_held", i32 * 3)]
+
+
 class RelocSearch(C.Structure):
     """kb_reloc_search: the hypothesis grid of kb_relocalize"""
     _fields_ = [("center", dbl * 16), ("half_cells_x", i32), ("half_cells_y", i32), ("step", dbl), ("n_yaw", i32),
@@ -262,6 +269,10 @@ SIGNATURES = {
     "kb_pipeline_last_constraints": (i32, [vp, C.POINTER(Constraints)]),
     "kb_pipeline_register_frames_constraints": (i32, [vp, vp, vp, vp, vp, sz, i32, vp, vp, vp]),
     "kb_debug_sym3_eig": (i32, [vp, vp, vp]),
+    "kb_pipeline_set_degeneracy_ratio": (i32, [vp, dbl]),
+    "kb_pipeline_degeneracy_ratio": (i32, [vp, C.POINTER(dbl)]),
+    "kb_pipeline_last_degeneracy": (i32, [vp, C.POINTER(Degeneracy)]),
+    "kb_pipeline_register_frames_degeneracy": (i32, [vp, vp, vp, vp, vp, sz, i32, vp, vp, vp, vp]),
     "kb_place_params_default": (None, [C.POINTER(PlaceParams)]),
     "kb_place_db_create": (i32, [C.POINTER(PlaceParams), C.POINTER(vp)]),
     "kb_place_db_destroy": (i32, [vp]),

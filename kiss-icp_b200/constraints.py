@@ -19,6 +19,35 @@ Constraints = namedtuple("Constraints", ["n_planes", "weight_sum", "plane_rmse",
 Degeneracy = namedtuple("Degeneracy", ["translation_eigenvalues", "translation_axes", "rotation_eigenvalues",
                                        "rotation_axes"])
 
+# the degeneracy-aware ICP's result for one scan (kb_degeneracy, KissICP(config, degeneracy_ratio=...)): the eigenvalues
+# (ascending) and axes (columns) of both blocks of the plane information at the scan's initial guess, centred at the
+# guess's position, which axes were held, and the pass's n_planes and weight_sum
+ScanDegeneracy = namedtuple("ScanDegeneracy", ["translation_eigenvalues", "translation_axes", "rotation_eigenvalues",
+                                               "rotation_axes", "translation_held", "rotation_held", "n_planes",
+                                               "weight_sum"])
+
+# the ratio the header recommends (DESIGN.md section 4.16): below both blocks' smallest measured eigenvalue ratio of the
+# well-conditioned synthetic streams, far above a corridor's ~1e-9
+RECOMMENDED_DEGENERACY_RATIO = 0.02
+
+
+def _scan_degeneracy(ds) -> ScanDegeneracy:
+    """a ScanDegeneracy from one kb_degeneracy, or one of arrays (leading axis: the frame) from a sequence of them"""
+    one = not isinstance(ds, (list, tuple)) and not hasattr(ds, "__len__")
+    seq = [ds] if one else list(ds)
+    out = ScanDegeneracy(
+        np.array([d.translation_eigenvalues[:] for d in seq], dtype=np.float64).reshape(-1, 3),
+        np.array([d.translation_axes[:] for d in seq], dtype=np.float64).reshape(-1, 3, 3),
+        np.array([d.rotation_eigenvalues[:] for d in seq], dtype=np.float64).reshape(-1, 3),
+        np.array([d.rotation_axes[:] for d in seq], dtype=np.float64).reshape(-1, 3, 3),
+        np.array([d.translation_held[:] for d in seq], dtype=bool).reshape(-1, 3),
+        np.array([d.rotation_held[:] for d in seq], dtype=bool).reshape(-1, 3),
+        np.array([d.n_planes for d in seq], dtype=np.int64),
+        np.array([d.weight_sum for d in seq], dtype=np.float64))
+    if one:
+        return ScanDegeneracy(*(x[0] if i < 6 else x[0].item() for i, x in enumerate(out)))
+    return out
+
 
 def _constraints_of(n_planes, weight_sum, sse, info):
     """a Constraints from the raw values; array arguments give a Constraints of arrays"""

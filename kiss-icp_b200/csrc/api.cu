@@ -399,6 +399,10 @@ struct kb_pipeline {
     // plane constraints (kb_pipeline_set_constraint_reporting)
     Report<FitResult> fit;
     Report<PlaneResult> planes;
+    // degeneracy-aware ICP (kb_pipeline_set_degeneracy_ratio): on while degen_ratio > 0; its report is the projector's
+    // eigen-decomposition per frame
+    Report<DegenResult> degen;
+    double degen_ratio = 0.0;
     Work ws;
     DBuf<PipeState> d_state;
     FrameResult last{};
@@ -1591,7 +1595,11 @@ static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, si
     static_cast<FrameParams &>(R) = P;
     R.fit = FitOut{p->fit.part.p, p->fit.dev.p + slot};
     if (p->planes.on()) R.planes = PlaneOut{p->planes.part.p, p->planes.dev.p + slot};
-    return ex.coop_raw(report_kernel(p->localizer, p->planes.on()), &R, smem, true);
+    if (!p->degen.on()) return ex.coop_raw(report_kernel(p->localizer, p->planes.on()), &R, smem, true);
+    DegenParams D{};
+    static_cast<ReportParams &>(D) = R;
+    D.degen = DegenOut{p->degen.part.p, p->degen.dev.p + slot, p->degen_ratio};
+    return ex.coop_raw(degeneracy_kernel(p->localizer, p->planes.on()), &D, smem, true);
 }
 
 // take over the result of a frame that ran (not vetoed): host mirror of the counters, history
@@ -1637,6 +1645,22 @@ static void fit_to_abi(const FitResult &f, kb_fit *out) {
     out->sum_sq_residual = f.sse;
 }
 
+static void degen_to_abi(const DegenResult &r, kb_degeneracy *out) {
+    *out = kb_degeneracy{};
+    out->n_planes = r.n_planes;
+    out->weight_sum = r.weight_sum;
+    for (int k = 0; k < 3; ++k) {
+        out->translation_eigenvalues[k] = r.lam_t[k];
+        out->rotation_eigenvalues[k] = r.lam_r[k];
+        out->translation_held[k] = r.held_t[k];
+        out->rotation_held[k] = r.held_r[k];
+    }
+    for (int k = 0; k < 9; ++k) {
+        out->translation_axes[k] = r.ax_t[k];
+        out->rotation_axes[k] = r.ax_r[k];
+    }
+}
+
 enum Taken { TAKEN_ABSORBED, TAKEN_VETOED, TAKEN_SKIPPED };
 
 // take over the result `r` of frame `id` (n points in) once its launch has ended:
@@ -1645,9 +1669,9 @@ enum Taken { TAKEN_ABSORBED, TAKEN_VETOED, TAKEN_SKIPPED };
 //   the frame can be replayed.
 // - skipped: the frame did not run.
 // - absorbed: pipeline_absorb; the pose goes to pose_out, and each report the pipeline computes (pinned copy `slot`)
-//   becomes the last one and goes to fit_out / constraints_out (any of them may be null).
+//   becomes the last one and goes to fit_out / constraints_out / degen_out (any of them may be null).
 static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long id, size_t slot, double *pose_out,
-                       kb_fit *fit_out, kb_constraints *constraints_out, Taken *taken) {
+                       kb_fit *fit_out, kb_constraints *constraints_out, kb_degeneracy *degen_out, Taken *taken) {
     RET(watchdog_check(p->ex->device));  // (a spin loop that gave up invalidates the launch)
     if (r.map_status & ST_NEED_GROW) {
         *taken = TAKEN_VETOED;
@@ -1668,6 +1692,7 @@ static int take_result(kb_pipeline *p, const FrameResult &r, size_t n, long long
     if (pose_out) std::memcpy(pose_out, r.pose, sizeof(double) * 16);
     p->fit.take(slot, fit_out, fit_to_abi);
     p->planes.take(slot, constraints_out, planes_to_abi);
+    p->degen.take(slot, degen_out, degen_to_abi);
     return KB_OK;
 }
 
@@ -1732,12 +1757,13 @@ static const char *const kNoFits =
 static const char *const kNoConstraints =
     "plane constraints are reported by pipelines with kb_pipeline_set_constraint_reporting on";
 
-// kb_pipeline_register_frames[_fit|_constraints] and, with count = 1, kb_pipeline_register_frame[_f32|_dev]; fits_out
-// (pipelines that report fits only, may be NULL) receives one fit per frame, constraints_out (pipelines that report
-// plane constraints only, may be NULL) one kb_constraints per frame
+// kb_pipeline_register_frames[_fit|_constraints|_degeneracy] and, with count = 1, kb_pipeline_register_frame[_f32|_dev];
+// fits_out (pipelines that report fits only, may be NULL) receives one fit per frame, constraints_out (pipelines that
+// report plane constraints only, may be NULL) one kb_constraints per frame, degen_out (pipelines with a degeneracy
+// ratio only, may be NULL) one kb_degeneracy per frame
 static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
                            const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out,
-                           kb_constraints *constraints_out) {
+                           kb_constraints *constraints_out, kb_degeneracy *degen_out = nullptr) {
     if (!p || (count && (!xyz || !n))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (layout != KB_FRAMES_HOST_F64 && layout != KB_FRAMES_HOST_F32 && layout != KB_FRAMES_DEVICE_F64)
         return fail(KB_ERR_INVALID_ARG, "unknown frame layout %d", layout);
@@ -1785,7 +1811,7 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
     auto take = [&](size_t k, Taken *taken) {  // the result of frame k, once its launch and read-back have ended
         return take_result(p, p->q_res.p[k % D], n[k], id0 + static_cast<long long>(k), k % D,
                            poses_out ? poses_out + 16 * k : nullptr, fits_out ? fits_out + k : nullptr,
-                           constraints_out ? constraints_out + k : nullptr, taken);
+                           constraints_out ? constraints_out + k : nullptr, degen_out ? degen_out + k : nullptr, taken);
     };
     auto run = [&]() -> int {
     while (next_absorb < valid) {
@@ -1822,6 +1848,7 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
                                    p->res_stream.p));
                 CK(p->fit.read_back(k % D, p->res_stream.p));
                 CK(p->planes.read_back(k % D, p->res_stream.p));
+                CK(p->degen.read_back(k % D, p->res_stream.p));
                 CK(cudaEventRecord(s.read.p, p->res_stream.p));
             }
             ++next_submit;
@@ -1909,6 +1936,8 @@ int kb_pipeline_set_fit_reporting(kb_pipeline *p, int enabled) {
     if (p->localizer) return enabled ? KB_OK : fail(KB_ERR_INVALID_ARG, "a localizer always reports fits");
     if (!enabled && p->planes.on())
         return fail(KB_ERR_INVALID_ARG, "plane constraint reporting needs the fits: turn it off first");
+    if (!enabled && p->degen.on())
+        return fail(KB_ERR_INVALID_ARG, "degeneracy-aware ICP needs the fits: set the degeneracy ratio to 0 first");
     return p->fit.set(enabled, FIT_VALS, *p->ex);
 }
 int kb_pipeline_set_constraint_reporting(kb_pipeline *p, int enabled) {
@@ -1923,6 +1952,39 @@ int kb_pipeline_last_constraints(const kb_pipeline *p, kb_constraints *out) {
     if (!p->planes.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoConstraints);
     planes_to_abi(p->planes.last, out);
     return KB_OK;
+}
+static const char *const kNoDegeneracy = "degeneracy results are reported by pipelines with a degeneracy ratio > 0";
+
+int kb_pipeline_set_degeneracy_ratio(kb_pipeline *p, double ratio) {
+    if (!p) return fail(KB_ERR_INVALID_ARG, "p == NULL");
+    if (!(ratio >= 0.0 && ratio < 1.0)) return fail(KB_ERR_INVALID_ARG, "degeneracy ratio %g is not in [0, 1)", ratio);
+    if (ratio > 0.0 && !p->fit.on())
+        return fail(KB_ERR_INVALID_ARG, "degeneracy-aware ICP runs next to the fit: a localizer, or an odometry pipeline "
+                                        "with kb_pipeline_set_fit_reporting on");
+    const int st = p->degen.set(ratio > 0.0, PLANE_VALS, *p->ex);
+    p->degen_ratio = p->degen.on() ? ratio : 0.0;  // (off when the buffers could not be allocated)
+    return st;
+}
+int kb_pipeline_degeneracy_ratio(const kb_pipeline *p, double *out) {
+    if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *out = p->degen_ratio;
+    return KB_OK;
+}
+int kb_pipeline_last_degeneracy(const kb_pipeline *p, kb_degeneracy *out) {
+    if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (!p->degen.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoDegeneracy);
+    degen_to_abi(p->degen.last, out);
+    return KB_OK;
+}
+int kb_pipeline_register_frames_degeneracy(kb_pipeline *p, const void *const *xyz, const size_t *n,
+                                           const double *const *timestamps, const size_t *n_timestamps, size_t count,
+                                           int layout, double *poses_out, kb_fit *fits_out, kb_constraints *constraints_out,
+                                           kb_degeneracy *degeneracy_out) {
+    if (p && fits_out && !p->fit.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
+    if (p && constraints_out && !p->planes.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoConstraints);
+    if (p && degeneracy_out && !p->degen.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoDegeneracy);
+    return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out, constraints_out,
+                           degeneracy_out);
 }
 int kb_pipeline_fit_reporting(const kb_pipeline *p, int *out) {
     if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");

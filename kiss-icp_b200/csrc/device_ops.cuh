@@ -1317,9 +1317,41 @@ __device__ __forceinline__ void icp_gather(const Scratch &sc, Shared &sh, unsign
 //   in its shared memory) and publishes {estimation, converged} as tagged chunks; all CTAs poll
 //   that record. No flags, no fences, no host round trip: two L2 hops per iteration.
 // ------------------------------------------------------------------------------------------
-__device__ __noinline__ void op_icp(Grid &g, const Scratch &sc, Shared &sh, const MapView &m, const double *src, double *work,
-                       int n, const SE3 &guess, double max_dist, double kscale, int max_iter, double conv,
-                       QCache *qcache, unsigned tag_base, bool fill_first = true) {
+// The degeneracy projector of one scan (DESIGN.md section 4.16), in the shared memory of the kernel that formed it:
+// pt, pr = upper triangles (xx, xy, xz, yy, yz, zz) of V M V^T for the translation and the rotation block of the plane
+// information in tangent coordinates centred at c, M = 0 on a held axis and 1 elsewhere; held = number of held axes.
+struct DegenProj {
+    double pt[6], pr[6];
+    V3 c;
+    int held;
+};
+__device__ __forceinline__ V3 sym3_apply(const double s[6], const V3 &x) {
+    return V3{(s[0] * x.x + s[1] * x.y) + s[2] * x.z, (s[1] * x.x + s[3] * x.y) + s[4] * x.z,
+              (s[2] * x.x + s[4] * x.y) + s[5] * x.z};
+}
+// dx <- A P A^-1 dx with A = [[I, [c]x], [0, I]]: the step in centred coordinates (v - c x w, w), projected blockwise,
+// mapped back (v' + c x w', w')
+__device__ __forceinline__ void degen_project(const DegenProj &P, double dx[6]) {
+    const V3 w{dx[3], dx[4], dx[5]};
+    const V3 cw = cross(P.c, w);
+    const V3 v = sym3_apply(P.pt, V3{dx[0] - cw.x, dx[1] - cw.y, dx[2] - cw.z});
+    const V3 wp = sym3_apply(P.pr, w);
+    const V3 cwp = cross(P.c, wp);
+    dx[0] = v.x + cwp.x;
+    dx[1] = v.y + cwp.y;
+    dx[2] = v.z + cwp.z;
+    dx[3] = wp.x;
+    dx[4] = wp.y;
+    dx[5] = wp.z;
+}
+
+// kProj: every step is projected by *proj (degen_project) before Exp and the convergence test (k_register_frame of the
+// degeneracy module with a held axis); otherwise AlignPointsToMap as the reference states it
+template <bool kProj>
+__device__ __forceinline__ void icp_iterate(Grid &g, const Scratch &sc, Shared &sh, const MapView &m, const double *src,
+                                            double *work, int n, const SE3 &guess, double max_dist, double kscale,
+                                            int max_iter, double conv, QCache *qcache, unsigned tag_base, bool fill_first,
+                                            const DegenProj *proj) {
     (void)g;
     if (__ldcg(&m.counters[C_LIVE]) == 0 || max_iter <= 0) {  // voxel_map.Empty() -> initial_guess (:143)
         __syncthreads();
@@ -1363,6 +1395,7 @@ __device__ __noinline__ void op_icp(Grid &g, const Scratch &sc, Shared &sh, cons
                     for (int i = 0; i < 6; ++i) rhs[i] = -JTr[i];
                     ldlt6_solve_fast(JTJ, rhs, dx);
                 }
+                if constexpr (kProj) degen_project(*proj, dx);
                 if (dbg_on) { KB_CYC(sc, 7); }
                 const SE3 est = se3_exp_fast(dx);                 // :157
                 if (dbg_on) { KB_CYC(sc, 8); }
@@ -1439,6 +1472,17 @@ __device__ __noinline__ void op_icp(Grid &g, const Scratch &sc, Shared &sh, cons
         sh.query_total = static_cast<double>(n) * (j + 1);
     }
     __syncthreads();
+}
+__device__ __noinline__ void op_icp(Grid &g, const Scratch &sc, Shared &sh, const MapView &m, const double *src, double *work,
+                       int n, const SE3 &guess, double max_dist, double kscale, int max_iter, double conv,
+                       QCache *qcache, unsigned tag_base, bool fill_first = true) {
+    icp_iterate<false>(g, sc, sh, m, src, work, n, guess, max_dist, kscale, max_iter, conv, qcache, tag_base, fill_first,
+                       nullptr);
+}
+__device__ __noinline__ void op_icp_proj(Grid &g, const Scratch &sc, Shared &sh, const MapView &m, const double *src,
+                                         double *work, int n, const SE3 &guess, double max_dist, double kscale, int max_iter,
+                                         double conv, QCache *qcache, unsigned tag_base, const DegenProj *proj) {
+    icp_iterate<true>(g, sc, sh, m, src, work, n, guess, max_dist, kscale, max_iter, conv, qcache, tag_base, true, proj);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -1,6 +1,7 @@
 // KissICP::RegisterFrame as one persistent kernel (k_register_frame) and what it works on. A header of its own:
 // the odometry instantiation is compiled with the other kernels (api.cu), the four that report fits and plane
-// constraints in a translation unit of their own (report.cu), so that they change no code generated for the first.
+// constraints in a translation unit of their own (report.cu), and the four of degeneracy-aware ICP in another
+// (degeneracy.cu), so that they change no code generated for the first.
 #pragma once
 
 #include <type_traits>
@@ -176,6 +177,110 @@ struct ReportParams : FrameParams {
     FitOut fit;
     PlaneOut planes;
 };
+// ---- degeneracy-aware ICP (kb_pipeline_set_degeneracy_ratio, DESIGN.md section 4.16) --------------------------------
+// Before ICP, at the initial guess G: the plane pass with the lever about c = G.t (op_fit_planes<false, true, true>),
+// H_c = sum a J_c^T J_c with J_c = [n, (p - c) x n]; each 3x3 block (translation, rotation) is eigen-decomposed with
+// sym3_eig, an axis with l_i < ratio * l_max is held (none in a block with l_max <= 0 or without a plane term), and
+// every ICP step is projected onto the kept axes (degen_project). Nothing held: the plain ICP loop runs.
+struct DegenResult {
+    double lam_t[3], lam_r[3];  // eigenvalues of each block, ascending
+    double ax_t[9], ax_r[9];    // row-major; column k is the axis of eigenvalue k
+    double weight_sum;
+    int n_planes;
+    int held_t[3], held_r[3];   // 1: axis k is held
+    int pad;
+};
+struct DegenOut {
+    double *part;      // [PLANE_VALS][grid] per-CTA partials of the pass
+    DegenResult *res;  // this frame's result
+    double ratio;      // in (0, 1)
+};
+// a pipeline with a degeneracy ratio (it reports fits too)
+struct DegenParams : ReportParams {
+    DegenOut degen;
+};
+
+// one block of the projector: eigen-decomposition, held axes, V M V^T (the kept axes' v v^T in ascending order)
+__device__ __forceinline__ int degen_block(const double c6[6], double ratio, bool evidence, double lam[3], V3 v[3],
+                                           int held[3], double proj[6]) {
+    sym3_eig(c6, lam, v);
+    double s[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    int n = 0;
+    for (int k = 0; k < 3; ++k) {
+        held[k] = (evidence && lam[2] > 0.0 && lam[k] < ratio * lam[2]) ? 1 : 0;
+        n += held[k];
+        if (held[k]) continue;
+        s[0] += v[k].x * v[k].x;
+        s[1] += v[k].x * v[k].y;
+        s[2] += v[k].x * v[k].z;
+        s[3] += v[k].y * v[k].y;
+        s[4] += v[k].y * v[k].z;
+        s[5] += v[k].z * v[k].z;
+    }
+    for (int i = 0; i < 6; ++i) proj[i] = s[i];
+    return n;
+}
+
+// after the barrier behind the pass, in every CTA: the partials added in CTA order (the same bits in every CTA; the
+// partials are staged in shared memory 64 CTAs at a time so that their loads are in flight together), the projector
+// formed into *pj (translation block by thread 0, rotation block by thread 32); the last CTA also writes the result.
+// Ends with a block barrier.
+__device__ __noinline__ void degen_form(Shared &sh, const DegenOut &D, const V3 &c, DegenProj *pj) {
+    constexpr int CH = 64;
+    static_assert(PLANE_VALS * CH * 8 <= DS_MAX_CHUNKS * 4, "the staged partials live in Shared::chunk_pref");
+    const int G = static_cast<int>(gridDim.x);
+    double *stage = reinterpret_cast<double *>(sh.chunk_pref);  // [PLANE_VALS][CH] (free: the pass is done with it)
+    double *sum = sh.warp_d[0];                                 // [PLANE_VALS] (free before the ICP)
+    double v = 0.0;
+    for (int c0 = 0; c0 < G; c0 += CH) {
+        const int m = min(CH, G - c0);
+        for (int e = threadIdx.x; e < PLANE_VALS * m; e += BLOCK) {
+            const int t = e / m, k = e - t * m;
+            stage[t * CH + k] = __ldcg(&D.part[t * G + c0 + k]);
+        }
+        __syncthreads();
+        if (threadIdx.x < PLANE_VALS)
+            for (int k = 0; k < m; ++k) v += stage[threadIdx.x * CH + k];
+        __syncthreads();
+    }
+    if (threadIdx.x < PLANE_VALS) sum[threadIdx.x] = v;
+    __syncthreads();
+    const int n_planes = static_cast<int>(sum[0]);
+    const double *H = sum + 3;  // upper triangle of the 6x6, row-major
+    double lam[3];
+    V3 ax[3];
+    int held[3];
+    const bool rot = threadIdx.x == 32;
+    if (threadIdx.x == 0 || rot) {
+        const double c6[6] = {rot ? H[15] : H[0], rot ? H[16] : H[1], rot ? H[17] : H[2],
+                              rot ? H[18] : H[6], rot ? H[19] : H[7], rot ? H[20] : H[11]};
+        const int n = degen_block(c6, D.ratio, n_planes > 0, lam, ax, held, rot ? pj->pr : pj->pt);
+        sh.warp_i[rot ? 1 : 0] = n;
+        if (blockIdx.x == gridDim.x - 1) {
+            DegenResult *r = D.res;
+            double *L = rot ? r->lam_r : r->lam_t, *A = rot ? r->ax_r : r->ax_t;
+            int *Hd = rot ? r->held_r : r->held_t;
+            for (int k = 0; k < 3; ++k) {
+                L[k] = lam[k];
+                A[k] = ax[k].x;
+                A[3 + k] = ax[k].y;
+                A[6 + k] = ax[k].z;
+                Hd[k] = held[k];
+            }
+            if (!rot) {
+                r->weight_sum = sum[1];
+                r->n_planes = n_planes;
+            }
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        pj->c = c;
+        pj->held = sh.warp_i[0] + sh.warp_i[1];
+    }
+    __syncthreads();
+}
+
 // the stand-alone pass (k_pose_pass): one source at one pose, the fit or the plane constraints
 struct PosePassParams {
     MapView m;
@@ -194,8 +299,10 @@ __device__ __forceinline__ double warp_sum(double v) {  // fixed butterfly: ever
     return v;
 }
 
-// the plane term of one correspondence (p, q) for this lane's value (lane < PLANE_VALS; warp-uniform arguments)
-__device__ __forceinline__ double plane_term(const MapView &m, const V3 &p, const V3 &q, int lane, int ji, int jj) {
+// the plane term of one correspondence (p, q) for this lane's value (lane < PLANE_VALS; warp-uniform arguments); the
+// rotational part of J is lever x n (lever = p about the map origin, p - c about a centre c)
+__device__ __forceinline__ double plane_term(const MapView &m, const V3 &p, const V3 &q, const V3 &lever, int lane, int ji,
+                                             int jj) {
     const int3 v = point_to_voxel(q.x, q.y, q.z, m.vdiv);
     int cnt = 0;
     const int slot = map_find(m, v.x, v.y, v.z, &cnt);  // q is stored in this voxel: found
@@ -228,7 +335,7 @@ __device__ __forceinline__ double plane_term(const MapView &m, const V3 &p, cons
     const V3 n = ev[0];
     const V3 r = p - q;
     const double e = (n.x * r.x + n.y * r.y) + n.z * r.z;
-    const V3 pn = cross(p, n);
+    const V3 pn = cross(lever, n);
     const double J[6] = {n.x, n.y, n.z, pn.x, pn.y, pn.z};
     double Ji = 0.0, Jj = 0.0;
 #pragma unroll
@@ -244,8 +351,9 @@ __device__ __forceinline__ double plane_term(const MapView &m, const V3 &p, cons
 
 // this CTA's partials of the fit (FIT: into fit_part[v][cta]) and of the plane constraints of the same correspondences
 // (PLANES: into plane_part[v][cta]), from one nearest-neighbour search per source point. The caller provides the grid
-// barrier behind it.
-template <bool FIT, bool PLANES>
+// barrier behind it. CENTRED: the plane Jacobian's lever is taken about the pose's position, J = [n, (p - pose.t) x n]
+// (the degeneracy pass, section 4.16 of DESIGN.md); otherwise about the map origin.
+template <bool FIT, bool PLANES, bool CENTRED = false>
 __device__ __noinline__ void op_fit_planes(Shared &sh, const MapView &m, const double *src, int n, const SE3 &pose,
                                            double max_dist, double kscale, double *fit_part, double *plane_part) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -268,7 +376,12 @@ __device__ __noinline__ void op_fit_planes(Shared &sh, const MapView &m, const d
                 sse += sqnorm(p - r.p);
                 ++corr;
             }
-            if constexpr (PLANES) pacc += plane_term(m, p, r.p, lane, ji, jj);
+            if constexpr (PLANES) {
+                if constexpr (CENTRED)
+                    pacc += plane_term(m, p, r.p, p - pose.t, lane, ji, jj);
+                else
+                    pacc += plane_term(m, p, r.p, p, lane, ji, jj);
+            }
         }
     }
     // (chunk_pref is free here: the ICP loop and the front end are done)
@@ -323,13 +436,16 @@ __device__ __forceinline__ void planes_finish(const PlaneOut &pl) {
 //   map update (all CTAs) | epilogue
 // Params = ReportParams: the fit pass (op_fit_planes) at the final pose, with PLANES the plane constraints of its
 // correspondences too, and fit_finish / planes_finish after the last barrier.
+// Params = DegenParams (a pipeline with a degeneracy ratio, which reports fits): the degeneracy pass at the initial guess
+// and one grid barrier in front of the ICP, whose steps are projected when the scan holds an axis (degen_form).
 // LOCALIZE (a localizer): the same statement against a read-only prior map, without local_map_.Update (KissICP.cpp:61).
 // Nothing is inserted, so there is no capacity check and no veto, and the map-update phase is the fit pass. Nothing
 // writes to the map. Otherwise (odometry) the fit pass runs in front of the map update, with one grid barrier between
 // them (op_fit_planes reads the table op_map_add writes).
 template <class Params, bool LOCALIZE = false, bool PLANES = false>
 __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
-    constexpr bool FIT = std::is_same<Params, ReportParams>::value;
+    constexpr bool FIT = std::is_base_of<ReportParams, Params>::value;
+    constexpr bool DEGEN = std::is_same<Params, DegenParams>::value;
     static_assert(FIT || (!LOCALIZE && !PLANES), "a localizer, and plane reporting, need the fit's ReportParams");
     __shared__ Shared sh;
     Grid g;
@@ -376,6 +492,18 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
     // sigma, initial guess (KissICP.cpp:44,47)
     const double sigma = sqrt(model_sse / num_samples);
     const SE3 guess = se3_mul(last_pose, last_delta);
+    DegenProj *proj = nullptr;  // the scan's projector when it holds an axis
+    if constexpr (DEGEN) {
+        __shared__ DegenProj s_proj;
+        const bool stamp = P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0;
+        if (stamp) P.sc.dbg[37] = globaltimer_ns();
+        op_fit_planes<false, true, true>(sh, P.m, fr.src, n_src, guess, 3.0 * sigma, sigma, nullptr, P.degen.part);
+        g.sync();
+        if (stamp) P.sc.dbg[38] = globaltimer_ns();
+        degen_form(sh, P.degen, guess.t, &s_proj);
+        if (stamp) P.sc.dbg[39] = globaltimer_ns();
+        if (s_proj.held > 0) proj = &s_proj;  // (the same in every CTA: formed from the same sums)
+    }
     // ICP (KissICP.cpp:50-54)
     const int G = static_cast<int>(gridDim.x);
     const int live = __ldcg(&P.m.counters[C_LIVE]);
@@ -390,8 +518,12 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
         kb_mark(0x400u + static_cast<unsigned>(T));
         if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.sc.dbg[32] = P.res->t_ns[7] = globaltimer_ns();
         if (static_cast<int>(blockIdx.x) < T) {
-            op_icp_team(P.team, P.sc, sh, P.m, n_src, guess, 3.0 * sigma, sigma, P.max_iter, P.conv,
-                        kb_dyn_smem, T, P.tag_base);
+            if (DEGEN && proj != nullptr)
+                op_icp_team_proj(P.team, P.sc, sh, P.m, n_src, guess, 3.0 * sigma, sigma, P.max_iter, P.conv,
+                                 kb_dyn_smem, T, P.tag_base, proj);
+            else
+                op_icp_team(P.team, P.sc, sh, P.m, n_src, guess, 3.0 * sigma, sigma, P.max_iter, P.conv,
+                            kb_dyn_smem, T, P.tag_base);
             if (blockIdx.x == 0 && threadIdx.x == 0) {
                 team_publish(P.team, sh);
                 if (P.sc.profile) P.res->t_ns[10] = globaltimer_ns();  // iterations done (team member 0)
@@ -414,8 +546,12 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
         if (threadIdx.x == 0) team_collect(P.team, sh);
         __syncthreads();
     } else {
-        op_icp(g, P.sc, sh, P.m, fr.src, P.ws.work, n_src, guess, 3.0 * sigma, sigma, P.max_iter, P.conv,
-               reinterpret_cast<QCache *>(kb_dyn_smem), P.tag_base);
+        if (DEGEN && proj != nullptr)
+            op_icp_proj(g, P.sc, sh, P.m, fr.src, P.ws.work, n_src, guess, 3.0 * sigma, sigma, P.max_iter, P.conv,
+                        reinterpret_cast<QCache *>(kb_dyn_smem), P.tag_base, proj);
+        else
+            op_icp(g, P.sc, sh, P.m, fr.src, P.ws.work, n_src, guess, 3.0 * sigma, sigma, P.max_iter, P.conv,
+                   reinterpret_cast<QCache *>(kb_dyn_smem), P.tag_base);
         // Without ICP (empty map, max_iter <= 0) op_icp has no grid-wide rendezvous, and with a prefetched front end
         // (the replay of a vetoed first frame) neither has anything above. Every CTA must have read the state the
         // decisions above depend on (vetoed, the map counters) before any CTA starts the map update, which changes it.
@@ -505,4 +641,6 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
 // defined in report.cu, the reporting device module: k_register_frame<ReportParams, localizer, planes> (takes a
 // ReportParams) and the stand-alone k_pose_pass with the fit or with the plane constraints (takes a PosePassParams)
 const void *report_kernel(bool localizer, bool planes);
+// defined in degeneracy.cu, a device module of its own: k_register_frame<DegenParams, localizer, planes>
+const void *degeneracy_kernel(bool localizer, bool planes);
 const void *pose_pass_kernel(bool fit);

@@ -715,10 +715,13 @@ __device__ __noinline__ SE3 team_exp_large(const double dx[6]) { return se3_exp_
 __device__ __noinline__ bool team_norm_below(double n2, double conv) { return sqrt(n2) < conv; }
 
 // dx = JTJ.ldlt().solve(-JTr) and estimation = SE3::exp(dx) (Registration.cpp:156-157) on the 16 accumulators; returns
-// the squared norm of dx. used_schur: the structured solve took the system.
-__device__ __forceinline__ double team_solve_step(const double sys[NACC], double dx[6], SE3 &est, bool &used_schur) {
+// the squared norm of dx. used_schur: the structured solve took the system. kProj: dx is projected by *proj first.
+template <bool kProj = false>
+__device__ __forceinline__ double team_solve_step(const double sys[NACC], double dx[6], SE3 &est, bool &used_schur,
+                                                  const DegenProj *proj = nullptr) {
     used_schur = icp_solve_schur(sys, dx);
     if (!used_schur) team_solve_ldlt(sys, dx);  // structured 3x3 Schur solve; cold: pivoted LDL^T
+    if constexpr (kProj) degen_project(*proj, dx);
     const double theta_sq = (dx[3] * dx[3] + dx[4] * dx[4]) + dx[5] * dx[5];
     if (theta_sq >= kEps * kEps && theta_sq < 0.01) {
         est = se3_exp_small(dx, theta_sq);
@@ -739,14 +742,15 @@ __device__ __forceinline__ bool team_converged(double n2, double conv) {
 }
 
 // one thread: the solver step of the iteration on the gathered sums -> sh.pending, sh.flag
-__device__ __forceinline__ void team_solve(Shared &sh, double conv, bool last_allowed) {
+template <bool kProj>
+__device__ __forceinline__ void team_solve(Shared &sh, double conv, bool last_allowed, const DegenProj *proj) {
     double sys[NACC];
 #pragma unroll
     for (int i = 0; i < NACC; ++i) sys[i] = sh.red[i];
     double dx[6];
     SE3 est;
     bool used_schur;
-    const double n2 = team_solve_step(sys, dx, est, used_schur);
+    const double n2 = team_solve_step<kProj>(sys, dx, est, used_schur, proj);
     sh.pending = est;
     sh.flag = (team_converged(n2, conv) || last_allowed) ? 1 : 0;
 }
@@ -756,11 +760,12 @@ __device__ __forceinline__ void team_solve(Shared &sh, double conv, bool last_al
 // kSlot = false: the team is CTAs [0, T) of the launch and ts.ll is sized for TEAM_MAX CTAs (k_register_frame, k_icp).
 // kSlot = true: this CTA is member `slot_member` of a slot of k_icp_batch whose all-gather region ts.ll holds
 // [2][slot_stride][slot_stride][NPART] chunks (slot_stride >= T).
-template <bool kSlot>
+// kProj: every step is projected by *proj (degen_project) before Exp and the convergence test.
+template <bool kSlot, bool kProj = false>
 __device__ __forceinline__ void icp_team_iterate(const TeamScratch &ts, const Scratch &sc, Shared &sh, const MapView &m, int n,
                                                  const SE3 &guess, double max_dist, double kscale, int max_iter, double conv,
                                                  unsigned char *dyn_smem, int T, unsigned tag_base, int slot_member,
-                                                 int slot_stride) {
+                                                 int slot_stride, const DegenProj *proj = nullptr) {
     const int member = kSlot ? slot_member : static_cast<int>(blockIdx.x);
     const int stride = kSlot ? slot_stride : TEAM_MAX;
     const int nq = member < n ? (n - member + T - 1) / T : 0;
@@ -814,7 +819,7 @@ __device__ __forceinline__ void icp_team_iterate(const TeamScratch &ts, const Sc
         if (stamp) sc.dbg[64 + 4 * member + 2] = globaltimer_ns();
 #endif
         KB_TCYC(6);
-        if (threadIdx.x == BLOCK - 1) team_solve(sh, conv, j + 1 >= max_iter);  // warp 15 owns no source point (TQ_MAX = 120)
+        if (threadIdx.x == BLOCK - 1) team_solve<kProj>(sh, conv, j + 1 >= max_iter, proj);  // warp 15 owns no source point (TQ_MAX = 120)
         __syncthreads();
         KB_TCYC(7);
         if (sh.flag) break;  // (T_icp = estimation * T_icp of this iteration: team_accumulate, off the critical path)
@@ -833,6 +838,13 @@ __device__ __noinline__ void op_icp_team(const TeamScratch &ts, const Scratch &s
                                          const SE3 &guess, double max_dist, double kscale, int max_iter, double conv,
                                          unsigned char *dyn_smem, int T, unsigned tag_base) {
     icp_team_iterate<false>(ts, sc, sh, m, n, guess, max_dist, kscale, max_iter, conv, dyn_smem, T, tag_base, 0, TEAM_MAX);
+}
+// the team of the degeneracy module's k_register_frame for a scan with a held axis: op_icp_team with projected steps
+__device__ __noinline__ void op_icp_team_proj(const TeamScratch &ts, const Scratch &sc, Shared &sh, const MapView &m, int n,
+                                              const SE3 &guess, double max_dist, double kscale, int max_iter, double conv,
+                                              unsigned char *dyn_smem, int T, unsigned tag_base, const DegenProj *proj) {
+    icp_team_iterate<false, true>(ts, sc, sh, m, n, guess, max_dist, kscale, max_iter, conv, dyn_smem, T, tag_base, 0,
+                                  TEAM_MAX, proj);
 }
 // one team of k_icp_batch: member `member` of a slot whose all-gather region (ts.ll) is sized for `stride` CTAs
 __device__ __noinline__ void op_icp_team_slot(const TeamScratch &ts, const Scratch &sc, Shared &sh, const MapView &m, int n,

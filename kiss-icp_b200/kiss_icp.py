@@ -20,6 +20,13 @@ before the scan's ``local_map.update``. Poses, thresholds and the map are the sa
 ``report_constraints=True`` (a localizer, or odometry, where it turns fit reporting on too) also reports, in
 ``last_constraints`` and ``register_frames(..., return_constraints=True)``, the plane constraints of each scan's fit
 (constraints.Constraints): which directions the scan pins down. Poses, fits and the map are the same as without it.
+
+``degeneracy_ratio=rho`` (0 < rho < 1; a localizer, or odometry, where it turns fit reporting on too) holds the
+prediction along directions a scan does not constrain: before ICP, the plane information at the initial guess
+(centred at its position) is eigen-decomposed blockwise, axes with an eigenvalue below rho times their block's largest
+are held, and every ICP step is projected off them (DESIGN.md section 4.16). ``last_degeneracy`` and
+``register_frames(..., return_degeneracy=True)`` report it per scan (constraints.ScanDegeneracy). A scan that holds
+nothing registers bit for bit as without it. ``constraints.RECOMMENDED_DEGENERACY_RATIO`` is the ratio to start from.
 """
 from __future__ import annotations
 
@@ -32,7 +39,7 @@ import numpy as np
 
 from . import _native as N
 from .config import KISSConfig, load_config
-from .constraints import Constraints, _constraints_of, _from_struct, _from_structs
+from .constraints import Constraints, ScanDegeneracy, _constraints_of, _from_struct, _from_structs, _scan_degeneracy
 from .mapping import VoxelHashMap, check_value, get_voxel_hash_map
 from .places import PlaceDatabase, PlaceRelocalizationResult
 from .preprocess import Preprocessor, get_preprocessor
@@ -121,7 +128,7 @@ class _PipelineThreshold:
 
 class KissICP:
     def __init__(self, config: KISSConfig | None = None, fused: bool = True, prior_map: VoxelHashMap | None = None,
-                 report_fit: bool = False, report_constraints: bool = False):
+                 report_fit: bool = False, report_constraints: bool = False, degeneracy_ratio: float = 0.0):
         if prior_map is not None and not isinstance(prior_map, VoxelHashMap):
             raise TypeError(f"prior_map must be a VoxelHashMap, not {type(prior_map).__name__}")
         self.config = config if config is not None else load_config()
@@ -130,8 +137,14 @@ class KissICP:
         self.fused = bool(fused) and self.config.adaptive_threshold.fixed_threshold is None
         self.localizer = prior_map is not None
         self._report_constraints = bool(report_constraints)
-        # (a localizer always reports fits; plane constraints are reported next to the fit)
-        self._report_fit = self.localizer or bool(report_fit) or self._report_constraints
+        rho = float(degeneracy_ratio)
+        if not 0.0 <= rho < 1.0:  # (NaN fails too)
+            raise ValueError(f"degeneracy_ratio {degeneracy_ratio} is not in [0, 1)")
+        if rho > 0.0 and not (bool(fused) and self.config.adaptive_threshold.fixed_threshold is None):
+            raise ValueError("degeneracy_ratio needs the fused pipeline (fused=True, an adaptive threshold)")
+        self._degeneracy_ratio = rho
+        # (a localizer always reports fits; plane constraints and the degeneracy pass run next to the fit)
+        self._report_fit = self.localizer or bool(report_fit) or self._report_constraints or rho > 0.0
         self._h = None
         if self.localizer:
             self._check_prior(prior_map)
@@ -160,6 +173,8 @@ class KissICP:
                     N.check(N.lib().kb_pipeline_set_fit_reporting(self._h, 1))
             if self._report_constraints:
                 N.check(N.lib().kb_pipeline_set_constraint_reporting(self._h, 1))
+            if rho > 0.0:
+                N.check(N.lib().kb_pipeline_set_degeneracy_ratio(self._h, rho))
             self.adaptive_threshold = _PipelineThreshold(self)
         else:
             self._last_pose = np.eye(4)
@@ -257,6 +272,23 @@ class KissICP:
         N.check(N.lib().kb_pipeline_last_constraints(self._h, C.byref(c)))
         return _from_struct(c)
 
+    @property
+    def degeneracy_ratio(self) -> float:
+        """the degeneracy ratio (0: off), KissICP(config, degeneracy_ratio=...)"""
+        return self._degeneracy_ratio
+
+    def _check_degeneracy(self):
+        if self._degeneracy_ratio <= 0.0:
+            raise ValueError("degeneracy results are reported by pipelines created with degeneracy_ratio > 0")
+
+    @property
+    def last_degeneracy(self) -> ScanDegeneracy:
+        """the degeneracy-aware ICP's result of the last scan (zeros before the first)"""
+        self._check_degeneracy()
+        d = N.Degeneracy()
+        N.check(N.lib().kb_pipeline_last_degeneracy(self._h, C.byref(d)))
+        return _scan_degeneracy(d)
+
     def _sigma_next(self):
         s = N.dbl(0)
         N.check(N.lib().kb_pipeline_threshold(self._h, C.byref(s)))
@@ -331,19 +363,23 @@ class KissICP:
         N.check(N.lib().kb_pipeline_last_clouds(self._h, N.ptr(pre), a.value, N.ptr(src), b.value))
         return pre, src
 
-    def register_frames(self, frames, timestamps=None, return_fits: bool = False, return_constraints: bool = False):
+    def register_frames(self, frames, timestamps=None, return_fits: bool = False, return_constraints: bool = False,
+                        return_degeneracy: bool = False):
         """Register a whole sequence (the dataset loop of python/kiss_icp/pipeline.py:106-112) -> poses (K,4,4).
 
         Same results as K ``register_frame`` calls; the frames are queued on the device (copy of frame k+1
         overlaps the registration of frame k, results are read behind the queue). ``frames`` is a sequence of
         (N_k,3) arrays, all float64 or all float32; ``timestamps`` a matching sequence (or None).
         ``return_fits`` (localizers and report_fit=True only) -> (poses, fits): a Fit of arrays, one entry per frame.
-        ``return_constraints`` (report_constraints=True only) appends a Constraints of arrays: (poses, [fits,] constraints)."""
+        ``return_constraints`` (report_constraints=True only) appends a Constraints of arrays: (poses, [fits,] constraints).
+        ``return_degeneracy`` (degeneracy_ratio > 0 only) appends a ScanDegeneracy of arrays, one entry per frame."""
         K = len(frames)
         if return_fits:
             self._check_reports_fits()
         if return_constraints:
             self._check_reports_constraints()
+        if return_degeneracy:
+            self._check_degeneracy()
         if timestamps is None:
             timestamps = [np.empty(0)] * K
         if len(timestamps) != K:
@@ -374,10 +410,10 @@ class KissICP:
         ts = [np.ascontiguousarray(np.asarray(t).ravel(), dtype=np.float64) for t in timestamps]
         return self._register_frames_raw([N.ptr(a) for a in pts], [len(a) for a in pts], [N.ptr(t) for t in ts],
                                          [len(t) for t in ts], 1 if f32 else 0, return_fits=return_fits,
-                                         return_constraints=return_constraints)
+                                         return_constraints=return_constraints, return_degeneracy=return_degeneracy)
 
     def _register_frames_raw(self, xyz_ptrs, sizes, ts_ptrs, ts_sizes, layout, return_fits: bool = False,
-                             return_constraints: bool = False):
+                             return_constraints: bool = False, return_degeneracy: bool = False):
         """raw-pointer form (host or device addresses): layout 0 host f64, 1 host f32, 2 device f64"""
         K = len(xyz_ptrs)
         as_vp = lambda v: v if isinstance(v, C.c_void_p) else C.c_void_p(int(v) if v else None)
@@ -388,13 +424,20 @@ class KissICP:
         poses = np.empty((K, 4, 4))
         fits = (N.Fit * K)() if return_fits else None
         cons = (N.Constraints * K)() if return_constraints else None
-        N.check(N.lib().kb_pipeline_register_frames_constraints(self._h, X, n, T, nt, K, int(layout), N.ptr(poses), fits,
-                                                                cons))
+        if return_degeneracy:
+            degs = (N.Degeneracy * K)()
+            N.check(N.lib().kb_pipeline_register_frames_degeneracy(self._h, X, n, T, nt, K, int(layout), N.ptr(poses),
+                                                                   fits, cons, degs))
+        else:
+            N.check(N.lib().kb_pipeline_register_frames_constraints(self._h, X, n, T, nt, K, int(layout), N.ptr(poses),
+                                                                    fits, cons))
         out = [poses]
         if return_fits:
             out.append(_fits_from_structs(fits))
         if return_constraints:
             out.append(_from_structs(cons))
+        if return_degeneracy:
+            out.append(_scan_degeneracy(degs))
         return out[0] if len(out) == 1 else tuple(out)
 
     def _register_frame_modular(self, frame, timestamps):

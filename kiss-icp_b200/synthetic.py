@@ -263,3 +263,36 @@ def surface_cloud(n_raw: int, seed: int = 0, density: float = 14.0, wall_spacing
     pts = np.concatenate([ground, walls])
     rng.shuffle(pts)
     return pts
+
+
+class Tunnel:
+    """A straight tunnel along x: floor z = 0, ceiling z = ``height``, walls y = +-width / 2, no other structure, so that
+    nothing constrains translation along x. A ring LiDAR (``beams`` x ``cols``, ``elev_deg``) at ``sensor_height`` on the
+    axis moves ``step`` metres along +x per scan; ranges up to ``max_ray``, Gaussian noise ``noise``, seeded per scan.
+    ``scan(k)`` -> (points in the sensor frame, no stamps), ``pose(k)`` -> the true 4x4 pose of scan k."""
+
+    def __init__(self, seed=0, beams=32, cols=512, elev_deg=(-25.0, 15.0), width=8.0, height=5.0, sensor_height=1.7,
+                 step=0.5, max_ray=100.0, noise=0.01):
+        self.seed, self.width, self.height, self.h0 = seed, width, height, sensor_height
+        self.step, self.max_ray, self.noise = step, max_ray, noise
+        el = np.radians(np.linspace(elev_deg[0], elev_deg[1], beams))
+        az = np.radians(np.arange(cols) * (360.0 / cols))
+        E, A = np.meshgrid(el, az, indexing="ij")
+        self.dirs = np.stack([np.cos(E) * np.cos(A), np.cos(E) * np.sin(A), np.sin(E)], -1).reshape(-1, 3)
+
+    def pose(self, k: float) -> np.ndarray:
+        T = np.eye(4)
+        T[0, 3] = self.step * k
+        return T
+
+    def scan(self, k: int):
+        D = self.dirs
+        t = np.full(len(D), np.inf)
+        for ax, val in ((1, self.width / 2), (1, -self.width / 2), (2, -self.h0), (2, self.height - self.h0)):
+            with np.errstate(divide="ignore", invalid="ignore"):
+                tt = val / D[:, ax]
+            t = np.where((tt > 0) & (tt < t), tt, t)
+        ok = np.isfinite(t) & (t < self.max_ray)
+        rng = np.random.default_rng((self.seed, int(k)))
+        pts = t[ok, None] * D[ok] + rng.normal(0.0, self.noise, (int(ok.sum()), 3))
+        return pts, np.empty(0)
