@@ -403,6 +403,54 @@ int kb_pipeline_register_frames_degeneracy(kb_pipeline *p, const void *const *xy
                                            int layout, double *poses_out, kb_fit *fits_out, kb_constraints *constraints_out,
                                            kb_degeneracy *degeneracy_out);
 
+/* ---- sampled motion: deskew and predict a scan from IMU or wheel-odometry samples --------------------------
+ * No reference counterpart (DESIGN.md section 4.17). The pipeline's own motion model is KISS-ICP's constant velocity:
+ * the previous frame's last_delta deskews the next scan and predicts its pose. A kb_motion replaces it for one frame
+ * with the LiDAR's measured trajectory T(t), sampled at times[k]:
+ *   T(t) = T_k Exp(tau xi_k), k the interval [t_k, t_k+1] holding t, tau = t - t_k, xi_k = Log(T_k^-1 T_k+1) / (t_k+1 - t_k)
+ * (= T_k Exp(alpha Log(T_k^-1 T_k+1)), alpha = tau / (t_k+1 - t_k)). Before t_0 and after t_m-1 the first and the last
+ * interval are extrapolated.
+ * Deskew (cfg.deskew on and the frame has stamps): point p with stamp s becomes T(end_time)^-1 T(s + stamp_offset) p, and
+ * the range crop follows as without a kb_motion. A NaN stamp makes a NaN point, which the crop drops. Constant stamps
+ * are valid. Without stamps, or with cfg.deskew = 0, the points are used as they are.
+ * Prediction: when the previous frame was registered with a kb_motion whose end_time (kb_pipeline_motion_time) lies in
+ * [t_0, t_m-1] of this frame's samples, the initial guess is last_pose * T(prev)^-1 T(end_time); otherwise it is the
+ * constant-velocity guess last_pose * last_delta. The model deviation of the adaptive threshold is guess^-1 new_pose,
+ * last_delta after the frame is last_pose^-1 new_pose and the degeneracy pass is taken at this guess, as always. */
+#define KB_MOTION_MAX_SAMPLES 65536
+typedef struct kb_motion {
+    const double *times;  /* [m], strictly increasing, finite, in the sample clock                           */
+    const double *poses;  /* [m][16] row-major SE(3): the LiDAR's pose at times[k] in any fixed frame        */
+    size_t m;             /* 2 <= m <= KB_MOTION_MAX_SAMPLES; 0 in a frame of kb_pipeline_register_frames_motion:
+                             no kb_motion for that frame                                                      */
+    double stamp_offset;  /* added to every point stamp to put it on the sample clock (per-scan stamps)      */
+    double end_time;      /* sample-clock time the scan's pose refers to; its points are deskewed to it      */
+} kb_motion;
+/* Host only (works without a device). KB_ERR_INVALID_ARG for a NULL motion, times or poses, m outside
+ * [2, KB_MOTION_MAX_SAMPLES], times that are not finite or not strictly increasing, consecutive samples whose relative
+ * rotation is within 1e-6 rad of pi or more (where Log is not unique), a non-finite stamp_offset or end_time;
+ * KB_ERR_NOT_SE3 for a pose outside SE(3). */
+int kb_motion_check(const kb_motion *motion);
+/* kb_pipeline_register_frames_degeneracy with a kb_motion per frame: motion[count] may be NULL (none at all), and a frame
+ * whose motion has m == 0 has none. Every motion is checked (kb_motion_check) before any device work; on error nothing is
+ * registered. A frame with a kb_motion does not depend on the previous frame's result, so, like a frame without stamps,
+ * its front end (deskew, crop, downsampling) may run in the launch of the frame before it. A frame vetoed for table
+ * capacity and replayed keeps its prediction. Outputs as kb_pipeline_register_frames_degeneracy. */
+int kb_pipeline_register_frames_motion(kb_pipeline *p, const void *const *xyz, const size_t *n,
+                                       const double *const *timestamps, const size_t *n_timestamps,
+                                       const kb_motion *motion, size_t count, int layout, double *poses_out,
+                                       kb_fit *fits_out, kb_constraints *constraints_out, kb_degeneracy *degeneracy_out);
+/* the end_time of the last frame registered, if it had a kb_motion, else NaN (also for a new pipeline). Part of a
+ * checkpoint next to kb_pipeline_state: set it back with kb_pipeline_set_motion_time (NaN: none; +-inf is
+ * KB_ERR_INVALID_ARG). */
+int kb_pipeline_motion_time(const kb_pipeline *p, double *out);
+int kb_pipeline_set_motion_time(kb_pipeline *p, double end_time);
+/* The deskew of one frame alone: out[k] = T(end_time)^-1 T(timestamps[k] + stamp_offset) xyz[k], no crop. Without
+ * stamps (n_timestamps == 0) out = xyz. KB_ERR_OUT_OF_RANGE for 0 < n_timestamps < n, the checks of kb_motion_check
+ * otherwise. Synchronous; out may alias xyz. */
+int kb_deskew_motion(const double *xyz, size_t n, const double *timestamps, size_t n_timestamps, const kb_motion *motion,
+                     double *out);
+
 /* ---- relocalization: a global pose search in a bounded region ----------------------------
  * No reference counterpart. Finds a scan's pose in a map without an initial pose: every hypothesis of a grid in x, y
  * and yaw around a centre is scored on the device, the best peaks are refined with kb_registration_align_batch, and

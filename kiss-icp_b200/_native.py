@@ -104,6 +104,11 @@ class Degeneracy(C.Structure):
                 ("translation_held", i32 * 3), ("rotation_held", i32 * 3)]
 
 
+class Motion(C.Structure):
+    """kb_motion: sampled poses of the LiDAR that deskew and predict one frame"""
+    _fields_ = [("times", vp), ("poses", vp), ("m", sz), ("stamp_offset", dbl), ("end_time", dbl)]
+
+
 class RelocSearch(C.Structure):
     """kb_reloc_search: the hypothesis grid of kb_relocalize"""
     _fields_ = [("center", dbl * 16), ("half_cells_x", i32), ("half_cells_y", i32), ("step", dbl), ("n_yaw", i32),
@@ -273,6 +278,11 @@ SIGNATURES = {
     "kb_pipeline_degeneracy_ratio": (i32, [vp, C.POINTER(dbl)]),
     "kb_pipeline_last_degeneracy": (i32, [vp, C.POINTER(Degeneracy)]),
     "kb_pipeline_register_frames_degeneracy": (i32, [vp, vp, vp, vp, vp, sz, i32, vp, vp, vp, vp]),
+    "kb_motion_check": (i32, [C.POINTER(Motion)]),
+    "kb_pipeline_register_frames_motion": (i32, [vp, vp, vp, vp, vp, vp, sz, i32, vp, vp, vp, vp]),
+    "kb_pipeline_motion_time": (i32, [vp, C.POINTER(dbl)]),
+    "kb_pipeline_set_motion_time": (i32, [vp, dbl]),
+    "kb_deskew_motion": (i32, [vp, sz, vp, sz, C.POINTER(Motion), vp]),
     "kb_place_params_default": (None, [C.POINTER(PlaceParams)]),
     "kb_place_db_create": (i32, [C.POINTER(PlaceParams), C.POINTER(vp)]),
     "kb_place_db_destroy": (i32, [vp]),

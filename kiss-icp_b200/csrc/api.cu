@@ -23,6 +23,7 @@
 #include "../../include/kiss_icp_b200_debug.h"
 #include "api.cuh"
 #include "kernels.cuh"
+#include "motion.cuh"
 #include "probe.cuh"
 #include "relocalize.cuh"
 
@@ -422,6 +423,18 @@ struct kb_pipeline {
         Event copied, done, read;
     };
     Slot q[Q_DEPTH];
+    // sampled motion (kb_pipeline_register_frames_motion): the end_time of the last frame registered if it had a
+    // kb_motion (NaN: it had none), and per queue slot the frame's interval table (pinned staging and device copy), its
+    // deskewed points, its prediction (pinned) and the state's last_delta as it was before the prediction was copied in
+    double motion_end = NAN;
+    struct MotionSlot {
+        PinBuf<MotionSeg> pin_tab;
+        DBuf<MotionSeg> tab;
+        DBuf<double> xyz;
+        PinBuf<SE3> pin_delta;
+        DBuf<SE3> saved;
+    };
+    MotionSlot mq[Q_DEPTH];
     Stream copy_stream, res_stream;
     PinBuf<FrameResult> q_res;    // [Q_DEPTH] host copies of the frame results
     DBuf<FrameResult> q_res_dev;  // [Q_DEPTH] device side: where the kernels write them
@@ -1441,6 +1454,40 @@ int kb_correct_kitti_scan_dev(const double *d_xyz, size_t n, double *d_out_xyz) 
     return correct_kitti_launch(*c->ex, d_xyz, d_out_xyz, n);  // asynchronous on the calling thread's stream
 }
 
+int kb_deskew_motion(const double *xyz, size_t n, const double *timestamps, size_t n_timestamps, const kb_motion *motion,
+                     double *out) {
+    if (n && (!xyz || !out)) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n_timestamps && !timestamps) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (n >= (size_t(1) << 30)) return fail(KB_ERR_INVALID_ARG, "frame too large");
+    RET(motion_check(motion));
+    if (n_timestamps && n_timestamps < n)
+        return fail(KB_ERR_OUT_OF_RANGE, "timestamps (%zu) shorter than frame (%zu)", n_timestamps, n);
+    DefaultCtx *c;
+    RET(default_ctx(&c));
+    if (!n_timestamps) {  // nothing to deskew with: the points as they are
+        if (n && out != xyz) std::memmove(out, xyz, n * 24);
+        return KB_OK;
+    }
+    Exec &ex = *c->ex;
+    CK(cudaSetDevice(ex.device));
+    const std::vector<MotionSeg> tab = motion_table(*motion);
+    DBuf<MotionSeg> d_tab;
+    CK(d_tab.alloc(tab.size()));
+    RET(c->ws.in.ensure(3 * std::max<size_t>(n, 1)));
+    RET(c->ws.tmp.ensure(3 * std::max<size_t>(n, 1)));
+    RET(c->ws.ts.ensure(std::max<size_t>(n, 1)));
+    CK(cudaMemcpyAsync(d_tab.p, tab.data(), tab.size() * sizeof(MotionSeg), cudaMemcpyHostToDevice, ex.stream));
+    if (n) {
+        CK(cudaMemcpyAsync(c->ws.in.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
+        CK(cudaMemcpyAsync(c->ws.ts.p, timestamps, n * 8, cudaMemcpyHostToDevice, ex.stream));
+    }
+    CK(motion_deskew(ex.stream, ex.sms, d_tab.p, static_cast<int>(tab.size()), c->ws.in.p, false, c->ws.ts.p,
+                     motion->stamp_offset, n, c->ws.tmp.p));
+    if (n) ++ex.launches;
+    if (n) CK(cudaMemcpyAsync(out, c->ws.tmp.p, n * 24, cudaMemcpyDeviceToHost, ex.stream));
+    return ex.sync();  // (d_tab is released after the kernel has read it)
+}
+
 // ------------------------------------------------------------------------------- KissICP pipeline
 void kb_config_default(kb_config *cfg) {
     if (!cfg) return;
@@ -1559,9 +1606,10 @@ static size_t pipeline_extra(const kb_pipeline *p, size_t n) {
 
 // enqueue one RegisterFrame on the pipeline's stream; the result, and the reports the pipeline computes, go to queue
 // slot `slot` on the device
-// `next_xyz` (may be null): the frame after this one, already on the device, no timestamps -> its front end is prefetched
+// `next_xyz` (may be null): the frame after this one, already on the device (float[n][3] if next_f32), no timestamps ->
+// its front end is prefetched
 static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, size_t n, const double *d_ts, size_t n_ts,
-                           bool in_f32, size_t slot, const double *next_xyz, size_t next_n) {
+                           bool in_f32, size_t slot, const double *next_xyz, size_t next_n, bool next_f32) {
     Exec &ex = *p->ex;
     FrameParams P;
     P.m = p->map->view();
@@ -1572,7 +1620,7 @@ static int pipeline_launch(kb_pipeline *p, long long id, const double *d_xyz, si
     P.id = id;
     P.next_in = next_xyz;
     P.next_n = static_cast<int>(next_n);
-    P.next_in_f32 = in_f32 ? 1 : 0;
+    P.next_in_f32 = next_f32 ? 1 : 0;
     P.ws = p->ws.view();
     P.st = p->d_state.p;
     P.res = p->q_res_dev.p + slot;
@@ -1760,13 +1808,22 @@ static const char *const kNoConstraints =
 // kb_pipeline_register_frames[_fit|_constraints|_degeneracy] and, with count = 1, kb_pipeline_register_frame[_f32|_dev];
 // fits_out (pipelines that report fits only, may be NULL) receives one fit per frame, constraints_out (pipelines that
 // report plane constraints only, may be NULL) one kb_constraints per frame, degen_out (pipelines with a degeneracy
-// ratio only, may be NULL) one kb_degeneracy per frame
+// ratio only, may be NULL) one kb_degeneracy per frame; motion (may be NULL) one kb_motion per frame (m == 0: none)
 static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
                            const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out,
-                           kb_constraints *constraints_out, kb_degeneracy *degen_out = nullptr) {
+                           kb_constraints *constraints_out, kb_degeneracy *degen_out = nullptr,
+                           const kb_motion *motion = nullptr) {
     if (!p || (count && (!xyz || !n))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (layout != KB_FRAMES_HOST_F64 && layout != KB_FRAMES_HOST_F32 && layout != KB_FRAMES_DEVICE_F64)
         return fail(KB_ERR_INVALID_ARG, "unknown frame layout %d", layout);
+    std::vector<char> has_motion(count, 0);
+    if (motion)
+        for (size_t k = 0; k < count; ++k)
+            if (motion[k].m) {
+                const int st = motion_check(motion + k);
+                if (st != KB_OK) return fail(st, "frame %zu: %s", k, tl_err.c_str());
+                has_motion[k] = 1;
+            }
     constexpr size_t D = kb_pipeline::Q_DEPTH;
     Exec &ex = *p->ex;
     CK(cudaSetDevice(ex.device));
@@ -1793,11 +1850,26 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
     RET(p->ws.ensure(max_n));
     RET(p->ws.ensure_pipeline(max_n));
     RET(queue_init(p, max_n, any_ts, dev_in));
+    // Sampled motion: a frame with stamps to deskew with (desk) gets its points deskewed by k_deskew_motion into its slot's
+    // buffer and registers them without stamps. Its prediction T(prev)^-1 T(end_time), where the previous frame's
+    // end_time is covered by its samples, is copied into the state's last_delta right before its launch.
+    std::vector<char> desk(valid, 0), predict(valid, 0);
+    std::vector<std::vector<MotionSeg>> tabs(valid);
+    std::vector<SE3> pred(valid);
+    for (size_t k = 0; k < valid; ++k) {
+        if (!has_motion[k]) continue;
+        const kb_motion &mk = motion[k];
+        desk[k] = use_ts[k];
+        if (desk[k]) tabs[k] = motion_table(mk);
+        const double prev = k ? (has_motion[k - 1] ? motion[k - 1].end_time : NAN) : p->motion_end;
+        predict[k] = prev >= mk.times[0] && prev <= mk.times[mk.m - 1];
+        if (predict[k]) pred[k] = motion_between(mk, prev, mk.end_time);
+    }
 
     // Pipeline: frame k is registered by launch k, whose idle CTAs also compute the front end of frame k + 1 when that
     // frame has no timestamps (nothing of it depends on frame k's pose then); so frame k + 1 must be on the device when
     // launch k starts: uploads run one frame ahead of the launches, Q_DEPTH - 1 launches may be in flight.
-    size_t next_submit = 0, next_absorb = 0, next_upload = 0;
+    size_t next_submit = 0, next_absorb = 0, next_upload = 0, next_deskew = 0;
     int attempts = 0;
     const long long id0 = p->next_id;
     auto upload = [&](size_t u) -> int {  // host layouts: frame u -> slot u % D on the copy stream
@@ -1808,10 +1880,36 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
         CK(cudaEventRecord(s.copied.p, p->copy_stream.p));
         return KB_OK;
     };
-    auto take = [&](size_t k, Taken *taken) {  // the result of frame k, once its launch and read-back have ended
-        return take_result(p, p->q_res.p[k % D], n[k], id0 + static_cast<long long>(k), k % D,
-                           poses_out ? poses_out + 16 * k : nullptr, fits_out ? fits_out + k : nullptr,
-                           constraints_out ? constraints_out + k : nullptr, degen_out ? degen_out + k : nullptr, taken);
+    auto take = [&](size_t k, Taken *taken) -> int {  // the result of frame k, once its launch and read-back have ended
+        RET(take_result(p, p->q_res.p[k % D], n[k], id0 + static_cast<long long>(k), k % D,
+                        poses_out ? poses_out + 16 * k : nullptr, fits_out ? fits_out + k : nullptr,
+                        constraints_out ? constraints_out + k : nullptr, degen_out ? degen_out + k : nullptr, taken));
+        if (*taken == TAKEN_ABSORBED) p->motion_end = has_motion[k] ? motion[k].end_time : NAN;
+        return KB_OK;
+    };
+    auto deskew = [&](size_t j) -> int {  // frame j (on the device) -> its slot's deskewed points, on the frame stream
+        auto &m = p->mq[j % D];
+        const std::vector<MotionSeg> &tab = tabs[j];
+        RET(m.pin_tab.ensure(tab.size()));
+        RET(m.tab.ensure(tab.size()));
+        RET(m.xyz.ensure(3 * std::max<size_t>(n[j], 1)));
+        std::memcpy(m.pin_tab.p, tab.data(), tab.size() * sizeof(MotionSeg));  // (frame j - D, its last reader, has ended)
+        CK(cudaMemcpyAsync(m.tab.p, m.pin_tab.p, tab.size() * sizeof(MotionSeg), cudaMemcpyHostToDevice, ex.stream));
+        const void *in = dev_in ? xyz[j] : p->q[j % D].in.p;
+        const double *ts = dev_in ? timestamps[j] : p->q[j % D].ts.p;
+        CK(motion_deskew(ex.stream, ex.sms, m.tab.p, static_cast<int>(tab.size()), in, f32, ts, motion[j].stamp_offset,
+                         n[j], m.xyz.p));
+        if (n[j]) ++ex.launches;
+        return KB_OK;
+    };
+    auto predict_delta = [&](size_t k) -> int {  // frame k's prediction into the state, the state's value kept
+        auto &m = p->mq[k % D];
+        if (!m.saved.p) CK(m.saved.alloc(1));
+        if (!m.pin_delta.p) CK(m.pin_delta.alloc(1));
+        *m.pin_delta.p = pred[k];
+        CK(cudaMemcpyAsync(m.saved.p, &p->d_state.p->last_delta, sizeof(SE3), cudaMemcpyDeviceToDevice, ex.stream));
+        CK(cudaMemcpyAsync(&p->d_state.p->last_delta, m.pin_delta.p, sizeof(SE3), cudaMemcpyHostToDevice, ex.stream));
+        return KB_OK;
     };
     auto run = [&]() -> int {
     while (next_absorb < valid) {
@@ -1819,10 +1917,11 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
         bool submit = next_submit < valid && inflight + 1 < D;
         if (submit && inflight > 0 && !p->localizer && p->map->would_grow(pipeline_extra(p, n[next_submit]))) submit = false;  // drain first
         if (submit) {
-            const size_t k = next_submit, nk = n[k], ntk = use_ts[k] ? n_timestamps[k] : 0;
+            const size_t k = next_submit, nk = n[k], ntk = use_ts[k] && !has_motion[k] ? n_timestamps[k] : 0;
             auto &s = p->q[k % D];
             if (!p->localizer) RET(p->map->ensure_capacity(pipeline_extra(p, nk)));  // rebuilds only with nothing in flight
-            const bool prefetch = k + 1 < valid && !use_ts[k + 1] && n[k + 1] > 0;
+            // a frame without stamps, or with a kb_motion, does not depend on this one's result
+            const bool prefetch = k + 1 < valid && (!use_ts[k + 1] || has_motion[k + 1]) && n[k + 1] > 0;
             const double *d_xyz, *d_ts = nullptr, *d_next = nullptr;
             if (dev_in) {
                 d_xyz = static_cast<const double *>(xyz[k]);
@@ -1836,10 +1935,19 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
                 d_ts = s.ts.p;
                 if (prefetch) d_next = p->q[(k + 1) % D].in.p;
             }
+            // deskewed frames (this one and the one this launch prefetches) are deskewed before the launch that reads them
+            for (; next_deskew <= k + (prefetch ? 1 : 0); ++next_deskew)
+                if (desk[next_deskew]) RET(deskew(next_deskew));
+            if (desk[k]) {
+                d_xyz = p->mq[k % D].xyz.p;
+                d_ts = nullptr;
+            }
+            if (prefetch && desk[k + 1]) d_next = p->mq[(k + 1) % D].xyz.p;
+            if (predict[k]) RET(predict_delta(k));
             {
                 StallTrace t("queue: launch");
-                RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32, k % D, d_next,
-                                    prefetch ? n[k + 1] : 0));
+                RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32 && !desk[k], k % D,
+                                    d_next, prefetch ? n[k + 1] : 0, f32 && !(prefetch && desk[k + 1])));
                 CK(cudaEventRecord(s.done.p, ex.stream));
                 // result read-back on its own stream: neither the next kernel nor the next H2D waits for it (letting
                 // the kernel write to mapped host memory instead was slower)
@@ -1863,8 +1971,17 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
         Taken taken;
         RET(take(k, &taken));
         if (taken == TAKEN_VETOED) {  // replay from k
+            // the frames queued behind it were skipped, but their predictions were copied into the state: the first
+            // one's copy of the state before it is the state frame k left
+            for (size_t j = k + 1; j < next_submit; ++j)
+                if (predict[j]) {
+                    CK(cudaMemcpyAsync(&p->d_state.p->last_delta, p->mq[j % D].saved.p, sizeof(SE3),
+                                       cudaMemcpyDeviceToDevice, ex.stream));
+                    break;
+                }
             next_submit = k;
             next_upload = k;
+            next_deskew = k;
             if (++attempts >= 3) return fail(KB_ERR_CUDA, "voxel table could not be grown (internal capacity bug)");
             continue;
         }
@@ -1985,6 +2102,27 @@ int kb_pipeline_register_frames_degeneracy(kb_pipeline *p, const void *const *xy
     if (p && degeneracy_out && !p->degen.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoDegeneracy);
     return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out, constraints_out,
                            degeneracy_out);
+}
+int kb_pipeline_register_frames_motion(kb_pipeline *p, const void *const *xyz, const size_t *n,
+                                       const double *const *timestamps, const size_t *n_timestamps,
+                                       const kb_motion *motion, size_t count, int layout, double *poses_out,
+                                       kb_fit *fits_out, kb_constraints *constraints_out, kb_degeneracy *degeneracy_out) {
+    if (p && fits_out && !p->fit.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
+    if (p && constraints_out && !p->planes.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoConstraints);
+    if (p && degeneracy_out && !p->degen.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoDegeneracy);
+    return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out, constraints_out,
+                           degeneracy_out, motion);
+}
+int kb_pipeline_motion_time(const kb_pipeline *p, double *out) {
+    if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *out = p->motion_end;
+    return KB_OK;
+}
+int kb_pipeline_set_motion_time(kb_pipeline *p, double end_time) {
+    if (!p) return fail(KB_ERR_INVALID_ARG, "p == NULL");
+    if (std::isinf(end_time)) return fail(KB_ERR_INVALID_ARG, "motion end time %g is not finite", end_time);
+    p->motion_end = end_time;
+    return KB_OK;
 }
 int kb_pipeline_fit_reporting(const kb_pipeline *p, int *out) {
     if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");

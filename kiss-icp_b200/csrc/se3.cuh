@@ -239,6 +239,27 @@ KB_HD void se3_log(const SE3 &T, double out[6]) {
     out[5] = omega.z;
 }
 
+// A sampled trajectory (kb_motion, DESIGN.md section 4.17) is T(t) = T_k Exp(tau xi_k) on interval k, tau = t - t_k,
+// xi_k = Log(T_k^-1 T_k+1) / (t_k+1 - t_k). motion_interval: the k in [0, m - 2] of t among the m sample times
+// times[0], times[stride], ...; before the first and after the last sample the first and the last interval (they are
+// extrapolated), and 0 for a NaN t.
+KB_HD int motion_interval(const double *times, int stride, int m, double t) {
+    int lo = 0, hi = m - 1;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (times[mid * stride] <= t)
+            lo = mid;
+        else
+            hi = mid;
+    }
+    return lo;
+}
+KB_HD SE3 motion_at(const SE3 &Tk, const double xi[6], double tau) {
+    double a[6];
+    for (int i = 0; i < 6; ++i) a[i] = tau * xi[i];
+    return se3_mul(Tk, se3_exp(a));
+}
+
 // Eigen::AngleAxisd(Matrix3d).angle()
 KB_HD double angle_axis_angle(const M3 &R) {
     const Q4 q = q_from_matrix(R);

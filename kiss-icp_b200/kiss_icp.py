@@ -27,6 +27,10 @@ prediction along directions a scan does not constrain: before ICP, the plane inf
 are held, and every ICP step is projected off them (DESIGN.md section 4.16). ``last_degeneracy`` and
 ``register_frames(..., return_degeneracy=True)`` report it per scan (constraints.ScanDegeneracy). A scan that holds
 nothing registers bit for bit as without it. ``constraints.RECOMMENDED_DEGENERACY_RATIO`` is the ratio to start from.
+
+``register_frame(frame, timestamps, motion=Motion(...))`` and ``register_frames(..., motions=[...])`` take the LiDAR's
+trajectory sampled by an IMU or wheel odometry (motion.Motion, DESIGN.md section 4.17) in place of the constant-velocity
+model: the scan is deskewed along it, and predicted from it when the previous scan's Motion ends within its samples.
 """
 from __future__ import annotations
 
@@ -41,6 +45,7 @@ from . import _native as N
 from .config import KISSConfig, load_config
 from .constraints import Constraints, ScanDegeneracy, _constraints_of, _from_struct, _from_structs, _scan_degeneracy
 from .mapping import VoxelHashMap, check_value, get_voxel_hash_map
+from .motion import Motion
 from .places import PlaceDatabase, PlaceRelocalizationResult
 from .preprocess import Preprocessor, get_preprocessor
 from .registration import get_registration
@@ -146,6 +151,7 @@ class KissICP:
         # (a localizer always reports fits; plane constraints and the degeneracy pass run next to the fit)
         self._report_fit = self.localizer or bool(report_fit) or self._report_constraints or rho > 0.0
         self._h = None
+        self._seen_motion = False  # (state_dict() carries motion_end_time once a Motion was registered)
         if self.localizer:
             self._check_prior(prior_map)
         if self.fused:
@@ -289,6 +295,14 @@ class KissICP:
         N.check(N.lib().kb_pipeline_last_degeneracy(self._h, C.byref(d)))
         return _scan_degeneracy(d)
 
+    @property
+    def motion_end_time(self) -> float:
+        """the end_time of the last scan if it was registered with a Motion, else NaN: a scan whose Motion covers it
+        is predicted from it"""
+        v = N.dbl(0)
+        N.check(N.lib().kb_pipeline_motion_time(self._h, C.byref(v)))
+        return v.value
+
     def _sigma_next(self):
         s = N.dbl(0)
         N.check(N.lib().kb_pipeline_threshold(self._h, C.byref(s)))
@@ -339,9 +353,13 @@ class KissICP:
         return list(arr)
 
     # -- RegisterFrame ---------------------------------------------------------------------------
-    def register_frame(self, frame, timestamps, return_clouds: bool = True):
+    def register_frame(self, frame, timestamps, return_clouds: bool = True, motion: Motion | None = None):
         """-> (preprocessed frame, source) like the reference; ``return_clouds=False`` skips the
-        two device-to-host cloud copies (the pose is available as ``last_pose`` either way)."""
+        two device-to-host cloud copies (the pose is available as ``last_pose`` either way).
+        ``motion``: the scan's sampled trajectory (motion.Motion) in place of the constant-velocity model."""
+        if motion is not None:  # (a blocking frame is a queue of one)
+            self.register_frames([frame], [timestamps], motions=[motion])
+            return self._last_clouds() if return_clouds else (None, None)
         if not self.fused:
             return self._register_frame_modular(frame, timestamps)
         ts = np.ascontiguousarray(np.asarray(timestamps).ravel(), dtype=np.float64)
@@ -356,6 +374,9 @@ class KissICP:
             N.check(N.lib().kb_pipeline_register_frame(self._h, N.ptr(pts), len(pts), N.ptr(ts), len(ts)))
         if not return_clouds:
             return None, None
+        return self._last_clouds()
+
+    def _last_clouds(self):
         a, b = N.sz(0), N.sz(0)
         N.check(N.lib().kb_pipeline_last_cloud_sizes(self._h, C.byref(a), C.byref(b)))
         pre = np.empty((a.value, 3))
@@ -364,7 +385,7 @@ class KissICP:
         return pre, src
 
     def register_frames(self, frames, timestamps=None, return_fits: bool = False, return_constraints: bool = False,
-                        return_degeneracy: bool = False):
+                        return_degeneracy: bool = False, motions=None):
         """Register a whole sequence (the dataset loop of python/kiss_icp/pipeline.py:106-112) -> poses (K,4,4).
 
         Same results as K ``register_frame`` calls; the frames are queued on the device (copy of frame k+1
@@ -372,8 +393,16 @@ class KissICP:
         (N_k,3) arrays, all float64 or all float32; ``timestamps`` a matching sequence (or None).
         ``return_fits`` (localizers and report_fit=True only) -> (poses, fits): a Fit of arrays, one entry per frame.
         ``return_constraints`` (report_constraints=True only) appends a Constraints of arrays: (poses, [fits,] constraints).
-        ``return_degeneracy`` (degeneracy_ratio > 0 only) appends a ScanDegeneracy of arrays, one entry per frame."""
+        ``return_degeneracy`` (degeneracy_ratio > 0 only) appends a ScanDegeneracy of arrays, one entry per frame.
+        ``motions``: a matching sequence of motion.Motion or None (None: the constant-velocity model for that frame)."""
         K = len(frames)
+        if motions is not None:
+            if len(motions) != K:
+                raise ValueError("frames and motions differ in length")
+            if any(m is not None and not isinstance(m, Motion) for m in motions):
+                raise TypeError("motions holds Motion objects or None")
+            if not self.fused and any(m is not None for m in motions):
+                raise ValueError("a Motion needs the fused pipeline (fused=True, an adaptive threshold)")
         if return_fits:
             self._check_reports_fits()
         if return_constraints:
@@ -408,13 +437,18 @@ class KissICP:
         f32 = K > 0 and all(a.dtype == np.float32 and a.ndim == 2 and a.shape[1] == 3 for a in arrs)
         pts = [np.ascontiguousarray(a) for a in arrs] if f32 else [N.points_arg(a) for a in arrs]
         ts = [np.ascontiguousarray(np.asarray(t).ravel(), dtype=np.float64) for t in timestamps]
+        mstructs = None
+        if motions is not None and any(m is not None for m in motions):
+            mstructs = [m._struct(m.resolved_end_time(t)) if m is not None else None for m, t in zip(motions, ts)]
         return self._register_frames_raw([N.ptr(a) for a in pts], [len(a) for a in pts], [N.ptr(t) for t in ts],
                                          [len(t) for t in ts], 1 if f32 else 0, return_fits=return_fits,
-                                         return_constraints=return_constraints, return_degeneracy=return_degeneracy)
+                                         return_constraints=return_constraints, return_degeneracy=return_degeneracy,
+                                         motions=mstructs)
 
     def _register_frames_raw(self, xyz_ptrs, sizes, ts_ptrs, ts_sizes, layout, return_fits: bool = False,
-                             return_constraints: bool = False, return_degeneracy: bool = False):
-        """raw-pointer form (host or device addresses): layout 0 host f64, 1 host f32, 2 device f64"""
+                             return_constraints: bool = False, return_degeneracy: bool = False, motions=None):
+        """raw-pointer form (host or device addresses): layout 0 host f64, 1 host f32, 2 device f64; motions: None or
+        one _native.Motion (None: no motion) per frame, with its end_time resolved"""
         K = len(xyz_ptrs)
         as_vp = lambda v: v if isinstance(v, C.c_void_p) else C.c_void_p(int(v) if v else None)
         X = (C.c_void_p * K)(*[as_vp(v) for v in xyz_ptrs])
@@ -424,8 +458,13 @@ class KissICP:
         poses = np.empty((K, 4, 4))
         fits = (N.Fit * K)() if return_fits else None
         cons = (N.Constraints * K)() if return_constraints else None
-        if return_degeneracy:
-            degs = (N.Degeneracy * K)()
+        degs = (N.Degeneracy * K)() if return_degeneracy else None
+        if motions is not None:
+            M = (N.Motion * K)(*[m if m is not None else N.Motion() for m in motions])
+            self._seen_motion = True
+            N.check(N.lib().kb_pipeline_register_frames_motion(self._h, X, n, T, nt, M, K, int(layout), N.ptr(poses),
+                                                               fits, cons, degs))
+        elif return_degeneracy:
             N.check(N.lib().kb_pipeline_register_frames_degeneracy(self._h, X, n, T, nt, K, int(layout), N.ptr(poses),
                                                                    fits, cons, degs))
         else:
@@ -563,6 +602,8 @@ class KissICP:
                 sse, ns = self.adaptive_threshold.get_state()
         d.update(pose_qt=pose_qt, delta_qt=delta_qt, pose=pose, delta=delta, model_sse=np.array(float(sse)),
                  num_samples=np.array(int(ns)))
+        if self._seen_motion:  # the end_time of the last scan if it had a Motion (NaN: none), for its successor's prediction
+            d["motion_end_time"] = np.array(self.motion_end_time)
         if not self.localizer:  # (a localizer's prior map is not part of its state)
             vox, cnt, pts = self.local_map.dump()
             d.update(voxels=vox, counts=cnt, points=pts)
@@ -599,6 +640,9 @@ class KissICP:
             new.pose[:] = [float(x) for x in _params_arg(d["pose_qt"])]
             new.delta[:] = [float(x) for x in _params_arg(d["delta_qt"])]
             new.model_sse, new.num_samples = sse, ns
+            mt = float(d["motion_end_time"]) if "motion_end_time" in d else math.nan
+            if math.isinf(mt):
+                raise ValueError("motion_end_time is not finite")
             N.check(N.lib().kb_pipeline_get_state(self._h, C.byref(old)))
             check_value(N.lib().kb_pipeline_set_state(self._h, C.byref(new)))
             try:
@@ -606,6 +650,8 @@ class KissICP:
             except Exception:
                 N.check(N.lib().kb_pipeline_set_state(self._h, C.byref(old)))
                 raise
+            N.check(N.lib().kb_pipeline_set_motion_time(self._h, mt))
+            self._seen_motion = self._seen_motion or "motion_end_time" in d
             return
         pose, delta = _pose_arg(d["pose"]), _pose_arg(d["delta"])
         if isinstance(self.adaptive_threshold, AdaptiveThreshold):

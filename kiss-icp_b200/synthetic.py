@@ -7,6 +7,9 @@ box city. Conventions reused from the reference's loaders (for shape only, no co
     (python/kiss_icp/datasets/kitti.py:57,66)  -> ``stamps='none'``, coords rounded to fp32
   * MulRan/Ouster style per-column stamps floor(i/H)/W (python/kiss_icp/datasets/mulran.py:54-58)
     -> ``stamps='column'`` (points are then motion-distorted so that deskew matters)
+  * ``stamps='sweep'``: column c captured at the TRUE pose(k - 1 + (c+1)/cols) rather than the constant-velocity
+    interpolation of 'column', stamped (c+1)/(cols hz) seconds after the scan's start ``scan_start_time(k)``; with
+    ``shake`` and ``motion_samples`` this is the stream for deskewing and predicting from IMU / odometry samples
 
 The ray caster is written with torch ops so the same code runs on the CPU (small test scans)
 and on the GPU (bench-size streams).
@@ -40,15 +43,18 @@ class SyntheticLidar:
 
     def __init__(self, seed=0, beams=64, cols=1024, elev_deg=(-24.8, 2.0), max_ray=120.0, noise=0.02,
                  stamps="none", speed=10.0, hz=10.0, loop_radius=150.0, sensor_height=1.73, n_boxes=260,
-                 device="cpu", movers=None):
+                 device="cpu", movers=None, shake=None):
         """movers: moving boxes (none by default). Each is (size, s0, lateral, speed) or (size, s0, lateral, speed,
         "cross"), with size = (sx, sy, sz) [m] of an axis-aligned box standing on the ground, and t = scan index / hz:
         along the road its centre is at arclength s0 + speed t of the loop, `lateral` metres to the left of it (a
         negative speed drives the other way); a crossing box stays at arclength s0 and moves across the road, its
-        centre at lateral + speed t."""
+        centre at lateral + speed t.
+        shake: (amplitude [rad], frequency [Hz]): a yaw oscillation A sin(2 pi f t), t = k / hz, added to pose() (a
+        handheld rig or a legged robot turning fast within a sweep); None: none."""
         self.seed, self.beams, self.cols = int(seed), int(beams), int(cols)
         self.hz = float(hz)
         self.movers = [tuple(m) for m in movers] if movers else []
+        self.shake = None if shake is None else (float(shake[0]), float(shake[1]))
         self.max_ray, self.noise, self.stamps = float(max_ray), float(noise), stamps
         self.device = torch.device(device)
         self.sensor_height = sensor_height
@@ -123,12 +129,39 @@ class SyntheticLidar:
         p = self._xy(s)
         t = (self._xy(s + e) - self._xy(s - e)) / (2 * e)
         yaw = math.atan2(t[1], t[0])
+        if self.shake is not None:
+            yaw += self.shake[0] * math.sin(2 * math.pi * self.shake[1] * k / self.hz)
         roll = math.radians(0.8) * math.sin(0.05 * s + self.phase)
         pitch = math.radians(0.6) * math.sin(0.08 * s + 1.0)
         T = np.eye(4)
         T[:3, :3] = _rpy(roll, pitch, yaw)
         T[:3, 3] = [p[0], p[1], self.sensor_height + 0.03 * math.sin(0.11 * s)]
         return T
+
+    def scan_start_time(self, k: int) -> float:
+        """the time [s] at which scan k's sweep starts (scan index k is at time k / hz, where its sweep ends)"""
+        return (k - 1) / self.hz
+
+    def motion_samples(self, k: int, rate_hz: float, eps: float = 1e-5):
+        """Ground truth sampled over scan k's sweep, at rate_hz from scan_start_time(k) to k / hz (both included):
+        (times (m,), poses (m, 4, 4) world <- sensor, body angular rates (m, 3) [rad/s] and body velocities (m, 3)
+        [m/s], both in the sensor frame at each time, by central differences of pose())."""
+        t0, t1 = self.scan_start_time(k), k / self.hz
+        m = int(round((t1 - t0) * rate_hz)) + 1
+        times = np.linspace(t0, t1, m)
+        poses = np.array([self.pose(t * self.hz) for t in times])
+        rates = np.empty((m, 3))
+        vel = np.empty((m, 3))
+        for i, t in enumerate(times):
+            A, B = self.pose((t - eps) * self.hz), self.pose((t + eps) * self.hz)
+            R = poses[i, :3, :3]
+            D = A[:3, :3].T @ B[:3, :3]
+            ang = math.acos(max(-1.0, min(1.0, (np.trace(D) - 1) / 2)))
+            w = np.array([D[2, 1] - D[1, 2], D[0, 2] - D[2, 0], D[1, 0] - D[0, 1]])
+            w = w * (0.5 if ang < 1e-12 else ang / (2 * math.sin(ang)))
+            rates[i] = w / (2 * eps)
+            vel[i] = R.T @ (B[:3, 3] - A[:3, 3]) / (2 * eps)
+        return times, poses, rates, vel
 
     # -- ray casting -------------------------------------------------------------------
     def mover_boxes(self, k: float):
@@ -187,7 +220,14 @@ class SyntheticLidar:
         g = torch.Generator(device="cpu")
         g.manual_seed(self.seed * 1_000_003 + int(k))
         n = self.dirs.shape[0]
-        if self.stamps == "column":
+        if self.stamps == "sweep":
+            # column c is captured at the true pose(k - 1 + (c+1)/cols)
+            Tc = [self.pose(k - 1 + (c + 1) / self.cols) for c in range(self.cols)]
+            Rt = torch.tensor(np.array([T[:3, :3] for T in Tc]), dtype=torch.float64, device=self.device)[self.col_of_point]
+            origins = torch.tensor(np.array([T[:3, 3] for T in Tc]), dtype=torch.float64,
+                                   device=self.device)[self.col_of_point]
+            dirs_w = torch.einsum("nij,nj->ni", Rt, self.dirs)
+        elif self.stamps == "column":
             # motion distortion: column c is captured at T(k-1+ (c+1)/cols)
             frac = (np.arange(self.cols) + 1) / self.cols
             Rs = np.empty((self.cols, 3, 3))
@@ -221,6 +261,9 @@ class SyntheticLidar:
         if self.stamps == "column":
             col = torch.tensor(self.col_of_point, device=self.device)[valid]
             ts = col.to(torch.float64) / self.cols
+        elif self.stamps == "sweep":
+            col = torch.tensor(self.col_of_point, device=self.device)[valid]
+            ts = (col.to(torch.float64) + 1.0) / (self.cols * self.hz)
         else:
             ts = torch.empty(0, dtype=torch.float64, device=self.device)
         if mover_mask:
