@@ -339,3 +339,43 @@ class Tunnel:
         rng = np.random.default_rng((self.seed, int(k)))
         pts = t[ok, None] * D[ok] + rng.normal(0.0, self.noise, (int(ok.sum()), 3))
         return pts, np.empty(0)
+
+
+class Shaft:
+    """A vertical shaft: the circular cylinder x^2 + y^2 = ``radius``^2 around the z axis and, with ``caps``, a floor at
+    z = ``floor`` and a ceiling at z = ``ceiling`` (a silo), no other structure. The ring LiDAR of Tunnel (``beams`` x
+    ``cols``, ``elev_deg``) starts at the origin on the axis and per scan moves ``step`` metres along +z and turns ``spin``
+    radians about z. Nothing constrains the rotation about the axis; without caps nothing constrains the translation along
+    it either. ``scan(k)`` -> (points in the sensor frame, no stamps), ``pose(k)`` -> the true 4x4 pose of scan k."""
+
+    def __init__(self, seed=0, beams=32, cols=512, elev_deg=(-60.0, 60.0), radius=5.0, caps=False, floor=-3.0,
+                 ceiling=4.0, step=0.05, spin=0.02, max_ray=100.0, noise=0.01):
+        self.seed, self.radius, self.caps, self.floor, self.ceiling = seed, radius, bool(caps), floor, ceiling
+        self.step, self.spin, self.max_ray, self.noise = step, spin, max_ray, noise
+        el = np.radians(np.linspace(elev_deg[0], elev_deg[1], beams))
+        az = np.radians(np.arange(cols) * (360.0 / cols))
+        E, A = np.meshgrid(el, az, indexing="ij")
+        self.dirs = np.stack([np.cos(E) * np.cos(A), np.cos(E) * np.sin(A), np.sin(E)], -1).reshape(-1, 3)
+
+    def pose(self, k: float) -> np.ndarray:
+        T = np.eye(4)
+        c, s = math.cos(self.spin * k), math.sin(self.spin * k)
+        T[:2, :2] = [[c, -s], [s, c]]
+        T[2, 3] = self.step * k
+        return T
+
+    def scan(self, k: int):
+        # (the scene is symmetric about the axis the sensor turns about: a ray's range depends on its sensor-frame
+        # direction and the sensor's height only)
+        D = self.dirs
+        z0 = self.step * k
+        with np.errstate(divide="ignore", invalid="ignore"):
+            t = self.radius / np.hypot(D[:, 0], D[:, 1])
+            if self.caps:
+                for val in (self.floor, self.ceiling):
+                    tt = (val - z0) / D[:, 2]
+                    t = np.where((tt > 0) & (tt < t), tt, t)
+        ok = np.isfinite(t) & (t < self.max_ray)
+        rng = np.random.default_rng((self.seed, int(k)))
+        pts = t[ok, None] * D[ok] + rng.normal(0.0, self.noise, (int(ok.sum()), 3))
+        return pts, np.empty(0)

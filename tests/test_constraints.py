@@ -8,8 +8,9 @@ import pytest
 
 
 # ---------------------------------------------------------------------------------------------- numpy restatement
-def _numpy_constraints(vmap, voxel_size, src, pose, max_dist):
-    """the definition, from closest_neighbors (bit-exact q) and the map's dump()"""
+def _numpy_constraints(vmap, voxel_size, src, pose, max_dist, centre=None):
+    """the definition, from closest_neighbors (bit-exact q) and the map's dump(); with a centre c, the lever about it:
+    J = [n, (p - c) x n], summed directly (A^T H A from the sum about the origin cancels digits far from it)"""
     p = src @ pose[:3, :3].T + pose[:3, 3]
     q, d = vmap.closest_neighbors(p)
     vox, cnt, pts = vmap.dump()
@@ -28,7 +29,7 @@ def _numpy_constraints(vmap, voxel_size, src, pose, max_dist):
         a = (lam[1] - lam[0]) / lam[2] if lam[2] > 0 else 0.0
         n = V[:, 0]
         e = n @ (p[i] - q[i])
-        J = np.concatenate([n, np.cross(p[i], n)])
+        J = np.concatenate([n, np.cross(p[i] if centre is None else p[i] - centre, n)])
         W += a
         S += a * e * e
         H += a * np.outer(J, J)
