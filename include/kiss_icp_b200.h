@@ -451,6 +451,55 @@ int kb_pipeline_set_motion_time(kb_pipeline *p, double end_time);
 int kb_deskew_motion(const double *xyz, size_t n, const double *timestamps, size_t n_timestamps, const kb_motion *motion,
                      double *out);
 
+/* ---- multi-LiDAR rigs: per-sensor extrinsics, range crops and clocks, merged on the device ------------------------
+ * No reference counterpart (DESIGN.md section 4.18). A rig is 1 <= S <= KB_RIG_MAX_SENSORS sensors mounted on a base
+ * (the vehicle). Sensor i has an extrinsic E_i (base <- sensor), a range crop (min_range_i, max_range_i) and, per frame,
+ * a stamp_offset_i that puts its point stamps on the common clock. A rig frame is S point arrays (and S stamp arrays:
+ * either every sensor with points has stamps or none has; a mix is KB_ERR_INVALID_ARG, a sensor without points may
+ * have none either way). Its merged frame is:
+ *   order   the sensors' points concatenated in sensor order, each sensor's in its own order (the downsample keeps the
+ *           first point per voxel);
+ *   crop    point p of sensor i is kept iff min_range_i < |p| < max_range_i in the sensor frame; a point that is not
+ *           becomes NaN (the frame's own crop drops it), its stamp is kept. A sensor with min_range 0 and max_range
+ *           +inf has no crop: its points pass as they are;
+ *   to base q = E_i p (an identity E_i passes the point without arithmetic);
+ *   stamps  s + stamp_offset_i.
+ * Then, with deskewing on and stamps given: without a kb_motion the merged frame and merged stamps are registered as a
+ * stamped frame (constant velocity: stamps normalised over the union's [min, max], deskewed to its end by last_delta,
+ * exactly KISS-ICP on the concatenated base-frame cloud); with a kb_motion (the BASE's poses) a point becomes
+ * T(end_time)^-1 T(s + stamp_offset_i + motion.stamp_offset) E_i p and the frame is registered without stamps. The
+ * frame's own crop (cfg.min_range / max_range, about the base origin) applies afterwards. Poses, last_delta, the map,
+ * fits, constraints and degeneracy refer to the base; the preprocessed cloud of kb_pipeline_last_clouds is the merged
+ * base-frame cloud. */
+#define KB_RIG_MAX_SENSORS 16
+typedef struct kb_sensor {
+    double extrinsic[16];        /* row-major SE(3), base <- sensor                             */
+    double min_range, max_range; /* 0 <= min_range < max_range (+inf allowed), in the sensor frame */
+} kb_sensor;
+/* Host only (works without a device). KB_ERR_INVALID_ARG for NULL sensors, n_sensors outside [1, KB_RIG_MAX_SENSORS],
+ * a NaN, negative or infinite min_range, a NaN max_range or min_range >= max_range; KB_ERR_NOT_SE3 for an extrinsic
+ * outside SE(3). */
+int kb_rig_check(const kb_sensor *sensors, size_t n_sensors);
+/* kb_pipeline_register_frames_motion for rig frames: frame k is xyz[k S + i], n[k S + i] (i < S) in the layout, stamps
+ * timestamps / n_timestamps likewise (both may be NULL: no stamps at all), stamp_offsets[k S + i] (NULL: all 0, each
+ * finite), motion as kb_pipeline_register_frames_motion (NULL or [count], m == 0: none). The merged frame must hold
+ * fewer than 2^30 points. The rig and every motion are checked before any device work (on error nothing is
+ * registered); an invalid frame stops the sequence after the frames before it were registered. Rig frames with stamps
+ * and without a kb_motion depend on the previous frame's result and are not prefetched; the others are. Outputs as
+ * kb_pipeline_register_frames_degeneracy. */
+int kb_pipeline_register_rig_frames(kb_pipeline *p, const kb_sensor *sensors, size_t n_sensors, const void *const *xyz,
+                                    const size_t *n, const double *const *timestamps, const size_t *n_timestamps,
+                                    const double *stamp_offsets, const kb_motion *motion, size_t count, int layout,
+                                    double *poses_out, kb_fit *fits_out, kb_constraints *constraints_out,
+                                    kb_degeneracy *degeneracy_out);
+/* The merge of one rig frame alone (host float64 arrays, synchronous): xyz_out[N][3] (N the sum of n) receives the
+ * merged base-frame points, deskewed along the motion when motion is not NULL and the frame has stamps, no frame
+ * crop; timestamps_out[N] (may be NULL) the merged stamps s + stamp_offset_i, when the frame has stamps. Checks of
+ * kb_rig_check, kb_motion_check and of the stamps as kb_pipeline_register_rig_frames. */
+int kb_merge_rig(const kb_sensor *sensors, size_t n_sensors, const double *const *xyz, const size_t *n,
+                 const double *const *timestamps, const size_t *n_timestamps, const double *stamp_offsets,
+                 const kb_motion *motion, double *xyz_out, double *timestamps_out);
+
 /* ---- relocalization: a global pose search in a bounded region ----------------------------
  * No reference counterpart. Finds a scan's pose in a map without an initial pose: every hypothesis of a grid in x, y
  * and yaw around a centre is scored on the device, the best peaks are refined with kb_registration_align_batch, and

@@ -18,5 +18,6 @@ from .voxelization import voxel_down_sample  # noqa: F401
 from .preprocess import correct_kitti_scan  # noqa: F401
 from .metrics import absolute_trajectory_error, sequence_error  # noqa: F401
 from .motion import Motion, deskew, motion_from_gyro  # noqa: F401
+from .rig import Rig, Sensor, merge_rig  # noqa: F401
 
 __version__ = "0.1.0"

@@ -109,6 +109,11 @@ class Motion(C.Structure):
     _fields_ = [("times", vp), ("poses", vp), ("m", sz), ("stamp_offset", dbl), ("end_time", dbl)]
 
 
+class Sensor(C.Structure):
+    """kb_sensor: one LiDAR of a rig, its extrinsic (base <- sensor) and its range crop"""
+    _fields_ = [("extrinsic", dbl * 16), ("min_range", dbl), ("max_range", dbl)]
+
+
 class RelocSearch(C.Structure):
     """kb_reloc_search: the hypothesis grid of kb_relocalize"""
     _fields_ = [("center", dbl * 16), ("half_cells_x", i32), ("half_cells_y", i32), ("step", dbl), ("n_yaw", i32),
@@ -283,6 +288,9 @@ SIGNATURES = {
     "kb_pipeline_motion_time": (i32, [vp, C.POINTER(dbl)]),
     "kb_pipeline_set_motion_time": (i32, [vp, dbl]),
     "kb_deskew_motion": (i32, [vp, sz, vp, sz, C.POINTER(Motion), vp]),
+    "kb_rig_check": (i32, [vp, sz]),
+    "kb_pipeline_register_rig_frames": (i32, [vp, vp, sz, vp, vp, vp, vp, vp, vp, sz, i32, vp, vp, vp, vp]),
+    "kb_merge_rig": (i32, [vp, sz, vp, vp, vp, vp, vp, vp, vp, vp]),
     "kb_place_params_default": (None, [C.POINTER(PlaceParams)]),
     "kb_place_db_create": (i32, [C.POINTER(PlaceParams), C.POINTER(vp)]),
     "kb_place_db_destroy": (i32, [vp]),

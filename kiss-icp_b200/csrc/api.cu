@@ -26,6 +26,7 @@
 #include "motion.cuh"
 #include "probe.cuh"
 #include "relocalize.cuh"
+#include "rig.cuh"
 
 using namespace kb;
 using namespace kb_host;
@@ -435,6 +436,14 @@ struct kb_pipeline {
         DBuf<SE3> saved;
     };
     MotionSlot mq[Q_DEPTH];
+    // rigs (kb_pipeline_register_rig_frames): per queue slot the frame's sensor table (pinned staging and device copy)
+    // and its merged points and stamps
+    struct RigSlot {
+        PinBuf<RigSensor> pin_tab;
+        DBuf<RigSensor> tab;
+        DBuf<double> xyz, ts;
+    };
+    RigSlot rq[Q_DEPTH];
     Stream copy_stream, res_stream;
     PinBuf<FrameResult> q_res;    // [Q_DEPTH] host copies of the frame results
     DBuf<FrameResult> q_res_dev;  // [Q_DEPTH] device side: where the kernels write them
@@ -1488,6 +1497,60 @@ int kb_deskew_motion(const double *xyz, size_t n, const double *timestamps, size
     return ex.sync();  // (d_tab is released after the kernel has read it)
 }
 
+int kb_merge_rig(const kb_sensor *sensors, size_t n_sensors, const double *const *xyz, const size_t *n,
+                 const double *const *timestamps, const size_t *n_timestamps, const double *stamp_offsets,
+                 const kb_motion *motion, double *xyz_out, double *timestamps_out) {
+    RET(rig_check(sensors, n_sensors));
+    if (!xyz || !n) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (motion) RET(motion_check(motion));
+    size_t total = 0;
+    bool stamped = false;
+    RET(rig_frame_check(n_sensors, reinterpret_cast<const void *const *>(xyz), n, timestamps, n_timestamps,
+                        stamp_offsets, true, &total, &stamped));
+    if (total && !xyz_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    DefaultCtx *c;
+    RET(default_ctx(&c));
+    if (!total) return KB_OK;
+    Exec &ex = *c->ex;
+    CK(cudaSetDevice(ex.device));
+    std::vector<RigSensor> tab = rig_table(sensors, n_sensors);
+    RET(c->ws.in.ensure(3 * total));
+    RET(c->ws.tmp.ensure(3 * total));
+    RET(c->ws.ts.ensure(total));
+    DBuf<double> d_ts_out;
+    if (stamped) CK(d_ts_out.alloc(total));
+    size_t begin = 0;
+    for (size_t i = 0; i < n_sensors; ++i) {
+        tab[i].stamp_offset = stamp_offsets ? stamp_offsets[i] : 0.0;
+        tab[i].begin = static_cast<long long>(begin);
+        tab[i].xyz = c->ws.in.p + 3 * begin;
+        tab[i].ts = stamped ? c->ws.ts.p + begin : nullptr;
+        if (n[i]) {
+            CK(cudaMemcpyAsync(c->ws.in.p + 3 * begin, xyz[i], n[i] * 24, cudaMemcpyHostToDevice, ex.stream));
+            if (stamped) CK(cudaMemcpyAsync(c->ws.ts.p + begin, timestamps[i], n[i] * 8, cudaMemcpyHostToDevice, ex.stream));
+        }
+        begin += n[i];
+    }
+    DBuf<RigSensor> d_tab;
+    CK(d_tab.alloc(n_sensors));
+    CK(cudaMemcpyAsync(d_tab.p, tab.data(), n_sensors * sizeof(RigSensor), cudaMemcpyHostToDevice, ex.stream));
+    const bool desk = motion && stamped;
+    std::vector<MotionSeg> mtab;
+    DBuf<MotionSeg> d_mtab;
+    if (desk) {
+        mtab = motion_table(*motion);
+        CK(d_mtab.alloc(mtab.size()));
+        CK(cudaMemcpyAsync(d_mtab.p, mtab.data(), mtab.size() * sizeof(MotionSeg), cudaMemcpyHostToDevice, ex.stream));
+    }
+    CK(rig_merge(ex.stream, ex.sms, d_tab.p, static_cast<int>(n_sensors), d_mtab.p, static_cast<int>(mtab.size()),
+                 desk ? motion->stamp_offset : 0.0, false, total, c->ws.tmp.p, stamped ? d_ts_out.p : nullptr));
+    ++ex.launches;
+    CK(cudaMemcpyAsync(xyz_out, c->ws.tmp.p, total * 24, cudaMemcpyDeviceToHost, ex.stream));
+    if (stamped && timestamps_out)
+        CK(cudaMemcpyAsync(timestamps_out, d_ts_out.p, total * 8, cudaMemcpyDeviceToHost, ex.stream));
+    return ex.sync();  // (the device tables are released after the kernel has read them)
+}
+
 // ------------------------------------------------------------------------------- KissICP pipeline
 void kb_config_default(kb_config *cfg) {
     if (!cfg) return;
@@ -1798,6 +1861,40 @@ static int queue_upload(kb_pipeline *p, void *dst, const void *src, size_t bytes
     return KB_OK;
 }
 
+// host -> device on the copy stream of `count` arrays back to back into dst, elem bytes per entry: pageable arrays
+// through the slot's pinned staging buffer at the same offsets, pinned ones copied directly
+static int queue_upload_parts(kb_pipeline *p, void *dst, const void *const *src, const size_t *cnt, size_t count,
+                              size_t elem, PinBuf<unsigned char> &pin) {
+    size_t staged = 0;  // bytes of the pageable parts, up to the last one (the staging buffer holds them at their offsets)
+    std::vector<char> pinned(count, 0);
+    for (size_t i = 0, off = 0; i < count; off += cnt[i] * elem, ++i)
+        if (cnt[i]) {
+            pinned[i] = is_pinned(src[i]);
+            if (!pinned[i]) staged = off + cnt[i] * elem;
+        }
+    if (staged) RET(pin.ensure(staged));
+    size_t off = 0;
+    for (size_t i = 0; i < count; ++i) {
+        const size_t bytes = cnt[i] * elem;
+        if (!bytes) continue;
+        const void *from = src[i];
+        if (!pinned[i]) {
+            std::memcpy(pin.p + off, src[i], bytes);
+            from = pin.p + off;
+        }
+        CK(cudaMemcpyAsync(static_cast<char *>(dst) + off, from, bytes, cudaMemcpyHostToDevice, p->copy_stream.p));
+        off += bytes;
+    }
+    return KB_OK;
+}
+
+// the rig of a kb_pipeline_register_rig_frames call: frame k is the arrays [k S, k S + S) of its sensors
+struct RigFrames {
+    size_t S;
+    const double *stamp_offsets;  // [count S] or null (all 0)
+    std::vector<RigSensor> tab;   // rig_table of the checked sensors
+};
+
 static const char *const kNoFits =
     "fits are computed by localizers (kb_pipeline_create_localizer) and by odometry pipelines with fit reporting on "
     "(kb_pipeline_set_fit_reporting)";
@@ -1808,12 +1905,13 @@ static const char *const kNoConstraints =
 // kb_pipeline_register_frames[_fit|_constraints|_degeneracy] and, with count = 1, kb_pipeline_register_frame[_f32|_dev];
 // fits_out (pipelines that report fits only, may be NULL) receives one fit per frame, constraints_out (pipelines that
 // report plane constraints only, may be NULL) one kb_constraints per frame, degen_out (pipelines with a degeneracy
-// ratio only, may be NULL) one kb_degeneracy per frame; motion (may be NULL) one kb_motion per frame (m == 0: none)
-static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n, const double *const *timestamps,
+// ratio only, may be NULL) one kb_degeneracy per frame; motion (may be NULL) one kb_motion per frame (m == 0: none);
+// rig (may be NULL): xyz, n_in, timestamps and n_timestamps hold rig->S arrays per frame, merged by k_merge_rig
+static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t *n_in, const double *const *timestamps,
                            const size_t *n_timestamps, size_t count, int layout, double *poses_out, kb_fit *fits_out,
                            kb_constraints *constraints_out, kb_degeneracy *degen_out = nullptr,
-                           const kb_motion *motion = nullptr) {
-    if (!p || (count && (!xyz || !n))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+                           const kb_motion *motion = nullptr, const RigFrames *rig = nullptr) {
+    if (!p || (count && (!xyz || !n_in))) return fail(KB_ERR_INVALID_ARG, "NULL argument");
     if (layout != KB_FRAMES_HOST_F64 && layout != KB_FRAMES_HOST_F32 && layout != KB_FRAMES_DEVICE_F64)
         return fail(KB_ERR_INVALID_ARG, "unknown frame layout %d", layout);
     std::vector<char> has_motion(count, 0);
@@ -1834,18 +1932,35 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
     int bad_status = KB_OK;
     std::string bad_msg;
     std::vector<char> use_ts(count, 0);
+    std::vector<size_t> n_rig(rig ? count : 0), nts(count, 0);  // (a rig frame's merged point and stamp counts)
     for (; valid < count; ++valid) {
         bool u = false;
-        const size_t nt = (timestamps && n_timestamps) ? n_timestamps[valid] : 0;
-        bad_status = pipeline_check(p, xyz[valid], n[valid], (timestamps && nt) ? timestamps[valid] : nullptr, nt, &u);
+        size_t nk, nt;
+        if (rig) {
+            const size_t o = valid * rig->S;
+            bool stamped = false;
+            bad_status = rig_frame_check(rig->S, xyz + o, n_in + o, timestamps ? timestamps + o : nullptr,
+                                         n_timestamps ? n_timestamps + o : nullptr,
+                                         rig->stamp_offsets ? rig->stamp_offsets + o : nullptr, p->cfg.deskew != 0, &nk,
+                                         &stamped);
+            u = p->cfg.deskew && stamped;
+            nt = nk;
+            if (bad_status == KB_OK) n_rig[valid] = nk;
+        } else {
+            nk = n_in[valid];
+            nt = (timestamps && n_timestamps) ? n_timestamps[valid] : 0;
+            bad_status = pipeline_check(p, xyz[valid], nk, (timestamps && nt) ? timestamps[valid] : nullptr, nt, &u);
+        }
         if (bad_status != KB_OK) {
             bad_msg = tl_err;
             break;
         }
         use_ts[valid] = u;
+        nts[valid] = nt;
         any_ts |= u;
-        max_n = std::max(max_n, std::max(n[valid], u ? nt : size_t(0)));
+        max_n = std::max(max_n, std::max(nk, u ? nt : size_t(0)));
     }
+    const size_t *n = rig ? n_rig.data() : n_in;  // points per frame (merged for a rig)
     RET(ex.sync());
     RET(p->ws.ensure(max_n));
     RET(p->ws.ensure_pipeline(max_n));
@@ -1875,8 +1990,16 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
     auto upload = [&](size_t u) -> int {  // host layouts: frame u -> slot u % D on the copy stream
         auto &s = p->q[u % D];
         StallTrace t("queue: H2D enqueue");
-        RET(queue_upload(p, s.in.p, xyz[u], n[u] * (f32 ? 12 : 24), s.pin_xyz));
-        if (use_ts[u]) RET(queue_upload(p, s.ts.p, timestamps[u], n_timestamps[u] * 8, s.pin_ts));
+        if (rig) {  // the sensors' arrays back to back (a sensor's first n stamps)
+            const size_t o = u * rig->S;
+            RET(queue_upload_parts(p, s.in.p, xyz + o, n_in + o, rig->S, f32 ? 12 : 24, s.pin_xyz));
+            if (use_ts[u])
+                RET(queue_upload_parts(p, s.ts.p, reinterpret_cast<const void *const *>(timestamps + o), n_in + o,
+                                       rig->S, 8, s.pin_ts));
+        } else {
+            RET(queue_upload(p, s.in.p, xyz[u], n[u] * (f32 ? 12 : 24), s.pin_xyz));
+            if (use_ts[u]) RET(queue_upload(p, s.ts.p, timestamps[u], n_timestamps[u] * 8, s.pin_ts));
+        }
         CK(cudaEventRecord(s.copied.p, p->copy_stream.p));
         return KB_OK;
     };
@@ -1887,19 +2010,58 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
         if (*taken == TAKEN_ABSORBED) p->motion_end = has_motion[k] ? motion[k].end_time : NAN;
         return KB_OK;
     };
-    auto deskew = [&](size_t j) -> int {  // frame j (on the device) -> its slot's deskewed points, on the frame stream
+    auto motion_tab = [&](size_t j) -> int {  // frame j's interval table -> its slot's device copy, on the frame stream
         auto &m = p->mq[j % D];
         const std::vector<MotionSeg> &tab = tabs[j];
         RET(m.pin_tab.ensure(tab.size()));
         RET(m.tab.ensure(tab.size()));
-        RET(m.xyz.ensure(3 * std::max<size_t>(n[j], 1)));
         std::memcpy(m.pin_tab.p, tab.data(), tab.size() * sizeof(MotionSeg));  // (frame j - D, its last reader, has ended)
         CK(cudaMemcpyAsync(m.tab.p, m.pin_tab.p, tab.size() * sizeof(MotionSeg), cudaMemcpyHostToDevice, ex.stream));
+        return KB_OK;
+    };
+    auto deskew = [&](size_t j) -> int {  // frame j (on the device) -> its slot's deskewed points, on the frame stream
+        auto &m = p->mq[j % D];
+        const std::vector<MotionSeg> &tab = tabs[j];
+        RET(motion_tab(j));
+        RET(m.xyz.ensure(3 * std::max<size_t>(n[j], 1)));
         const void *in = dev_in ? xyz[j] : p->q[j % D].in.p;
         const double *ts = dev_in ? timestamps[j] : p->q[j % D].ts.p;
         CK(motion_deskew(ex.stream, ex.sms, m.tab.p, static_cast<int>(tab.size()), in, f32, ts, motion[j].stamp_offset,
                          n[j], m.xyz.p));
         if (n[j]) ++ex.launches;
+        return KB_OK;
+    };
+    // Rigs: every frame is merged by k_merge_rig into its slot's buffers (with its stamps where it registers with them,
+    // deskewed along its kb_motion where it has one to deskew with) and registers the merged points as float64.
+    auto merge = [&](size_t j) -> int {  // rig frame j (on the device) -> its slot's merged frame, on the frame stream
+        auto &r = p->rq[j % D];
+        const size_t S = rig->S, o = j * S, nj = n[j];
+        const bool with_ts = use_ts[j] && !has_motion[j];
+        RET(r.pin_tab.ensure(S));
+        RET(r.tab.ensure(S));
+        RET(r.xyz.ensure(3 * std::max<size_t>(nj, 1)));
+        if (with_ts) RET(r.ts.ensure(std::max<size_t>(nj, 1)));
+        size_t begin = 0;
+        for (size_t i = 0; i < S; ++i) {  // (frame j - D, the last reader of the staging table, has ended)
+            RigSensor &t = r.pin_tab.p[i];
+            t = rig->tab[i];
+            t.stamp_offset = rig->stamp_offsets ? rig->stamp_offsets[o + i] : 0.0;
+            t.begin = static_cast<long long>(begin);
+            if (dev_in) {
+                t.xyz = xyz[o + i];
+                t.ts = use_ts[j] ? timestamps[o + i] : nullptr;
+            } else {
+                t.xyz = reinterpret_cast<const char *>(p->q[j % D].in.p) + begin * (f32 ? 12 : 24);
+                t.ts = use_ts[j] ? p->q[j % D].ts.p + begin : nullptr;
+            }
+            begin += n_in[o + i];
+        }
+        CK(cudaMemcpyAsync(r.tab.p, r.pin_tab.p, S * sizeof(RigSensor), cudaMemcpyHostToDevice, ex.stream));
+        if (desk[j]) RET(motion_tab(j));
+        CK(rig_merge(ex.stream, ex.sms, r.tab.p, static_cast<int>(S), desk[j] ? p->mq[j % D].tab.p : nullptr,
+                     desk[j] ? static_cast<int>(tabs[j].size()) : 0, desk[j] ? motion[j].stamp_offset : 0.0, f32, nj,
+                     r.xyz.p, with_ts ? r.ts.p : nullptr));
+        if (nj) ++ex.launches;
         return KB_OK;
     };
     auto predict_delta = [&](size_t k) -> int {  // frame k's prediction into the state, the state's value kept
@@ -1917,17 +2079,17 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
         bool submit = next_submit < valid && inflight + 1 < D;
         if (submit && inflight > 0 && !p->localizer && p->map->would_grow(pipeline_extra(p, n[next_submit]))) submit = false;  // drain first
         if (submit) {
-            const size_t k = next_submit, nk = n[k], ntk = use_ts[k] && !has_motion[k] ? n_timestamps[k] : 0;
+            const size_t k = next_submit, nk = n[k], ntk = use_ts[k] && !has_motion[k] ? nts[k] : 0;
             auto &s = p->q[k % D];
             if (!p->localizer) RET(p->map->ensure_capacity(pipeline_extra(p, nk)));  // rebuilds only with nothing in flight
             // a frame without stamps, or with a kb_motion, does not depend on this one's result
             const bool prefetch = k + 1 < valid && (!use_ts[k + 1] || has_motion[k + 1]) && n[k + 1] > 0;
-            const double *d_xyz, *d_ts = nullptr, *d_next = nullptr;
-            if (dev_in) {
+            const double *d_xyz = nullptr, *d_ts = nullptr, *d_next = nullptr;
+            if (dev_in && !rig) {
                 d_xyz = static_cast<const double *>(xyz[k]);
                 if (ntk) d_ts = timestamps[k];
                 if (prefetch) d_next = static_cast<const double *>(xyz[k + 1]);
-            } else {
+            } else if (!dev_in) {
                 for (; next_upload <= k + (prefetch ? 1 : 0); ++next_upload) RET(upload(next_upload));
                 CK(cudaStreamWaitEvent(ex.stream, s.copied.p, 0));
                 if (prefetch) CK(cudaStreamWaitEvent(ex.stream, p->q[(k + 1) % D].copied.p, 0));
@@ -1937,17 +2099,25 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
             }
             // deskewed frames (this one and the one this launch prefetches) are deskewed before the launch that reads them
             for (; next_deskew <= k + (prefetch ? 1 : 0); ++next_deskew)
-                if (desk[next_deskew]) RET(deskew(next_deskew));
-            if (desk[k]) {
+                if (rig)
+                    RET(merge(next_deskew));
+                else if (desk[next_deskew])
+                    RET(deskew(next_deskew));
+            if (rig) {
+                d_xyz = p->rq[k % D].xyz.p;
+                d_ts = ntk ? p->rq[k % D].ts.p : nullptr;
+                if (prefetch) d_next = p->rq[(k + 1) % D].xyz.p;
+            } else if (desk[k]) {
                 d_xyz = p->mq[k % D].xyz.p;
                 d_ts = nullptr;
             }
-            if (prefetch && desk[k + 1]) d_next = p->mq[(k + 1) % D].xyz.p;
+            if (!rig && prefetch && desk[k + 1]) d_next = p->mq[(k + 1) % D].xyz.p;
+            const bool raw_f32 = f32 && !rig;  // (merged and deskewed frames are float64)
             if (predict[k]) RET(predict_delta(k));
             {
                 StallTrace t("queue: launch");
-                RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, f32 && !desk[k], k % D,
-                                    d_next, prefetch ? n[k + 1] : 0, f32 && !(prefetch && desk[k + 1])));
+                RET(pipeline_launch(p, id0 + static_cast<long long>(k), d_xyz, nk, d_ts, ntk, raw_f32 && !desk[k], k % D,
+                                    d_next, prefetch ? n[k + 1] : 0, raw_f32 && !(prefetch && desk[k + 1])));
                 CK(cudaEventRecord(s.done.p, ex.stream));
                 // result read-back on its own stream: neither the next kernel nor the next H2D waits for it (letting
                 // the kernel write to mapped host memory instead was slower)
@@ -2112,6 +2282,19 @@ int kb_pipeline_register_frames_motion(kb_pipeline *p, const void *const *xyz, c
     if (p && degeneracy_out && !p->degen.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoDegeneracy);
     return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out, constraints_out,
                            degeneracy_out, motion);
+}
+int kb_pipeline_register_rig_frames(kb_pipeline *p, const kb_sensor *sensors, size_t n_sensors, const void *const *xyz,
+                                    const size_t *n, const double *const *timestamps, const size_t *n_timestamps,
+                                    const double *stamp_offsets, const kb_motion *motion, size_t count, int layout,
+                                    double *poses_out, kb_fit *fits_out, kb_constraints *constraints_out,
+                                    kb_degeneracy *degeneracy_out) {
+    if (p && fits_out && !p->fit.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoFits);
+    if (p && constraints_out && !p->planes.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoConstraints);
+    if (p && degeneracy_out && !p->degen.on()) return fail(KB_ERR_INVALID_ARG, "%s", kNoDegeneracy);
+    RET(rig_check(sensors, n_sensors));
+    const RigFrames rig{n_sensors, stamp_offsets, rig_table(sensors, n_sensors)};
+    return register_frames(p, xyz, n, timestamps, n_timestamps, count, layout, poses_out, fits_out, constraints_out,
+                           degeneracy_out, motion, &rig);
 }
 int kb_pipeline_motion_time(const kb_pipeline *p, double *out) {
     if (!p || !out) return fail(KB_ERR_INVALID_ARG, "NULL argument");

@@ -31,6 +31,10 @@ nothing registers bit for bit as without it. ``constraints.RECOMMENDED_DEGENERAC
 ``register_frame(frame, timestamps, motion=Motion(...))`` and ``register_frames(..., motions=[...])`` take the LiDAR's
 trajectory sampled by an IMU or wheel odometry (motion.Motion, DESIGN.md section 4.17) in place of the constant-velocity
 model: the scan is deskewed along it, and predicted from it when the previous scan's Motion ends within its samples.
+
+``register_rig_frame(scans, rig, ...)`` and ``register_rig_frames(frames, rig, ...)`` register frames of a multi-LiDAR rig
+(rig.Rig, DESIGN.md section 4.18): each frame's per-sensor scans are cropped per sensor, mapped to the base and merged on
+the device; the pipeline then tracks the base.
 """
 from __future__ import annotations
 
@@ -50,6 +54,7 @@ from .places import PlaceDatabase, PlaceRelocalizationResult
 from .preprocess import Preprocessor, get_preprocessor
 from .registration import get_registration
 from .relocalization import RelocalizationResult, RelocalizationSearch
+from .rig import Rig, _check_rig, _end_time, _frame
 from .threshold import AdaptiveThreshold, get_threshold_estimator
 from .voxelization import voxel_down_sample
 
@@ -396,13 +401,7 @@ class KissICP:
         ``return_degeneracy`` (degeneracy_ratio > 0 only) appends a ScanDegeneracy of arrays, one entry per frame.
         ``motions``: a matching sequence of motion.Motion or None (None: the constant-velocity model for that frame)."""
         K = len(frames)
-        if motions is not None:
-            if len(motions) != K:
-                raise ValueError("frames and motions differ in length")
-            if any(m is not None and not isinstance(m, Motion) for m in motions):
-                raise TypeError("motions holds Motion objects or None")
-            if not self.fused and any(m is not None for m in motions):
-                raise ValueError("a Motion needs the fused pipeline (fused=True, an adaptive threshold)")
+        self._check_motions(motions, K)
         if return_fits:
             self._check_reports_fits()
         if return_constraints:
@@ -445,6 +444,104 @@ class KissICP:
                                          return_constraints=return_constraints, return_degeneracy=return_degeneracy,
                                          motions=mstructs)
 
+    def _check_motions(self, motions, K):
+        if motions is None:
+            return
+        if len(motions) != K:
+            raise ValueError("frames and motions differ in length")
+        if any(m is not None and not isinstance(m, Motion) for m in motions):
+            raise TypeError("motions holds Motion objects or None")
+        if not self.fused and any(m is not None for m in motions):
+            raise ValueError("a Motion needs the fused pipeline (fused=True, an adaptive threshold)")
+
+    def register_rig_frame(self, scans, rig: Rig, timestamps=None, stamp_offsets=None, motion: Motion | None = None,
+                           return_clouds: bool = True):
+        """Register one frame of a multi-LiDAR rig: ``scans`` one (N_i, 3) array per sensor of ``rig``, ``timestamps``
+        None or one stamp array per sensor, ``stamp_offsets`` None or one offset per sensor (added to its stamps),
+        ``motion`` the base's sampled trajectory (motion.Motion) or None. -> (preprocessed frame, source) like
+        register_frame: the merged base-frame cloud after the pipeline's crop, and its source."""
+        self.register_rig_frames([scans], rig, None if timestamps is None else [timestamps],
+                                 None if stamp_offsets is None else [stamp_offsets],
+                                 motions=None if motion is None else [motion])
+        return self._last_clouds() if return_clouds else (None, None)
+
+    def register_rig_frames(self, frames, rig: Rig, timestamps=None, stamp_offsets=None, motions=None,
+                            return_fits: bool = False, return_constraints: bool = False, return_degeneracy: bool = False):
+        """Register a sequence of rig frames, queued like register_frames -> poses (K, 4, 4) of the base, with the
+        same ``return_fits`` / ``return_constraints`` / ``return_degeneracy`` rules. ``frames`` is a sequence of frames,
+        each one (N_i, 3) array per sensor (all float64 or all float32); ``timestamps`` and ``stamp_offsets`` None or one
+        entry per frame as in register_rig_frame; ``motions`` None or one Motion (the base's poses) or None per frame.
+        Everything is checked before anything is registered, except a frame's own arrays: an invalid frame stops the
+        sequence after the frames before it."""
+        _check_rig(rig)
+        if not self.fused:
+            raise ValueError("a rig needs the fused pipeline (fused=True, an adaptive threshold)")
+        K = len(frames)
+        self._check_motions(motions, K)
+        if return_fits:
+            self._check_reports_fits()
+        if return_constraints:
+            self._check_reports_constraints()
+        if return_degeneracy:
+            self._check_degeneracy()
+        timestamps = [None] * K if timestamps is None else timestamps
+        stamp_offsets = [None] * K if stamp_offsets is None else stamp_offsets
+        if len(timestamps) != K or len(stamp_offsets) != K:
+            raise ValueError("frames, timestamps and stamp_offsets differ in length")
+        f32 = K > 0 and all(isinstance(a, np.ndarray) and a.dtype == np.float32 and a.ndim == 2 and a.shape[1] == 3
+                            for f in frames for a in f)
+        parts = [_frame(f, rig, t, o, f32) for f, t, o in zip(frames, timestamps, stamp_offsets)]
+        pts = [a for p in parts for a in p[0]]
+        ts = [t for p in parts for t in p[1]]
+        offs = [o for p in parts for o in p[2]]
+        mstructs = None
+        if motions is not None and any(m is not None for m in motions):
+            mstructs = [m._struct(_end_time(m, p[1], p[2])) if m is not None else None for m, p in zip(motions, parts)]
+        return self._register_rig_frames_raw(rig, [N.ptr(a) for a in pts], [len(a) for a in pts],
+                                             [N.ptr(t) if t.size else None for t in ts], [len(t) for t in ts], offs,
+                                             1 if f32 else 0, return_fits=return_fits,
+                                             return_constraints=return_constraints,
+                                             return_degeneracy=return_degeneracy, motions=mstructs)
+
+    def _register_rig_frames_raw(self, rig: Rig, xyz_ptrs, sizes, ts_ptrs, ts_sizes, stamp_offsets, layout,
+                                 return_fits: bool = False, return_constraints: bool = False,
+                                 return_degeneracy: bool = False, motions=None):
+        """raw-pointer form of register_rig_frames (host or device addresses, S per frame, layout as
+        _register_frames_raw); stamp_offsets: None or one float per array; motions: None or one _native.Motion (None:
+        no motion) per frame, with its end_time resolved"""
+        S = rig.n_sensors
+        K = len(xyz_ptrs) // S
+        if len(xyz_ptrs) != K * S:
+            raise ValueError(f"{len(xyz_ptrs)} arrays are not frames of {S} sensors")
+        as_vp = lambda v: v if isinstance(v, C.c_void_p) else C.c_void_p(int(v) if v else None)
+        X = (C.c_void_p * (K * S))(*[as_vp(v) for v in xyz_ptrs])
+        T = (C.c_void_p * (K * S))(*[as_vp(v) for v in ts_ptrs])
+        n = (N.sz * (K * S))(*sizes)
+        nt = (N.sz * (K * S))(*ts_sizes)
+        O = None if stamp_offsets is None else (N.dbl * (K * S))(*stamp_offsets)
+        M = None
+        if motions is not None:
+            M = (N.Motion * K)(*[m if m is not None else N.Motion() for m in motions])
+            self._seen_motion = True
+        poses = np.empty((K, 4, 4))
+        fits = (N.Fit * K)() if return_fits else None
+        cons = (N.Constraints * K)() if return_constraints else None
+        degs = (N.Degeneracy * K)() if return_degeneracy else None
+        N.check(N.lib().kb_pipeline_register_rig_frames(self._h, rig._structs, S, X, n, T, nt, O, M, K, int(layout),
+                                                        N.ptr(poses), fits, cons, degs))
+        return self._results(poses, fits, cons, degs)
+
+    @staticmethod
+    def _results(poses, fits, cons, degs):
+        out = [poses]
+        if fits is not None:
+            out.append(_fits_from_structs(fits))
+        if cons is not None:
+            out.append(_from_structs(cons))
+        if degs is not None:
+            out.append(_scan_degeneracy(degs))
+        return out[0] if len(out) == 1 else tuple(out)
+
     def _register_frames_raw(self, xyz_ptrs, sizes, ts_ptrs, ts_sizes, layout, return_fits: bool = False,
                              return_constraints: bool = False, return_degeneracy: bool = False, motions=None):
         """raw-pointer form (host or device addresses): layout 0 host f64, 1 host f32, 2 device f64; motions: None or
@@ -470,14 +567,7 @@ class KissICP:
         else:
             N.check(N.lib().kb_pipeline_register_frames_constraints(self._h, X, n, T, nt, K, int(layout), N.ptr(poses),
                                                                     fits, cons))
-        out = [poses]
-        if return_fits:
-            out.append(_fits_from_structs(fits))
-        if return_constraints:
-            out.append(_from_structs(cons))
-        if return_degeneracy:
-            out.append(_scan_degeneracy(degs))
-        return out[0] if len(out) == 1 else tuple(out)
+        return self._results(poses, fits, cons, degs)
 
     def _register_frame_modular(self, frame, timestamps):
         # python/kiss_icp/kiss_icp.py:43-75, line for line, on the per-module device API

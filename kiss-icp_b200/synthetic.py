@@ -379,3 +379,92 @@ class Shaft:
         rng = np.random.default_rng((self.seed, int(k)))
         pts = t[ok, None] * D[ok] + rng.normal(0.0, self.noise, (int(ok.sum()), 3))
         return pts, np.empty(0)
+
+
+class RigLidar:
+    """Several spinning LiDARs on the base of a SyntheticLidar's ground-truth trajectory (a multi-LiDAR rig).
+
+    ``lidar.pose(k)`` is the base's pose. Sensor i is mounted at ``mounts[i]`` (4x4, base <- sensor) and, where
+    ``shapes`` gives one, has its own (beams, cols, elev_deg); otherwise the lidar's. ``stamps``: 'none' (every sensor
+    captured at the base pose of scan k) or 'sweep' (column c of sensor i captured at the true base pose
+    k - 1 + phases[i] + (c+1)/cols, stamped (c+1)/(cols hz) after its own sweep's start, which is phases[i] / hz after
+    scan_start_time(k): scan(k) returns that as its stamp offset). ``body`` (lo, hi) [m]: an axis-aligned box fixed to
+    the base (the vehicle's body) that every sensor's rays hit, or None. Noise and fp32 rounding as SyntheticLidar.
+    ``scan(k)`` -> (points per sensor in its own frame, stamps per sensor, stamp offsets per sensor)."""
+
+    def __init__(self, lidar: SyntheticLidar, mounts, shapes=None, phases=None, stamps="none", body=None):
+        self.lidar = lidar
+        self.mounts = [np.asarray(M, dtype=np.float64) for M in mounts]
+        S = len(self.mounts)
+        self.phases = [0.0] * S if phases is None else [float(p) for p in phases]
+        if stamps not in ("none", "sweep"):
+            raise ValueError("a rig's stamps are 'none' or 'sweep'")
+        self.stamps = stamps
+        self.body = None if body is None else (np.asarray(body[0], dtype=np.float64), np.asarray(body[1], dtype=np.float64))
+        self.shapes = []
+        for i in range(S):
+            shape = shapes[i] if shapes is not None and shapes[i] is not None else None
+            if shape is None:
+                self.shapes.append((lidar.dirs, lidar.cols, lidar.col_of_point))
+                continue
+            beams, cols, elev = int(shape[0]), int(shape[1]), shape[2]
+            el = np.deg2rad(np.linspace(elev[0], elev[1], beams))
+            az = -2 * math.pi * np.arange(cols) / cols
+            ce, se = np.cos(el), np.sin(el)
+            d = np.stack([np.outer(np.cos(az), ce), np.outer(np.sin(az), ce), np.outer(np.ones_like(az), se)], -1)
+            self.shapes.append((torch.tensor(d.reshape(-1, 3), dtype=torch.float64, device=lidar.device), cols,
+                                np.repeat(np.arange(cols), beams)))
+
+    def pose(self, k: float) -> np.ndarray:
+        """the base's ground-truth pose at (fractional) scan index k"""
+        return self.lidar.pose(k)
+
+    def _body_range(self, M, dirs):
+        """range along each sensor-frame ray of a sensor mounted at M to the body (inf: missed)"""
+        lo = torch.tensor(self.body[0], dtype=torch.float64, device=dirs.device)
+        hi = torch.tensor(self.body[1], dtype=torch.float64, device=dirs.device)
+        o = torch.tensor(M[:3, 3], dtype=torch.float64, device=dirs.device)
+        d = dirs @ torch.tensor(M[:3, :3], dtype=torch.float64, device=dirs.device).T
+        inv = 1.0 / torch.where(d.abs() < 1e-12, torch.full_like(d, 1e-12), d)
+        t0, t1 = (lo - o) * inv, (hi - o) * inv
+        tn, tf = torch.minimum(t0, t1).amax(-1), torch.maximum(t0, t1).amin(-1)
+        return torch.where((tn <= tf) & (tn > 0.05), tn, torch.full_like(tn, float("inf")))
+
+    def scan(self, k: int, body_mask: bool = False):
+        """-> (points, stamps, stamp offsets), one entry per sensor; with body_mask also a bool mask per sensor of
+        its points that hit the body"""
+        L = self.lidar
+        pts, ts, offs, masks = [], [], [], []
+        for i, (M, (dirs, cols, col_of_point)) in enumerate(zip(self.mounts, self.shapes)):
+            g = torch.Generator(device="cpu")
+            g.manual_seed((L.seed * 1_000_003 + int(k)) * 31 + i + 1)
+            n = dirs.shape[0]
+            if self.stamps == "sweep":
+                Tc = [L.pose(k - 1 + self.phases[i] + (c + 1) / cols) @ M for c in range(cols)]
+                Rt = torch.tensor(np.array([T[:3, :3] for T in Tc]), dtype=torch.float64, device=L.device)[col_of_point]
+                origins = torch.tensor(np.array([T[:3, 3] for T in Tc]), dtype=torch.float64, device=L.device)[col_of_point]
+                dirs_w = torch.einsum("nij,nj->ni", Rt, dirs)
+            else:
+                T = L.pose(k) @ M
+                origins = torch.tensor(T[:3, 3], dtype=torch.float64, device=L.device).expand(n, 3)
+                dirs_w = dirs @ torch.tensor(T[:3, :3], dtype=torch.float64, device=L.device).T
+            rng_ = L._cast(origins, dirs_w, k) if L.movers else L._cast(origins, dirs_w)
+            hit_body = torch.zeros(n, dtype=torch.bool, device=L.device)
+            if self.body is not None:
+                tb = self._body_range(M, dirs)
+                hit_body = tb < rng_
+                rng_ = torch.minimum(rng_, tb)
+            noise = torch.randn(n, generator=g, dtype=torch.float64).to(L.device) * L.noise
+            valid = rng_ < L.max_ray
+            r = (rng_ + noise)[valid]
+            pts.append((dirs[valid] * r[:, None]).to(torch.float32).to(torch.float64).cpu().numpy())
+            masks.append(hit_body[valid].cpu().numpy())
+            if self.stamps == "sweep":
+                col = torch.tensor(col_of_point, device=L.device)[valid]
+                ts.append(((col.to(torch.float64) + 1.0) / (cols * L.hz)).cpu().numpy())
+            else:
+                ts.append(np.empty(0))
+            offs.append(self.phases[i] / L.hz)
+        if body_mask:
+            return pts, ts, offs, masks
+        return pts, ts, offs
