@@ -1490,8 +1490,8 @@ int kb_deskew_motion(const double *xyz, size_t n, const double *timestamps, size
         CK(cudaMemcpyAsync(c->ws.in.p, xyz, n * 24, cudaMemcpyHostToDevice, ex.stream));
         CK(cudaMemcpyAsync(c->ws.ts.p, timestamps, n * 8, cudaMemcpyHostToDevice, ex.stream));
     }
-    CK(motion_deskew(ex.stream, ex.sms, d_tab.p, static_cast<int>(tab.size()), c->ws.in.p, false, c->ws.ts.p,
-                     motion->stamp_offset, n, c->ws.tmp.p));
+    CK(motion_deskew(ex.stream, ex.sms, d_tab.p, static_cast<int>(tab.size()), c->ws.in.p, false, c->ws.ts.p, n,
+                     c->ws.tmp.p));
     if (n) ++ex.launches;
     if (n) CK(cudaMemcpyAsync(out, c->ws.tmp.p, n * 24, cudaMemcpyDeviceToHost, ex.stream));
     return ex.sync();  // (d_tab is released after the kernel has read it)
@@ -1542,8 +1542,8 @@ int kb_merge_rig(const kb_sensor *sensors, size_t n_sensors, const double *const
         CK(d_mtab.alloc(mtab.size()));
         CK(cudaMemcpyAsync(d_mtab.p, mtab.data(), mtab.size() * sizeof(MotionSeg), cudaMemcpyHostToDevice, ex.stream));
     }
-    CK(rig_merge(ex.stream, ex.sms, d_tab.p, static_cast<int>(n_sensors), d_mtab.p, static_cast<int>(mtab.size()),
-                 desk ? motion->stamp_offset : 0.0, false, total, c->ws.tmp.p, stamped ? d_ts_out.p : nullptr));
+    CK(rig_merge(ex.stream, ex.sms, d_tab.p, static_cast<int>(n_sensors), d_mtab.p, static_cast<int>(mtab.size()), false,
+                 total, c->ws.tmp.p, stamped ? d_ts_out.p : nullptr));
     ++ex.launches;
     CK(cudaMemcpyAsync(xyz_out, c->ws.tmp.p, total * 24, cudaMemcpyDeviceToHost, ex.stream));
     if (stamped && timestamps_out)
@@ -2026,8 +2026,7 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
         RET(m.xyz.ensure(3 * std::max<size_t>(n[j], 1)));
         const void *in = dev_in ? xyz[j] : p->q[j % D].in.p;
         const double *ts = dev_in ? timestamps[j] : p->q[j % D].ts.p;
-        CK(motion_deskew(ex.stream, ex.sms, m.tab.p, static_cast<int>(tab.size()), in, f32, ts, motion[j].stamp_offset,
-                         n[j], m.xyz.p));
+        CK(motion_deskew(ex.stream, ex.sms, m.tab.p, static_cast<int>(tab.size()), in, f32, ts, n[j], m.xyz.p));
         if (n[j]) ++ex.launches;
         return KB_OK;
     };
@@ -2059,8 +2058,7 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
         CK(cudaMemcpyAsync(r.tab.p, r.pin_tab.p, S * sizeof(RigSensor), cudaMemcpyHostToDevice, ex.stream));
         if (desk[j]) RET(motion_tab(j));
         CK(rig_merge(ex.stream, ex.sms, r.tab.p, static_cast<int>(S), desk[j] ? p->mq[j % D].tab.p : nullptr,
-                     desk[j] ? static_cast<int>(tabs[j].size()) : 0, desk[j] ? motion[j].stamp_offset : 0.0, f32, nj,
-                     r.xyz.p, with_ts ? r.ts.p : nullptr));
+                     desk[j] ? static_cast<int>(tabs[j].size()) : 0, f32, nj, r.xyz.p, with_ts ? r.ts.p : nullptr));
         if (nj) ++ex.launches;
         return KB_OK;
     };

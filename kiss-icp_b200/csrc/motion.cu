@@ -15,11 +15,10 @@ namespace kb_motion_dev {
 
 constexpr double kMotionMaxAngle = 3.141592653589793 - 1e-6;  // below pi, Log(T_k^-1 T_k+1) is unique
 
-// one point per thread: the binary search of the stamp among the intervals, then A_k Exp(tau xi_k) p. The output is
-// the pipeline's own buffer, never the caller's.
+// one point per thread: motion_deskew_point of its stamp along the rebased table (the stamps' own clock, o = 0). The
+// output is the pipeline's own buffer, never the caller's.
 __global__ void __launch_bounds__(256) k_deskew_motion(const MotionSeg *tab, int segs, const void *xyz, int f32,
-                                                       const double *ts, double offset, size_t n, double *out) {
-    constexpr int stride = sizeof(MotionSeg) / sizeof(double);
+                                                       const double *ts, size_t n, double *out) {
     static_assert(sizeof(MotionSeg) % sizeof(double) == 0, "MotionSeg is an array of doubles");
     for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
          i += static_cast<size_t>(gridDim.x) * blockDim.x) {
@@ -31,10 +30,7 @@ __global__ void __launch_bounds__(256) k_deskew_motion(const MotionSeg *tab, int
             const double *d = static_cast<const double *>(xyz) + 3 * i;
             p = kb::V3{d[0], d[1], d[2]};
         }
-        const double t = ts[i] + offset;
-        const int k = motion_interval(&tab[0].t, stride, segs + 1, t);
-        const MotionSeg &s = tab[k];
-        const kb::V3 q = kb::se3_act(motion_at(s.A, s.xi, t - s.t), p);
+        const kb::V3 q = motion_deskew_point(tab, segs, ts[i], 0.0, p);
         out[3 * i] = q.x;
         out[3 * i + 1] = q.y;
         out[3 * i + 2] = q.z;
@@ -100,8 +96,11 @@ SE3 motion_pose(const std::vector<MotionSeg> &iv, double t) {
 
 std::vector<MotionSeg> motion_table(const kb_motion &m) {
     std::vector<MotionSeg> iv = motion_intervals(m);
-    const SE3 end_inv = kb::se3_inverse(motion_pose(iv, m.end_time));
-    for (MotionSeg &s : iv) s.A = kb::se3_mul(end_inv, s.A);
+    const SE3 end_inv = kb::se3_inverse(motion_pose(iv, m.end_time));  // (end_time - t_k: exact, one clock)
+    for (MotionSeg &s : iv) {
+        s.A = kb::se3_mul(end_inv, s.A);
+        s.t -= m.stamp_offset;  // exact for an epoch offset and epoch sample times, and unchanged for offset 0
+    }
     return iv;
 }
 
@@ -111,10 +110,10 @@ SE3 motion_between(const kb_motion &m, double a, double b) {
 }
 
 cudaError_t motion_deskew(cudaStream_t stream, int sms, const MotionSeg *d_tab, int segs, const void *xyz, bool f32,
-                          const double *ts, double offset, size_t n, double *out) {
+                          const double *ts, size_t n, double *out) {
     if (!n) return cudaSuccess;
     const unsigned blocks = static_cast<unsigned>(std::min<size_t>((n + 255) / 256, static_cast<size_t>(sms) * 8));
-    k_deskew_motion<<<blocks, 256, 0, stream>>>(d_tab, segs, xyz, f32 ? 1 : 0, ts, offset, n, out);
+    k_deskew_motion<<<blocks, 256, 0, stream>>>(d_tab, segs, xyz, f32 ? 1 : 0, ts, n, out);
     return cudaGetLastError();
 }
 

@@ -9,21 +9,18 @@
 #include "se3.cuh"
 
 using namespace kb_host;
-using kb::motion_at;
-using kb::motion_interval;
 
 namespace kb_rig_dev {
 
 // one merged point per thread: its sensor from the table's first indices (<= 16, in shared memory), the sensor crop,
-// the extrinsic, then the stamp offset or the deskew along the motion table (as k_deskew_motion). The outputs are the
-// pipeline's own buffers, never the caller's.
+// the extrinsic, then the merged stamp s + stamp_offset and/or the deskew along the rebased motion table
+// (motion_deskew_point of s with the sensor's stamp offset, as k_deskew_motion). The outputs are the pipeline's own
+// buffers, never the caller's.
 __global__ void __launch_bounds__(256) k_merge_rig(const RigSensor *sensors, int S, const MotionSeg *tab, int segs,
-                                                   double motion_offset, int f32, size_t n, double *out,
-                                                   double *out_ts) {
+                                                   int f32, size_t n, double *out, double *out_ts) {
     __shared__ RigSensor sh[KB_RIG_MAX_SENSORS];
     if (threadIdx.x < S) sh[threadIdx.x] = sensors[threadIdx.x];
     __syncthreads();
-    constexpr int stride = sizeof(MotionSeg) / sizeof(double);
     for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
          i += static_cast<size_t>(gridDim.x) * blockDim.x) {
         int si = 0;  // the last sensor that begins at or before i (begin is non-decreasing; empty sensors are skipped)
@@ -44,13 +41,9 @@ __global__ void __launch_bounds__(256) k_merge_rig(const RigSensor *sensors, int
         }
         if (!s.identity) p = kb::se3_act(s.E, p);
         if (s.ts) {
-            const double t = s.ts[j] + s.stamp_offset;
-            if (out_ts) out_ts[i] = t;
-            if (segs) {
-                const double tm = t + motion_offset;
-                const MotionSeg &m = tab[motion_interval(&tab[0].t, stride, segs + 1, tm)];
-                p = kb::se3_act(motion_at(m.A, m.xi, tm - m.t), p);
-            }
+            const double t = s.ts[j];
+            if (out_ts) out_ts[i] = t + s.stamp_offset;
+            if (segs) p = motion_deskew_point(tab, segs, t, s.stamp_offset, p);
         }
         out[3 * i] = p.x;
         out[3 * i + 1] = p.y;
@@ -130,10 +123,10 @@ int rig_frame_check(size_t S, const void *const *xyz, const size_t *n, const dou
 }
 
 cudaError_t rig_merge(cudaStream_t stream, int sms, const RigSensor *d_sensors, int S, const MotionSeg *d_tab, int segs,
-                      double motion_offset, bool f32, size_t n, double *out, double *out_ts) {
+                      bool f32, size_t n, double *out, double *out_ts) {
     if (!n) return cudaSuccess;
     const unsigned blocks = static_cast<unsigned>(std::min<size_t>((n + 255) / 256, static_cast<size_t>(sms) * 8));
-    k_merge_rig<<<blocks, 256, 0, stream>>>(d_sensors, S, d_tab, segs, motion_offset, f32 ? 1 : 0, n, out, out_ts);
+    k_merge_rig<<<blocks, 256, 0, stream>>>(d_sensors, S, d_tab, segs, f32 ? 1 : 0, n, out, out_ts);
     return cudaGetLastError();
 }
 

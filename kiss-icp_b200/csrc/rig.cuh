@@ -33,10 +33,11 @@ std::vector<RigSensor> rig_table(const kb_sensor *sensors, size_t n_sensors);
 int rig_frame_check(size_t S, const void *const *xyz, const size_t *n, const double *const *ts, const size_t *n_ts,
                     const double *stamp_offsets, bool needed, size_t *total, bool *stamped);
 // k_merge_rig on `stream`: the merged frame of the device table d_sensors[S] (n points in all) into out[n][3] and,
-// when out_ts is not null, its stamps into out_ts[n]; with a motion table (segs > 0) the points are deskewed along it,
-// a merged stamp t taken at t + motion_offset
+// when out_ts is not null, its stamps into out_ts[n]; with a motion_table (segs > 0, rebased by the motion's
+// stamp_offset) the points are deskewed along it, a merged stamp s + stamp_offset taken at s + stamp_offset +
+// the motion's stamp_offset
 cudaError_t rig_merge(cudaStream_t stream, int sms, const RigSensor *d_sensors, int S, const MotionSeg *d_tab, int segs,
-                      double motion_offset, bool f32, size_t n, double *out, double *out_ts);
+                      bool f32, size_t n, double *out, double *out_ts);
 #pragma GCC visibility pop
 
 }  // namespace kb_host

@@ -43,16 +43,21 @@ class SyntheticLidar:
 
     def __init__(self, seed=0, beams=64, cols=1024, elev_deg=(-24.8, 2.0), max_ray=120.0, noise=0.02,
                  stamps="none", speed=10.0, hz=10.0, loop_radius=150.0, sensor_height=1.73, n_boxes=260,
-                 device="cpu", movers=None, shake=None):
+                 device="cpu", movers=None, shake=None, t0=0.0):
         """movers: moving boxes (none by default). Each is (size, s0, lateral, speed) or (size, s0, lateral, speed,
         "cross"), with size = (sx, sy, sz) [m] of an axis-aligned box standing on the ground, and t = scan index / hz:
         along the road its centre is at arclength s0 + speed t of the loop, `lateral` metres to the left of it (a
         negative speed drives the other way); a crossing box stays at arclength s0 and moves across the road, its
         centre at lateral + speed t.
         shake: (amplitude [rad], frequency [Hz]): a yaw oscillation A sin(2 pi f t), t = k / hz, added to pose() (a
-        handheld rig or a legged robot turning fast within a sweep); None: none."""
+        handheld rig or a legged robot turning fast within a sweep); None: none.
+        t0: the clock's base [s]: scan k's sweep starts at t0 + (k - 1) / hz on the clock of scan_start_time() and
+        motion_samples() (a ROS header.stamp near 1.7e9 s, say); poses and the per-point stamps, relative to the sweep's
+        start, do not depend on it. With hz and sample rates on a dyadic grid and a dyadic t0 every clock value is exact,
+        and streams at two bases carry the same relative times bit for bit."""
         self.seed, self.beams, self.cols = int(seed), int(beams), int(cols)
         self.hz = float(hz)
+        self.t0 = float(t0)
         self.movers = [tuple(m) for m in movers] if movers else []
         self.shake = None if shake is None else (float(shake[0]), float(shake[1]))
         self.max_ray, self.noise, self.stamps = float(max_ray), float(noise), stamps
@@ -139,20 +144,22 @@ class SyntheticLidar:
         return T
 
     def scan_start_time(self, k: int) -> float:
-        """the time [s] at which scan k's sweep starts (scan index k is at time k / hz, where its sweep ends)"""
-        return (k - 1) / self.hz
+        """the clock time [s] at which scan k's sweep starts (scan index k is at time t0 + k / hz, where its sweep ends)"""
+        return self.t0 + (k - 1) / self.hz
 
     def motion_samples(self, k: int, rate_hz: float, eps: float = 1e-5):
-        """Ground truth sampled over scan k's sweep, at rate_hz from scan_start_time(k) to k / hz (both included):
-        (times (m,), poses (m, 4, 4) world <- sensor, body angular rates (m, 3) [rad/s] and body velocities (m, 3)
-        [m/s], both in the sensor frame at each time, by central differences of pose())."""
-        t0, t1 = self.scan_start_time(k), k / self.hz
+        """Ground truth sampled over scan k's sweep, at rate_hz from scan_start_time(k) to t0 + k / hz (both included):
+        (times (m,) on the clock, poses (m, 4, 4) world <- sensor, body angular rates (m, 3) [rad/s] and body
+        velocities (m, 3) [m/s], both in the sensor frame at each time, by central differences of pose()). The poses
+        are those at the times relative to t0."""
+        t0, t1 = (k - 1) / self.hz, k / self.hz
         m = int(round((t1 - t0) * rate_hz)) + 1
-        times = np.linspace(t0, t1, m)
-        poses = np.array([self.pose(t * self.hz) for t in times])
+        rel = np.linspace(t0, t1, m)
+        times = self.t0 + rel
+        poses = np.array([self.pose(t * self.hz) for t in rel])
         rates = np.empty((m, 3))
         vel = np.empty((m, 3))
-        for i, t in enumerate(times):
+        for i, t in enumerate(rel):
             A, B = self.pose((t - eps) * self.hz), self.pose((t + eps) * self.hz)
             R = poses[i, :3, :3]
             D = A[:3, :3].T @ B[:3, :3]
@@ -390,10 +397,14 @@ class RigLidar:
     k - 1 + phases[i] + (c+1)/cols, stamped (c+1)/(cols hz) after its own sweep's start, which is phases[i] / hz after
     scan_start_time(k): scan(k) returns that as its stamp offset). ``body`` (lo, hi) [m]: an axis-aligned box fixed to
     the base (the vehicle's body) that every sensor's rays hit, or None. Noise and fp32 rounding as SyntheticLidar.
+    ``clock_offsets``: the stamp offsets are the sensors' sweep starts on the lidar's clock (scan_start_time(k) +
+    phases[i] / hz, with its base t0) rather than relative to scan_start_time(k).
     ``scan(k)`` -> (points per sensor in its own frame, stamps per sensor, stamp offsets per sensor)."""
 
-    def __init__(self, lidar: SyntheticLidar, mounts, shapes=None, phases=None, stamps="none", body=None):
+    def __init__(self, lidar: SyntheticLidar, mounts, shapes=None, phases=None, stamps="none", body=None,
+                 clock_offsets=False):
         self.lidar = lidar
+        self.clock_offsets = bool(clock_offsets)
         self.mounts = [np.asarray(M, dtype=np.float64) for M in mounts]
         S = len(self.mounts)
         self.phases = [0.0] * S if phases is None else [float(p) for p in phases]
@@ -464,7 +475,7 @@ class RigLidar:
                 ts.append(((col.to(torch.float64) + 1.0) / (cols * L.hz)).cpu().numpy())
             else:
                 ts.append(np.empty(0))
-            offs.append(self.phases[i] / L.hz)
+            offs.append(L.scan_start_time(k) + self.phases[i] / L.hz if self.clock_offsets else self.phases[i] / L.hz)
         if body_mask:
             return pts, ts, offs, masks
         return pts, ts, offs
