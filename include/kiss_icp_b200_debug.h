@@ -109,6 +109,12 @@ int kb_pipeline_get_history(const kb_pipeline *p, kb_frame_stats *out, size_t ca
  * end phases, [7] candidate lists done, [10] ICP iterations done, [11] next frame's front end done (prefetch), [4] ICP result
  * everywhere, [5] map updated, [6] kernel end, [8,9] map phases, [12..19] downsample phases */
 int kb_pipeline_history_stamps(const kb_pipeline *p, double *out, size_t capacity, size_t *n_out);
+/* the launch boundary of the logged frames (profiling on), ns modulo 2^40, 3 per frame, over all CTAs of the launch:
+ * [0] the first CTA entered, [1] the last CTA finished the prologue (state read, veto decided), [2] the last CTA left */
+int kb_pipeline_history_grid_stamps(const kb_pipeline *p, double *out, size_t capacity, size_t *n_out);
+/* 0: queued calls compute no frame's front end in the launch before it, every launch runs its own (default 1: frames
+ * without timestamps are prefetched). Results do not change; the ICP team then runs without the front end beside it. */
+int kb_pipeline_debug_prefetch(kb_pipeline *p, int enabled);
 
 #ifdef __cplusplus
 }

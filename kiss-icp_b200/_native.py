@@ -240,6 +240,8 @@ SIGNATURES = {
     "kb_pipeline_last_sigma": (i32, [vp, C.POINTER(dbl)]),
     "kb_pipeline_debug_stamps": (i32, [vp, vp, i32]),
     "kb_pipeline_history_stamps": (i32, [vp, vp, sz, C.POINTER(sz)]),
+    "kb_pipeline_history_grid_stamps": (i32, [vp, vp, sz, C.POINTER(sz)]),
+    "kb_pipeline_debug_prefetch": (i32, [vp, i32]),
     "kb_debug_icp_solve_fast": (i32, [vp, vp, vp, vp]),
     "kb_debug_icp_schur": (i32, [vp, vp, vp, C.POINTER(i32)]),
     "kb_debug_nn_reuse": (i32, [vp, vp, vp, sz, i32, vp, vp, vp]),

@@ -414,8 +414,10 @@ struct kb_pipeline {
     Work vox_ws;            // scratch of kb_pipeline_voxelize (must not clobber the clouds of the last frame)
     unsigned long long grow_retries = 0;
     std::vector<kb_frame_stats> history;
-    std::vector<std::array<double, 20>> history_stamps;  // the frames' %globaltimer stamps, ns modulo 2^40 (profiling on)
+    // the frames' %globaltimer stamps, ns modulo 2^40 (profiling on): FrameResult::t_ns[20], then t_grid[3]
+    std::vector<std::array<double, 23>> history_stamps;
     size_t history_cap = 0;
+    bool prefetch = true;  // kb_pipeline_debug_prefetch
     // frame queue of every registration call (a blocking call is a queue of one frame): frame k+1 is copied in while
     // frame k is registered
     struct Slot {
@@ -1740,8 +1742,9 @@ static int pipeline_absorb(kb_pipeline *p, const FrameResult &r, size_t n, long 
         st.map_voxels = p->last.map_live;
         st.team = p->last.team;
         p->history.push_back(st);
-        std::array<double, 20> ts;
+        std::array<double, 23> ts;
         for (int i = 0; i < 20; ++i) ts[i] = static_cast<double>(p->last.t_ns[i] & ((1ull << 40) - 1));
+        for (int i = 0; i < 3; ++i) ts[20 + i] = static_cast<double>(p->last.t_grid[i] & ((1ull << 40) - 1));
         p->history_stamps.push_back(ts);
     }
     if (p->last.map_status & ST_TABLE_FULL) return fail(KB_ERR_CUDA, "voxel table overflow (internal capacity bug)");
@@ -2081,7 +2084,7 @@ static int register_frames(kb_pipeline *p, const void *const *xyz, const size_t 
             auto &s = p->q[k % D];
             if (!p->localizer) RET(p->map->ensure_capacity(pipeline_extra(p, nk)));  // rebuilds only with nothing in flight
             // a frame without stamps, or with a kb_motion, does not depend on this one's result
-            const bool prefetch = k + 1 < valid && (!use_ts[k + 1] || has_motion[k + 1]) && n[k + 1] > 0;
+            const bool prefetch = p->prefetch && k + 1 < valid && (!use_ts[k + 1] || has_motion[k + 1]) && n[k + 1] > 0;
             const double *d_xyz = nullptr, *d_ts = nullptr, *d_next = nullptr;
             if (dev_in && !rig) {
                 d_xyz = static_cast<const double *>(xyz[k]);
@@ -2643,6 +2646,19 @@ int kb_pipeline_history_stamps(const kb_pipeline *p, double *out, size_t capacit
     if (!out) return KB_OK;
     if (capacity < p->history_stamps.size()) return fail(KB_ERR_CAPACITY, "stamp buffer too small");
     for (size_t i = 0; i < p->history_stamps.size(); ++i) std::memcpy(out + 20 * i, p->history_stamps[i].data(), 20 * sizeof(double));
+    return KB_OK;
+}
+int kb_pipeline_history_grid_stamps(const kb_pipeline *p, double *out, size_t capacity, size_t *n_out) {
+    if (!p || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    *n_out = p->history_stamps.size();
+    if (!out) return KB_OK;
+    if (capacity < p->history_stamps.size()) return fail(KB_ERR_CAPACITY, "stamp buffer too small");
+    for (size_t i = 0; i < p->history_stamps.size(); ++i) std::memcpy(out + 3 * i, p->history_stamps[i].data() + 20, 3 * sizeof(double));
+    return KB_OK;
+}
+int kb_pipeline_debug_prefetch(kb_pipeline *p, int enabled) {
+    if (!p) return fail(KB_ERR_INVALID_ARG, "p == NULL");
+    p->prefetch = enabled != 0;
     return KB_OK;
 }
 int kb_pipeline_launch_count(const kb_pipeline *p, unsigned long long *out) {

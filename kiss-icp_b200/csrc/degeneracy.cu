@@ -9,10 +9,10 @@
 #undef kb
 
 namespace kb_degen {
-template __global__ void k_register_frame<DegenParams, false, false>(const DegenParams P);
-template __global__ void k_register_frame<DegenParams, false, true>(const DegenParams P);
-template __global__ void k_register_frame<DegenParams, true, false>(const DegenParams P);
-template __global__ void k_register_frame<DegenParams, true, true>(const DegenParams P);
+template __global__ void k_register_frame<DegenParams, false, false>(const __grid_constant__ DegenParams P);
+template __global__ void k_register_frame<DegenParams, false, true>(const __grid_constant__ DegenParams P);
+template __global__ void k_register_frame<DegenParams, true, false>(const __grid_constant__ DegenParams P);
+template __global__ void k_register_frame<DegenParams, true, true>(const __grid_constant__ DegenParams P);
 }  // namespace kb_degen
 
 const void *degeneracy_kernel(bool localizer, bool planes) {

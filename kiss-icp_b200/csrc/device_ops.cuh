@@ -174,14 +174,16 @@ struct Grid {
     }
     // every CTA, once, after its last sync(): the last one to leave re-arms the barrier for the next launch, which
     // saves the host a memset node in front of every launch (kernels launched with Exec::coop(..., self_reset))
-    // (full-grid object only; also re-arms the team counter word)
-    __device__ __forceinline__ void finish() {
+    // (full-grid object only; also re-arms the team counter word). True in thread 0 of the last CTA to leave.
+    __device__ __forceinline__ bool finish() {
         if (threadIdx.x == 0 && atomicAdd(bar + BAR_ARRIVE, 1u) == gridDim.x - 1) {
             atomicExch(bar + BAR_ARRIVE, 0u);
             atomicExch(bar + BAR_TEAM, 0u);
             atomicExch(bar + BAR_TICKET, 0u);
             atomicExch(bar, 0u);
+            return true;
         }
+        return false;
     }
 };
 

@@ -38,6 +38,7 @@ struct FrameResult {
     double icp_queries;     // GetClosestNeighbor calls (iterations x source points)
     double cache_stats[3];  // NN-cache hits / fills / overflows over all iterations
     unsigned long long t_ns[20];  // %globaltimer at phase boundaries (CTA 0): start, pre, ds1, ds2, icp, map, end
+    unsigned long long t_grid[3];  // %globaltimer over all CTAs: first CTA entered, last CTA past the prologue, last CTA left
 };
 
 // output of the front end of one frame (Preprocess + Voxelize, KissICP.cpp:38,41): two sets, so that the next
@@ -100,6 +101,15 @@ __device__ __forceinline__ void threshold_update(const SE3 &dev, double min_moti
 
 #define KB_STAMP(i) \
     if (P.sc.profile && blockIdx.x == 0 && threadIdx.x == 0) P.res->t_ns[i] = globaltimer_ns()
+
+// every CTA of k_register_frame, once, at its end: Grid::finish, and with profiling the last CTA to leave completes the
+// launch-boundary stamps (FrameResult::t_grid) and re-arms their word
+__device__ __forceinline__ void frame_leave(Grid &g, const Scratch &sc, FrameResult *res) {
+    if (g.finish() && sc.profile) {
+        res->t_grid[0] = ~atomicExch(reinterpret_cast<unsigned long long *>(sc.bar + BAR_FIRST_IN), 0ull);
+        res->t_grid[2] = globaltimer_ns();
+    }
+}
 
 extern __shared__ __align__(16) unsigned char kb_dyn_smem[];  // QCache[NWARPS][QC_SLOTS] (op_icp) or the TeamSmem layout (op_icp_team)
 
@@ -443,13 +453,14 @@ __device__ __forceinline__ void planes_finish(const PlaneOut &pl) {
 // writes to the map. Otherwise (odometry) the fit pass runs in front of the map update, with one grid barrier between
 // them (op_fit_planes reads the table op_map_add writes).
 template <class Params, bool LOCALIZE = false, bool PLANES = false>
-__global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
+__global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const __grid_constant__ Params P) {
     constexpr bool FIT = std::is_base_of<ReportParams, Params>::value;
     constexpr bool DEGEN = std::is_same<Params, DegenParams>::value;
     static_assert(FIT || (!LOCALIZE && !PLANES), "a localizer, and plane reporting, need the fit's ReportParams");
     __shared__ Shared sh;
     Grid g;
     g.init(P.sc.bar);
+    const unsigned long long t_in = P.sc.profile && threadIdx.x == 0 ? globaltimer_ns() : 0ull;
     KB_STAMP(0);
     const SE3 last_pose = P.st->last_pose;
     const SE3 last_delta = P.st->last_delta;
@@ -458,11 +469,15 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
     const long long front_id = P.st->front_id;
     if (!LOCALIZE && P.st->vetoed) {  // written only by an EARLIER launch: uniform across the grid
         if (blockIdx.x == 0 && threadIdx.x == 0) P.res->map_status = ST_SKIPPED;
-        g.finish();
+        frame_leave(g, P.sc, P.res);
         return;
     }
     const Front fr = P.ws.fr[P.id & 1];
     kb_mark(0x100u + (static_cast<unsigned>(P.id) & 0xffu) * 0x10000u);
+    if (P.sc.profile && threadIdx.x == 0) {  // the launch boundary (t_grid): earliest entry, latest end of the prologue (state read, veto decided)
+        atomicMax(reinterpret_cast<unsigned long long *>(P.sc.bar + BAR_FIRST_IN), ~t_in);
+        atomicMax(&P.res->t_grid[1], globaltimer_ns());  // (the slot's last frame stamped earlier times)
+    }
     if (front_id != P.id) {  // uniform: written only by an earlier launch
         op_front(g, P.sc, sh, P.ws, fr, P.in, P.n, P.ts, P.n_ts, P.deskew != 0, last_delta, P.max_range, P.min_range,
                  P.voxel_size, P.in_f32 != 0, P.sc.profile ? P.res->t_ns : nullptr);
@@ -484,7 +499,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
                 P.st->vetoed = 1;     // every CTA read it before the first grid barrier
                 P.st->front_id = P.id;  // fr[id & 1] holds this frame's front end: the replay skips it
             }
-            g.finish();
+            frame_leave(g, P.sc, P.res);
             return;  // uniform across the grid
         }
     }
@@ -633,7 +648,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_register_frame(const Params P) {
         r->map_status = P.m.counters[C_STATUS];
         if (P.sc.profile) r->t_ns[6] = globaltimer_ns();
     }
-    g.finish();
+    frame_leave(g, P.sc, P.res);
 }
 
 }  // namespace kb

@@ -14,10 +14,10 @@
 #undef kb
 
 namespace kb_report {
-template __global__ void k_register_frame<ReportParams, false, false>(const ReportParams P);
-template __global__ void k_register_frame<ReportParams, false, true>(const ReportParams P);
-template __global__ void k_register_frame<ReportParams, true, false>(const ReportParams P);
-template __global__ void k_register_frame<ReportParams, true, true>(const ReportParams P);
+template __global__ void k_register_frame<ReportParams, false, false>(const __grid_constant__ ReportParams P);
+template __global__ void k_register_frame<ReportParams, false, true>(const __grid_constant__ ReportParams P);
+template __global__ void k_register_frame<ReportParams, true, false>(const __grid_constant__ ReportParams P);
+template __global__ void k_register_frame<ReportParams, true, true>(const __grid_constant__ ReportParams P);
 
 // cooperative: the pass, one grid barrier, the partials added by the last CTA (as in the pipeline kernels)
 template <bool FIT, bool PLANES>

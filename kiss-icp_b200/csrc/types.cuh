@@ -15,6 +15,7 @@ constexpr int BLOCK = 512;  // threads per CTA of every cooperative kernel
 constexpr int NACC = 16;  // unique accumulators of the 6x6 normal equations (see icp_accumulate)
 constexpr int NPART = NACC + 5;  // per-CTA partial: accumulators, #correspondences, #candidate points, cache hits/fills/overflows
 constexpr int BAR_ARRIVE = 32, BAR_TEAM = 64, BAR_TICKET = 96, BAR_WORDS = 128;  // word offsets inside Scratch::bar (one 128-byte line each)
+constexpr int BAR_FIRST_IN = BAR_ARRIVE + 2;  // 64-bit (profiling): ~(earliest CTA entry %globaltimer) of this launch, 0 when idle
 constexpr int LL_RES = 16;        // est(7) + done flag, final pose(7), spare      // est(7) t_icp(7) final(7) conv cand_total query_total ...
 constexpr int QC_MAX = 64;   // cached candidates per query
 
