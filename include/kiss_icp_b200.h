@@ -499,6 +499,44 @@ int kb_pipeline_register_rig_frames(kb_pipeline *p, const kb_sensor *sensors, si
 int kb_merge_rig(const kb_sensor *sensors, size_t n_sensors, const double *const *xyz, const size_t *n,
                  const double *const *timestamps, const size_t *n_timestamps, const double *stamp_offsets,
                  const kb_motion *motion, double *xyz_out, double *timestamps_out);
+/* Extrinsic calibration of a rig from a recorded run (DESIGN.md section 4.19). Given a map in the world frame, the base
+ * poses T_k (world <- base) of K frames and, per frame k and sensor j, a scan p in the sensor frame without stamps, every
+ * refined sensor j (refine[j] = 1; refine NULL: all) minimises over E_j
+ *   sum_k sum_i rho(|T_k E_j p - q|),  q the nearest map point of T_k E_j p, kept when closer than
+ *   max_correspondence_distance, rho KISS-ICP's Geman-McClure (w = kernel_scale^2 / (kernel_scale + |r|^2)^2).
+ * A point counts only if min_range_j < |p| < max_range_j (strict; a non-finite point fails). Each iteration builds,
+ * per refined sensor, KISS-ICP's system with source p and target (T_k E_j)^-1 q, solves it as the ICP loop does and
+ * sets E_j <- E_j Exp(dx), tangent (translation, rotation) along the sensor's own axes. Sensors are independent: each
+ * stops at |dx| < convergence_criterion or after max_iterations. A sensor without correspondences keeps its extrinsic.
+ * At the returned extrinsics one more pass gives each refined sensor its kb_fit (n_source: points that passed the crop;
+ * JTJ in the sensor tangent) and its kb_constraints over the same correspondences, J = [n_s^T, (p x n_s)^T] with the
+ * voxel normal rotated into the sensor frame, n_s = (R_k R_j)^T n. A sensor that is not refined is not read: its
+ * extrinsic comes back bit for bit and its report is zeros. A refined extrinsic that no step moved comes back bit for
+ * bit too.
+ * frames: xyz[k S + j], n[k S + j] in `layout` (device frames on the map's device are read in place). Synchronous;
+ * only reads the map (allowed while localizers hold it). Bit-identical from run to run for a given grid size
+ * (kb_set_grid_blocks). Every argument is checked before any device is looked for, and on error nothing is written:
+ * KB_ERR_INVALID_ARG for a NULL argument (an array of a refined sensor with points included), a refine entry other
+ * than 0 or 1, an option that is NaN or out of range, a layout that is none of kb_frame_layout, or 2^31 or more points
+ * of the refined sensors in all; the checks of kb_rig_check; KB_ERR_NOT_SE3 for a pose outside SE(3). K = 0, or no
+ * refined sensor, returns the extrinsics and zero reports without device work. KB_ERR_CUDA when a device allocation
+ * fails. */
+typedef struct kb_rig_calibration_options {
+    double max_correspondence_distance;  /* > 0, finite                                      */
+    double kernel_scale;                 /* > 0, finite                                      */
+    int    max_iterations;               /* >= 0; 0: only the report at the given extrinsics */
+    double convergence_criterion;        /* >= 0, finite                                     */
+} kb_rig_calibration_options;
+typedef struct kb_sensor_calibration {
+    int iterations, converged;
+    kb_fit fit;                  /* at the returned extrinsic, sensor tangent          */
+    kb_constraints constraints;  /* same correspondences, sensor tangent, lever = p    */
+} kb_sensor_calibration;
+int kb_calibrate_rig(const kb_map *map, const double *poses /* [K][16] */, size_t K,
+                     const kb_sensor *sensors, size_t n_sensors, const int *refine /* [S], NULL: all */,
+                     const void *const *xyz /* [K S] */, const size_t *n /* [K S] */, int layout,
+                     const kb_rig_calibration_options *opt,
+                     double *extrinsics_out /* [S][16] */, kb_sensor_calibration *report_out /* [S] */);
 
 /* ---- relocalization: a global pose search in a bounded region ----------------------------
  * No reference counterpart. Finds a scan's pose in a map without an initial pose: every hypothesis of a grid in x, y

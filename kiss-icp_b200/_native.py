@@ -114,6 +114,17 @@ class Sensor(C.Structure):
     _fields_ = [("extrinsic", dbl * 16), ("min_range", dbl), ("max_range", dbl)]
 
 
+class RigCalibrationOptions(C.Structure):
+    """kb_rig_calibration_options"""
+    _fields_ = [("max_correspondence_distance", dbl), ("kernel_scale", dbl), ("max_iterations", i32),
+                ("convergence_criterion", dbl)]
+
+
+class SensorCalibration(C.Structure):
+    """kb_sensor_calibration: one sensor's result of kb_calibrate_rig"""
+    _fields_ = [("iterations", i32), ("converged", i32), ("fit", Fit), ("constraints", Constraints)]
+
+
 class RelocSearch(C.Structure):
     """kb_reloc_search: the hypothesis grid of kb_relocalize"""
     _fields_ = [("center", dbl * 16), ("half_cells_x", i32), ("half_cells_y", i32), ("step", dbl), ("n_yaw", i32),
@@ -293,6 +304,8 @@ SIGNATURES = {
     "kb_rig_check": (i32, [vp, sz]),
     "kb_pipeline_register_rig_frames": (i32, [vp, vp, sz, vp, vp, vp, vp, vp, vp, sz, i32, vp, vp, vp, vp]),
     "kb_merge_rig": (i32, [vp, sz, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "kb_calibrate_rig": (i32, [vp, vp, sz, vp, sz, vp, vp, vp, i32, C.POINTER(RigCalibrationOptions), vp,
+                               vp]),
     "kb_place_params_default": (None, [C.POINTER(PlaceParams)]),
     "kb_place_db_create": (i32, [C.POINTER(PlaceParams), C.POINTER(vp)]),
     "kb_place_db_destroy": (i32, [vp]),
