@@ -537,6 +537,60 @@ int kb_calibrate_rig(const kb_map *map, const double *poses /* [K][16] */, size_
                      const void *const *xyz /* [K S] */, const size_t *n /* [K S] */, int layout,
                      const kb_rig_calibration_options *opt,
                      double *extrinsics_out /* [S][16] */, kb_sensor_calibration *report_out /* [S] */);
+/* Clock-offset and extrinsic calibration of a rig from a recorded run with per-point stamps (DESIGN.md section 4.20).
+ * The base moves along one trajectory over the whole run, T(t) = T_i Exp((t - t_i) xi_i) (the kb_motion's samples,
+ * world <- base; end_time is ignored). Point p of frame k, sensor j, with stamp s is at trajectory-clock time
+ *   t = s + stamp_offsets[k S + j] + o_j + trajectory->stamp_offset
+ * (the stamp offsets of all frames on one clock, e.g. each sweep's start time), o_j the sensor's unknown clock offset,
+ * and at m = T(t) E_j p in the world. Every processed sensor (refine[j] or refine_time[j]) minimises
+ *   sum rho(|m - q|),  q the nearest map point of m, kept when closer than max_correspondence_distance, rho as in
+ *   kb_calibrate_rig,
+ * over E_j <- E_j Exp(dx) (refine[j]) and o_j <- o_j + do (refine_time[j]). Per correspondence, in the sensor
+ * coordinates of kb_calibrate_rig (source p, target q_s = (T(t) E_j)^-1 q), the extrinsic columns are KISS-ICP's
+ * J = [I, -[p]x] and the time column J_o = R_j^T (v_i + w_i x E_j p), (v_i, w_i) = xi_i of the point's interval.
+ * The 7x7 system [H_ee h; h^T H_oo] [dx; do] = -[g_e; g_o] is solved by a Schur complement on the offset: H_ee (the
+ * ICP loop's 6x6 rule) is solved for -g_e and for h, s = H_oo - h^T H_ee^-1 h, do = -(g_o + h^T H_ee^-1 g_e) / s,
+ * dx = H_ee^-1 (-g_e - h do). The offset is held (do = 0, and dx is exactly kb_calibrate_rig's step on the same sums)
+ * when the sensor's offset is not refined, H_oo is 0, or s <= KB_CLOCK_HOLD_RATIO H_oo (the offset is confounded with
+ * the extrinsic). With only the offset refined, do = -g_o / H_oo under the same rule. Without motion (xi = 0, which
+ * two bit-identical consecutive samples give exactly) J_o is 0 and the offset comes back bit for bit. A sensor stops
+ * when every unknown it refines moved less than its criterion (|dx| < convergence_criterion, |do| <
+ * time_convergence_criterion) or after max_iterations. A point counts if it passes its sensor's crop and its stamp is
+ * finite. At the returned values one more pass reports, per processed sensor, the kb_fit and kb_constraints of
+ * kb_calibrate_rig, time_row = (H_oe, H_oo) and time_schur = s (0: the run does not pin the offset).
+ * Frames: xyz[k S + j], n[k S + j] in `layout`; timestamps[k S + j] (n_timestamps[k S + j] == n[k S + j]) are host
+ * float64 in every layout: the host reads them to bound each frame's interval search. stamp_offsets NULL: all 0;
+ * time_offsets NULL: all 0. Sensors that neither flag selects are not read: their extrinsics and offsets come back
+ * bit for bit and their reports are zeros. Synchronous, reads the map only (allowed while localizers hold it),
+ * bit-identical from run to run for a given grid size (kb_set_grid_blocks). Every argument is checked before any
+ * device is looked for, and on error nothing is written: the checks of kb_calibrate_rig (without poses), and
+ * KB_ERR_INVALID_ARG for a refine_time entry other than 0 or 1, a processed sensor's frame with points but NULL stamps
+ * or n_timestamps != n, a non-finite stamp offset or time offset of a processed sensor, or a time_convergence_criterion
+ * that is NaN, negative or infinite; the checks of kb_motion_check on the trajectory. K = 0, or no processed sensor,
+ * returns the values as given and zero reports without device work. */
+#define KB_CLOCK_HOLD_RATIO 1e-10
+typedef struct kb_rig_clock_calibration_options {
+    double max_correspondence_distance;  /* > 0, finite                                    */
+    double kernel_scale;                 /* > 0, finite                                    */
+    int    max_iterations;               /* >= 0; 0: only the report at the given values   */
+    double convergence_criterion;        /* >= 0, finite; of |dx|                          */
+    double time_convergence_criterion;   /* >= 0, finite; of |do| [s]                      */
+} kb_rig_clock_calibration_options;
+typedef struct kb_sensor_clock_calibration {
+    int iterations, converged;
+    kb_fit fit;                  /* at the returned values, sensor tangent                               */
+    kb_constraints constraints;  /* same correspondences, sensor tangent, lever = p                      */
+    double time_row[7];          /* (H_oe[6], H_oo) at the returned values                               */
+    double time_schur;           /* s = H_oo - H_oe H_ee^-1 H_eo: the offset's information with E_j free */
+} kb_sensor_clock_calibration;
+int kb_calibrate_rig_clocks(const kb_map *map, const kb_motion *trajectory, const kb_sensor *sensors, size_t n_sensors,
+                            const int *refine /* [S], NULL: all */, const int *refine_time /* [S], NULL: all */,
+                            const double *time_offsets /* [S], NULL: all 0 */,
+                            const void *const *xyz /* [K S] */, const size_t *n /* [K S] */,
+                            const double *const *timestamps /* [K S] */, const size_t *n_timestamps /* [K S] */,
+                            const double *stamp_offsets /* [K S], NULL: all 0 */, size_t K, int layout,
+                            const kb_rig_clock_calibration_options *opt, double *extrinsics_out /* [S][16] */,
+                            double *time_offsets_out /* [S] */, kb_sensor_clock_calibration *report_out /* [S] */);
 
 /* ---- relocalization: a global pose search in a bounded region ----------------------------
  * No reference counterpart. Finds a scan's pose in a map without an initial pose: every hypothesis of a grid in x, y

@@ -20,5 +20,6 @@ from .metrics import absolute_trajectory_error, sequence_error  # noqa: F401
 from .motion import Motion, deskew, motion_from_gyro  # noqa: F401
 from .rig import Rig, Sensor, merge_rig  # noqa: F401
 from .calibration import RigCalibration, SensorCalibration, calibrate_rig  # noqa: F401
+from .calibration import RigClockCalibration, SensorClockCalibration, calibrate_rig_clocks  # noqa: F401
 
 __version__ = "0.1.0"

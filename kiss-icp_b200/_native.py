@@ -125,6 +125,18 @@ class SensorCalibration(C.Structure):
     _fields_ = [("iterations", i32), ("converged", i32), ("fit", Fit), ("constraints", Constraints)]
 
 
+class RigClockCalibrationOptions(C.Structure):
+    """kb_rig_clock_calibration_options"""
+    _fields_ = [("max_correspondence_distance", dbl), ("kernel_scale", dbl), ("max_iterations", i32),
+                ("convergence_criterion", dbl), ("time_convergence_criterion", dbl)]
+
+
+class SensorClockCalibration(C.Structure):
+    """kb_sensor_clock_calibration: one sensor's result of kb_calibrate_rig_clocks"""
+    _fields_ = [("iterations", i32), ("converged", i32), ("fit", Fit), ("constraints", Constraints),
+                ("time_row", dbl * 7), ("time_schur", dbl)]
+
+
 class RelocSearch(C.Structure):
     """kb_reloc_search: the hypothesis grid of kb_relocalize"""
     _fields_ = [("center", dbl * 16), ("half_cells_x", i32), ("half_cells_y", i32), ("step", dbl), ("n_yaw", i32),
@@ -306,6 +318,8 @@ SIGNATURES = {
     "kb_merge_rig": (i32, [vp, sz, vp, vp, vp, vp, vp, vp, vp, vp]),
     "kb_calibrate_rig": (i32, [vp, vp, sz, vp, sz, vp, vp, vp, i32, C.POINTER(RigCalibrationOptions), vp,
                                vp]),
+    "kb_calibrate_rig_clocks": (i32, [vp, C.POINTER(Motion), vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, sz, i32,
+                                      C.POINTER(RigClockCalibrationOptions), vp, vp, vp]),
     "kb_place_params_default": (None, [C.POINTER(PlaceParams)]),
     "kb_place_db_create": (i32, [C.POINTER(PlaceParams), C.POINTER(vp)]),
     "kb_place_db_destroy": (i32, [vp]),
