@@ -61,15 +61,66 @@ def _calibrate(voxel_map: VoxelHashMap, poses, rig: Rig, ptrs, sizes, layout: in
     K = len(P)
     if len(ptrs) != K * S or len(sizes) != K * S:
         raise ValueError(f"{len(ptrs)} arrays are not {K} frames of {S} sensors")
-    X = (C.c_void_p * max(K * S, 1))(*[C.c_void_p(int(p)) if p else None for p in ptrs])
-    n = (N.sz * max(K * S, 1))(*sizes)
-    ref = None if refine is None else (N.i32 * S)(*[int(bool(r)) for r in refine])
+    X, n = _frame_arrays(ptrs, sizes)
     opt = N.RigCalibrationOptions(float(max_dist), float(kscale), int(max_iter), float(conv))
     E = np.empty((S, 4, 4))
     rep = (N.SensorCalibration * S)()
-    check_value(N.lib().kb_calibrate_rig(voxel_map._h, N.ptr(P), K, rig._structs, S, ref, X, n, int(layout),
-                                         C.byref(opt), N.ptr(E), rep))
+    check_value(N.lib().kb_calibrate_rig(voxel_map._h, N.ptr(P), K, rig._structs, S, _flag_array(refine, S), X, n,
+                                         int(layout), C.byref(opt), N.ptr(E), rep))
     return E, list(rep)
+
+
+def _frame_arrays(ptrs, sizes):
+    X = (C.c_void_p * max(len(ptrs), 1))(*[C.c_void_p(int(p)) if p else None for p in ptrs])
+    return X, (N.sz * max(len(sizes), 1))(*sizes)
+
+
+def _flag_array(flags, S: int):
+    return None if flags is None else (N.i32 * S)(*[int(bool(r)) for r in flags])
+
+
+def _check_run(rig: Rig, frames: list, reference, *per_frame) -> tuple[int, int, int]:
+    """K frames of S scans (and of S entries in each of per_frame's K lists) and a reference sensor -> (S, K, reference)"""
+    S, K = rig.n_sensors, len(frames)
+    if any(len(x) != K for x in per_frame):
+        raise ValueError("frames, timestamps and stamp_offsets differ in length")
+    for f in zip(frames, *per_frame):
+        if any(len(x) != S for x in f):
+            raise ValueError(f"a frame of this rig has {S} scans, stamp arrays and stamp offsets" if per_frame else
+                             f"a frame of this rig has {S} scans, not {len(f[0])}")
+    if not 0 <= int(reference) < S:
+        raise ValueError(f"reference {reference} is not a sensor of this {S}-sensor rig")
+    return S, K, int(reference)
+
+
+def _config_stages(config, stages):
+    """the KISSConfig (default: load_config(); voxel size defaulted to max_range / 100 as the pipeline does) and the
+    stages in metres (default: DEFAULT_STAGES_VOXELS times the voxel size) -> (cfg, voxel size, stages)"""
+    cfg = config if config is not None else load_config()
+    if cfg.mapping.voxel_size is None:
+        cfg.mapping.voxel_size = float(cfg.data.max_range / 100.0)
+    v = float(cfg.mapping.voxel_size)
+    stages = [(d * v, k * v) for d, k in DEFAULT_STAGES_VOXELS] if stages is None else [tuple(s) for s in stages]
+    if not stages or any(len(s) != 2 for s in stages):
+        raise ValueError("stages: one or more pairs (max_correspondence_distance, kernel_scale)")
+    return cfg, v, stages
+
+
+def _run_stages(rig: Rig, stages, call):
+    """call(rig, max_dist, kscale) -> (extrinsics (S, 4, 4), reports) once per stage, each stage on the rig the last
+    one returned -> (the calibrated Rig, the last extrinsics, the last reports, iterations summed over the stages)"""
+    cur = rig
+    iters = np.zeros(rig.n_sensors, dtype=np.int64)
+    for max_dist, kscale in stages:
+        E, rep = call(cur, max_dist, kscale)
+        iters += [r.iterations for r in rep]
+        cur = Rig([Sensor(E[j], s.min_range, s.max_range) for j, s in enumerate(rig.sensors)])
+    return cur, E, rep, iters
+
+
+def _fit_and_constraints(r):
+    return (_fit_of(r.fit.n_correspondences, r.fit.n_source, r.fit.sum_sq_residual, np.array(r.fit.JTJ[:])),
+            _from_struct(r.constraints))
 
 
 def _crop(points, sensor: Sensor) -> np.ndarray:
@@ -97,28 +148,10 @@ def calibrate_rig(frames, rig: Rig, poses=None, reference: int = 0, refine=None,
     ``stages``: (max_correspondence_distance, kernel_scale) pairs in metres, one kb_calibrate_rig call each, every
     one starting from the last one's result (default: DEFAULT_STAGES_VOXELS times the voxel size)."""
     _check_rig(rig)
-    S = rig.n_sensors
     frames = list(frames)
-    K = len(frames)
-    for f in frames:
-        if len(f) != S:
-            raise ValueError(f"a frame of this rig has {S} scans, not {len(f)}")
-    if not 0 <= int(reference) < S:
-        raise ValueError(f"reference {reference} is not a sensor of this {S}-sensor rig")
-    reference = int(reference)
-    sel = [j != reference for j in range(S)] if refine is None else [False] * S
-    if refine is not None:
-        for j in refine:
-            if not 0 <= int(j) < S:
-                raise ValueError(f"refine: {j} is not a sensor of this {S}-sensor rig")
-            sel[int(j)] = True
-    cfg = config if config is not None else load_config()
-    if cfg.mapping.voxel_size is None:
-        cfg.mapping.voxel_size = float(cfg.data.max_range / 100.0)
-    v = float(cfg.mapping.voxel_size)
-    stages = [(d * v, k * v) for d, k in DEFAULT_STAGES_VOXELS] if stages is None else [tuple(s) for s in stages]
-    if not stages or any(len(s) != 2 for s in stages):
-        raise ValueError("stages: one or more pairs (max_correspondence_distance, kernel_scale)")
+    S, K, reference = _check_run(rig, frames, reference)
+    sel = _flags(refine, S, [j != reference for j in range(S)], "refine")
+    cfg, v, stages = _config_stages(config, stages)
     if voxel_map is not None and poses is None:
         raise ValueError("a caller's voxel_map needs the poses in its frame")
     if poses is None:
@@ -149,17 +182,10 @@ def calibrate_rig(frames, rig: Rig, poses=None, reference: int = 0, refine=None,
     flat = [a for f in sources for a in f]
     ptrs = [a.ctypes.data if len(a) else None for a in flat]
     sizes = [len(a) for a in flat]
-    cur = rig
-    iters = np.zeros(S, dtype=np.int64)
-    for max_dist, kscale in stages:
-        E, rep = _calibrate(voxel_map, poses, cur, ptrs, sizes, 0, sel, max_dist, kscale,  # (0: KB_FRAMES_HOST_F64)
-                            cfg.registration.max_num_iterations, cfg.registration.convergence_criterion)
-        iters += [r.iterations for r in rep]
-        cur = Rig([Sensor(E[j], s.min_range, s.max_range) for j, s in enumerate(rig.sensors)])
-    sensors = [SensorCalibration(int(iters[j]), bool(r.converged),
-                                 _fit_of(r.fit.n_correspondences, r.fit.n_source, r.fit.sum_sq_residual,
-                                         np.array(r.fit.JTJ[:])),
-                                 _from_struct(r.constraints)) for j, r in enumerate(rep)]
+    cur, E, rep, iters = _run_stages(rig, stages, lambda cur, max_dist, kscale: _calibrate(
+        voxel_map, poses, cur, ptrs, sizes, 0, sel, max_dist, kscale,  # (0: KB_FRAMES_HOST_F64)
+        cfg.registration.max_num_iterations, cfg.registration.convergence_criterion))
+    sensors = [SensorCalibration(int(iters[j]), bool(r.converged), *_fit_and_constraints(r)) for j, r in enumerate(rep)]
     return RigCalibration(cur, E, sensors)
 
 
@@ -174,20 +200,17 @@ def _calibrate_clocks(voxel_map: VoxelHashMap, trajectory: Motion, rig: Rig, ptr
     if KS % S or len(sizes) != KS or len(stamps) != KS or len(stamp_offsets) != KS:
         raise ValueError(f"{len(ptrs)} arrays are not frames of {S} sensors with stamps and stamp offsets")
     stamps = [np.ascontiguousarray(np.asarray(t, dtype=np.float64).ravel()) for t in stamps]
-    X = (C.c_void_p * max(KS, 1))(*[C.c_void_p(int(p)) if p else None for p in ptrs])
-    n = (N.sz * max(KS, 1))(*sizes)
-    T = (C.c_void_p * max(KS, 1))(*[t.ctypes.data if t.size else None for t in stamps])
-    nt = (N.sz * max(KS, 1))(*[t.size for t in stamps])
+    X, n = _frame_arrays(ptrs, sizes)
+    T, nt = _frame_arrays([t.ctypes.data if t.size else None for t in stamps], [t.size for t in stamps])
     so = (N.dbl * max(KS, 1))(*[float(o) for o in stamp_offsets])
-    flags = lambda f: None if f is None else (N.i32 * S)(*[int(bool(r)) for r in f])
     o0 = None if time_offsets is None else (N.dbl * S)(*[float(o) for o in time_offsets])
     opt = N.RigClockCalibrationOptions(float(max_dist), float(kscale), int(max_iter), float(conv), float(tconv))
     E = np.empty((S, 4, 4))
     o = np.empty(S)
     rep = (N.SensorClockCalibration * S)()
     m = trajectory._struct(0.0)  # (end_time is not used)
-    check_value(N.lib().kb_calibrate_rig_clocks(voxel_map._h, C.byref(m), rig._structs, S, flags(refine),
-                                                flags(refine_time), o0, X, n, T, nt, so, KS // S, int(layout),
+    check_value(N.lib().kb_calibrate_rig_clocks(voxel_map._h, C.byref(m), rig._structs, S, _flag_array(refine, S),
+                                                _flag_array(refine_time, S), o0, X, n, T, nt, so, KS // S, int(layout),
                                                 C.byref(opt), N.ptr(E), N.ptr(o), rep))
     return E, o, list(rep)
 
@@ -281,32 +304,17 @@ def calibrate_rig_clocks(frames, timestamps, stamp_offsets, rig: Rig, trajectory
     sensor's range and downsampled in its own frame with the pipeline's source rule; each kept point keeps its stamp.
     To register with the result, add ``time_offsets[j]`` to sensor j's ``stamp_offsets`` (and use ``rig``)."""
     _check_rig(rig)
-    S = rig.n_sensors
     frames = list(frames)
-    K = len(frames)
     timestamps = list(timestamps)
     stamp_offsets = [[float(o) for o in f] for f in stamp_offsets]
-    if len(timestamps) != K or len(stamp_offsets) != K:
-        raise ValueError("frames, timestamps and stamp_offsets differ in length")
-    for f, t, o in zip(frames, timestamps, stamp_offsets):
-        if len(f) != S or len(t) != S or len(o) != S:
-            raise ValueError(f"a frame of this rig has {S} scans, stamp arrays and stamp offsets")
-    if not 0 <= int(reference) < S:
-        raise ValueError(f"reference {reference} is not a sensor of this {S}-sensor rig")
-    reference = int(reference)
+    S, K, reference = _check_run(rig, frames, reference, timestamps, stamp_offsets)
     others = [j != reference for j in range(S)]
     sel = _flags(refine, S, others, "refine")
     sel_t = _flags(refine_time, S, others, "refine_time")
     o0 = np.zeros(S) if time_offsets is None else np.array(time_offsets, dtype=np.float64).reshape(-1)
     if o0.shape != (S,):
         raise ValueError(f"time_offsets must hold {S} offsets")
-    cfg = config if config is not None else load_config()
-    if cfg.mapping.voxel_size is None:
-        cfg.mapping.voxel_size = float(cfg.data.max_range / 100.0)
-    v = float(cfg.mapping.voxel_size)
-    stages = [(d * v, k * v) for d, k in DEFAULT_STAGES_VOXELS] if stages is None else [tuple(s) for s in stages]
-    if not stages or any(len(s) != 2 for s in stages):
-        raise ValueError("stages: one or more pairs (max_correspondence_distance, kernel_scale)")
+    cfg, v, stages = _config_stages(config, stages)
     if voxel_map is not None and trajectory is None:
         raise ValueError("a caller's voxel_map needs the trajectory in its frame")
     if trajectory is not None and not isinstance(trajectory, Motion):
@@ -347,20 +355,17 @@ def calibrate_rig_clocks(frames, timestamps, stamp_offsets, rig: Rig, trajectory
             src_ts.append(t[_first_rows(src, p)] if len(src) else np.empty(0))
     ptrs = [a.ctypes.data if len(a) else None for a in srcs]
     sizes = [len(a) for a in srcs]
-    cur, o = rig, o0.copy()
-    iters = np.zeros(S, dtype=np.int64)
-    for max_dist, kscale in stages:
+    o = o0.copy()
+
+    def stage(cur, max_dist, kscale):  # (each stage starts from the last one's offsets)
+        nonlocal o
         E, o, rep = _calibrate_clocks(voxel_map, trajectory, cur, ptrs, sizes, src_ts, offs, 0, sel, sel_t, o,
                                       max_dist, kscale, cfg.registration.max_num_iterations,
                                       cfg.registration.convergence_criterion, DEFAULT_TIME_CONVERGENCE)
-        iters += [r.iterations for r in rep]
-        cur = Rig([Sensor(E[j], s.min_range, s.max_range) for j, s in enumerate(rig.sensors)])
-    sensors = []
-    for j, r in enumerate(rep):
-        hoo = r.time_row[6]
-        sensors.append(SensorClockCalibration(int(iters[j]), bool(r.converged),
-                                              _fit_of(r.fit.n_correspondences, r.fit.n_source, r.fit.sum_sq_residual,
-                                                      np.array(r.fit.JTJ[:])),
-                                              _from_struct(r.constraints), float(r.time_schur),
-                                              float(r.time_schur / hoo) if hoo > 0 else 0.0))
+        return E, rep
+
+    cur, E, rep, iters = _run_stages(rig, stages, stage)
+    sensors = [SensorClockCalibration(int(iters[j]), bool(r.converged), *_fit_and_constraints(r), float(r.time_schur),
+                                      float(r.time_schur / r.time_row[6]) if r.time_row[6] > 0 else 0.0)
+               for j, r in enumerate(rep)]
     return RigClockCalibration(cur, E, o, sensors)
