@@ -867,6 +867,79 @@ struct kb_pose_graph_factor_info {
  * name: C and C++ refer to it as struct kb_pose_graph_factor_info) */
 int kb_pose_graph_factor_info(kb_pose_graph *g, struct kb_pose_graph_factor_info *out);
 
+/* ---- pose graph: adjustment to the planes of the map ----------------------------------------------------------------
+ * No reference counterpart. After loop closure the graph fits its edges, but each edge summarises a pair of keyframes by
+ * one measurement; this call aligns every keyframe's points with the planes the other keyframes' points form.
+ * Inputs: the graph's N nodes T_k and, per node, a cloud P_k of n_k >= 0 points p in the node's body frame, the clouds
+ * concatenated in node order: xyz[offsets[k] .. offsets[k + 1]) (offsets[N + 1], offsets[0] = 0, offsets[N] = n_points).
+ * Parameters: voxel size s, min_points m, planarity rho, point sigma [m], Cauchy scale c (in units of sigma; 0: squared
+ * loss), rounds R, round_tolerance.
+ * A round:
+ *   1. Planes from the others. Every point goes to the world frame at the current poses, q = T_k p, and into the voxel
+ *      floor(q / s) (the map's point_to_voxel). For each pair (voxel v, node k) of a free node k with points in v, the
+ *      points of v from all other nodes (fixed ones included) give the pair's plane, leave-one-out so that a keyframe is
+ *      never pulled toward itself: the pair counts when there are at least m of them and the eigenvalues of their
+ *      covariance (1/count) satisfy lambda_0 <= rho lambda_1 with lambda_1 > 0; its plane is n = the unit eigenvector of
+ *      lambda_0 and d = n^T c_bar (c_bar their mean). The moments are summed about the voxel's centre, per voxel and
+ *      per (voxel, node), and the leave-one-out moments are (the voxel's) - (the node's own).
+ *   2. Terms. Each point p of a free node k in a planar pair (v, k): r = n^T (T_k p) - d, s = r^2 / sigma^2, the cost
+ *      1/2 rho_c(s) (the edges' loss), the IRLS weight w = rho_c'(s), dr/dd_k = n^T R_k [I | -[p]x] (the graph's right
+ *      perturbation and tangent order). F = F_graph (edges and priors, unchanged) + 1/2 sum_points rho_c(s).
+ *   3. Levenberg-Marquardt with the planes held: kb_pose_graph_optimize_direct's loop and exact solve (options as
+ *      there), where H_kk gains sum J^T (w / sigma^2) J and g_k gains sum J^T (w / sigma^2) r, the damping is lambda diag
+ *      of the whole block, and every cost includes the plane terms. The plane terms touch diagonal blocks only, so the
+ *      symbolic analysis of the marginals is reused as it is.
+ * The rounds stop after R, when a round moves no node by more than round_tolerance (max |Log(T_before^-1 T_after)| over
+ * the free nodes, the largest component), or after a round without a planar pair: that round was exactly
+ * kb_pose_graph_optimize_direct (same poses and report, bit for bit), and another would only repeat it.
+ * The poses are written back into the graph as optimize writes them (fixed nodes untouched). The edges, priors and
+ * marginals keep their meaning: kb_pose_graph_marginals afterwards is of the graph's edges and priors alone, at the new
+ * poses (the cached factor is dropped).
+ * Determinism: no floating-point atomics; every sum is formed in a fixed order (a voxel's points are sorted stably by
+ * voxel key and summed per node in input order, the nodes in index order; the terms over fixed chunks of a node's
+ * points, folded in chunk order). The results are bit-identical from run to run and for every kb_set_grid_blocks.
+ * The points are uploaded once per call into buffers the graph owns; they grow as needed and are released by destroy.
+ * Checked before any device work, writing nothing on error (KB_ERR_INVALID_ARG): NULL g, p, or xyz / offsets where
+ * needed; a non-finite coordinate; offsets that do not rise monotonically from 0 to n_points, or n_points >= 2^31; a
+ * point whose voxel coordinate at the current poses lies outside [-2^19, 2^19) (half the packed key's range, so that
+ * the rounds cannot leave it); parameters out of range (below); the options as kb_pose_graph_optimize; the gauge as
+ * kb_pose_graph_optimize (plane terms do not connect nodes); rounds_out with rounds_cap < p->rounds; a graph whose
+ * factorization needs more than 2^30 block updates. Then KB_ERR_NO_DEVICE without a device. */
+typedef struct kb_plane_adjust_params {
+    double voxel_size;       /* s > 0 */
+    int min_points;          /* m >= 3 */
+    double planarity;        /* rho in [0, 1] */
+    double sigma;            /* > 0 [m] */
+    double robust_scale;     /* c >= 0 (units of sigma) */
+    int rounds;              /* R in [1, 1000] */
+    double round_tolerance;  /* >= 0 */
+} kb_plane_adjust_params;
+/* voxel_size s, min_points 5, planarity 0.1, sigma 0.2 s, robust_scale 3, rounds 20, round_tolerance 1e-4 (DESIGN.md
+ * §4.21 has the measurements behind them); needs no device */
+void kb_plane_adjust_params_default(kb_plane_adjust_params *p, double voxel_size);
+typedef struct kb_plane_round {
+    unsigned long long planar_pairs;     /* (voxel, free node) pairs with a plane */
+    unsigned long long points_used;      /* points with a plane */
+    double initial_cost, final_cost;     /* F (graph + planes) at the round's start and end, with its planes */
+    double final_plane_cost;             /* the plane part of final_cost */
+    int iterations, accepted;            /* LM steps, accepted steps */
+    int termination;                     /* KB_PG_* */
+    double max_change;                   /* max |Log(T_before^-1 T_after)| over the nodes */
+} kb_plane_round;
+typedef struct kb_plane_adjust_report {
+    int rounds;                          /* rounds run */
+    int converged;                       /* 1: stopped by round_tolerance or a round without a planar pair */
+    double initial_cost, final_cost;     /* of the first round's start and the last round's end */
+} kb_plane_adjust_report;
+/* report (may be NULL); rounds_out (kb_plane_round[rounds_cap], may be NULL) receives each round's record; node_rms and
+ * node_points (double[N] / unsigned long long[N], may be NULL) receive each node's RMS point-to-plane residual [m] and
+ * points with a plane at the returned poses with the last round's planes (0 and 0 for a node without any). o may be
+ * NULL (the defaults). */
+int kb_pose_graph_adjust_planes(kb_pose_graph *g, const double *xyz, size_t n_points, const size_t *offsets,
+                                const kb_plane_adjust_params *p, const kb_pose_graph_options *o,
+                                kb_plane_adjust_report *report, kb_plane_round *rounds_out, size_t rounds_cap,
+                                double *node_rms, unsigned long long *node_points);
+
 /* ---- free space: removing moving objects from a map ----------------------------------------------------------------
  * No reference counterpart. A map keeps everything the sensor ever hit, including a car that drove past or was parked
  * and left. The scans of a run that saw through such a place are evidence that it is free; this call counts that

@@ -115,6 +115,16 @@ int kb_pipeline_history_grid_stamps(const kb_pipeline *p, double *out, size_t ca
 /* 0: queued calls compute no frame's front end in the launch before it, every launch runs its own (default 1: frames
  * without timestamps are prefetched). Results do not change; the ICP team then runs without the front end beside it. */
 int kb_pipeline_debug_prefetch(kb_pipeline *p, int enabled);
+/* The plane terms of kb_pose_graph_adjust_planes alone, at the graph's current poses and without a step: the planes of
+ * one round (step 1), then per node H (double[N][36]) and g (double[N][6]), and per point its residual r (double[n],
+ * 0 without a plane) and its plane's id (int[n], -1: none; points share an id when they share a (voxel, node) pair).
+ * Every output may be NULL; arguments are checked as there. The poses do not change. */
+/* device time [ms] of the last kb_pose_graph_adjust_planes on g (CUDA events), summed over its rounds: ms[0] the plane
+ * fits, ms[1] the Levenberg-Marquardt launches */
+int kb_debug_pose_graph_plane_ms(const kb_pose_graph *g, float ms[2]);
+int kb_debug_pose_graph_plane_terms(kb_pose_graph *g, const double *xyz, size_t n_points, const size_t *offsets,
+                                    const kb_plane_adjust_params *p, double *H, double *grad, double *residual,
+                                    int *plane_id);
 
 #ifdef __cplusplus
 }

@@ -196,6 +196,24 @@ class FreeSpaceReport(C.Structure):
                                              "ray_point_tests")]
 
 
+class PlaneAdjustParams(C.Structure):
+    """kb_plane_adjust_params"""
+    _fields_ = [("voxel_size", dbl), ("min_points", i32), ("planarity", dbl), ("sigma", dbl), ("robust_scale", dbl),
+                ("rounds", i32), ("round_tolerance", dbl)]
+
+
+class PlaneRound(C.Structure):
+    """kb_plane_round: one round of kb_pose_graph_adjust_planes"""
+    _fields_ = [("planar_pairs", C.c_ulonglong), ("points_used", C.c_ulonglong), ("initial_cost", dbl),
+                ("final_cost", dbl), ("final_plane_cost", dbl), ("iterations", i32), ("accepted", i32),
+                ("termination", i32), ("max_change", dbl)]
+
+
+class PlaneAdjustReport(C.Structure):
+    """kb_plane_adjust_report"""
+    _fields_ = [("rounds", i32), ("converged", i32), ("initial_cost", dbl), ("final_cost", dbl)]
+
+
 class PoseGraphFactorInfo(C.Structure):
     """kb_pose_graph_factor_info"""
     _fields_ = [("free_nodes", sz), ("h_blocks", sz), ("l_blocks", sz), ("etree_height", sz), ("flops", dbl)]
@@ -353,6 +371,11 @@ SIGNATURES = {
     "kb_debug_pose_graph_symbolic": (i32, [vp, sz, C.POINTER(sz), vp, vp, vp]),
     "kb_debug_pose_graph_rows": (i32, [vp, sz, C.POINTER(sz), vp, vp]),
     "kb_debug_pose_graph_cov_ms": (i32, [vp, vp]),
+    "kb_plane_adjust_params_default": (None, [C.POINTER(PlaneAdjustParams), dbl]),
+    "kb_pose_graph_adjust_planes": (i32, [vp, vp, sz, vp, C.POINTER(PlaneAdjustParams), C.POINTER(PoseGraphOptions),
+                                          C.POINTER(PlaneAdjustReport), vp, sz, vp, vp]),
+    "kb_debug_pose_graph_plane_ms": (i32, [vp, vp]),
+    "kb_debug_pose_graph_plane_terms": (i32, [vp, vp, sz, vp, C.POINTER(PlaneAdjustParams), vp, vp, vp, vp]),
     "kb_free_space_params_default": (None, [C.POINTER(FreeSpaceParams), dbl]),
     "kb_map_free_space": (i32, [vp, vp, sz, vp, sz, vp, C.POINTER(FreeSpaceParams), vp, vp, vp,
                                 C.POINTER(FreeSpaceReport)]),

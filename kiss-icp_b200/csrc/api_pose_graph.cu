@@ -1,5 +1,5 @@
-// Host side of the pose graph and its marginal covariances (kb_pose_graph_* and their kb_debug_* calls). The kernels
-// are in pose_graph.cu, pose_graph_cov.cu and pose_graph_direct.cu.
+// Host side of the pose graph, its marginal covariances and its plane adjustment (kb_pose_graph_* and their kb_debug_*
+// calls). The kernels are in pose_graph.cu, pose_graph_cov.cu, pose_graph_direct.cu and plane_adjust.cu.
 #include <algorithm>
 #include <cmath>
 #include <memory>
@@ -10,6 +10,7 @@
 #include "../../include/kiss_icp_b200_debug.h"
 #include "host.cuh"
 #include "pose_graph.cuh"
+#include "plane_adjust.cuh"
 #include "pose_graph_cov.cuh"
 #include "se3.cuh"
 
@@ -60,6 +61,9 @@ struct kb_pose_graph {
     DBuf<int> cov_flag, cov_req, cov_path;
     DBuf<double> Lx, cov_X, cov_out;
     DBuf<double> dir_val, dir_chunk;  // kb_pose_graph_optimize_direct: per edge and node values, their chunk partials
+    PaBuffers pa;                     // kb_pose_graph_adjust_planes: the points, the fit and the plane terms
+    Event pev[3];                     // around a round's fit and its optimizer launch
+    float pa_ms[2] = {-1.0f, -1.0f};  // the last adjustment's fit and optimizer time, summed over its rounds
     Event cev[4];                    // around the last factorization and the last marginal solves (kb_debug_pose_graph_cov_ms)
     size_t n() const { return fixed.size(); }
     size_t m() const { return robust.size(); }
@@ -444,6 +448,47 @@ int kb_pose_graph_poses(const kb_pose_graph *g, double *poses, size_t cap, size_
 static int pg_symbolic(kb_pose_graph *g);
 static int pg_sym_upload(kb_pose_graph *g);
 
+// the exact-step optimizer's parameters (k_pgc_optimize, k_pa_optimize) over O->F.P as pg_upload left it: the symbolic
+// analysis on the device, L's blocks, the step and the chunk partials (pg_symbolic has run)
+static int pg_direct_params(kb_pose_graph *g, PgcOptimizeParams *out) {
+    const PgcSymbolic &S = g->sym;
+    const size_t N = g->n(), NF = g->m() + g->np();
+    cudaStream_t s = g->ex->stream;
+    PgcOptimizeParams &O = *out;
+    RET(pg_sym_upload(g));
+    const size_t V = std::max({N, NF, size_t(1)});
+    RET(g->Lx.ensure(std::max<size_t>(36 * S.blocks(), 1)));
+    RET(g->cov_flag.ensure(1));
+    RET(g->dir_val.ensure(2 * V));
+    RET(g->dir_chunk.ensure(2 * ((V + PGC_CHUNK - 1) / PGC_CHUNK)));
+    CK(cudaMemsetAsync(g->cov_flag.p, 0, sizeof(int), s));
+    PgcFactorParams &F = O.F;
+    F.nf = S.nf;
+    F.levels = S.levels();
+    F.n_blocks = static_cast<int>(S.blocks());
+    F.order = g->s_order.p;
+    F.lev_ptr = g->s_lev_ptr.p;
+    F.colptr = g->s_colptr.p;
+    F.brow = g->s_brow.p;
+    F.bcol = g->s_bcol.p;
+    F.hptr = g->s_hptr.p;
+    F.hedge = g->s_hedge.p;
+    F.uptr = g->s_uptr.p;
+    F.upd = g->s_upd.p;
+    F.Lx = g->Lx.p;
+    F.flag = g->cov_flag.p;
+    O.Fd = F;
+    O.Fd.P.hd = F.P.D;
+    O.rptr = g->s_rptr.p;
+    O.rblk = g->s_rblk.p;
+    O.pos = g->s_pos.p;
+    O.y = F.P.x;  // (6 N doubles of the PCG vectors: nf <= N)
+    O.val = g->dir_val.p;
+    O.chunk = g->dir_chunk.p;
+    O.stride = static_cast<int>(V);
+    return KB_OK;
+}
+
 // One optimizer launch between the graph's events (kb_debug_pose_graph_ms): PCG (k_pose_graph) or, `direct`, exact
 // steps (k_pgc_optimize). Then its result: the report, the free nodes' poses and s_e, w_e. Nothing is written to the
 // caller's buffers on error.
@@ -470,39 +515,7 @@ static int pg_optimize(kb_pose_graph *g, const kb_pose_graph_options *opt, kb_po
     RET(pg_upload(g, &pq, &O.F.P));
     pg_set_options(o, &O.F.P);
     cudaStream_t s = ex.stream;
-    if (direct) {
-        RET(pg_sym_upload(g));
-        const size_t V = std::max({N, NF, size_t(1)});
-        RET(g->Lx.ensure(std::max<size_t>(36 * S.blocks(), 1)));
-        RET(g->cov_flag.ensure(1));
-        RET(g->dir_val.ensure(2 * V));
-        RET(g->dir_chunk.ensure(2 * ((V + PGC_CHUNK - 1) / PGC_CHUNK)));
-        CK(cudaMemsetAsync(g->cov_flag.p, 0, sizeof(int), s));
-        PgcFactorParams &F = O.F;
-        F.nf = S.nf;
-        F.levels = S.levels();
-        F.n_blocks = static_cast<int>(S.blocks());
-        F.order = g->s_order.p;
-        F.lev_ptr = g->s_lev_ptr.p;
-        F.colptr = g->s_colptr.p;
-        F.brow = g->s_brow.p;
-        F.bcol = g->s_bcol.p;
-        F.hptr = g->s_hptr.p;
-        F.hedge = g->s_hedge.p;
-        F.uptr = g->s_uptr.p;
-        F.upd = g->s_upd.p;
-        F.Lx = g->Lx.p;
-        F.flag = g->cov_flag.p;
-        O.Fd = F;
-        O.Fd.P.hd = F.P.D;
-        O.rptr = g->s_rptr.p;
-        O.rblk = g->s_rblk.p;
-        O.pos = g->s_pos.p;
-        O.y = F.P.x;  // (6 N doubles of the PCG vectors: nf <= N)
-        O.val = g->dir_val.p;
-        O.chunk = g->dir_chunk.p;
-        O.stride = static_cast<int>(V);
-    }
+    if (direct) RET(pg_direct_params(g, &O));
     RET(events_on(g->ev, ex.device));
     CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
     ex.bar_dirty = true;
@@ -801,6 +814,272 @@ int kb_debug_pose_graph_cov_ms(const kb_pose_graph *g, float ms[2]) {
     CK(cudaEventElapsedTime(&m, g->cev[2].p, g->cev[3].p));
     ms[0] = f;
     ms[1] = m;
+    return KB_OK;
+}
+
+// ------------------------------------------------------------------------------- Pose graph: plane adjustment
+void kb_plane_adjust_params_default(kb_plane_adjust_params *p, double voxel_size) {
+    if (p) *p = kb_plane_adjust_params{voxel_size, 5, 0.1, 0.2 * voxel_size, 3.0, 20, 1e-4};
+}
+
+static int pa_params_check(const kb_plane_adjust_params &p) {
+    if (!(p.voxel_size > 0.0) || !std::isfinite(p.voxel_size)) return fail(KB_ERR_INVALID_ARG, "voxel_size must be finite and > 0");
+    if (p.min_points < 3) return fail(KB_ERR_INVALID_ARG, "min_points must be >= 3");
+    if (!(p.planarity >= 0.0 && p.planarity <= 1.0)) return fail(KB_ERR_INVALID_ARG, "planarity must be in [0, 1]");
+    if (!(p.sigma > 0.0) || !std::isfinite(p.sigma)) return fail(KB_ERR_INVALID_ARG, "sigma must be finite and > 0");
+    if (!(p.robust_scale >= 0.0) || !std::isfinite(p.robust_scale))
+        return fail(KB_ERR_INVALID_ARG, "robust_scale must be finite and >= 0");
+    if (p.rounds < 1 || p.rounds > 1000) return fail(KB_ERR_INVALID_ARG, "rounds must be in [1, 1000]");
+    if (!(p.round_tolerance >= 0.0) || !std::isfinite(p.round_tolerance))
+        return fail(KB_ERR_INVALID_ARG, "round_tolerance must be finite and >= 0");
+    return KB_OK;
+}
+
+// A call's points, checked, with each point's node and the chunks of PA_CHUNK points of every free node
+struct PaHost {
+    std::vector<int> node, cptr, cnode;
+    std::vector<int2> chunk;
+};
+static int pa_inputs(const kb_pose_graph *g, const double *xyz, size_t n, const size_t *off, const kb_plane_adjust_params *p,
+                     PaHost *h) {
+    if (!g || !p || !off || (n && !xyz)) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(pa_params_check(*p));
+    const size_t N = g->n();
+    if (n >= (size_t(1) << 31)) return fail(KB_ERR_INVALID_ARG, "n_points must be < 2^31");
+    if (off[0] != 0 || off[N] != n) return fail(KB_ERR_INVALID_ARG, "offsets must run from 0 to n_points (%zu)", n);
+    for (size_t k = 0; k < N; ++k)
+        if (off[k + 1] < off[k]) return fail(KB_ERR_INVALID_ARG, "offsets must not decrease (node %zu)", k);
+    const double lim = static_cast<double>(PA_HALF_RANGE);
+    for (size_t k = 0; k < N; ++k)
+        for (size_t i = off[k]; i < off[k + 1]; ++i) {
+            const double *a = xyz + 3 * i;
+            if (!std::isfinite(a[0]) || !std::isfinite(a[1]) || !std::isfinite(a[2]))
+                return fail(KB_ERR_INVALID_ARG, "point %zu is not finite", i);
+            const V3 q = se3_act(g->pose[k], V3{a[0], a[1], a[2]});
+            const double v[3] = {std::floor(q.x / p->voxel_size), std::floor(q.y / p->voxel_size), std::floor(q.z / p->voxel_size)};
+            for (double c : v)
+                if (!(c >= -lim && c < lim))
+                    return fail(KB_ERR_INVALID_ARG, "point %zu lies outside the voxel key's range ([-2^19, 2^19) voxels)", i);
+        }
+    h->node.resize(n);
+    h->cptr.assign(N + 1, 0);
+    h->chunk.clear();
+    h->cnode.clear();
+    for (size_t k = 0; k < N; ++k) {
+        for (size_t i = off[k]; i < off[k + 1]; ++i) h->node[i] = static_cast<int>(k);
+        if (!g->fixed[k])
+            for (size_t i = off[k]; i < off[k + 1]; i += PA_CHUNK) {
+                h->chunk.push_back(make_int2(static_cast<int>(i), static_cast<int>(std::min(off[k + 1], i + PA_CHUNK))));
+                h->cnode.push_back(static_cast<int>(k));
+            }
+        h->cptr[k + 1] = static_cast<int>(h->chunk.size());
+    }
+    return KB_OK;
+}
+
+// Everything up to the first round: the checks, the graph and the points on the device, the launch parameters
+static int pa_setup(kb_pose_graph *g, const double *xyz, size_t n, const size_t *off, const kb_plane_adjust_params *p,
+                    const kb_pose_graph_options *opt, PaOptimizeParams *A, int *grid, std::vector<double> *pq) {
+    PaHost h;
+    RET(pa_inputs(g, xyz, n, off, p, &h));
+    kb_pose_graph_options o;
+    RET(pg_options(opt, &o));
+    RET(pg_gauge_check(*g));
+    RET(pg_symbolic(g));
+    RET(require_device());
+    if (!g->ex) RET(make_exec(&g->ex, g->device, g->user_stream));
+    Exec &ex = *g->ex;
+    CK(cudaSetDevice(ex.device));
+    const size_t N = g->n(), NF = g->m() + g->np(), C = h.chunk.size();
+    int co_resident = 0;
+    CK(pa_optimize_max_grid(ex.sms, &co_resident));
+    *grid = pg_grid(ex, co_resident, std::max({N, NF, g->sym.blocks(), C}), PGC_BLOCK);
+    RET(pg_reserve(g, *grid));
+    *A = PaOptimizeParams{};
+    RET(pg_upload(g, pq, &A->O.F.P));
+    pg_set_options(o, &A->O.F.P);
+    RET(pg_direct_params(g, &A->O));
+    cudaStream_t s = ex.stream;
+    PaBuffers &b = g->pa;
+    RET(pa_reserve(b, n, N, C, s));
+    if (n) {
+        CK(cudaMemcpyAsync(b.xyz.p, xyz, 3 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(b.node.p, h.node.data(), n * sizeof(int), cudaMemcpyHostToDevice, s));
+    }
+    CK(cudaMemcpyAsync(b.cptr.p, h.cptr.data(), (N + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (C) {
+        CK(cudaMemcpyAsync(b.chunk.p, h.chunk.data(), C * sizeof(int2), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(b.cnode.p, h.cnode.data(), C * sizeof(int), cudaMemcpyHostToDevice, s));
+    }
+    PaTerms &T = A->T;
+    T.xyz = b.xyz.p;
+    T.node = b.node.p;
+    T.n = static_cast<int>(n);
+    T.cptr = b.cptr.p;
+    T.chunk = b.chunk.p;
+    T.cnode = b.cnode.p;
+    T.n_chunks = static_cast<int>(C);
+    T.plane_of = b.plane_of.p;
+    T.plane = b.plane.p;
+    T.cpart = b.cpart.p;
+    T.nh = b.nh.p;
+    T.ng = b.ng.p;
+    T.nstat = b.nstat.p;
+    T.inv_var = 1.0 / (p->sigma * p->sigma);
+    T.robust = p->robust_scale;
+    T.plane_cost = b.cost.p;
+    CK(cudaMemsetAsync(b.nstat.p, 0, 3 * std::max<size_t>(N, 1) * sizeof(double), s));
+    return KB_OK;
+}
+
+// the fit of one round at the poses on the device, then one k_pa_optimize launch, between the graph's events
+static int pa_round(kb_pose_graph *g, const PaOptimizeParams &A, const kb_plane_adjust_params &p, int grid) {
+    Exec &ex = *g->ex;
+    cudaStream_t s = ex.stream;
+    RET(events_on(g->pev, ex.device));
+    const PaFitArgs a{A.O.F.P.pose, A.O.F.P.fixed, p.voxel_size, p.planarity, p.min_points};
+    CK(cudaEventRecord(g->pev[0].p, s));
+    RET(pa_fit(g->pa, A.T, a, s));
+    CK(cudaMemsetAsync(ex.sc.bar, 0, BAR_WORDS * sizeof(unsigned), s));
+    ex.bar_dirty = true;
+    CK(cudaEventRecord(g->pev[1].p, s));
+    CK(pa_optimize_launch(A, grid, s));
+    ++ex.launches;
+    CK(cudaEventRecord(g->pev[2].p, s));
+    return KB_OK;
+}
+// after the stream ran: a round's times added to the call's
+static int pa_round_ms(kb_pose_graph *g, float ms[2]) {
+    float a = 0.0f, b = 0.0f;
+    CK(cudaEventElapsedTime(&a, g->pev[0].p, g->pev[1].p));
+    CK(cudaEventElapsedTime(&b, g->pev[1].p, g->pev[2].p));
+    ms[0] += a;
+    ms[1] += b;
+    return KB_OK;
+}
+
+int kb_pose_graph_adjust_planes(kb_pose_graph *g, const double *xyz, size_t n_points, const size_t *offsets,
+                                const kb_plane_adjust_params *p, const kb_pose_graph_options *o,
+                                kb_plane_adjust_report *report, kb_plane_round *rounds_out, size_t rounds_cap,
+                                double *node_rms, unsigned long long *node_points) {
+    if (!g || !p) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (rounds_out && rounds_cap < static_cast<size_t>(std::max(p->rounds, 0)))
+        return fail(KB_ERR_INVALID_ARG, "rounds_cap (%zu) is below rounds (%d)", rounds_cap, p->rounds);
+    PaOptimizeParams A;
+    int grid = 0;
+    std::vector<double> pq;
+    RET(pa_setup(g, xyz, n_points, offsets, p, o, &A, &grid, &pq));
+    Exec &ex = *g->ex;
+    cudaStream_t s = ex.stream;
+    const size_t N = g->n();
+    g->factored = false;  // (the poses move; Lx holds a damped system's factor)
+    std::vector<kb_plane_round> rec;
+    std::vector<double> stat(3 * N), prev(pq);
+    bool converged = false;
+    float ms[2] = {0.0f, 0.0f};
+    for (int r = 0; r < p->rounds; ++r) {
+        RET(pa_round(g, A, *p, grid));
+        kb_pose_graph_report rep{};
+        unsigned long long pairs = 0;
+        double plane_cost = 0.0;
+        CK(cudaMemcpyAsync(&rep, g->report.p, sizeof(rep), cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(&pairs, g->pa.count.p, sizeof(pairs), cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(&plane_cost, g->pa.cost.p, sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (N) {
+            CK(cudaMemcpyAsync(pq.data(), g->pose_d.p, 8 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(stat.data(), g->pa.nstat.p, 3 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
+        }
+        RET(ex.sync());
+        if (r == 0) pg_uploaded(g);
+        RET(pa_round_ms(g, ms));
+        kb_plane_round rd{};
+        rd.planar_pairs = pairs;
+        for (size_t k = 0; k < N; ++k) rd.points_used += static_cast<unsigned long long>(stat[3 * k + 2]);
+        rd.initial_cost = rep.initial_cost;
+        rd.final_cost = rep.final_cost;
+        rd.final_plane_cost = plane_cost;
+        rd.iterations = rep.iterations;
+        rd.accepted = rep.accepted;
+        rd.termination = rep.termination;
+        for (size_t k = 0; k < N; ++k) {
+            const double *a = &prev[8 * k], *b = &pq[8 * k];
+            const SE3 Ta{{a[0], a[1], a[2], a[3]}, {a[4], a[5], a[6]}}, Tb{{b[0], b[1], b[2], b[3]}, {b[4], b[5], b[6]}};
+            double d[6];
+            se3_log(se3_mul(se3_inverse(Ta), Tb), d);
+            for (double v : d) rd.max_change = std::max(rd.max_change, std::fabs(v));
+        }
+        rec.push_back(rd);
+        prev = pq;
+        if (pairs == 0 || rd.max_change <= p->round_tolerance) {
+            converged = true;
+            break;
+        }
+    }
+    for (size_t k = 0; k < N; ++k) {
+        if (g->fixed[k]) continue;
+        const double *v = &pq[8 * k];
+        g->pose[k] = SE3{{v[0], v[1], v[2], v[3]}, {v[4], v[5], v[6]}};
+        se3_to_matrix(g->pose[k], &g->mat[16 * k]);
+    }
+    g->pa_ms[0] = ms[0];
+    g->pa_ms[1] = ms[1];
+    if (report) {
+        kb_plane_adjust_report out{};
+        out.rounds = static_cast<int>(rec.size());
+        out.converged = converged ? 1 : 0;
+        out.initial_cost = rec.front().initial_cost;
+        out.final_cost = rec.back().final_cost;
+        *report = out;
+    }
+    if (rounds_out) std::copy(rec.begin(), rec.end(), rounds_out);
+    for (size_t k = 0; k < N; ++k) {
+        const double c = stat[3 * k + 2];
+        if (node_rms) node_rms[k] = c > 0.0 ? std::sqrt(stat[3 * k + 1] / c) : 0.0;
+        if (node_points) node_points[k] = static_cast<unsigned long long>(c);
+    }
+    return KB_OK;
+}
+
+int kb_debug_pose_graph_plane_ms(const kb_pose_graph *g, float ms[2]) {
+    if (!g || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (g->pa_ms[0] < 0.0f) return fail(KB_ERR_INVALID_ARG, "no plane adjustment has run on this graph");
+    ms[0] = g->pa_ms[0];
+    ms[1] = g->pa_ms[1];
+    return KB_OK;
+}
+
+int kb_debug_pose_graph_plane_terms(kb_pose_graph *g, const double *xyz, size_t n_points, const size_t *offsets,
+                                    const kb_plane_adjust_params *p, double *H, double *grad, double *residual,
+                                    int *plane_id) {
+    kb_pose_graph_options o;
+    kb_pose_graph_options_default(&o);
+    o.max_iterations = 0;  // (lm_optimize linearizes at the current poses and takes no step)
+    PaOptimizeParams A;
+    int grid = 0;
+    std::vector<double> pq;
+    RET(pa_setup(g, xyz, n_points, offsets, p, &o, &A, &grid, &pq));
+    Exec &ex = *g->ex;
+    cudaStream_t s = ex.stream;
+    const size_t N = g->n(), n = n_points;
+    RET(pa_round(g, A, *p, grid));
+    CK(pa_residuals_launch(A.T, A.O.F.P.pose, g->pa.resid.p, s));
+    std::vector<double> h(36 * N), gr(6 * N), r(n);
+    std::vector<int> id(n);
+    if (N) {
+        CK(cudaMemcpyAsync(h.data(), g->pa.nh.p, 36 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(gr.data(), g->pa.ng.p, 6 * N * sizeof(double), cudaMemcpyDeviceToHost, s));
+    }
+    if (n) {
+        CK(cudaMemcpyAsync(r.data(), g->pa.resid.p, n * sizeof(double), cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(id.data(), g->pa.plane_of.p, n * sizeof(int), cudaMemcpyDeviceToHost, s));
+    }
+    RET(ex.sync());
+    pg_uploaded(g);
+    g->factored = false;
+    if (H) std::copy(h.begin(), h.end(), H);
+    if (grad) std::copy(gr.begin(), gr.end(), grad);
+    if (residual) std::copy(r.begin(), r.end(), residual);
+    if (plane_id) std::copy(id.begin(), id.end(), plane_id);
     return KB_OK;
 }
 

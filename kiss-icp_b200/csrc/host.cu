@@ -11,7 +11,7 @@
 // (device_ops.cuh: watchdog_arm), named after its file; and where api.cu's module keeps its phase marks (g_kb_marks)
 using WatchdogArm = cudaError_t(unsigned *d_host_words, const unsigned *init);
 WatchdogArm core_watchdog, report_watchdog, relocalize_watchdog, probe_watchdog, pose_graph_watchdog, pose_graph_cov_watchdog,
-    pose_graph_direct_watchdog, free_space_watchdog, degeneracy_watchdog, calib_watchdog;
+    pose_graph_direct_watchdog, free_space_watchdog, degeneracy_watchdog, calib_watchdog, plane_adjust_watchdog;
 const void *phase_marks_symbol();
 #pragma GCC visibility pop
 
@@ -45,7 +45,8 @@ int device_count() {
 
 WatchdogArm *const kWatchdogs[] = {core_watchdog,           report_watchdog,            relocalize_watchdog, probe_watchdog,
                                    pose_graph_watchdog,     pose_graph_cov_watchdog,    pose_graph_direct_watchdog,
-                                   free_space_watchdog,     degeneracy_watchdog,        calib_watchdog};
+                                   free_space_watchdog,     degeneracy_watchdog,        calib_watchdog,
+                                   plane_adjust_watchdog};
 
 // the device watchdog's report (device_ops.cuh): mapped host words per device, checked after every synchronisation
 struct WatchdogHost {

@@ -14,6 +14,9 @@ odometry frame into the corrected map frame, so the odometry pipeline itself is 
         if lc.add(pre, odometry.last_pose) is not None:
             lc.optimize()
     current = lc.correction @ odometry.last_pose
+
+adjust() then aligns the keyframes with the planes of their own map (PoseGraph.adjust_to_planes), so that two passes
+of one wall fall on one plane.
 """
 from __future__ import annotations
 
@@ -25,7 +28,7 @@ import numpy as np
 from .config import KISSConfig
 from .mapping import VoxelHashMap
 from .places import PlaceDatabase, PlaceDescriptorParams
-from .pose_graph import PoseGraph, PoseGraphOptions, PoseGraphReport
+from .pose_graph import PlaneAdjustmentParams, PlaneAdjustmentReport, PoseGraph, PoseGraphOptions, PoseGraphReport
 from .registration import get_registration
 from .voxelization import voxel_down_sample
 
@@ -169,6 +172,15 @@ class LoopCloser:
         """optimize the keyframe graph from its current poses (PoseGraph.optimize; options.linear_solver="cholesky"
         solves every step exactly, which pays on graphs with loops)"""
         return self._graph.optimize(options)
+
+    def adjust(self, params: PlaneAdjustmentParams | None = None,
+               options: PoseGraphOptions | None = None) -> PlaneAdjustmentReport:
+        """adjust the keyframe poses to the planes of their own map (PoseGraph.adjust_to_planes) with every keyframe's
+        frame_downsample; params None: the defaults at the config's voxel size. Run it after optimize(): poses,
+        correction, global_map() and place_database() then reflect the adjusted poses."""
+        if params is None:
+            params = PlaneAdjustmentParams(self.config.mapping.voxel_size)
+        return self._graph.adjust_to_planes([c[1] for c in self._clouds], params, options)
 
     # -- corrected products -----------------------------------------------------------------------------------------
     def global_map(self) -> VoxelHashMap:

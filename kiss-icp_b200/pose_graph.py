@@ -9,7 +9,8 @@ may be added afterwards and optimize() called again (the online use of loop clos
 Priors anchor nodes to absolute measurements: add_pose_prior() (a surveyed or relocalized pose) and
 add_position_prior() (a GNSS antenna position through a lever arm); a graph with priors needs no fixed node.
 marginal_covariances() and joint_marginal_covariances() say how well the poses are known: blocks of H^-1 at the
-current poses, from a sparse block Cholesky factorization on the device.
+current poses, from a sparse block Cholesky factorization on the device. adjust_to_planes() aligns every node's point
+cloud with the planes the other nodes' points form (point-to-plane terms in the same Levenberg-Marquardt, exact steps).
 """
 from __future__ import annotations
 
@@ -87,6 +88,91 @@ class PoseGraphFactorInfo:
     l_blocks: int
     etree_height: int
     flops: float
+
+
+@dataclass
+class PlaneAdjustmentParams:
+    """kb_plane_adjust_params. voxel_size [m] is required; a field left as None takes its default for that voxel size
+    s: min_points 5, planarity 0.1 (lambda_0 <= planarity lambda_1), sigma 0.2 s [m], robust_scale 3 (Cauchy, in units
+    of sigma; 0: squared loss), rounds 20, round_tolerance 1e-4 (DESIGN.md §4.21)."""
+    voxel_size: float
+    min_points: int | None = None
+    planarity: float | None = None
+    sigma: float | None = None
+    robust_scale: float | None = None
+    rounds: int | None = None
+    round_tolerance: float | None = None
+
+    def resolve(self) -> "PlaneAdjustmentParams":
+        """every field set: the given ones as they are, the others from the voxel size"""
+        d = N.PlaneAdjustParams()
+        N.lib().kb_plane_adjust_params_default(C.byref(d), float(self.voxel_size))
+        out = PlaneAdjustmentParams(float(self.voxel_size))
+        for name, _ in N.PlaneAdjustParams._fields_[1:]:
+            v = getattr(self, name)
+            setattr(out, name, getattr(d, name) if v is None else v)
+        return out
+
+    def _struct(self):
+        r = self.resolve()
+        c = N.PlaneAdjustParams()
+        c.voxel_size = float(r.voxel_size)
+        for name in ("min_points", "rounds"):
+            v = operator.index(getattr(r, name))
+            if not -2 ** 31 <= v < 2 ** 31:
+                raise ValueError(f"{name} = {v} is out of range")
+            setattr(c, name, v)
+        for name in ("planarity", "sigma", "robust_scale", "round_tolerance"):
+            setattr(c, name, float(getattr(r, name)))
+        return c
+
+
+@dataclass
+class PlaneRound:
+    """one round of adjust_to_planes: planar (voxel, free node) pairs and the points with a plane; F (graph + planes)
+    at the round's start and end with its planes, the plane part of the end; LM steps, accepted steps and termination
+    (one of TERMINATIONS); max_change: max |Log(T_before^-1 T_after)| over the nodes"""
+    planar_pairs: int
+    points_used: int
+    initial_cost: float
+    final_cost: float
+    final_plane_cost: float
+    iterations: int
+    accepted: int
+    termination: str
+    max_change: float
+
+
+@dataclass
+class PlaneAdjustmentReport:
+    """rounds: one PlaneRound per round run; converged: stopped by round_tolerance or by a round without a planar
+    pair; initial_cost / final_cost: F at the first round's start and the last round's end; node_rms [m] and node_points:
+    each node's RMS point-to-plane residual and points with a plane at the returned poses (0 and 0 without any)"""
+    rounds: list
+    converged: bool
+    initial_cost: float
+    final_cost: float
+    node_rms: np.ndarray
+    node_points: np.ndarray
+
+
+def _clouds_arg(clouds, n_nodes):
+    """(xyz (n, 3), offsets (N + 1,)) of one cloud per node"""
+    clouds = list(clouds)
+    if len(clouds) != n_nodes:
+        raise ValueError(f"clouds must hold one cloud per node ({n_nodes}), not {len(clouds)}")
+    pts = []
+    for k, c in enumerate(clouds):
+        a = np.asarray(c, dtype=np.float64)
+        if a.size == 0:
+            a = a.reshape(0, 3)
+        if a.ndim != 2 or a.shape[1] != 3:
+            raise ValueError(f"cloud {k} must have the shape (n, 3), not {a.shape}")
+        pts.append(a)
+    off = np.zeros(n_nodes + 1, dtype=np.uintp)
+    off[1:] = np.cumsum([len(a) for a in pts], dtype=np.uint64)
+    xyz = np.ascontiguousarray(np.concatenate(pts) if pts else np.empty((0, 3)))
+    return xyz, off
 
 
 def _nodes_arg(nodes, shape_tail, what):
@@ -242,6 +328,44 @@ class PoseGraph:
                                termination=TERMINATIONS[r.termination], initial_cost=r.initial_cost,
                                final_cost=r.final_cost, lambda_=r.lambda_, chi2=chi2, weight=weight)
 
+    def adjust_to_planes(self, clouds, params: PlaneAdjustmentParams, options: PoseGraphOptions | None = None
+                         ) -> PlaneAdjustmentReport:
+        """align every node's cloud with the planes of the other nodes' clouds (kb_pose_graph_adjust_planes states
+        the problem): clouds is a list of one (n_k, 3) array per node, in the node's body frame. Rounds of a
+        leave-one-out plane fit per (voxel, node) and Levenberg-Marquardt with exact steps (options as for optimize();
+        linear_solver is not read). The poses are written back as optimize() writes them; marginals stay those of the
+        edges and priors. ValueError for a rejected argument, the graph unchanged."""
+        options = PoseGraphOptions() if options is None else options
+        n = len(self)
+        xyz, off = _clouds_arg(clouds, n)
+        prm = params._struct()
+        o = options._struct()
+        rep = N.PlaneAdjustReport()
+        rounds = (N.PlaneRound * max(prm.rounds, 1))()
+        rms = np.zeros(n)
+        pts = np.zeros(n, dtype=np.uint64)
+        check_value(N.lib().kb_pose_graph_adjust_planes(
+            self._h, N.ptr(xyz), len(xyz), off.ctypes.data_as(C.c_void_p), C.byref(prm), C.byref(o), C.byref(rep),
+            rounds, max(prm.rounds, 0), N.ptr(rms), N.ptr(pts)))
+        rec = [PlaneRound(planar_pairs=int(r.planar_pairs), points_used=int(r.points_used),
+                          initial_cost=r.initial_cost, final_cost=r.final_cost, final_plane_cost=r.final_plane_cost,
+                          iterations=r.iterations, accepted=r.accepted, termination=TERMINATIONS[r.termination],
+                          max_change=r.max_change) for r in rounds[:rep.rounds]]
+        return PlaneAdjustmentReport(rounds=rec, converged=bool(rep.converged), initial_cost=rep.initial_cost,
+                                     final_cost=rep.final_cost, node_rms=rms, node_points=pts)
+
+    def plane_terms(self, clouds, params: PlaneAdjustmentParams):
+        """the plane terms of one round at the current poses, without a step (kb_debug_pose_graph_plane_terms):
+        (H (N, 6, 6), g (N, 6), residual (n,), plane_id (n,)) over the concatenated clouds; the poses do not change"""
+        n = len(self)
+        xyz, off = _clouds_arg(clouds, n)
+        prm = params._struct()
+        H, g = np.zeros((n, 6, 6)), np.zeros((n, 6))
+        r, pid = np.zeros(len(xyz)), np.zeros(len(xyz), dtype=np.int32)
+        check_value(N.lib().kb_debug_pose_graph_plane_terms(self._h, N.ptr(xyz), len(xyz), off.ctypes.data_as(C.c_void_p),
+                                                            C.byref(prm), N.ptr(H), N.ptr(g), N.ptr(r), N.ptr(pid)))
+        return H, g, r, pid
+
     def marginal_covariances(self, nodes=None) -> np.ndarray:
         """the (n, 6, 6) marginal covariances Sigma_kk of ``nodes`` (None: every node) at the current poses: blocks of
         H^-1, tangent order (translation, rotation) of the right perturbation T_k Exp(d_k); zero for a fixed node. The
@@ -285,6 +409,13 @@ class PoseGraph:
         """device time [ms] of the last numeric factorization and of the last marginal solves (CUDA events)"""
         ms = (C.c_float * 2)()
         N.check(N.lib().kb_debug_pose_graph_cov_ms(self._h, ms))
+        return float(ms[0]), float(ms[1])
+
+    def plane_kernel_ms(self) -> tuple[float, float]:
+        """device time [ms] of the last adjust_to_planes() (CUDA events), summed over its rounds: the plane fits and
+        the Levenberg-Marquardt launches"""
+        ms = (C.c_float * 2)()
+        N.check(N.lib().kb_debug_pose_graph_plane_ms(self._h, ms))
         return float(ms[0]), float(ms[1])
 
     def kernel_ms(self) -> float:
