@@ -706,6 +706,26 @@ typedef struct kb_place_match {
  * NULL) receive every searched entry's distance and shift, in entry order. */
 int kb_place_query(kb_place_db *db, const double *xyz, size_t n, int max_entry, double separation, int top_k,
                    kb_place_match *out, size_t *n_out, double *entry_distances, int *entry_shifts);
+typedef struct kb_place_match_report {
+    size_t queries, entries; /* Q, and the entries of db */
+    size_t pairs;            /* (query, entry) pairs searched: the sum of the queries' ranges */
+    size_t fallbacks;        /* queries whose walk read back their whole row */
+    size_t chunks;           /* device passes: the queries are split so that a chunk's pairs stay within a fixed budget */
+} kb_place_match_report;
+/* Every entry of `queries` (Q of them, its unit columns and masks; `queries` may be db itself) as a query of db:
+ * out[q][top_k] and n_out[q] are, bit for bit, the matches kb_place_query gives for the cloud entry q was added from
+ * (entry, shift, yaw, distance, guess), with the same max_entry, separation and top_k. max_entry (int[Q], may be NULL:
+ * every entry): max_entry[q] < 0 searches every entry, otherwise [0, min(max_entry[q], N)); an empty range gives
+ * n_out[q] = 0 (unlike kb_place_query, it fails no call). Q = 0 does nothing.
+ * On the device every (query, entry) pair's distance and shift are computed as kb_place_query computes them, and each
+ * query's pairs are sorted by (distance, entry); the first 8 top_k of them (all, when fewer) are read back and walked
+ * as kb_place_query walks its entries. A query whose walk uses them up with fewer than top_k matches while entries
+ * remain reads back its whole row and walks that (report->fallbacks). report (may be NULL) receives the counts.
+ * KB_ERR_INVALID_ARG for top_k outside [1, 256], a separation that is negative or not finite, NULL out, n_out, db or
+ * queries, databases of different place parameters or on different devices; every check is made before any device
+ * work, and on error nothing is written. */
+int kb_place_db_match(kb_place_db *db, const kb_place_db *queries, const int *max_entry, double separation, int top_k,
+                      kb_place_match *out, int *n_out, kb_place_match_report *report);
 typedef struct kb_place_search {
     int top_k, max_entry;   /* as kb_place_query */
     double separation;      /* metres, >= 0: of the candidate walk and of the runner-up */

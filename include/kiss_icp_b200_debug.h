@@ -44,6 +44,15 @@ int kb_debug_fast_rcp_dev(const double *x, size_t n, double *out);
 int kb_debug_reloc_score_ms(const kb_registration *reg, float *ms);
 /* time of the last k_place_distance launch of a kb_place_query or kb_place_relocalize on db [ms] (CUDA events) */
 int kb_debug_place_distance_ms(const kb_place_db *db, float *ms);
+/* device time of the last kb_place_db_match on db [ms] (CUDA events), summed over its chunks: ms[0] the k_place_match
+ * launches, ms[1] the sorts; KB_ERR_INVALID_ARG before the first */
+int kb_debug_place_match_ms(const kb_place_db *db, float ms[2]);
+/* the most (query, entry) pairs a chunk of kb_place_db_match holds on this thread (a chunk always holds one query):
+ * 0 = the default (2^23), else at most 2^28. The results do not depend on it. */
+int kb_debug_place_match_chunk(size_t pairs);
+/* every pair's distance and shift of kb_place_db_match's kernel, every query of `queries` against every entry of db:
+ * dist[Q][N], shift[Q][N] (checks as kb_place_db_match's) */
+int kb_debug_place_match_pairs(kb_place_db *db, const kb_place_db *queries, double *dist, int *shift);
 /* time of the last kb_pose_graph_optimize or kb_pose_graph_optimize_direct launch on g [ms] (CUDA events);
  * KB_ERR_INVALID_ARG before the first */
 int kb_debug_pose_graph_ms(const kb_pose_graph *g, float *ms);

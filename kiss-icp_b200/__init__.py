@@ -10,7 +10,7 @@ from .mapping import VoxelHashMap, get_voxel_hash_map  # noqa: F401
 from .places import PlaceDatabase, PlaceDescriptorParams, PlaceMatch, PlaceRelocalizationResult  # noqa: F401
 from .pose_graph import PoseGraph, PoseGraphFactorInfo, PoseGraphOptions, PoseGraphReport  # noqa: F401
 from .pose_graph import PlaneAdjustmentParams, PlaneAdjustmentReport, PlaneRound  # noqa: F401
-from .loop_closure import LoopCloser, LoopClosure  # noqa: F401
+from .loop_closure import LoopCloser, LoopClosure, SessionMatch, SessionMerge, SessionMergeReport, session_consensus  # noqa: F401
 from .preprocess import Preprocessor, get_preprocessor  # noqa: F401
 from .registration import Registration, get_registration  # noqa: F401
 from .relocalization import RelocalizationResult, RelocalizationSearch  # noqa: F401

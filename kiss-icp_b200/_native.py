@@ -160,6 +160,11 @@ class PlaceMatch(C.Structure):
     _fields_ = [("entry", i32), ("shift", i32), ("yaw", dbl), ("distance", dbl), ("guess", dbl * 16)]
 
 
+class PlaceMatchReport(C.Structure):
+    """kb_place_match_report: the counts of a kb_place_db_match"""
+    _fields_ = [("queries", sz), ("entries", sz), ("pairs", sz), ("fallbacks", sz), ("chunks", sz)]
+
+
 class PlaceSearch(C.Structure):
     """kb_place_search: the query and refinement of kb_place_relocalize"""
     _fields_ = [("top_k", i32), ("max_entry", i32), ("separation", dbl), ("max_correspondence_distance", dbl),
@@ -349,6 +354,10 @@ SIGNATURES = {
     "kb_place_query": (i32, [vp, vp, sz, i32, dbl, i32, vp, C.POINTER(sz), vp, vp]),
     "kb_place_relocalize": (i32, [vp, vp, vp, sz, vp, sz, vp, C.POINTER(PlaceSearch), C.POINTER(PlaceResult), vp]),
     "kb_debug_place_distance_ms": (i32, [vp, C.POINTER(C.c_float)]),
+    "kb_place_db_match": (i32, [vp, vp, vp, dbl, i32, vp, vp, C.POINTER(PlaceMatchReport)]),
+    "kb_debug_place_match_ms": (i32, [vp, vp]),
+    "kb_debug_place_match_chunk": (i32, [sz]),
+    "kb_debug_place_match_pairs": (i32, [vp, vp, vp, vp]),
     "kb_pose_graph_create": (i32, [C.POINTER(vp)]),
     "kb_pose_graph_destroy": (i32, [vp]),
     "kb_pose_graph_add_node": (i32, [vp, vp, i32, C.POINTER(sz)]),

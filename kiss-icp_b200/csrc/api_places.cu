@@ -4,6 +4,7 @@
 #include <climits>
 #include <cmath>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <vector>
 
@@ -34,6 +35,14 @@ struct kb_place_db {
     DBuf<double> dist;              // [entries searched] of the last query
     DBuf<int> shift;
     Event ev[2];                    // around the last k_place_distance (kb_debug_place_distance_ms)
+    // kb_place_db_match's chunk: keys and values [queries][row] as k_place_match wrote them and sorted, the queries'
+    // ranges and segments, the sort's scratch
+    DBuf<unsigned long long> m_key, m_val, m_skey, m_sval;
+    DBuf<int> m_off;
+    DBuf<unsigned char> m_tmp;
+    Event mev[3];                   // around one chunk's k_place_match and sort
+    float match_ms[2] = {0.0f, 0.0f};  // of the last kb_place_db_match (kb_debug_place_match_ms)
+    bool matched = false;
     size_t cells() const { return static_cast<size_t>(prm.n_rings) * prm.n_sectors; }
 };
 
@@ -105,6 +114,41 @@ static int place_query_check(const double *xyz, size_t n, double separation, int
     if (!(separation >= 0.0) || !std::isfinite(separation)) return fail(KB_ERR_INVALID_ARG, "separation must be finite and >= 0");
     return KB_OK;
 }
+// The candidate walk of kb_place_query and kb_place_db_match: pairs o < n in (distance, entry) order, pair o being
+// entry[o] at dist[o] and shift[o], into *matches (cleared first). Returns the pairs it used.
+static size_t place_walk(const kb_place_db *db, size_t n, const int *entry, const double *dist, const int *shift,
+                         double separation, int top_k, std::vector<kb_place_match> *matches) {
+    const double width = place_sector_width(db->prm);
+    matches->clear();
+    size_t o = 0;
+    for (; o < n && matches->size() < static_cast<size_t>(top_k); ++o) {
+        const int i = entry[o];
+        const double *T = &db->poses[16 * static_cast<size_t>(i)];
+        bool near = false;
+        for (const kb_place_match &c : *matches) {
+            const double *U = &db->poses[16 * static_cast<size_t>(c.entry)];
+            if (std::hypot(T[3] - U[3], T[7] - U[7]) < separation) {
+                near = true;
+                break;
+            }
+        }
+        if (near) continue;
+        kb_place_match m{};
+        m.entry = i;
+        m.shift = shift[o];
+        m.yaw = m.shift * width;
+        m.distance = dist[o];
+        const double cs = std::cos(m.yaw), sn = std::sin(m.yaw);
+        const double Rz[9] = {cs, -sn, 0.0, sn, cs, 0.0, 0.0, 0.0, 1.0};
+        for (int r = 0; r < 3; ++r) {
+            for (int c = 0; c < 3; ++c) m.guess[4 * r + c] = (T[4 * r] * Rz[c] + T[4 * r + 1] * Rz[3 + c]) + T[4 * r + 2] * Rz[6 + c];
+            m.guess[4 * r + 3] = T[4 * r + 3];
+        }
+        for (int c = 0; c < 4; ++c) m.guess[12 + c] = T[12 + c];
+        matches->push_back(m);
+    }
+    return o;
+}
 // the query of xyz[n] against entries [0, M): every entry's distance and shift, then the candidate walk
 static int place_search(kb_place_db *db, const double *xyz, size_t n, int max_entry, double separation, int top_k,
                  std::vector<kb_place_match> *matches, std::vector<double> *dist, std::vector<int> *shift) {
@@ -132,34 +176,13 @@ static int place_search(kb_place_db *db, const double *xyz, size_t n, int max_en
     std::vector<int> order(M);
     for (size_t i = 0; i < M; ++i) order[i] = static_cast<int>(i);
     std::sort(order.begin(), order.end(), [&](int a, int b) { return (*dist)[a] != (*dist)[b] ? (*dist)[a] < (*dist)[b] : a < b; });
-    const double width = place_sector_width(db->prm);
-    matches->clear();
-    for (size_t o = 0; o < M && matches->size() < static_cast<size_t>(top_k); ++o) {
-        const int i = order[o];
-        const double *T = &db->poses[16 * static_cast<size_t>(i)];
-        bool near = false;
-        for (const kb_place_match &c : *matches) {
-            const double *U = &db->poses[16 * static_cast<size_t>(c.entry)];
-            if (std::hypot(T[3] - U[3], T[7] - U[7]) < separation) {
-                near = true;
-                break;
-            }
-        }
-        if (near) continue;
-        kb_place_match m{};
-        m.entry = i;
-        m.shift = (*shift)[i];
-        m.yaw = m.shift * width;
-        m.distance = (*dist)[i];
-        const double cs = std::cos(m.yaw), sn = std::sin(m.yaw);
-        const double Rz[9] = {cs, -sn, 0.0, sn, cs, 0.0, 0.0, 0.0, 1.0};
-        for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) m.guess[4 * r + c] = (T[4 * r] * Rz[c] + T[4 * r + 1] * Rz[3 + c]) + T[4 * r + 2] * Rz[6 + c];
-            m.guess[4 * r + 3] = T[4 * r + 3];
-        }
-        for (int c = 0; c < 4; ++c) m.guess[12 + c] = T[12 + c];
-        matches->push_back(m);
+    std::vector<double> od(M);
+    std::vector<int> os(M);
+    for (size_t o = 0; o < M; ++o) {
+        od[o] = (*dist)[order[o]];
+        os[o] = (*shift)[order[o]];
     }
+    place_walk(db, M, order.data(), od.data(), os.data(), separation, top_k, matches);
     return KB_OK;
 }
 
@@ -364,6 +387,194 @@ int kb_place_relocalize(kb_registration *reg, kb_place_db *db, const double *des
     }
     *out = r;
     if (candidates) std::copy(m.begin(), m.end(), candidates);
+    return KB_OK;
+}
+
+// kb_place_db_match reads back the first kMatchListFactor top_k pairs of each query's sorted row: the walk skips a pair
+// only for an entry within `separation` of a candidate, and keyframes ~2 m apart put a handful of entries within a
+// candidate's separation, so 8 top_k pairs fill the list in all but crowded databases (which read their whole row).
+static constexpr size_t kMatchListFactor = 8;
+static constexpr size_t kMatchChunkPairs = size_t(1) << 23;  // 8 Mi pairs a chunk: 256 MiB of keys and values
+static constexpr size_t kMatchMaxChunkQueries = 262140;      // place_match's limit
+thread_local size_t tl_match_chunk_pairs = 0;                 // kb_debug_place_match_chunk (0: kMatchChunkPairs)
+
+static double place_key_distance(unsigned long long k) {
+    const unsigned long long b = (k >> 63) ? k & ~(1ull << 63) : ~k;
+    double d;
+    std::memcpy(&d, &b, sizeof d);
+    return d;
+}
+// k_place_match of every query of qdb against its entries [0, ends[q]) of db, in chunks of queries whose rows stay within
+// the chunk budget; with `sort` each row's range is sorted stably by distance. chunk(q0, qc, row) then takes the chunk's
+// rows (db->m_skey / m_sval sorted, else m_key / m_val, row stride `row`) before the next chunk overwrites them.
+static int place_match_chunks(kb_place_db *db, const kb_place_db *qdb, const std::vector<int> &ends, bool sort,
+                              size_t *chunks, const std::function<int(size_t, size_t, size_t)> &chunk) {
+    Exec &ex = *db->ex;
+    const size_t Q = ends.size(), C = db->cells();
+    const int S = db->prm.n_sectors;
+    *chunks = 0;
+    db->match_ms[0] = db->match_ms[1] = 0.0f;
+    const size_t row = Q ? static_cast<size_t>(*std::max_element(ends.begin(), ends.end())) : 0;
+    if (row == 0) return KB_OK;
+    const size_t budget = tl_match_chunk_pairs ? tl_match_chunk_pairs : kMatchChunkPairs;
+    const size_t qmax = std::min({std::max<size_t>(1, budget / row), kMatchMaxChunkQueries, Q});
+    RET(db->m_key.ensure(qmax * row));
+    RET(db->m_val.ensure(qmax * row));
+    RET(db->m_off.ensure(3 * qmax));
+    if (sort) {
+        RET(db->m_skey.ensure(qmax * row));
+        RET(db->m_sval.ensure(qmax * row));
+    }
+    RET(events_on(db->mev, ex.device));
+    std::vector<int> off(3 * qmax);
+    for (size_t q0 = 0; q0 < Q; q0 += qmax) {
+        const size_t qc = std::min(qmax, Q - q0);
+        for (size_t q = 0; q < qc; ++q) {
+            off[q] = ends[q0 + q];                                        // the range searched
+            off[qmax + q] = static_cast<int>(q * row);                    // its segment in the chunk's rows
+            off[2 * qmax + q] = static_cast<int>(q * row) + ends[q0 + q];
+        }
+        CK(cudaMemcpyAsync(db->m_off.p, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice, ex.stream));
+        CK(cudaEventRecord(db->mev[0].p, ex.stream));
+        const int count = *std::max_element(off.begin(), off.begin() + qc);
+        CK(place_match(qdb->unit.p + q0 * C, qdb->mask.p + q0 * S, db->m_off.p, static_cast<int>(qc), count, db->unit.p,
+                       db->mask.p, db->prm.n_rings, S, row, db->m_key.p, db->m_val.p, ex.grid, ex.stream));
+        ++ex.launches;
+        CK(cudaEventRecord(db->mev[1].p, ex.stream));
+        if (sort) {
+            const int items = static_cast<int>(qc * row);
+            size_t bytes = 0;
+            CK(place_match_sort(nullptr, &bytes, db->m_key.p, db->m_skey.p, db->m_val.p, db->m_sval.p, items,
+                                static_cast<int>(qc), db->m_off.p + qmax, db->m_off.p + 2 * qmax, ex.stream));
+            RET(db->m_tmp.ensure(std::max<size_t>(bytes, 1)));
+            CK(place_match_sort(db->m_tmp.p, &bytes, db->m_key.p, db->m_skey.p, db->m_val.p, db->m_sval.p, items,
+                                static_cast<int>(qc), db->m_off.p + qmax, db->m_off.p + 2 * qmax, ex.stream));
+            ++ex.launches;
+        }
+        CK(cudaEventRecord(db->mev[2].p, ex.stream));
+        RET(chunk(q0, qc, row));  // (synchronizes the stream)
+        float a = 0.0f, b = 0.0f;
+        CK(cudaEventElapsedTime(&a, db->mev[0].p, db->mev[1].p));
+        CK(cudaEventElapsedTime(&b, db->mev[1].p, db->mev[2].p));
+        db->match_ms[0] += a;
+        db->match_ms[1] += b;
+        ++*chunks;
+    }
+    return KB_OK;
+}
+// the arguments kb_place_db_match and kb_debug_place_match_pairs share, once a device is there
+static int place_match_pair_check(const kb_place_db *db, const kb_place_db *queries) {
+    if (!db || !queries) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    const kb_place_params &a = db->prm, &b = queries->prm;
+    if (a.n_rings != b.n_rings || a.n_sectors != b.n_sectors || a.max_radius != b.max_radius || a.z_offset != b.z_offset)
+        return fail(KB_ERR_INVALID_ARG, "the databases have different place parameters");
+    if (db->ex->device != queries->ex->device) return fail(KB_ERR_INVALID_ARG, "the databases are on different devices");
+    return KB_OK;
+}
+
+int kb_place_db_match(kb_place_db *db, const kb_place_db *queries, const int *max_entry, double separation, int top_k,
+                      kb_place_match *out, int *n_out, kb_place_match_report *report) {
+    if (top_k < 1 || top_k > 256) return fail(KB_ERR_INVALID_ARG, "top_k must be in [1, 256]");
+    if (!(separation >= 0.0) || !std::isfinite(separation)) return fail(KB_ERR_INVALID_ARG, "separation must be finite and >= 0");
+    if (!out || !n_out) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(require_device());
+    RET(place_match_pair_check(db, queries));
+    CK(cudaSetDevice(db->ex->device));
+    const size_t Q = queries->n, N = db->n;
+    std::vector<int> ends(Q);
+    size_t pairs = 0;
+    for (size_t q = 0; q < Q; ++q) {
+        ends[q] = static_cast<int>(!max_entry || max_entry[q] < 0 ? N : std::min(static_cast<size_t>(max_entry[q]), N));
+        pairs += ends[q];
+    }
+    const size_t K = static_cast<size_t>(top_k);
+    std::vector<kb_place_match> res(Q * K);
+    std::vector<int> cnt(Q, 0);
+    size_t fallbacks = 0, chunks = 0;
+    std::vector<unsigned long long> hk, hv;
+    std::vector<int> entry, shift;
+    std::vector<double> dist;
+    std::vector<kb_place_match> m;
+    // decode pairs [0, n) of the host rows k / v and walk them into query q's result; returns the pairs walked
+    auto walk = [&](size_t q, const unsigned long long *k, const unsigned long long *v, size_t n) {
+        entry.resize(n);
+        shift.resize(n);
+        dist.resize(n);
+        for (size_t o = 0; o < n; ++o) {
+            entry[o] = static_cast<int>(v[o] >> 32);
+            shift[o] = static_cast<int>(v[o] & 0xffffffffu);
+            dist[o] = place_key_distance(k[o]);
+        }
+        const size_t used = place_walk(db, n, entry.data(), dist.data(), shift.data(), separation, top_k, &m);
+        std::copy(m.begin(), m.end(), res.begin() + q * K);
+        cnt[q] = static_cast<int>(m.size());
+        return used;
+    };
+    RET(place_match_chunks(db, queries, ends, true, &chunks, [&](size_t q0, size_t qc, size_t row) -> int {
+        Exec &ex = *db->ex;
+        const size_t L = std::min(row, kMatchListFactor * K);
+        hk.resize(qc * L);
+        hv.resize(qc * L);
+        CK(cudaMemcpy2DAsync(hk.data(), L * sizeof(unsigned long long), db->m_skey.p, row * sizeof(unsigned long long),
+                             L * sizeof(unsigned long long), qc, cudaMemcpyDeviceToHost, ex.stream));
+        CK(cudaMemcpy2DAsync(hv.data(), L * sizeof(unsigned long long), db->m_sval.p, row * sizeof(unsigned long long),
+                             L * sizeof(unsigned long long), qc, cudaMemcpyDeviceToHost, ex.stream));
+        RET(ex.sync());
+        std::vector<unsigned long long> fk, fv;
+        for (size_t q = 0; q < qc; ++q) {
+            const size_t M = static_cast<size_t>(ends[q0 + q]), n = std::min(L, M);
+            walk(q0 + q, &hk[q * L], &hv[q * L], n);
+            if (cnt[q0 + q] < top_k && n < M) {  // the list ran out: walk the whole row
+                fk.resize(M);
+                fv.resize(M);
+                CK(cudaMemcpyAsync(fk.data(), db->m_skey.p + q * row, M * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                                   ex.stream));
+                CK(cudaMemcpyAsync(fv.data(), db->m_sval.p + q * row, M * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                                   ex.stream));
+                RET(ex.sync());
+                walk(q0 + q, fk.data(), fv.data(), M);
+                ++fallbacks;
+            }
+        }
+        return KB_OK;
+    }));
+    db->matched = true;
+    std::copy(res.begin(), res.end(), out);
+    std::copy(cnt.begin(), cnt.end(), n_out);
+    if (report) *report = kb_place_match_report{Q, N, pairs, fallbacks, chunks};
+    return KB_OK;
+}
+
+int kb_debug_place_match_pairs(kb_place_db *db, const kb_place_db *queries, double *dist, int *shift) {
+    if (!dist || !shift) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    RET(require_device());
+    RET(place_match_pair_check(db, queries));
+    CK(cudaSetDevice(db->ex->device));
+    const size_t Q = queries->n, N = db->n;
+    const std::vector<int> ends(Q, static_cast<int>(N));
+    std::vector<unsigned long long> hk(Q * N), hv(Q * N);
+    size_t chunks = 0;
+    RET(place_match_chunks(db, queries, ends, false, &chunks, [&](size_t q0, size_t qc, size_t row) -> int {
+        CK(cudaMemcpyAsync(&hk[q0 * N], db->m_key.p, qc * row * sizeof(unsigned long long), cudaMemcpyDeviceToHost, db->ex->stream));
+        CK(cudaMemcpyAsync(&hv[q0 * N], db->m_val.p, qc * row * sizeof(unsigned long long), cudaMemcpyDeviceToHost, db->ex->stream));
+        return db->ex->sync();
+    }));
+    for (size_t i = 0; i < Q * N; ++i) {
+        dist[i] = place_key_distance(hk[i]);
+        shift[i] = static_cast<int>(hv[i] & 0xffffffffu);
+    }
+    return KB_OK;
+}
+int kb_debug_place_match_chunk(size_t pairs) {
+    if (pairs > (size_t(1) << 28)) return fail(KB_ERR_INVALID_ARG, "at most 2^28 pairs a chunk");
+    tl_match_chunk_pairs = pairs;
+    return KB_OK;
+}
+int kb_debug_place_match_ms(const kb_place_db *db, float ms[2]) {
+    if (!db || !ms) return fail(KB_ERR_INVALID_ARG, "NULL argument");
+    if (!db->matched) return fail(KB_ERR_INVALID_ARG, "no kb_place_db_match on this database yet");
+    ms[0] = db->match_ms[0];
+    ms[1] = db->match_ms[1];
     return KB_OK;
 }
 

@@ -20,3 +20,15 @@ cudaError_t place_columns(const double *raw, size_t count, int n_rings, int n_se
 // multiprocessor of a grid-sized launch); the results do not depend on it.
 cudaError_t place_distance(const double *q_unit, const unsigned char *q_mask, const double *unit, const unsigned char *mask,
                            int count, int n_rings, int n_sectors, double *dist, int *shift, int max_ctas, cudaStream_t s);
+// place_distance of n_q queries (q_unit + q entry, q_mask + q entry) at once, query q against the entries [0, q_end[q])
+// (count = the largest q_end): pair (q, e) into key[q row + e] (the distance as an unsigned key in its order: bits
+// inverted when negative, else the sign bit set) and val[q row + e] = e << 32 | shift. Every pair's distance and shift
+// are place_distance's; neither depends on max_ctas. n_q <= 262140.
+cudaError_t place_match(const double *q_unit, const unsigned char *q_mask, const int *q_end, int n_q, int count,
+                        const double *unit, const unsigned char *mask, int n_rings, int n_sectors, size_t row,
+                        unsigned long long *key, unsigned long long *val, int max_ctas, cudaStream_t s);
+// a stable sort of every segment [begin[q], end[q]) of (key, val) by key (cub::DeviceSegmentedSort); tmp NULL: only
+// *tmp_bytes is set
+cudaError_t place_match_sort(void *tmp, size_t *tmp_bytes, const unsigned long long *key, unsigned long long *sorted_key,
+                             const unsigned long long *val, unsigned long long *sorted_val, int n_items, int n_q,
+                             const int *begin, const int *end, cudaStream_t s);

@@ -154,6 +154,47 @@ class PlaceDatabase:
         m = _matches(buf, n.value)
         return (m, dist, shift) if return_distances else m
 
+    def match(self, queries: "PlaceDatabase | None" = None, top_k: int = 8, max_entry=None, separation: float = 3.0,
+              return_report: bool = False):
+        """every entry of ``queries`` (None: this database) as a query of this one, in one device search
+        (kb_place_db_match): one PlaceMatch list per query, each equal to what query() gives for the cloud that entry
+        was added from. max_entry: None (every entry), an int for all queries or a (Q,) array; < 0 searches every
+        entry, and an empty range gives an empty list. With return_report also the counts (N.PlaceMatchReport)."""
+        q = self if queries is None else queries
+        if not isinstance(q, PlaceDatabase):
+            raise TypeError(f"queries must be a PlaceDatabase, not {type(q).__name__}")
+        top_k = _int32(top_k, "top_k")
+        Q = len(q)
+        if max_entry is None:
+            me = None
+        else:
+            me = np.asarray(max_entry)
+            if me.ndim == 0:
+                me = np.full(Q, _int32(int(me), "max_entry"), dtype=np.int64)
+            if me.shape != (Q,) or not np.issubdtype(me.dtype, np.integer):
+                raise ValueError(f"max_entry must be None, an int or ({Q},) integers, not {me.dtype} {me.shape}")
+            if Q and (me.min() < -2 ** 31 or me.max() >= 2 ** 31):
+                raise ValueError("max_entry is out of range")
+            me = np.ascontiguousarray(me, dtype=np.int32)
+        buf = (N.PlaceMatch * max(Q * max(top_k, 1), 1))()
+        n = np.zeros(max(Q, 1), dtype=np.int32)
+        rep = N.PlaceMatchReport()
+        check_value(N.lib().kb_place_db_match(self._h, q._h, N.ptr(me) if me is not None else None, float(separation),
+                                              top_k, buf, N.ptr(n), C.byref(rep)))
+        K = max(top_k, 1)
+        out = [_matches(buf[i * K:(i + 1) * K], int(n[i])) for i in range(Q)]
+        return (out, rep) if return_report else out
+
+    def pair_distances(self, queries: "PlaceDatabase | None" = None):
+        """(distances (Q, N), shifts (Q, N)): every query's distance and shift to every entry, from match()'s kernel
+        (kb_debug_place_match_pairs)"""
+        q = self if queries is None else queries
+        Q, M = len(q), len(self)
+        d = np.empty((Q, M))
+        s = np.empty((Q, M), dtype=np.int32)
+        check_value(N.lib().kb_debug_place_match_pairs(self._h, q._h, N.ptr(d), N.ptr(s)))
+        return d, s
+
     def state_dict(self):
         """the database as numpy arrays (np.savez-safe): format_version, the parameters, descriptors (N, n_rings,
         n_sectors) and poses (N, 4, 4)"""
