@@ -2,6 +2,7 @@
 the cost F and its gradient (itself checked against central finite differences) is the yardstick: the device result
 must be a stationary point of F, equal scipy's least_squares on the same problem, and recover noise-free graphs."""
 import ctypes as C
+import math
 
 import numpy as np
 import pytest
@@ -52,12 +53,14 @@ def jr_inv(x):
     rho, phi = -x[:3], -x[3:]
     t = np.linalg.norm(phi)
     P, R = hat(phi), hat(rho)
-    if t < 0.1:  # (Taylor series to t^4: the closed forms cancel below)
-        t2, t4 = t * t, t ** 4
-        c, c1 = 1 / 12 + t2 / 720 + t4 / 30240, 1 / 6 - t2 / 120 + t4 / 5040
-        c2, c3 = 1 / 24 - t2 / 720 + t4 / 40320, 1 / 120 - t2 / 2520 + t4 / 120960
-    else:
-        c = 1 / t ** 2 - (1 + np.cos(t)) / (2 * t * np.sin(t))
+    if t < 0.5:  # (Taylor series to t^12: the closed forms cancel below)
+        t2 = t * t
+        c = np.polyval([1 / 74724249600, 691 / 1307674368000, 1 / 47900160, 1 / 1209600, 1 / 30240, 1 / 720, 1 / 12], t2)
+        c1 = np.polyval([1 / math.factorial(2 * k + 3) * (-1) ** k for k in range(6, -1, -1)], t2)
+        c2 = np.polyval([1 / math.factorial(2 * k + 4) * (-1) ** k for k in range(6, -1, -1)], t2)
+        c3 = np.polyval([(k - 1) / math.factorial(2 * k + 1) * (-1) ** k for k in range(8, 1, -1)], t2)
+    else:  # (cot(t/2) rather than (1 + cos t) / sin t, which loses 1 + cos t near pi)
+        c = 1 / t ** 2 - np.cos(t / 2) / (2 * t * np.sin(t / 2))
         c1 = (t - np.sin(t)) / t ** 3
         c2 = (t * t + 2 * np.cos(t) - 2) / (2 * t ** 4)
         c3 = (2 * t - 3 * np.sin(t) + t * np.cos(t)) / (2 * t ** 5)
